@@ -25,23 +25,39 @@ def _oracle(line: bytes, begin: int, end: int, sep: int, quote: int, cap: int):
 
 
 def _rand_line(rng, alphabet, lo, hi):
-    return bytes(rng.choice(alphabet) for _ in range(rng.randint(lo, hi)))
+    return bytes(rng.choices(alphabet, k=rng.randint(lo, hi)))
+
+
+# the blank as separator and as quote (both interact with the processor's trim), next to the usual pairs
+CONFIGS = ((ord(","), ord('"')), (ord("|"), ord("'")), (ord("\t"), ord('"')), (ord(" "), ord('"')),
+           (ord(","), ord(" ")))
+
+
+def _long_fields(sep, quote):
+    """fields of 31, 33 and 200 bytes, plain and quoted (with separators and doubled quotes inside): one 32-byte step of
+    the kernels and either side of it, and a field over more than one 128-byte stage"""
+    q, s = bytes([quote]), bytes([sep])
+    out = []
+    for n in (31, 33, 200):
+        body = (b"0123456789abcdefxyz" * 11)[:n]
+        out += [body, q + body[:n - 2] + q, q + (s + q * 2 + body)[:n - 2] + q]
+    return out
 
 
 def test_run_skipping_fsm_equals_per_byte_fsm():
     rng = random.Random(4242)
     checked = errors = 0
-    for sep, quote in ((ord(","), ord('"')), (ord("|"), ord("'")), (ord("\t"), ord('"'))):
+    for sep, quote in CONFIGS:
         soup = bytes([sep, sep, quote, quote]) + b"abc d0123456789xyz"
         wellformed_fields = [b"", b"a", b"abc", b"0123456789abcdefghij",
                              bytes([quote]) + b"q" + bytes([sep]) + b"x" + bytes([quote]),
                              bytes([quote, quote, quote]) + b"in" + bytes([quote, quote, quote]),
-                             bytes([quote, quote])]
+                             bytes([quote, quote])] + _long_fields(sep, quote)
         for it in range(6000):
             if it % 3 == 0:
-                line = bytes([sep]).join(rng.choice(wellformed_fields) for _ in range(rng.randint(1, 14)))
+                line = bytes([sep]).join(rng.choice(wellformed_fields) for _ in range(rng.randint(1, 14)))[:400]
             else:
-                line = _rand_line(rng, soup, 0, 70)
+                line = _rand_line(rng, soup, 0, 400 if it % 3 == 1 else 70)
             if not line:
                 continue
             pad = rng.randint(16, 31)  # every alignment of the line start within a 16-byte chunk
@@ -65,17 +81,18 @@ def test_bit_parallel_path_equals_the_machine_where_it_applies():
     every quote is one the machine accepts, and never claim an erroneous one."""
     rng = random.Random(99)
     taken = handed = 0
-    for sep, quote in ((ord(","), ord('"')), (ord("|"), ord("'")), (ord("\t"), ord('"'))):
+    for sep, quote in CONFIGS:
         soup = bytes([sep, sep, quote, quote]) + b"abc d0123456789xyz"
         q = bytes([quote])
         wellformed_fields = [b"", b"a", b"abc", b"0123456789abcdefghij", b"a b  c", q + b"q" + bytes([sep]) + b"x" + q,
                              q * 3 + b"in" + q * 3, q * 2, q * 4, q + b"0123456789abcdef" + q, q + b"a" + q * 2 + b"b" + q,
                              q + bytes([sep]) * 3 + q]
+        wellformed_fields += _long_fields(sep, quote)
         for it in range(8000):
             if it % 2 == 0:
-                line = bytes([sep]).join(rng.choice(wellformed_fields) for _ in range(rng.randint(1, 14)))
+                line = bytes([sep]).join(rng.choice(wellformed_fields) for _ in range(rng.randint(1, 14)))[:400]
             else:
-                line = _rand_line(rng, soup, 0, 70)
+                line = _rand_line(rng, soup, 0, 400 if it % 4 == 1 else 70)
             if not line:
                 continue
             pad = rng.randint(16, 31)

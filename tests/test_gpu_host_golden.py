@@ -96,21 +96,28 @@ def test_merge_multiline_random_groups_match_oracle():
     assert checked > 150
 
 
-@pytest.mark.parametrize("treatment", ["extend", "keep", "discard"])
-def test_delimiter_lines_with_far_more_columns_than_keys(treatment):
+@pytest.mark.parametrize("treatment,nkeys", [(t, k) for k in (3, 20) for t in ("extend", "keep", "discard")],
+                         ids=[t if k == 3 else "%s-%dkeys" % (t, k) for k in (3, 20) for t in ("extend", "keep", "discard")])
+def test_delimiter_lines_with_far_more_columns_than_keys(treatment, nkeys):
     """Untrusted content: a few lines with hundreds / thousands of columns among ordinary ones.  The host class parses
     them again on their own (bounded tables, no group-wide re-run) and still produces exactly the reference's events
-    (`__columnN__` keys in extend mode, the joined remainder in keep mode)."""
+    (`__columnN__` keys in extend mode, the joined remainder in keep mode).  With 20 keys the tables are 36 columns
+    wide, which the direct kernel (more than 32 columns) fills; long and blank-padded lines ride along."""
     import json
 
     import loongcollector_b200 as lc
     from oracle import oracle as orc
 
     name = "processor_parse_delimiter_native"
-    cfg = {"SourceKey": "content", "Separator": ",", "Quote": '"', "Keys": ["a", "b", "c"],
+    keys = ["a", "b", "c"] if nkeys == 3 else ["k%d" % i for i in range(nkeys)]
+    cfg = {"SourceKey": "content", "Separator": ",", "Quote": '"', "Keys": keys,
            "OverflowedFieldsTreatment": treatment, "KeepingSourceWhenParseFail": True}
     lines = ["1,2,3", "x,y", ",".join(str(i) for i in range(300)), "p,\"q,r\",s,t", ",".join(["z"] * 5000),
              "\"a\"\"b\",c", ",".join("\"v%d\"\"w\"" % i for i in range(40)), ""]
+    lines += [" " * 300 + ",".join(str(i) for i in range(25)) + " \r" * 150, " " * 257, " \r" * 140,
+              "\r" + " " * 40 + "a,b",
+              ",".join("f%d" % i for i in range(19)) + ",\"" + "q,\"\"" * 1000 + "\"," + "y" * 4097,
+              "m," * 33 + "\"" + "x" * 70001 + "\"", "u," * 10 + "\"" + "open" * 1100, " " * 129 + "d,\"e\"x"]
     evs = [{"type": 1, "timestamp": 5, "timestampNanosecond": 0, "contents": {"content": ln}} for ln in lines]
     root = {"events": evs}
     host, ora = lc.HostProcessor(name, cfg), orc.PROCESSORS[name](cfg)

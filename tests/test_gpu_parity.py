@@ -321,7 +321,7 @@ def test_delim_matches_oracle(eng, sep, quote, extend, allow_short):
     rng = random.Random(len(sep) * 7 + quote)
     lines = _csv_lines(rng, 3000, sep, quote) + [b"", b"   ", b" \r", b"a", sep, sep * 3]
     base, off, ln = _events(lines)
-    for nkeys, mf in ((4, 5), (4, 16), (1, 2), (9, 3)):
+    for nkeys, mf in ((4, 5), (4, 16), (1, 2), (9, 3), (4, 33), (20, 64)):
         got = eng.delim_parse(base, off, ln, sep, quote, nkeys, extend, allow_short, mf)
         want = orc.delim_parse_batch(base, off, ln, sep, quote, nkeys, extend, allow_short, mf)
         for g, w, name in zip(got, want, ("status", "nfields", "f_off", "f_len", "f_dq")):
