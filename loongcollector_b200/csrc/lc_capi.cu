@@ -87,8 +87,7 @@ struct lc_engine {
     int smem_per_sm = 0;
     bool force_basic_regex = false;   // env LC_B200_REGEX_KERNEL=basic   (tables in global memory)
     int regex_variant = 0; // env LC_B200_REGEX_KERNEL: 0 auto, 1 "fast" (stride-1), 2 "fast2" (stride-2), 3 "generic",
-                           // 4 "tdfa" (single pass, staged input), 5 "tdfa_direct" (single pass, per-lane loads),
-                           // 6 "tdfa_pc" (single pass, producer warps fill the tiles)
+                           // 4 "tdfa" (single pass); "basic" sets force_basic_regex, anything else means auto
     uint64_t scratch_hint = 0;
     int length_order = -1; // env LC_B200_LENGTH_ORDER: 1 = always order ragged batches by length, 0 = never, unset = auto
     uint32_t max_warps = 32;   // env LC_B200_MAX_WARPS (tuning knob: resident warps per block of the regex kernels)
@@ -96,7 +95,7 @@ struct lc_engine {
     // staging / workspace (grow-only)
     DevBuf in, ev_off, ev_len, out_a, out_b, out_c, out_d, out_e;
     DevBuf lines_off, lines_len, flags, state, cnt, pos, lab_sizes, lab_off, lab, order;
-    DevBuf desc;   // look-back descriptors (3 regions)
+    DevBuf desc;   // look-back descriptors of exclusive sums
     DevBuf split_scratch; // masks + per-tile counts of the three-pass split (lck::split_scratch_bytes)
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
@@ -174,19 +173,12 @@ int bind(lc_engine* e) {
     return LC_OK;
 }
 
-// descriptor regions: [0] split tiles, [1] state tiles, [2] sum tiles
-struct DescPlan {
-    uint64_t* r[3];
-};
-
-int prep_desc(lc_engine* e, size_t n0, size_t n1, size_t n2, DescPlan& plan) {
-    size_t tot = n0 + n1 + n2 + 3;
-    CU_TRY(e->desc.ensure(tot * 8));
-    CU_TRY(cudaMemsetAsync(e->desc.p, 0, tot * 8, e->stream));
+// zeroed look-back descriptors for an exclusive sum over `ntiles` tiles (lck::scan_tiles); zeroes Small too
+int prep_desc(lc_engine* e, size_t ntiles, uint64_t** desc) {
+    CU_TRY(e->desc.ensure((ntiles + 1) * 8));
+    CU_TRY(cudaMemsetAsync(e->desc.p, 0, (ntiles + 1) * 8, e->stream));
     CU_TRY(cudaMemsetAsync(e->small.p, 0, sizeof(Small), e->stream));
-    plan.r[0] = e->desc.as<uint64_t>();
-    plan.r[1] = plan.r[0] + n0 + 1;
-    plan.r[2] = plan.r[1] + n1 + 1;
+    *desc = e->desc.as<uint64_t>();
     return LC_OK;
 }
 
@@ -292,7 +284,7 @@ int lc_engine_create(int device, lc_engine_t** out) {
         e->multi_split = msp && !strcmp(msp, "1");
         const char* lo = getenv("LC_B200_LENGTH_ORDER");
         e->length_order = !lo ? -1 : (!strcmp(lo, "1") ? 1 : 0);
-        e->regex_variant = !k ? 0 : (!strcmp(k, "fast") ? 1 : (!strcmp(k, "fast2") ? 2 : (!strcmp(k, "generic") ? 3 : (!strcmp(k, "tdfa") ? 4 : (!strcmp(k, "tdfa_direct") ? 5 : (!strcmp(k, "tdfa_pc") ? 6 : 0))))));
+        e->regex_variant = !k ? 0 : (!strcmp(k, "fast") ? 1 : (!strcmp(k, "fast2") ? 2 : (!strcmp(k, "generic") ? 3 : (!strcmp(k, "tdfa") ? 4 : 0))));
     }
     CU_TRY(e->small.ensure(sizeof(Small)));
     CU_TRY(cudaMallocHost(&e->h_small, sizeof(Small)));
@@ -433,17 +425,12 @@ int lc_split_lines_dev(lc_engine_t* e, const uint8_t* d_buf, uint64_t len, uint8
     int rc = bind(e);
     if (rc)
         return rc;
-    uint32_t shift = (uint32_t)((uintptr_t)d_buf & 15u);
-    DescPlan plan;
-    rc = prep_desc(e, lck::split_tiles(len, shift), 0, 0, plan);
-    if (rc)
-        return rc;
+    CU_TRY(cudaMemsetAsync(e->small.p, 0, sizeof(Small), e->stream)); // n_out, total_chars
     Small* ds = e->small.as<Small>();
     uint32_t cap32 = cap > 0x3FFFFFFFull ? 0x3FFFFFFFu : (uint32_t)cap;
     CU_TRY(e->split_scratch.ensure(lck::split_scratch_bytes(len, false)));
-    e->launches += lck::launch_split(d_buf, (uint32_t)len, split_char, d_out_off, d_out_len, cap32, plan.r[0],
-                                     &ds->tickets[0], &ds->n_out, &ds->total_chars, e->split_scratch.as<uint64_t>(),
-                                     e->stream);
+    e->launches += lck::launch_split(d_buf, (uint32_t)len, split_char, d_out_off, d_out_len, cap32, &ds->n_out,
+                                     &ds->total_chars, e->split_scratch.as<uint64_t>(), e->stream);
     CU_TRY(cudaGetLastError());
     Small* hs = (Small*)e->h_small;
     CU_TRY(cudaMemcpyAsync(hs, ds, sizeof(Small), cudaMemcpyDeviceToHost, e->stream));
@@ -588,28 +575,14 @@ static int regex_parse_dev_impl(lc_engine_t* e, const lc_regex_t* re, const uint
     // ---- single-pass tagged DFA: the preferred kernel whenever the pattern's TDFA fits shared memory.  Nothing on
     // this path waits for the device: ragged-batch ordering is decided by a device-side flag and events too long for
     // the 16-bit capture registers are redone by a follow-up kernel that exits at once when there was none.
-    if (!force_basic && (e->regex_variant == 0 || e->regex_variant >= 4) && !re->res.tdfa_blob.empty()) {
+    if (!force_basic && (e->regex_variant == 0 || e->regex_variant == 4) && !re->res.tdfa_blob.empty()) {
         const LcTdfaHeader* th = reinterpret_cast<const LcTdfaHeader*>(re->res.tdfa_blob.data());
         const uint32_t tb = (uint32_t)re->res.tdfa_blob.size();
-        const bool staged = e->regex_variant != 5 || ev_stride != 1;
-        auto smem_need = [&](uint32_t warps) {
-            return staged ? lck::tdfa_staged_smem_bytes(tb, th->nregs, warps * 32)
-                          : lck::tdfa_smem_bytes(tb, th->nregs, warps * 32);
-        };
+        auto smem_need = [&](uint32_t warps) { return lck::tdfa_staged_smem_bytes(tb, th->nregs, warps * 32); };
         uint32_t warps = e->max_warps;
         while (warps > 4 && smem_need(warps) > smem_max)
             warps -= 2;
-        bool usable = smem_need(warps) <= smem_max;
-        if (usable && !staged && base_len >= 65535) { // A/B kernel without the long-event hand-over: host-side check
-            CU_TRY(cudaMemsetAsync(ds->counters, 0, sizeof ds->counters, e->stream));
-            lck::launch_len_stats(d_ev_len, n, ds->counters, e->stream);
-            e->launches++;
-            CU_TRY(cudaMemcpyAsync(hs->counters, ds->counters, sizeof ds->counters, cudaMemcpyDeviceToHost,
-                                   e->stream));
-            CU_TRY(cudaStreamSynchronize(e->stream));
-            usable = hs->counters[0] < 65535;
-        }
-        if (usable) {
+        if (smem_need(warps) <= smem_max) {
             const void* d_tblob;
             CU_TRY(engine_blob(e, re, &d_tblob, 3));
             const uint32_t threads = warps * 32;
@@ -621,7 +594,7 @@ static int regex_parse_dev_impl(lc_engine_t* e, const lc_regex_t* re, const uint
             // LC_B200_LENGTH_ORDER=1 forces the pre-pass, =0 disables it.
             const uint32_t* d_order = nullptr;
             const uint32_t* d_order_flag = nullptr;
-            if (staged && ev_stride == 1 && n >= 4096 && e->length_order != 0 &&
+            if (ev_stride == 1 && n >= 4096 && e->length_order != 0 &&
                 (e->length_order == 1 || span_bytes / n >= 1024)) {
                 CU_TRY(e->order.ensure(n * 4 + 512));
                 uint32_t* hist = e->order.as<uint32_t>() + n;
@@ -632,29 +605,15 @@ static int regex_parse_dev_impl(lc_engine_t* e, const lc_regex_t* re, const uint
             }
             CU_TRY(cudaMemsetAsync(&ds->overflow, 0, offsetof(Small, total_chars) - offsetof(Small, overflow),
                                    e->stream));
-            int er;
-            if (staged && e->regex_variant == 6 && !d_order &&
-                lck::tdfa_pc_smem_bytes(tb, th->nregs, 1024) <= smem_max)
-                er = lck::launch_regex_tdfa_pc(d_tblob, tb, th->has_slow != 0, th->nregs, d_base, d_ev_off, d_ev_len,
-                                               ev_stride, n, nkeys, d_status, bool_only ? nullptr : d_cap_off,
-                                               bool_only ? nullptr : d_cap_len, 1024,
-                                               (uint32_t)std::min<uint64_t>((n + 895) / 896, (uint64_t)e->num_sms),
-                                               &ds->next_batch, &ds->overflow, e->stream);
-            else if (staged)
-                er = lck::launch_regex_tdfa_staged(d_tblob, tb, th->has_slow != 0, th->nregs, d_base, d_ev_off,
+            int er = lck::launch_regex_tdfa_staged(d_tblob, tb, th->has_slow != 0, th->nregs, d_base, d_ev_off,
                                                    d_ev_len, ev_stride, n, nkeys, d_status,
                                                    bool_only ? nullptr : d_cap_off, bool_only ? nullptr : d_cap_len,
                                                    threads, grid, &ds->next_batch, &ds->overflow, d_order,
                                                    d_order_flag, e->stream);
-            else
-                er = lck::launch_regex_tdfa(d_tblob, tb, th->has_slow != 0, th->nregs, d_base, d_ev_off, d_ev_len, n,
-                                            nkeys, d_status, bool_only ? nullptr : d_cap_off,
-                                            bool_only ? nullptr : d_cap_len, threads, grid, &ds->next_batch, nullptr,
-                                            e->stream);
             e->launches++;
             if (er)
                 return fail(LC_ERR_CUDA, std::string("regex kernel launch: ") + cudaGetErrorString((cudaError_t)er));
-            if (staged && base_len >= 65535) {
+            if (base_len >= 65535) {
                 lck::TdfaMultiArgs ma;
                 memset(&ma, 0, sizeof ma);
                 ma.blob[0] = d_tblob;
@@ -829,14 +788,14 @@ static int regex_parse_dev_impl(lc_engine_t* e, const lc_regex_t* re, const uint
     const uint64_t* d_lab_off = nullptr;
     uint16_t* d_lab = nullptr;
     if (h->mode == LC_MODE_TWOPASS) {
-        DescPlan plan;
-        rc = prep_desc(e, 0, 0, lck::scan_tiles(n), plan);
+        uint64_t* desc;
+        rc = prep_desc(e, lck::scan_tiles(n), &desc);
         if (rc)
             return rc;
         CU_TRY(e->lab_sizes.ensure(n * 4));
         CU_TRY(e->lab_off.ensure(n * 8));
         lck::launch_label_sizes(d_ev_len, n, e->lab_sizes.as<uint32_t>(), e->stream);
-        lck::launch_exclusive_sum(e->lab_sizes.as<uint32_t>(), n, e->lab_off.as<uint64_t>(), &ds->total, plan.r[2],
+        lck::launch_exclusive_sum(e->lab_sizes.as<uint32_t>(), n, e->lab_off.as<uint64_t>(), &ds->total, desc,
                                   &ds->tickets[2], e->stream);
         e->launches += 2;
         CU_TRY(cudaGetLastError());
@@ -1373,129 +1332,42 @@ int lc_multiline_split_dev(lc_engine_t* e, const uint8_t* d_buf, uint64_t len, c
 
     Small* ds = e->small.as<Small>();
     Small* hs = (Small*)e->h_small;
-    uint32_t shift = (uint32_t)((uintptr_t)d_buf & 15u);
-    static const bool fused = [] {
-        const char* k = getenv("LC_B200_ML_FUSED"); // A/B knob: 0 = the five-kernel formulation
-        return !(k && !strcmp(k, "0"));
-    }();
-    if (fused) {
-        // Two launches, no host round trip in between: (1) split + per-line probes, (2) state scan + counts + slots +
-        // emission; the second reads the line count from device memory.  The line table is sized from an estimate and
-        // the call repeats with the exact size in the rare case it was too small.
-        uint64_t lcap = len / 24 + 4096;
-        for (;;) {
-            if (lcap > len)
-                lcap = len;
-            if (lcap > 0x3FFFFFF0ull)
-                lcap = 0x3FFFFFF0ull;
-            CU_TRY(e->lines_off.ensure((lcap + 1) * 4));
-            CU_TRY(e->lines_len.ensure((lcap + 1) * 4));
-            CU_TRY(e->flags.ensure(lcap + 1));
-            const uint32_t ftiles = lck::ml_fused_tiles(lcap);
-            DescPlan plan;
-            rc = prep_desc(e, lck::split_tiles(len, shift), ftiles, ftiles, plan);
-            if (rc)
-                return rc;
-            CU_TRY(e->split_scratch.ensure(lck::split_scratch_bytes(len, true)));
-            e->launches += lck::launch_split_probe(cfg, d_buf, (uint32_t)len, e->lines_off.as<uint32_t>(),
-                                                   e->lines_len.as<uint32_t>(), e->flags.as<uint8_t>(), (uint32_t)lcap,
-                                                   plan.r[0], &ds->tickets[0], &ds->n_out, &ds->total_chars,
-                                                   e->split_scratch.as<uint64_t>(), e->stream) - 1;
-            static const bool ml_lookback = [] {
-                const char* v = getenv("LC_B200_ML"); // A/B knob: "lookback" = ml_fused_kernel (two chained look-backs)
-                return v && !strcmp(v, "lookback");
-            }();
-            if (ml_lookback) {
-                lck::launch_ml_fused(cfg, e->flags.as<uint8_t>(), e->lines_off.as<uint32_t>(),
-                                     e->lines_len.as<uint32_t>(), &ds->n_out, (uint32_t)lcap, (uint32_t)len, d_out_off,
-                                     d_out_len, d_out_flags, cap, plan.r[1], plan.r[2], &ds->tickets[1], ds->counters,
-                                     &ds->total, e->stream);
-                e->launches += 2;
-            } else {
-                CU_TRY(e->state.ensure((size_t)lck::ml_pass_scratch_bytes(lcap)));
-                e->launches += 1 + lck::launch_ml_passes(cfg, e->flags.as<uint8_t>(), e->lines_off.as<uint32_t>(),
-                                                         e->lines_len.as<uint32_t>(), &ds->n_out, (uint32_t)lcap,
-                                                         (uint32_t)len, d_out_off, d_out_len, d_out_flags, cap,
-                                                         e->state.as<uint64_t>(), ds->counters, &ds->total, e->stream);
-            }
-            CU_TRY(cudaGetLastError());
-            CU_TRY(cudaMemcpyAsync(hs, ds, sizeof(Small), cudaMemcpyDeviceToHost, e->stream));
-            CU_TRY(cudaStreamSynchronize(e->stream));
-            if (hs->total_chars >= (1ull << 30) - 2)
-                return fail(LC_ERR_TOO_LARGE, "more than 2^30 lines in one call");
-            if (hs->n_out <= lcap)
-                break;
-            lcap = hs->n_out;
-        }
-        *n_out = hs->total;
-        if (counters) {
-            counters[0] += hs->counters[0];
-            counters[1] += hs->n_out;
-            counters[2] += hs->counters[1];
-        }
-        if (*n_out > cap)
-            return fail(LC_ERR_CAPACITY, "lc_multiline_split: output capacity too small");
-        return LC_OK;
-    }
-    // 1. line table (grow the workspace until it fits; typical logs fit the first estimate)
+    // Two steps, no host round trip in between: (1) split + per-line probes, (2) the multiline passes (state scan,
+    // counts, slots, emission), which read the line count from device memory.  The line table is sized from an
+    // estimate and the call repeats with the exact size in the rare case it was too small.
     uint64_t lcap = len / 24 + 4096;
-    uint64_t n = 0;
     for (;;) {
         if (lcap > len)
             lcap = len;
+        if (lcap > 0x3FFFFFF0ull)
+            lcap = 0x3FFFFFF0ull;
         CU_TRY(e->lines_off.ensure((lcap + 1) * 4));
         CU_TRY(e->lines_len.ensure((lcap + 1) * 4));
-        DescPlan plan;
-        rc = prep_desc(e, lck::split_tiles(len, shift), 0, 0, plan);
-        if (rc)
-            return rc;
-        CU_TRY(e->split_scratch.ensure(lck::split_scratch_bytes(len, false)));
-        e->launches += lck::launch_split(d_buf, (uint32_t)len, '\n', e->lines_off.as<uint32_t>(),
-                                         e->lines_len.as<uint32_t>(),
-                                         (uint32_t)(lcap > 0x3FFFFFFFull ? 0x3FFFFFFFull : lcap), plan.r[0],
-                                         &ds->tickets[0], &ds->n_out, &ds->total_chars,
-                                         e->split_scratch.as<uint64_t>(), e->stream);
+        CU_TRY(e->flags.ensure(lcap + 1));
+        CU_TRY(cudaMemsetAsync(e->small.p, 0, sizeof(Small), e->stream)); // n_out, total_chars, total, counters
+        CU_TRY(e->split_scratch.ensure(lck::split_scratch_bytes(len, true)));
+        e->launches += lck::launch_split_probe(cfg, d_buf, (uint32_t)len, e->lines_off.as<uint32_t>(),
+                                               e->lines_len.as<uint32_t>(), e->flags.as<uint8_t>(), (uint32_t)lcap,
+                                               &ds->n_out, &ds->total_chars, e->split_scratch.as<uint64_t>(),
+                                               e->stream) - 1;
+        CU_TRY(e->state.ensure((size_t)lck::ml_pass_scratch_bytes(lcap)));
+        e->launches += 1 + lck::launch_ml_passes(cfg, e->flags.as<uint8_t>(), e->lines_off.as<uint32_t>(),
+                                                 e->lines_len.as<uint32_t>(), &ds->n_out, (uint32_t)lcap,
+                                                 (uint32_t)len, d_out_off, d_out_len, d_out_flags, cap,
+                                                 e->state.as<uint64_t>(), ds->counters, &ds->total, e->stream);
         CU_TRY(cudaGetLastError());
         CU_TRY(cudaMemcpyAsync(hs, ds, sizeof(Small), cudaMemcpyDeviceToHost, e->stream));
         CU_TRY(cudaStreamSynchronize(e->stream));
         if (hs->total_chars >= (1ull << 30) - 2)
             return fail(LC_ERR_TOO_LARGE, "more than 2^30 lines in one call");
-        n = hs->n_out;
-        if (n <= lcap)
+        if (hs->n_out <= lcap)
             break;
-        lcap = n;
+        lcap = hs->n_out;
     }
-    if (n >= (1ull << 30) - 2)
-        return fail(LC_ERR_TOO_LARGE, "more than 2^30 lines in one call");
-    // 2. per-line prefix probes
-    CU_TRY(e->flags.ensure(n + 1));
-    lck::launch_ml_probe(cfg, d_buf, e->lines_off.as<uint32_t>(), e->lines_len.as<uint32_t>(), n,
-                         e->flags.as<uint8_t>(), e->stream);
-    // 3. state scan + event counts, 4. output slots
-    DescPlan plan;
-    rc = prep_desc(e, 0, lck::scan_tiles(n + 1), lck::scan_tiles(n + 1), plan);
-    if (rc)
-        return rc;
-    CU_TRY(e->state.ensure((n + 1) * 4));
-    CU_TRY(e->cnt.ensure((n + 1) * 4));
-    CU_TRY(e->pos.ensure((n + 1) * 8));
-    lck::launch_ml_state(cfg, e->flags.as<uint8_t>(), e->lines_len.as<uint32_t>(), n, e->state.as<uint32_t>(),
-                         e->cnt.as<uint32_t>(), plan.r[1],
-                         &ds->tickets[1], e->stream);
-    lck::launch_exclusive_sum(e->cnt.as<uint32_t>(), n + 1, e->pos.as<uint64_t>(), &ds->total, plan.r[2],
-                              &ds->tickets[2], e->stream);
-    // 5. emission
-    lck::launch_ml_emit(cfg, e->flags.as<uint8_t>(), e->lines_off.as<uint32_t>(), e->lines_len.as<uint32_t>(), n,
-                        (uint32_t)len, e->state.as<uint32_t>(), e->pos.as<uint64_t>(), d_out_off, d_out_len,
-                        d_out_flags, cap, ds->counters, e->stream);
-    e->launches += 4;
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(hs, ds, sizeof(Small), cudaMemcpyDeviceToHost, e->stream));
-    CU_TRY(cudaStreamSynchronize(e->stream));
     *n_out = hs->total;
     if (counters) {
         counters[0] += hs->counters[0];
-        counters[1] += n;
+        counters[1] += hs->n_out;
         counters[2] += hs->counters[1];
     }
     if (*n_out > cap)
@@ -1564,7 +1436,6 @@ int lc_remove_last_incomplete_log_dev(lc_engine_t* e, const uint8_t* d_buf, uint
     fill_probe_slot(cfg, 2, end);
     Small* ds = e->small.as<Small>();
     Small* hs = (Small*)e->h_small;
-    const uint32_t shift = (uint32_t)((uintptr_t)d_buf & 15u);
     uint64_t lcap = len / 24 + 4096;
     for (;;) {
         if (lcap > len)
@@ -1572,15 +1443,12 @@ int lc_remove_last_incomplete_log_dev(lc_engine_t* e, const uint8_t* d_buf, uint
         CU_TRY(e->lines_off.ensure((lcap + 1) * 4));
         CU_TRY(e->lines_len.ensure((lcap + 1) * 4));
         CU_TRY(e->flags.ensure(lcap + 1));
-        DescPlan plan;
-        rc = prep_desc(e, lck::split_tiles(len, shift), 0, 0, plan);
-        if (rc)
-            return rc;
+        CU_TRY(cudaMemsetAsync(e->small.p, 0, sizeof(Small), e->stream)); // n_out, total_chars, counters
         CU_TRY(e->split_scratch.ensure(lck::split_scratch_bytes(len, true)));
         e->launches += lck::launch_split_probe(cfg, d_buf, (uint32_t)len, e->lines_off.as<uint32_t>(),
                                                e->lines_len.as<uint32_t>(), e->flags.as<uint8_t>(), (uint32_t)lcap,
-                                               plan.r[0], &ds->tickets[0], &ds->n_out, &ds->total_chars,
-                                               e->split_scratch.as<uint64_t>(), e->stream) - 1;
+                                               &ds->n_out, &ds->total_chars, e->split_scratch.as<uint64_t>(),
+                                               e->stream) - 1;
         lck::launch_last_record(e->flags.as<uint8_t>(), e->lines_off.as<uint32_t>(), e->lines_len.as<uint32_t>(),
                                 &ds->n_out, (uint32_t)lcap, (uint32_t)len, start != nullptr, end != nullptr,
                                 ds->counters, e->stream);
@@ -1818,8 +1686,8 @@ int lc_sls_serialize_logs(lc_engine_t* e, const uint8_t* base, uint64_t base_len
     CU_TRY(e->lab_sizes.ensure(n * 4));
     CU_TRY(e->cnt.ensure(n * 4));
     CU_TRY(e->lab_off.ensure(n * 8));
-    DescPlan plan;
-    rc = prep_desc(e, 0, 0, lck::scan_tiles(n), plan);
+    uint64_t* desc;
+    rc = prep_desc(e, lck::scan_tiles(n), &desc);
     if (rc)
         return rc;
     Small* ds = e->small.as<Small>();
@@ -1838,7 +1706,7 @@ int lc_sls_serialize_logs(lc_engine_t* e, const uint8_t* base, uint64_t base_len
     const uint32_t* d_ns = ev_time_ns ? e->lines_len.as<uint32_t>() : nullptr;
     lck::launch_sls_sizes(e->pos.as<uint64_t>(), e->ev_len.as<uint32_t>(), e->out_c.as<uint32_t>(), d_ns, n,
                           e->lab_sizes.as<uint32_t>(), e->cnt.as<uint32_t>(), e->stream);
-    lck::launch_exclusive_sum(e->lab_sizes.as<uint32_t>(), n, e->lab_off.as<uint64_t>(), &ds->total, plan.r[2],
+    lck::launch_exclusive_sum(e->lab_sizes.as<uint32_t>(), n, e->lab_off.as<uint64_t>(), &ds->total, desc,
                               &ds->tickets[2], e->stream);
     e->launches += 2;
     CU_TRY(cudaGetLastError());
@@ -1908,14 +1776,14 @@ int lc_sls_serialize_parsed_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t 
     CU_TRY(e->lab_sizes.ensure(n * 4));
     CU_TRY(e->cnt.ensure(n * 4));
     CU_TRY(e->lab_off.ensure(n * 8));
-    DescPlan plan;
-    rc = prep_desc(e, 0, 0, lck::scan_tiles(n), plan);
+    uint64_t* desc;
+    rc = prep_desc(e, lck::scan_tiles(n), &desc);
     if (rc)
         return rc;
     Small* ds = e->small.as<Small>();
     Small* hs = (Small*)e->h_small;
     lck::launch_sls_parsed_sizes(a, d_ev_time_ns, n, e->lab_sizes.as<uint32_t>(), e->cnt.as<uint32_t>(), e->stream);
-    lck::launch_exclusive_sum(e->lab_sizes.as<uint32_t>(), n, e->lab_off.as<uint64_t>(), &ds->total, plan.r[2],
+    lck::launch_exclusive_sum(e->lab_sizes.as<uint32_t>(), n, e->lab_off.as<uint64_t>(), &ds->total, desc,
                               &ds->tickets[2], e->stream);
     e->launches += 2;
     CU_TRY(cudaGetLastError());

@@ -1,8 +1,8 @@
 // lc_kernels.cu -- sm_90a kernels of the log-parsing engine.
 //
-// All work is HBM-bound byte / integer indexing (no tensor cores): the split kernel streams the
-// SourceBuffer bytes once with 16-byte coalesced loads and ranks every line with a single-pass
-// decoupled look-back scan; the regex kernels interpret the automaton tables produced by
+// All work is HBM-bound byte / integer indexing (no tensor cores): the split passes stream the
+// SourceBuffer bytes once with 16-byte coalesced loads and number every line from a scan of
+// per-tile line counts; the regex kernels interpret the automaton tables produced by
 // regex_compiler.cpp once per log line; the multiline splitter turns the reference's sequential
 // start/continue/end state machine into a prefix scan over 2-state transition functions.
 //
@@ -13,13 +13,11 @@
 //   delimiter  core/plugin/processor/ProcessorParseDelimiterNative.cpp:219-409, core/parser/DelimiterModeFsmParser.cpp:49-294
 #include "lc_kernels.cuh"
 
-#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
 #include <type_traits>
-#include <vector>
 
 #include "lc_exec.cuh"
 #include "lc_scan.cuh"
@@ -41,13 +39,6 @@ __device__ __forceinline__ uint32_t match16(uint4 v, uint32_t splat) {
     return m;
 }
 
-// Each thread owns SEGS x 64 contiguous bytes (4 x 16-byte chunks and one 64-bit newline mask per segment): ONE
-// block scan and ONE look-back per tile of THREADS x SEGS x 64 bytes.  A warp's loads cover contiguous memory, so
-// every 128-byte line is fetched once (lanes share it through L1).  Tiles are deliberately LARGE (1024 threads,
-// 64 KiB): the block waits at a barrier while its first warp walks back over the descriptors of unfinished
-// predecessors, and that walk gets longer with the number of tiles in flight (on C1, 16 and 32 KiB tiles were slower;
-// so were 128 KiB tiles = 2 segments per thread, whose 57 registers leave one block per SM, and one tile per WARP with
-// no barrier at all).
 // PROBE (multiline, a2): the anchored prefix probes of the start / continue / end patterns (regex_search +
 // match_continuous, StringTools.cpp:263-288) are evaluated by the same pass that finds the lines -- a line's first bytes
 // were fetched a moment ago (same tile or the one before: L1 / L2 hits), so the separate probe pass that re-read the
@@ -62,7 +53,6 @@ struct SplitProbe {
     uint32_t empty_flags;  // flags of an empty line (patterns that match the empty prefix)
     uint8_t* flags;        // [line] bit0/1/2 = start / continue / end matches a prefix
 };
-constexpr uint32_t kProbeQueue = 4096;
 constexpr uint32_t kProbeTable = 2048; // u16 entries of a prefix DFA that is staged in shared memory (states x classes)
 
 // The prefix DFAs of the (up to three) patterns, staged in shared memory by every block of the split + probe pass: a
@@ -169,209 +159,8 @@ __device__ __forceinline__ uint32_t match16b(uint4 v, uint32_t splat) {
     return m;
 }
 
-// Each thread owns 64 contiguous bytes (4 x 16-byte chunks, one 64-bit newline mask): ONE block scan and ONE look-back
-// per 64 KiB tile.  The pass is bound by instruction issue and barrier waits rather than by HBM, so the code is kept
-// lean: byte compares without the emulated SIMD-video
-// instructions, range checks only in the last tile, a 32-bit shuffle scan for the counts, and the "start of my first
-// line" taken from the nearest previous thread that holds a newline (ballot + one shuffle) instead of a max-scan.
-__device__ __forceinline__ uint64_t globaltimer_ns() {
-    uint64_t t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-
-// TRACE (debug, LC_B200_SPLIT_TRACE=<file>): thread 0 of every block stamps %globaltimer at the phase boundaries into
-// trace[tile * 8 ..]: 0 block start, 1 ticket known, 2 own loads + masks done, 3 whole block scanned, 4 look-back done,
-// 5 stores issued, 6 end.
-template <int THREADS, int LBW, bool PROBE, bool TRACE = false>
-__global__ void __launch_bounds__(THREADS, 2048 / THREADS)
-    split_kernel(const uint8_t* __restrict__ buf, uint32_t len, uint32_t shift, uint32_t splat,
-                 uint32_t* __restrict__ out_off, uint32_t* __restrict__ out_len, uint32_t cap, volatile uint64_t* desc,
-                 uint32_t* ticket, uint32_t ntiles, uint32_t* n_out, unsigned long long* total_chars, SplitProbe pr,
-                 uint64_t* trace = nullptr) {
-    constexpr int NW = THREADS / 32;
-    uint64_t tr[7];
-    if (TRACE)
-        tr[0] = globaltimer_ns();
-    __shared__ uint32_t s_cnt[NW];   // per warp: newline count, then its exclusive prefix inside the tile
-    __shared__ uint32_t s_last[NW];  // per warp: end (offset + 1) of its last newline, 0 = none
-    __shared__ uint32_t s_start[NW]; // per warp: start of the line that is open when the warp's bytes begin (0 = none in tile)
-    __shared__ uint32_t s_tile, s_tot, s_tlast;
-    __shared__ uint64_t s_prefix;
-    __shared__ uint64_t s_part[LBW > 1 ? LBW : 1];
-    __shared__ uint32_t s_flag[LBW > 1 ? LBW : 1];
-    __shared__ uint32_t s_qn;
-    __shared__ uint32_t s_q[PROBE ? kProbeQueue : 1];
-    __shared__ typename std::conditional<PROBE, ProbeSmem, uint32_t>::type s_probe;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    if (tid == 0) {
-        s_tile = atomicAdd(ticket, 1u);
-        s_qn = 0;
-    }
-    if constexpr (PROBE)
-        probe_stage(pr, s_probe);
-    __syncthreads();
-    const uint32_t tile = s_tile;
-    if (TRACE)
-        tr[1] = globaltimer_ns();
-    const uint4* vbuf = reinterpret_cast<const uint4*>(buf - shift);
-    const uint64_t total_v = (uint64_t)len + shift; // virtual length including the alignment lead-in
-    const uint64_t chunk0 = ((uint64_t)tile * THREADS + tid) * 4;
-    const uint64_t vpos0 = chunk0 * 16;
-    const bool full = ((uint64_t)(tile + 1) * THREADS * 64 <= total_v) && !(tile == 0 && shift);
-
-    uint64_t mk = 0;
-    if (full) {
-        uint4 v[4];
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-            v[r] = __ldg(vbuf + chunk0 + r);
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-            mk |= (uint64_t)match16b(v[r], splat) << (16 * r);
-    } else {
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const uint64_t vpos = vpos0 + (uint64_t)r * 16;
-            if (vpos < total_v) {
-                uint32_t m = match16b(__ldg(vbuf + chunk0 + r), splat);
-                if (vpos == 0 && shift) // alignment lead-in bytes in front of the buffer (shift < 16)
-                    m &= ~((1u << shift) - 1u);
-                const uint64_t rem = total_v - vpos;
-                if (rem < 16)
-                    m &= (1u << rem) - 1u;
-                mk |= (uint64_t)m << (16 * r);
-            }
-        }
-    }
-    const uint32_t cnt = __popcll(mk);
-    const uint32_t last = mk ? (uint32_t)(vpos0 + (63 - __clzll((long long)mk)) + 1 - shift) : 0u;
-    if (TRACE)
-        tr[2] = globaltimer_ns() + (cnt >> 31);
-    // ---- counts: inclusive warp scan; starts: nearest previous holder of a newline
-    uint32_t inc = cnt;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, inc, d);
-        if (lane >= d)
-            inc += t;
-    }
-    const uint32_t has = __ballot_sync(0xFFFFFFFFu, mk != 0);
-    const uint32_t below = has & ((1u << lane) - 1u);
-    const uint32_t prev_last = __shfl_sync(0xFFFFFFFFu, last, below ? 31 - __clz(below) : 0);
-    const uint32_t warp_last = __shfl_sync(0xFFFFFFFFu, last, has ? 31 - __clz(has) : 0);
-    if (lane == 31) {
-        s_cnt[wid] = inc;
-        s_last[wid] = has ? warp_last : 0u;
-    }
-    __syncthreads();
-    if (wid == 0) {
-        uint32_t c = lane < NW ? s_cnt[lane] : 0u;
-        const uint32_t wl = lane < NW ? s_last[lane] : 0u;
-        uint32_t ci = c;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, ci, d);
-            if (lane >= d)
-                ci += t;
-        }
-        const uint32_t whas = __ballot_sync(0xFFFFFFFFu, c != 0);
-        const uint32_t wbelow = whas & ((1u << lane) - 1u);
-        const uint32_t st = __shfl_sync(0xFFFFFFFFu, wl, wbelow ? 31 - __clz(wbelow) : 0);
-        const uint32_t tl = __shfl_sync(0xFFFFFFFFu, wl, whas ? 31 - __clz(whas) : 0);
-        if (lane < NW) {
-            s_cnt[lane] = ci - c; // exclusive prefix of the warp inside the tile
-            s_start[lane] = wbelow ? st : 0u;
-        }
-        const uint32_t totv = __shfl_sync(0xFFFFFFFFu, ci, NW - 1);
-        if (lane == 0) {
-            s_tot = totv;
-            s_tlast = whas ? tl : 0u;
-        }
-    }
-    __syncthreads();
-    if (TRACE)
-        tr[3] = globaltimer_ns();
-    const uint64_t tot = OpCountMax::make(s_tot, s_tlast);
-    uint64_t tile_prefix;
-    if (LBW > 1) {
-        tile_prefix = lookback_block<OpCountMax, LBW>(desc, tile, tot, s_part, s_flag);
-    } else {
-        if (tid < 32) {
-            uint64_t p = LBW < 0 ? lookback_deep<OpCountMax, (LBW < 0 ? -LBW : 1)>(desc, tile, tot)
-                                 : lookback<OpCountMax>(desc, tile, tot);
-            if (tid == 0)
-                s_prefix = p;
-        }
-        __syncthreads();
-        tile_prefix = s_prefix;
-    }
-    if (TRACE)
-        tr[4] = globaltimer_ns() + (tile_prefix >> 63);
-    if (tid == 0 && s_tot) // un-truncated count (the payload keeps 30 bits): > 2^30 pieces is an error
-        atomicAdd(total_chars, (unsigned long long)s_tot);
-    uint32_t k = (OpCountMax::count(tile_prefix) + s_cnt[wid] + (inc - cnt)) & 0x3FFFFFFFu;
-    uint32_t start = below ? prev_last : (s_start[wid] ? s_start[wid] : OpCountMax::maxv(tile_prefix));
-    while (mk) {
-        const int b = __ffsll((long long)mk) - 1;
-        mk &= mk - 1;
-        const uint32_t p = (uint32_t)(vpos0 + b - shift);
-        if (k < cap) {
-            out_off[k] = start;
-            out_len[k] = p - start;
-            if (PROBE) {
-                const uint32_t ll = p - start;
-                const uint32_t cand = ll ? probe_first(pr, buf[start]) : 0u;
-                if (!cand) {
-                    pr.flags[k] = ll ? 0 : (uint8_t)pr.empty_flags;
-                } else {
-                    const uint32_t q = atomicAdd(&s_qn, 1u);
-                    if (q < kProbeQueue)
-                        s_q[q] = k;
-                    else
-                        pr.flags[k] = probe_line(pr, buf + start, ll); // queue full: probe in place
-                }
-            }
-        }
-        ++k;
-        start = p + 1;
-    }
-    if (tile == ntiles - 1 && tid == THREADS - 1) {
-        // inclusive total of the whole buffer: the unterminated last piece, if any
-        if (start < len) {
-            if (k < cap) {
-                out_off[k] = start;
-                out_len[k] = len - start;
-                if (PROBE)
-                    pr.flags[k] = probe_line(pr, buf + start, len - start);
-            }
-            ++k;
-        }
-        *n_out = k;
-    }
-    if (TRACE)
-        tr[5] = globaltimer_ns() + (k >> 31);
-    if constexpr (PROBE) {
-        __syncthreads(); // the queue is complete and this tile's line table entries are visible to the block
-        const uint32_t qn = min(s_qn, kProbeQueue);
-        for (uint32_t q = tid; q < qn; q += THREADS) {
-            const uint32_t kk = s_q[q];
-            pr.flags[kk] = probe_line_smem(pr, s_probe, buf + out_off[kk], out_len[kk]);
-        }
-    }
-    if (TRACE) {
-        __syncthreads();
-        tr[6] = globaltimer_ns();
-        if (tid == 0) {
-            for (int q = 0; q < 7; ++q)
-                trace[(uint64_t)tile * 8 + q] = tr[q];
-            trace[(uint64_t)tile * 8 + 7] = blockIdx.x;
-        }
-    }
-}
-
 // ---- three-pass split: masks -> tile scan -> emission ------------------------------------------------------------------
-// What the single-pass kernel above cannot get around (measured with LC_B200_SPLIT_TRACE, three restructurings tried:
+// What a single-pass kernel cannot get around (measured with per-tile phase timestamps, three restructurings tried:
 // persistent + prefetched tiles, a scanner warp beside the byte work, two tiles of slack, 256-descriptor walks): lines
 // must be numbered in buffer order, so with a decoupled look-back a tile finishes only after EVERY earlier tile has
 // published its count, and the per-tile service time has a heavy tail (with two 1024-thread blocks on an SM).  All the
@@ -379,7 +168,8 @@ __global__ void __launch_bounds__(THREADS, 2048 / THREADS)
 // the look-back was the largest phase in every variant: persistent blocks with cp.async-prefetched tiles (the loads
 // fully hidden), 8 descriptors per lane and round, a scanner warp beside 31 data warps with two tiles of slack (one
 // round of 256 descriptors, re-polled while it waits for unpublished predecessors), and three tickets per block (a
-// serial chain).  (Those kernels are not kept; split_kernel is, behind LC_B200_SPLIT=lookback.)
+// serial chain).  (None of those kernels is kept; the plain single-pass look-back split was 5 % slower than the three
+// passes below on an H100.)
 // The order constraint only concerns the NUMBERS, though, not the bytes:
 //   pass 1  split_mask_kernel   reads the buffer once (a warp covers 2 KiB with four 16-byte loads per lane), and
 //                               writes one mask bit per byte (len/8 bytes) plus {count, end of last newline} per tile;
@@ -747,15 +537,6 @@ __global__ void __launch_bounds__(1024, 2)
         probe_step(0, qn); // what is left in the warp's queue
 }
 
-static int split_lookback_warps() {
-    static const int w = [] {
-        const char* e = getenv("LC_B200_LOOKBACK_WARPS"); // A/B knob of the single-pass kernel: 1 (default) = one warp walks,
-        int t = e ? atoi(e) : 1;                          // 4 = block-wide (slower), -8 = one warp, 8
-        return t == 4 ? 4 : (t == -8) ? t : 1;            // descriptors per lane (slower)
-    }();
-    return w;
-}
-
 uint64_t split_scratch_bytes(uint64_t len, bool probe) {
     const uint64_t nt = (len + 16 + kSplitTileChunks * 16 - 1) / (kSplitTileChunks * 16);
     return nt * 16 + nt * 256 + nt * kSplitTileChunks * (probe ? 4 : 2) + 256;
@@ -763,94 +544,40 @@ uint64_t split_scratch_bytes(uint64_t len, bool probe) {
 
 template <bool PROBE>
 static int launch_split_impl(const uint8_t* d_buf, uint32_t len, uint8_t split_char, uint32_t* d_off, uint32_t* d_len,
-                             uint32_t cap, uint64_t* d_desc, uint32_t* d_ticket, uint32_t* d_n_out,
-                             unsigned long long* d_total, uint64_t* d_scratch, const SplitProbe& pr, cudaStream_t st) {
+                             uint32_t cap, uint32_t* d_n_out, unsigned long long* d_total, uint64_t* d_scratch,
+                             const SplitProbe& pr, cudaStream_t st) {
     uint32_t shift = (uint32_t)((uintptr_t)d_buf & 15u);
     uint32_t splat = split_char * 0x01010101u;
-    static const bool lookback_mode = [] {
-        const char* e = getenv("LC_B200_SPLIT"); // A/B knob: "lookback" = the single-pass kernel (split_kernel)
-        return e && !strcmp(e, "lookback");
-    }();
-    if (d_scratch && !lookback_mode && !getenv("LC_B200_SPLIT_TRACE")) {
-        const uint32_t nt = (uint32_t)(((uint64_t)len + shift + kSplitTileChunks * 16 - 1) / (kSplitTileChunks * 16));
-        uint64_t* agg = d_scratch;
-        uint64_t* prefix = d_scratch + nt;
-        uint64_t* wagg = d_scratch + 2 * (uint64_t)nt;
-        uint16_t* masks = reinterpret_cast<uint16_t*>(d_scratch + 34 * (uint64_t)nt);
-        split_mask_kernel<PROBE><<<nt, 1024, 0, st>>>(d_buf, len, shift, splat, masks, (uint64_t)nt * kSplitTileChunks, agg,
-                                                     wagg, pr);
-        split_scan_kernel<<<1, 1024, 0, st>>>(agg, nt, prefix, d_total);
-        static int sms = 0;
-        if (!sms) {
-            int dev = 0;
-            cudaGetDevice(&dev);
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        }
-        const uint32_t grid = std::min<uint32_t>((nt + 3) / 4, (uint32_t)sms * 2);
-        split_emit_kernel<PROBE><<<grid, 1024, 0, st>>>(d_buf, len, shift, masks, prefix, wagg, nt, d_off, d_len, cap,
-                                                       d_n_out, pr);
-        return 3;
+    const uint32_t nt = (uint32_t)(((uint64_t)len + shift + kSplitTileChunks * 16 - 1) / (kSplitTileChunks * 16));
+    uint64_t* agg = d_scratch;
+    uint64_t* prefix = d_scratch + nt;
+    uint64_t* wagg = d_scratch + 2 * (uint64_t)nt;
+    uint16_t* masks = reinterpret_cast<uint16_t*>(d_scratch + 34 * (uint64_t)nt);
+    split_mask_kernel<PROBE><<<nt, 1024, 0, st>>>(d_buf, len, shift, splat, masks, (uint64_t)nt * kSplitTileChunks, agg,
+                                                 wagg, pr);
+    split_scan_kernel<<<1, 1024, 0, st>>>(agg, nt, prefix, d_total);
+    static int sms = 0;
+    if (!sms) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     }
-    static const int cfg = [] {
-        const char* e = getenv("LC_B200_SPLIT_TILE_KB"); // A/B knob: 16, 32 or 64 (descriptors are sized for 16)
-        int t = e ? atoi(e) : 64;
-        return (t == 16 || t == 32) ? t : 64;
-    }();
-    volatile uint64_t* desc = (volatile uint64_t*)d_desc;
-    const uint64_t tile_bytes = (uint64_t)cfg * 1024;
-    uint32_t ntiles = (uint32_t)((len + shift + tile_bytes - 1) / tile_bytes);
-    const bool wide = split_lookback_warps() > 1;
-    const int deep = split_lookback_warps() < 0 ? -split_lookback_warps() : 0;
-#define LC_SPLIT_LAUNCH(T, W)                                                                                          \
-    split_kernel<T, W, PROBE><<<ntiles, T, 0, st>>>(d_buf, len, shift, splat, d_off, d_len, cap, desc, d_ticket, ntiles, \
-                                                    d_n_out, d_total, pr)
-    if (const char* tf = getenv("LC_B200_SPLIT_TRACE")) { // debug: per-tile phase timestamps -> file (blocks the stream)
-        uint64_t* d_tr = nullptr;
-        cudaMalloc(&d_tr, (size_t)ntiles * 64);
-        cudaMemsetAsync(d_tr, 0, (size_t)ntiles * 64, st);
-        split_kernel<1024, 1, PROBE, true><<<ntiles, 1024, 0, st>>>(d_buf, len, shift, splat, d_off, d_len, cap, desc,
-                                                                    d_ticket, ntiles, d_n_out, d_total, pr, d_tr);
-        std::vector<uint64_t> h((size_t)ntiles * 8);
-        cudaStreamSynchronize(st);
-        cudaMemcpy(h.data(), d_tr, h.size() * 8, cudaMemcpyDeviceToHost);
-        cudaFree(d_tr);
-        if (FILE* f = fopen(tf, "wb")) {
-            fwrite(h.data(), 8, h.size(), f);
-            fclose(f);
-        }
-        return 1;
-    }
-    if (cfg == 64) {
-        if (wide)
-            LC_SPLIT_LAUNCH(1024, 4);
-        else if (deep == 8)
-            LC_SPLIT_LAUNCH(1024, -8);
-        else
-            LC_SPLIT_LAUNCH(1024, 1);
-    } else if (cfg == 32) {
-        LC_SPLIT_LAUNCH(512, 1);
-    } else {
-        if (wide)
-            LC_SPLIT_LAUNCH(256, 4);
-        else
-            LC_SPLIT_LAUNCH(256, 1);
-    }
-#undef LC_SPLIT_LAUNCH
-    return 1;
+    const uint32_t grid = std::min<uint32_t>((nt + 3) / 4, (uint32_t)sms * 2);
+    split_emit_kernel<PROBE><<<grid, 1024, 0, st>>>(d_buf, len, shift, masks, prefix, wagg, nt, d_off, d_len, cap,
+                                                   d_n_out, pr);
+    return 3;
 }
 
 int launch_split(const uint8_t* d_buf, uint32_t len, uint8_t split_char, uint32_t* d_off, uint32_t* d_len,
-                 uint32_t cap, uint64_t* d_desc, uint32_t* d_ticket, uint32_t* d_n_out, unsigned long long* d_total,
-                 uint64_t* d_scratch, cudaStream_t st) {
+                 uint32_t cap, uint32_t* d_n_out, unsigned long long* d_total, uint64_t* d_scratch, cudaStream_t st) {
     SplitProbe pr;
     memset(&pr, 0, sizeof pr);
-    return launch_split_impl<false>(d_buf, len, split_char, d_off, d_len, cap, d_desc, d_ticket, d_n_out, d_total,
-                                    d_scratch, pr, st);
+    return launch_split_impl<false>(d_buf, len, split_char, d_off, d_len, cap, d_n_out, d_total, d_scratch, pr, st);
 }
 
 int launch_split_probe(const MlConfig& cfg, const uint8_t* d_buf, uint32_t len, uint32_t* d_off, uint32_t* d_len,
-                       uint8_t* d_flags, uint32_t cap, uint64_t* d_desc, uint32_t* d_ticket, uint32_t* d_n_out,
-                       unsigned long long* d_total, uint64_t* d_scratch, cudaStream_t st) {
+                       uint8_t* d_flags, uint32_t cap, uint32_t* d_n_out, unsigned long long* d_total,
+                       uint64_t* d_scratch, cudaStream_t st) {
     SplitProbe pr;
     memset(&pr, 0, sizeof pr);
     pr.blob[0] = cfg.blob_start;
@@ -863,8 +590,7 @@ int launch_split_probe(const MlConfig& cfg, const uint8_t* d_buf, uint32_t len, 
     }
     pr.empty_flags = cfg.empty_flags;
     pr.flags = d_flags;
-    return launch_split_impl<true>(d_buf, len, '\n', d_off, d_len, cap, d_desc, d_ticket, d_n_out, d_total, d_scratch,
-                                   pr, st);
+    return launch_split_impl<true>(d_buf, len, '\n', d_off, d_len, cap, d_n_out, d_total, d_scratch, pr, st);
 }
 
 // ================================================================================================ sums
@@ -1823,206 +1549,7 @@ int launch_regex_fast2(const void* d_blob, uint32_t blob_bytes, bool multi, bool
 //   bytes 2,3 of e -> up to two predicated 16-bit STS into the thread's register file in shared memory
 // The per-line state is the register file alone (2 * groups + spares halfwords), so all 32 warps stay resident
 // whatever the line length, and the input is read exactly once.
-struct TdfaDev {
-    const uint8_t* cls;
-    const uint8_t* t2;
-    uint32_t row_bytes, ncls;
-};
-
-#define LCT_PAIR(X, HI, POS)                                                                                           \
-    {                                                                                                                  \
-        const uint32_t b0 = __byte_perm((X), 0, (HI) ? 0x4442 : 0x4440), b1 = __byte_perm((X), 0, (HI) ? 0x4443 : 0x4441); \
-        const uint32_t c0 = t.cls[b0], c1 = t.cls[b1];                                                                 \
-        const uint32_t prow = row;                                                                                     \
-        const uint32_t e = *reinterpret_cast<const uint32_t*>(t.t2 + row + ((c0 * t.ncls + c1) << 2));                \
-        row = e & 0xFFFFu;                                                                                             \
-        const uint32_t sa = (e >> 16) & 0x7Fu, sb = e >> 24;                                                           \
-        if (sa)                                                                                                        \
-            *reinterpret_cast<uint16_t*>(regs_m2 + sa) = (uint16_t)(POS);                                              \
-        if (sb)                                                                                                        \
-            *reinterpret_cast<uint16_t*>(regs_m2 + sb) = (uint16_t)((POS) + 1);                                        \
-        if (SLOW && (e & LC_TDFA_SLOW)) {                                                                              \
-            uint16_t* rg = reinterpret_cast<uint16_t*>(regs_m2 + 2);                                                   \
-            const uint32_t s1 = lc_tdfa_single(v, prow / t.row_bytes, b0, (POS), rg);                                  \
-            row = lc_tdfa_single(v, s1, b1, (POS) + 1, rg) * t.row_bytes;                                              \
-        }                                                                                                              \
-    }
-
-// One 16-byte chunk: the byte pairs at virtual positions [lo, lo + 16) restricted to [qlo, Qe).
-template <bool SLOW>
-__device__ __forceinline__ void tdfa_chunk(const LcTdfaView& v, const TdfaDev& t, const uint4 vv, uint32_t lo,
-                                           uint32_t mis, uint32_t qlo, uint32_t Qe, uint32_t& row, uint8_t* regs_m2) {
-    const uint32_t pos0 = lo - mis;
-    if (lo >= qlo && lo + 16 <= Qe) {
-        LCT_PAIR(vv.x, 0, pos0 + 0)
-        LCT_PAIR(vv.x, 1, pos0 + 2)
-        LCT_PAIR(vv.y, 0, pos0 + 4)
-        LCT_PAIR(vv.y, 1, pos0 + 6)
-        LCT_PAIR(vv.z, 0, pos0 + 8)
-        LCT_PAIR(vv.z, 1, pos0 + 10)
-        LCT_PAIR(vv.w, 0, pos0 + 12)
-        LCT_PAIR(vv.w, 1, pos0 + 14)
-    } else {
-        const uint32_t wd[4] = {vv.x, vv.y, vv.z, vv.w};
-#pragma unroll
-        for (int pi = 0; pi < 8; ++pi) {
-            const uint32_t q = lo + 2 * pi;
-            if (q >= qlo && q < Qe)
-                LCT_PAIR(wd[pi >> 1], pi & 1, q - mis)
-        }
-    }
-}
-
-template <bool SLOW>
-__device__ __forceinline__ bool tdfa_event(const LcTdfaView& v, const TdfaDev& t, const uint8_t* __restrict__ s,
-                                           const uint4* __restrict__ chunks, uint32_t mis, uint32_t n,
-                                           uint8_t* regs_m2) {
-    const uint32_t Q = n + mis;
-    const uint32_t qlo = mis + (mis & 1); // first even virtual position whose pair lies inside the event
-    const uint32_t Qe = Q & ~1u;          // pairs cover [qlo, Qe)
-    uint16_t* rg = reinterpret_cast<uint16_t*>(regs_m2 + 2);
-    uint32_t st = v.h->start;
-    if ((mis & 1) && n) // odd first byte: single step
-        st = lc_tdfa_single(v, st, s[0], 0, rg);
-    uint32_t row = st * t.row_bytes;
-    if (Qe > qlo) {
-        const int c_lo = (int)(qlo >> 4), c_hi = (int)((Qe - 1) >> 4);
-        uint4 nxt = __ldg(chunks + c_lo);
-        for (int qc = c_lo; qc <= c_hi; ++qc) {
-            const uint4 vv = nxt;
-            if (qc < c_hi)
-                nxt = __ldg(chunks + qc + 1);
-            tdfa_chunk<SLOW>(v, t, vv, (uint32_t)qc * 16, mis, qlo, Qe, row, regs_m2);
-            if (row == 0)
-                return false;
-        }
-    }
-    st = row / t.row_bytes;
-    if ((Q & 1) && Q - 1 >= qlo) // odd last byte
-        st = lc_tdfa_single(v, st, s[n - 1], n - 1, rg);
-    const uint32_t fin = v.eof[st];
-    if (fin == LC_NONE_ENTRY)
-        return false;
-    lc_tdfa_run_ops(v, fin, n, rg);
-    return true;
-}
-
-template <bool SLOW>
-__global__ void __launch_bounds__(1024, 1)
-    regex_tdfa_kernel(const uint4* __restrict__ blob, uint32_t blob_bytes, const uint8_t* __restrict__ base,
-                      const uint32_t* __restrict__ ev_off, const uint32_t* __restrict__ ev_len, uint64_t n,
-                      uint32_t nkeys, uint8_t* __restrict__ status, uint32_t* __restrict__ cap_off,
-                      uint32_t* __restrict__ cap_len, uint32_t reg_pitch /* halfwords */,
-                      unsigned long long* next_batch, const uint32_t* __restrict__ order) {
-    extern __shared__ uint4 smem[];
-    for (uint32_t k = threadIdx.x; k < blob_bytes / 16; k += blockDim.x)
-        smem[k] = __ldg(blob + k);
-    __syncthreads();
-    const LcTdfaView v = lc_tdfa_view(smem);
-    TdfaDev t;
-    t.cls = v.cls;
-    t.t2 = v.t2;
-    t.ncls = v.h->ncls;
-    t.row_bytes = v.h->row_bytes;
-    const uint32_t G = v.h->ngroups;
-    // shared memory: [blob][register files: threads x reg_pitch halfwords]
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    uint16_t* wregs = reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(smem) + blob_bytes) +
-                      (size_t)wid * 32 * reg_pitch; // this warp's 32 register files
-    uint16_t* regs = wregs + (size_t)lane * reg_pitch;
-    uint8_t* regs_m2 = reinterpret_cast<uint8_t*>(regs) - 2;
-    const bool bool_only = cap_off == nullptr; // lc_regex_match: status[i] = 1 match / 0 no match, no captures
-    for (;;) {
-        unsigned long long batch = 0;
-        if (lane == 0)
-            batch = atomicAdd(next_batch, 32ull);
-        batch = __shfl_sync(0xFFFFFFFFu, batch, 0);
-        if (batch >= n)
-            break;
-        const bool valid = batch + lane < n;
-        const uint64_t i = valid ? (order ? order[batch + lane] : batch + lane) : 0;
-        uint32_t off = 0, len = 0;
-        uint32_t st = 1;
-        if (valid) {
-            off = ev_off[i];
-            len = ev_len[i];
-            for (uint32_t k = 0; k < G; ++k)
-                reinterpret_cast<uint32_t*>(regs)[k] = 0xFFFFFFFFu; // home registers = LC_SLOT16_UNSET
-            const uint8_t* s = base + off;
-            const uint64_t a16 = (uint64_t)(uintptr_t)s;
-            const uint32_t mis16 = (uint32_t)(a16 & 15u);
-            const uint4* chunks = reinterpret_cast<const uint4*>(a16 - mis16);
-            const bool ok = tdfa_event<SLOW>(v, t, s, chunks, mis16, len, regs_m2);
-            st = ok ? (G + 1 <= nkeys ? 2 : 0) : 1;
-            status[i] = bool_only ? (ok ? 1 : 0) : (uint8_t)st;
-        }
-        if (bool_only || G == 0)
-            continue;
-        if (order == nullptr) {
-            // coalesced result rows: element j of the batch's [32][G] tables is produced by lane j % 32 straight
-            // from the owning line's register file (one 32-bit LDS = begin | end << 16)
-            __syncwarp();
-            const uint64_t left = n - batch;
-            const uint32_t total = (uint32_t)(left < 32 ? left : 32) * G;
-            uint32_t* go = cap_off + batch * G;
-            uint32_t* gl = cap_len + batch * G;
-            for (uint32_t j0 = 0; j0 < total; j0 += 32) {
-                const uint32_t j = j0 + lane;
-                const uint32_t line = j < total ? j / G : 0, g = j - line * G;
-                const uint32_t l_off = __shfl_sync(0xFFFFFFFFu, off, line);
-                const uint32_t l_len = __shfl_sync(0xFFFFFFFFu, len, line);
-                const uint32_t l_st = __shfl_sync(0xFFFFFFFFu, st, line);
-                if (j < total) {
-                    uint32_t o = 0, l = 0;
-                    if (l_st == 0) {
-                        const uint32_t be = reinterpret_cast<const uint32_t*>(wregs + (size_t)line * reg_pitch)[g];
-                        const uint32_t b = be & 0xFFFFu, en = be >> 16;
-                        if (b == LC_SLOT16_UNSET || en == LC_SLOT16_UNSET || en < b) {
-                            o = l_off + l_len;
-                        } else {
-                            o = l_off + b;
-                            l = en - b;
-                        }
-                    }
-                    go[j] = o;
-                    gl[j] = l;
-                }
-            }
-            __syncwarp();
-        } else if (valid) {
-            uint32_t* co = cap_off + i * G;
-            uint32_t* cl = cap_len + i * G;
-            for (uint32_t g = 0; g < G; ++g) {
-                uint32_t o = 0, l = 0;
-                if (st == 0) {
-                    lc_slots16_to_cap(regs, g, len, &o, &l);
-                    o += off;
-                }
-                co[g] = o;
-                cl[g] = l;
-            }
-        }
-    }
-}
-
-int launch_regex_tdfa(const void* d_blob, uint32_t blob_bytes, bool slow, uint32_t nregs, const uint8_t* d_base,
-                      const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, uint32_t nkeys,
-                      uint8_t* d_status, uint32_t* d_cap_off, uint32_t* d_cap_len, uint32_t threads, uint32_t grid,
-                      unsigned long long* d_next_batch, const uint32_t* d_order, cudaStream_t st) {
-    if (!n)
-        return 0;
-    const uint32_t reg_pitch = tdfa_reg_pitch(nregs);
-    size_t smem = tdfa_smem_bytes(blob_bytes, nregs, threads);
-    auto k = slow ? regex_tdfa_kernel<true> : regex_tdfa_kernel<false>;
-    cudaError_t er = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (er != cudaSuccess)
-        return (int)er;
-    k<<<grid, threads, smem, st>>>((const uint4*)d_blob, blob_bytes, d_base, d_ev_off, d_ev_len, n, nkeys, d_status,
-                                   d_cap_off, d_cap_len, reg_pitch, d_next_batch, d_order);
-    return (int)cudaGetLastError();
-}
-
-// ---- staged single-pass kernel: the same automaton as regex_tdfa_kernel, fed through shared memory -----------
+// ---- staged input: the automaton fed through shared memory -----------------------------------------------------
 // Why: with one line per lane, a per-lane 16-byte LDG touches 32 different 128-byte lines, i.e. 32 L1 tag
 // wavefronts for 512 bytes -- measured to cost more than the automaton's own look-ups.  Here the warp fetches its
 // 32 lines COOPERATIVELY: one cp.async (LDGSTS) instruction moves 4 full 128-byte lines (8 lanes x 16 B each, 4
@@ -2070,9 +1597,6 @@ __device__ __forceinline__ void sts_u16(uint32_t a, uint32_t v) {
 __device__ __forceinline__ void sts_u64(uint32_t a, uint32_t x, uint32_t y) {
     asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(a), "r"(x), "r"(y) : "memory");
 }
-__device__ __forceinline__ void sts_u128(uint32_t a, const uint4& v) {
-    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
 __device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
@@ -2098,22 +1622,16 @@ struct TdfaAbs {
 // one LEA.HI -- (entry >> 16) + index -- instead of a mask and an add, one instruction less on the dependent chain of
 // every pair: PRMT PRMT LDS.U8 LDS.U8 IMAD LEA.HI LDS + two predicated STS.U16 for capture boundaries.
 // ROWX = the address of the current row: `row` for the first pair of a chunk, (e_prev >> 16) afterwards.
-// UNC (A/B knob LC_B200_TDFA_STORE=uncond): both boundary stores are issued unconditionally (no-op slot at offset 0).
 #define LCS_PAIR(ROWX, X, HI, POS)                                                                                     \
     {                                                                                                                  \
         const uint32_t c0 = lds_u8(__byte_perm((X), t.cls, (HI) ? 0x7652 : 0x7650));                                   \
         const uint32_t c1 = lds_u8(__byte_perm((X), t.cls, (HI) ? 0x7653 : 0x7651));                                   \
         const uint32_t e = lds_u32((ROWX) + (c0 * t.ncls + c1));                                                       \
-        if (UNC) {                                                                                                     \
-            sts_u16(regs_m2 + (e & 0x7Fu), (POS));                                                                     \
-            sts_u16(regs_m2 + ((e >> 8) & 0x7Fu), (POS) + 1);                                                          \
-        } else {                                                                                                       \
-            const uint32_t sa = e & 0x7Fu, sb = e & 0x7F00u;                                                           \
-            if (sa)                                                                                                    \
-                sts_u16(regs_m2 + sa, (POS));                                                                          \
-            if (sb)                                                                                                    \
-                sts_u16(regs_m2 + (sb >> 8), (POS) + 1);                                                               \
-        }                                                                                                              \
+        const uint32_t sa = e & 0x7Fu, sb = e & 0x7F00u;                                                               \
+        if (sa)                                                                                                        \
+            sts_u16(regs_m2 + sa, (POS));                                                                              \
+        if (sb)                                                                                                        \
+            sts_u16(regs_m2 + (sb >> 8), (POS) + 1);                                                                   \
         e_prev = e;                                                                                                    \
     }
 
@@ -2196,8 +1714,8 @@ struct TdfaLoader {
     }
 };
 
-template <bool SLOW, bool UNC, class Fetch>
-__device__ __forceinline__ uint32_t tdfa_walk_lines(const LcTdfaView& v, const TdfaAbs& t, Fetch& L,
+template <bool SLOW>
+__device__ __forceinline__ uint32_t tdfa_walk_lines(const LcTdfaView& v, const TdfaAbs& t, TdfaLoader& L,
                                                     uint32_t dead, uint32_t sink, uint32_t row, uint32_t len,
                                                     uint32_t mis, uint32_t max_nch, uint32_t regs_m2, uint16_t* rg) {
     // frame of the line: byte j of the line sits at frame index mis + j; pairs cover the even-aligned [qlo, Qe)
@@ -2254,88 +1772,6 @@ __device__ __forceinline__ uint32_t tdfa_walk_lines(const LcTdfaView& v, const T
     return row;
 }
 
-// ---- software-pipelined tile fill (A/B: LC_B200_TDFA_FETCH=prefetch) ------------------------------------------------
-// The cp.async fill above costs 32 shared-memory wavefronts per instruction (LDGSTS lands one 16-byte wavefront per
-// lane): ~500 of the ~1270 wavefronts a 32-line batch of 256-byte lines needs, on a kernel whose l1tex pipe is the
-// busiest unit.  LDG.128 + STS.128 needs 4 per instruction, but holding a whole stage in registers spills and the loads stall
-// the warp.  Here a stage is 4 chunks (64 bytes per line) and the tile is two 2 KB buffers: while the lanes walk
-// chunk k of stage s out of one buffer, slice k of stage s + 1 travels global -> ONE uint4 register -> the other
-// buffer (LDG before the chunk's work, STS.128 after it), so one load is in flight per lane for the time a chunk takes
-// and nobody waits for it.  Loader role: lane -> chunk column (lane & 3) of line (lane >> 2) * 4 + k; the slot of
-// (chunk q, line) is q * 512 + ((line ^ q) << 4): conflict-free for the 8-lane STS.128 / LDS.128 phases.
-template <bool SLOW, bool UNC>
-__device__ __forceinline__ uint32_t tdfa_walk_lines_pf(const LcTdfaView& v, const TdfaAbs& t, const TdfaLoader& L,
-                                                       uint32_t info_abs, uint32_t dead, uint32_t sink, uint32_t row,
-                                                       uint32_t len, uint32_t mis, uint32_t max_nch, uint32_t regs_m2,
-                                                       uint16_t* rg) {
-    const uint32_t Q = len + mis, qlo = mis + (mis & 1), Qe = Q & ~1u;
-    const uint32_t kf_lo = (qlo + 15) >> 4, kf_hi = Qe >> 4; // fully paired chunks: [kf_lo, kf_hi)
-    const uint32_t k_tail = len ? (Q - 1) >> 4 : 0;
-    const bool has_head = len && !(kf_lo == 0 && kf_hi > 0);
-    const bool has_tail = len && k_tail >= kf_hi && !(has_head && k_tail == 0);
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t pq = lane & 3, pL0 = (lane >> 2) * 4;
-    const uint32_t rd16 = L.rd_lane16;
-    if (max_nch == 0)
-        return row;
-    // prologue: stage 0 into buffer 0
-#pragma unroll
-    for (uint32_t k = 0; k < 4; ++k) {
-        const uint32_t line = pL0 + k;
-        const uint2 inf = lds_u64_v(info_abs + line * 8);
-        if (pq < inf.y)
-            sts_u128(L.tile_abs + (pq << 9) + ((line ^ pq) << 4), __ldg(L.gbase16 + inf.x + pq));
-    }
-    uint32_t buf = 0;
-    for (uint32_t s0 = 0; s0 < max_nch; s0 += 4, buf ^= 2048u) {
-        __syncwarp(); // the buffer of this stage is complete, the other one is free
-        const uint32_t cur = L.tile_abs + buf, nxt = L.tile_abs + (buf ^ 2048u);
-        const bool more = s0 + 4 < max_nch;
-#pragma unroll
-        for (uint32_t kk = 0; kk < 4; ++kk) {
-            // ---- slice kk of the next stage: issue the load
-            uint4 pf = make_uint4(0, 0, 0, 0);
-            bool pf_on = false;
-            const uint32_t pline = pL0 + kk;
-            if (more) {
-                const uint2 inf = lds_u64_v(info_abs + pline * 8);
-                pf_on = s0 + 4 + pq < inf.y;
-                if (pf_on)
-                    pf = __ldg(L.gbase16 + inf.x + s0 + 4 + pq);
-            }
-            // ---- this lane's own line: chunk k of the current stage
-            const uint32_t k = s0 + kk;
-            if (row != dead && len) {
-                const uint32_t caddr = cur + (kk << 9) + (rd16 ^ (kk << 4));
-                if (k >= kf_lo && k < kf_hi) {
-                    const uint4 vv = lds_u128_v(caddr);
-                    const uint32_t pos0 = k * 16 - mis;
-                    const uint32_t row_in = row;
-                    uint32_t e_prev;
-                    LCS_PAIR(row, vv.x, 0, pos0 + 0)
-                    LCS_PAIR(e_prev >> 16, vv.x, 1, pos0 + 2)
-                    LCS_PAIR(e_prev >> 16, vv.y, 0, pos0 + 4)
-                    LCS_PAIR(e_prev >> 16, vv.y, 1, pos0 + 6)
-                    LCS_PAIR(e_prev >> 16, vv.z, 0, pos0 + 8)
-                    LCS_PAIR(e_prev >> 16, vv.z, 1, pos0 + 10)
-                    LCS_PAIR(e_prev >> 16, vv.w, 0, pos0 + 12)
-                    LCS_PAIR(e_prev >> 16, vv.w, 1, pos0 + 14)
-                    row = e_prev >> 16;
-                    if (SLOW && row == sink)
-                        row = t.t2 + t.row_bytes * tdfa_chunk_slow(v, __umulhi(row_in - t.t2, t.inv_row), vv, pos0, rg);
-                } else if ((k == 0 && has_head) || (k == k_tail && has_tail)) {
-                    row = tdfa_partial_chunk(v, t, row, caddr, k * 16, mis, len, regs_m2, rg, sink);
-                }
-            }
-            // ---- land the prefetched slice in the other buffer
-            if (pf_on)
-                sts_u128(nxt + (pq << 9) + ((pline ^ pq) << 4), pf);
-        }
-    }
-    __syncwarp();
-    return row;
-}
-
 // Stages one automaton: class table at the 256-byte aligned shared address cls_abs, blob right behind it; pair-table
 // entries are rebased so that their low 16 bits are the ABSOLUTE shared address of the next row.  All threads call;
 // the caller synchronises afterwards.
@@ -2362,7 +1798,7 @@ __device__ __forceinline__ void tdfa_stage_blob(uint8_t* g_cls, uint32_t cls_abs
     }
 }
 
-template <bool SLOW, bool UNC, bool PF>
+template <bool SLOW>
 __global__ void __launch_bounds__(1024, 1)
     regex_tdfa_staged_kernel(const uint4* __restrict__ blob, uint32_t blob_bytes, const uint8_t* __restrict__ base,
                              const uint32_t* __restrict__ ev_off, const uint32_t* __restrict__ ev_len,
@@ -2390,7 +1826,7 @@ __global__ void __launch_bounds__(1024, 1)
     const uint32_t G = v.h->ngroups;
     const uint32_t invG = G ? 0xFFFFFFFFu / G + 1 : 0; // umulhi(j, invG) == j / G for j < 65536
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-    uint8_t* g_regs0 = reinterpret_cast<uint8_t*>(g_blob) + blob_bytes + 16; // (+16: no-op slot of the first thread)
+    uint8_t* g_regs0 = reinterpret_cast<uint8_t*>(g_blob) + blob_bytes + 16; // (+16: spare slot)
     uint16_t* wregs = reinterpret_cast<uint16_t*>(g_regs0) + (size_t)wid * 32 * reg_pitch;
     uint16_t* regs = wregs + (size_t)lane * reg_pitch;
     const uint32_t regs_abs = (uint32_t)__cvta_generic_to_shared(regs);
@@ -2448,10 +1884,7 @@ __global__ void __launch_bounds__(1024, 1)
         const uint32_t max_nch = __reduce_max_sync(0xFFFFFFFFu, nch);
         uint32_t row = t.t2 + v.h->start * t.row_bytes;
         __syncwarp();
-        if (PF)
-            row = tdfa_walk_lines_pf<SLOW, UNC>(v, t, L, info_abs, dead, sink, row, len, mis, max_nch, regs_m2, rg);
-        else
-            row = tdfa_walk_lines<SLOW, UNC>(v, t, L, dead, sink, row, len, mis, max_nch, regs_m2, rg);
+        row = tdfa_walk_lines<SLOW>(v, t, L, dead, sink, row, len, mis, max_nch, regs_m2, rg);
         uint32_t st = 1;
         if (valid) {
             bool ok = false;
@@ -2521,286 +1954,13 @@ int launch_regex_tdfa_staged(const void* d_blob, uint32_t blob_bytes, bool slow,
         return 0;
     const uint32_t reg_pitch = tdfa_reg_pitch(nregs);
     size_t smem = tdfa_staged_smem_bytes(blob_bytes, nregs, threads);
-    static const bool unc_env = [] {
-        const char* e = getenv("LC_B200_TDFA_STORE");
-        return e && !strcmp(e, "uncond");
-    }();
-    const bool unc = unc_env && reg_pitch > nregs; // the no-op slot is the spare halfword of the neighbouring file
-    static const bool pf = [] {
-        const char* e = getenv("LC_B200_TDFA_FETCH");
-        return e && !strcmp(e, "prefetch");
-    }();
-    auto k = pf ? (slow ? regex_tdfa_staged_kernel<true, false, true> : regex_tdfa_staged_kernel<false, false, true>)
-                : (slow ? (unc ? regex_tdfa_staged_kernel<true, true, false> : regex_tdfa_staged_kernel<true, false, false>)
-                        : (unc ? regex_tdfa_staged_kernel<false, true, false>
-                               : regex_tdfa_staged_kernel<false, false, false>));
+    auto k = slow ? regex_tdfa_staged_kernel<true> : regex_tdfa_staged_kernel<false>;
     cudaError_t er = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (er != cudaSuccess)
         return (int)er;
     k<<<grid, threads, smem, st>>>((const uint4*)d_blob, blob_bytes, d_base, d_ev_off, d_ev_len, ev_stride, n, nkeys,
                                    d_status, d_cap_off, d_cap_len, reg_pitch, d_next_batch, d_overflow, d_order,
                                    d_order_flag);
-    return (int)cudaGetLastError();
-}
-
-// ---- producer / consumer variant of the staged kernel (A/B: LC_B200_REGEX_KERNEL=tdfa_pc) ------------------------------
-// The staged kernel's tile fill is its single largest shared-memory cost: LDGSTS writes one 16-byte wavefront per lane
-// (32 per instruction, ~500 of the ~1270 wavefronts a 32-line batch of 256-byte lines costs).  Here the
-// first NP warps of the block only move data: a producer warp takes a consumer's request (stage number + the 32 lines'
-// chunk lists in the consumer's info slots), pulls the 8 x 512 bytes with LDG.128 into registers and writes them with
-// STS.128 -- 4 wavefronts per instruction in the same [chunk][line ^ chunk] layout -- then completes the consumer's
-// `full` mbarrier.  Consumers never touch global input memory and never execute staging instructions; they run the
-// automaton exactly as in the staged kernel (shared tdfa_walk_lines).  Requests travel through one word per consumer
-// and a per-producer bit mask; an idle producer naps (nanosleep) instead of spinning on issue slots.
-constexpr uint32_t kPcProducers = 4;
-constexpr uint32_t kPcExit = 0xFFFFFFFFu;
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-                     : "=r"(ok)
-                     : "r"(bar), "r"(parity)
-                     : "memory");
-    } while (!ok);
-}
-
-struct TdfaPcFetch {
-    uint32_t tile_abs;   // this consumer's 4 KB tile
-    uint32_t rd_lane16;  // lane << 4
-    uint32_t req_abs;    // request word of this consumer (stage number / kPcExit)
-    uint32_t* req_mask;  // request mask of the producer serving this consumer
-    uint32_t req_bit;
-    uint32_t full_bar;   // mbarrier the producer completes when the tile is filled
-    uint32_t parity;
-    __device__ __forceinline__ void stage(uint32_t s0) {
-        // (all lanes are past their reads of the tile and their writes of the info slots: the walk ends every stage with
-        // __syncwarp, and the batch set-up synchronises before the walk)
-        if ((threadIdx.x & 31) == 0) {
-            asm volatile("st.volatile.shared.u32 [%0], %1;" ::"r"(req_abs), "r"(s0) : "memory");
-            __threadfence_block();
-            atomicOr(req_mask, req_bit);
-        }
-        mbar_wait(full_bar, parity);
-        parity ^= 1u;
-    }
-};
-
-template <bool SLOW, bool UNC>
-__global__ void __launch_bounds__(1024, 1)
-    regex_tdfa_pc_kernel(const uint4* __restrict__ blob, uint32_t blob_bytes, const uint8_t* __restrict__ base,
-                         const uint32_t* __restrict__ ev_off, const uint32_t* __restrict__ ev_len, uint32_t ev_stride,
-                         uint64_t n, uint32_t nkeys, uint8_t* __restrict__ status, uint32_t* __restrict__ cap_off,
-                         uint32_t* __restrict__ cap_len, uint32_t reg_pitch /* halfwords */,
-                         unsigned long long* next_batch, uint32_t* overflow) {
-    extern __shared__ uint4 smem[];
-    // carve-out: [pad][class table][blob][16 B][register files: consumers][line info: consumers x 256 B]
-    // [tiles: consumers x 4 KB][full barriers: consumers x 8 B][request words: consumers x 4 B][request masks: NP x 4 B]
-    const uint32_t s0abs = (uint32_t)__cvta_generic_to_shared(smem);
-    const uint32_t cls_abs = (s0abs + 255u) & ~255u;
-    uint8_t* g_cls = reinterpret_cast<uint8_t*>(smem) + (cls_abs - s0abs);
-    uint4* g_blob = reinterpret_cast<uint4*>(g_cls + 256);
-    tdfa_stage_blob(g_cls, cls_abs, blob, blob_bytes);
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-    const uint32_t NC = nwarps - kPcProducers; // consumer warps
-    uint8_t* g_regs0 = reinterpret_cast<uint8_t*>(g_blob) + blob_bytes + 16;
-    uint8_t* g_aux = g_regs0 + (size_t)NC * 32 * reg_pitch * 2;
-    const uint32_t aux_abs = (uint32_t)__cvta_generic_to_shared(g_aux);
-    const uint32_t tiles_abs = aux_abs + NC * 256;
-    const uint32_t bars_abs = tiles_abs + NC * (LCT_STAGE_CHUNKS * 512);
-    const uint32_t reqs_abs = bars_abs + NC * 8;
-    uint32_t* g_masks = reinterpret_cast<uint32_t*>(g_aux + (size_t)NC * 256 + (size_t)NC * (LCT_STAGE_CHUNKS * 512) +
-                                                    (size_t)NC * 8 + (size_t)NC * 4);
-    if (threadIdx.x < NC)
-        mbar_init(bars_abs + threadIdx.x * 8, 1);
-    if (threadIdx.x < kPcProducers)
-        g_masks[threadIdx.x] = 0;
-    __syncthreads();
-    const uint4* gbase16 = reinterpret_cast<const uint4*>((uintptr_t)base & ~(uintptr_t)15);
-
-    if (wid < kPcProducers) {
-        // ------------------------------------------------------------------------------------------------ producer
-        uint32_t live = 0;
-        for (uint32_t c = wid; c < NC; c += kPcProducers)
-            ++live;
-        const uint32_t ld_q = lane & 7, ld_L0 = (lane >> 3) * 8;
-        while (live) {
-            uint32_t mask = 0;
-            if (lane == 0)
-                mask = atomicExch(&g_masks[wid], 0u);
-            mask = __shfl_sync(0xFFFFFFFFu, mask, 0);
-            if (!mask) {
-                __nanosleep(64);
-                continue;
-            }
-            __threadfence_block();
-            while (mask) {
-                const uint32_t b = __ffs((int)mask) - 1;
-                mask &= mask - 1;
-                const uint32_t c = b * kPcProducers + wid;
-                uint32_t s0;
-                asm volatile("ld.volatile.shared.u32 %0, [%1];" : "=r"(s0) : "r"(reqs_abs + c * 4) : "memory");
-                if (s0 == kPcExit) {
-                    --live;
-                    continue;
-                }
-                const uint32_t ld_info = aux_abs + c * 256 + ld_L0 * 8;
-                const uint32_t ld_dst = tiles_abs + c * (LCT_STAGE_CHUNKS * 512) + (ld_q << 9) + (ld_L0 << 4);
-                const uint32_t cidx = s0 + ld_q;
-                uint4 v[8];
-#pragma unroll
-                for (uint32_t r = 0; r < 8; ++r) {
-                    const uint2 inf = lds_u64_v(ld_info + r * 8);
-                    v[r] = make_uint4(0, 0, 0, 0);
-                    if (cidx < inf.y)
-                        v[r] = __ldg(gbase16 + inf.x + cidx);
-                }
-#pragma unroll
-                for (uint32_t r = 0; r < 8; ++r) {
-                    const uint2 inf = lds_u64_v(ld_info + r * 8);
-                    if (cidx < inf.y)
-                        sts_u128(ld_dst + ((r ^ ld_q) << 4), v[r]);
-                }
-                __syncwarp();
-                if (lane == 0)
-                    mbar_arrive(bars_abs + c * 8);
-            }
-        }
-        return;
-    }
-    // ---------------------------------------------------------------------------------------------------- consumer
-    const uint32_t ci = wid - kPcProducers;
-    const LcTdfaView v = lc_tdfa_view(g_blob);
-    TdfaAbs t;
-    t.cls = cls_abs;
-    t.t2 = cls_abs + 256 + v.h->off_t2;
-    t.ncls = v.h->ncls;
-    t.row_bytes = v.h->row_bytes;
-    t.inv_row = (uint32_t)((0x100000000ull + t.row_bytes - 1) / t.row_bytes);
-    t.skip = cls_abs + 256 + v.h->off_skip;
-    const uint32_t G = v.h->ngroups;
-    const uint32_t invG = G ? 0xFFFFFFFFu / G + 1 : 0;
-    uint16_t* wregs = reinterpret_cast<uint16_t*>(g_regs0) + (size_t)ci * 32 * reg_pitch;
-    uint16_t* regs = wregs + (size_t)lane * reg_pitch;
-    const uint32_t regs_abs = (uint32_t)__cvta_generic_to_shared(regs);
-    const uint32_t regs_m2 = regs_abs - 2;
-    const uint32_t info_abs = aux_abs + ci * 256;
-    sts_u64(info_abs + lane * 8, cls_abs, 0);
-    asm volatile("ld.volatile.shared.u32 %0, [%1];" : "=r"(t.cls) : "r"(info_abs + lane * 8) : "memory");
-    __syncwarp();
-    const uint32_t base_mis = (uint32_t)((uintptr_t)base & 15);
-    const bool bool_only = cap_off == nullptr;
-    const uint32_t dead = t.t2, sink = t.t2 + v.h->sink * t.row_bytes;
-    uint16_t* rg = regs;
-    TdfaPcFetch L;
-    L.tile_abs = tiles_abs + ci * (LCT_STAGE_CHUNKS * 512);
-    L.rd_lane16 = lane << 4;
-    L.req_abs = reqs_abs + ci * 4;
-    L.req_mask = &g_masks[ci % kPcProducers];
-    L.req_bit = 1u << (ci / kPcProducers);
-    L.full_bar = bars_abs + ci * 8;
-    L.parity = 0;
-    for (;;) {
-        unsigned long long batch = 0;
-        if (lane == 0)
-            batch = atomicAdd(next_batch, 32ull);
-        batch = __shfl_sync(0xFFFFFFFFu, batch, 0);
-        if (batch >= n)
-            break;
-        const bool valid = batch + lane < n;
-        const uint64_t i = batch + lane;
-        uint32_t off = 0, len = 0, mis = 0, nch = 0, g0 = 0;
-        if (valid) {
-            off = ev_off[i * ev_stride];
-            len = ev_len[i * ev_stride];
-            if (len >= 65535u) { // regex_tdfa_long_kernel redoes this event afterwards
-                atomicExch(overflow, 1u);
-                len = 0;
-            }
-            const uint64_t a = (uint64_t)base_mis + off;
-            mis = (uint32_t)(a & 15);
-            g0 = (uint32_t)(a >> 4);
-            nch = len ? (mis + len + 15) >> 4 : 0;
-            for (uint32_t k = 0; k < G; ++k)
-                reinterpret_cast<uint32_t*>(regs)[k] = 0xFFFFFFFFu;
-        }
-        sts_u64(info_abs + lane * 8, g0, nch);
-        const uint32_t max_nch = __reduce_max_sync(0xFFFFFFFFu, nch);
-        uint32_t row = t.t2 + v.h->start * t.row_bytes;
-        __syncwarp();
-        row = tdfa_walk_lines<SLOW, UNC>(v, t, L, dead, sink, row, len, mis, max_nch, regs_m2, rg);
-        uint32_t st = 1;
-        if (valid) {
-            bool ok = false;
-            const uint32_t fin = v.eof[__umulhi(row - t.t2, t.inv_row)];
-            if (fin != LC_NONE_ENTRY) {
-                lc_tdfa_run_ops(v, fin, len, rg);
-                ok = true;
-            }
-            st = ok ? (G + 1 <= nkeys ? 2 : 0) : 1;
-            status[i] = bool_only ? (ok ? 1 : 0) : (uint8_t)st;
-        }
-        if (bool_only || G == 0)
-            continue;
-        sts_u64(info_abs + lane * 8, off, st == 0 ? len : 0xFFFFFFFFu);
-        __syncwarp();
-        const uint64_t left = n - batch;
-        const uint32_t total = (uint32_t)(left < 32 ? left : 32) * G;
-        uint32_t* go = cap_off + batch * G + lane;
-        uint32_t* gl = cap_len + batch * G + lane;
-        const uint32_t wbase = regs_m2 + 2 - lane * reg_pitch * 2;
-        for (uint32_t j = lane; j < total; j += 32, go += 32, gl += 32) {
-            const uint32_t line = G == 1 ? j : __umulhi(j, invG), g = j - line * G;
-            const uint2 inf = lds_u64_v(info_abs + line * 8);
-            uint32_t o = 0, l = 0;
-            if (inf.y != 0xFFFFFFFFu) {
-                const uint32_t be = lds_u32_v(wbase + line * reg_pitch * 2 + g * 4);
-                const uint32_t b = be & 0xFFFFu, en = be >> 16;
-                if (b == LC_SLOT16_UNSET || en == LC_SLOT16_UNSET || en < b) {
-                    o = inf.x + inf.y;
-                } else {
-                    o = inf.x + b;
-                    l = en - b;
-                }
-            }
-            *go = o;
-            *gl = l;
-        }
-        __syncwarp();
-    }
-    if (lane == 0) { // tell the producer this consumer is done
-        asm volatile("st.volatile.shared.u32 [%0], %1;" ::"r"(L.req_abs), "r"(kPcExit) : "memory");
-        __threadfence_block();
-        atomicOr(L.req_mask, L.req_bit);
-    }
-}
-
-int launch_regex_tdfa_pc(const void* d_blob, uint32_t blob_bytes, bool slow, uint32_t nregs, const uint8_t* d_base,
-                         const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint32_t ev_stride, uint64_t n,
-                         uint32_t nkeys, uint8_t* d_status, uint32_t* d_cap_off, uint32_t* d_cap_len, uint32_t threads,
-                         uint32_t grid, unsigned long long* d_next_batch, uint32_t* d_overflow, cudaStream_t st) {
-    if (!n)
-        return 0;
-    const uint32_t reg_pitch = tdfa_reg_pitch(nregs);
-    size_t smem = tdfa_pc_smem_bytes(blob_bytes, nregs, threads);
-    static const bool unc_env = [] {
-        const char* e = getenv("LC_B200_TDFA_STORE");
-        return e && !strcmp(e, "uncond");
-    }();
-    const bool unc = unc_env && reg_pitch > nregs;
-    auto k = slow ? (unc ? regex_tdfa_pc_kernel<true, true> : regex_tdfa_pc_kernel<true, false>)
-                  : (unc ? regex_tdfa_pc_kernel<false, true> : regex_tdfa_pc_kernel<false, false>);
-    cudaError_t er = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (er != cudaSuccess)
-        return (int)er;
-    k<<<grid, threads, smem, st>>>((const uint4*)d_blob, blob_bytes, d_base, d_ev_off, d_ev_len, ev_stride, n, nkeys,
-                                   d_status, d_cap_off, d_cap_len, reg_pitch, d_next_batch, d_overflow);
     return (int)cudaGetLastError();
 }
 
@@ -2938,7 +2098,7 @@ __global__ void __launch_bounds__(1024, 1)
             const uint32_t max_nch = __reduce_max_sync(0xFFFFFFFFu, nch_p);
             uint32_t row = act ? start_row : dead;
             __syncwarp();
-            row = tdfa_walk_lines<SLOW, false>(v, t, L, dead, sink, row, len, mis, max_nch, regs_m2, regs);
+            row = tdfa_walk_lines<SLOW>(v, t, L, dead, sink, row, len, mis, max_nch, regs_m2, regs);
             if (act) {
                 const uint32_t fin = v.eof[__umulhi(row - t.t2, t.inv_row)];
                 if (fin != LC_NONE_ENTRY) {
@@ -3213,33 +2373,6 @@ void launch_prefix_match(const void* d_blob, const uint8_t* d_base, const uint32
 }
 
 // ================================================================================================ multiline
-__global__ void __launch_bounds__(128)
-    ml_probe_kernel(const void* __restrict__ bs, const void* __restrict__ bc, const void* __restrict__ be,
-                    const uint8_t* __restrict__ buf, const uint32_t* __restrict__ off, const uint32_t* __restrict__ len,
-                    uint64_t n, uint8_t* __restrict__ flags) {
-    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n)
-        return;
-    const uint8_t* s = buf + off[i];
-    uint32_t l = len[i];
-    uint8_t f = 0;
-    if (bs && lc_prefix_match(lc_view(bs), s, l))
-        f |= 1;
-    if (bc && lc_prefix_match(lc_view(bc), s, l))
-        f |= 2;
-    if (be && lc_prefix_match(lc_view(be), s, l))
-        f |= 4;
-    flags[i] = f;
-}
-
-void launch_ml_probe(const MlConfig& cfg, const uint8_t* d_buf, const uint32_t* d_off, const uint32_t* d_len,
-                     uint64_t n, uint8_t* d_flags, cudaStream_t st) {
-    if (!n)
-        return;
-    ml_probe_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(cfg.blob_start, cfg.blob_cont, cfg.blob_end, d_buf,
-                                                                  d_off, d_len, n, d_flags);
-}
-
 struct MlMode {
     bool S, C, E, discard;
 };
@@ -3384,83 +2517,6 @@ struct MlCountSink {
     }
 };
 
-template <int THREADS, int ITEMS>
-__global__ void __launch_bounds__(THREADS)
-    ml_state_kernel(MlMode m, const uint8_t* __restrict__ flags, const uint32_t* __restrict__ len, uint64_t n,
-                    uint32_t* __restrict__ state,
-                    uint32_t* __restrict__ cnt, volatile uint64_t* desc, uint32_t* ticket) {
-    __shared__ uint64_t s_scan[THREADS / 32 + 1];
-    __shared__ uint32_t s_tile;
-    __shared__ uint64_t s_prefix;
-    const int tid = threadIdx.x;
-    if (tid == 0)
-        s_tile = atomicAdd(ticket, 1u);
-    __syncthreads();
-    const uint32_t tile = s_tile;
-    const uint64_t base = (uint64_t)tile * THREADS * ITEMS + (uint64_t)tid * ITEMS;
-    // elements 0..n-1 are lines, element n is the virtual end-of-buffer (identity transition)
-    uint64_t el[ITEMS];
-    uint32_t fl[ITEMS];
-    uint64_t agg = OpMlState::identity();
-#pragma unroll
-    for (int k = 0; k < ITEMS; ++k) {
-        uint64_t j = base + k;
-        uint64_t e = OpMlState::identity();
-        fl[k] = 0;
-        if (j < n) {
-            fl[k] = flags[j];
-            uint32_t o0, b0, o1, b1;
-            ml_trans(m, fl[k], 0, o0, b0);
-            ml_trans(m, fl[k], 1, o1, b1);
-            uint32_t l0 = b0 ? (uint32_t)j + b0 : 0u; // (index + 1) of the opening line
-            uint32_t l1 = b1 ? (uint32_t)j + b1 : 0u;
-            e = OpMlState::make(o0, o1, l0, l1);
-        }
-        el[k] = e;
-        agg = OpMlState::combine(agg, e);
-    }
-    uint64_t tot;
-    uint64_t ex = block_exclusive_scan<OpMlState, THREADS>(agg, tot, s_scan);
-    if (tid < 32) {
-        uint64_t p = lookback<OpMlState>(desc, tile, tot);
-        if (tid == 0)
-            s_prefix = p;
-    }
-    __syncthreads();
-    uint64_t run = OpMlState::combine(s_prefix, ex);
-    // initial condition (:165-169): End-only mode starts partial with multiStartIndex = line 0
-    const uint32_t s0 = (!m.S && !m.C && m.E) ? 1u : 0u;
-    const uint32_t lb_init = s0 ? 1u : 0u;
-#pragma unroll
-    for (int k = 0; k < ITEMS; ++k) {
-        uint64_t j = base + k;
-        if (j <= n) {
-            uint32_t s_in = OpMlState::f(run, s0);
-            uint32_t lbp = OpMlState::lb(run, s0);
-            if (!lbp)
-                lbp = lb_init;
-            uint32_t lb = lbp ? lbp - 1 : 0u; // line index of multiStartIndex (valid only when s_in)
-            state[j] = (s_in << 31) | lb;
-            MlCountSink sink;
-            sink.discard = m.discard;
-            sink.len = len;
-            sink.n = (uint32_t)n;
-            ml_actions(m, fl[k], s_in, lb, (uint32_t)j, (uint32_t)n, sink);
-            cnt[j] = sink.cnt;
-        }
-        run = OpMlState::combine(run, el[k]);
-    }
-}
-
-void launch_ml_state(const MlConfig& cfg, const uint8_t* d_flags, const uint32_t* d_len, uint64_t n, uint32_t* d_state,
-                     uint32_t* d_cnt,
-                     uint64_t* d_desc, uint32_t* d_ticket, cudaStream_t st) {
-    MlMode m{cfg.blob_start != nullptr, cfg.blob_cont != nullptr, cfg.blob_end != nullptr, cfg.discard != 0};
-    uint32_t ntiles = scan_tiles(n + 1);
-    ml_state_kernel<kScanThreads, kScanItems>
-        <<<ntiles, kScanThreads, 0, st>>>(m, d_flags, d_len, n, d_state, d_cnt, (volatile uint64_t*)d_desc, d_ticket);
-}
-
 struct MlEmitSink {
     bool discard;
     const uint32_t* off;
@@ -3519,202 +2575,9 @@ struct MlEmitSink {
     }
 };
 
-__global__ void __launch_bounds__(128)
-    ml_emit_kernel(MlMode m, const uint8_t* __restrict__ flags, const uint32_t* __restrict__ off,
-                   const uint32_t* __restrict__ len, uint64_t n, uint32_t total_len, const uint32_t* __restrict__ state,
-                   const uint64_t* __restrict__ pos, uint32_t* __restrict__ out_off, uint32_t* __restrict__ out_len,
-                   uint8_t* __restrict__ out_flags, uint64_t cap, unsigned long long* counters) {
-    uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    uint32_t me = 0, ul = 0;
-    if (j <= n) {
-        uint32_t st = state[j];
-        MlEmitSink sink;
-        sink.discard = m.discard;
-        sink.off = off;
-        sink.len = len;
-        sink.total_len = total_len;
-        sink.out_off = out_off;
-        sink.out_len = out_len;
-        sink.out_flags = out_flags;
-        sink.cap = cap;
-        sink.pos = pos[j];
-        sink.n = (uint32_t)n;
-        // begin + content.size() == sourceVal.size() (:174); the end-of-buffer element always passes true
-        sink.is_last = (j == n) ? 1u : ((off[j] + len[j] == total_len) ? 1u : 0u);
-        ml_actions(m, j < n ? flags[j] : 0u, st >> 31, st & 0x7FFFFFFFu, (uint32_t)j, (uint32_t)n, sink);
-        me = sink.matched_events;
-        ul = sink.unmatch_lines;
-    }
-    // block reduction of the two counters
-    for (int d = 16; d; d >>= 1) {
-        me += __shfl_down_sync(0xFFFFFFFFu, me, d);
-        ul += __shfl_down_sync(0xFFFFFFFFu, ul, d);
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (me)
-            atomicAdd(&counters[0], (unsigned long long)me);
-        if (ul)
-            atomicAdd(&counters[1], (unsigned long long)ul);
-    }
-}
-
-void launch_ml_emit(const MlConfig& cfg, const uint8_t* d_flags, const uint32_t* d_off, const uint32_t* d_len,
-                    uint64_t n, uint32_t total_len, const uint32_t* d_state, const uint64_t* d_pos, uint32_t* d_out_off,
-                    uint32_t* d_out_len, uint8_t* d_out_flags, uint64_t cap, unsigned long long* d_counters,
-                    cudaStream_t st) {
-    MlMode m{cfg.blob_start != nullptr, cfg.blob_cont != nullptr, cfg.blob_end != nullptr, cfg.discard != 0};
-    ml_emit_kernel<<<(unsigned)((n + 1 + 127) / 128), 128, 0, st>>>(m, d_flags, d_off, d_len, n, total_len, d_state,
-                                                                    d_pos, d_out_off, d_out_len, d_out_flags, cap,
-                                                                    d_counters);
-}
-
-// ---- fused back half of the multiline split: state scan -> output counts -> output slots -> emission in ONE kernel.
-// Two chained decoupled look-backs per tile (the 2-state transition functions, then the event counts); the per-line
-// state / count / slot arrays of the three-kernel formulation never exist.  The number of lines is read from device
-// memory (the split kernel's counter), so the launch follows the split without a host round trip: the grid covers
-// the line CAPACITY and surplus tiles return at once.  Elements 0..n-1 are lines, element n is the virtual
-// end-of-buffer.
-constexpr int kMlFusedThreads = 256;
-constexpr int kMlFusedItems = 16; // lines per thread: 4096-line tiles, two look-backs per tile
-
-__device__ __forceinline__ uint64_t ml_element(const MlMode& m, uint32_t fl, uint64_t j) {
-    uint32_t o0, b0, o1, b1;
-    ml_trans(m, fl, 0, o0, b0);
-    ml_trans(m, fl, 1, o1, b1);
-    const uint32_t l0 = b0 ? (uint32_t)j + b0 : 0u; // (index + 1) of the opening line
-    const uint32_t l1 = b1 ? (uint32_t)j + b1 : 0u;
-    return OpMlState::make(o0, o1, l0, l1);
-}
-
-template <int THREADS, int ITEMS>
-__global__ void __launch_bounds__(THREADS)
-    ml_fused_kernel(MlMode m, const uint8_t* __restrict__ flags, const uint32_t* __restrict__ off,
-                    const uint32_t* __restrict__ len, const uint32_t* __restrict__ n_lines, uint32_t line_cap,
-                    uint32_t total_len, uint32_t* __restrict__ out_off, uint32_t* __restrict__ out_len,
-                    uint8_t* __restrict__ out_flags, uint64_t cap, volatile uint64_t* desc_state,
-                    volatile uint64_t* desc_sum, uint32_t* ticket, unsigned long long* counters, uint64_t* total_out) {
-    static_assert(ITEMS == 16, "one 16-byte load of flags per thread");
-    __shared__ uint64_t s_scan[THREADS / 32 + 1];
-    __shared__ uint32_t s_tile;
-    __shared__ uint64_t s_part[4];
-    __shared__ uint32_t s_flag[4];
-    const int tid = threadIdx.x;
-    if (tid == 0)
-        s_tile = atomicAdd(ticket, 1u);
-    __syncthreads();
-    const uint32_t tile = s_tile;
-    const uint64_t n = min(*n_lines, line_cap); // (more lines than the table holds: the host repeats the call)
-    if ((uint64_t)tile * THREADS * ITEMS > n)
-        return;
-    const uint64_t base = (uint64_t)tile * THREADS * ITEMS + (uint64_t)tid * ITEMS;
-    // the thread's 16 flag bytes (per-line state, counts and slots are recomputed from them in every pass instead of
-    // being kept in 16-entry register arrays)
-    uint32_t fw[4] = {0, 0, 0, 0};
-    if (base + ITEMS <= n) {
-        const uint4 f4 = *reinterpret_cast<const uint4*>(flags + base);
-        fw[0] = f4.x, fw[1] = f4.y, fw[2] = f4.z, fw[3] = f4.w;
-    } else {
-        for (int k = 0; k < ITEMS; ++k)
-            if (base + k < n)
-                fw[k >> 2] |= (uint32_t)flags[base + k] << (8 * (k & 3));
-    }
-    auto flag_of = [&](int k) { return (fw[k >> 2] >> (8 * (k & 3))) & 0xFFu; };
-    // ---- pass 1: compose the 2-state transition functions of the thread's lines
-    uint64_t agg = OpMlState::identity();
-#pragma unroll 4
-    for (int k = 0; k < ITEMS; ++k)
-        if (base + k < n)
-            agg = OpMlState::combine(agg, ml_element(m, flag_of(k), base + k));
-    uint64_t tot;
-    const uint64_t ex = block_exclusive_scan<OpMlState, THREADS>(agg, tot, s_scan);
-    const uint64_t pre = lookback_block<OpMlState, 4>(desc_state, tile, tot, s_part, s_flag);
-    const uint64_t run0 = OpMlState::combine(pre, ex);
-    // initial condition (:165-169): End-only mode starts partial with multiStartIndex = line 0
-    const uint32_t s0 = (!m.S && !m.C && m.E) ? 1u : 0u;
-    const uint32_t lb_init = s0 ? 1u : 0u;
-    // ---- pass 2: output events of the thread's lines (element n = the virtual end-of-buffer)
-    uint64_t run = run0;
-    uint64_t csum = 0;
-#pragma unroll 1
-    for (int k = 0; k < ITEMS; ++k) {
-        const uint64_t j = base + k;
-        if (j <= n) {
-            const uint32_t s_in = OpMlState::f(run, s0);
-            uint32_t lbp = OpMlState::lb(run, s0);
-            if (!lbp)
-                lbp = lb_init;
-            const uint32_t lb = lbp ? lbp - 1 : 0u; // line index of multiStartIndex (valid only when s_in)
-            MlCountSink sink;
-            sink.discard = m.discard;
-            sink.len = len;
-            sink.n = (uint32_t)n;
-            const uint32_t fl = j < n ? flag_of(k) : 0u;
-            ml_actions(m, fl, s_in, lb, (uint32_t)j, (uint32_t)n, sink);
-            csum += sink.cnt;
-            if (j < n)
-                run = OpMlState::combine(run, ml_element(m, fl, j));
-        }
-    }
-    uint64_t tot2;
-    const uint64_t ex2 = block_exclusive_scan<OpSum, THREADS>(csum, tot2, s_scan);
-    const uint64_t pre2 = lookback_block<OpSum, 4>(desc_sum, tile, tot2, s_part, s_flag);
-    // ---- pass 3: emission at the exclusive prefix of the counts
-    uint64_t pos = pre2 + ex2;
-    run = run0;
-    uint32_t me = 0, ul = 0;
-#pragma unroll 1
-    for (int k = 0; k < ITEMS; ++k) {
-        const uint64_t j = base + k;
-        if (j <= n) {
-            const uint32_t s_in = OpMlState::f(run, s0);
-            uint32_t lbp = OpMlState::lb(run, s0);
-            if (!lbp)
-                lbp = lb_init;
-            const uint32_t lb = lbp ? lbp - 1 : 0u;
-            const uint32_t fl = j < n ? flag_of(k) : 0u;
-            MlEmitSink sink;
-            sink.discard = m.discard;
-            sink.off = off;
-            sink.len = len;
-            sink.total_len = total_len;
-            sink.out_off = out_off;
-            sink.out_len = out_len;
-            sink.out_flags = out_flags;
-            sink.cap = cap;
-            sink.pos = pos;
-            sink.n = (uint32_t)n;
-            // begin + content.size() == sourceVal.size() (:174); the end-of-buffer element always passes true
-            sink.is_last = (j == n) ? 1u : ((off[j] + len[j] == total_len) ? 1u : 0u);
-            ml_actions(m, fl, s_in, lb, (uint32_t)j, (uint32_t)n, sink);
-            me += sink.matched_events;
-            ul += sink.unmatch_lines;
-            pos = sink.pos;
-            if (j == n)
-                *total_out = pos;
-            else
-                run = OpMlState::combine(run, ml_element(m, fl, j));
-        }
-    }
-    for (int d = 16; d; d >>= 1) {
-        me += __shfl_down_sync(0xFFFFFFFFu, me, d);
-        ul += __shfl_down_sync(0xFFFFFFFFu, ul, d);
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (me)
-            atomicAdd(&counters[0], (unsigned long long)me);
-        if (ul)
-            atomicAdd(&counters[1], (unsigned long long)ul);
-    }
-}
-
-uint32_t ml_fused_tiles(uint64_t line_cap) {
-    const uint64_t per = (uint64_t)kMlFusedThreads * kMlFusedItems;
-    return (uint32_t)((line_cap + 1 + per - 1) / per);
-}
-
-// ---- the same back half without look-backs: state pass -> scan -> count pass -> scan -> emission ------------------------
-// ml_fused_kernel chains two decoupled look-backs per tile, and a look-back waits for the slowest of the resident tiles
-// (see the split above: same effect).  The arithmetic, however,
+// ---- back half of the multiline split, without look-backs: state pass -> scan -> count pass -> scan -> emission ------
+// A single kernel would chain two decoupled look-backs per tile, and a look-back waits for the slowest of the resident
+// tiles (see the split above: same effect; measured 12 % slower on an H100).  The arithmetic, however,
 // only needs the FLAGS (one byte per line) until the very last step, so the passes are cheap to repeat:
 //   pass 1  per tile of 16384 lines: the composed 2-state transition function           -> agg1[tile]
 //   scan    one block, OpMlState (ordered)                                              -> pre1[tile]
@@ -4111,17 +2974,6 @@ int launch_ml_passes(const MlConfig& cfg, const uint8_t* d_flags, const uint32_t
     LC_ML_PASS(3);
 #undef LC_ML_PASS
     return 5;
-}
-
-void launch_ml_fused(const MlConfig& cfg, const uint8_t* d_flags, const uint32_t* d_off, const uint32_t* d_len,
-                     const uint32_t* d_n_lines, uint32_t line_cap, uint32_t total_len, uint32_t* d_out_off,
-                     uint32_t* d_out_len, uint8_t* d_out_flags, uint64_t cap, uint64_t* d_desc_state,
-                     uint64_t* d_desc_sum, uint32_t* d_ticket, unsigned long long* d_counters, uint64_t* d_total,
-                     cudaStream_t st) {
-    MlMode m{cfg.blob_start != nullptr, cfg.blob_cont != nullptr, cfg.blob_end != nullptr, cfg.discard != 0};
-    ml_fused_kernel<kMlFusedThreads, kMlFusedItems><<<ml_fused_tiles(line_cap), kMlFusedThreads, 0, st>>>(
-        m, d_flags, d_off, d_len, d_n_lines, line_cap, total_len, d_out_off, d_out_len, d_out_flags, cap,
-        (volatile uint64_t*)d_desc_state, (volatile uint64_t*)d_desc_sum, d_ticket, d_counters, d_total);
 }
 
 // ---- f3 (next row): LogFileReader::RemoveLastIncompleteLog over the line table + probe flags of the split pass --------

@@ -6,27 +6,20 @@
 
 namespace lck {
 
-// smallest split tile (16 KiB): look-back descriptors are sized for it; the kernel normally runs 128 KiB tiles
-constexpr uint32_t kSplitTileBytes = 256 * 4 * 16;
-
 constexpr int kScanThreads = 256;
 constexpr int kScanItems = 4;
 constexpr uint32_t kScanTile = kScanThreads * kScanItems;
 
-inline uint32_t split_tiles(uint64_t len, uint32_t shift) {
-    return (uint32_t)((len + shift + kSplitTileBytes - 1) / kSplitTileBytes);
-}
 inline uint32_t scan_tiles(uint64_t n) { return (uint32_t)((n + kScanTile - 1) / kScanTile); }
 
-// a1: newline split.  desc: >= split_tiles() u64 (zeroed), ticket: u32 (zeroed), n_out: u32 device counter.
-// d_total: u64 device counter (zeroed) that receives the un-truncated number of split chars (the look-back payload
-// keeps 30 bits of count: the caller reports LC_ERR_TOO_LARGE beyond that).
-// d_scratch: split_scratch_bytes(len, probe) bytes (not initialised) for the three-pass formulation (masks, per-tile
-// counts and prefixes); nullptr selects the single-pass look-back kernel.  Returns the number of kernels launched.
+// a1: newline split in three passes (masks, tile scan, emission).  n_out: u32 device counter.
+// d_total: u64 device counter (zeroed) that receives the un-truncated number of split chars (the line numbers keep
+// 30 bits of count: the caller reports LC_ERR_TOO_LARGE beyond that).
+// d_scratch: split_scratch_bytes(len, probe) bytes (not initialised): masks, per-tile counts and prefixes.
+// Returns the number of kernels launched.
 uint64_t split_scratch_bytes(uint64_t len, bool probe);
 int launch_split(const uint8_t* d_buf, uint32_t len, uint8_t split_char, uint32_t* d_off, uint32_t* d_len,
-                 uint32_t cap, uint64_t* d_desc, uint32_t* d_ticket, uint32_t* d_n_out, unsigned long long* d_total,
-                 uint64_t* d_scratch, cudaStream_t st);
+                 uint32_t cap, uint32_t* d_n_out, unsigned long long* d_total, uint64_t* d_scratch, cudaStream_t st);
 
 // exclusive sum of u32 -> u64 (out has n entries; *d_total receives the grand total)
 void launch_exclusive_sum(const uint32_t* d_in, uint64_t n, uint64_t* d_out, uint64_t* d_total, uint64_t* d_desc,
@@ -88,19 +81,10 @@ int launch_regex_fast2(const void* d_blob, uint32_t blob_bytes, bool multi, bool
                        const uint32_t* d_order, cudaStream_t st);
 
 // a3 single-pass tagged-DFA path (LcTdfaHeader): no labels; per thread only nregs u16 registers in shared memory.
-// Only valid when every event is shorter than 65535 bytes (the staged kernel raises *d_overflow otherwise and the
-// host repeats the call on a kernel with 32-bit slots; the direct kernel relies on a host-side length check).
+// Events of 65535 bytes or more raise *d_overflow and are left to launch_regex_tdfa_long (32-bit slots).
+// Lines are fetched cooperatively (cp.async, 4 full 128-byte lines per instruction) into a per-warp 4 KB tile;
+// carve-out = 512 B (aligned class table) + blob + register files + 256 B line info and 4 KB tile per warp
 inline uint32_t tdfa_reg_pitch(uint32_t nregs) { return (((nregs + 1) / 2) | 1u) * 2; } // halfwords; odd WORD pitch
-inline size_t tdfa_smem_bytes(uint32_t blob_bytes, uint32_t nregs, uint32_t threads) {
-    return (size_t)blob_bytes + (size_t)threads * tdfa_reg_pitch(nregs) * 2;
-}
-int launch_regex_tdfa(const void* d_blob, uint32_t blob_bytes, bool slow, uint32_t nregs, const uint8_t* d_base,
-                      const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, uint32_t nkeys,
-                      uint8_t* d_status, uint32_t* d_cap_off, uint32_t* d_cap_len, uint32_t threads, uint32_t grid,
-                      unsigned long long* d_next_batch, const uint32_t* d_order, cudaStream_t st);
-
-// staged variant: lines are fetched cooperatively (cp.async, 4 full 128-byte lines per instruction) into a per-warp
-// 4 KB tile; carve-out = 512 B (aligned class table) + blob + register files + 256 B line info and 4 KB tile per warp
 inline size_t tdfa_staged_smem_bytes(uint32_t blob_bytes, uint32_t nregs, uint32_t threads) {
     return 512 + (size_t)blob_bytes + 16 + (size_t)threads * tdfa_reg_pitch(nregs) * 2 +
            (size_t)(threads / 32) * (256 + 4096);
@@ -111,17 +95,6 @@ int launch_regex_tdfa_staged(const void* d_blob, uint32_t blob_bytes, bool slow,
                              uint32_t threads, uint32_t grid, unsigned long long* d_next_batch, uint32_t* d_overflow,
                              const uint32_t* d_order /* or nullptr */, const uint32_t* d_order_flag /* or nullptr */,
                              cudaStream_t st);
-
-// producer / consumer variant (A/B): the first 4 warps of the block only fill the other warps' tiles (LDG.128 + STS.128);
-// threads counts ALL warps, consumers = threads / 32 - 4
-inline size_t tdfa_pc_smem_bytes(uint32_t blob_bytes, uint32_t nregs, uint32_t threads) {
-    const size_t nc = threads / 32 - 4;
-    return 512 + (size_t)blob_bytes + 16 + nc * 32 * tdfa_reg_pitch(nregs) * 2 + nc * (256 + 4096 + 8 + 4) + 16 + 64;
-}
-int launch_regex_tdfa_pc(const void* d_blob, uint32_t blob_bytes, bool slow, uint32_t nregs, const uint8_t* d_base,
-                         const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint32_t ev_stride, uint64_t n,
-                         uint32_t nkeys, uint8_t* d_status, uint32_t* d_cap_off, uint32_t* d_cap_len, uint32_t threads,
-                         uint32_t grid, unsigned long long* d_next_batch, uint32_t* d_overflow, cudaStream_t st);
 
 // several patterns in one grid: all tagged-DFA blobs co-resident in shared memory, tried per line in array order
 constexpr uint32_t LC_MULTI_MAX = 8;
@@ -160,7 +133,7 @@ void launch_status_to_bool(uint8_t* d_status, uint64_t n, cudaStream_t st);
 void launch_prefix_match(const void* d_blob, const uint8_t* d_base, const uint32_t* d_ev_off,
                          const uint32_t* d_ev_len, uint64_t n, uint8_t* d_out, cudaStream_t st);
 
-// a2: multiline.  Lines (d_off,d_len,n) come from launch_split over the same buffer.
+// a2: multiline.  Lines (d_off, d_len) and per-line flags come from launch_split_probe over the same buffer.
 struct MlConfig {
     const void* blob_start; // device blobs or nullptr
     const void* blob_cont;
@@ -171,37 +144,20 @@ struct MlConfig {
     uint32_t first[3][8];
     uint32_t empty_flags;
 };
-// flags[i] bit0/1/2 = start/continue/end pattern matches a prefix of line i
-void launch_ml_probe(const MlConfig& cfg, const uint8_t* d_buf, const uint32_t* d_off, const uint32_t* d_len,
-                     uint64_t n, uint8_t* d_flags, cudaStream_t st);
-// state scan over n lines + 1 virtual EOF element: d_state[i] = (s_in << 31) | lb_in, d_cnt[i] = output events
-void launch_ml_state(const MlConfig& cfg, const uint8_t* d_flags, const uint32_t* d_len, uint64_t n, uint32_t* d_state,
-                     uint32_t* d_cnt, uint64_t* d_desc, uint32_t* d_ticket, cudaStream_t st);
-// emission: d_pos = exclusive sum of d_cnt; d_counters[0..1] += matched_events, unmatch_lines
-void launch_ml_emit(const MlConfig& cfg, const uint8_t* d_flags, const uint32_t* d_off, const uint32_t* d_len,
-                    uint64_t n, uint32_t total_len, const uint32_t* d_state, const uint64_t* d_pos, uint32_t* d_out_off,
-                    uint32_t* d_out_len, uint8_t* d_out_flags, uint64_t cap, unsigned long long* d_counters,
-                    cudaStream_t st);
-
-// fused multiline path: split + per-line probes in one pass (flags[line]), then state scan + counts + slots + emission
-// in one kernel that reads the line count from d_n_lines (no host round trip in between).  d_desc_state / d_desc_sum:
-// ml_fused_tiles(line_cap) + 1 zeroed u64 each.
+// split + per-line probes in one formulation (the three split passes): d_flags[i] bit0/1/2 = start/continue/end
+// pattern matches a prefix of line i.  Other arguments and the result as for launch_split.
 int launch_split_probe(const MlConfig& cfg, const uint8_t* d_buf, uint32_t len, uint32_t* d_off, uint32_t* d_len,
-                       uint8_t* d_flags, uint32_t cap, uint64_t* d_desc, uint32_t* d_ticket, uint32_t* d_n_out,
-                       unsigned long long* d_total, uint64_t* d_scratch, cudaStream_t st);
-uint32_t ml_fused_tiles(uint64_t line_cap);
-// the same result without look-backs (five launches; d_scratch: ml_pass_scratch_bytes(line_cap), not initialised)
+                       uint8_t* d_flags, uint32_t cap, uint32_t* d_n_out, unsigned long long* d_total,
+                       uint64_t* d_scratch, cudaStream_t st);
+// state scan + counts + slots + emission over the split's line table; reads the line count from d_n_lines (no host
+// round trip in between).  Five launches; d_scratch: ml_pass_scratch_bytes(line_cap), not initialised.
+// d_counters[0..1] += matched_events, unmatch_lines; *d_total = number of output events.
 uint32_t ml_pass_tiles(uint64_t line_cap);
 uint64_t ml_pass_scratch_bytes(uint64_t line_cap);
 int launch_ml_passes(const MlConfig& cfg, const uint8_t* d_flags, const uint32_t* d_off, const uint32_t* d_len,
                      const uint32_t* d_n_lines, uint32_t line_cap, uint32_t total_len, uint32_t* d_out_off,
                      uint32_t* d_out_len, uint8_t* d_out_flags, uint64_t cap, uint64_t* d_scratch,
                      unsigned long long* d_counters, uint64_t* d_total, cudaStream_t st);
-void launch_ml_fused(const MlConfig& cfg, const uint8_t* d_flags, const uint32_t* d_off, const uint32_t* d_len,
-                     const uint32_t* d_n_lines, uint32_t line_cap, uint32_t total_len, uint32_t* d_out_off,
-                     uint32_t* d_out_len, uint8_t* d_out_flags, uint64_t cap, uint64_t* d_desc_state,
-                     uint64_t* d_desc_sum, uint32_t* d_ticket, unsigned long long* d_counters, uint64_t* d_total,
-                     cudaStream_t st);
 
 // f3: last complete record of a chunk from the split pass's line table + flags; d_out[0] = keep bytes, [1] = rollback
 void launch_last_record(const uint8_t* d_flags, const uint32_t* d_off, const uint32_t* d_len, const uint32_t* d_n_lines,

@@ -2,15 +2,16 @@
 // associative (not necessarily commutative) operator on a 62-bit payload.
 //
 // Every tile publishes a 64-bit descriptor {flag:2 | payload:62}; a tile first publishes its local
-// AGGREGATE, then walks its predecessors (one warp, 32 descriptors per step) until it meets an
+// AGGREGATE, then walks its predecessors (32 descriptors per warp and step) until it meets an
 // INCLUSIVE prefix, and finally publishes its own inclusive prefix.  Flag and payload share one
 // 8-byte word, so a plain 64-bit store/load is atomic and no fence is needed between them.
 // Tiles take their index from an atomic ticket so that a tile can only wait on tiles that are
 // already running (forward-progress guarantee independent of block scheduling order).
 //
-// Used for: (1) newline split -- payload {count:30 | line_start:32}; (2) the multiline
-// start/continue/end state machine -- payload = a 2-state transition function plus the index of
-// the line that opened the pending record, per incoming state; (3) plain 62-bit sums (output slots).
+// The look-back serves plain 62-bit sums (output slots).  The other operators serve scans without
+// look-back: OpCountMax reads the split's tile prefixes {count:30 | line_start:32}, and OpMlState
+// is the multiline state machine -- a 2-state transition function plus the index of the line that
+// opened the pending record, per incoming state.
 #pragma once
 #include <stdint.h>
 
@@ -117,109 +118,6 @@ __device__ __forceinline__ uint64_t block_exclusive_scan(uint64_t v, uint64_t& b
 }
 
 __device__ __forceinline__ uint64_t ld_desc(const volatile uint64_t* p) { return *p; }
-
-// Executed by ONE full warp of the tile.  Returns the exclusive prefix of `tile` (all lanes).
-template <class Op>
-__device__ __forceinline__ uint64_t lookback(volatile uint64_t* desc, uint32_t tile, uint64_t aggregate) {
-    const int lane = threadIdx.x & 31;
-    if (tile == 0) {
-        if (lane == 0)
-            desc[0] = kFlagInclusive | (aggregate & kPayloadMask);
-        return Op::identity();
-    }
-    if (lane == 0)
-        desc[tile] = kFlagAggregate | (aggregate & kPayloadMask);
-    uint64_t prefix = Op::identity();
-    int64_t base = (int64_t)tile - 1;
-    for (;;) {
-        int64_t idx = base - lane;
-        uint64_t d;
-        if (idx >= 0) {
-            do {
-                d = ld_desc(desc + idx);
-            } while ((d >> 62) == 0);
-        } else {
-            d = kFlagInclusive | Op::identity();
-        }
-        unsigned incl = __ballot_sync(0xFFFFFFFFu, (d >> 62) == 2);
-        int stop = incl ? (__ffs(incl) - 1) : 31;
-        uint64_t r = (lane <= stop) ? (d & kPayloadMask) : Op::identity();
-        // ordered reduction: higher lanes are EARLIER tiles
-#pragma unroll
-        for (int s = 1; s < 32; s <<= 1) {
-            uint64_t t = shfl_down64(r, s);
-            if (lane + s < 32)
-                r = Op::combine(t, r);
-        }
-        uint64_t seg = shfl64(r, 0);
-        prefix = Op::combine(seg, prefix);
-        if (incl)
-            break;
-        base -= 32;
-    }
-    if (lane == 0)
-        desc[tile] = kFlagInclusive | (Op::combine(prefix, aggregate) & kPayloadMask);
-    return prefix;
-}
-
-// Deep variant: every lane holds D consecutive descriptors (D independent loads in flight), so one L2 round trip covers
-// 32 * D predecessors -- with D = 8 that is more than the tiles that are resident at once (2 x 132 blocks on an H100), i.e. the
-// nearest INCLUSIVE prefix is inside the first window.  Lanes do not spin on descriptors that lie beyond the nearest
-// inclusive one; a window is re-polled only while a not-yet-published tile sits in front of it.
-template <class Op, int D>
-__device__ __forceinline__ uint64_t lookback_deep(volatile uint64_t* desc, uint32_t tile, uint64_t aggregate) {
-    const int lane = threadIdx.x & 31;
-    if (tile == 0) {
-        if (lane == 0)
-            desc[0] = kFlagInclusive | (aggregate & kPayloadMask);
-        return Op::identity();
-    }
-    if (lane == 0)
-        desc[tile] = kFlagAggregate | (aggregate & kPayloadMask);
-    uint64_t prefix = Op::identity();
-    int64_t base = (int64_t)tile - 1;
-    for (;;) {
-        uint64_t d[D];
-#pragma unroll
-        for (int j = 0; j < D; ++j) {
-            const int64_t idx = base - (lane * D + j);
-            d[j] = idx >= 0 ? ld_desc(desc + idx) : (kFlagInclusive | Op::identity());
-        }
-        uint64_t r = Op::identity();
-        bool found = false, blocked = false;
-#pragma unroll
-        for (int j = 0; j < D; ++j) { // nearest first; stop at the first inclusive or unpublished descriptor
-            const uint32_t fl = (uint32_t)(d[j] >> 62);
-            if (!found && !blocked) {
-                if (fl == 0) {
-                    blocked = true;
-                } else {
-                    r = Op::combine(d[j] & kPayloadMask, r);
-                    found = fl == 2;
-                }
-            }
-        }
-        const unsigned incl = __ballot_sync(0xFFFFFFFFu, found), blk = __ballot_sync(0xFFFFFFFFu, blocked);
-        const int fi = incl ? (__ffs(incl) - 1) : 32, bi = blk ? (__ffs(blk) - 1) : 32;
-        if (bi < fi)
-            continue; // an unpublished tile in front of the nearest inclusive prefix: poll the window again
-        if (lane > fi)
-            r = Op::identity();
-#pragma unroll
-        for (int s = 1; s < 32; s <<= 1) { // ordered reduction: higher lanes are EARLIER tiles
-            const uint64_t t = shfl_down64(r, s);
-            if (lane + s < 32)
-                r = Op::combine(t, r);
-        }
-        prefix = Op::combine(shfl64(r, 0), prefix);
-        if (incl)
-            break;
-        base -= 32 * D;
-    }
-    if (lane == 0)
-        desc[tile] = kFlagInclusive | (Op::combine(prefix, aggregate) & kPayloadMask);
-    return prefix;
-}
 
 // Block-cooperative look-back: ALL threads of the block call (uniform control flow); the first WARPS warps poll
 // WARPS * 32 predecessors per round.  Why: a tile's walk ends at the nearest predecessor that already holds an
