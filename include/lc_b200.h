@@ -275,6 +275,49 @@ int lc_sls_serialize_parsed_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t 
                                 const uint32_t* d_ev_time, const uint32_t* d_ev_time_ns, uint8_t* d_out,
                                 uint64_t out_cap, uint64_t* out_len);
 
+/* Device-fed variant for the delimiter -> serialise hand-over: the `Logs` fields of the events a
+ * ProcessorParseDelimiterNative leaves behind (ProcessorParseDelimiterNative.cpp:206-364), written straight from the
+ * DEVICE tables of one lc_delim_parse_dev call (d_status, d_nfields, [n][max_fields] d_f_off / d_f_len / d_f_dq) and
+ * the configuration the parse ran with.  Every event is taken to be flat: a LogEvent whose only content is
+ * source_key -> its line.  Per event:
+ *   LC_DELIM_OK: keys[j] -> column j in column order, doubled quotes collapsed (AddFieldWithUnQuote); in discard mode
+ *     keys "_" and columns >= nkeys are skipped; in extend mode (extend != 0) column j >= nkeys gets "__column<j>__";
+ *     in keep mode (neither flag) columns nkeys.. are re-joined as sep[0] + column each under "__column<nkeys>__"
+ *     (the multi-byte split's remainder column already holds its separator).  A key equal to source_key replaces the
+ *     source content in place (it comes first; a row too short to reach it keeps the line there).  keep_succeed adds
+ *     renamed_key -> line unless that key is present.  A row with more columns than max_fields is walked again on the
+ *     device from the start of its line.
+ *   LC_DELIM_PARSE_FAIL / LC_DELIM_COLUMNS: with keep_fail, renamed_key -> line, then "__raw_log__" -> line if copy_raw
+ *     and renamed_key is another key; without keep_fail the event is erased.
+ *   LC_DELIM_BLANK: untouched, source_key -> the untrimmed line.
+ * renamed_key is CommonParserOptions' RenamedSourceKey (source_key when not configured).  Events without contents
+ * emit nothing.  Refused with LC_ERR_INVALID_ARG: repeated keys (except "_" in discard mode), keys or a source_key of
+ * the form "__column<digits>__" in extend or keep mode, max_fields < nkeys + 1.  d_ev_time_ns may be NULL;
+ * LC_SLS_NO_NS per event = no Time_ns.  d_out receives the bytes on the device; *out_len (host) their count;
+ * LC_ERR_CAPACITY if > out_cap (nothing written). */
+int lc_sls_serialize_delim_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t base_len, const uint32_t* d_ev_off,
+                               const uint32_t* d_ev_len, uint64_t n, const uint8_t* d_status, const uint32_t* d_nfields,
+                               const uint32_t* d_f_off, const uint32_t* d_f_len, const uint32_t* d_f_dq,
+                               uint32_t max_fields, const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend,
+                               int discard, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                               const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                               uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                               const uint32_t* d_ev_time, const uint32_t* d_ev_time_ns, uint8_t* d_out,
+                               uint64_t out_cap, uint64_t* out_len);
+
+/* The same with HOST buffers: parse (lc_delim_parse with allow_short, tables max_fields wide) and serialise in one
+ * call.  The arena goes up once, in chunks of whole events on a copy stream while earlier chunks are parsed; the
+ * tables stay on the device and only the wire bytes come back (out, in event order).  counters[4] = successful,
+ * failed (parse failures), discarded (erased failures), blank events -- ProcessorParseDelimiterNative's out_successful,
+ * discarded, and out_failed = failed + blank.  *out_len and counters are set on LC_OK and on LC_ERR_CAPACITY. */
+int lc_delim_parse_sls(lc_engine_t* e, const uint8_t* base, uint64_t base_len, const uint32_t* ev_off,
+                       const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time, const uint32_t* ev_time_ns,
+                       const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard, int allow_short,
+                       uint32_t max_fields, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                       const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                       uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, uint8_t* out,
+                       uint64_t out_cap, uint64_t* out_len, uint64_t counters[4]);
+
 #ifdef __cplusplus
 }
 #endif

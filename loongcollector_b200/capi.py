@@ -82,6 +82,11 @@ def lib():
     L.lc_delim_parse_tap_dev.argtypes = dl_args + [u32, vp, vp]
     L.lc_delim_regex_chain.argtypes = dl_args + [u32, vp, u32, vp, vp, vp]
     L.lc_sls_serialize_logs.argtypes = [vp, vp, u64, u64, vp, vp, vp, vp, vp, vp, vp, vp, u64, C.POINTER(u64)]
+    sls_cfg = [vp, vp, u32, C.c_char_p, u32, C.c_char_p, u32, i32, i32, i32]  # keys .. copy_raw
+    L.lc_sls_serialize_delim_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, vp, u32, vp, u32, u8, i32,
+                                             i32] + sls_cfg + [vp, vp, vp, u64, C.POINTER(u64)]
+    L.lc_delim_parse_sls.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32, u8, i32, i32, i32, u32] + sls_cfg + \
+        [vp, u64, C.POINTER(u64), vp]
     _LIB = L
     return L
 
@@ -334,6 +339,63 @@ class Engine:
                                                  _p(d_ev_time_ns), _p(d_out), out_cap, C.byref(need)))
         return int(need.value)
 
+    @staticmethod
+    def _delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw):
+        """keys / source_key / renamed_key: bytes (renamed_key None = source_key); returns the C arguments"""
+        arr = (C.c_char_p * max(len(keys), 1))(*keys)
+        kl = np.array([len(k) for k in keys] or [0], np.uint32)
+        rk = source_key if renamed_key is None else renamed_key
+        return (arr, kl), [C.cast(arr, C.c_void_p), _p(kl), len(keys), source_key, len(source_key), rk, len(rk),
+                           int(bool(keep_fail)), int(bool(keep_succeed)), int(bool(copy_raw))]
+
+    def sls_serialize_delim_dev(self, d_base, base_len, d_ev_off, d_ev_len, n, d_status, d_nf, d_fo, d_fl, d_fd,
+                                max_fields, sep: bytes, quote, treatment, keys, source_key, renamed_key=None,
+                                keep_fail=False, keep_succeed=False, copy_raw=False, d_ev_time=None,
+                                d_ev_time_ns=None, d_out=None, out_cap=0):
+        """Wire bytes of the events ProcessorParseDelimiterNative leaves behind, from the device tables of one
+        delim_parse_dev call (treatment: "extend" / "keep" / "discard").  Returns the byte count written to d_out, or
+        with d_out None the byte count needed."""
+        sp = np.frombuffer(sep, np.uint8)
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        need = C.c_uint64(0)
+        rc = lib().lc_sls_serialize_delim_dev(self._h, _p(d_base), base_len, _p(d_ev_off), _p(d_ev_len), n,
+                                              _p(d_status), _p(d_nf), _p(d_fo), _p(d_fl), _p(d_fd), max_fields, _p(sp),
+                                              len(sep), quote, int(treatment == "extend"), int(treatment == "discard"),
+                                              *cfg, _p(d_ev_time), _p(d_ev_time_ns), _p(d_out), out_cap, C.byref(need))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value)  # a sizing query
+        _check(rc)
+        return int(need.value)
+
+    def delim_parse_sls(self, base, ev_off, ev_len, ev_time, sep: bytes, quote, treatment, keys, source_key,
+                        renamed_key=None, keep_fail=False, keep_succeed=False, copy_raw=False, allow_short=True,
+                        max_fields=None, ev_time_ns=None, out_cap=None):
+        """Host buffers in, wire bytes out (lc_delim_parse_sls).  Returns (bytes, counters[4] = successful, failed,
+        discarded, blank).  Without out_cap the output is sized by a first estimate and, if short, the exact size."""
+        a = _u8(base)
+        ev_off = np.ascontiguousarray(ev_off, np.uint32)
+        ev_len = np.ascontiguousarray(ev_len, np.uint32)
+        t = np.ascontiguousarray(ev_time, np.uint32)
+        ns = None if ev_time_ns is None else np.ascontiguousarray(ev_time_ns, np.uint32)
+        n = ev_off.size
+        mf = int(max_fields if max_fields is not None else len(keys) + 16)
+        sp = np.frombuffer(sep, np.uint8)
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        cap = int(out_cap if out_cap is not None else 2 * a.size + 64 * n + 64)
+        for _ in range(2):
+            out = np.empty(max(cap, 1), np.uint8)
+            need = C.c_uint64(0)
+            ctr = np.zeros(4, np.uint64)
+            rc = lib().lc_delim_parse_sls(self._h, _p(a), a.size, _p(ev_off), _p(ev_len), n, _p(t), _p(ns), _p(sp),
+                                          len(sep), quote, int(treatment == "extend"), int(treatment == "discard"),
+                                          int(bool(allow_short)), mf, *cfg, _p(out), cap, C.byref(need), _p(ctr))
+            if rc == LC_ERR_CAPACITY and out_cap is None:
+                cap = int(need.value)
+                continue
+            _check(rc)
+            return bytes(out[:need.value]), ctr
+        _check(rc)
+
     def split_lines_dev(self, d_buf, length, split_char, d_off, d_len, cap):
         n = C.c_uint64(0)
         _check(lib().lc_split_lines_dev(self._h, _p(d_buf), length, split_char, _p(d_off), _p(d_len), cap,
@@ -434,6 +496,36 @@ class HostProcessor:
                 lib().lc_host_processor_destroy(self._h)
         except Exception:
             pass
+
+
+    def serialize_sls(self, group, enable_ns=False, process_then_serialize=False):
+        """ProcessorParseDelimiterNative::SerializeSls on a JSON group: (bytes, None) or (None, error).  With
+        process_then_serialize, Process + SLSEventGroupSerializer::Serialize on the same in-memory group instead."""
+        import json
+        L = lib()
+        L.lc_host_processor_serialize_sls.restype = C.c_void_p
+        L.lc_host_processor_serialize_sls.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int,
+                                                      C.POINTER(C.c_ulonglong), C.POINTER(C.c_void_p),
+                                                      C.POINTER(C.c_void_p)]
+        L.lc_host_string_free.argtypes = [C.c_void_p]
+        err = C.c_void_p()
+        fail = C.c_void_p()
+        n = C.c_ulonglong(0)
+        out = L.lc_host_processor_serialize_sls(self._h, json.dumps(group).encode("utf-8"), int(bool(enable_ns)),
+                                                int(bool(process_then_serialize)), C.byref(n), C.byref(err),
+                                                C.byref(fail))
+        if fail.value:
+            msg = C.string_at(fail.value).decode()
+            L.lc_host_string_free(fail)
+            raise LcError(LC_ERR_CUDA, msg)
+        if not out:
+            msg = C.string_at(err.value).decode() if err.value else "unknown error"
+            if err.value:
+                L.lc_host_string_free(err)
+            return None, msg
+        data = C.string_at(out, n.value)
+        L.lc_host_string_free(out)
+        return data, None
 
 
 def host_sls_serialize(group, enable_ns=False):

@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "../../include/lc_b200.h"
+#include "lc_exec.cuh"
 #include "lc_kernels.cuh"
 #include "lc_tables.h"
 #include "regex_compiler.h"
@@ -1800,6 +1801,212 @@ int lc_sls_serialize_parsed_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t 
                                 d_out, e->stream);
     e->launches++;
     CU_TRY(cudaGetLastError());
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    return LC_OK;
+}
+
+} // extern "C"
+
+// ------------------------------------------------------------------------------------------------ delimiter -> SLS
+namespace {
+
+// the configuration of the delimiter-fed serialiser, its key strings staged on the device (engine `order` buffer)
+int delim_sls_config(lc_engine_t* e, const char* what, uint32_t max_fields, const uint8_t* sep, uint32_t sep_len,
+                     uint8_t quote, int extend, int discard, const char* const* keys, const uint32_t* key_lens,
+                     uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                     uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, LcDelimSlsCfg* c) {
+    if (!sep || (nkeys && (!keys || !key_lens)) || (source_key_len && !source_key) ||
+        (renamed_key_len && !renamed_key))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    for (uint32_t k = 0; k < nkeys; ++k)
+        if (key_lens[k] && !keys[k])
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    uint64_t kbytes = (uint64_t)source_key_len + renamed_key_len + 11;
+    for (uint32_t k = 0; k < nkeys; ++k)
+        kbytes += key_lens[k];
+    if (kbytes >= (1ull << 31))
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": keys too long");
+    std::vector<uint8_t> kb(kbytes + 1);
+    std::vector<uint32_t> at(nkeys + 4);
+    const char* why = lc_delim_sls_setup(sep, sep_len, quote, extend, discard, keys, key_lens, nkeys, source_key,
+                                         source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed, copy_raw,
+                                         max_fields, c, kb.data(), at.data());
+    if (why)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    const size_t at_bytes = at.size() * 4;
+    CU_TRY(e->order.ensure(at_bytes + kb.size() + 16));
+    CU_TRY(cudaMemcpyAsync(e->order.p, at.data(), at_bytes, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(e->order.as<uint8_t>() + at_bytes, kb.data(), kb.size(), cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream)); // (pageable sources: their bytes must be on the device before they die)
+    c->key_at = e->order.as<uint32_t>();
+    c->keys = e->order.as<uint8_t>() + at_bytes;
+    return LC_OK;
+}
+
+} // namespace
+
+extern "C" {
+
+int lc_sls_serialize_delim_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t base_len, const uint32_t* d_ev_off,
+                               const uint32_t* d_ev_len, uint64_t n, const uint8_t* d_status, const uint32_t* d_nfields,
+                               const uint32_t* d_f_off, const uint32_t* d_f_len, const uint32_t* d_f_dq,
+                               uint32_t max_fields, const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend,
+                               int discard, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                               const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                               uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                               const uint32_t* d_ev_time, const uint32_t* d_ev_time_ns, uint8_t* d_out,
+                               uint64_t out_cap, uint64_t* out_len) {
+    static const char* what = "lc_sls_serialize_delim_dev";
+    if (!e || !out_len || (n && (!d_base || !d_ev_off || !d_ev_len || !d_status || !d_nfields || !d_f_off || !d_f_len ||
+                                 !d_f_dq || !d_ev_time)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (base_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 events and < 2^32 columns per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcDelimSlsCfg c;
+    rc = delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, keys, key_lens, nkeys, source_key,
+                          source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed, copy_raw, &c);
+    if (rc || n == 0)
+        return rc;
+    const lck::DelimSlsTables t{d_base, d_ev_off, d_ev_len, d_status, d_nfields, d_f_off, d_f_len, d_f_dq};
+    CU_TRY(e->lab_sizes.ensure(n * 4));
+    CU_TRY(e->cnt.ensure(n * 4));
+    CU_TRY(e->lab_off.ensure(n * 8));
+    uint64_t* desc;
+    rc = prep_desc(e, lck::scan_tiles(n), &desc);
+    if (rc)
+        return rc;
+    Small* ds = e->small.as<Small>();
+    Small* hs = (Small*)e->h_small;
+    lck::launch_delim_sls_sizes(c, t, d_ev_time_ns, n, e->lab_sizes.as<uint32_t>(), e->cnt.as<uint32_t>(), nullptr,
+                                e->stream);
+    lck::launch_exclusive_sum(e->lab_sizes.as<uint32_t>(), n, e->lab_off.as<uint64_t>(), &ds->total, desc,
+                              &ds->tickets[2], e->stream);
+    e->launches += 2;
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(&hs->total, &ds->total, 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    *out_len = hs->total;
+    if (hs->total > out_cap)
+        return fail(LC_ERR_CAPACITY, std::string(what) + ": output capacity too small");
+    if (hs->total == 0)
+        return LC_OK;
+    if (!d_out)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    lck::launch_delim_sls_emit(c, t, d_ev_time, d_ev_time_ns, n, e->lab_off.as<uint64_t>(), e->cnt.as<uint32_t>(), d_out,
+                               e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    return LC_OK;
+}
+
+int lc_delim_parse_sls(lc_engine_t* e, const uint8_t* base, uint64_t base_len, const uint32_t* ev_off,
+                       const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time, const uint32_t* ev_time_ns,
+                       const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard, int allow_short,
+                       uint32_t max_fields, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                       const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                       uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, uint8_t* out,
+                       uint64_t out_cap, uint64_t* out_len, uint64_t counters[4]) {
+    static const char* what = "lc_delim_parse_sls";
+    if (!e || !out_len || !counters || (n && (!ev_off || !ev_len || !ev_time)) || (base_len && !base))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    memset(counters, 0, 4 * sizeof(uint64_t));
+    if (base_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 events and < 2^32 columns per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcDelimSlsCfg c;
+    rc = delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, keys, key_lens, nkeys, source_key,
+                          source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed, copy_raw, &c);
+    if (rc || n == 0)
+        return rc;
+    // workspace: in / ev_off / ev_len = arena and event table, out_a..out_e = the delimiter tables, lines_off /
+    // lines_len = time / ns, lab_sizes / cnt = record / body sizes, lab_off = record offsets, state = counters,
+    // lab = the wire bytes
+    const uint64_t MF = max_fields, fbytes = n * MF * 4;
+    CU_TRY(e->in.ensure(base_len + 16));
+    CU_TRY(e->ev_off.ensure(n * 4));
+    CU_TRY(e->ev_len.ensure(n * 4));
+    CU_TRY(e->out_a.ensure(n));
+    CU_TRY(e->out_b.ensure(n * 4));
+    CU_TRY(e->out_c.ensure(fbytes));
+    CU_TRY(e->out_d.ensure(fbytes));
+    CU_TRY(e->out_e.ensure(fbytes));
+    CU_TRY(e->lines_off.ensure(n * 4));
+    CU_TRY(e->lines_len.ensure(n * 4));
+    CU_TRY(e->lab_sizes.ensure(n * 4));
+    CU_TRY(e->cnt.ensure(n * 4));
+    CU_TRY(e->lab_off.ensure(n * 8));
+    CU_TRY(e->state.ensure(4 * sizeof(unsigned long long)));
+    uint64_t* desc;
+    rc = prep_desc(e, lck::scan_tiles(n), &desc);
+    if (rc)
+        return rc;
+    unsigned long long* d_ctr = e->state.as<unsigned long long>();
+    CU_TRY(cudaMemsetAsync(d_ctr, 0, 4 * sizeof(unsigned long long), e->stream));
+    uint32_t* d_time = e->lines_off.as<uint32_t>();
+    uint32_t* d_ns = ev_time_ns ? e->lines_len.as<uint32_t>() : nullptr;
+    // per chunk of whole events: arena + event table up (copy stream), times up, delimiter parse, record sizes; no
+    // table comes back
+    auto run = [&](uint64_t, uint64_t i0, uint64_t cnt, uint64_t) {
+        CU_TRY(cudaMemcpyAsync(d_time + i0, ev_time + i0, cnt * 4, cudaMemcpyHostToDevice, e->stream));
+        if (d_ns)
+            CU_TRY(cudaMemcpyAsync(d_ns + i0, ev_time_ns + i0, cnt * 4, cudaMemcpyHostToDevice, e->stream));
+        int r = lc_delim_parse_dev(e, e->in.as<uint8_t>(), base_len, e->ev_off.as<uint32_t>() + i0,
+                                   e->ev_len.as<uint32_t>() + i0, cnt, sep, sep_len, quote, nkeys, extend, allow_short,
+                                   max_fields, e->out_a.as<uint8_t>() + i0, e->out_b.as<uint32_t>() + i0,
+                                   e->out_c.as<uint32_t>() + i0 * MF, e->out_d.as<uint32_t>() + i0 * MF,
+                                   e->out_e.as<uint32_t>() + i0 * MF);
+        if (r)
+            return r;
+        const lck::DelimSlsTables t{e->in.as<uint8_t>(), e->ev_off.as<uint32_t>() + i0, e->ev_len.as<uint32_t>() + i0,
+                                    e->out_a.as<uint8_t>() + i0, e->out_b.as<uint32_t>() + i0,
+                                    e->out_c.as<uint32_t>() + i0 * MF, e->out_d.as<uint32_t>() + i0 * MF,
+                                    e->out_e.as<uint32_t>() + i0 * MF};
+        lck::launch_delim_sls_sizes(c, t, d_ns ? d_ns + i0 : nullptr, cnt, e->lab_sizes.as<uint32_t>() + i0,
+                                    e->cnt.as<uint32_t>() + i0, d_ctr, e->stream);
+        e->launches++;
+        CU_TRY(cudaGetLastError());
+        return (int)LC_OK;
+    };
+    auto down = [&](uint64_t, uint64_t, uint64_t) { return (int)LC_OK; };
+    rc = pipelined_events(e, base, base_len, ev_off, ev_len, n, pipeline_chunks(base_len, n), what, run, down);
+    if (rc)
+        return rc;
+    Small* ds = e->small.as<Small>();
+    Small* hs = (Small*)e->h_small;
+    lck::launch_exclusive_sum(e->lab_sizes.as<uint32_t>(), n, e->lab_off.as<uint64_t>(), &ds->total, desc,
+                              &ds->tickets[2], e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(&hs->total, &ds->total, 8, cudaMemcpyDeviceToHost, e->stream));
+    unsigned long long ctr[4];
+    CU_TRY(cudaMemcpyAsync(ctr, d_ctr, sizeof ctr, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    for (int k = 0; k < 4; ++k)
+        counters[k] = ctr[k];
+    *out_len = hs->total;
+    if (hs->total > out_cap)
+        return fail(LC_ERR_CAPACITY, std::string(what) + ": output capacity too small");
+    if (hs->total == 0)
+        return LC_OK;
+    if (!out)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    CU_TRY(e->lab.ensure(hs->total));
+    const lck::DelimSlsTables t{e->in.as<uint8_t>(), e->ev_off.as<uint32_t>(), e->ev_len.as<uint32_t>(),
+                                e->out_a.as<uint8_t>(), e->out_b.as<uint32_t>(), e->out_c.as<uint32_t>(),
+                                e->out_d.as<uint32_t>(), e->out_e.as<uint32_t>()};
+    lck::launch_delim_sls_emit(c, t, d_time, d_ns, n, e->lab_off.as<uint64_t>(), e->cnt.as<uint32_t>(),
+                               e->lab.as<uint8_t>(), e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(out, e->lab.p, hs->total, cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(cudaStreamSynchronize(e->stream));
     return LC_OK;
 }

@@ -2,7 +2,8 @@
 // that the sm_90a kernels execute once per log line.  Written as __host__ __device__ so that the
 // exact same statements can be exercised on the CPU by the test-only emulation library under
 // tests/emul/ (which validates the COMPILER's tables against the oracle without a GPU).  The product
-// library only ever calls these from device code.
+// library only ever calls these from device code, apart from the host-side configuration check of the
+// delimiter-fed SLS serialiser (lc_delim_sls_setup).
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -838,3 +839,383 @@ LC_HD void lc_sls_emit_log_t(uint8_t* out, uint32_t time, bool has_ns, uint32_t 
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// f4, delimiter-fed: the Log record of one event that ProcessorParseDelimiterNative::Process leaves behind, written
+// straight from the delimiter stage's result tables (ProcessorParseDelimiterNative.cpp:206-364; the host class's
+// ProcessImpl in Processors.cpp).  The event is "flat" on entry: a LogEvent whose only content is SourceKey -> line.
+//
+// One body function serves both passes: with LcSlsCount it only counts the bytes, with LcSlsWrite it writes them.
+// Sink interface: put(p, n) = tag / length bytes (lane 0 writes), copy(p, n) = key / value bytes (all lanes share),
+// unquote(p, n, out_n, quote) = a quoted column with its doubled quotes collapsed (AddFieldWithUnQuote, :83-113).
+
+// multi-byte separator (or quote == separator): ProcessorParseDelimiterNative::SplitString (:366-409), the statements
+// of the delimiter kernel's split branch; push(field_start, field_len, 0) per column
+template <class Push>
+LC_HD void lc_delim_split(const uint8_t* v, int32_t begIdx, int32_t endIdx, const uint8_t* sep, uint32_t d,
+                          uint32_t nkeys, bool extend, Push& push) {
+    const uint32_t size = (uint32_t)(endIdx - begIdx);
+    if (d > size) {
+        push((uint32_t)begIdx, size, 0u);
+        return;
+    }
+    uint32_t nf = 0, pos = (uint32_t)begIdx;
+    const uint32_t top = (uint32_t)endIdx - d;
+    bool done = false;
+    while (pos <= top && !done) {
+        uint32_t pos2 = (uint32_t)endIdx;
+        for (uint32_t q = pos; q + d <= (uint32_t)endIdx; ++q) {
+            bool eq = true;
+            for (uint32_t t = 0; t < d; ++t)
+                eq = eq && v[q + t] == sep[t];
+            if (eq) {
+                pos2 = q;
+                break;
+            }
+        }
+        push(pos, pos2 - pos, 0u);
+        ++nf;
+        if (pos2 == (uint32_t)endIdx) {
+            done = true;
+            break;
+        }
+        pos = pos2 + d;
+        if (nf >= nkeys && !extend) {
+            push(pos2, (uint32_t)endIdx - pos2, 0u);
+            ++nf;
+            done = true;
+        }
+    }
+    if (!done && pos <= (uint32_t)endIdx)
+        push(pos, (uint32_t)endIdx - pos, 0u);
+}
+
+#define LC_DELIM_SLS_EXTEND 0u
+#define LC_DELIM_SLS_KEEP 1u
+#define LC_DELIM_SLS_DISCARD 2u
+#define LC_DELIM_SLS_NONE 0xFFFFFFFFu
+
+// Configuration.  Every key string lives in `keys`: key k < nkeys is [key_at[k], key_at[k + 1]), then come SourceKey,
+// RenamedSourceKey and "__raw_log__" (key_at has nkeys + 4 entries).
+struct LcDelimSlsCfg {
+    uint8_t sep[4];
+    uint32_t sep_len;
+    uint8_t quote;
+    uint32_t use_quote;  // sep_len == 1 && quote != sep[0]: the quote state machine parsed the rows
+    uint32_t mode;       // LC_DELIM_SLS_EXTEND / KEEP / DISCARD (OverflowedFieldsTreatment)
+    uint32_t nkeys;
+    uint32_t max_fields; // row width of the tables
+    const uint8_t* keys;
+    const uint32_t* key_at;
+    uint32_t src_overwritten; // SourceKey is one of the keys (mSourceKeyOverwritten)
+    uint32_t src_col;         // the column that replaces the source content in place, or NONE
+    uint32_t ren_col;         // the column whose key is RenamedSourceKey (not a skipped "_"), or NONE
+    uint32_t ren_xcol;        // N when RenamedSourceKey is "__column<N>__", or NONE
+    uint32_t ren_is_src;      // RenamedSourceKey == SourceKey
+    uint32_t ren_is_raw;      // RenamedSourceKey == "__raw_log__"
+    uint32_t keep_fail, keep_succeed, copy_raw;
+};
+
+// One event: its line base[eo, eo + elen) and its row of the delimiter tables (f_off holds offsets into base).
+struct LcDelimSlsRow {
+    uint32_t eo, elen;
+    uint32_t status, nf;
+    const uint32_t* fo;
+    const uint32_t* fl;
+    const uint32_t* fd;
+    uint32_t time;
+    bool has_ns;
+    uint32_t ns;
+};
+
+struct LcSlsCount {
+    uint32_t n;
+    LC_HD void put(const uint8_t*, uint32_t k) { n += k; }
+    LC_HD void copy(const uint8_t*, uint32_t k) { n += k; }
+    LC_HD void unquote(const uint8_t*, uint32_t, uint32_t out_n, uint8_t) { n += out_n; }
+};
+
+// writes at out[at...], never at or beyond `lim` (the record's size); nlanes lanes share the copies
+struct LcSlsWrite {
+    uint8_t* out;
+    uint32_t at, lim, lane, nlanes;
+    LC_HD void put(const uint8_t* p, uint32_t k) {
+        if (lane == 0)
+            for (uint32_t j = 0; j < k; ++j)
+                if (at + j < lim)
+                    out[at + j] = p[j];
+        at += k;
+    }
+    LC_HD void copy(const uint8_t* p, uint32_t k) {
+        for (uint32_t j = lane; j < k; j += nlanes)
+            if (at + j < lim)
+                out[at + j] = p[j];
+        at += k;
+    }
+    LC_HD void unquote(const uint8_t* p, uint32_t k, uint32_t out_n, uint8_t q) {
+        if (lane == 0) {
+            uint32_t w = 0;
+            for (uint32_t i = 0; i < k && w < out_n; ++i) {
+                if (p[i] == q) {
+                    if (i + 1 < k && p[i + 1] == q) {
+                        if (at + w < lim)
+                            out[at + w] = q;
+                        ++w;
+                        ++i;
+                    }
+                } else {
+                    if (at + w < lim)
+                        out[at + w] = p[i];
+                    ++w;
+                }
+            }
+        }
+        at += out_n;
+    }
+};
+
+// "__column" + decimal(idx) + "__" into k[20]; returns its length
+LC_HD uint32_t lc_delim_column_key(uint32_t idx, uint8_t* k) {
+    k[0] = '_', k[1] = '_', k[2] = 'c', k[3] = 'o', k[4] = 'l', k[5] = 'u', k[6] = 'm', k[7] = 'n';
+    uint32_t digits = 1;
+    for (uint32_t t = idx; t >= 10; t /= 10)
+        ++digits;
+    uint32_t t = idx;
+    for (uint32_t d = digits; d-- > 0; t /= 10)
+        k[8 + d] = (uint8_t)('0' + t % 10);
+    k[8 + digits] = '_';
+    k[9 + digits] = '_';
+    return 10 + digits;
+}
+
+// tag + length prefixes of one Contents entry, its key bytes, then the value's tag + length (the value follows)
+template <class S>
+LC_HD void lc_sls_pair_open(S& s, const uint8_t* key, uint32_t kl, uint32_t vl) {
+    uint8_t h[12];
+    uint32_t n = 0;
+    h[n++] = 0x12;
+    n += lc_put_varint(h + n, lc_sls_pair_inner(kl, vl));
+    h[n++] = 0x0A;
+    n += lc_put_varint(h + n, kl);
+    s.put(h, n);
+    s.copy(key, kl);
+    n = 0;
+    h[n++] = 0x12;
+    n += lc_put_varint(h + n, vl);
+    s.put(h, n);
+}
+
+// Columns j0 <= j < j1 of the row in order: f(j, offset in base, raw length, doubled quotes).  From the table when it
+// holds them; a row with more columns than the table holds is walked again from the start of its line with the same
+// state machine (or split) that produced the table.  Only such rows, which are rare, pay for the walk.
+template <class F>
+LC_HD void lc_delim_sls_columns(const LcDelimSlsCfg& c, const uint8_t* base, const LcDelimSlsRow& r, uint32_t j0,
+                                uint32_t j1, F& f) {
+    if (r.nf <= c.max_fields || j1 <= c.max_fields) {
+        for (uint32_t j = j0; j < j1 && j < r.nf; ++j)
+            f(j, r.fo[j], r.fl[j], r.fd[j]);
+        return;
+    }
+    const uint8_t* v = base + r.eo;
+    int32_t end = (int32_t)r.elen, beg = 0; // the delimiter kernel's trim (:226-238)
+    while (end > 0 && (v[end - 1] == ' ' || v[end - 1] == '\r'))
+        --end;
+    while (beg < end && v[beg] == ' ')
+        ++beg;
+    uint32_t j = 0;
+    auto push = [&](uint32_t o, uint32_t l, uint32_t dq) {
+        if (j >= j0 && j < j1)
+            f(j, r.eo + o, l, dq);
+        ++j;
+    };
+    if (c.use_quote)
+        lc_delim_fsm(v, beg, end, c.sep[0], c.quote, push);
+    else
+        lc_delim_split(v, beg, end, c.sep, c.sep_len, c.nkeys, c.mode == LC_DELIM_SLS_EXTEND, push);
+}
+
+// The body of the event's Log record -- everything inside its Logs field: Time, Contents, Time_ns -- into sink s.
+// Returns the number of contents; 0 = the event has none (erased, or LogEvent::Empty) and emits no record.
+//   OK:      keys[j] -> column j in column order ("_" skipped and columns >= nkeys dropped in discard mode;
+//            __column<j>__ in extend mode; keep mode joins columns nkeys.. into __column<nkeys>__); a column whose key
+//            is SourceKey replaces the source content in place (first); then RenamedSourceKey -> line if
+//            KeepingSourceWhenParseSucceed and that key is not present yet
+//   failed:  RenamedSourceKey -> line [, __raw_log__ -> line] with KeepingSourceWhenParseFail, else erased
+//   blank:   untouched: SourceKey -> the whole, untrimmed line
+template <class S>
+LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, const LcDelimSlsRow& r, S& s) {
+    const uint32_t K_SRC = c.nkeys, K_REN = c.nkeys + 1, K_RAW = c.nkeys + 2;
+    auto kp = [&](uint32_t k) { return c.keys + c.key_at[k]; };
+    auto kl = [&](uint32_t k) { return c.key_at[k + 1] - c.key_at[k]; };
+    const uint8_t* line = base + r.eo;
+    {
+        uint8_t h[6];
+        h[0] = 0x08;
+        const uint32_t n = 1 + lc_put_varint(h + 1, r.time < (1u << 28) ? (1u << 28) : r.time); // always 5 bytes
+        s.put(h, n);
+    }
+    uint32_t cnt = 0;
+    auto whole_line = [&](uint32_t k) {
+        lc_sls_pair_open(s, kp(k), kl(k), r.elen);
+        s.copy(line, r.elen);
+        ++cnt;
+    };
+    auto value = [&](uint32_t off, uint32_t len, uint32_t dq) {
+        if (c.use_quote && dq)
+            s.unquote(base + off, len, len - dq, c.quote);
+        else
+            s.copy(base + off, len);
+    };
+    if (r.status == 2) { // LC_DELIM_BLANK
+        whole_line(K_SRC);
+    } else if (r.status != 0) { // LC_DELIM_PARSE_FAIL / LC_DELIM_COLUMNS
+        if (c.keep_fail) {
+            whole_line(K_REN);
+            if (c.copy_raw && !c.ren_is_raw)
+                whole_line(K_RAW);
+        }
+    } else {
+        const uint32_t nf = r.nf, nk = c.nkeys;
+        if (c.src_overwritten) {
+            if (c.src_col != LC_DELIM_SLS_NONE && c.src_col < nf) {
+                const uint32_t j = c.src_col; // < nkeys < max_fields: always in the table
+                const uint32_t dq = c.use_quote ? r.fd[j] : 0u;
+                lc_sls_pair_open(s, kp(K_SRC), kl(K_SRC), r.fl[j] - dq);
+                value(r.fo[j], r.fl[j], dq);
+                ++cnt;
+            } else {
+                whole_line(K_SRC);
+            }
+        }
+        const bool joined = c.mode == LC_DELIM_SLS_KEEP && c.use_quote;
+        const uint32_t jend = c.mode == LC_DELIM_SLS_EXTEND                 ? 0xFFFFFFFFu
+                              : (c.mode == LC_DELIM_SLS_KEEP && !joined) ? nk + 1 // the split's remainder column
+                                                                          : nk;
+        auto col = [&](uint32_t j, uint32_t off, uint32_t len, uint32_t dq) {
+            if (j == c.src_col)
+                return;
+            if (!c.use_quote)
+                dq = 0;
+            if (j < nk) {
+                if (c.mode == LC_DELIM_SLS_DISCARD && kl(j) == 1 && kp(j)[0] == '_')
+                    return;
+                lc_sls_pair_open(s, kp(j), kl(j), len - dq);
+            } else {
+                uint8_t k[20];
+                lc_sls_pair_open(s, k, lc_delim_column_key(j, k), len - dq);
+            }
+            value(off, len, dq);
+            ++cnt;
+        };
+        lc_delim_sls_columns(c, base, r, 0u, jend, col);
+        if (joined && nf > nk) { // sep[0] + unquoted column, for each column from nkeys on
+            uint32_t vl = 0;
+            auto measure = [&](uint32_t, uint32_t, uint32_t len, uint32_t dq) { vl += 1 + len - dq; };
+            lc_delim_sls_columns(c, base, r, nk, 0xFFFFFFFFu, measure);
+            uint8_t k[20];
+            lc_sls_pair_open(s, k, lc_delim_column_key(nk, k), vl);
+            auto piece = [&](uint32_t, uint32_t off, uint32_t len, uint32_t dq) {
+                s.put(c.sep, 1);
+                value(off, len, dq);
+            };
+            lc_delim_sls_columns(c, base, r, nk, 0xFFFFFFFFu, piece);
+            ++cnt;
+        }
+        if (c.keep_succeed) { // AddLog(RenamedSourceKey, line, false): only when that key is not present
+            const bool present =
+                (c.ren_is_src && c.src_overwritten) || (c.ren_col != LC_DELIM_SLS_NONE && c.ren_col < nf) ||
+                (c.ren_xcol != LC_DELIM_SLS_NONE && c.ren_xcol >= nk && c.ren_xcol < nf &&
+                 (c.mode == LC_DELIM_SLS_EXTEND || (c.mode == LC_DELIM_SLS_KEEP && c.ren_xcol == nk)));
+            if (!present)
+                whole_line(K_REN);
+        }
+    }
+    if (r.has_ns) {
+        const uint8_t h[5] = {0x25, (uint8_t)r.ns, (uint8_t)(r.ns >> 8), (uint8_t)(r.ns >> 16), (uint8_t)(r.ns >> 24)};
+        s.put(h, 5);
+    }
+    return cnt;
+}
+
+
+// Host side: checks a configuration of the delimiter-fed serialiser and fills `c` and the key strings.  key_bytes
+// needs sum(key_lens) + source_len + renamed_len + 11 bytes, key_at nkeys + 4 entries; c.keys / c.key_at are left to
+// the caller (device copies).  Returns nullptr, or why the configuration is refused: each refused case would need
+// SetContentNoCopy's replace-in-place of an earlier content, which the flat-event model does not describe.
+inline const char* lc_delim_sls_setup(const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard,
+                                      const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                                      const char* source_key, uint32_t source_len, const char* renamed_key,
+                                      uint32_t renamed_len, int keep_fail, int keep_succeed, int copy_raw,
+                                      uint32_t max_fields, LcDelimSlsCfg* c, uint8_t* key_bytes, uint32_t* key_at) {
+    if (sep_len < 1 || sep_len > 4 || (extend && discard))
+        return "bad arguments (separator must be 1..4 bytes; extend and discard exclude each other)";
+    if (max_fields < nkeys + 1)
+        return "max_fields must be at least nkeys + 1";
+    const bool disc = discard != 0, overflow_keys = !disc;
+    auto eq = [](const char* a, uint32_t la, const char* b, uint32_t lb) { return la == lb && !memcmp(a, b, la); };
+    auto is_skip = [&](uint32_t k) { return disc && key_lens[k] == 1 && keys[k][0] == '_'; };
+    // "__column<digits>__": the form of the generated overflow keys; *idx = the value when it is canonical decimal
+    auto column_form = [](const char* s, uint32_t l, uint32_t* idx) {
+        if (l < 11 || memcmp(s, "__column", 8) || s[l - 1] != '_' || s[l - 2] != '_')
+            return false;
+        uint64_t v = 0;
+        for (uint32_t i = 8; i < l - 2; ++i) {
+            if (s[i] < '0' || s[i] > '9')
+                return false;
+            v = v * 10 + (uint64_t)(s[i] - '0');
+            if (v >= LC_DELIM_SLS_NONE)
+                v = LC_DELIM_SLS_NONE;
+        }
+        const bool canonical = (l - 10 == 1 || s[8] != '0') && v < LC_DELIM_SLS_NONE;
+        *idx = canonical ? (uint32_t)v : LC_DELIM_SLS_NONE;
+        return true;
+    };
+    uint32_t dummy;
+    for (uint32_t a = 0; a < nkeys; ++a) {
+        if (overflow_keys && column_form(keys[a], key_lens[a], &dummy))
+            return "a key of the form __column<digits>__ collides with the generated overflow keys";
+        for (uint32_t b = a + 1; b < nkeys; ++b)
+            if (eq(keys[a], key_lens[a], keys[b], key_lens[b]) && !is_skip(a))
+                return "keys must be distinct (a repeated key overwrites its earlier content)";
+    }
+    if (overflow_keys && column_form(source_key, source_len, &dummy))
+        return "a source key of the form __column<digits>__ collides with the generated overflow keys";
+    memset(c, 0, sizeof *c);
+    memcpy(c->sep, sep, sep_len);
+    c->sep_len = sep_len;
+    c->quote = quote;
+    c->use_quote = sep_len == 1 && quote != sep[0];
+    c->mode = extend ? LC_DELIM_SLS_EXTEND : (disc ? LC_DELIM_SLS_DISCARD : LC_DELIM_SLS_KEEP);
+    c->nkeys = nkeys;
+    c->max_fields = max_fields;
+    c->src_col = c->ren_col = LC_DELIM_SLS_NONE;
+    for (uint32_t k = 0; k < nkeys; ++k) {
+        if (eq(keys[k], key_lens[k], source_key, source_len)) {
+            c->src_overwritten = 1;
+            if (!is_skip(k))
+                c->src_col = k;
+        }
+        if (eq(keys[k], key_lens[k], renamed_key, renamed_len) && !is_skip(k))
+            c->ren_col = k;
+    }
+    if (!overflow_keys || !column_form(renamed_key, renamed_len, &c->ren_xcol))
+        c->ren_xcol = LC_DELIM_SLS_NONE;
+    c->ren_is_src = eq(renamed_key, renamed_len, source_key, source_len);
+    c->ren_is_raw = eq(renamed_key, renamed_len, "__raw_log__", 11);
+    c->keep_fail = keep_fail != 0;
+    c->keep_succeed = keep_succeed != 0;
+    c->copy_raw = copy_raw != 0;
+    uint32_t at = 0;
+    auto add = [&](uint32_t k, const char* s, uint32_t l) {
+        key_at[k] = at;
+        if (l)
+            memcpy(key_bytes + at, s, l);
+        at += l;
+    };
+    for (uint32_t k = 0; k < nkeys; ++k)
+        add(k, keys[k], key_lens[k]);
+    add(nkeys, source_key, source_len);
+    add(nkeys + 1, renamed_key, renamed_len);
+    add(nkeys + 2, "__raw_log__", 11);
+    key_at[nkeys + 3] = at;
+    return nullptr;
+}

@@ -3603,4 +3603,94 @@ void launch_sls_parsed_emit(const SlsParsedArgs& a, const uint32_t* d_ev_time, c
                                                                              d_body_size, d_out);
 }
 
+// ---- f4, delimiter-fed: Log records of the events a ProcessorParseDelimiterNative leaves behind, straight from the
+// delimiter stage's tables.  Both passes run the same per-row function (lc_exec.cuh: lc_delim_sls_body) -- the size
+// pass with a counting sink, one thread per event; the emit pass with a writing sink, one warp per event.
+__device__ __forceinline__ LcDelimSlsRow delim_sls_row(const LcDelimSlsCfg& c, const DelimSlsTables& t,
+                                                       const uint32_t* ev_time, const uint32_t* ev_ns, uint64_t i) {
+    LcDelimSlsRow r;
+    r.eo = t.ev_off[i];
+    r.elen = t.ev_len[i];
+    r.status = t.status[i];
+    r.nf = t.nfields[i];
+    r.fo = t.f_off + i * c.max_fields;
+    r.fl = t.f_len + i * c.max_fields;
+    r.fd = t.f_dq + i * c.max_fields;
+    r.time = ev_time ? ev_time[i] : 0u;
+    r.has_ns = ev_ns && ev_ns[i] != 0xFFFFFFFFu;
+    r.ns = r.has_ns ? ev_ns[i] : 0u;
+    return r;
+}
+
+__global__ void __launch_bounds__(256)
+    delim_sls_size_kernel(LcDelimSlsCfg c, DelimSlsTables t, const uint32_t* __restrict__ ev_ns, uint64_t n,
+                          uint32_t* __restrict__ rec_size, uint32_t* __restrict__ body_size,
+                          unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t ok = 0, failed = 0, erased = 0, blank = 0;
+    if (i < n) {
+        const LcDelimSlsRow r = delim_sls_row(c, t, nullptr, ev_ns, i);
+        LcSlsCount s{0};
+        const uint32_t cnt = lc_delim_sls_body(c, t.base, r, s);
+        const uint32_t body = cnt ? s.n : 0u;
+        rec_size[i] = cnt ? 1 + lc_varint_size(body) + body : 0u;
+        body_size[i] = body;
+        ok = r.status == 0;
+        blank = r.status == 2;
+        failed = !ok && !blank;
+        erased = failed && !c.keep_fail;
+    }
+    if (counters) { // successful, failed, discarded, blank: one atomic per warp and counter
+        ok = __reduce_add_sync(0xFFFFFFFFu, ok);
+        failed = __reduce_add_sync(0xFFFFFFFFu, failed);
+        erased = __reduce_add_sync(0xFFFFFFFFu, erased);
+        blank = __reduce_add_sync(0xFFFFFFFFu, blank);
+        if ((threadIdx.x & 31) == 0) {
+            if (ok)
+                atomicAdd(counters + 0, (unsigned long long)ok);
+            if (failed)
+                atomicAdd(counters + 1, (unsigned long long)failed);
+            if (erased)
+                atomicAdd(counters + 2, (unsigned long long)erased);
+            if (blank)
+                atomicAdd(counters + 3, (unsigned long long)blank);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    delim_sls_emit_kernel(LcDelimSlsCfg c, DelimSlsTables t, const uint32_t* __restrict__ ev_time,
+                          const uint32_t* __restrict__ ev_ns, uint64_t n, const uint64_t* __restrict__ rec_off,
+                          const uint32_t* __restrict__ body_size, uint8_t* __restrict__ out) {
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n)
+        return;
+    const uint32_t body = body_size[i];
+    if (!body)
+        return; // erased or LogEvent::Empty: no record (SLSSerializer.cpp:383-385)
+    const LcDelimSlsRow r = delim_sls_row(c, t, ev_time, ev_ns, i);
+    uint8_t h[6];
+    h[0] = 0x0A;
+    const uint32_t hn = 1 + lc_put_varint(h + 1, body);
+    LcSlsWrite s{out + rec_off[i], 0u, hn + body, threadIdx.x & 31, 32};
+    s.put(h, hn);
+    lc_delim_sls_body(c, t.base, r, s);
+}
+
+void launch_delim_sls_sizes(const LcDelimSlsCfg& c, const DelimSlsTables& t, const uint32_t* d_ev_ns, uint64_t n,
+                            uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                            cudaStream_t st) {
+    if (n)
+        delim_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, d_ev_ns, n, d_rec_size, d_body_size,
+                                                                            d_counters);
+}
+
+void launch_delim_sls_emit(const LcDelimSlsCfg& c, const DelimSlsTables& t, const uint32_t* d_ev_time,
+                           const uint32_t* d_ev_ns, uint64_t n, const uint64_t* d_rec_off, const uint32_t* d_body_size,
+                           uint8_t* d_out, cudaStream_t st) {
+    if (n)
+        delim_sls_emit_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, t, d_ev_time, d_ev_ns, n, d_rec_off,
+                                                                                 d_body_size, d_out);
+}
+
 } // namespace lck

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+struct LcDelimSlsCfg; // lc_exec.cuh
+
 namespace lck {
 
 constexpr int kScanThreads = 256;
@@ -212,5 +214,25 @@ void launch_sls_parsed_sizes(const SlsParsedArgs& a, const uint32_t* d_ev_ns, ui
                              uint32_t* d_body_size, cudaStream_t st);
 void launch_sls_parsed_emit(const SlsParsedArgs& a, const uint32_t* d_ev_time, const uint32_t* d_ev_ns, uint64_t n,
                             const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out, cudaStream_t st);
+
+// f4, delimiter-fed: Log records from the delimiter stage's result tables (launch_delim) + the configuration of
+// lc_exec.cuh (LcDelimSlsCfg, key strings on the device).  Sizes as for launch_sls_sizes; d_counters (or nullptr):
+// u64 [4] += successful, failed, discarded, blank events.
+struct DelimSlsTables {
+    const uint8_t* base;
+    const uint32_t* ev_off;
+    const uint32_t* ev_len;
+    const uint8_t* status;
+    const uint32_t* nfields;
+    const uint32_t* f_off; // [n][max_fields]
+    const uint32_t* f_len;
+    const uint32_t* f_dq;
+};
+void launch_delim_sls_sizes(const LcDelimSlsCfg& c, const DelimSlsTables& t, const uint32_t* d_ev_ns, uint64_t n,
+                            uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                            cudaStream_t st);
+void launch_delim_sls_emit(const LcDelimSlsCfg& c, const DelimSlsTables& t, const uint32_t* d_ev_time,
+                           const uint32_t* d_ev_ns, uint64_t n, const uint64_t* d_rec_off, const uint32_t* d_body_size,
+                           uint8_t* d_out, cudaStream_t st);
 
 } // namespace lck

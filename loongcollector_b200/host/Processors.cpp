@@ -1,5 +1,7 @@
 #include "Processors.h"
 
+#include "../csrc/lc_exec.cuh" // lc_delim_sls_setup: the configuration checks of lc_delim_parse_sls
+
 #include <stdlib.h>
 #include <string.h>
 
@@ -966,7 +968,28 @@ bool ProcessorParseDelimiterNative::Init(const Json::Value& config) {
             mOverflowedFieldsTreatment = OverflowedFieldsTreatment::DISCARD;
     }
     mExtractingPartialFields = mOverflowedFieldsTreatment == OverflowedFieldsTreatment::DISCARD;
-    return mCommonParserOptions.Init(config);
+    if (!mCommonParserOptions.Init(config))
+        return false;
+    // SerializeSls's one-pass device path takes the configurations lc_delim_parse_sls accepts
+    std::vector<const char*> kp;
+    std::vector<uint32_t> kl;
+    size_t kbytes = mSourceKey.size() + mCommonParserOptions.mRenamedSourceKey.size() + 11;
+    for (const auto& k : mKeys) {
+        kp.push_back(k.data());
+        kl.push_back((uint32_t)k.size());
+        kbytes += k.size();
+    }
+    std::vector<uint8_t> kb(kbytes + 1);
+    std::vector<uint32_t> at(mKeys.size() + 4);
+    LcDelimSlsCfg c;
+    mDeviceSls = lc_delim_sls_setup(reinterpret_cast<const uint8_t*>(mSeparator.data()), (uint32_t)mSeparator.size(),
+                                    (uint8_t)mQuote, mOverflowedFieldsTreatment == OverflowedFieldsTreatment::EXTEND,
+                                    mExtractingPartialFields, kp.data(), kl.data(), (uint32_t)mKeys.size(),
+                                    mSourceKey.data(), (uint32_t)mSourceKey.size(),
+                                    mCommonParserOptions.mRenamedSourceKey.data(),
+                                    (uint32_t)mCommonParserOptions.mRenamedSourceKey.size(), 0, 0, 0,
+                                    (uint32_t)mKeys.size() + 16, &c, kb.data(), at.data()) == nullptr;
+    return true;
 }
 
 std::vector<std::pair<std::string, uint64_t>> ProcessorParseDelimiterNative::Counters() const {
@@ -1746,6 +1769,37 @@ void PutString(std::string& out, StringView s) {
     PutVarint(out, (uint32_t)s.size());
     out.append(s.data(), s.size());
 }
+
+// group-level fields in tag (map) order, SLSSerializer.cpp:203-213,239-249
+std::string SlsGroupTail(PipelineEventGroup& group) {
+    std::string tail;
+    for (auto& tag : group.GetTags()) {
+        if (tag.first == StringView("__topic__")) {
+            tail.push_back(0x1A);
+            PutString(tail, tag.second);
+        } else if (tag.first == StringView("__source__")) {
+            tail.push_back(0x22);
+            PutString(tail, tag.second);
+        } else if (tag.first == StringView("__machine_uuid__")) {
+            tail.push_back(0x2A);
+            PutString(tail, tag.second);
+        } else {
+            std::string inner;
+            inner.push_back(0x0A);
+            PutString(inner, tag.first);
+            inner.push_back(0x12);
+            PutString(inner, tag.second);
+            tail.push_back(0x32);
+            PutVarint(tail, (uint32_t)inner.size());
+            tail += inner;
+        }
+    }
+    return tail;
+}
+
+std::string SizeLimitError(uint64_t size, int32_t limit) {
+    return "log group exceeds size limit\tgroup size: " + ToString(size) + "\tsize limit: " + ToString((uint64_t)limit);
+}
 } // namespace
 
 bool SLSEventGroupSerializer::Serialize(PipelineEventGroup& group, std::string& res, std::string& errorMsg) const {
@@ -1820,37 +1874,14 @@ bool SLSEventGroupSerializer::Serialize(PipelineEventGroup& group, std::string& 
         base = packed.data();
         baseLen = total;
     }
-    // group-level fields in tag (map) order, :203-213,239-249
-    std::string tail;
-    for (auto& tag : group.GetTags()) {
-        if (tag.first == StringView("__topic__")) {
-            tail.push_back(0x1A);
-            PutString(tail, tag.second);
-        } else if (tag.first == StringView("__source__")) {
-            tail.push_back(0x22);
-            PutString(tail, tag.second);
-        } else if (tag.first == StringView("__machine_uuid__")) {
-            tail.push_back(0x2A);
-            PutString(tail, tag.second);
-        } else {
-            std::string inner;
-            inner.push_back(0x0A);
-            PutString(inner, tag.first);
-            inner.push_back(0x12);
-            PutString(inner, tag.second);
-            tail.push_back(0x32);
-            PutVarint(tail, (uint32_t)inner.size());
-            tail += inner;
-        }
-    }
+    const std::string tail = SlsGroupTail(group);
     uint64_t need = 0;
     int rc = lc_sls_serialize_logs(Engine(), base, baseLen, n, evTime.data(), evNs.data(), entBegin.data(), kOff.data(),
                                    kLen.data(), vOff.data(), vLen.data(), nullptr, 0, &need);
     if (rc != LC_OK && rc != LC_ERR_CAPACITY)
         Check(rc, "lc_sls_serialize_logs");
     if ((int64_t)(need + tail.size()) > (int64_t)mMaxSendLogGroupSize) {
-        errorMsg = "log group exceeds size limit\tgroup size: " + ToString(need + tail.size())
-                   + "\tsize limit: " + ToString((uint64_t)mMaxSendLogGroupSize);
+        errorMsg = SizeLimitError(need + tail.size(), mMaxSendLogGroupSize);
         return false;
     }
     res.resize(need);
@@ -1858,6 +1889,88 @@ bool SLSEventGroupSerializer::Serialize(PipelineEventGroup& group, std::string& 
                                 kLen.data(), vOff.data(), vLen.data(), reinterpret_cast<uint8_t*>(&res[0]), need, &need),
           "lc_sls_serialize_logs");
     res += tail;
+    return true;
+}
+
+bool ProcessorParseDelimiterNative::SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out,
+                                                 std::string& err) {
+    SLSEventGroupSerializer ser;
+    ser.mEnableTimestampNanosecond = enableNs;
+    EventsContainer& events = group.MutableEvents();
+    bool flat = mDeviceSls && !group.HasMetadata(EventGroupMetaKey::LOG_FILE_OFFSET_KEY);
+    for (size_t i = 0; flat && i < events.size(); ++i) {
+        if (!events[i].Is<LogEvent>()) {
+            flat = false;
+            break;
+        }
+        const LogEvent& ev = events[i].Cast<LogEvent>();
+        const LogEvent::Content* c = ev.FirstLive();
+        flat = ev.Size() == 1 && c && c->first.first == StringView(mSourceKey);
+    }
+    if (!flat) {
+        Process(group);
+        return ser.Serialize(group, out, err);
+    }
+    // every event is SourceKey -> line: parse and serialise in one device pass, only the wire bytes come back
+    const size_t n = events.size();
+    FlatBatch batch;
+    std::vector<uint32_t> evTime(n), evNs(n, LC_SLS_NO_NS);
+    for (size_t i = 0; i < n; ++i) {
+        const LogEvent& ev = events[i].Cast<LogEvent>();
+        batch.Add(i, ev.FirstLive()->first.second);
+        evTime[i] = (uint32_t)ev.GetTimestamp();
+        if (enableNs && ev.GetTimestampNanosecond())
+            evNs[i] = ev.GetTimestampNanosecond().value();
+    }
+    batch.Finish(*group.GetSourceBuffer());
+    std::vector<const char*> kp;
+    std::vector<uint32_t> kl;
+    size_t keyBytes = 0;
+    for (const auto& k : mKeys) {
+        kp.push_back(k.data());
+        kl.push_back((uint32_t)k.size());
+        keyBytes += k.size();
+    }
+    const std::string& renamed = mCommonParserOptions.mRenamedSourceKey;
+    std::string res((size_t)(2 * batch.baseLen + n * (64 + keyBytes + renamed.size()) + 64), '\0');
+    uint64_t need = 0, ctr[4] = {0, 0, 0, 0};
+    const std::string tail = SlsGroupTail(group);
+    auto call = [&]() {
+        return lc_delim_parse_sls(
+            Engine(), batch.base, batch.baseLen, batch.off.data(), batch.len.data(), n, evTime.data(), evNs.data(),
+            reinterpret_cast<const uint8_t*>(mSeparator.data()), (uint32_t)mSeparator.size(), (uint8_t)mQuote,
+            mOverflowedFieldsTreatment == OverflowedFieldsTreatment::EXTEND, mExtractingPartialFields,
+            mAllowingShortenedFields, (uint32_t)mKeys.size() + 16, kp.data(), kl.data(), (uint32_t)mKeys.size(),
+            mSourceKey.data(), (uint32_t)mSourceKey.size(), renamed.data(), (uint32_t)renamed.size(),
+            mCommonParserOptions.mKeepingSourceWhenParseFail, mCommonParserOptions.mKeepingSourceWhenParseSucceed,
+            mCommonParserOptions.mCopingRawLog, reinterpret_cast<uint8_t*>(&res[0]), res.size(), &need, ctr);
+    };
+    int rc = call();
+    if (rc == LC_ERR_CAPACITY && (int64_t)(need + tail.size()) <= (int64_t)ser.mMaxSendLogGroupSize) {
+        res.resize(need);
+        rc = call();
+    }
+    if (rc != LC_ERR_CAPACITY)
+        Check(rc, "lc_delim_parse_sls");
+    // the counters Process would have moved (a blank value counts as out_failed, :220-242)
+    mOutSuccessfulEventsTotal.Add(ctr[0]);
+    mOutFailedEventsTotal.Add(ctr[1] + ctr[3]);
+    mDiscardedEventsTotal.Add(ctr[2]);
+    // SLSEventGroupSerializer::Serialize's checks, in its order
+    if (n == ctr[2]) {
+        err = "empty event group";
+        return false;
+    }
+    if (need == 0) {
+        err = "all empty logs";
+        return false;
+    }
+    if ((int64_t)(need + tail.size()) > (int64_t)ser.mMaxSendLogGroupSize) {
+        err = SizeLimitError(need + tail.size(), ser.mMaxSendLogGroupSize);
+        return false;
+    }
+    res.resize(need);
+    out = res + tail;
     return true;
 }
 

@@ -214,12 +214,19 @@ public:
     bool mExtractingPartialFields = false;
     CommonParserOptions mCommonParserOptions;
     Counter mDiscardedEventsTotal, mOutFailedEventsTotal, mOutKeyNotFoundEventsTotal, mOutSuccessfulEventsTotal;
+    // Process(group) followed by SLSEventGroupSerializer::Serialize (enableNs = its mEnableTimestampNanosecond): the
+    // same bytes or error message, and the same counter updates.  When every event is flat (a LogEvent whose only
+    // content is SourceKey -> line), the group carries no log.file.offset metadata and the configuration is one
+    // lc_delim_parse_sls accepts, the group is parsed and serialised in one device pass (lc_delim_parse_sls): the
+    // delimiter tables never leave the GPU and the group's events are left as they were.  Otherwise Process runs.
+    bool SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out, std::string& err);
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
     bool mSourceKeyOverwritten = false;
+    bool mDeviceSls = false; // the configuration passes lc_delim_parse_sls's checks
 };
 
 // First "next" row (SURVEY.md 8f): regex include / exclude filter.  Every regex leaf of the rule / expression is

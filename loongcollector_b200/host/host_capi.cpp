@@ -122,6 +122,52 @@ char* lc_host_sls_serialize(const char* group_json, int enable_ns, unsigned long
     }
 }
 
+char* lc_host_processor_serialize_sls(lc_host_processor_t* p, const char* group_json, int enable_ns,
+                                      int process_then_serialize, unsigned long long* len_out, char** err_out,
+                                      char** fail_out) {
+    if (err_out)
+        *err_out = nullptr;
+    if (fail_out)
+        *fail_out = nullptr;
+    if (len_out)
+        *len_out = 0;
+    try {
+        auto* d = dynamic_cast<ProcessorParseDelimiterNative*>(p->proc.get());
+        if (!d)
+            throw std::runtime_error("not a processor_parse_delimiter_native");
+        PipelineEventGroup group(std::make_shared<SourceBuffer>());
+        if (!group.FromJsonString(group_json ? group_json : "null"))
+            throw std::runtime_error("group JSON does not parse");
+        const uint64_t errs = d->EngineErrors();
+        std::string res, err;
+        bool ok;
+        if (process_then_serialize) {
+            d->Process(group);
+            SLSEventGroupSerializer ser;
+            ser.mEnableTimestampNanosecond = enable_ns != 0;
+            ok = ser.Serialize(group, res, err);
+        } else {
+            ok = d->SerializeSls(group, enable_ns != 0, res, err);
+        }
+        if (d->EngineErrors() != errs)
+            throw std::runtime_error("engine error inside Process: " + d->LastError());
+        if (!ok) {
+            if (err_out)
+                *err_out = dup(err);
+            return nullptr;
+        }
+        char* out = (char*)malloc(res.size() + 1);
+        memcpy(out, res.data(), res.size());
+        out[res.size()] = 0;
+        if (len_out)
+            *len_out = res.size();
+        return out;
+    } catch (const std::exception& e) {
+        if (fail_out)
+            *fail_out = dup(std::string("SerializeSls threw: ") + e.what());
+        return nullptr;
+    }
+}
 
 // What PluginRegistry::LoadProcessorPlugin + DynamicCProcessorProxy do with a dynamic plugin
 // (PluginRegistry.cpp:218-275, DynamicCProcessorProxy.cpp:21-36), step by step, on the plugin at so_path.
