@@ -267,13 +267,53 @@ int lc_sls_serialize_logs(lc_engine_t* e, const uint8_t* base, uint64_t base_len
  * :153-155); a failed event carries the one content fail_key -> the whole line when fail_key != NULL
  * (KeepingSourceWhenParseFail with RenamedSourceKey, :156-158) and is skipped otherwise (erased,
  * CommonParserOptions.cpp:99-117).  keys must be distinct.  d_ev_time_ns may be NULL; LC_SLS_NO_NS per event = no
- * Time_ns.  d_out receives the bytes on the device; *out_len (host) their count; LC_ERR_CAPACITY if > out_cap. */
+ * Time_ns.  d_out receives the bytes on the device; *out_len (host) their count; LC_ERR_CAPACITY if > out_cap.
+ * The fixed configuration of lc_sls_serialize_regex_dev below, which this calls with its own two content plans. */
 int lc_sls_serialize_parsed_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t base_len, const uint32_t* d_ev_off,
                                 const uint32_t* d_ev_len, const uint8_t* d_status, const uint32_t* d_cap_off,
                                 const uint32_t* d_cap_len, uint32_t row_pitch, uint64_t n, const char* const* keys,
                                 const uint32_t* key_lens, uint32_t nkeys, const char* fail_key, uint32_t fail_key_len,
                                 const uint32_t* d_ev_time, const uint32_t* d_ev_time_ns, uint8_t* d_out,
                                 uint64_t out_cap, uint64_t* out_len);
+
+/* The full regex -> serialise hand-over: the `Logs` fields of the events ProcessorParseRegexNative::Process leaves
+ * behind (ProcessorParseRegexNative.cpp:132-168, CommonParserOptions.cpp:91-117), written straight from the DEVICE
+ * tables of one lc_regex_parse_dev call (d_status, [n][row_pitch] d_cap_off / d_cap_len, parsed with nkeys keys) and
+ * the processor's configuration.  Every event is taken to be flat: a LogEvent whose only content is source_key -> its
+ * line.  The contents such an event ends with depend only on the configuration and its status, so the configuration is
+ * compiled once into two content plans -- LogEvent's SetContentNoCopy / DelContent applied to "the line" and
+ * "capture j" -- which the kernels walk per event:
+ *   LC_REGEX_OK: keys[j] -> capture j in key order; a repeated key overwrites the earlier content in place; a key
+ *     equal to source_key replaces the line in place and the source is not deleted, else it is; then renamed_key ->
+ *     line if keep_succeed and that key is not present.
+ *   LC_REGEX_NOMATCH / LC_REGEX_KEYS_MISMATCH: the source is deleted; with keep_fail renamed_key -> line, then
+ *     "__raw_log__" -> line if copy_raw, each unless that key is present; without keep_fail the event is erased.
+ *   whole_line != 0 (Regex "(.*)", :147-148): no regex ran and d_status / d_cap_off / d_cap_len may be NULL; every
+ *     event gets keys[0] (or "content" when nkeys == 0) -> line, and the source is deleted unless it is one of the keys.
+ * renamed_key is CommonParserOptions' RenamedSourceKey (source_key when not configured).  Events without contents
+ * emit nothing.  counters[3] (host, may be NULL) = ProcessorParseRegexNative's out_successful (every event not
+ * erased), out_failed (LC_REGEX_NOMATCH only, :227-244) and discarded.  d_ev_time_ns may be NULL; LC_SLS_NO_NS per
+ * event = no Time_ns.  d_out receives the bytes on the device; *out_len (host) their count; LC_ERR_CAPACITY if
+ * > out_cap (nothing written, *out_len and counters set). */
+int lc_sls_serialize_regex_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t base_len, const uint32_t* d_ev_off,
+                               const uint32_t* d_ev_len, uint64_t n, const uint8_t* d_status, const uint32_t* d_cap_off,
+                               const uint32_t* d_cap_len, uint32_t row_pitch, const char* const* keys,
+                               const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+                               uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+                               int keep_fail, int keep_succeed, int copy_raw, int whole_line,
+                               const uint32_t* d_ev_time, const uint32_t* d_ev_time_ns, uint8_t* d_out,
+                               uint64_t out_cap, uint64_t* out_len, uint64_t counters[3]);
+
+/* The same with HOST buffers: parse (lc_regex_parse with nkeys keys; re may be NULL in whole-line mode) and serialise
+ * in one call.  The arena goes up once, in chunks of whole events on a copy stream while earlier chunks are parsed and
+ * sized; the capture tables stay on the device and only the wire bytes (out, in event order) and counters[3] come
+ * back.  *out_len and counters are set on LC_OK and on LC_ERR_CAPACITY. */
+int lc_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base, uint64_t base_len,
+                       const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time,
+                       const uint32_t* ev_time_ns, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                       const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                       uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, int whole_line,
+                       uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[3]);
 
 /* Device-fed variant for the delimiter -> serialise hand-over: the `Logs` fields of the events a
  * ProcessorParseDelimiterNative leaves behind (ProcessorParseDelimiterNative.cpp:206-364), written straight from the

@@ -31,9 +31,9 @@ void lc_host_string_free(char* s);
  * bytes (free with lc_host_string_free) and their length, or NULL + *err_out = the reference's error message. */
 char* lc_host_sls_serialize(const char* group_json, int enable_ns, unsigned long long* len_out, char** err_out);
 
-/* ProcessorParseDelimiterNative::SerializeSls on the group described by group_json (p must be a
- * "processor_parse_delimiter_native"): the malloc'd wire bytes and their length, or NULL + *err_out = the serializer's
- * error message.  With process_then_serialize != 0 it runs Process(group) + SLSEventGroupSerializer::Serialize on the
+/* SerializeSls of the parse processor p on the group described by group_json (p must be a
+ * "processor_parse_delimiter_native" or a "processor_parse_regex_native"): the malloc'd wire bytes and their length,
+ * or NULL + *err_out = the serializer's error message.  With process_then_serialize != 0 it runs Process(group) + SLSEventGroupSerializer::Serialize on the
  * same in-memory group instead -- the result SerializeSls must equal byte for byte.  (lc_host_processor_process +
  * lc_host_sls_serialize differ from both in content order: a JSON round trip lists the contents by key.)  An engine
  * failure or a bad group returns NULL + *fail_out instead. */

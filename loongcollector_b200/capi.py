@@ -87,6 +87,9 @@ def lib():
                                              i32] + sls_cfg + [vp, vp, vp, u64, C.POINTER(u64)]
     L.lc_delim_parse_sls.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32, u8, i32, i32, i32, u32] + sls_cfg + \
         [vp, u64, C.POINTER(u64), vp]
+    L.lc_sls_serialize_regex_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32] + sls_cfg + \
+        [i32, vp, vp, vp, u64, C.POINTER(u64), vp]
+    L.lc_regex_parse_sls.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp] + sls_cfg + [i32, vp, u64, C.POINTER(u64), vp]
     _LIB = L
     return L
 
@@ -396,6 +399,51 @@ class Engine:
             return bytes(out[:need.value]), ctr
         _check(rc)
 
+    def sls_serialize_regex_dev(self, d_base, base_len, d_ev_off, d_ev_len, n, d_status, d_cap_off, d_cap_len,
+                                row_pitch, keys, source_key, renamed_key=None, keep_fail=False, keep_succeed=False,
+                                copy_raw=False, whole_line=False, d_ev_time=None, d_ev_time_ns=None, d_out=None,
+                                out_cap=0):
+        """Wire bytes of the events ProcessorParseRegexNative leaves behind, from the device tables of one
+        regex_parse_dev call (d_status / d_cap_* may be None in whole-line mode).  Returns (byte count written to d_out,
+        counters[3] = successful, failed, discarded); with d_out None the byte count needed."""
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        need = C.c_uint64(0)
+        ctr = np.zeros(3, np.uint64)
+        rc = lib().lc_sls_serialize_regex_dev(self._h, _p(d_base), base_len, _p(d_ev_off), _p(d_ev_len), n,
+                                              _p(d_status), _p(d_cap_off), _p(d_cap_len), row_pitch, *cfg,
+                                              int(bool(whole_line)), _p(d_ev_time), _p(d_ev_time_ns), _p(d_out),
+                                              out_cap, C.byref(need), _p(ctr))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value), ctr  # a sizing query
+        _check(rc)
+        return int(need.value), ctr
+
+    def regex_parse_sls(self, rx, base, ev_off, ev_len, ev_time, keys, source_key, renamed_key=None, keep_fail=False,
+                        keep_succeed=False, copy_raw=False, whole_line=False, ev_time_ns=None, out_cap=None):
+        """Host buffers in, wire bytes out (lc_regex_parse_sls; rx may be None in whole-line mode).  Returns (bytes,
+        counters[3] = successful, failed, discarded).  Without out_cap the output is sized by a first estimate and,
+        if short, the exact size."""
+        a = _u8(base)
+        ev_off = np.ascontiguousarray(ev_off, np.uint32)
+        ev_len = np.ascontiguousarray(ev_len, np.uint32)
+        t = np.ascontiguousarray(ev_time, np.uint32)
+        ns = None if ev_time_ns is None else np.ascontiguousarray(ev_time_ns, np.uint32)
+        n = ev_off.size
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        cap = int(out_cap if out_cap is not None else 2 * a.size + 64 * n + 64)
+        for _ in range(2):
+            out = np.empty(max(cap, 1), np.uint8)
+            need = C.c_uint64(0)
+            ctr = np.zeros(3, np.uint64)
+            rc = lib().lc_regex_parse_sls(self._h, _rh(rx), _p(a), a.size, _p(ev_off), _p(ev_len), n, _p(t), _p(ns),
+                                          *cfg, int(bool(whole_line)), _p(out), cap, C.byref(need), _p(ctr))
+            if rc == LC_ERR_CAPACITY and out_cap is None:
+                cap = int(need.value)
+                continue
+            _check(rc)
+            return bytes(out[:need.value]), ctr
+        _check(rc)
+
     def split_lines_dev(self, d_buf, length, split_char, d_off, d_len, cap):
         n = C.c_uint64(0)
         _check(lib().lc_split_lines_dev(self._h, _p(d_buf), length, split_char, _p(d_off), _p(d_len), cap,
@@ -499,8 +547,9 @@ class HostProcessor:
 
 
     def serialize_sls(self, group, enable_ns=False, process_then_serialize=False):
-        """ProcessorParseDelimiterNative::SerializeSls on a JSON group: (bytes, None) or (None, error).  With
-        process_then_serialize, Process + SLSEventGroupSerializer::Serialize on the same in-memory group instead."""
+        """SerializeSls of a processor_parse_delimiter_native or processor_parse_regex_native on a JSON group: (bytes,
+        None) or (None, error).  With process_then_serialize, Process + SLSEventGroupSerializer::Serialize on the same
+        in-memory group instead."""
         import json
         L = lib()
         L.lc_host_processor_serialize_sls.restype = C.c_void_p

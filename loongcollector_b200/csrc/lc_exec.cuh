@@ -2,8 +2,8 @@
 // that the sm_90a kernels execute once per log line.  Written as __host__ __device__ so that the
 // exact same statements can be exercised on the CPU by the test-only emulation library under
 // tests/emul/ (which validates the COMPILER's tables against the oracle without a GPU).  The product
-// library only ever calls these from device code, apart from the host-side configuration check of the
-// delimiter-fed SLS serialiser (lc_delim_sls_setup).
+// library only ever calls these from device code, apart from the host-side configuration steps of the
+// delimiter- and regex-fed SLS serialisers (lc_delim_sls_setup, lc_regex_sls_setup).
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -771,74 +771,6 @@ LC_HD void lc_sls_emit_log(uint8_t* out, const uint8_t* base, uint32_t time, boo
     }
 }
 
-// ---- the same writer over an abstract contents list (entry k = key bytes + value bytes), so that the contents can come
-// from the regex stage's capture tables instead of host-built span lists.  En: uint32_t klen(k), vlen(k);
-// const uint8_t* key(k), val(k).
-template <class En>
-LC_HD uint32_t lc_sls_log_size_t(const En& en, uint32_t count, bool has_ns, uint32_t* body_out) {
-    if (count == 0) {
-        *body_out = 0;
-        return 0;
-    }
-    uint32_t body = 1 + 5 + (has_ns ? 1 + 4 : 0);
-    for (uint32_t k = 0; k < count; ++k) {
-        const uint32_t in = lc_sls_pair_inner(en.klen(k), en.vlen(k));
-        body += 1 + lc_varint_size(in) + in;
-    }
-    *body_out = body;
-    return 1 + lc_varint_size(body) + body;
-}
-
-template <class En>
-LC_HD void lc_sls_emit_log_t(uint8_t* out, uint32_t time, bool has_ns, uint32_t ns, const En& en, uint32_t count,
-                             uint32_t body, uint32_t lane, uint32_t nlanes) {
-    uint32_t at = 0;
-    uint8_t hdr[16];
-    uint32_t h = 0;
-    hdr[h++] = 0x0A;
-    h += lc_put_varint(hdr + h, body);
-    hdr[h++] = 0x08;
-    h += lc_put_varint(hdr + h, time < (1u << 28) ? (1u << 28) : time); // always 5 bytes
-    if (lane == 0)
-        for (uint32_t j = 0; j < h; ++j)
-            out[j] = hdr[j];
-    at = h;
-    for (uint32_t k = 0; k < count; ++k) {
-        const uint32_t kl = en.klen(k), vl = en.vlen(k);
-        const uint8_t* kp = en.key(k);
-        const uint8_t* vp = en.val(k);
-        h = 0;
-        hdr[h++] = 0x12;
-        h += lc_put_varint(hdr + h, lc_sls_pair_inner(kl, vl));
-        hdr[h++] = 0x0A;
-        h += lc_put_varint(hdr + h, kl);
-        if (lane == 0)
-            for (uint32_t j = 0; j < h; ++j)
-                out[at + j] = hdr[j];
-        at += h;
-        for (uint32_t j = lane; j < kl; j += nlanes)
-            out[at + j] = kp[j];
-        at += kl;
-        h = 0;
-        hdr[h++] = 0x12;
-        h += lc_put_varint(hdr + h, vl);
-        if (lane == 0)
-            for (uint32_t j = 0; j < h; ++j)
-                out[at + j] = hdr[j];
-        at += h;
-        for (uint32_t j = lane; j < vl; j += nlanes)
-            out[at + j] = vp[j];
-        at += vl;
-    }
-    if (has_ns && lane == 0) {
-        out[at] = 0x25;
-        out[at + 1] = (uint8_t)ns;
-        out[at + 2] = (uint8_t)(ns >> 8);
-        out[at + 3] = (uint8_t)(ns >> 16);
-        out[at + 4] = (uint8_t)(ns >> 24);
-    }
-}
-
 // ------------------------------------------------------------------------------------------------------------
 // f4, delimiter-fed: the Log record of one event that ProcessorParseDelimiterNative::Process leaves behind, written
 // straight from the delimiter stage's result tables (ProcessorParseDelimiterNative.cpp:206-364; the host class's
@@ -1217,5 +1149,205 @@ inline const char* lc_delim_sls_setup(const uint8_t* sep, uint32_t sep_len, uint
     add(nkeys + 1, renamed_key, renamed_len);
     add(nkeys + 2, "__raw_log__", 11);
     key_at[nkeys + 3] = at;
+    return nullptr;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, regex-fed: the Log record of one event that ProcessorParseRegexNative::Process leaves behind, written straight
+// from the regex stage's result tables (ProcessorParseRegexNative.cpp:132-168, CommonParserOptions.cpp:91-117; the
+// host class's FinishEvent).  The event is flat on entry: a LogEvent whose only content is SourceKey -> line.  The
+// contents Process leaves on such an event depend only on the configuration and the row's status, so the host compiles
+// the configuration once into two content plans (lc_regex_sls_setup) and the device walks the plan of each row.  The
+// same body function serves the counting and the writing pass (sinks LcSlsCount / LcSlsWrite above).
+
+#define LC_REGEX_SLS_LINE 0xFFFFFFFFu // value source of a plan entry: the whole line (else capture j)
+
+// Plan entry e = (plan[2e] = key id, plan[2e + 1] = capture index or LC_REGEX_SLS_LINE), key id k naming the key
+// bytes [key_at[k], key_at[k + 1]) of `keys`.  Entries [0, n_ok) are the plan of parsed rows, [n_ok, n_ok + n_fail)
+// the plan of failed rows, both in content order.
+struct LcRegexSlsCfg {
+    const uint32_t* plan;
+    const uint32_t* key_at;
+    const uint8_t* keys;
+    uint32_t n_ok, n_fail;
+    uint32_t pitch;      // row pitch of the capture tables
+    uint32_t whole_line; // Regex "(.*)": no regex ran, every row is parsed (no status or capture tables)
+    uint32_t ok_fits;    // the parsed plan's captures lie inside a row; otherwise no row can be LC_REGEX_OK
+    uint32_t keep_fail;  // KeepingSourceWhenParseFail: failed rows are kept, else erased
+};
+
+// One event: its line base[eo, eo + elen) and its row of the capture tables (offsets into base).
+struct LcRegexSlsRow {
+    uint32_t eo, elen;
+    uint32_t status;
+    const uint32_t* co;
+    const uint32_t* cl;
+    uint32_t time;
+    bool has_ns;
+    uint32_t ns;
+};
+
+// The row's verdict: 0 = parsed (LC_REGEX_OK, or whole-line mode), else its failure status.  A row that claims
+// LC_REGEX_OK with more keys than the tables have columns cannot come from lc_regex_parse (which reports
+// LC_REGEX_KEYS_MISMATCH for it) and is taken as one, so no capture beyond the row is read.
+LC_HD uint32_t lc_regex_sls_verdict(const LcRegexSlsCfg& c, uint32_t status) {
+    if (c.whole_line)
+        return 0u;
+    return status == 0u && !c.ok_fits ? 2u : status;
+}
+
+// The body of the event's Log record -- Time, the contents of its plan, Time_ns -- into sink s.  Returns the number of
+// contents; 0 = the event has none (erased, or LogEvent::Empty) and emits no record.
+template <class S>
+LC_HD uint32_t lc_regex_sls_body(const LcRegexSlsCfg& c, const uint8_t* base, const LcRegexSlsRow& r, S& s) {
+    {
+        uint8_t h[6];
+        h[0] = 0x08;
+        const uint32_t n = 1 + lc_put_varint(h + 1, r.time < (1u << 28) ? (1u << 28) : r.time); // always 5 bytes
+        s.put(h, n);
+    }
+    const bool ok = lc_regex_sls_verdict(c, r.status) == 0u;
+    const uint32_t* e = c.plan + (ok ? 0u : 2u * c.n_ok);
+    const uint32_t m = ok ? c.n_ok : c.n_fail;
+    for (uint32_t k = 0; k < m; ++k) {
+        const uint32_t kid = e[2 * k], src = e[2 * k + 1];
+        const bool line = src == LC_REGEX_SLS_LINE;
+        const uint32_t vo = line ? r.eo : r.co[src];
+        const uint32_t vl = line ? r.elen : r.cl[src];
+        lc_sls_pair_open(s, c.keys + c.key_at[kid], c.key_at[kid + 1] - c.key_at[kid], vl);
+        s.copy(base + vo, vl);
+    }
+    if (r.has_ns) {
+        const uint8_t h[5] = {0x25, (uint8_t)r.ns, (uint8_t)(r.ns >> 8), (uint8_t)(r.ns >> 16), (uint8_t)(r.ns >> 24)};
+        s.put(h, 5);
+    }
+    return m;
+}
+
+// Host side: strings[0..count) back to back into key_bytes (sum of lens bytes) with key_at[count + 1] offsets.
+inline void lc_sls_key_table(const char* const* strings, const uint32_t* lens, uint32_t count, uint8_t* key_bytes,
+                             uint32_t* key_at) {
+    uint32_t at = 0;
+    for (uint32_t k = 0; k < count; ++k) {
+        key_at[k] = at;
+        if (lens[k])
+            memcpy(key_bytes + at, strings[k], lens[k]);
+        at += lens[k];
+    }
+    key_at[count] = at;
+}
+
+// Host side: compiles a configuration of the regex-fed serialiser into its two content plans.  The plans index the key
+// table keys[0..nkeys), SourceKey, RenamedSourceKey, "__raw_log__", "content" (ids nkeys .. nkeys + 3; build it with
+// lc_sls_key_table).  `plan` needs 3 * nkeys + 12 words (scratch included); c.plan / c.key_at / c.keys are left to the
+// caller (device copies).  Returns nullptr, or why the arguments are refused.
+//
+// Each plan is LogEvent's content algebra (SetContentNoCopy / DelContent, LogEvent.cpp:50-106) run once on symbolic
+// values -- "the line" and "capture j" -- starting from the flat event [SourceKey -> line]:
+//   parsed: set(keys[j], capture j) for each key in order (whole-line mode: set(keys[0] or "content", line)); a
+//           repeated key overwrites the earlier content in place, a key equal to SourceKey replaces the line in place;
+//           then delete(SourceKey) unless it is one of the keys; then RenamedSourceKey -> line if
+//           KeepingSourceWhenParseSucceed and that key is not live
+//   failed: delete(SourceKey); with KeepingSourceWhenParseFail RenamedSourceKey -> line, then "__raw_log__" -> line
+//           with CopingRawLog, each only if that key is not live; without it the event is empty and erased
+// so the kernels need no branch per quirk.
+inline const char* lc_regex_sls_setup(const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                                      const char* source_key, uint32_t source_len, const char* renamed_key,
+                                      uint32_t renamed_len, int keep_fail, int keep_succeed, int copy_raw,
+                                      int whole_line, uint32_t pitch, LcRegexSlsCfg* c, uint32_t* plan) {
+    if ((nkeys && (!keys || !key_lens)) || (source_len && !source_key) || (renamed_len && !renamed_key) || !c || !plan)
+        return "bad arguments";
+    for (uint32_t k = 0; k < nkeys; ++k)
+        if (key_lens[k] && !keys[k])
+            return "bad arguments";
+    const uint32_t K_SRC = nkeys, K_REN = nkeys + 1, K_RAW = nkeys + 2, K_CONTENT = nkeys + 3;
+    auto str = [&](uint32_t k, uint32_t* l) -> const char* {
+        if (k < nkeys) {
+            *l = key_lens[k];
+            return keys[k];
+        }
+        *l = k == K_SRC ? source_len : k == K_REN ? renamed_len : k == K_RAW ? 11u : 7u;
+        return k == K_SRC ? source_key : k == K_REN ? renamed_key : k == K_RAW ? "__raw_log__" : "content";
+    };
+    auto same = [&](uint32_t a, uint32_t b) {
+        uint32_t la, lb;
+        const char* pa = str(a, &la);
+        const char* pb = str(b, &lb);
+        return la == lb && (la == 0 || !memcmp(pa, pb, la));
+    };
+    // symbolic contents: triples (key id, value source, live) from `list` on; LogEvent::FindContent looks from the back
+    uint32_t* list = plan;
+    uint32_t len = 0;
+    auto find = [&](uint32_t key) -> int64_t {
+        for (uint32_t i = len; i-- > 0;)
+            if (list[3 * i + 2] && same(list[3 * i], key))
+                return (int64_t)i;
+        return -1;
+    };
+    auto set = [&](uint32_t key, uint32_t src) {
+        const int64_t i = find(key);
+        if (i >= 0) {
+            list[3 * i] = key;
+            list[3 * i + 1] = src;
+        } else {
+            list[3 * len] = key, list[3 * len + 1] = src, list[3 * len + 2] = 1u;
+            ++len;
+        }
+    };
+    auto add_absent = [&](uint32_t key) { // AddLog(key, line, false)
+        if (find(key) < 0)
+            set(key, LC_REGEX_SLS_LINE);
+    };
+    auto del = [&](uint32_t key) {
+        const int64_t i = find(key);
+        if (i >= 0)
+            list[3 * i + 2] = 0u;
+    };
+    // drops the dead entries, packs the triples into (key id, source) pairs in place; returns the entry count
+    auto finish = [&]() {
+        uint32_t m = 0;
+        for (uint32_t i = 0; i < len; ++i)
+            if (list[3 * i + 2]) {
+                const uint32_t k = list[3 * i], s = list[3 * i + 1];
+                list[2 * m] = k, list[2 * m + 1] = s;
+                ++m;
+            }
+        return m;
+    };
+    bool src_overwritten = false;
+    for (uint32_t k = 0; k < nkeys; ++k)
+        src_overwritten = src_overwritten || same(k, K_SRC);
+    memset(c, 0, sizeof *c);
+    // parsed rows
+    list[0] = K_SRC, list[1] = LC_REGEX_SLS_LINE, list[2] = 1u;
+    len = 1;
+    if (whole_line)
+        set(nkeys ? 0u : K_CONTENT, LC_REGEX_SLS_LINE);
+    else
+        for (uint32_t k = 0; k < nkeys; ++k)
+            set(k, k);
+    if (!src_overwritten)
+        del(K_SRC);
+    if (keep_succeed)
+        add_absent(K_REN);
+    c->n_ok = finish();
+    // failed rows (none in whole-line mode)
+    list = plan + 2 * c->n_ok;
+    len = 0;
+    if (!whole_line) {
+        list[0] = K_SRC, list[1] = LC_REGEX_SLS_LINE, list[2] = 1u;
+        len = 1;
+        del(K_SRC);
+        if (keep_fail) {
+            add_absent(K_REN);
+            if (copy_raw)
+                add_absent(K_RAW);
+        }
+    }
+    c->n_fail = finish();
+    c->pitch = pitch;
+    c->whole_line = whole_line != 0;
+    c->ok_fits = whole_line || nkeys <= pitch;
+    c->keep_fail = keep_fail != 0;
     return nullptr;
 }

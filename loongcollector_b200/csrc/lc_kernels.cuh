@@ -5,6 +5,7 @@
 #include <stdint.h>
 
 struct LcDelimSlsCfg; // lc_exec.cuh
+struct LcRegexSlsCfg;
 
 namespace lck {
 
@@ -196,24 +197,23 @@ void launch_sls_emit(const uint8_t* d_base, const uint32_t* d_ev_time, const uin
                      const uint32_t* d_voff, const uint32_t* d_vlen, uint64_t n, const uint64_t* d_rec_off,
                      const uint32_t* d_body_size, uint8_t* d_out, cudaStream_t st);
 
-// f4, device-fed: Log records from the regex stage's result tables + constant key strings (all device pointers)
-struct SlsParsedArgs {
+// f4, regex-fed: Log records from the regex stage's result tables (lc_regex_parse_dev) + the content plans of
+// lc_exec.cuh (LcRegexSlsCfg, plans and key strings on the device).  Sizes as for launch_sls_sizes; d_counters (or
+// nullptr): u64 [3] += successful, failed (LC_REGEX_NOMATCH), discarded events.
+struct RegexSlsTables {
     const uint8_t* base;
     const uint32_t* ev_off;
     const uint32_t* ev_len;
-    const uint8_t* status;
-    const uint32_t* cap_off;
+    const uint8_t* status;  // nullptr in whole-line mode
+    const uint32_t* cap_off; // [n][pitch], or nullptr when no plan reads a capture
     const uint32_t* cap_len;
-    uint32_t pitch;
-    const uint8_t* keys;
-    const uint32_t* key_at; // [nkeys + 2]
-    uint32_t nkeys;
-    uint32_t has_fail_key;
 };
-void launch_sls_parsed_sizes(const SlsParsedArgs& a, const uint32_t* d_ev_ns, uint64_t n, uint32_t* d_rec_size,
-                             uint32_t* d_body_size, cudaStream_t st);
-void launch_sls_parsed_emit(const SlsParsedArgs& a, const uint32_t* d_ev_time, const uint32_t* d_ev_ns, uint64_t n,
-                            const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out, cudaStream_t st);
+void launch_regex_sls_sizes(const LcRegexSlsCfg& c, const RegexSlsTables& t, const uint32_t* d_ev_ns, uint64_t n,
+                            uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                            cudaStream_t st);
+void launch_regex_sls_emit(const LcRegexSlsCfg& c, const RegexSlsTables& t, const uint32_t* d_ev_time,
+                           const uint32_t* d_ev_ns, uint64_t n, const uint64_t* d_rec_off, const uint32_t* d_body_size,
+                           uint8_t* d_out, cudaStream_t st);
 
 // f4, delimiter-fed: Log records from the delimiter stage's result tables (launch_delim) + the configuration of
 // lc_exec.cuh (LcDelimSlsCfg, key strings on the device).  Sizes as for launch_sls_sizes; d_counters (or nullptr):

@@ -1800,6 +1800,76 @@ std::string SlsGroupTail(PipelineEventGroup& group) {
 std::string SizeLimitError(uint64_t size, int32_t limit) {
     return "log group exceeds size limit\tgroup size: " + ToString(size) + "\tsize limit: " + ToString((uint64_t)limit);
 }
+
+// ---- shared by the SerializeSls methods of the parse processors
+// Whether the one-pass device path applies: every event is flat (a LogEvent whose only content is sourceKey -> line)
+// and the group carries no log.file.offset metadata (ShouldEraseEvent keys off it, CommonParserOptions.cpp:99-117).
+bool IsFlatSlsGroup(PipelineEventGroup& group, const std::string& sourceKey) {
+    if (group.HasMetadata(EventGroupMetaKey::LOG_FILE_OFFSET_KEY))
+        return false;
+    for (const PipelineEventPtr& e : group.GetEvents()) {
+        if (!e.Is<LogEvent>())
+            return false;
+        const LogEvent& ev = e.Cast<LogEvent>();
+        const LogEvent::Content* c = ev.FirstLive();
+        if (!(ev.Size() == 1 && c && c->first.first == StringView(sourceKey)))
+            return false;
+    }
+    return true;
+}
+
+// the lines of a flat group (batch, finished) and the times the serialiser writes
+void GatherFlatSls(PipelineEventGroup& group, bool enableNs, FlatBatch& batch, std::vector<uint32_t>& evTime,
+                   std::vector<uint32_t>& evNs) {
+    const EventsContainer& events = group.GetEvents();
+    const size_t n = events.size();
+    evTime.assign(n, 0);
+    evNs.assign(n, LC_SLS_NO_NS);
+    for (size_t i = 0; i < n; ++i) {
+        const LogEvent& ev = events[i].Cast<LogEvent>();
+        batch.Add(i, ev.FirstLive()->first.second);
+        evTime[i] = (uint32_t)ev.GetTimestamp();
+        if (enableNs && ev.GetTimestampNanosecond())
+            evNs[i] = ev.GetTimestampNanosecond().value();
+    }
+    batch.Finish(*group.GetSourceBuffer());
+}
+
+// The device pass of SerializeSls: call(out, cap, &need) parses and serialises the group into res, sized by
+// `estimate` first and by the exact size when that was short (unless the group is over the size limit anyway).
+template <class Call>
+void RunSlsDevicePass(Call call, size_t estimate, size_t tailSize, int32_t limit, std::string& res, uint64_t& need,
+                      const char* what) {
+    res.assign(estimate, '\0');
+    int rc = call(reinterpret_cast<uint8_t*>(&res[0]), (uint64_t)res.size(), &need);
+    if (rc == LC_ERR_CAPACITY && (int64_t)(need + tailSize) <= (int64_t)limit) {
+        res.resize(need);
+        rc = call(reinterpret_cast<uint8_t*>(&res[0]), (uint64_t)res.size(), &need);
+    }
+    if (rc != LC_ERR_CAPACITY)
+        Check(rc, what);
+}
+
+// SLSEventGroupSerializer::Serialize's checks, in its order, on the result of the device pass (n events in,
+// `discarded` of them erased, need wire bytes of Logs records)
+bool FinishSls(const SLSEventGroupSerializer& ser, uint64_t n, uint64_t discarded, uint64_t need, std::string& res,
+               const std::string& tail, std::string& out, std::string& err) {
+    if (n == discarded) {
+        err = "empty event group";
+        return false;
+    }
+    if (need == 0) {
+        err = "all empty logs";
+        return false;
+    }
+    if ((int64_t)(need + tail.size()) > (int64_t)ser.mMaxSendLogGroupSize) {
+        err = SizeLimitError(need + tail.size(), ser.mMaxSendLogGroupSize);
+        return false;
+    }
+    res.resize(need);
+    out = res + tail;
+    return true;
+}
 } // namespace
 
 bool SLSEventGroupSerializer::Serialize(PipelineEventGroup& group, std::string& res, std::string& errorMsg) const {
@@ -1896,33 +1966,15 @@ bool ProcessorParseDelimiterNative::SerializeSls(PipelineEventGroup& group, bool
                                                  std::string& err) {
     SLSEventGroupSerializer ser;
     ser.mEnableTimestampNanosecond = enableNs;
-    EventsContainer& events = group.MutableEvents();
-    bool flat = mDeviceSls && !group.HasMetadata(EventGroupMetaKey::LOG_FILE_OFFSET_KEY);
-    for (size_t i = 0; flat && i < events.size(); ++i) {
-        if (!events[i].Is<LogEvent>()) {
-            flat = false;
-            break;
-        }
-        const LogEvent& ev = events[i].Cast<LogEvent>();
-        const LogEvent::Content* c = ev.FirstLive();
-        flat = ev.Size() == 1 && c && c->first.first == StringView(mSourceKey);
-    }
-    if (!flat) {
+    if (!mDeviceSls || !IsFlatSlsGroup(group, mSourceKey)) {
         Process(group);
         return ser.Serialize(group, out, err);
     }
     // every event is SourceKey -> line: parse and serialise in one device pass, only the wire bytes come back
-    const size_t n = events.size();
+    const size_t n = group.GetEvents().size();
     FlatBatch batch;
-    std::vector<uint32_t> evTime(n), evNs(n, LC_SLS_NO_NS);
-    for (size_t i = 0; i < n; ++i) {
-        const LogEvent& ev = events[i].Cast<LogEvent>();
-        batch.Add(i, ev.FirstLive()->first.second);
-        evTime[i] = (uint32_t)ev.GetTimestamp();
-        if (enableNs && ev.GetTimestampNanosecond())
-            evNs[i] = ev.GetTimestampNanosecond().value();
-    }
-    batch.Finish(*group.GetSourceBuffer());
+    std::vector<uint32_t> evTime, evNs;
+    GatherFlatSls(group, enableNs, batch, evTime, evNs);
     std::vector<const char*> kp;
     std::vector<uint32_t> kl;
     size_t keyBytes = 0;
@@ -1932,46 +1984,70 @@ bool ProcessorParseDelimiterNative::SerializeSls(PipelineEventGroup& group, bool
         keyBytes += k.size();
     }
     const std::string& renamed = mCommonParserOptions.mRenamedSourceKey;
-    std::string res((size_t)(2 * batch.baseLen + n * (64 + keyBytes + renamed.size()) + 64), '\0');
+    std::string res;
     uint64_t need = 0, ctr[4] = {0, 0, 0, 0};
     const std::string tail = SlsGroupTail(group);
-    auto call = [&]() {
-        return lc_delim_parse_sls(
-            Engine(), batch.base, batch.baseLen, batch.off.data(), batch.len.data(), n, evTime.data(), evNs.data(),
-            reinterpret_cast<const uint8_t*>(mSeparator.data()), (uint32_t)mSeparator.size(), (uint8_t)mQuote,
-            mOverflowedFieldsTreatment == OverflowedFieldsTreatment::EXTEND, mExtractingPartialFields,
-            mAllowingShortenedFields, (uint32_t)mKeys.size() + 16, kp.data(), kl.data(), (uint32_t)mKeys.size(),
-            mSourceKey.data(), (uint32_t)mSourceKey.size(), renamed.data(), (uint32_t)renamed.size(),
-            mCommonParserOptions.mKeepingSourceWhenParseFail, mCommonParserOptions.mKeepingSourceWhenParseSucceed,
-            mCommonParserOptions.mCopingRawLog, reinterpret_cast<uint8_t*>(&res[0]), res.size(), &need, ctr);
-    };
-    int rc = call();
-    if (rc == LC_ERR_CAPACITY && (int64_t)(need + tail.size()) <= (int64_t)ser.mMaxSendLogGroupSize) {
-        res.resize(need);
-        rc = call();
-    }
-    if (rc != LC_ERR_CAPACITY)
-        Check(rc, "lc_delim_parse_sls");
+    RunSlsDevicePass(
+        [&](uint8_t* o, uint64_t cap, uint64_t* len) {
+            return lc_delim_parse_sls(
+                Engine(), batch.base, batch.baseLen, batch.off.data(), batch.len.data(), n, evTime.data(), evNs.data(),
+                reinterpret_cast<const uint8_t*>(mSeparator.data()), (uint32_t)mSeparator.size(), (uint8_t)mQuote,
+                mOverflowedFieldsTreatment == OverflowedFieldsTreatment::EXTEND, mExtractingPartialFields,
+                mAllowingShortenedFields, (uint32_t)mKeys.size() + 16, kp.data(), kl.data(), (uint32_t)mKeys.size(),
+                mSourceKey.data(), (uint32_t)mSourceKey.size(), renamed.data(), (uint32_t)renamed.size(),
+                mCommonParserOptions.mKeepingSourceWhenParseFail, mCommonParserOptions.mKeepingSourceWhenParseSucceed,
+                mCommonParserOptions.mCopingRawLog, o, cap, len, ctr);
+        },
+        (size_t)(2 * batch.baseLen + n * (64 + keyBytes + renamed.size()) + 64), tail.size(), ser.mMaxSendLogGroupSize,
+        res, need, "lc_delim_parse_sls");
     // the counters Process would have moved (a blank value counts as out_failed, :220-242)
     mOutSuccessfulEventsTotal.Add(ctr[0]);
     mOutFailedEventsTotal.Add(ctr[1] + ctr[3]);
     mDiscardedEventsTotal.Add(ctr[2]);
-    // SLSEventGroupSerializer::Serialize's checks, in its order
-    if (n == ctr[2]) {
-        err = "empty event group";
-        return false;
+    return FinishSls(ser, n, ctr[2], need, res, tail, out, err);
+}
+
+bool ProcessorParseRegexNative::SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out,
+                                             std::string& err) {
+    SLSEventGroupSerializer ser;
+    ser.mEnableTimestampNanosecond = enableNs;
+    if (!IsFlatSlsGroup(group, mSourceKey)) {
+        Process(group);
+        return ser.Serialize(group, out, err);
     }
-    if (need == 0) {
-        err = "all empty logs";
-        return false;
+    // every event is SourceKey -> line: parse and serialise in one device pass, only the wire bytes come back
+    const size_t n = group.GetEvents().size();
+    FlatBatch batch;
+    std::vector<uint32_t> evTime, evNs;
+    GatherFlatSls(group, enableNs, batch, evTime, evNs);
+    std::vector<const char*> kp;
+    std::vector<uint32_t> kl;
+    size_t keyBytes = 0;
+    for (const auto& k : mKeys) {
+        kp.push_back(k.data());
+        kl.push_back((uint32_t)k.size());
+        keyBytes += k.size();
     }
-    if ((int64_t)(need + tail.size()) > (int64_t)ser.mMaxSendLogGroupSize) {
-        err = SizeLimitError(need + tail.size(), ser.mMaxSendLogGroupSize);
-        return false;
-    }
-    res.resize(need);
-    out = res + tail;
-    return true;
+    const std::string& renamed = mCommonParserOptions.mRenamedSourceKey;
+    std::string res;
+    uint64_t need = 0, ctr[3] = {0, 0, 0};
+    const std::string tail = SlsGroupTail(group);
+    RunSlsDevicePass(
+        [&](uint8_t* o, uint64_t cap, uint64_t* len) {
+            return lc_regex_parse_sls(
+                Engine(), mIsWholeLineMode ? nullptr : mReg.get(), batch.base, batch.baseLen, batch.off.data(),
+                batch.len.data(), n, evTime.data(), evNs.data(), kp.data(), kl.data(), (uint32_t)mKeys.size(),
+                mSourceKey.data(), (uint32_t)mSourceKey.size(), renamed.data(), (uint32_t)renamed.size(),
+                mCommonParserOptions.mKeepingSourceWhenParseFail, mCommonParserOptions.mKeepingSourceWhenParseSucceed,
+                mCommonParserOptions.mCopingRawLog, mIsWholeLineMode, o, cap, len, ctr);
+        },
+        (size_t)(2 * batch.baseLen + n * (64 + keyBytes + renamed.size()) + 64), tail.size(), ser.mMaxSendLogGroupSize,
+        res, need, "lc_regex_parse_sls");
+    // the counters Process would have moved (LC_REGEX_KEYS_MISMATCH is not out_failed, :227-244)
+    mOutSuccessfulEventsTotal.Add(ctr[0]);
+    mOutFailedEventsTotal.Add(ctr[1]);
+    mDiscardedEventsTotal.Add(ctr[2]);
+    return FinishSls(ser, n, ctr[2], need, res, tail, out, err);
 }
 
 Processor* CreateProcessor(const std::string& type) {

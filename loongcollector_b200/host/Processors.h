@@ -163,6 +163,12 @@ public:
     std::vector<std::string> mKeys;
     CommonParserOptions mCommonParserOptions;
     Counter mDiscardedEventsTotal, mOutFailedEventsTotal, mOutKeyNotFoundEventsTotal, mOutSuccessfulEventsTotal;
+    // Process(group) followed by SLSEventGroupSerializer::Serialize (enableNs = its mEnableTimestampNanosecond): the
+    // same bytes or error message, and the same counter updates.  When every event is flat (a LogEvent whose only
+    // content is SourceKey -> line) and the group carries no log.file.offset metadata, the group is parsed and
+    // serialised in one device pass (lc_regex_parse_sls): the capture tables never leave the GPU, no LogEvent is
+    // touched and the group's events are left as they were.  Otherwise Process runs.
+    bool SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out, std::string& err);
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }

@@ -132,25 +132,28 @@ char* lc_host_processor_serialize_sls(lc_host_processor_t* p, const char* group_
     if (len_out)
         *len_out = 0;
     try {
+        // the two parse processors with a one-pass device path: the same calls on either
         auto* d = dynamic_cast<ProcessorParseDelimiterNative*>(p->proc.get());
-        if (!d)
-            throw std::runtime_error("not a processor_parse_delimiter_native");
+        auto* r = dynamic_cast<ProcessorParseRegexNative*>(p->proc.get());
+        if (!d && !r)
+            throw std::runtime_error("not a processor_parse_delimiter_native or processor_parse_regex_native");
+        Processor* proc = p->proc.get();
         PipelineEventGroup group(std::make_shared<SourceBuffer>());
         if (!group.FromJsonString(group_json ? group_json : "null"))
             throw std::runtime_error("group JSON does not parse");
-        const uint64_t errs = d->EngineErrors();
+        const uint64_t errs = proc->EngineErrors();
         std::string res, err;
         bool ok;
         if (process_then_serialize) {
-            d->Process(group);
+            proc->Process(group);
             SLSEventGroupSerializer ser;
             ser.mEnableTimestampNanosecond = enable_ns != 0;
             ok = ser.Serialize(group, res, err);
         } else {
-            ok = d->SerializeSls(group, enable_ns != 0, res, err);
+            ok = d ? d->SerializeSls(group, enable_ns != 0, res, err) : r->SerializeSls(group, enable_ns != 0, res, err);
         }
-        if (d->EngineErrors() != errs)
-            throw std::runtime_error("engine error inside Process: " + d->LastError());
+        if (proc->EngineErrors() != errs)
+            throw std::runtime_error("engine error inside Process: " + proc->LastError());
         if (!ok) {
             if (err_out)
                 *err_out = dup(err);
