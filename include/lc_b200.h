@@ -358,6 +358,34 @@ int lc_delim_parse_sls(lc_engine_t* e, const uint8_t* base, uint64_t base_len, c
                        uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, uint8_t* out,
                        uint64_t out_cap, uint64_t* out_len, uint64_t counters[4]);
 
+/* Device-fed variant for the split -> serialise hand-over: the `Logs` fields of the events ProcessorSplitLogStringNative
+ * or ProcessorSplitMultilineLogStringNative cut from ONE source value (ProcessorSplitLogStringNative.cpp:131-161,
+ * ProcessorSplitMultilineLogStringNative.cpp:311-340), written straight from the DEVICE piece tables of one
+ * lc_split_lines_dev or lc_multiline_split_dev call over d_src[0, src_len).  Piece k = d_src[d_off[k], +d_len[k])
+ * becomes one record with the source event's time / time_ns (LC_SLS_NO_NS = no Time_ns):
+ *   offset_key == NULL:      key -> piece  (a RAW event: pass key "content")
+ *   offset_key != key:       key -> piece, offset_key -> decimal(src_pos + d_off[k])  (log.file.offset metadata)
+ *   offset_key == key:       key -> decimal(src_pos + d_off[k])  (SetContentNoCopy replaces the piece in place)
+ * Records are never empty.  d_out receives the bytes on the device; *out_len (host) their count; LC_ERR_CAPACITY if
+ * > out_cap (nothing written).  LC_ERR_TOO_LARGE when src_len + key_len + offset_key_len + 96 >= 2^32. */
+int lc_sls_serialize_spans_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+                               const uint32_t* d_len, uint64_t n, const char* key, uint32_t key_len,
+                               const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+                               uint32_t time_ns, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len);
+
+/* The same with a HOST source value: upload it once, split it on the device (lc_split_lines / lc_multiline_split
+ * rules), serialise the pieces as above and bring back only the wire bytes.  *n_events (may be NULL) = number of
+ * pieces; the multiline call adds to counters[3] as lc_multiline_split does.  *out_len, *n_events and counters are
+ * set on LC_OK and on LC_ERR_CAPACITY. */
+int lc_split_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, uint8_t split_char, const char* key,
+                 uint32_t key_len, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+                 uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events);
+int lc_multiline_split_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+                           const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, const char* key,
+                           uint32_t key_len, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+                           uint32_t time, uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                           uint64_t* n_events, uint64_t counters[3]);
+
 #ifdef __cplusplus
 }
 #endif

@@ -90,6 +90,11 @@ def lib():
     L.lc_sls_serialize_regex_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32] + sls_cfg + \
         [i32, vp, vp, vp, u64, C.POINTER(u64), vp]
     L.lc_regex_parse_sls.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp] + sls_cfg + [i32, vp, u64, C.POINTER(u64), vp]
+    span_keys = [C.c_char_p, u32, C.c_char_p, u32, u64, u32, u32]  # key .. time_ns
+    L.lc_sls_serialize_spans_dev.argtypes = [vp, vp, u64, vp, vp, u64] + span_keys + [vp, u64, C.POINTER(u64)]
+    L.lc_split_sls.argtypes = [vp, vp, u64, u8] + span_keys + [vp, u64, C.POINTER(u64), C.POINTER(u64)]
+    L.lc_multiline_split_sls.argtypes = [vp, vp, u64, vp, vp, vp, i32] + span_keys + [vp, u64, C.POINTER(u64),
+                                                                                         C.POINTER(u64), vp]
     _LIB = L
     return L
 
@@ -444,6 +449,58 @@ class Engine:
             return bytes(out[:need.value]), ctr
         _check(rc)
 
+    @staticmethod
+    def _span_keys(key, offset_key, src_pos, time, time_ns):
+        """key / offset_key: bytes (offset_key None = no offset key); time_ns None = no Time_ns"""
+        return [key, len(key), offset_key, len(offset_key) if offset_key is not None else 0, int(src_pos),
+                int(time) & 0xFFFFFFFF, 0xFFFFFFFF if time_ns is None else int(time_ns)]
+
+    def sls_serialize_spans_dev(self, d_src, src_len, d_off, d_len, n, key, offset_key=None, src_pos=0, time=0,
+                                time_ns=None, d_out=None, out_cap=0):
+        """Wire bytes of the events a splitter cuts from one source value, from the device piece tables of one
+        split_lines_dev / multiline_split_dev call (lc_sls_serialize_spans_dev).  Returns the byte count written to
+        d_out, or with d_out None the byte count needed."""
+        need = C.c_uint64(0)
+        rc = lib().lc_sls_serialize_spans_dev(self._h, _p(d_src), src_len, _p(d_off), _p(d_len), n,
+                                              *self._span_keys(key, offset_key, src_pos, time, time_ns), _p(d_out),
+                                              out_cap, C.byref(need))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value)  # a sizing query
+        _check(rc)
+        return int(need.value)
+
+    def _split_sls(self, fn, buf, extra, key, offset_key, src_pos, time, time_ns, out_cap, tail):
+        a = _u8(buf)
+        cap = int(out_cap if out_cap is not None else 2 * a.size + 4096)
+        for _ in range(2):
+            out = np.empty(max(cap, 1), np.uint8)
+            need, nev = C.c_uint64(0), C.c_uint64(0)
+            for t in tail:
+                t[:] = 0  # (the counters are added to: a second, exactly sized call starts again from zero)
+            rc = fn(self._h, _p(a), a.size, *extra, *self._span_keys(key, offset_key, src_pos, time, time_ns), _p(out),
+                    cap, C.byref(need), C.byref(nev), *(_p(t) for t in tail))
+            if rc == LC_ERR_CAPACITY and out_cap is None:
+                cap = int(need.value)
+                continue
+            _check(rc)
+            return bytes(out[:need.value]), int(nev.value)
+        _check(rc)
+
+    def split_sls(self, buf, split_char, key, offset_key=None, src_pos=0, time=0, time_ns=None, out_cap=None):
+        """Host source value in, wire bytes out (lc_split_sls).  Returns (bytes, number of pieces)."""
+        return self._split_sls(lib().lc_split_sls, buf, [split_char], key, offset_key, src_pos, time, time_ns, out_cap,
+                               [])
+
+    def multiline_split_sls(self, buf, start, cont, end, discard, key, offset_key=None, src_pos=0, time=0,
+                            time_ns=None, out_cap=None):
+        """Host source value in, wire bytes out (lc_multiline_split_sls).  Returns (bytes, number of events,
+        counters[3] = matched_events, input_lines, unmatched_lines)."""
+        ctr = np.zeros(3, np.uint64)
+        data, nev = self._split_sls(lib().lc_multiline_split_sls, buf,
+                                    [_rh(start), _rh(cont), _rh(end), int(bool(discard))], key, offset_key, src_pos,
+                                    time, time_ns, out_cap, [ctr])
+        return data, nev, ctr
+
     def split_lines_dev(self, d_buf, length, split_char, d_off, d_len, cap):
         n = C.c_uint64(0)
         _check(lib().lc_split_lines_dev(self._h, _p(d_buf), length, split_char, _p(d_off), _p(d_len), cap,
@@ -547,8 +604,8 @@ class HostProcessor:
 
 
     def serialize_sls(self, group, enable_ns=False, process_then_serialize=False):
-        """SerializeSls of a processor_parse_delimiter_native or processor_parse_regex_native on a JSON group: (bytes,
-        None) or (None, error).  With process_then_serialize, Process + SLSEventGroupSerializer::Serialize on the same
+        """SerializeSls of a processor_parse_delimiter_native, processor_parse_regex_native, processor_split_string_native
+        or processor_split_multiline_log_string_native on a JSON group: (bytes, None) or (None, error).  With process_then_serialize, Process + SLSEventGroupSerializer::Serialize on the same
         in-memory group instead."""
         import json
         L = lib()

@@ -1935,6 +1935,105 @@ int regex_sls_config(lc_engine_t* e, const char* what, const char* const* keys, 
     return stage_regex_sls(e, what, plan.data(), strings.data(), lens.data(), nkeys + 4, c);
 }
 
+// The configuration of the split-fed serialiser over one source value d_src[0, src_len); the keys are staged on the
+// device in the engine's `sls_plan` buffer, which neither splitter uses.  A record is its piece plus at most
+// key_len + offset_key_len + 96 bytes of framing and digits, so record sizes stay below 2^32.
+int span_sls_config(lc_engine_t* e, const char* what, const uint8_t* d_src, uint64_t src_len, const char* key,
+                    uint32_t key_len, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+                    uint32_t time, uint32_t time_ns, LcSpanSlsCfg* c) {
+    if ((key_len && !key) || (src_len && !d_src))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    if (src_len + key_len + (uint64_t)offset_key_len + 96 > 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": source value and keys must stay below 4 GiB");
+    const bool replace = offset_key && offset_key_len == key_len && !memcmp(offset_key, key, key_len);
+    std::vector<uint8_t> kb(key_len + (offset_key ? offset_key_len : 0u) + 1);
+    if (key_len)
+        memcpy(kb.data(), key, key_len);
+    if (offset_key && offset_key_len)
+        memcpy(kb.data() + key_len, offset_key, offset_key_len);
+    CU_TRY(e->sls_plan.ensure(kb.size() + 16));
+    CU_TRY(cudaMemcpyAsync(e->sls_plan.p, kb.data(), kb.size(), cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream)); // (pageable source: its bytes must be on the device before it dies)
+    memset(c, 0, sizeof *c);
+    c->src = d_src;
+    c->src_len = src_len;
+    c->key = e->sls_plan.as<uint8_t>();
+    c->klen = key_len;
+    c->okey = c->key + key_len;
+    c->oklen = offset_key ? offset_key_len : 0u;
+    c->mode = !offset_key ? LC_SPAN_PIECE : replace ? LC_SPAN_OFFSET : LC_SPAN_PIECE_OFFSET;
+    c->time = time < (1u << 28) ? (1u << 28) : time;
+    c->has_ns = time_ns != LC_SLS_NO_NS;
+    c->ns = c->has_ns ? time_ns : 0u;
+    c->src_pos = src_pos;
+    return LC_OK;
+}
+
+// size pass, exclusive sum and the output-tiled emit over the pieces d_off / d_len (serialize_sls_dev)
+int serialize_spans(lc_engine_t* e, const char* what, LcSpanSlsCfg& c, const uint32_t* d_off, const uint32_t* d_len,
+                    uint64_t n, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len) {
+    c.off = d_off;
+    c.len = d_len;
+    return serialize_sls_dev(
+        e, what, n, 0, [&](uint32_t* rec, uint32_t*, unsigned long long*) { lck::launch_span_sls_sizes(c, n, rec, e->stream); },
+        // serialize_sls_dev has set *out_len to the total before it queues the emit
+        [&](const uint64_t* rec_off, const uint32_t*, uint8_t* out) {
+            lck::launch_span_sls_emit(c, rec_off, n, *out_len, out, e->stream);
+        },
+        d_out, out_cap, out_len, nullptr);
+}
+
+// Host-buffer split + serialise (lc_split_sls, lc_multiline_split_sls): the source goes up once into `in`,
+// `split(&n)` cuts it into the piece tables out_a / out_b (and out_c flags), the records are written to `lab` and only
+// they come back.  The serialiser's tables (lab_sizes, cnt, lab_off, desc, sls_plan) are none of the splitters'.
+template <class Split>
+int split_sls_host(lc_engine_t* e, const char* what, const uint8_t* buf, uint64_t len, Split split, const char* key,
+                   uint32_t key_len, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+                   uint32_t time, uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                   uint64_t* n_events) {
+    if (!e || !out_len || (len && !buf))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (n_events)
+        *n_events = 0;
+    if (len == 0)
+        return LC_OK;
+    if (len >= 0xFFFFFFF0ull)
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    CU_TRY(e->in.ensure(len + 16));
+    CU_TRY(e->out_a.ensure((len + 1) * 4));
+    CU_TRY(e->out_b.ensure((len + 1) * 4));
+    CU_TRY(e->out_c.ensure(len + 1));
+    CU_TRY(cudaMemcpyAsync(e->in.p, buf, len, cudaMemcpyHostToDevice, e->stream));
+    uint64_t n = 0;
+    rc = split(&n);
+    if (rc)
+        return rc;
+    if (n_events)
+        *n_events = n;
+    LcSpanSlsCfg c;
+    rc = span_sls_config(e, what, e->in.as<uint8_t>(), len, key, key_len, offset_key, offset_key_len, src_pos, time,
+                         time_ns, &c);
+    if (rc)
+        return rc;
+    // the wire bytes never exceed the pieces plus a record's framing each
+    const uint64_t bound = len + n * ((uint64_t)key_len + offset_key_len + 128);
+    const uint64_t cap = out_cap < bound ? out_cap : bound;
+    CU_TRY(e->lab.ensure(cap));
+    rc = serialize_spans(e, what, c, e->out_a.as<uint32_t>(), e->out_b.as<uint32_t>(), n, e->lab.as<uint8_t>(), cap,
+                         out_len);
+    if (rc == LC_OK && *out_len) {
+        if (!out)
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+        CU_TRY(cudaMemcpyAsync(out, e->lab.p, *out_len, cudaMemcpyDeviceToHost, e->stream));
+        CU_TRY(cudaStreamSynchronize(e->stream));
+    }
+    return rc;
+}
+
 } // namespace
 
 extern "C" {
@@ -2180,6 +2279,58 @@ int lc_delim_parse_sls(lc_engine_t* e, const uint8_t* base, uint64_t base_len, c
     };
     return parse_sls_host(e, what, base, base_len, ev_off, ev_len, n, ev_time, ev_time_ns, 4, parse, sizes, emit, out,
                           out_cap, out_len, counters);
+}
+
+int lc_sls_serialize_spans_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+                               const uint32_t* d_len, uint64_t n, const char* key, uint32_t key_len,
+                               const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+                               uint32_t time_ns, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len) {
+    static const char* what = "lc_sls_serialize_spans_dev";
+    if (!e || !out_len || (n && (!d_off || !d_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (n == 0)
+        return LC_OK;
+    if (n >= (1ull << 30))
+        return fail(LC_ERR_TOO_LARGE, "< 2^30 pieces per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcSpanSlsCfg c;
+    rc = span_sls_config(e, what, d_src, src_len, key, key_len, offset_key, offset_key_len, src_pos, time, time_ns, &c);
+    if (rc)
+        return rc;
+    return serialize_spans(e, what, c, d_off, d_len, n, d_out, out_cap, out_len);
+}
+
+int lc_split_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, uint8_t split_char, const char* key,
+                 uint32_t key_len, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+                 uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events) {
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_sls_host(e, "lc_split_sls", buf, len, split, key, key_len, offset_key, offset_key_len, src_pos, time,
+                          time_ns, out, out_cap, out_len, n_events);
+}
+
+int lc_multiline_split_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+                           const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, const char* key,
+                           uint32_t key_len, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+                           uint32_t time, uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                           uint64_t* n_events, uint64_t counters[3]) {
+    for (const lc_regex_t* r : {start, cont, end}) {
+        int rc;
+        if (r && (rc = check_regex_usable(r, "lc_multiline_split_sls")))
+            return rc;
+    }
+    auto split = [&](uint64_t* n) {
+        return lc_multiline_split_dev(e, e->in.as<uint8_t>(), len, start, cont, end, discard_unmatched,
+                                      e->out_a.as<uint32_t>(), e->out_b.as<uint32_t>(), e->out_c.as<uint8_t>(), len, n,
+                                      counters);
+    };
+    return split_sls_host(e, "lc_multiline_split_sls", buf, len, split, key, key_len, offset_key, offset_key_len,
+                          src_pos, time, time_ns, out, out_cap, out_len, n_events);
 }
 
 } // extern "C"

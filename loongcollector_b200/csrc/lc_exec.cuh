@@ -1351,3 +1351,268 @@ inline const char* lc_regex_sls_setup(const char* const* keys, const uint32_t* k
     c->keep_fail = keep_fail != 0;
     return nullptr;
 }
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, split-fed: the Log records of the events ProcessorSplitLogStringNative / ProcessorSplitMultilineLogStringNative
+// cut from one source value (ProcessorSplitLogStringNative.cpp:131-161, ProcessorSplitMultilineLogStringNative.cpp:
+// 311-340), written straight from the piece tables of lc_split_lines_dev / lc_multiline_split_dev.  Piece k =
+// src[off[k], +len[k]) becomes one record:
+//   LC_SPAN_PIECE:        key -> piece                        (RAW events: key = "content")
+//   LC_SPAN_PIECE_OFFSET: key -> piece, okey -> decimal(src_pos + off[k])
+//   LC_SPAN_OFFSET:       key -> decimal(src_pos + off[k])    (the offset key is the source key: replaced in place)
+// A record's size is a closed function of len[k] and the digit count, so the size pass is elementwise.  The emit pass
+// is tiled over the OUTPUT: lc_span_sls_tile writes exactly the bytes [t0, t1) of the wire output, whatever records,
+// headers or varints the tile cuts through, so one long record never holds up a launch.  Value bytes (almost all the
+// output) go out as 16-byte stores aligned on the output, loaded from the misaligned source by funnel-shifting two
+// aligned 16-byte loads.
+#define LC_SPAN_PIECE 0u
+#define LC_SPAN_PIECE_OFFSET 1u
+#define LC_SPAN_OFFSET 2u
+
+struct LcSpanSlsCfg {
+    const uint8_t* src;  // the source value (the buffer the split ran over)
+    uint64_t src_len;
+    const uint32_t* off; // piece tables
+    const uint32_t* len;
+    const uint8_t* key;  // device copies of the keys
+    const uint8_t* okey;
+    uint32_t klen, oklen;
+    uint32_t mode; // LC_SPAN_*
+    uint32_t time; // raised to 2^28 already
+    uint32_t ns;
+    uint32_t has_ns;
+    uint64_t src_pos; // the source event's file offset
+};
+
+struct LcSpanRec {
+    uint64_t num; // src_pos + off (modes with an offset)
+    uint32_t nd;  // its decimal digits
+    uint32_t va;  // value of the first pair: the piece or the digits
+    uint32_t pa;  // inner size of the first pair, of the second (0 = none)
+    uint32_t pb;
+    uint32_t body;
+    uint32_t vat;  // record position of the first pair's value
+    uint32_t size; // bytes of the record
+};
+
+LC_HD uint32_t lc_dec_digits(uint64_t v) {
+    uint32_t d = 1;
+    uint64_t p = 10;
+    while (d < 20 && v >= p) {
+        ++d;
+        p *= 10;
+    }
+    return d;
+}
+
+LC_HD LcSpanRec lc_span_sls_rec(const LcSpanSlsCfg& c, uint32_t off, uint32_t len) {
+    LcSpanRec r;
+    r.num = c.src_pos + off;
+    r.nd = c.mode == LC_SPAN_PIECE ? 0u : lc_dec_digits(r.num);
+    r.va = c.mode == LC_SPAN_OFFSET ? r.nd : len;
+    r.pa = lc_sls_pair_inner(c.klen, r.va);
+    r.pb = c.mode == LC_SPAN_PIECE_OFFSET ? lc_sls_pair_inner(c.oklen, r.nd) : 0u;
+    r.body = 6 + 1 + lc_varint_size(r.pa) + r.pa + (r.pb ? 1 + lc_varint_size(r.pb) + r.pb : 0u) + (c.has_ns ? 5u : 0u);
+    const uint32_t hb = 1 + lc_varint_size(r.body);
+    r.vat = hb + 6 + 1 + lc_varint_size(r.pa) + 1 + lc_varint_size(c.klen) + c.klen + 1 + lc_varint_size(r.va);
+    r.size = hb + r.body;
+    return r;
+}
+
+// byte j of the n-byte varint of v
+LC_HD uint8_t lc_varint_byte(uint32_t v, uint32_t j, uint32_t n) {
+    return (uint8_t)(((v >> (7 * j)) & 0x7Fu) | (j + 1 < n ? 0x80u : 0u));
+}
+
+// digit j (from the left) of the nd-digit decimal v
+LC_HD uint8_t lc_dec_digit(uint64_t v, uint32_t j, uint32_t nd) {
+    for (uint32_t k = j + 1; k < nd; ++k)
+        v /= 10;
+    return (uint8_t)('0' + v % 10);
+}
+
+// byte p of a record outside the source bytes of its value: tags, lengths, keys, digits, the ns trailer
+LC_HD uint8_t lc_span_sls_meta(const LcSpanSlsCfg& c, const LcSpanRec& r, uint32_t p) {
+    uint32_t n;
+    if (p == 0)
+        return 0x0A;
+    p -= 1;
+    if (p < (n = lc_varint_size(r.body)))
+        return lc_varint_byte(r.body, p, n);
+    p -= n;
+    if (p == 0)
+        return 0x08;
+    p -= 1;
+    if (p < 5)
+        return lc_varint_byte(c.time, p, 5);
+    p -= 5;
+    if (p == 0)
+        return 0x12;
+    p -= 1;
+    if (p < (n = lc_varint_size(r.pa)))
+        return lc_varint_byte(r.pa, p, n);
+    p -= n;
+    if (p == 0)
+        return 0x0A;
+    p -= 1;
+    if (p < (n = lc_varint_size(c.klen)))
+        return lc_varint_byte(c.klen, p, n);
+    p -= n;
+    if (p < c.klen)
+        return c.key[p];
+    p -= c.klen;
+    if (p == 0)
+        return 0x12;
+    p -= 1;
+    if (p < (n = lc_varint_size(r.va)))
+        return lc_varint_byte(r.va, p, n);
+    p -= n;
+    if (c.mode == LC_SPAN_OFFSET) {
+        if (p < r.nd)
+            return lc_dec_digit(r.num, p, r.nd);
+        p -= r.nd;
+    } else {
+        p -= r.va; // (the source bytes are not asked for)
+    }
+    if (r.pb) {
+        if (p == 0)
+            return 0x12;
+        p -= 1;
+        if (p < (n = lc_varint_size(r.pb)))
+            return lc_varint_byte(r.pb, p, n);
+        p -= n;
+        if (p == 0)
+            return 0x0A;
+        p -= 1;
+        if (p < (n = lc_varint_size(c.oklen)))
+            return lc_varint_byte(c.oklen, p, n);
+        p -= n;
+        if (p < c.oklen)
+            return c.okey[p];
+        p -= c.oklen;
+        if (p == 0)
+            return 0x12;
+        p -= 1;
+        if (p == 0)
+            return (uint8_t)r.nd; // < 128: one varint byte
+        p -= 1;
+        if (p < r.nd)
+            return lc_dec_digit(r.num, p, r.nd);
+        p -= r.nd;
+    }
+    if (p == 0)
+        return 0x25;
+    return (uint8_t)(c.ns >> (8 * (p - 1)));
+}
+
+struct LcU4 {
+    uint32_t x, y, z, w;
+};
+
+LC_HD LcU4 lc_ld16(const uint8_t* p) { // p 16-byte aligned
+#if defined(__CUDA_ARCH__)
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
+    return LcU4{v.x, v.y, v.z, v.w};
+#else
+    LcU4 v;
+    memcpy(&v, p, 16);
+    return v;
+#endif
+}
+
+LC_HD void lc_st16(uint8_t* p, const LcU4& v) { // p 16-byte aligned
+#if defined(__CUDA_ARCH__)
+    *reinterpret_cast<uint4*>(p) = make_uint4(v.x, v.y, v.z, v.w);
+#else
+    memcpy(p, &v, 16);
+#endif
+}
+
+LC_HD uint32_t lc_funnel_r(uint32_t lo, uint32_t hi, uint32_t bits) { // bits in [0, 32)
+#if defined(__CUDA_ARCH__)
+    return __funnelshift_r(lo, hi, bits);
+#else
+    return bits ? (lo >> bits) | (hi << (32 - bits)) : lo;
+#endif
+}
+
+// the 16 bytes at s (any alignment).  [lo, hi) = the 16-byte aligned window of the source buffer: two aligned loads
+// and a funnel shift when both lie inside it, byte loads at the buffer's ragged ends.
+LC_HD LcU4 lc_ld16_any(const uint8_t* s, uintptr_t lo, uintptr_t hi) {
+    const uintptr_t a = (uintptr_t)s & ~(uintptr_t)15;
+    const uint32_t sh = (uint32_t)((uintptr_t)s & 15);
+    if (sh == 0)
+        return lc_ld16(s);
+    if (a >= lo && a + 32 <= hi) {
+        const LcU4 u = lc_ld16(reinterpret_cast<const uint8_t*>(a));
+        const LcU4 v = lc_ld16(reinterpret_cast<const uint8_t*>(a + 16));
+        const uint32_t q = sh >> 2, b = (sh & 3) * 8;
+        // words q .. q+4 of u:v without a dynamically indexed array
+        const uint32_t y0 = q == 0 ? u.x : q == 1 ? u.y : q == 2 ? u.z : u.w;
+        const uint32_t y1 = q == 0 ? u.y : q == 1 ? u.z : q == 2 ? u.w : v.x;
+        const uint32_t y2 = q == 0 ? u.z : q == 1 ? u.w : q == 2 ? v.x : v.y;
+        const uint32_t y3 = q == 0 ? u.w : q == 1 ? v.x : q == 2 ? v.y : v.z;
+        const uint32_t y4 = q == 0 ? v.x : q == 1 ? v.y : q == 2 ? v.z : v.w;
+        return LcU4{lc_funnel_r(y0, y1, b), lc_funnel_r(y1, y2, b), lc_funnel_r(y2, y3, b), lc_funnel_r(y3, y4, b)};
+    }
+    uint32_t w[4];
+    for (uint32_t i = 0; i < 4; ++i)
+        w[i] = (uint32_t)s[4 * i] | ((uint32_t)s[4 * i + 1] << 8) | ((uint32_t)s[4 * i + 2] << 16) |
+               ((uint32_t)s[4 * i + 3] << 24);
+    return LcU4{w[0], w[1], w[2], w[3]};
+}
+
+// dst[0, n) = s[0, n): the bytes before dst's first and after its last 16-byte boundary one by one, the words between
+// as aligned 16-byte stores; lanes share both
+LC_HD void lc_copy_span(uint8_t* dst, const uint8_t* s, uint32_t n, uintptr_t lo, uintptr_t hi, uint32_t lane,
+                        uint32_t nlanes) {
+    uint32_t head = (uint32_t)((16 - ((uintptr_t)dst & 15)) & 15);
+    if (head > n)
+        head = n;
+    const uint32_t nw = (n - head) >> 4, tail = head + nw * 16;
+    for (uint32_t j = lane; j < head + (n - tail); j += nlanes) {
+        const uint32_t k = j < head ? j : tail + (j - head);
+        dst[k] = s[k];
+    }
+    for (uint32_t w = lane; w < nw; w += nlanes)
+        lc_st16(dst + head + 16 * w, lc_ld16_any(s + head + 16 * w, lo, hi));
+}
+
+// the record holding output byte t: the last k with rec_off[k] <= t (rec_off[0] == 0, t < total)
+LC_HD uint64_t lc_span_sls_find(const uint64_t* rec_off, uint64_t n, uint64_t t) {
+    uint64_t lo = 0, hi = n;
+    while (hi - lo > 1) {
+        const uint64_t mid = lo + (hi - lo) / 2;
+        if (rec_off[mid] <= t)
+            lo = mid;
+        else
+            hi = mid;
+    }
+    return lo;
+}
+
+// Writes exactly the bytes [t0, t1) of the wire output (records back to back, record k at rec_off[k]), starting at
+// record r = lc_span_sls_find(rec_off, n, t0).  Called by `nlanes` cooperating lanes with identical arguments except
+// `lane`.
+LC_HD void lc_span_sls_tile(const LcSpanSlsCfg& c, const uint64_t* rec_off, uint64_t n, uint64_t r, uint64_t t0,
+                            uint64_t t1, uint8_t* out, uint32_t lane, uint32_t nlanes) {
+    const uintptr_t lo = ((uintptr_t)c.src + 15) & ~(uintptr_t)15;
+    const uintptr_t hi = ((uintptr_t)c.src + c.src_len) & ~(uintptr_t)15;
+    for (; r < n && rec_off[r] < t1; ++r) {
+        const uint64_t b = rec_off[r];
+        const uint32_t off = c.off[r];
+        const LcSpanRec R = lc_span_sls_rec(c, off, c.len[r]);
+        const uint32_t p0 = t0 > b ? (uint32_t)(t0 - b) : 0u;
+        const uint32_t p1 = t1 - b < R.size ? (uint32_t)(t1 - b) : R.size;
+        // the source bytes of the value: [vs, ve) of the record (none when the value is the offset)
+        const uint32_t vs = R.vat, ve = c.mode == LC_SPAN_OFFSET ? R.vat : R.vat + R.va;
+        uint8_t* o = out + b;
+        for (uint32_t p = p0 + lane; p < (p1 < vs ? p1 : vs); p += nlanes)
+            o[p] = lc_span_sls_meta(c, R, p);
+        for (uint32_t p = (p0 > ve ? p0 : ve) + lane; p < p1; p += nlanes)
+            o[p] = lc_span_sls_meta(c, R, p);
+        const uint32_t a = p0 > vs ? p0 : vs, z = p1 < ve ? p1 : ve;
+        if (a < z)
+            lc_copy_span(o + a, c.src + off + (a - vs), z - a, lo, hi, lane, nlanes);
+    }
+}

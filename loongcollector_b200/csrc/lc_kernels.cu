@@ -3692,4 +3692,36 @@ void launch_delim_sls_emit(const LcDelimSlsCfg& c, const DelimSlsTables& t, cons
                                                                                  d_body_size, d_out);
 }
 
+// ---- f4, split-fed: Log records of the pieces a splitter cuts from one source value (lc_exec.cuh: lc_span_sls_rec,
+// lc_span_sls_tile).  The size pass runs one thread per piece; the emit pass one warp per kSpanTile bytes of OUTPUT,
+// so records of 0 B and of many MiB share a launch without one warp copying a whole long record.
+__global__ void __launch_bounds__(256)
+    span_sls_size_kernel(LcSpanSlsCfg c, uint64_t n, uint32_t* __restrict__ rec_size) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n)
+        rec_size[i] = lc_span_sls_rec(c, c.off[i], c.len[i]).size;
+}
+
+__global__ void __launch_bounds__(256)
+    span_sls_emit_kernel(LcSpanSlsCfg c, const uint64_t* __restrict__ rec_off, uint64_t n, uint64_t total,
+                         uint8_t* __restrict__ out) {
+    const uint64_t t0 = (((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * kSpanTile;
+    if (t0 >= total)
+        return;
+    const uint64_t t1 = t0 + kSpanTile < total ? t0 + kSpanTile : total;
+    lc_span_sls_tile(c, rec_off, n, lc_span_sls_find(rec_off, n, t0), t0, t1, out, threadIdx.x & 31, 32);
+}
+
+void launch_span_sls_sizes(const LcSpanSlsCfg& c, uint64_t n, uint32_t* d_rec_size, cudaStream_t st) {
+    if (n)
+        span_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, n, d_rec_size);
+}
+
+void launch_span_sls_emit(const LcSpanSlsCfg& c, const uint64_t* d_rec_off, uint64_t n, uint64_t total, uint8_t* d_out,
+                          cudaStream_t st) {
+    const uint64_t warps = (total + kSpanTile - 1) / kSpanTile;
+    if (n && total)
+        span_sls_emit_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(c, d_rec_off, n, total, d_out);
+}
+
 } // namespace lck

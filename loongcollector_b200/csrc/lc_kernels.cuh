@@ -6,6 +6,7 @@
 
 struct LcDelimSlsCfg; // lc_exec.cuh
 struct LcRegexSlsCfg;
+struct LcSpanSlsCfg;
 
 namespace lck {
 
@@ -234,5 +235,13 @@ void launch_delim_sls_sizes(const LcDelimSlsCfg& c, const DelimSlsTables& t, con
 void launch_delim_sls_emit(const LcDelimSlsCfg& c, const DelimSlsTables& t, const uint32_t* d_ev_time,
                            const uint32_t* d_ev_ns, uint64_t n, const uint64_t* d_rec_off, const uint32_t* d_body_size,
                            uint8_t* d_out, cudaStream_t st);
+
+// f4, split-fed: Log records of the pieces of one source value (lc_exec.cuh: LcSpanSlsCfg, keys on the device).
+// rec_size[k] = bytes of piece k's record (never 0); the emit pass writes the `total` bytes from the record offsets,
+// one warp per kSpanTile bytes of output.
+constexpr uint32_t kSpanTile = 1024;
+void launch_span_sls_sizes(const LcSpanSlsCfg& c, uint64_t n, uint32_t* d_rec_size, cudaStream_t st);
+void launch_span_sls_emit(const LcSpanSlsCfg& c, const uint64_t* d_rec_off, uint64_t n, uint64_t total, uint8_t* d_out,
+                          cudaStream_t st);
 
 } // namespace lck

@@ -123,6 +123,10 @@ public:
     std::string mSourceKey = "content";
     char mSplitChar = '\n';
     bool mEnableRawContent = false;
+    // SLSEventGroupSerializer::Serialize after Process(group): the same bytes or error message and the same counters.
+    // A group whose events are all LogEvents {SourceKey -> value} is split and serialised on the device, one source
+    // event per call, and only the wire bytes come back; any other group runs Process + Serialize.
+    bool SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out, std::string& err);
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
@@ -140,6 +144,10 @@ public:
     std::string mSourceKey = "content";
     MultilineOptions mMultiline;
     bool mEnableRawContent = false;
+    // SLSEventGroupSerializer::Serialize after Process(group): the same bytes or error message and the same counters.
+    // A group whose events are all LogEvents {SourceKey -> value} is split and serialised on the device, one source
+    // event per call, and only the wire bytes come back; any other group runs Process + Serialize.
+    bool SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out, std::string& err);
     Counter mMatchedEventsTotal, mMatchedLinesTotal, mUnmatchedLinesTotal;
 
 protected:

@@ -132,11 +132,14 @@ char* lc_host_processor_serialize_sls(lc_host_processor_t* p, const char* group_
     if (len_out)
         *len_out = 0;
     try {
-        // the two parse processors with a one-pass device path: the same calls on either
+        // the processors with a device path to the wire format: the same calls on any of them
         auto* d = dynamic_cast<ProcessorParseDelimiterNative*>(p->proc.get());
         auto* r = dynamic_cast<ProcessorParseRegexNative*>(p->proc.get());
-        if (!d && !r)
-            throw std::runtime_error("not a processor_parse_delimiter_native or processor_parse_regex_native");
+        auto* s = dynamic_cast<ProcessorSplitLogStringNative*>(p->proc.get());
+        auto* m = dynamic_cast<ProcessorSplitMultilineLogStringNative*>(p->proc.get());
+        if (!d && !r && !s && !m)
+            throw std::runtime_error("not a processor_parse_delimiter_native, processor_parse_regex_native, "
+                                     "processor_split_string_native or processor_split_multiline_log_string_native");
         Processor* proc = p->proc.get();
         PipelineEventGroup group(std::make_shared<SourceBuffer>());
         if (!group.FromJsonString(group_json ? group_json : "null"))
@@ -150,7 +153,11 @@ char* lc_host_processor_serialize_sls(lc_host_processor_t* p, const char* group_
             ser.mEnableTimestampNanosecond = enable_ns != 0;
             ok = ser.Serialize(group, res, err);
         } else {
-            ok = d ? d->SerializeSls(group, enable_ns != 0, res, err) : r->SerializeSls(group, enable_ns != 0, res, err);
+            const bool ns = enable_ns != 0;
+            ok = d   ? d->SerializeSls(group, ns, res, err)
+                 : r ? r->SerializeSls(group, ns, res, err)
+                 : s ? s->SerializeSls(group, ns, res, err)
+                     : m->SerializeSls(group, ns, res, err);
         }
         if (proc->EngineErrors() != errs)
             throw std::runtime_error("engine error inside Process: " + proc->LastError());
