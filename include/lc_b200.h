@@ -386,6 +386,43 @@ int lc_multiline_split_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, con
                            uint32_t time, uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
                            uint64_t* n_events, uint64_t counters[3]);
 
+/* lc_regex_parse_sls / lc_delim_parse_sls finished as the SLS flusher finishes a group: the records, followed by
+ * tail[0, tail_len) (the group-level fields: topic, source, machine uuid, tags), become ONE LZ4 block (the block format
+ * of lc_lz4_compress_dev) and only the block comes back.  *raw_len = records + tail bytes (x-log-bodyrawsize),
+ * *out_len = the block's size; if it exceeds out_cap, LC_ERR_CAPACITY and nothing is written to out.  *raw_len,
+ * *out_len and counters are set on LC_OK and on LC_ERR_CAPACITY; the counters are those of the sibling call. */
+int lc_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base, uint64_t base_len,
+                           const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time,
+                           const uint32_t* ev_time_ns, const char* const* keys, const uint32_t* key_lens,
+                           uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                           uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, int whole_line,
+                           const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                           uint64_t* raw_len, uint64_t counters[3]);
+int lc_delim_parse_sls_lz4(lc_engine_t* e, const uint8_t* base, uint64_t base_len, const uint32_t* ev_off,
+                           const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time, const uint32_t* ev_time_ns,
+                           const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard,
+                           int allow_short, uint32_t max_fields, const char* const* keys, const uint32_t* key_lens,
+                           uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                           uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                           const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                           uint64_t* raw_len, uint64_t counters[4]);
+
+/* LZ4 compression of serialised groups (FlusherSLS's default compressor, LZ4Compressor::Compress =
+ * LZ4_compress_default): segment g = d_in[d_seg_off[g], + d_seg_len[g]) becomes one LZ4 *block* (not a frame), the
+ * blocks packed back to back in d_out: block g = d_out[d_blk_off[g], + d_blk_len[g]).  The bytes are deterministic;
+ * they need not equal liblz4's.  A block is never larger than LZ4_compressBound(n) = n + n / 255 + 16, and an empty
+ * segment is the single byte 0x00.  *out_len (host) = the total; if it exceeds out_cap, LC_ERR_CAPACITY and nothing is
+ * written.  A segment over LZ4_MAX_INPUT_SIZE (0x7E000000) is refused with LC_ERR_TOO_LARGE. */
+int lc_lz4_compress_dev(lc_engine_t* e, const uint8_t* d_in, uint64_t nseg, const uint64_t* d_seg_off,
+                        const uint32_t* d_seg_len, uint8_t* d_out, uint64_t out_cap, uint64_t* d_blk_off,
+                        uint32_t* d_blk_len, uint64_t* out_len);
+
+/* The same with HOST segments seg_ptr[g][0, seg_len[g]): they go up in groups of whole segments while earlier groups
+ * are parsed, and only the blocks come back (out, blk_off, blk_len on the host).  *out_len is set on LC_OK and on
+ * LC_ERR_CAPACITY. */
+int lc_lz4_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr, const uint32_t* seg_len,
+                    uint8_t* out, uint64_t out_cap, uint64_t* blk_off, uint32_t* blk_len, uint64_t* out_len);
+
 #ifdef __cplusplus
 }
 #endif

@@ -42,6 +42,21 @@ char* lc_host_processor_serialize_sls(lc_host_processor_t* p, const char* group_
                                       int process_then_serialize, unsigned long long* len_out, char** err_out,
                                       char** fail_out);
 
+/* SerializeSlsLz4 of p (a "processor_parse_delimiter_native" or a "processor_parse_regex_native") on the group
+ * described by group_json: the malloc'd LZ4 block and its length, *raw_len_out = the size of the wire bytes it
+ * decompresses to; or NULL + *err_out = the serializer's error message; NULL + *fail_out on an engine failure or a bad
+ * group. */
+char* lc_host_processor_serialize_sls_lz4(lc_host_processor_t* p, const char* group_json, int enable_ns,
+                                          unsigned long long* len_out, unsigned long long* raw_len_out, char** err_out,
+                                          char** fail_out);
+
+/* LZ4Compressor::Compress (core/common/compression/LZ4Compressor.cpp:25-44), GPU-backed: the n inputs
+ * (data[k], len[k]) in one device call, one LZ4 block each.  Returns the malloc'd blocks back to back, their total
+ * length and blk_len[k]; or NULL + *err_out = the compressor's error message ("input size is incorrect") or an engine
+ * failure. */
+char* lc_host_lz4_compress(const char* const* data, const unsigned long long* len, unsigned long long n,
+                           unsigned long long* len_out, unsigned long long* blk_len, char** err_out);
+
 /* Loads a dynamic plugin the way the agent does (dlopen, dlsym("processor_interface"), version == 100 --
  * PluginRegistry.cpp:255-275) and drives it like DynamicCProcessorProxy (.cpp:21-36): init(ins, &config, &context),
  * process(plugin_state, &group), finalize(plugin_state).  Returns the processed group's JSON ("null" when group_json

@@ -95,6 +95,12 @@ def lib():
     L.lc_split_sls.argtypes = [vp, vp, u64, u8] + span_keys + [vp, u64, C.POINTER(u64), C.POINTER(u64)]
     L.lc_multiline_split_sls.argtypes = [vp, vp, u64, vp, vp, vp, i32] + span_keys + [vp, u64, C.POINTER(u64),
                                                                                          C.POINTER(u64), vp]
+    L.lc_lz4_compress_dev.argtypes = [vp, vp, u64, vp, vp, vp, u64, vp, vp, C.POINTER(u64)]
+    L.lc_lz4_compress.argtypes = [vp, u64, vp, vp, vp, u64, vp, vp, C.POINTER(u64)]
+    L.lc_delim_parse_sls_lz4.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32, u8, i32, i32, i32, u32] + \
+        sls_cfg + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp] + sls_cfg + \
+        [i32, vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
     _LIB = L
     return L
 
@@ -450,6 +456,62 @@ class Engine:
         _check(rc)
 
     @staticmethod
+    def _sls_lz4(call, nctr, tail, out_cap, est):
+        """runs call(tail, out, cap, &need, &raw, ctr) of a fused LZ4 call, sized by est first and by the exact block
+        size when that was short; returns (block, raw_len, counters)"""
+        tl = np.frombuffer(bytes(tail), np.uint8)
+        cap = int(out_cap if out_cap is not None else est + est // 255 + 16)
+        for _ in range(2):
+            out = np.empty(max(cap, 1), np.uint8)
+            need, raw = C.c_uint64(0), C.c_uint64(0)
+            ctr = np.zeros(nctr, np.uint64)
+            rc = call(_p(tl) if tl.size else None, tl.size, _p(out), cap, C.byref(need), C.byref(raw), _p(ctr))
+            if rc == LC_ERR_CAPACITY and out_cap is None:
+                cap = int(need.value)
+                continue
+            _check(rc)
+            return bytes(out[:need.value]), int(raw.value), ctr
+        _check(rc)
+
+    def regex_parse_sls_lz4(self, rx, base, ev_off, ev_len, ev_time, keys, source_key, renamed_key=None,
+                            keep_fail=False, keep_succeed=False, copy_raw=False, whole_line=False, ev_time_ns=None,
+                            tail=b"", out_cap=None):
+        """regex_parse_sls's records followed by `tail` (the group-level fields) as ONE LZ4 block
+        (lc_regex_parse_sls_lz4).  Returns (block, raw_len, counters[3])."""
+        a = _u8(base)
+        ev_off = np.ascontiguousarray(ev_off, np.uint32)
+        ev_len = np.ascontiguousarray(ev_len, np.uint32)
+        t = np.ascontiguousarray(ev_time, np.uint32)
+        ns = None if ev_time_ns is None else np.ascontiguousarray(ev_time_ns, np.uint32)
+        n = ev_off.size
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        return self._sls_lz4(
+            lambda *rest: lib().lc_regex_parse_sls_lz4(self._h, _rh(rx), _p(a), a.size, _p(ev_off), _p(ev_len), n,
+                                                       _p(t), _p(ns), *cfg, int(bool(whole_line)), *rest),
+            3, tail, out_cap, 2 * a.size + 64 * n + 64 + len(tail))
+
+    def delim_parse_sls_lz4(self, base, ev_off, ev_len, ev_time, sep: bytes, quote, treatment, keys, source_key,
+                            renamed_key=None, keep_fail=False, keep_succeed=False, copy_raw=False, allow_short=True,
+                            max_fields=None, ev_time_ns=None, tail=b"", out_cap=None):
+        """delim_parse_sls's records followed by `tail` (the group-level fields) as ONE LZ4 block
+        (lc_delim_parse_sls_lz4).  Returns (block, raw_len, counters[4])."""
+        a = _u8(base)
+        ev_off = np.ascontiguousarray(ev_off, np.uint32)
+        ev_len = np.ascontiguousarray(ev_len, np.uint32)
+        t = np.ascontiguousarray(ev_time, np.uint32)
+        ns = None if ev_time_ns is None else np.ascontiguousarray(ev_time_ns, np.uint32)
+        n = ev_off.size
+        mf = int(max_fields if max_fields is not None else len(keys) + 16)
+        sp = np.frombuffer(sep, np.uint8)
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        return self._sls_lz4(
+            lambda *rest: lib().lc_delim_parse_sls_lz4(self._h, _p(a), a.size, _p(ev_off), _p(ev_len), n, _p(t),
+                                                       _p(ns), _p(sp), len(sep), quote, int(treatment == "extend"),
+                                                       int(treatment == "discard"), int(bool(allow_short)), mf, *cfg,
+                                                       *rest),
+            4, tail, out_cap, 2 * a.size + 64 * n + 64 + len(tail))
+
+    @staticmethod
     def _span_keys(key, offset_key, src_pos, time, time_ns):
         """key / offset_key: bytes (offset_key None = no offset key); time_ns None = no Time_ns"""
         return [key, len(key), offset_key, len(offset_key) if offset_key is not None else 0, int(src_pos),
@@ -500,6 +562,33 @@ class Engine:
                                     [_rh(start), _rh(cont), _rh(end), int(bool(discard))], key, offset_key, src_pos,
                                     time, time_ns, out_cap, [ctr])
         return data, nev, ctr
+
+    def lz4_compress_dev(self, d_in, nseg, d_seg_off, d_seg_len, d_out=None, out_cap=0, d_blk_off=None,
+                         d_blk_len=None):
+        """One LZ4 block per device segment d_in[d_seg_off[g], + d_seg_len[g]) (u64 / u32 tables), packed in d_out
+        with the table d_blk_off (u64) / d_blk_len (u32) (lc_lz4_compress_dev).  Returns the byte count written to
+        d_out, or with d_out None the byte count needed."""
+        need = C.c_uint64(0)
+        rc = lib().lc_lz4_compress_dev(self._h, _p(d_in), nseg, _p(d_seg_off), _p(d_seg_len), _p(d_out), out_cap,
+                                       _p(d_blk_off), _p(d_blk_len), C.byref(need))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value)  # a sizing query
+        _check(rc)
+        return int(need.value)
+
+    def lz4_compress(self, segments, out_cap=None):
+        """Host segments (bytes-like) in, one LZ4 block each out (lc_lz4_compress).  Returns the list of blocks."""
+        segs = [_u8(s) for s in segments]
+        n = len(segs)
+        ptrs = (C.c_void_p * max(n, 1))(*[s.ctypes.data for s in segs])
+        lens = np.array([s.size for s in segs] or [0], np.uint32)
+        cap = int(out_cap if out_cap is not None else sum(int(x) + int(x) // 255 + 16 for x in lens))
+        out = np.empty(max(cap, 1), np.uint8)
+        boff, blen = np.zeros(max(n, 1), np.uint64), np.zeros(max(n, 1), np.uint32)
+        need = C.c_uint64(0)
+        _check(lib().lc_lz4_compress(self._h, n, C.cast(ptrs, C.c_void_p), _p(lens), _p(out), cap, _p(boff),
+                                     _p(blen), C.byref(need)))
+        return [bytes(out[int(o):int(o) + int(ln)]) for o, ln in zip(boff[:n], blen[:n])]
 
     def split_lines_dev(self, d_buf, length, split_char, d_off, d_len, cap):
         n = C.c_uint64(0)
@@ -632,6 +721,62 @@ class HostProcessor:
         data = C.string_at(out, n.value)
         L.lc_host_string_free(out)
         return data, None
+
+    def serialize_sls_lz4(self, group, enable_ns=False):
+        """SerializeSlsLz4 of a processor_parse_delimiter_native or processor_parse_regex_native on a JSON group:
+        (block, raw_len, None) or (None, 0, error)."""
+        import json
+        L = lib()
+        L.lc_host_processor_serialize_sls_lz4.restype = C.c_void_p
+        L.lc_host_processor_serialize_sls_lz4.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_ulonglong),
+                                                          C.POINTER(C.c_ulonglong), C.POINTER(C.c_void_p),
+                                                          C.POINTER(C.c_void_p)]
+        L.lc_host_string_free.argtypes = [C.c_void_p]
+        err, fail = C.c_void_p(), C.c_void_p()
+        n, raw = C.c_ulonglong(0), C.c_ulonglong(0)
+        out = L.lc_host_processor_serialize_sls_lz4(self._h, json.dumps(group).encode("utf-8"), int(bool(enable_ns)),
+                                                    C.byref(n), C.byref(raw), C.byref(err), C.byref(fail))
+        if fail.value:
+            msg = C.string_at(fail.value).decode()
+            L.lc_host_string_free(fail)
+            raise LcError(LC_ERR_CUDA, msg)
+        if not out:
+            msg = C.string_at(err.value).decode() if err.value else "unknown error"
+            if err.value:
+                L.lc_host_string_free(err)
+            return None, 0, msg
+        data = C.string_at(out, n.value)
+        L.lc_host_string_free(out)
+        return data, int(raw.value), None
+
+
+def host_lz4_compress(inputs):
+    """The host layer's GPU-backed LZ4Compressor::Compress over a list of byte strings in one device call
+    (lc_host_lz4_compress): (list of blocks, None) or (None, error)."""
+    L = lib()
+    L.lc_host_lz4_compress.restype = C.c_void_p
+    L.lc_host_lz4_compress.argtypes = [C.c_void_p, C.c_void_p, C.c_ulonglong, C.POINTER(C.c_ulonglong), C.c_void_p,
+                                       C.POINTER(C.c_void_p)]
+    L.lc_host_string_free.argtypes = [C.c_void_p]
+    bufs = [bytes(x) for x in inputs]
+    n = len(bufs)
+    ptrs = (C.c_char_p * max(n, 1))(*bufs)
+    lens = np.array([len(b) for b in bufs] or [0], np.uint64)
+    blen = np.zeros(max(n, 1), np.uint64)
+    total, err = C.c_ulonglong(0), C.c_void_p()
+    out = L.lc_host_lz4_compress(C.cast(ptrs, C.c_void_p), _p(lens), n, C.byref(total), _p(blen), C.byref(err))
+    if not out:
+        msg = C.string_at(err.value).decode() if err.value else "unknown error"
+        if err.value:
+            L.lc_host_string_free(err)
+        return None, msg
+    data = C.string_at(out, total.value)
+    L.lc_host_string_free(out)
+    res, o = [], 0
+    for k in range(n):
+        res.append(data[o:o + int(blen[k])])
+        o += int(blen[k])
+    return res, None
 
 
 def host_sls_serialize(group, enable_ns=False):

@@ -99,6 +99,9 @@ struct lc_engine {
     DevBuf desc;   // look-back descriptors of exclusive sums
     DevBuf split_scratch; // masks + per-tile counts of the three-pass split (lck::split_scratch_bytes)
     DevBuf sls_plan; // content plans + key strings of the regex-fed SLS serialiser (`order` is the regex stage's)
+    // LZ4 compressor: sequences, chunk summaries, chunk sizes / anchors, chunk and block offsets, host-call tables and
+    // output; no parse or SLS stage uses them
+    DevBuf z_seq, z_info, z_size, z_first, z_choff, z_tab, z_out;
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
     std::unordered_map<uint64_t, void*> blobs; // regex id * 4 + layout -> device blob
@@ -310,7 +313,8 @@ void lc_engine_destroy(lc_engine_t* e) {
         cudaStreamSynchronize(e->stream);
     DevBuf* bufs[] = {&e->in, &e->ev_off, &e->ev_len, &e->out_a, &e->out_b, &e->out_c, &e->out_d, &e->out_e,
                       &e->lines_off, &e->lines_len, &e->flags, &e->state, &e->cnt, &e->pos, &e->lab_sizes,
-                      &e->lab_off, &e->lab, &e->order, &e->desc, &e->small, &e->split_scratch, &e->sls_plan};
+                      &e->lab_off, &e->lab, &e->order, &e->desc, &e->small, &e->split_scratch, &e->sls_plan,
+                      &e->z_seq, &e->z_info, &e->z_size, &e->z_first, &e->z_choff, &e->z_tab, &e->z_out};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -1785,18 +1789,42 @@ int serialize_sls_dev(lc_engine_t* e, const char* what, uint64_t n, uint32_t nco
     return LC_OK;
 }
 
+// The fused LZ4 calls (lc_regex_parse_sls_lz4, lc_delim_parse_sls_lz4): the group-level fields that follow the
+// records, and where the records' size plus theirs goes
+struct Lz4Tail {
+    const uint8_t* tail;
+    uint64_t len;
+    uint64_t* raw_len;
+};
+int lz4_one_block(lc_engine_t* e, const char* what, const uint8_t* d_src, uint64_t raw, uint8_t* out, uint64_t out_cap,
+                  uint64_t* out_len);
+
+// a fused call without events: the block of the tail alone
+int lz4_tail_only(lc_engine_t* e, const char* what, const Lz4Tail& z, uint8_t* out, uint64_t out_cap,
+                  uint64_t* out_len) {
+    *z.raw_len = z.len;
+    if (z.len > LC_LZ4_MAX_INPUT)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": tail larger than LZ4_MAX_INPUT_SIZE");
+    CU_TRY(e->lab.ensure(z.len + 16));
+    if (z.len)
+        CU_TRY(cudaMemcpyAsync(e->lab.p, z.tail, z.len, cudaMemcpyHostToDevice, e->stream));
+    return lz4_one_block(e, what, e->lab.as<uint8_t>(), z.len, out, out_cap, out_len);
+}
+
 // Parse and serialise host buffers in one call (lc_delim_parse_sls, lc_regex_parse_sls).  The arena goes up once, in
 // chunks of whole events on a copy stream (pipelined_events); per chunk the event times go up, `parse(i0, cnt, span)`
 // queues the processor's kernels and `sizes(i0, cnt, d_ns, rec_size, body_size, d_counters)` the size pass.  No table
 // comes back.  Then one exclusive sum, `emit(d_time, d_ns, rec_off, body_size, d_wire)` over all n events, and one
 // copy of the wire bytes.  Workspace besides the arena, the event table and the processor's own tables: lines_off /
 // lines_len = times / ns, flags / cnt = record / body sizes, pos = record offsets, state = the counters, lab = the
-// wire bytes.  The regex and delimiter stages touch none of them while the chunks are parsed.
+// wire bytes.  The regex and delimiter stages touch none of them while the chunks are parsed.  With z (the fused LZ4
+// calls) the tail lands after the records in `lab`, records ‖ tail become one LZ4 block and only the block comes back:
+// out_cap and *out_len are then the block's.
 template <class Parse, class Sizes, class Emit>
 int parse_sls_host(lc_engine_t* e, const char* what, const uint8_t* base, uint64_t base_len, const uint32_t* ev_off,
                    const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time, const uint32_t* ev_time_ns,
                    uint32_t ncounters, Parse parse, Sizes sizes, Emit emit, uint8_t* out, uint64_t out_cap,
-                   uint64_t* out_len, uint64_t* counters) {
+                   uint64_t* out_len, uint64_t* counters, const Lz4Tail* z = nullptr) {
     CU_TRY(e->in.ensure(base_len + 16));
     CU_TRY(e->ev_off.ensure(n * 4));
     CU_TRY(e->ev_len.ensure(n * 4));
@@ -1843,6 +1871,21 @@ int parse_sls_host(lc_engine_t* e, const char* what, const uint8_t* base, uint64
     CU_TRY(cudaStreamSynchronize(e->stream));
     for (uint32_t k = 0; k < ncounters; ++k)
         counters[k] = ctr[k];
+    if (z) {
+        const uint64_t total = hs->total, raw = total + z->len;
+        *z->raw_len = raw;
+        if (raw > LC_LZ4_MAX_INPUT)
+            return fail(LC_ERR_TOO_LARGE, std::string(what) + ": records and tail are larger than LZ4_MAX_INPUT_SIZE");
+        CU_TRY(e->lab.ensure(raw + 16));
+        if (total) {
+            emit(d_time, d_ns, e->pos.as<uint64_t>(), d_body, e->lab.as<uint8_t>());
+            e->launches++;
+            CU_TRY(cudaGetLastError());
+        }
+        if (z->len)
+            CU_TRY(cudaMemcpyAsync(e->lab.as<uint8_t>() + total, z->tail, z->len, cudaMemcpyHostToDevice, e->stream));
+        return lz4_one_block(e, what, e->lab.as<uint8_t>(), raw, out, out_cap, out_len);
+    }
     *out_len = hs->total;
     if (hs->total > out_cap)
         return fail(LC_ERR_CAPACITY, std::string(what) + ": output capacity too small");
@@ -2133,17 +2176,21 @@ int lc_sls_serialize_regex_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t b
         d_out, out_cap, out_len, counters);
 }
 
-int lc_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base, uint64_t base_len,
-                       const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time,
-                       const uint32_t* ev_time_ns, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
-                       const char* source_key, uint32_t source_key_len, const char* renamed_key,
-                       uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, int whole_line,
-                       uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[3]) {
-    static const char* what = "lc_regex_parse_sls";
+} // extern "C"
+
+static int regex_parse_sls_impl(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* base,
+                                uint64_t base_len, const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n,
+                                const uint32_t* ev_time, const uint32_t* ev_time_ns, const char* const* keys,
+                                const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+                                uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+                                int keep_fail, int keep_succeed, int copy_raw, int whole_line, uint8_t* out,
+                                uint64_t out_cap, uint64_t* out_len, uint64_t counters[3], const Lz4Tail* z) {
     if (!e || (!re && !whole_line) || !out_len || !counters || (n && (!ev_off || !ev_len || !ev_time)) ||
-        (base_len && !base))
+        (base_len && !base) || (z && (!z->raw_len || (z->len && !z->tail))))
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
     *out_len = 0;
+    if (z)
+        *z->raw_len = 0;
     memset(counters, 0, 3 * sizeof(uint64_t));
     int rc = whole_line ? (int)LC_OK : check_regex_usable(re, what);
     if (rc)
@@ -2158,7 +2205,7 @@ int lc_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base
     rc = regex_sls_config(e, what, keys, key_lens, nkeys, source_key, source_key_len, renamed_key, renamed_key_len,
                           keep_fail, keep_succeed, copy_raw, whole_line, G, &c);
     if (rc || n == 0)
-        return rc;
+        return rc || !z ? rc : lz4_tail_only(e, what, *z, out, out_cap, out_len);
     // the regex tables (out_a = status, out_b / out_c = captures) stay on the device; whole-line mode runs no regex
     if (!whole_line) {
         CU_TRY(e->out_a.ensure(n));
@@ -2188,7 +2235,35 @@ int lc_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base
         lck::launch_regex_sls_emit(c, tables(0), d_time, d_ns, n, rec_off, body, d_wire, e->stream);
     };
     return parse_sls_host(e, what, base, base_len, ev_off, ev_len, n, ev_time, ev_time_ns, 3, parse, sizes, emit, out,
-                          out_cap, out_len, counters);
+                          out_cap, out_len, counters, z);
+}
+
+extern "C" {
+
+int lc_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base, uint64_t base_len,
+                       const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time,
+                       const uint32_t* ev_time_ns, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                       const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                       uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, int whole_line,
+                       uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[3]) {
+    return regex_parse_sls_impl(e, "lc_regex_parse_sls", re, base, base_len, ev_off, ev_len, n, ev_time, ev_time_ns,
+                                keys, key_lens, nkeys, source_key, source_key_len, renamed_key, renamed_key_len,
+                                keep_fail, keep_succeed, copy_raw, whole_line, out, out_cap, out_len, counters,
+                                nullptr);
+}
+
+int lc_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base, uint64_t base_len,
+                           const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time,
+                           const uint32_t* ev_time_ns, const char* const* keys, const uint32_t* key_lens,
+                           uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                           uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, int whole_line,
+                           const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                           uint64_t* raw_len, uint64_t counters[3]) {
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return regex_parse_sls_impl(e, "lc_regex_parse_sls_lz4", re, base, base_len, ev_off, ev_len, n, ev_time,
+                                ev_time_ns, keys, key_lens, nkeys, source_key, source_key_len, renamed_key,
+                                renamed_key_len, keep_fail, keep_succeed, copy_raw, whole_line, out, out_cap, out_len,
+                                counters, &z);
 }
 
 int lc_sls_serialize_delim_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t base_len, const uint32_t* d_ev_off,
@@ -2227,17 +2302,22 @@ int lc_sls_serialize_delim_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t b
         d_out, out_cap, out_len, nullptr);
 }
 
-int lc_delim_parse_sls(lc_engine_t* e, const uint8_t* base, uint64_t base_len, const uint32_t* ev_off,
-                       const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time, const uint32_t* ev_time_ns,
-                       const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard, int allow_short,
-                       uint32_t max_fields, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
-                       const char* source_key, uint32_t source_key_len, const char* renamed_key,
-                       uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, uint8_t* out,
-                       uint64_t out_cap, uint64_t* out_len, uint64_t counters[4]) {
-    static const char* what = "lc_delim_parse_sls";
-    if (!e || !out_len || !counters || (n && (!ev_off || !ev_len || !ev_time)) || (base_len && !base))
+} // extern "C"
+
+static int delim_parse_sls_impl(lc_engine_t* e, const char* what, const uint8_t* base, uint64_t base_len,
+                                const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time,
+                                const uint32_t* ev_time_ns, const uint8_t* sep, uint32_t sep_len, uint8_t quote,
+                                int extend, int discard, int allow_short, uint32_t max_fields, const char* const* keys,
+                                const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+                                uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+                                int keep_fail, int keep_succeed, int copy_raw, uint8_t* out, uint64_t out_cap,
+                                uint64_t* out_len, uint64_t counters[4], const Lz4Tail* z) {
+    if (!e || !out_len || !counters || (n && (!ev_off || !ev_len || !ev_time)) || (base_len && !base) ||
+        (z && (!z->raw_len || (z->len && !z->tail))))
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
     *out_len = 0;
+    if (z)
+        *z->raw_len = 0;
     memset(counters, 0, 4 * sizeof(uint64_t));
     if (base_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32))
         return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 events and < 2^32 columns per call");
@@ -2248,7 +2328,7 @@ int lc_delim_parse_sls(lc_engine_t* e, const uint8_t* base, uint64_t base_len, c
     rc = delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, keys, key_lens, nkeys, source_key,
                           source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed, copy_raw, &c);
     if (rc || n == 0)
-        return rc;
+        return rc || !z ? rc : lz4_tail_only(e, what, *z, out, out_cap, out_len);
     // the delimiter tables (out_a = status, out_b = column counts, out_c..out_e = [n][max_fields]) stay on the device
     const uint64_t MF = max_fields, fbytes = n * MF * 4;
     CU_TRY(e->out_a.ensure(n));
@@ -2278,7 +2358,37 @@ int lc_delim_parse_sls(lc_engine_t* e, const uint8_t* base, uint64_t base_len, c
         lck::launch_delim_sls_emit(c, tables(0), d_time, d_ns, n, rec_off, body, d_wire, e->stream);
     };
     return parse_sls_host(e, what, base, base_len, ev_off, ev_len, n, ev_time, ev_time_ns, 4, parse, sizes, emit, out,
-                          out_cap, out_len, counters);
+                          out_cap, out_len, counters, z);
+}
+
+extern "C" {
+
+int lc_delim_parse_sls(lc_engine_t* e, const uint8_t* base, uint64_t base_len, const uint32_t* ev_off,
+                       const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time, const uint32_t* ev_time_ns,
+                       const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard, int allow_short,
+                       uint32_t max_fields, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                       const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                       uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, uint8_t* out,
+                       uint64_t out_cap, uint64_t* out_len, uint64_t counters[4]) {
+    return delim_parse_sls_impl(e, "lc_delim_parse_sls", base, base_len, ev_off, ev_len, n, ev_time, ev_time_ns, sep,
+                                sep_len, quote, extend, discard, allow_short, max_fields, keys, key_lens, nkeys,
+                                source_key, source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed,
+                                copy_raw, out, out_cap, out_len, counters, nullptr);
+}
+
+int lc_delim_parse_sls_lz4(lc_engine_t* e, const uint8_t* base, uint64_t base_len, const uint32_t* ev_off,
+                           const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time, const uint32_t* ev_time_ns,
+                           const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard,
+                           int allow_short, uint32_t max_fields, const char* const* keys, const uint32_t* key_lens,
+                           uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                           uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                           const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                           uint64_t* raw_len, uint64_t counters[4]) {
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return delim_parse_sls_impl(e, "lc_delim_parse_sls_lz4", base, base_len, ev_off, ev_len, n, ev_time, ev_time_ns,
+                                sep, sep_len, quote, extend, discard, allow_short, max_fields, keys, key_lens, nkeys,
+                                source_key, source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed,
+                                copy_raw, out, out_cap, out_len, counters, &z);
 }
 
 int lc_sls_serialize_spans_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
@@ -2331,6 +2441,232 @@ int lc_multiline_split_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, con
     };
     return split_sls_host(e, "lc_multiline_split_sls", buf, len, split, key, key_len, offset_key, offset_key_len,
                           src_pos, time, time_ns, out, out_cap, out_len, n_events);
+}
+
+} // extern "C"
+
+// ------------------------------------------------------------------------------------------------ LZ4
+namespace {
+
+// chunk tables of the segments in g (g.in, g.seg_off, g.seg_len, g.nseg set): g.first / g.nchunks, and room for the
+// parse.  first_host (or nullptr): the chunk table already built on the host, uploaded instead of counted.
+int lz4_chunk_tables(lc_engine_t* e, const char* what, lck::Lz4Segs& g, const uint64_t* first_host,
+                     uint64_t nchunks_host) {
+    CU_TRY(e->z_first.ensure(g.nseg * 8 + 8));
+    uint64_t* d_first = e->z_first.as<uint64_t>();
+    if (first_host) {
+        CU_TRY(cudaMemcpyAsync(d_first, first_host, g.nseg * 8, cudaMemcpyHostToDevice, e->stream));
+        g.nchunks = nchunks_host;
+    } else {
+        CU_TRY(e->z_size.ensure(g.nseg * 4 + 4));
+        uint64_t* desc;
+        int rc = prep_desc(e, lck::scan_tiles(g.nseg), &desc);
+        if (rc)
+            return rc;
+        Small* ds = e->small.as<Small>();
+        Small* hs = (Small*)e->h_small;
+        lck::launch_lz4_chunks(g.seg_len, g.nseg, e->z_size.as<uint32_t>(), &ds->overflow, e->stream);
+        lck::launch_exclusive_sum(e->z_size.as<uint32_t>(), g.nseg, d_first, &ds->total, desc, &ds->tickets[2],
+                                  e->stream);
+        e->launches += 2;
+        CU_TRY(cudaGetLastError());
+        CU_TRY(cudaMemcpyAsync(hs, ds, sizeof(Small), cudaMemcpyDeviceToHost, e->stream));
+        CU_TRY(cudaStreamSynchronize(e->stream));
+        if (hs->overflow)
+            return fail(LC_ERR_TOO_LARGE, std::string(what) + ": a segment is larger than LZ4_MAX_INPUT_SIZE");
+        g.nchunks = hs->total;
+    }
+    g.first = d_first;
+    CU_TRY(e->z_seq.ensure(g.nchunks * LC_LZ4_SEQ_CAP * sizeof(LcLz4Seq)));
+    CU_TRY(e->z_info.ensure(g.nchunks * sizeof(LcLz4Chunk)));
+    CU_TRY(e->z_size.ensure(g.nchunks * 8));
+    CU_TRY(e->z_choff.ensure(g.nchunks * 8 + 8));
+    return LC_OK;
+}
+
+// After the parse of every chunk: sizes, block offsets, and (when the total fits out_cap) the blocks at d_out and the
+// per-segment table.  *out_len = the total on LC_OK and on LC_ERR_CAPACITY.  d_out == nullptr: the engine's z_out.
+int lz4_finish(lc_engine_t* e, const char* what, const lck::Lz4Segs& g, uint8_t* d_out, uint64_t out_cap,
+               uint64_t* d_blk_off, uint32_t* d_blk_len, uint64_t* out_len) {
+    LcLz4Chunk* d_info = e->z_info.as<LcLz4Chunk>();
+    uint32_t* d_csize = e->z_size.as<uint32_t>();
+    uint32_t* d_anchor = d_csize + g.nchunks;
+    lck::launch_lz4_sizes(g, d_info, d_csize, d_anchor, e->stream);
+    uint64_t* desc;
+    int rc = prep_desc(e, lck::scan_tiles(g.nchunks), &desc);
+    if (rc)
+        return rc;
+    Small* ds = e->small.as<Small>();
+    Small* hs = (Small*)e->h_small;
+    lck::launch_exclusive_sum(d_csize, g.nchunks, e->z_choff.as<uint64_t>(), &ds->total, desc, &ds->tickets[2],
+                              e->stream);
+    e->launches += 2;
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(&hs->total, &ds->total, 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    *out_len = hs->total;
+    if (hs->total > out_cap)
+        return fail(LC_ERR_CAPACITY, std::string(what) + ": output capacity too small");
+    if (!d_out) {
+        CU_TRY(e->z_out.ensure(hs->total));
+        d_out = e->z_out.as<uint8_t>();
+    }
+    lck::launch_lz4_emit(g, e->z_seq.as<LcLz4Seq>(), d_info, d_anchor, e->z_choff.as<uint64_t>(), &ds->total, d_out,
+                         d_blk_off, d_blk_len, e->stream);
+    e->launches += 2;
+    CU_TRY(cudaGetLastError());
+    return LC_OK;
+}
+
+// One block of d_src[0, raw) (the fused calls' records ‖ tail) in z_out; only the block comes back to out.
+int lz4_one_block(lc_engine_t* e, const char* what, const uint8_t* d_src, uint64_t raw, uint8_t* out, uint64_t out_cap,
+                  uint64_t* out_len) {
+    CU_TRY(e->z_tab.ensure(24));
+    uint64_t* d_soff = e->z_tab.as<uint64_t>();
+    uint64_t* d_boff = d_soff + 1;
+    uint32_t* d_slen = reinterpret_cast<uint32_t*>(d_boff + 1);
+    uint32_t* d_blen = d_slen + 1;
+    const uint64_t zero = 0;
+    const uint32_t len32 = (uint32_t)raw;
+    CU_TRY(cudaMemcpyAsync(d_soff, &zero, 8, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(d_slen, &len32, 4, cudaMemcpyHostToDevice, e->stream));
+    lck::Lz4Segs g{d_src, d_soff, d_slen, nullptr, 1, 0};
+    int rc = lz4_chunk_tables(e, what, g, &zero, lc_lz4_nchunks(len32));
+    if (rc)
+        return rc;
+    lck::launch_lz4_parse(g, 0, g.nchunks, e->z_seq.as<LcLz4Seq>(), e->z_info.as<LcLz4Chunk>(), e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    rc = lz4_finish(e, what, g, nullptr, out_cap, d_boff, d_blen, out_len);
+    if (rc)
+        return rc;
+    if (!out)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    CU_TRY(cudaMemcpyAsync(out, e->z_out.p, *out_len, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    return LC_OK;
+}
+
+} // namespace
+
+extern "C" {
+
+int lc_lz4_compress_dev(lc_engine_t* e, const uint8_t* d_in, uint64_t nseg, const uint64_t* d_seg_off,
+                        const uint32_t* d_seg_len, uint8_t* d_out, uint64_t out_cap, uint64_t* d_blk_off,
+                        uint32_t* d_blk_len, uint64_t* out_len) {
+    static const char* what = "lc_lz4_compress_dev";
+    if (!e || !out_len || (nseg && (!d_in || !d_seg_off || !d_seg_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (nseg == 0)
+        return LC_OK;
+    if (nseg >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^32 segments per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    lck::Lz4Segs g{d_in, d_seg_off, d_seg_len, nullptr, nseg, 0};
+    rc = lz4_chunk_tables(e, what, g, nullptr, 0);
+    if (rc)
+        return rc;
+    lck::launch_lz4_parse(g, 0, g.nchunks, e->z_seq.as<LcLz4Seq>(), e->z_info.as<LcLz4Chunk>(), e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    // without an output (a sizing query) every total is over capacity: blocks are at least one byte
+    rc = lz4_finish(e, what, g, d_out, d_out && d_blk_off && d_blk_len ? out_cap : 0, d_blk_off, d_blk_len, out_len);
+    if (rc)
+        return rc;
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    return LC_OK;
+}
+
+int lc_lz4_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr, const uint32_t* seg_len,
+                    uint8_t* out, uint64_t out_cap, uint64_t* blk_off, uint32_t* blk_len, uint64_t* out_len) {
+    static const char* what = "lc_lz4_compress";
+    if (!e || !out_len || (nseg && (!seg_ptr || !seg_len || !blk_off || !blk_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (nseg == 0)
+        return LC_OK;
+    if (nseg >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^32 segments per call");
+    // the segments are packed at 16-byte aligned offsets of the engine's input buffer; the chunk table is built here
+    std::vector<uint64_t> soff(nseg), first(nseg);
+    uint64_t total_in = 0, nchunks = 0;
+    for (uint64_t k = 0; k < nseg; ++k) {
+        if (seg_len[k] && !seg_ptr[k])
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+        if (seg_len[k] > LC_LZ4_MAX_INPUT)
+            return fail(LC_ERR_TOO_LARGE, std::string(what) + ": a segment is larger than LZ4_MAX_INPUT_SIZE");
+        soff[k] = total_in;
+        total_in += (seg_len[k] + 15ull) & ~15ull;
+        first[k] = nchunks;
+        nchunks += lc_lz4_nchunks(seg_len[k]);
+    }
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    CU_TRY(e->in.ensure(total_in + 16));
+    CU_TRY(e->z_tab.ensure(nseg * 24));
+    uint64_t* d_soff = e->z_tab.as<uint64_t>();
+    uint64_t* d_boff = d_soff + nseg;
+    uint32_t* d_slen = reinterpret_cast<uint32_t*>(d_boff + nseg);
+    uint32_t* d_blen = d_slen + nseg;
+    CU_TRY(cudaMemcpyAsync(d_soff, soff.data(), nseg * 8, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(d_slen, seg_len, nseg * 4, cudaMemcpyHostToDevice, e->stream));
+    lck::Lz4Segs g{e->in.as<uint8_t>(), d_soff, d_slen, nullptr, nseg, 0};
+    rc = lz4_chunk_tables(e, what, g, first.data(), nchunks);
+    if (rc)
+        return rc;
+    // groups of whole segments go up on the copy stream; each group's chunks are parsed as soon as it has landed
+    const uint64_t kGroupBytes = 32ull << 20;
+    uint64_t ngroups = (total_in + kGroupBytes - 1) / kGroupBytes;
+    ngroups = ngroups < 1 ? 1 : ngroups > 64 ? 64 : ngroups;
+    if (ngroups > nseg)
+        ngroups = nseg;
+    rc = ensure_copy_streams(e, (int)ngroups);
+    if (rc)
+        return rc;
+    auto drain = [&](int code) {
+        cudaStreamSynchronize(e->s_h2d);
+        cudaStreamSynchronize(e->stream);
+        return code;
+    };
+    if (cudaEventRecord(e->ev_comp[0], e->stream) != cudaSuccess ||
+        cudaStreamWaitEvent(e->s_h2d, e->ev_comp[0], 0) != cudaSuccess)
+        return drain(fail(LC_ERR_CUDA, "stream ordering failed"));
+    uint8_t* d_in = e->in.as<uint8_t>();
+    uint64_t s0 = 0;
+    for (uint64_t c = 0; c < ngroups; ++c) {
+        uint64_t s1 = s0;
+        const uint64_t goal = total_in * (c + 1) / ngroups;
+        while (s1 < nseg && (s1 == s0 || soff[s1] < goal || c + 1 == ngroups))
+            ++s1;
+        for (uint64_t k = s0; k < s1; ++k)
+            if (seg_len[k] && cudaMemcpyAsync(d_in + soff[k], seg_ptr[k], seg_len[k], cudaMemcpyHostToDevice,
+                                              e->s_h2d) != cudaSuccess)
+                return drain(fail(LC_ERR_CUDA, std::string(what) + ": upload failed"));
+        if (cudaEventRecord(e->ev_h2d[c], e->s_h2d) != cudaSuccess ||
+            cudaStreamWaitEvent(e->stream, e->ev_h2d[c], 0) != cudaSuccess)
+            return drain(fail(LC_ERR_CUDA, "stream ordering failed"));
+        const uint64_t k1 = s1 < nseg ? first[s1] : nchunks;
+        lck::launch_lz4_parse(g, s0 < nseg ? first[s0] : nchunks, k1, e->z_seq.as<LcLz4Seq>(),
+                              e->z_info.as<LcLz4Chunk>(), e->stream);
+        e->launches++;
+        s0 = s1;
+    }
+    if (cudaGetLastError() != cudaSuccess)
+        return drain(fail(LC_ERR_CUDA, std::string(what) + ": parse launch failed"));
+    rc = lz4_finish(e, what, g, nullptr, out_cap, d_boff, d_blen, out_len);
+    if (rc)
+        return drain(rc);
+    if (*out_len && !out)
+        return drain(fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments"));
+    CU_TRY(cudaMemcpyAsync(out, e->z_out.p, *out_len, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(blk_off, d_boff, nseg * 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(blk_len, d_blen, nseg * 4, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    return LC_OK;
 }
 
 } // extern "C"

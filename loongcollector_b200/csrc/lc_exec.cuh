@@ -1616,3 +1616,245 @@ LC_HD void lc_span_sls_tile(const LcSpanSlsCfg& c, const uint64_t* rec_off, uint
             lc_copy_span(o + a, c.src + off + (a - vs), z - a, lo, hi, lane, nlanes);
     }
 }
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, LZ4: one LZ4 *block* (what LZ4_compress_default emits and the SLS server decodes with x-log-bodyrawsize) per
+// segment.  A segment is cut into chunks of LC_LZ4_CHUNK bytes; the bytes are a sequential function of the segment:
+//   candidate(p)  = the latest q < p with hash(q) == hash(p), kept as q mod 2^16 (so read as the q' = p - d with
+//                   d = (p - q) mod 2^16 in [0, 65535]); table entries nothing wrote read as 0 mod 2^16
+//   match at p    = p >= the end of the chunk's previous match, d != 0, d <= p, the 4 bytes at p and p - d equal,
+//                   p + 12 <= n (the last match starts 12 bytes before the end) and p + 4 <= the chunk's end
+//   match length  = the longest run of equal bytes at p and p - d that ends by min(chunk end, n - 5)
+// Greedy: the first match in a chunk is taken, the parse resumes at its end.  The table of a chunk is seeded with the
+// positions from max(0, c0 - 65535) so that matches reach back into earlier chunks; matches end at the chunk's end, so
+// chunks parse independently.  A literal run belongs to the chunk holding the match that ends it (or to the segment's
+// last chunk), so a run may span many chunks.  The parse runs W positions at a time: W lanes of a warp on the device
+// (W = 32), any W on the host (tests/emul), with the same result, since table updates in a batch are resolved in
+// position order.
+#define LC_LZ4_CHUNK 65536u
+#define LC_LZ4_HASH_LOG 12
+#define LC_LZ4_SEQ_CAP (LC_LZ4_CHUNK / 4) // sequences per chunk: matches are >= 4 bytes and end inside the chunk
+#define LC_LZ4_MAX_INPUT 0x7E000000u      // LZ4_MAX_INPUT_SIZE
+#define LC_LZ4_NOHASH 0xFFFFFFFFu
+
+struct LcLz4Warp { // per-warp scratch (shared memory on the device)
+    uint16_t tbl[1u << LC_LZ4_HASH_LOG];
+    uint32_t h[32]; // the batch's hashes (LC_LZ4_NOHASH = no position)
+    uint32_t d[32]; // candidate distance of each position
+    uint32_t v[32]; // per-lane predicate of a ballot
+};
+
+struct LcLz4Seq { // one match of a chunk: a = (p - c0) | d << 16, b = length
+    uint32_t a, b;
+};
+
+struct LcLz4Chunk { // parse pass result of one chunk
+    uint32_t nseq;
+    uint32_t isize;    // encoded bytes of its sequences, less the first one's token, literal-length bytes and literals
+    uint32_t first;    // position of the first match
+    uint32_t last_end; // end of the last match
+};
+
+LC_HD uint32_t lc_lz4_ext(uint32_t len) { return len >= 15 ? (len - 15) / 255 + 1 : 0u; }
+LC_HD uint32_t lc_lz4_rd32(const uint8_t* p) {
+    return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
+}
+LC_HD uint32_t lc_lz4_hash(uint32_t v) { return (v * 2654435761u) >> (32 - LC_LZ4_HASH_LOG); }
+LC_HD uint32_t lc_lz4_bound(uint32_t n) { return n + n / 255 + 16; } // LZ4_compressBound
+LC_HD uint32_t lc_lz4_nchunks(uint32_t n) { return n ? (n + LC_LZ4_CHUNK - 1) / LC_LZ4_CHUNK : 1u; }
+
+LC_HD uint32_t lc_lo_bit(uint32_t m) { // m != 0
+#if defined(__CUDA_ARCH__)
+    return __ffs(m) - 1;
+#else
+    return __builtin_ctz(m);
+#endif
+}
+LC_HD uint32_t lc_hi_bit(uint32_t m) { // m != 0
+#if defined(__CUDA_ARCH__)
+    return 31 - __clz(m);
+#else
+    return 31 - __builtin_clz(m);
+#endif
+}
+
+// The lanes of a batch: on the device each lane runs the body once for itself and the warp synchronises between
+// phases; the host runs the body for each of the W lanes in turn, which is a valid interleaving of the same phases.
+#if defined(__CUDA_ARCH__)
+#define LC_LANES(l) for (uint32_t l = lane, l##_once = 1; l##_once; l##_once = 0)
+#define LC_WARP_SYNC() __syncwarp()
+#else
+#define LC_LANES(l) for (uint32_t l = 0; l < W; ++l)
+#define LC_WARP_SYNC() ((void)0)
+#endif
+
+// bit l = v[l] != 0 for the W lanes (all lanes call it)
+LC_HD uint32_t lc_lz4_ballot(const uint32_t* v, uint32_t lane, uint32_t W) {
+#if defined(__CUDA_ARCH__)
+    (void)W;
+    return __ballot_sync(0xFFFFFFFFu, v[lane] != 0);
+#else
+    (void)lane;
+    uint32_t m = 0;
+    for (uint32_t j = 0; j < W; ++j)
+        m |= (v[j] != 0) << j;
+    return m;
+#endif
+}
+
+// bit j = lane j of the batch has lane l's hash (all lanes call it, each with l = its lane)
+LC_HD uint32_t lc_lz4_peers(const uint32_t* h, uint32_t l, uint32_t W) {
+#if defined(__CUDA_ARCH__)
+    (void)W;
+    return __match_any_sync(0xFFFFFFFFu, h[l]);
+#else
+    uint32_t m = 0;
+    for (uint32_t j = 0; j < W; ++j)
+        m |= (h[j] == h[l]) << j;
+    return m;
+#endif
+}
+
+// Parse pass of chunk [c0, c1) of the segment s[0, n): its matches go to seq[0, nseq), the summary to *info.
+LC_HD void lc_lz4_parse_chunk(const uint8_t* s, uint32_t n, uint32_t c0, uint32_t c1, LcLz4Warp& w, LcLz4Seq* seq,
+                              LcLz4Chunk* info, uint32_t lane, uint32_t W) {
+    LC_LANES(l) {
+        for (uint32_t i = l; i < (1u << LC_LZ4_HASH_LOG); i += W)
+            w.tbl[i] = 0;
+    }
+    LC_WARP_SYNC();
+    const uint32_t full = W == 32 ? 0xFFFFFFFFu : (1u << W) - 1u;
+    const uint32_t seed = c0 > 65535u ? c0 - 65535u : 0u;
+    const uint32_t hend = n >= 4 && c1 > n - 4 ? n - 3 : (n >= 4 ? c1 : 0u); // positions with 4 bytes, < c1
+    const uint32_t mend = n >= 12 ? n - 11 : 0u;                              // match starts: p + 12 <= n
+    const uint32_t lim = n >= 5 && c1 > n - 5 ? n - 5 : c1;                   // match ends
+    uint32_t cur = c0, nseq = 0, isize = 0, first = 0, last_end = 0;
+    for (int64_t b = (int64_t)c0 - (int64_t)((c0 - seed + W - 1) / W * W); b < (int64_t)hend; b += W) {
+        LC_LANES(l) {
+            const int64_t p = b + l;
+            w.h[l] = p >= (int64_t)seed && p < (int64_t)hend ? lc_lz4_hash(lc_lz4_rd32(s + p)) : LC_LZ4_NOHASH;
+        }
+        LC_WARP_SYNC();
+        // candidates: the latest earlier lane of the batch with the same hash, else the table
+        LC_LANES(l) {
+            const uint32_t pr = lc_lz4_peers(w.h, l, W);
+            const uint32_t below = pr & ((1u << l) - 1u);
+            const uint32_t p = (uint32_t)(b + l);
+            w.d[l] = w.h[l] == LC_LZ4_NOHASH ? 0u
+                     : below                 ? l - lc_hi_bit(below)
+                                             : (uint32_t)(uint16_t)(p - w.tbl[w.h[l]]);
+        }
+        LC_WARP_SYNC();
+        // the table keeps the last lane of each hash
+        LC_LANES(l) {
+            const uint32_t pr = lc_lz4_peers(w.h, l, W);
+            if (w.h[l] != LC_LZ4_NOHASH && !((pr >> l) >> 1))
+                w.tbl[w.h[l]] = (uint16_t)(b + l);
+        }
+        LC_WARP_SYNC();
+        if (b + W <= (int64_t)cur)
+            continue;
+        LC_LANES(l) {
+            const int64_t p = b + l;
+            const uint32_t d = w.d[l];
+            w.v[l] = p >= (int64_t)cur && p < (int64_t)mend && p + 4 <= (int64_t)c1 && w.h[l] != LC_LZ4_NOHASH && d &&
+                     d <= p && lc_lz4_rd32(s + p) == lc_lz4_rd32(s + p - d);
+        }
+        uint32_t m = lc_lz4_ballot(w.v, lane, W);
+        LC_WARP_SYNC();
+        while (m) {
+            const uint32_t j = lc_lo_bit(m);
+            const uint32_t p = (uint32_t)(b + j), d = w.d[j];
+            uint32_t len = 4;
+            for (;;) { // extend W bytes at a time
+                LC_LANES(l) {
+                    const uint32_t x = p + len + l;
+                    w.v[l] = x < lim && s[x] == s[x - d];
+                }
+                const uint32_t eq = lc_lz4_ballot(w.v, lane, W);
+                LC_WARP_SYNC();
+                const uint32_t run = eq == full ? W : lc_lo_bit(~eq);
+                len += run;
+                if (run < W)
+                    break;
+            }
+            if (lane == 0)
+                seq[nseq] = LcLz4Seq{(p - c0) | (d << 16), len};
+            isize += (nseq ? 1 + lc_lz4_ext(p - last_end) + (p - last_end) : 0u) + 2 + lc_lz4_ext(len - 4);
+            if (!nseq)
+                first = p;
+            ++nseq;
+            last_end = cur = p + len;
+            m = (int64_t)cur >= b + W ? 0u : m & (full << (uint32_t)(cur - b));
+        }
+    }
+    if (lane == 0)
+        *info = LcLz4Chunk{nseq, isize, first, last_end};
+}
+
+// Size pass of one segment of n bytes and nch chunks: the block bytes of each chunk and the literal anchor it starts
+// from (the end of the latest match in an earlier chunk).  The last chunk ends the block with a literals-only sequence.
+LC_HD void lc_lz4_seg_sizes(uint32_t n, uint32_t nch, const LcLz4Chunk* info, uint32_t* csize, uint32_t* anchor) {
+    uint32_t a = 0;
+    for (uint32_t k = 0; k < nch; ++k) {
+        anchor[k] = a;
+        uint32_t sz = 0;
+        if (info[k].nseq) {
+            const uint32_t l0 = info[k].first - a;
+            sz = info[k].isize + 1 + lc_lz4_ext(l0) + l0;
+            a = info[k].last_end;
+        }
+        if (k + 1 == nch)
+            sz += 1 + lc_lz4_ext(n - a) + (n - a);
+        csize[k] = sz;
+    }
+}
+
+// a length's extension bytes (len >= 15) at o[0, lc_lz4_ext(len)), lanes share them
+LC_HD void lc_lz4_put_ext(uint8_t* o, uint32_t len, uint32_t lane, uint32_t W) {
+    const uint32_t nb = lc_lz4_ext(len);
+    LC_LANES(l) {
+        for (uint32_t j = l; j < nb; j += W)
+            o[j] = j + 1 < nb ? 255 : (uint8_t)((len - 15) % 255);
+    }
+}
+
+// one sequence at o: lit literals from s + a, then (mlen != 0) a match of mlen bytes at distance d.  Returns its bytes.
+LC_HD uint32_t lc_lz4_put_seq(const uint8_t* s, uint32_t a, uint32_t lit, uint32_t d, uint32_t mlen, uint8_t* o,
+                              uint32_t lane, uint32_t W) {
+    const uint32_t ml = mlen ? mlen - 4 : 0u;
+    if (lane == 0)
+        o[0] = (uint8_t)(((lit < 15 ? lit : 15) << 4) | (ml < 15 ? ml : 15));
+    uint32_t q = 1;
+    lc_lz4_put_ext(o + q, lit, lane, W);
+    q += lc_lz4_ext(lit);
+    LC_LANES(l) {
+        for (uint32_t j = l; j < lit; j += W)
+            o[q + j] = s[a + j];
+    }
+    q += lit;
+    if (!mlen)
+        return q;
+    if (lane == 0) {
+        o[q] = (uint8_t)d;
+        o[q + 1] = (uint8_t)(d >> 8);
+    }
+    q += 2;
+    lc_lz4_put_ext(o + q, ml, lane, W);
+    return q + lc_lz4_ext(ml);
+}
+
+// Emit pass of chunk [c0, ..) of the segment s[0, n): its sequences (from its anchor) and, for the segment's last
+// chunk, the closing literals, at o.
+LC_HD void lc_lz4_emit_chunk(const uint8_t* s, uint32_t n, uint32_t c0, const LcLz4Seq* seq, uint32_t nseq,
+                             uint32_t anchor, bool last, uint8_t* o, uint32_t lane, uint32_t W) {
+    uint32_t a = anchor;
+    for (uint32_t i = 0; i < nseq; ++i) {
+        const LcLz4Seq q = seq[i];
+        const uint32_t p = c0 + (q.a & 0xFFFFu);
+        o += lc_lz4_put_seq(s, a, p - a, q.a >> 16, q.b, o, lane, W);
+        a = p + q.b;
+    }
+    if (last)
+        lc_lz4_put_seq(s, a, n - a, 0, 0, o, lane, W);
+}

@@ -3724,4 +3724,121 @@ void launch_span_sls_emit(const LcSpanSlsCfg& c, const uint64_t* d_rec_off, uint
         span_sls_emit_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(c, d_rec_off, n, total, d_out);
 }
 
+// ---- f4, LZ4: one block per segment (lc_exec.cuh: lc_lz4_parse_chunk, lc_lz4_seg_sizes, lc_lz4_emit_chunk).  The
+// parse and emit passes run one warp per chunk of LC_LZ4_CHUNK bytes, each warp with its own hash table in shared
+// memory; the size pass one thread per segment over that segment's chunk summaries.
+constexpr int kLz4Warps = 4; // warps per block of the parse and emit kernels
+
+__global__ void __launch_bounds__(256)
+    lz4_chunks_kernel(const uint32_t* __restrict__ seg_len, uint64_t nseg, uint32_t* __restrict__ nch,
+                      uint32_t* too_large) {
+    const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= nseg)
+        return;
+    const uint32_t n = seg_len[s];
+    if (n > LC_LZ4_MAX_INPUT)
+        atomicOr(too_large, 1u);
+    nch[s] = lc_lz4_nchunks(n > LC_LZ4_MAX_INPUT ? 0u : n);
+}
+
+// chunk k of [k0, k1): its segment, its range [c0, c1) and the segment's bytes
+struct Lz4ChunkRef {
+    const uint8_t* s;
+    uint32_t n, c0, c1;
+    bool last;
+};
+__device__ __forceinline__ Lz4ChunkRef lz4_chunk(const uint8_t* in, const uint64_t* seg_off, const uint32_t* seg_len,
+                                                 const uint64_t* first, uint64_t nseg, uint64_t nchunks, uint64_t k) {
+    const uint64_t g = lc_span_sls_find(first, nseg, k);
+    const uint64_t next = g + 1 < nseg ? first[g + 1] : nchunks;
+    Lz4ChunkRef r;
+    r.s = in + seg_off[g];
+    r.n = seg_len[g];
+    r.c0 = (uint32_t)(k - first[g]) * LC_LZ4_CHUNK;
+    r.c1 = r.n - r.c0 < LC_LZ4_CHUNK ? r.n : r.c0 + LC_LZ4_CHUNK;
+    r.last = k + 1 == next;
+    return r;
+}
+
+__global__ void __launch_bounds__(32 * kLz4Warps)
+    lz4_parse_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ seg_off,
+                     const uint32_t* __restrict__ seg_len, const uint64_t* __restrict__ first, uint64_t nseg,
+                     uint64_t nchunks, uint64_t k0, uint64_t k1, LcLz4Seq* __restrict__ seq,
+                     LcLz4Chunk* __restrict__ info) {
+    __shared__ LcLz4Warp s_w[kLz4Warps];
+    const uint32_t wid = threadIdx.x >> 5;
+    const uint64_t k = k0 + (uint64_t)blockIdx.x * kLz4Warps + wid;
+    if (k >= k1)
+        return;
+    const Lz4ChunkRef r = lz4_chunk(in, seg_off, seg_len, first, nseg, nchunks, k);
+    lc_lz4_parse_chunk(r.s, r.n, r.c0, r.c1, s_w[wid], seq + k * LC_LZ4_SEQ_CAP, info + k, threadIdx.x & 31, 32);
+}
+
+__global__ void __launch_bounds__(256)
+    lz4_sizes_kernel(const uint32_t* __restrict__ seg_len, const uint64_t* __restrict__ first, uint64_t nseg,
+                     uint64_t nchunks, const LcLz4Chunk* __restrict__ info, uint32_t* __restrict__ csize,
+                     uint32_t* __restrict__ anchor) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= nseg)
+        return;
+    const uint64_t k = first[g], next = g + 1 < nseg ? first[g + 1] : nchunks;
+    lc_lz4_seg_sizes(seg_len[g], (uint32_t)(next - k), info + k, csize + k, anchor + k);
+}
+
+__global__ void __launch_bounds__(256)
+    lz4_blocks_kernel(const uint64_t* __restrict__ first, const uint64_t* __restrict__ choff,
+                      const uint64_t* __restrict__ total, uint64_t nseg, uint64_t* __restrict__ blk_off,
+                      uint32_t* __restrict__ blk_len) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= nseg)
+        return;
+    const uint64_t a = choff[first[g]], b = g + 1 < nseg ? choff[first[g + 1]] : *total;
+    blk_off[g] = a;
+    blk_len[g] = (uint32_t)(b - a);
+}
+
+__global__ void __launch_bounds__(32 * kLz4Warps, 1)
+    lz4_emit_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ seg_off,
+                    const uint32_t* __restrict__ seg_len, const uint64_t* __restrict__ first, uint64_t nseg,
+                    uint64_t nchunks, const LcLz4Seq* __restrict__ seq, const LcLz4Chunk* __restrict__ info,
+                    const uint32_t* __restrict__ anchor, const uint64_t* __restrict__ choff, uint8_t* __restrict__ out) {
+    const uint64_t k = (uint64_t)blockIdx.x * kLz4Warps + (threadIdx.x >> 5);
+    if (k >= nchunks)
+        return;
+    const Lz4ChunkRef r = lz4_chunk(in, seg_off, seg_len, first, nseg, nchunks, k);
+    lc_lz4_emit_chunk(r.s, r.n, r.c0, seq + k * LC_LZ4_SEQ_CAP, info[k].nseq, anchor[k], r.last, out + choff[k],
+                      threadIdx.x & 31, 32);
+}
+
+void launch_lz4_chunks(const uint32_t* d_seg_len, uint64_t nseg, uint32_t* d_nch, uint32_t* d_too_large,
+                       cudaStream_t st) {
+    if (nseg)
+        lz4_chunks_kernel<<<(unsigned)((nseg + 255) / 256), 256, 0, st>>>(d_seg_len, nseg, d_nch, d_too_large);
+}
+
+void launch_lz4_parse(const Lz4Segs& g, uint64_t k0, uint64_t k1, LcLz4Seq* d_seq, LcLz4Chunk* d_info,
+                      cudaStream_t st) {
+    if (k1 > k0)
+        lz4_parse_kernel<<<(unsigned)((k1 - k0 + kLz4Warps - 1) / kLz4Warps), 32 * kLz4Warps, 0, st>>>(
+            g.in, g.seg_off, g.seg_len, g.first, g.nseg, g.nchunks, k0, k1, d_seq, d_info);
+}
+
+void launch_lz4_sizes(const Lz4Segs& g, const LcLz4Chunk* d_info, uint32_t* d_csize, uint32_t* d_anchor,
+                      cudaStream_t st) {
+    if (g.nseg)
+        lz4_sizes_kernel<<<(unsigned)((g.nseg + 255) / 256), 256, 0, st>>>(g.seg_len, g.first, g.nseg, g.nchunks,
+                                                                            d_info, d_csize, d_anchor);
+}
+
+void launch_lz4_emit(const Lz4Segs& g, const LcLz4Seq* d_seq, const LcLz4Chunk* d_info, const uint32_t* d_anchor,
+                     const uint64_t* d_choff, const uint64_t* d_total, uint8_t* d_out, uint64_t* d_blk_off,
+                     uint32_t* d_blk_len, cudaStream_t st) {
+    if (!g.nseg)
+        return;
+    lz4_blocks_kernel<<<(unsigned)((g.nseg + 255) / 256), 256, 0, st>>>(g.first, d_choff, d_total, g.nseg, d_blk_off,
+                                                                         d_blk_len);
+    lz4_emit_kernel<<<(unsigned)((g.nchunks + kLz4Warps - 1) / kLz4Warps), 32 * kLz4Warps, 0, st>>>(
+        g.in, g.seg_off, g.seg_len, g.first, g.nseg, g.nchunks, d_seq, d_info, d_anchor, d_choff, d_out);
+}
+
 } // namespace lck

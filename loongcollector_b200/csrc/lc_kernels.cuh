@@ -7,6 +7,8 @@
 struct LcDelimSlsCfg; // lc_exec.cuh
 struct LcRegexSlsCfg;
 struct LcSpanSlsCfg;
+struct LcLz4Seq;
+struct LcLz4Chunk;
 
 namespace lck {
 
@@ -243,5 +245,28 @@ constexpr uint32_t kSpanTile = 1024;
 void launch_span_sls_sizes(const LcSpanSlsCfg& c, uint64_t n, uint32_t* d_rec_size, cudaStream_t st);
 void launch_span_sls_emit(const LcSpanSlsCfg& c, const uint64_t* d_rec_off, uint64_t n, uint64_t total, uint8_t* d_out,
                           cudaStream_t st);
+
+// f4, LZ4: one LZ4 block per segment g = in[seg_off[g], + seg_len[g]) (lc_exec.cuh).  Chunk k of LC_LZ4_CHUNK bytes
+// belongs to the segment g with first[g] <= k < first[g + 1] (first = exclusive sum of lc_lz4_nchunks per segment).
+// launch_lz4_chunks: nch[g] = chunks of segment g; *d_too_large |= 1 for a segment over LC_LZ4_MAX_INPUT.
+// launch_lz4_parse: the matches of chunks [k0, k1) (seq: LC_LZ4_SEQ_CAP entries per chunk).
+// launch_lz4_sizes: block bytes per chunk and its literal anchor.  After an exclusive sum of d_csize (d_choff,
+// *d_total), launch_lz4_emit writes the blocks and the per-segment table (blk_off, blk_len).
+struct Lz4Segs {
+    const uint8_t* in;
+    const uint64_t* seg_off;
+    const uint32_t* seg_len;
+    const uint64_t* first;
+    uint64_t nseg, nchunks;
+};
+void launch_lz4_chunks(const uint32_t* d_seg_len, uint64_t nseg, uint32_t* d_nch, uint32_t* d_too_large,
+                       cudaStream_t st);
+void launch_lz4_parse(const Lz4Segs& g, uint64_t k0, uint64_t k1, LcLz4Seq* d_seq, LcLz4Chunk* d_info,
+                      cudaStream_t st);
+void launch_lz4_sizes(const Lz4Segs& g, const LcLz4Chunk* d_info, uint32_t* d_csize, uint32_t* d_anchor,
+                      cudaStream_t st);
+void launch_lz4_emit(const Lz4Segs& g, const LcLz4Seq* d_seq, const LcLz4Chunk* d_info, const uint32_t* d_anchor,
+                     const uint64_t* d_choff, const uint64_t* d_total, uint8_t* d_out, uint64_t* d_blk_off,
+                     uint32_t* d_blk_len, cudaStream_t st);
 
 } // namespace lck

@@ -1874,6 +1874,48 @@ bool FinishSls(const SLSEventGroupSerializer& ser, uint64_t n, uint64_t discarde
     return true;
 }
 
+// SerializeSls's bytes as one LZ4 block (the path for groups the one-pass device call does not take)
+bool CompressSls(bool ok, std::string& raw, std::string& block, uint64_t& rawSize, std::string& err) {
+    if (!ok)
+        return false;
+    rawSize = raw.size();
+    LZ4Compressor c;
+    return c.Compress(raw, block, err);
+}
+
+// The fused device pass: call(out, cap, &blockLen, &raw) parses, serialises and compresses records ‖ tail, sized by
+// `estimate` first and by the exact block size when that was short (unless the group is over the size limit anyway).
+// Then SLSEventGroupSerializer::Serialize's checks, in its order, on the raw size.
+template <class Call>
+bool RunSlsLz4DevicePass(Call call, size_t estimate, const SLSEventGroupSerializer& ser, uint64_t n,
+                         const uint64_t& discarded, size_t tailSize, std::string& block, uint64_t& rawSize,
+                         std::string& err, const char* what) {
+    uint64_t blen = 0, raw = 0;
+    block.assign(estimate + estimate / 255 + 16, '\0');
+    int rc = call(reinterpret_cast<uint8_t*>(&block[0]), (uint64_t)block.size(), &blen, &raw);
+    if (rc == LC_ERR_CAPACITY && (int64_t)raw <= (int64_t)ser.mMaxSendLogGroupSize) {
+        block.resize(blen);
+        rc = call(reinterpret_cast<uint8_t*>(&block[0]), (uint64_t)block.size(), &blen, &raw);
+    }
+    if (rc != LC_ERR_CAPACITY)
+        Check(rc, what);
+    if (n == discarded) {
+        err = "empty event group";
+        return false;
+    }
+    if (raw == tailSize) {
+        err = "all empty logs";
+        return false;
+    }
+    if ((int64_t)raw > (int64_t)ser.mMaxSendLogGroupSize) {
+        err = SizeLimitError(raw, ser.mMaxSendLogGroupSize);
+        return false;
+    }
+    block.resize(blen);
+    rawSize = raw;
+    return true;
+}
+
 // The device path of the splitters' SerializeSls on a flat group: every source event's value is split and serialised
 // by `call(val, key, okey, pos, time, ns, out, cap, &need, &nevents, ctr)` (lc_split_sls / lc_multiline_split_sls) and
 // the records are concatenated in event order; counters[3] += the ctr of each source event's last call.  The records
@@ -2076,11 +2118,26 @@ bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& gr
 
 bool ProcessorParseDelimiterNative::SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out,
                                                  std::string& err) {
+    return SerializeSlsImpl(group, enableNs, out, nullptr, err);
+}
+
+bool ProcessorParseDelimiterNative::SerializeSlsLz4(PipelineEventGroup& group, bool enableNs, std::string& block,
+                                                    uint64_t& rawSize, std::string& err) {
+    return SerializeSlsImpl(group, enableNs, block, &rawSize, err);
+}
+
+// out = the wire bytes (rawSize null) or their LZ4 block (rawSize = their size)
+bool ProcessorParseDelimiterNative::SerializeSlsImpl(PipelineEventGroup& group, bool enableNs, std::string& out,
+                                                     uint64_t* rawSize, std::string& err) {
     SLSEventGroupSerializer ser;
     ser.mEnableTimestampNanosecond = enableNs;
     if (!mDeviceSls || !IsFlatSlsGroup(group, mSourceKey)) {
         Process(group);
-        return ser.Serialize(group, out, err);
+        if (!rawSize)
+            return ser.Serialize(group, out, err);
+        std::string raw;
+        const bool ok = ser.Serialize(group, raw, err);
+        return CompressSls(ok, raw, out, *rawSize, err);
     }
     // every event is SourceKey -> line: parse and serialise in one device pass, only the wire bytes come back
     const size_t n = group.GetEvents().size();
@@ -2099,33 +2156,58 @@ bool ProcessorParseDelimiterNative::SerializeSls(PipelineEventGroup& group, bool
     std::string res;
     uint64_t need = 0, ctr[4] = {0, 0, 0, 0};
     const std::string tail = SlsGroupTail(group);
-    RunSlsDevicePass(
-        [&](uint8_t* o, uint64_t cap, uint64_t* len) {
-            return lc_delim_parse_sls(
-                Engine(), batch.base, batch.baseLen, batch.off.data(), batch.len.data(), n, evTime.data(), evNs.data(),
-                reinterpret_cast<const uint8_t*>(mSeparator.data()), (uint32_t)mSeparator.size(), (uint8_t)mQuote,
-                mOverflowedFieldsTreatment == OverflowedFieldsTreatment::EXTEND, mExtractingPartialFields,
-                mAllowingShortenedFields, (uint32_t)mKeys.size() + 16, kp.data(), kl.data(), (uint32_t)mKeys.size(),
-                mSourceKey.data(), (uint32_t)mSourceKey.size(), renamed.data(), (uint32_t)renamed.size(),
-                mCommonParserOptions.mKeepingSourceWhenParseFail, mCommonParserOptions.mKeepingSourceWhenParseSucceed,
-                mCommonParserOptions.mCopingRawLog, o, cap, len, ctr);
-        },
-        (size_t)(2 * batch.baseLen + n * (64 + keyBytes + renamed.size()) + 64), tail.size(), ser.mMaxSendLogGroupSize,
-        res, need, "lc_delim_parse_sls");
+    const size_t estimate = (size_t)(2 * batch.baseLen + n * (64 + keyBytes + renamed.size()) + 64);
+    // the arguments both device calls share, up to copy_raw
+    auto args = [&](auto fn, auto... rest) {
+        return fn(Engine(), batch.base, batch.baseLen, batch.off.data(), batch.len.data(), n, evTime.data(),
+                  evNs.data(), reinterpret_cast<const uint8_t*>(mSeparator.data()), (uint32_t)mSeparator.size(),
+                  (uint8_t)mQuote, mOverflowedFieldsTreatment == OverflowedFieldsTreatment::EXTEND,
+                  mExtractingPartialFields, mAllowingShortenedFields, (uint32_t)mKeys.size() + 16, kp.data(), kl.data(),
+                  (uint32_t)mKeys.size(), mSourceKey.data(), (uint32_t)mSourceKey.size(), renamed.data(),
+                  (uint32_t)renamed.size(), mCommonParserOptions.mKeepingSourceWhenParseFail,
+                  mCommonParserOptions.mKeepingSourceWhenParseSucceed, mCommonParserOptions.mCopingRawLog, rest...);
+    };
+    bool ok;
+    if (rawSize) {
+        ok = RunSlsLz4DevicePass(
+            [&](uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw) {
+                return args(lc_delim_parse_sls_lz4, reinterpret_cast<const uint8_t*>(tail.data()),
+                            (uint64_t)tail.size(), o, cap, len, raw, ctr);
+            },
+            estimate + tail.size(), ser, n, ctr[2], tail.size(), out, *rawSize, err, "lc_delim_parse_sls_lz4");
+    } else {
+        RunSlsDevicePass([&](uint8_t* o, uint64_t cap, uint64_t* len) { return args(lc_delim_parse_sls, o, cap, len, ctr); },
+                         estimate, tail.size(), ser.mMaxSendLogGroupSize, res, need, "lc_delim_parse_sls");
+    }
     // the counters Process would have moved (a blank value counts as out_failed, :220-242)
     mOutSuccessfulEventsTotal.Add(ctr[0]);
     mOutFailedEventsTotal.Add(ctr[1] + ctr[3]);
     mDiscardedEventsTotal.Add(ctr[2]);
-    return FinishSls(ser, n, ctr[2], need, res, tail, out, err);
+    return rawSize ? ok : FinishSls(ser, n, ctr[2], need, res, tail, out, err);
 }
 
 bool ProcessorParseRegexNative::SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out,
                                              std::string& err) {
+    return SerializeSlsImpl(group, enableNs, out, nullptr, err);
+}
+
+bool ProcessorParseRegexNative::SerializeSlsLz4(PipelineEventGroup& group, bool enableNs, std::string& block,
+                                                uint64_t& rawSize, std::string& err) {
+    return SerializeSlsImpl(group, enableNs, block, &rawSize, err);
+}
+
+// out = the wire bytes (rawSize null) or their LZ4 block (rawSize = their size)
+bool ProcessorParseRegexNative::SerializeSlsImpl(PipelineEventGroup& group, bool enableNs, std::string& out,
+                                                 uint64_t* rawSize, std::string& err) {
     SLSEventGroupSerializer ser;
     ser.mEnableTimestampNanosecond = enableNs;
     if (!IsFlatSlsGroup(group, mSourceKey)) {
         Process(group);
-        return ser.Serialize(group, out, err);
+        if (!rawSize)
+            return ser.Serialize(group, out, err);
+        std::string raw;
+        const bool ok = ser.Serialize(group, raw, err);
+        return CompressSls(ok, raw, out, *rawSize, err);
     }
     // every event is SourceKey -> line: parse and serialise in one device pass, only the wire bytes come back
     const size_t n = group.GetEvents().size();
@@ -2144,22 +2226,72 @@ bool ProcessorParseRegexNative::SerializeSls(PipelineEventGroup& group, bool ena
     std::string res;
     uint64_t need = 0, ctr[3] = {0, 0, 0};
     const std::string tail = SlsGroupTail(group);
-    RunSlsDevicePass(
-        [&](uint8_t* o, uint64_t cap, uint64_t* len) {
-            return lc_regex_parse_sls(
-                Engine(), mIsWholeLineMode ? nullptr : mReg.get(), batch.base, batch.baseLen, batch.off.data(),
-                batch.len.data(), n, evTime.data(), evNs.data(), kp.data(), kl.data(), (uint32_t)mKeys.size(),
-                mSourceKey.data(), (uint32_t)mSourceKey.size(), renamed.data(), (uint32_t)renamed.size(),
-                mCommonParserOptions.mKeepingSourceWhenParseFail, mCommonParserOptions.mKeepingSourceWhenParseSucceed,
-                mCommonParserOptions.mCopingRawLog, mIsWholeLineMode, o, cap, len, ctr);
-        },
-        (size_t)(2 * batch.baseLen + n * (64 + keyBytes + renamed.size()) + 64), tail.size(), ser.mMaxSendLogGroupSize,
-        res, need, "lc_regex_parse_sls");
+    const size_t estimate = (size_t)(2 * batch.baseLen + n * (64 + keyBytes + renamed.size()) + 64);
+    // the arguments both device calls share, up to whole_line
+    auto args = [&](auto fn, auto... rest) {
+        return fn(Engine(), mIsWholeLineMode ? nullptr : mReg.get(), batch.base, batch.baseLen, batch.off.data(),
+                  batch.len.data(), n, evTime.data(), evNs.data(), kp.data(), kl.data(), (uint32_t)mKeys.size(),
+                  mSourceKey.data(), (uint32_t)mSourceKey.size(), renamed.data(), (uint32_t)renamed.size(),
+                  mCommonParserOptions.mKeepingSourceWhenParseFail,
+                  mCommonParserOptions.mKeepingSourceWhenParseSucceed, mCommonParserOptions.mCopingRawLog,
+                  mIsWholeLineMode, rest...);
+    };
+    bool ok;
+    if (rawSize) {
+        ok = RunSlsLz4DevicePass(
+            [&](uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw) {
+                return args(lc_regex_parse_sls_lz4, reinterpret_cast<const uint8_t*>(tail.data()),
+                            (uint64_t)tail.size(), o, cap, len, raw, ctr);
+            },
+            estimate + tail.size(), ser, n, ctr[2], tail.size(), out, *rawSize, err, "lc_regex_parse_sls_lz4");
+    } else {
+        RunSlsDevicePass([&](uint8_t* o, uint64_t cap, uint64_t* len) { return args(lc_regex_parse_sls, o, cap, len, ctr); },
+                         estimate, tail.size(), ser.mMaxSendLogGroupSize, res, need, "lc_regex_parse_sls");
+    }
     // the counters Process would have moved (LC_REGEX_KEYS_MISMATCH is not out_failed, :227-244)
     mOutSuccessfulEventsTotal.Add(ctr[0]);
     mOutFailedEventsTotal.Add(ctr[1]);
     mDiscardedEventsTotal.Add(ctr[2]);
-    return FinishSls(ser, n, ctr[2], need, res, tail, out, err);
+    return rawSize ? ok : FinishSls(ser, n, ctr[2], need, res, tail, out, err);
+}
+
+bool LZ4Compressor::Compress(const std::string& input, std::string& output, std::string& errorMsg) {
+    std::vector<std::string> out;
+    if (!Compress(std::vector<std::string>{input}, out, errorMsg))
+        return false;
+    output.swap(out[0]);
+    return true;
+}
+
+bool LZ4Compressor::Compress(const std::vector<std::string>& inputs, std::vector<std::string>& outputs,
+                             std::string& errorMsg) {
+    std::vector<const uint8_t*> ptr;
+    std::vector<uint32_t> len;
+    uint64_t cap = 0;
+    for (const std::string& in : inputs) {
+        // LZ4_compressBound(n) is 0 for n > LZ4_MAX_INPUT_SIZE (lz4.h)
+        if (in.size() > LC_LZ4_MAX_INPUT) {
+            errorMsg = "input size is incorrect";
+            return false;
+        }
+        ptr.push_back(reinterpret_cast<const uint8_t*>(in.data()));
+        len.push_back((uint32_t)in.size());
+        cap += lc_lz4_bound((uint32_t)in.size());
+    }
+    outputs.clear();
+    if (inputs.empty())
+        return true;
+    std::string all(cap, '\0');
+    std::vector<uint64_t> boff(inputs.size());
+    std::vector<uint32_t> blen(inputs.size());
+    uint64_t total = 0;
+    Check(lc_lz4_compress(Engine(), inputs.size(), ptr.data(), len.data(), reinterpret_cast<uint8_t*>(&all[0]), cap,
+                          boff.data(), blen.data(), &total),
+          "lc_lz4_compress");
+    outputs.reserve(inputs.size());
+    for (size_t k = 0; k < inputs.size(); ++k)
+        outputs.emplace_back(all, boff[k], blen[k]);
+    return true;
 }
 
 Processor* CreateProcessor(const std::string& type) {

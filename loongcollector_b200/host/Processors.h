@@ -177,6 +177,17 @@ public:
     // serialised in one device pass (lc_regex_parse_sls): the capture tables never leave the GPU, no LogEvent is
     // touched and the group's events are left as they were.  Otherwise Process runs.
     bool SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out, std::string& err);
+    // SerializeSls followed by LZ4Compressor::Compress: on success `block` is one LZ4 block that decompresses to exactly
+    // SerializeSls's bytes, and rawSize is their size.  Errors and counters are SerializeSls's.  The one-pass path
+    // compresses on the device (lc_regex_parse_sls_lz4): only the block comes back.
+    bool SerializeSlsLz4(PipelineEventGroup& group, bool enableNs, std::string& block, uint64_t& rawSize,
+                         std::string& err);
+
+private:
+    bool SerializeSlsImpl(PipelineEventGroup& group, bool enableNs, std::string& out, uint64_t* rawSize,
+                          std::string& err);
+
+public:
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
@@ -234,11 +245,16 @@ public:
     // lc_delim_parse_sls accepts, the group is parsed and serialised in one device pass (lc_delim_parse_sls): the
     // delimiter tables never leave the GPU and the group's events are left as they were.  Otherwise Process runs.
     bool SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out, std::string& err);
+    // SerializeSls followed by LZ4Compressor::Compress, as for ProcessorParseRegexNative (lc_delim_parse_sls_lz4).
+    bool SerializeSlsLz4(PipelineEventGroup& group, bool enableNs, std::string& block, uint64_t& rawSize,
+                         std::string& err);
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
+    bool SerializeSlsImpl(PipelineEventGroup& group, bool enableNs, std::string& out, uint64_t* rawSize,
+                          std::string& err);
     bool mSourceKeyOverwritten = false;
     bool mDeviceSls = false; // the configuration passes lc_delim_parse_sls's checks
 };
@@ -323,6 +339,17 @@ public:
     bool mEnableTimestampNanosecond = false;      // GlobalConfig::mEnableTimestampNanosecond
     int32_t mMaxSendLogGroupSize = 10 * 1024 * 1024; // flag max_send_log_group_size (FlusherSLS.cpp:61)
     bool Serialize(PipelineEventGroup& group, std::string& res, std::string& errorMsg) const;
+};
+
+// FlusherSLS's default compressor (core/common/compression/LZ4Compressor.cpp:25-44) on the GPU: one LZ4 block per
+// input (lc_lz4_compress).  The blocks are valid LZ4 blocks of the input, not liblz4's exact bytes.  The batched
+// overload compresses many serialised groups in one device call, as the flusher holds many queue items
+// (FlusherSLS.cpp:1065-1144); a lone small group is faster through liblz4 on the CPU (DESIGN.md §5), so callers with
+// one group at a time should batch them.
+class LZ4Compressor {
+public:
+    bool Compress(const std::string& input, std::string& output, std::string& errorMsg);
+    bool Compress(const std::vector<std::string>& inputs, std::vector<std::string>& outputs, std::string& errorMsg);
 };
 
 // Factory by plugin type name (the names the reference registers, PluginRegistry.cpp:183-200).

@@ -6,6 +6,7 @@
 #include <memory>
 #include <stdexcept>
 #include <string>
+#include <vector>
 
 #include "../../include/lc_b200_host.h"
 #include "PluginBench.h"
@@ -175,6 +176,86 @@ char* lc_host_processor_serialize_sls(lc_host_processor_t* p, const char* group_
     } catch (const std::exception& e) {
         if (fail_out)
             *fail_out = dup(std::string("SerializeSls threw: ") + e.what());
+        return nullptr;
+    }
+}
+
+char* lc_host_processor_serialize_sls_lz4(lc_host_processor_t* p, const char* group_json, int enable_ns,
+                                          unsigned long long* len_out, unsigned long long* raw_len_out, char** err_out,
+                                          char** fail_out) {
+    if (err_out)
+        *err_out = nullptr;
+    if (fail_out)
+        *fail_out = nullptr;
+    if (len_out)
+        *len_out = 0;
+    if (raw_len_out)
+        *raw_len_out = 0;
+    try {
+        auto* d = dynamic_cast<ProcessorParseDelimiterNative*>(p->proc.get());
+        auto* r = dynamic_cast<ProcessorParseRegexNative*>(p->proc.get());
+        if (!d && !r)
+            throw std::runtime_error("not a processor_parse_delimiter_native or processor_parse_regex_native");
+        Processor* proc = p->proc.get();
+        PipelineEventGroup group(std::make_shared<SourceBuffer>());
+        if (!group.FromJsonString(group_json ? group_json : "null"))
+            throw std::runtime_error("group JSON does not parse");
+        const uint64_t errs = proc->EngineErrors();
+        std::string block, err;
+        uint64_t raw = 0;
+        const bool ok = d ? d->SerializeSlsLz4(group, enable_ns != 0, block, raw, err)
+                          : r->SerializeSlsLz4(group, enable_ns != 0, block, raw, err);
+        if (proc->EngineErrors() != errs)
+            throw std::runtime_error("engine error inside Process: " + proc->LastError());
+        if (!ok) {
+            if (err_out)
+                *err_out = dup(err);
+            return nullptr;
+        }
+        char* out = (char*)malloc(block.size() + 1);
+        memcpy(out, block.data(), block.size());
+        if (len_out)
+            *len_out = block.size();
+        if (raw_len_out)
+            *raw_len_out = raw;
+        return out;
+    } catch (const std::exception& e) {
+        if (fail_out)
+            *fail_out = dup(std::string("SerializeSlsLz4 threw: ") + e.what());
+        return nullptr;
+    }
+}
+
+char* lc_host_lz4_compress(const char* const* data, const unsigned long long* len, unsigned long long n,
+                           unsigned long long* len_out, unsigned long long* blk_len, char** err_out) {
+    if (err_out)
+        *err_out = nullptr;
+    if (len_out)
+        *len_out = 0;
+    try {
+        std::vector<std::string> in, out;
+        for (unsigned long long k = 0; k < n; ++k)
+            in.emplace_back(data[k], len[k]);
+        std::string err;
+        LZ4Compressor c;
+        if (!c.Compress(in, out, err)) {
+            if (err_out)
+                *err_out = dup(err);
+            return nullptr;
+        }
+        std::string all;
+        for (unsigned long long k = 0; k < n; ++k) {
+            blk_len[k] = out[k].size();
+            all += out[k];
+        }
+        char* res = (char*)malloc(all.size() + 1);
+        memcpy(res, all.data(), all.size());
+        if (len_out)
+            *len_out = all.size();
+        return res;
+    } catch (const std::exception& e) {
+        if (err_out)
+            *err_out = dup(std::string("LZ4Compressor::Compress threw: ") + e.what());
         return nullptr;
     }
 }
