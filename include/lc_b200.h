@@ -407,6 +407,93 @@ int lc_delim_parse_sls_lz4(lc_engine_t* e, const uint8_t* base, uint64_t base_le
                            const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
                            uint64_t* raw_len, uint64_t counters[4]);
 
+/* ---- f4: the delimiter -> regex chain (ProcessorParseDelimiterNative::Process, then ProcessorParseRegexNative::Process
+ * whose SourceKey is one of the delimiter's keys -- BASELINE config C4) to the SLS wire format.  Every event is taken
+ * to be flat: a LogEvent whose only content is source_key -> its line.  The chain's configuration is both stages'
+ * arguments: the delimiter's (sep .. copy_raw, as for lc_sls_serialize_delim_dev) and the regex stage's (rkeys ..
+ * rcopy_raw, whole_line, as for lc_sls_serialize_regex_dev; rsource_key = key k of the delimiter).
+ * The regex stage reads key k's value: column k with its doubled quotes collapsed (AddFieldWithUnQuote) when the row
+ * parsed and has the column; the whole line when the line stayed under key k (a short row whose source_key is key k,
+ * a short row with keep_succeed whose renamed_key is key k, a kept failure whose renamed_key or "__raw_log__" is key
+ * k, a blank row whose source_key is key k); otherwise no value (out_key_not_found; the delimiter's record is left as
+ * it is).  With a value, key k's content is deleted in place -- or overwritten in place by the capture of a regex key
+ * equal to k -- and the regex stage's other contents follow the delimiter's (ProcessorParseRegexNative.cpp:132-168).
+ * Refused with LC_ERR_INVALID_ARG, besides each stage's own refusals: an rsource_key that is not one of the
+ * delimiter's keys ("_" in discard mode is none), and a regex key, rrenamed_key or (rkeep_fail + rcopy_raw)
+ * "__raw_log__" equal to a content the delimiter stage may leave besides key k's: another key, source_key,
+ * renamed_key, "__raw_log__", "__column<digits>__" in extend or keep mode; also "_time_" and "_source_" both among
+ * those without rkeep_fail (ShouldEraseEvent's rule would depend on the row).
+ *
+ * lc_delim_regex_tap_dev: the regex stage's event table from the DEVICE tables of one lc_delim_parse_dev call: value
+ * i = d_base[d_val_off[i], + d_val_len[i]); a row without a value gets (its line's offset, 0).  A column with doubled
+ * quotes is copied, collapsed, into d_base's side region [align16(base_len), base_cap), one slot per row in row order,
+ * so captures stay offsets from d_base; *side_len = the bytes the copies take.  If they do not fit, LC_ERR_CAPACITY
+ * and nothing is written (a sizing query); LC_ERR_TOO_LARGE when align16(base_len) + *side_len reaches 4 GiB.
+ * Queued on the engine stream after one synchronise (the side size). */
+int lc_delim_regex_tap_dev(lc_engine_t* e, uint8_t* d_base, uint64_t base_len, uint64_t base_cap,
+                           const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, const uint8_t* d_status,
+                           const uint32_t* d_nfields, const uint32_t* d_f_off, const uint32_t* d_f_len,
+                           const uint32_t* d_f_dq, uint32_t max_fields, const uint8_t* sep, uint32_t sep_len,
+                           uint8_t quote, int extend, int discard, const char* const* keys, const uint32_t* key_lens,
+                           uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                           uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                           const char* const* rkeys, const uint32_t* rkey_lens, uint32_t rnkeys,
+                           const char* rsource_key, uint32_t rsource_key_len, const char* rrenamed_key,
+                           uint32_t rrenamed_key_len, int rkeep_fail, int rkeep_succeed, int rcopy_raw, int whole_line,
+                           uint32_t* d_val_off, uint32_t* d_val_len, uint64_t* side_len /* host */);
+
+/* The `Logs` fields of the events the chain leaves behind, from the delimiter tables, the value table of
+ * lc_delim_regex_tap_dev and the DEVICE tables of lc_regex_parse_dev over it (d_re_status, [n][row_pitch]
+ * d_cap_off / d_cap_len, parsed with rnkeys keys; NULL in whole-line mode).  base_len covers the side copies.
+ * counters[8] (host, may be NULL) = the delimiter's successful, failed, discarded, blank events (as lc_delim_parse_sls)
+ * and the regex stage's out_successful, out_failed (LC_REGEX_NOMATCH), out_key_not_found and discarded events.
+ * d_ev_time_ns may be NULL; LC_SLS_NO_NS per event = no Time_ns.  d_out receives the bytes on the device; *out_len
+ * (host) their count; LC_ERR_CAPACITY if > out_cap (nothing written, *out_len and counters set). */
+int lc_sls_serialize_delim_regex_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t base_len,
+                                     const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n,
+                                     const uint8_t* d_status, const uint32_t* d_nfields, const uint32_t* d_f_off,
+                                     const uint32_t* d_f_len, const uint32_t* d_f_dq, uint32_t max_fields,
+                                     const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard,
+                                     const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                                     const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                                     uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                                     const char* const* rkeys, const uint32_t* rkey_lens, uint32_t rnkeys,
+                                     const char* rsource_key, uint32_t rsource_key_len, const char* rrenamed_key,
+                                     uint32_t rrenamed_key_len, int rkeep_fail, int rkeep_succeed, int rcopy_raw,
+                                     int whole_line, const uint32_t* d_val_off, const uint32_t* d_val_len,
+                                     const uint8_t* d_re_status, const uint32_t* d_cap_off, const uint32_t* d_cap_len,
+                                     uint32_t row_pitch, const uint32_t* d_ev_time, const uint32_t* d_ev_time_ns,
+                                     uint8_t* d_out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[8]);
+
+/* The same with HOST buffers: the arena goes up once, in chunks of whole events; per chunk the delimiter stage
+ * (lc_delim_parse with allow_short, tables max_fields wide), the value tap, the regex stage over the values (re may be
+ * NULL in whole-line mode) and the size pass run on the device, and only the wire bytes (out, in event order) and
+ * counters[8] come back.  The device holds the lines plus at most their total length of side copies, which must stay
+ * below 4 GiB (LC_ERR_TOO_LARGE).  *out_len and counters are set on LC_OK and on LC_ERR_CAPACITY.  The _lz4 variant
+ * puts tail[0, tail_len) behind the records and returns ONE LZ4 block, as lc_delim_parse_sls_lz4 does. */
+int lc_delim_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base, uint64_t base_len,
+                             const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time,
+                             const uint32_t* ev_time_ns, int allow_short, uint32_t max_fields, const uint8_t* sep,
+                             uint32_t sep_len, uint8_t quote, int extend, int discard, const char* const* keys,
+                             const uint32_t* key_lens, uint32_t nkeys, const char* source_key, uint32_t source_key_len,
+                             const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed,
+                             int copy_raw, const char* const* rkeys, const uint32_t* rkey_lens, uint32_t rnkeys,
+                             const char* rsource_key, uint32_t rsource_key_len, const char* rrenamed_key,
+                             uint32_t rrenamed_key_len, int rkeep_fail, int rkeep_succeed, int rcopy_raw,
+                             int whole_line, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[8]);
+int lc_delim_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base, uint64_t base_len,
+                                 const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time,
+                                 const uint32_t* ev_time_ns, int allow_short, uint32_t max_fields, const uint8_t* sep,
+                                 uint32_t sep_len, uint8_t quote, int extend, int discard, const char* const* keys,
+                                 const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+                                 uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+                                 int keep_fail, int keep_succeed, int copy_raw, const char* const* rkeys,
+                                 const uint32_t* rkey_lens, uint32_t rnkeys, const char* rsource_key,
+                                 uint32_t rsource_key_len, const char* rrenamed_key, uint32_t rrenamed_key_len,
+                                 int rkeep_fail, int rkeep_succeed, int rcopy_raw, int whole_line, const uint8_t* tail,
+                                 uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                                 uint64_t* raw_len, uint64_t counters[8]);
+
 /* LZ4 compression of serialised groups (FlusherSLS's default compressor, LZ4Compressor::Compress =
  * LZ4_compress_default): segment g = d_in[d_seg_off[g], + d_seg_len[g]) becomes one LZ4 *block* (not a frame), the
  * blocks packed back to back in d_out: block g = d_out[d_blk_off[g], + d_blk_len[g]).  The bytes are deterministic;

@@ -101,6 +101,15 @@ def lib():
         sls_cfg + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
     L.lc_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp] + sls_cfg + \
         [i32, vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
+    chain_cfg = [vp, u32, u8, i32, i32] + sls_cfg + sls_cfg + [i32]  # sep .. copy_raw, rkeys .. rcopy_raw, whole_line
+    dtab = [vp, vp, u64, vp, vp, vp, vp, vp, u32]  # d_ev_off .. max_fields
+    L.lc_delim_regex_tap_dev.argtypes = [vp, vp, u64, u64] + dtab + chain_cfg + [vp, vp, C.POINTER(u64)]
+    L.lc_sls_serialize_delim_regex_dev.argtypes = [vp, vp, u64] + dtab + chain_cfg + \
+        [vp, vp, vp, vp, vp, u32, vp, vp, vp, u64, C.POINTER(u64), vp]
+    L.lc_delim_regex_parse_sls.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp, i32, u32] + chain_cfg + \
+        [vp, u64, C.POINTER(u64), vp]
+    L.lc_delim_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp, i32, u32] + chain_cfg + \
+        [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
     _LIB = L
     return L
 
@@ -512,6 +521,94 @@ class Engine:
             4, tail, out_cap, 2 * a.size + 64 * n + 64 + len(tail))
 
     @staticmethod
+    def _chain_cfg(delim, regex):
+        """the C arguments of a delimiter -> regex chain.  delim: dict(sep, quote, treatment, keys, source_key,
+        renamed_key=None, keep_fail=False, keep_succeed=False, copy_raw=False); regex: dict(keys, source_key,
+        renamed_key=None, keep_fail=False, keep_succeed=False, copy_raw=False, whole_line=False); keys as bytes."""
+        sp = np.frombuffer(delim["sep"], np.uint8)
+        dk, dcfg = Engine._delim_sls_cfg(delim["keys"], delim["source_key"], delim.get("renamed_key"),
+                                         delim.get("keep_fail"), delim.get("keep_succeed"), delim.get("copy_raw"))
+        rk, rcfg = Engine._delim_sls_cfg(regex["keys"], regex["source_key"], regex.get("renamed_key"),
+                                         regex.get("keep_fail"), regex.get("keep_succeed"), regex.get("copy_raw"))
+        tr = delim["treatment"]
+        return (sp, dk, rk), [_p(sp), sp.size, delim["quote"], int(tr == "extend"), int(tr == "discard")] + dcfg + \
+            rcfg + [int(bool(regex.get("whole_line")))]
+
+    def delim_regex_tap_dev(self, d_base, base_len, base_cap, d_ev_off, d_ev_len, n, d_status, d_nf, d_fo, d_fl, d_fd,
+                            max_fields, delim, regex, d_val_off, d_val_len):
+        """The regex stage's event table of a delimiter -> regex chain (lc_delim_regex_tap_dev) into d_val_off /
+        d_val_len, side copies behind base_len in d_base (capacity base_cap).  Returns the side bytes; raises
+        LcError(LC_ERR_CAPACITY) when they do not fit (nothing written; .need = the side bytes)."""
+        _keep, cfg = self._chain_cfg(delim, regex)
+        side = C.c_uint64(0)
+        rc = lib().lc_delim_regex_tap_dev(self._h, _p(d_base), base_len, base_cap, _p(d_ev_off), _p(d_ev_len), n,
+                                          _p(d_status), _p(d_nf), _p(d_fo), _p(d_fl), _p(d_fd), max_fields, *cfg,
+                                          _p(d_val_off), _p(d_val_len), C.byref(side))
+        if rc != LC_OK:
+            err = LcError(rc, lib().lc_last_error().decode())
+            err.need = int(side.value)
+            raise err
+        return int(side.value)
+
+    def sls_serialize_delim_regex_dev(self, d_base, base_len, d_ev_off, d_ev_len, n, d_status, d_nf, d_fo, d_fl, d_fd,
+                                      max_fields, delim, regex, d_val_off, d_val_len, d_re_status, d_cap_off,
+                                      d_cap_len, row_pitch, d_ev_time, d_ev_time_ns=None, d_out=None, out_cap=0):
+        """Wire bytes of a delimiter -> regex chain from device tables (lc_sls_serialize_delim_regex_dev).  Returns
+        (byte count written to d_out, counters[8]); with d_out None the byte count needed."""
+        _keep, cfg = self._chain_cfg(delim, regex)
+        need = C.c_uint64(0)
+        ctr = np.zeros(8, np.uint64)
+        rc = lib().lc_sls_serialize_delim_regex_dev(self._h, _p(d_base), base_len, _p(d_ev_off), _p(d_ev_len), n,
+                                                    _p(d_status), _p(d_nf), _p(d_fo), _p(d_fl), _p(d_fd), max_fields,
+                                                    *cfg, _p(d_val_off), _p(d_val_len), _p(d_re_status), _p(d_cap_off),
+                                                    _p(d_cap_len), row_pitch, _p(d_ev_time), _p(d_ev_time_ns),
+                                                    _p(d_out), out_cap, C.byref(need), _p(ctr))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value), ctr  # a sizing query
+        _check(rc)
+        return int(need.value), ctr
+
+    def _chain_host(self, rx, base, ev_off, ev_len, ev_time, ev_time_ns, allow_short, max_fields, delim, regex):
+        a = _u8(base)
+        ev_off = np.ascontiguousarray(ev_off, np.uint32)
+        ev_len = np.ascontiguousarray(ev_len, np.uint32)
+        t = np.ascontiguousarray(ev_time, np.uint32)
+        ns = None if ev_time_ns is None else np.ascontiguousarray(ev_time_ns, np.uint32)
+        n = ev_off.size
+        mf = int(max_fields if max_fields is not None else len(delim["keys"]) + 16)
+        keep, cfg = self._chain_cfg(delim, regex)
+        head = [self._h, _rh(rx), _p(a), a.size, _p(ev_off), _p(ev_len), n, _p(t), _p(ns), int(bool(allow_short)), mf]
+        return (a, ev_off, ev_len, t, ns, keep), head + cfg, 2 * a.size + 96 * n + 64
+
+    def delim_regex_parse_sls(self, rx, base, ev_off, ev_len, ev_time, delim, regex, allow_short=True,
+                              max_fields=None, ev_time_ns=None, out_cap=None):
+        """Host buffers in, wire bytes of the delimiter -> regex chain out (lc_delim_regex_parse_sls; rx may be None
+        in whole-line mode).  Returns (bytes, counters[8])."""
+        _keep, args, est = self._chain_host(rx, base, ev_off, ev_len, ev_time, ev_time_ns, allow_short, max_fields,
+                                            delim, regex)
+        cap = int(out_cap if out_cap is not None else est)
+        for _ in range(2):
+            out = np.empty(max(cap, 1), np.uint8)
+            need = C.c_uint64(0)
+            ctr = np.zeros(8, np.uint64)
+            rc = lib().lc_delim_regex_parse_sls(*args, _p(out), cap, C.byref(need), _p(ctr))
+            if rc == LC_ERR_CAPACITY and out_cap is None:
+                cap = int(need.value)
+                continue
+            _check(rc)
+            return bytes(out[:need.value]), ctr
+        _check(rc)
+
+    def delim_regex_parse_sls_lz4(self, rx, base, ev_off, ev_len, ev_time, delim, regex, allow_short=True,
+                                  max_fields=None, ev_time_ns=None, tail=b"", out_cap=None):
+        """delim_regex_parse_sls's records followed by `tail` as ONE LZ4 block (lc_delim_regex_parse_sls_lz4).
+        Returns (block, raw_len, counters[8])."""
+        _keep, args, est = self._chain_host(rx, base, ev_off, ev_len, ev_time, ev_time_ns, allow_short, max_fields,
+                                            delim, regex)
+        return self._sls_lz4(lambda *rest: lib().lc_delim_regex_parse_sls_lz4(*args, *rest), 8, tail, out_cap,
+                             est + len(tail))
+
+    @staticmethod
     def _span_keys(key, offset_key, src_pos, time, time_ns):
         """key / offset_key: bytes (offset_key None = no offset key); time_ns None = no Time_ns"""
         return [key, len(key), offset_key, len(offset_key) if offset_key is not None else 0, int(src_pos),
@@ -748,6 +845,35 @@ class HostProcessor:
         data = C.string_at(out, n.value)
         L.lc_host_string_free(out)
         return data, int(raw.value), None
+
+
+def host_chain_serialize_sls(delim, regex, group, enable_ns=False, mode=0):
+    """The delimiter -> regex chain of two HostProcessors on a JSON group (lc_host_chain_serialize_sls).  mode 0:
+    delim's SerializeSls(group, regex); 1: Process + Process + Serialize; 2: SerializeSlsLz4.  Returns (bytes, raw_len,
+    None) or (None, 0, error)."""
+    import json
+    L = lib()
+    L.lc_host_chain_serialize_sls.restype = C.c_void_p
+    L.lc_host_chain_serialize_sls.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p, C.c_int, C.c_int,
+                                              C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong),
+                                              C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    L.lc_host_string_free.argtypes = [C.c_void_p]
+    err, fail = C.c_void_p(), C.c_void_p()
+    n, raw = C.c_ulonglong(0), C.c_ulonglong(0)
+    out = L.lc_host_chain_serialize_sls(delim._h, regex._h, json.dumps(group).encode("utf-8"), int(bool(enable_ns)),
+                                        mode, C.byref(n), C.byref(raw), C.byref(err), C.byref(fail))
+    if fail.value:
+        msg = C.string_at(fail.value).decode()
+        L.lc_host_string_free(fail)
+        raise LcError(LC_ERR_CUDA, msg)
+    if not out:
+        msg = C.string_at(err.value).decode() if err.value else "unknown error"
+        if err.value:
+            L.lc_host_string_free(err)
+        return None, 0, msg
+    data = C.string_at(out, n.value)
+    L.lc_host_string_free(out)
+    return data, int(raw.value), None
 
 
 def host_lz4_compress(inputs):

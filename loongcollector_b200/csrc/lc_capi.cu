@@ -102,6 +102,9 @@ struct lc_engine {
     // LZ4 compressor: sequences, chunk summaries, chunk sizes / anchors, chunk and block offsets, host-call tables and
     // output; no parse or SLS stage uses them
     DevBuf z_seq, z_info, z_size, z_first, z_choff, z_tab, z_out;
+    // delimiter -> regex -> SLS chain: the delimiter's key strings, the value table, the regex tables over it, side-copy
+    // sizes and slots, the per-chunk scan descriptors of the tap; no stage of the chain uses them for anything else
+    DevBuf dr_keys, dr_val_off, dr_val_len, dr_status, dr_cap_off, dr_cap_len, dr_copy, dr_slot, dr_desc;
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
     std::unordered_map<uint64_t, void*> blobs; // regex id * 4 + layout -> device blob
@@ -314,7 +317,9 @@ void lc_engine_destroy(lc_engine_t* e) {
     DevBuf* bufs[] = {&e->in, &e->ev_off, &e->ev_len, &e->out_a, &e->out_b, &e->out_c, &e->out_d, &e->out_e,
                       &e->lines_off, &e->lines_len, &e->flags, &e->state, &e->cnt, &e->pos, &e->lab_sizes,
                       &e->lab_off, &e->lab, &e->order, &e->desc, &e->small, &e->split_scratch, &e->sls_plan,
-                      &e->z_seq, &e->z_info, &e->z_size, &e->z_first, &e->z_choff, &e->z_tab, &e->z_out};
+                      &e->z_seq, &e->z_info, &e->z_size, &e->z_first, &e->z_choff, &e->z_tab, &e->z_out,
+                      &e->dr_keys, &e->dr_val_off, &e->dr_val_len, &e->dr_status, &e->dr_cap_off, &e->dr_cap_len,
+                      &e->dr_copy, &e->dr_slot, &e->dr_desc};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -1769,7 +1774,7 @@ int serialize_sls_dev(lc_engine_t* e, const char* what, uint64_t n, uint32_t nco
     e->launches += 2;
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(&hs->total, &ds->total, 8, cudaMemcpyDeviceToHost, e->stream));
-    unsigned long long ctr[4] = {0, 0, 0, 0};
+    unsigned long long ctr[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     if (d_ctr)
         CU_TRY(cudaMemcpyAsync(ctr, d_ctr, ncounters * sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(cudaStreamSynchronize(e->stream));
@@ -1866,7 +1871,7 @@ int parse_sls_host(lc_engine_t* e, const char* what, const uint8_t* base, uint64
     e->launches++;
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(&hs->total, &ds->total, 8, cudaMemcpyDeviceToHost, e->stream));
-    unsigned long long ctr[4] = {0, 0, 0, 0};
+    unsigned long long ctr[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     CU_TRY(cudaMemcpyAsync(ctr, d_ctr, ncounters * sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(cudaStreamSynchronize(e->stream));
     for (uint32_t k = 0; k < ncounters; ++k)
@@ -1902,11 +1907,13 @@ int parse_sls_host(lc_engine_t* e, const char* what, const uint8_t* base, uint64
     return LC_OK;
 }
 
-// the configuration of the delimiter-fed serialiser, its key strings staged on the device (engine `order` buffer)
+// the configuration of the delimiter-fed serialiser, its key strings staged on the device (`dst`, by default the engine
+// `order` buffer)
 int delim_sls_config(lc_engine_t* e, const char* what, uint32_t max_fields, const uint8_t* sep, uint32_t sep_len,
                      uint8_t quote, int extend, int discard, const char* const* keys, const uint32_t* key_lens,
                      uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
-                     uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, LcDelimSlsCfg* c) {
+                     uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, LcDelimSlsCfg* c,
+                     DevBuf* dst = nullptr) {
     if (!sep || (nkeys && (!keys || !key_lens)) || (source_key_len && !source_key) ||
         (renamed_key_len && !renamed_key))
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
@@ -1926,12 +1933,13 @@ int delim_sls_config(lc_engine_t* e, const char* what, uint32_t max_fields, cons
     if (why)
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
     const size_t at_bytes = at.size() * 4;
-    CU_TRY(e->order.ensure(at_bytes + kb.size() + 16));
-    CU_TRY(cudaMemcpyAsync(e->order.p, at.data(), at_bytes, cudaMemcpyHostToDevice, e->stream));
-    CU_TRY(cudaMemcpyAsync(e->order.as<uint8_t>() + at_bytes, kb.data(), kb.size(), cudaMemcpyHostToDevice, e->stream));
+    DevBuf& d = dst ? *dst : e->order;
+    CU_TRY(d.ensure(at_bytes + kb.size() + 16));
+    CU_TRY(cudaMemcpyAsync(d.p, at.data(), at_bytes, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(d.as<uint8_t>() + at_bytes, kb.data(), kb.size(), cudaMemcpyHostToDevice, e->stream));
     CU_TRY(cudaStreamSynchronize(e->stream)); // (pageable sources: their bytes must be on the device before they die)
-    c->key_at = e->order.as<uint32_t>();
-    c->keys = e->order.as<uint8_t>() + at_bytes;
+    c->key_at = d.as<uint32_t>();
+    c->keys = d.as<uint8_t>() + at_bytes;
     return LC_OK;
 }
 
@@ -1976,6 +1984,55 @@ int regex_sls_config(lc_engine_t* e, const char* what, const char* const* keys, 
     strings.insert(strings.end(), {source_key, renamed_key, "__raw_log__", "content"});
     lens.insert(lens.end(), {source_key_len, renamed_key_len, 11u, 7u});
     return stage_regex_sls(e, what, plan.data(), strings.data(), lens.data(), nkeys + 4, c);
+}
+
+// The configuration of the delimiter -> regex chain (both stages' arguments, CHAIN_ARGS below): the delimiter's
+// configuration and keys (engine `dr_keys` buffer), the regex plans over its key k (`sls_plan`) and the chain's own
+// checks (lc_delim_regex_sls_link).  pitch = the regex tables' row pitch.
+#define CHAIN_PARAMS                                                                                                   \
+    const uint8_t *sep, uint32_t sep_len, uint8_t quote, int extend, int discard, const char *const *keys,             \
+        const uint32_t *key_lens, uint32_t nkeys, const char *source_key, uint32_t source_key_len,                     \
+        const char *renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,              \
+        const char *const *rkeys, const uint32_t *rkey_lens, uint32_t rnkeys, const char *rsource_key,                 \
+        uint32_t rsource_key_len, const char *rrenamed_key, uint32_t rrenamed_key_len, int rkeep_fail,                 \
+        int rkeep_succeed, int rcopy_raw, int whole_line
+#define CHAIN_ARGS                                                                                                     \
+    sep, sep_len, quote, extend, discard, keys, key_lens, nkeys, source_key, source_key_len, renamed_key,              \
+        renamed_key_len, keep_fail, keep_succeed, copy_raw, rkeys, rkey_lens, rnkeys, rsource_key, rsource_key_len,    \
+        rrenamed_key, rrenamed_key_len, rkeep_fail, rkeep_succeed, rcopy_raw, whole_line
+int chain_config(lc_engine_t* e, const char* what, uint32_t max_fields, CHAIN_PARAMS, uint32_t pitch,
+                 LcDelimRegexSlsCfg* c) {
+    memset(c, 0, sizeof *c);
+    int rc = delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, keys, key_lens, nkeys,
+                              source_key, source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed,
+                              copy_raw, &c->d, &e->dr_keys);
+    if (rc)
+        return rc;
+    rc = regex_sls_config(e, what, rkeys, rkey_lens, rnkeys, rsource_key, rsource_key_len, rrenamed_key,
+                          rrenamed_key_len, rkeep_fail, rkeep_succeed, rcopy_raw, whole_line, pitch, &c->x);
+    if (rc)
+        return rc;
+    const char* why = lc_delim_regex_sls_link(c->d, keys, key_lens, source_key, source_key_len, renamed_key,
+                                              renamed_key_len, rkeys, rkey_lens, rnkeys, rsource_key, rsource_key_len,
+                                              rrenamed_key, rrenamed_key_len, rkeep_fail, rkeep_succeed, rcopy_raw,
+                                              whole_line, c);
+    if (why)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    return LC_OK;
+}
+
+// Queues the value tap of n rows: copy sizes into d_copy, their exclusive sum into d_slot (look-back descriptors
+// `desc`, zeroed, scan_tiles(n) + 3 words: the total and the ticket follow them), then the value table and the side
+// copies at d_base[side_at + slot).
+void queue_tap(lc_engine_t* e, const LcDelimRegexSlsCfg& c, const lck::DelimSlsTables& t, uint64_t n,
+               uint64_t side_at, uint8_t* d_base, uint32_t* d_copy, uint64_t* d_slot, uint64_t* desc,
+               uint32_t* d_val_off, uint32_t* d_val_len) {
+    const uint32_t tiles = lck::scan_tiles(n);
+    lck::launch_delim_regex_tap_sizes(c, t, n, d_copy, e->stream);
+    lck::launch_exclusive_sum(d_copy, n, d_slot, desc + tiles + 1, desc, reinterpret_cast<uint32_t*>(desc + tiles + 2),
+                              e->stream);
+    lck::launch_delim_regex_tap(c, t, n, d_slot, side_at, d_base, d_val_off, d_val_len, e->stream);
+    e->launches += 3;
 }
 
 // The configuration of the split-fed serialiser over one source value d_src[0, src_len); the keys are staged on the
@@ -2389,6 +2446,226 @@ int lc_delim_parse_sls_lz4(lc_engine_t* e, const uint8_t* base, uint64_t base_le
                                 sep, sep_len, quote, extend, discard, allow_short, max_fields, keys, key_lens, nkeys,
                                 source_key, source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed,
                                 copy_raw, out, out_cap, out_len, counters, &z);
+}
+
+int lc_delim_regex_tap_dev(lc_engine_t* e, uint8_t* d_base, uint64_t base_len, uint64_t base_cap,
+                           const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, const uint8_t* d_status,
+                           const uint32_t* d_nfields, const uint32_t* d_f_off, const uint32_t* d_f_len,
+                           const uint32_t* d_f_dq, uint32_t max_fields, CHAIN_PARAMS, uint32_t* d_val_off,
+                           uint32_t* d_val_len, uint64_t* side_len) {
+    static const char* what = "lc_delim_regex_tap_dev";
+    if (!e || !side_len || (n && (!d_base || !d_ev_off || !d_ev_len || !d_status || !d_nfields || !d_f_off ||
+                                  !d_f_len || !d_f_dq || !d_val_off || !d_val_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *side_len = 0;
+    const uint64_t side_at = (base_len + 15) & ~15ull;
+    if (base_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 events and < 2^32 columns per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcDelimRegexSlsCfg c;
+    rc = chain_config(e, what, max_fields, CHAIN_ARGS, 0, &c);
+    if (rc || n == 0)
+        return rc;
+    const lck::DelimSlsTables t{d_base, d_ev_off, d_ev_len, d_status, d_nfields, d_f_off, d_f_len, d_f_dq};
+    const uint32_t tiles = lck::scan_tiles(n);
+    CU_TRY(e->dr_copy.ensure(n * 4));
+    CU_TRY(e->dr_slot.ensure(n * 8));
+    CU_TRY(e->dr_desc.ensure(((uint64_t)tiles + 3) * 8));
+    uint64_t* desc = e->dr_desc.as<uint64_t>();
+    CU_TRY(cudaMemsetAsync(desc, 0, ((uint64_t)tiles + 3) * 8, e->stream));
+    // sizes and slots first: nothing is written before the side region is known to fit
+    lck::launch_delim_regex_tap_sizes(c, t, n, e->dr_copy.as<uint32_t>(), e->stream);
+    lck::launch_exclusive_sum(e->dr_copy.as<uint32_t>(), n, e->dr_slot.as<uint64_t>(), desc + tiles + 1, desc,
+                              reinterpret_cast<uint32_t*>(desc + tiles + 2), e->stream);
+    e->launches += 2;
+    CU_TRY(cudaGetLastError());
+    uint64_t need = 0;
+    CU_TRY(cudaMemcpyAsync(&need, desc + tiles + 1, 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    *side_len = need;
+    if (side_at + need + 16 >= 0xFFFFFFF0ull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": line buffer and side copies must stay below 4 GiB");
+    if (need && side_at + need > base_cap)
+        return fail(LC_ERR_CAPACITY, std::string(what) + ": no room for the side copies behind base_len");
+    lck::launch_delim_regex_tap(c, t, n, e->dr_slot.as<uint64_t>(), side_at, d_base, d_val_off, d_val_len, e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    return LC_OK;
+}
+
+int lc_sls_serialize_delim_regex_dev(lc_engine_t* e, const uint8_t* d_base, uint64_t base_len,
+                                     const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n,
+                                     const uint8_t* d_status, const uint32_t* d_nfields, const uint32_t* d_f_off,
+                                     const uint32_t* d_f_len, const uint32_t* d_f_dq, uint32_t max_fields,
+                                     CHAIN_PARAMS, const uint32_t* d_val_off, const uint32_t* d_val_len,
+                                     const uint8_t* d_re_status, const uint32_t* d_cap_off, const uint32_t* d_cap_len,
+                                     uint32_t row_pitch, const uint32_t* d_ev_time, const uint32_t* d_ev_time_ns,
+                                     uint8_t* d_out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[8]) {
+    static const char* what = "lc_sls_serialize_delim_regex_dev";
+    const bool caps = !whole_line && rnkeys && rnkeys <= row_pitch; // the parsed plan reads the capture tables
+    if (!e || !out_len || (n && (!d_base || !d_ev_off || !d_ev_len || !d_status || !d_nfields || !d_f_off || !d_f_len ||
+                                 !d_f_dq || !d_val_off || !d_val_len || !d_ev_time)) ||
+        (n && !whole_line && !d_re_status) || (n && caps && (!d_cap_off || !d_cap_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (counters)
+        memset(counters, 0, 8 * sizeof(uint64_t));
+    if (base_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32) ||
+        n * (uint64_t)row_pitch >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 events and < 2^32 columns per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcDelimRegexSlsCfg c;
+    rc = chain_config(e, what, max_fields, CHAIN_ARGS, row_pitch, &c);
+    if (rc || n == 0)
+        return rc;
+    const lck::DelimRegexSlsTables t{{d_base, d_ev_off, d_ev_len, d_status, d_nfields, d_f_off, d_f_len, d_f_dq},
+                                     d_val_off,
+                                     d_val_len,
+                                     whole_line ? nullptr : d_re_status,
+                                     caps ? d_cap_off : nullptr,
+                                     caps ? d_cap_len : nullptr};
+    return serialize_sls_dev(
+        e, what, n, 8,
+        [&](uint32_t* rec, uint32_t* body, unsigned long long* ctr) {
+            lck::launch_delim_regex_sls_sizes(c, t, d_ev_time_ns, n, rec, body, ctr, e->stream);
+        },
+        [&](const uint64_t* rec_off, const uint32_t* body, uint8_t* out) {
+            lck::launch_delim_regex_sls_emit(c, t, d_ev_time, d_ev_time_ns, n, rec_off, body, out, e->stream);
+        },
+        d_out, out_cap, out_len, counters);
+}
+
+} // extern "C"
+
+// lc_delim_regex_parse_sls[_lz4]: per upload chunk the delimiter stage, the value tap, the regex stage over the values
+// and the size pass; the tables never leave the device.  The side copies of chunk c go behind the arena at a bound the
+// host knows without a round trip: a copy is never longer than its line, so chunk c's copies fit in the sum of its
+// line lengths, and chunk c starts where the bounds of the chunks before it end.
+static int delim_regex_parse_sls_impl(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* base,
+                                      uint64_t base_len, const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n,
+                                      const uint32_t* ev_time, const uint32_t* ev_time_ns, int allow_short,
+                                      uint32_t max_fields, CHAIN_PARAMS, uint8_t* out, uint64_t out_cap,
+                                      uint64_t* out_len, uint64_t counters[8], const Lz4Tail* z) {
+    if (!e || (!re && !whole_line) || !out_len || !counters || (n && (!ev_off || !ev_len || !ev_time)) ||
+        (base_len && !base) || (z && (!z->raw_len || (z->len && !z->tail))))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (z)
+        *z->raw_len = 0;
+    memset(counters, 0, 8 * sizeof(uint64_t));
+    int rc = whole_line ? (int)LC_OK : check_regex_usable(re, what);
+    if (rc)
+        return rc;
+    const uint32_t G = whole_line ? 0u : re->res.ngroups;
+    uint64_t side_cap = 0;
+    for (uint64_t i = 0; i < n; ++i)
+        side_cap += ev_len[i];
+    const uint64_t side_at = (base_len + 15) & ~15ull, arena = side_at + side_cap;
+    if (arena + 16 >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32) ||
+        n * (uint64_t)G >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "lines plus their total length must be < 4 GiB, < 2^30 events, < 2^32 columns "
+                                      "and < 2^32 captures per call");
+    rc = bind(e);
+    if (rc)
+        return rc;
+    LcDelimRegexSlsCfg c;
+    rc = chain_config(e, what, max_fields, CHAIN_ARGS, G, &c);
+    if (rc || n == 0)
+        return rc || !z ? rc : lz4_tail_only(e, what, *z, out, out_cap, out_len);
+    // delimiter tables out_a .. out_e, value table, regex tables, tap scratch: all stay on the device
+    const uint64_t MF = max_fields, fbytes = n * MF * 4, nchunks = pipeline_chunks(base_len, n);
+    const uint64_t dwords = lck::scan_tiles(n) + 4 * nchunks + 8;
+    CU_TRY(e->in.ensure(arena + 16));
+    CU_TRY(e->out_a.ensure(n));
+    CU_TRY(e->out_b.ensure(n * 4));
+    CU_TRY(e->out_c.ensure(fbytes));
+    CU_TRY(e->out_d.ensure(fbytes));
+    CU_TRY(e->out_e.ensure(fbytes));
+    CU_TRY(e->dr_val_off.ensure(n * 4));
+    CU_TRY(e->dr_val_len.ensure(n * 4));
+    CU_TRY(e->dr_status.ensure(n));
+    CU_TRY(e->dr_cap_off.ensure(n * G * 4 + 4));
+    CU_TRY(e->dr_cap_len.ensure(n * G * 4 + 4));
+    CU_TRY(e->dr_copy.ensure(n * 4));
+    CU_TRY(e->dr_slot.ensure(n * 8));
+    CU_TRY(e->dr_desc.ensure(dwords * 8));
+    CU_TRY(cudaMemsetAsync(e->dr_desc.p, 0, dwords * 8, e->stream));
+    const bool caps = !whole_line && rnkeys && rnkeys <= G;
+    auto dtables = [&](uint64_t i0) {
+        return lck::DelimSlsTables{e->in.as<uint8_t>(),          e->ev_off.as<uint32_t>() + i0,
+                                   e->ev_len.as<uint32_t>() + i0, e->out_a.as<uint8_t>() + i0,
+                                   e->out_b.as<uint32_t>() + i0,  e->out_c.as<uint32_t>() + i0 * MF,
+                                   e->out_d.as<uint32_t>() + i0 * MF, e->out_e.as<uint32_t>() + i0 * MF};
+    };
+    auto tables = [&](uint64_t i0) {
+        return lck::DelimRegexSlsTables{dtables(i0),
+                                        e->dr_val_off.as<uint32_t>() + i0,
+                                        e->dr_val_len.as<uint32_t>() + i0,
+                                        whole_line ? nullptr : e->dr_status.as<uint8_t>() + i0,
+                                        caps ? e->dr_cap_off.as<uint32_t>() + i0 * G : nullptr,
+                                        caps ? e->dr_cap_len.as<uint32_t>() + i0 * G : nullptr};
+    };
+    uint64_t side_used = 0, dpos = 0; // the side bound and the scan descriptors of the chunks queued so far
+    auto parse = [&](uint64_t i0, uint64_t cnt, uint64_t span) {
+        const lck::DelimSlsTables t = dtables(i0);
+        int r = lc_delim_parse_dev(e, t.base, base_len, t.ev_off, t.ev_len, cnt, sep, sep_len, quote, nkeys, extend,
+                                   allow_short, max_fields, e->out_a.as<uint8_t>() + i0, e->out_b.as<uint32_t>() + i0,
+                                   e->out_c.as<uint32_t>() + i0 * MF, e->out_d.as<uint32_t>() + i0 * MF,
+                                   e->out_e.as<uint32_t>() + i0 * MF);
+        if (r)
+            return r;
+        uint64_t bound = 0;
+        for (uint64_t i = i0; i < i0 + cnt; ++i)
+            bound += ev_len[i];
+        queue_tap(e, c, t, cnt, side_at + side_used, e->in.as<uint8_t>(), e->dr_copy.as<uint32_t>() + i0,
+                  e->dr_slot.as<uint64_t>() + i0, e->dr_desc.as<uint64_t>() + dpos, e->dr_val_off.as<uint32_t>() + i0,
+                  e->dr_val_len.as<uint32_t>() + i0);
+        CU_TRY(cudaGetLastError());
+        side_used += bound;
+        dpos += lck::scan_tiles(cnt) + 3;
+        if (whole_line)
+            return (int)LC_OK;
+        return regex_parse_dev_impl(e, re, e->in.as<uint8_t>(), arena, span + bound, e->dr_val_off.as<uint32_t>() + i0,
+                                    e->dr_val_len.as<uint32_t>() + i0, 1, cnt, rnkeys, e->dr_status.as<uint8_t>() + i0,
+                                    e->dr_cap_off.as<uint32_t>() + i0 * G, e->dr_cap_len.as<uint32_t>() + i0 * G,
+                                    false);
+    };
+    auto sizes = [&](uint64_t i0, uint64_t cnt, const uint32_t* d_ns, uint32_t* rec, uint32_t* body,
+                     unsigned long long* ctr) {
+        lck::launch_delim_regex_sls_sizes(c, tables(i0), d_ns, cnt, rec, body, ctr, e->stream);
+    };
+    auto emit = [&](const uint32_t* d_time, const uint32_t* d_ns, const uint64_t* rec_off, const uint32_t* body,
+                    uint8_t* d_wire) {
+        lck::launch_delim_regex_sls_emit(c, tables(0), d_time, d_ns, n, rec_off, body, d_wire, e->stream);
+    };
+    return parse_sls_host(e, what, base, base_len, ev_off, ev_len, n, ev_time, ev_time_ns, 8, parse, sizes, emit, out,
+                          out_cap, out_len, counters, z);
+}
+
+extern "C" {
+
+int lc_delim_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base, uint64_t base_len,
+                             const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time,
+                             const uint32_t* ev_time_ns, int allow_short, uint32_t max_fields, CHAIN_PARAMS,
+                             uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[8]) {
+    return delim_regex_parse_sls_impl(e, "lc_delim_regex_parse_sls", re, base, base_len, ev_off, ev_len, n, ev_time,
+                                      ev_time_ns, allow_short, max_fields, CHAIN_ARGS, out, out_cap, out_len, counters,
+                                      nullptr);
+}
+
+int lc_delim_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* base, uint64_t base_len,
+                                 const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* ev_time,
+                                 const uint32_t* ev_time_ns, int allow_short, uint32_t max_fields, CHAIN_PARAMS,
+                                 const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+                                 uint64_t* out_len, uint64_t* raw_len, uint64_t counters[8]) {
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return delim_regex_parse_sls_impl(e, "lc_delim_regex_parse_sls_lz4", re, base, base_len, ev_off, ev_len, n,
+                                      ev_time, ev_time_ns, allow_short, max_fields, CHAIN_ARGS, out, out_cap, out_len,
+                                      counters, &z);
 }
 
 int lc_sls_serialize_spans_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,

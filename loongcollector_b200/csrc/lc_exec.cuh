@@ -973,8 +973,21 @@ LC_HD void lc_delim_sls_columns(const LcDelimSlsCfg& c, const uint8_t* base, con
 //            KeepingSourceWhenParseSucceed and that key is not present yet
 //   failed:  RenamedSourceKey -> line [, __raw_log__ -> line] with KeepingSourceWhenParseFail, else erased
 //   blank:   untouched: SourceKey -> the whole, untrimmed line
-template <class S>
-LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, const LcDelimSlsRow& r, S& s) {
+//
+// x is the stage chained behind the delimiter (LcDelimNoChain: none).  Before each content the body asks x.own(kid) --
+// kid = the key id of the content: key j < nkeys, or nkeys + 0 / 1 / 2 = SourceKey / RenamedSourceKey / "__raw_log__"
+// -- and when x owns it, x.in_place(s) is written in its place instead; x.tail(s) runs after the contents, before
+// Time_ns.  The count returned is the delimiter stage's, owned content included.
+struct LcDelimNoChain {
+    LC_HD bool own(uint32_t) const { return false; }
+    template <class S>
+    LC_HD void in_place(S&) {}
+    template <class S>
+    LC_HD void tail(S&) {}
+};
+
+template <class S, class X>
+LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, const LcDelimSlsRow& r, S& s, X& x) {
     const uint32_t K_SRC = c.nkeys, K_REN = c.nkeys + 1, K_RAW = c.nkeys + 2;
     auto kp = [&](uint32_t k) { return c.keys + c.key_at[k]; };
     auto kl = [&](uint32_t k) { return c.key_at[k + 1] - c.key_at[k]; };
@@ -987,9 +1000,13 @@ LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, co
     }
     uint32_t cnt = 0;
     auto whole_line = [&](uint32_t k) {
+        ++cnt;
+        if (x.own(k)) {
+            x.in_place(s);
+            return;
+        }
         lc_sls_pair_open(s, kp(k), kl(k), r.elen);
         s.copy(line, r.elen);
-        ++cnt;
     };
     auto value = [&](uint32_t off, uint32_t len, uint32_t dq) {
         if (c.use_quote && dq)
@@ -1011,8 +1028,12 @@ LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, co
             if (c.src_col != LC_DELIM_SLS_NONE && c.src_col < nf) {
                 const uint32_t j = c.src_col; // < nkeys < max_fields: always in the table
                 const uint32_t dq = c.use_quote ? r.fd[j] : 0u;
-                lc_sls_pair_open(s, kp(K_SRC), kl(K_SRC), r.fl[j] - dq);
-                value(r.fo[j], r.fl[j], dq);
+                if (x.own(K_SRC)) {
+                    x.in_place(s);
+                } else {
+                    lc_sls_pair_open(s, kp(K_SRC), kl(K_SRC), r.fl[j] - dq);
+                    value(r.fo[j], r.fl[j], dq);
+                }
                 ++cnt;
             } else {
                 whole_line(K_SRC);
@@ -1030,6 +1051,11 @@ LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, co
             if (j < nk) {
                 if (c.mode == LC_DELIM_SLS_DISCARD && kl(j) == 1 && kp(j)[0] == '_')
                     return;
+                if (x.own(j)) {
+                    x.in_place(s);
+                    ++cnt;
+                    return;
+                }
                 lc_sls_pair_open(s, kp(j), kl(j), len - dq);
             } else {
                 uint8_t k[20];
@@ -1061,11 +1087,36 @@ LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, co
                 whole_line(K_REN);
         }
     }
+    x.tail(s);
     if (r.has_ns) {
         const uint8_t h[5] = {0x25, (uint8_t)r.ns, (uint8_t)(r.ns >> 8), (uint8_t)(r.ns >> 16), (uint8_t)(r.ns >> 24)};
         s.put(h, 5);
     }
     return cnt;
+}
+
+template <class S>
+LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, const LcDelimSlsRow& r, S& s) {
+    LcDelimNoChain x;
+    return lc_delim_sls_body(c, base, r, s, x);
+}
+
+// "__column<digits>__": the form of the delimiter's generated overflow keys; *idx = the value when it is canonical
+// decimal, else LC_DELIM_SLS_NONE
+inline bool lc_delim_column_form(const char* s, uint32_t l, uint32_t* idx) {
+    if (l < 11 || memcmp(s, "__column", 8) || s[l - 1] != '_' || s[l - 2] != '_')
+        return false;
+    uint64_t v = 0;
+    for (uint32_t i = 8; i < l - 2; ++i) {
+        if (s[i] < '0' || s[i] > '9')
+            return false;
+        v = v * 10 + (uint64_t)(s[i] - '0');
+        if (v >= LC_DELIM_SLS_NONE)
+            v = LC_DELIM_SLS_NONE;
+    }
+    const bool canonical = (l - 10 == 1 || s[8] != '0') && v < LC_DELIM_SLS_NONE;
+    *idx = canonical ? (uint32_t)v : LC_DELIM_SLS_NONE;
+    return true;
 }
 
 
@@ -1085,22 +1136,7 @@ inline const char* lc_delim_sls_setup(const uint8_t* sep, uint32_t sep_len, uint
     const bool disc = discard != 0, overflow_keys = !disc;
     auto eq = [](const char* a, uint32_t la, const char* b, uint32_t lb) { return la == lb && !memcmp(a, b, la); };
     auto is_skip = [&](uint32_t k) { return disc && key_lens[k] == 1 && keys[k][0] == '_'; };
-    // "__column<digits>__": the form of the generated overflow keys; *idx = the value when it is canonical decimal
-    auto column_form = [](const char* s, uint32_t l, uint32_t* idx) {
-        if (l < 11 || memcmp(s, "__column", 8) || s[l - 1] != '_' || s[l - 2] != '_')
-            return false;
-        uint64_t v = 0;
-        for (uint32_t i = 8; i < l - 2; ++i) {
-            if (s[i] < '0' || s[i] > '9')
-                return false;
-            v = v * 10 + (uint64_t)(s[i] - '0');
-            if (v >= LC_DELIM_SLS_NONE)
-                v = LC_DELIM_SLS_NONE;
-        }
-        const bool canonical = (l - 10 == 1 || s[8] != '0') && v < LC_DELIM_SLS_NONE;
-        *idx = canonical ? (uint32_t)v : LC_DELIM_SLS_NONE;
-        return true;
-    };
+    auto column_form = lc_delim_column_form;
     uint32_t dummy;
     for (uint32_t a = 0; a < nkeys; ++a) {
         if (overflow_keys && column_form(keys[a], key_lens[a], &dummy))
@@ -1174,6 +1210,7 @@ struct LcRegexSlsCfg {
     uint32_t whole_line; // Regex "(.*)": no regex ran, every row is parsed (no status or capture tables)
     uint32_t ok_fits;    // the parsed plan's captures lie inside a row; otherwise no row can be LC_REGEX_OK
     uint32_t keep_fail;  // KeepingSourceWhenParseFail: failed rows are kept, else erased
+    uint32_t ok_in_place; // entry 0 of the parsed plan is the source content, overwritten in place (not appended)
 };
 
 // One event: its line base[eo, eo + elen) and its row of the capture tables (offsets into base).
@@ -1330,6 +1367,7 @@ inline const char* lc_regex_sls_setup(const char* const* keys, const uint32_t* k
         del(K_SRC);
     if (keep_succeed)
         add_absent(K_REN);
+    c->ok_in_place = list[2];
     c->n_ok = finish();
     // failed rows (none in whole-line mode)
     list = plan + 2 * c->n_ok;
@@ -1349,6 +1387,198 @@ inline const char* lc_regex_sls_setup(const char* const* keys, const uint32_t* k
     c->whole_line = whole_line != 0;
     c->ok_fits = whole_line || nkeys <= pitch;
     c->keep_fail = keep_fail != 0;
+    return nullptr;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, delimiter -> regex chain: the Log record of one event that ProcessorParseDelimiterNative::Process followed by
+// ProcessorParseRegexNative::Process (regex SourceKey = key k of the delimiter) leaves behind.  The event is flat on
+// entry.  The regex stage reads key k's value, which after the delimiter stage is one of
+//   column k, unquoted (AddFieldWithUnQuote)   delimiter OK and nfields > k
+//   the whole line                             the line stayed under key k: a short row whose SourceKey is key k, a
+//                                              short row with KeepingSourceWhenParseSucceed whose RenamedSourceKey is
+//                                              key k, a kept failure whose RenamedSourceKey / "__raw_log__" is key k,
+//                                              a blank row whose SourceKey is key k
+//   absent                                     otherwise: out_key_not_found, the delimiter's record is left as it is
+// The value table (lc_delim_regex_tap) is the regex stage's event table; a column with doubled quotes is copied,
+// collapsed, into a side region of the line buffer, so captures stay offsets from one base.  The record is then the
+// delimiter's body (lc_delim_sls_body) with key k's content deleted -- or overwritten in place by the capture of a
+// regex key equal to k -- and the rest of the regex plan (lc_regex_sls_setup, SourceKey = k, "the line" = the value)
+// appended.  lc_delim_regex_sls_link refuses the configurations in which a regex content could land on a delimiter
+// content other than key k's, so no other in-place overwrite depends on the row.
+#define LC_DR_ABSENT 0u
+#define LC_DR_COLUMN 1u
+#define LC_DR_LINE 2u
+
+struct LcDelimRegexSlsCfg {
+    LcDelimSlsCfg d;
+    LcRegexSlsCfg x; // the regex plans, over "the line" = the value
+    uint32_t col;    // k
+    uint32_t src_is_k, ren_is_k, raw_is_k; // the delimiter's SourceKey / RenamedSourceKey / "__raw_log__" is key k
+};
+
+LC_HD uint32_t lc_delim_regex_value(const LcDelimRegexSlsCfg& c, uint32_t status, uint32_t nf) {
+    if (status == 2) // LC_DELIM_BLANK: untouched
+        return c.src_is_k ? LC_DR_LINE : LC_DR_ABSENT;
+    if (status != 0) // failed: RenamedSourceKey [, "__raw_log__"] -> line when kept, else erased
+        return c.d.keep_fail && (c.ren_is_k || (c.d.copy_raw && c.raw_is_k)) ? LC_DR_LINE : LC_DR_ABSENT;
+    if (nf > c.col)
+        return LC_DR_COLUMN;
+    return c.src_is_k || (c.d.keep_succeed && c.ren_is_k) ? LC_DR_LINE : LC_DR_ABSENT;
+}
+
+// The value of one row: base[off, + len) (absent: the empty value at the line), and the bytes of its side copy (0: the
+// value lies in the line as it is).
+struct LcDrTap {
+    uint32_t off, len, copy;
+};
+LC_HD LcDrTap lc_delim_regex_tap(const LcDelimRegexSlsCfg& c, const LcDelimSlsRow& r) {
+    const uint32_t v = lc_delim_regex_value(c, r.status, r.nf);
+    if (v == LC_DR_COLUMN) { // k < nkeys < max_fields: always in the table
+        const uint32_t dq = c.d.use_quote ? r.fd[c.col] : 0u, n = r.fl[c.col] - dq;
+        return {r.fo[c.col], n, dq ? n : 0u};
+    }
+    return {r.eo, v == LC_DR_LINE ? r.elen : 0u, 0u};
+}
+
+// writes the collapsed column of a tap with copy > 0 to dst[0, t.copy)
+LC_HD void lc_delim_regex_copy(const LcDelimRegexSlsCfg& c, const uint8_t* base, const LcDelimSlsRow& r, uint8_t* dst,
+                               uint32_t copy) {
+    LcSlsWrite w{dst, 0u, copy, 0u, 1u};
+    w.unquote(base + r.fo[c.col], r.fl[c.col], copy, c.d.quote);
+}
+
+// One event: its delimiter row, its value (the tap table) and the regex stage's row over that value.
+struct LcDelimRegexSlsRow {
+    LcDelimSlsRow d;
+    uint32_t vo, vl;
+    uint32_t status;
+    const uint32_t* co;
+    const uint32_t* cl;
+};
+
+// the regex stage as the delimiter body's chained stage (LcDelimNoChain's interface)
+struct LcDelimRegexStage {
+    const LcDelimRegexSlsCfg& c;
+    const uint8_t* base;
+    const LcDelimRegexSlsRow& r;
+    bool present, ok;
+    uint32_t m; // contents the regex stage wrote
+    LC_HD bool own(uint32_t kid) const {
+        const uint32_t nk = c.d.nkeys;
+        return present && (kid == c.col || (kid == nk && c.src_is_k) || (kid == nk + 1 && c.ren_is_k) ||
+                           (kid == nk + 2 && c.raw_is_k));
+    }
+    template <class S>
+    LC_HD void entry(S& s, uint32_t e) { // entry e of the row's plan
+        const uint32_t* p = c.x.plan + (ok ? 0u : 2u * c.x.n_ok) + 2 * e;
+        const bool line = p[1] == LC_REGEX_SLS_LINE;
+        const uint32_t vo = line ? r.vo : r.co[p[1]], vl = line ? r.vl : r.cl[p[1]];
+        lc_sls_pair_open(s, c.x.keys + c.x.key_at[p[0]], c.x.key_at[p[0] + 1] - c.x.key_at[p[0]], vl);
+        s.copy(base + vo, vl);
+        ++m;
+    }
+    template <class S>
+    LC_HD void in_place(S& s) {
+        if (ok && c.x.ok_in_place)
+            entry(s, 0);
+    }
+    template <class S>
+    LC_HD void tail(S& s) {
+        if (!present)
+            return;
+        const uint32_t n = ok ? c.x.n_ok : c.x.n_fail;
+        for (uint32_t e = ok && c.x.ok_in_place ? 1u : 0u; e < n; ++e)
+            entry(s, e);
+    }
+};
+
+// The body of the event's Log record into sink s (LcSlsCount / LcSlsWrite).  Returns the number of contents; 0 = the
+// event has none (erased by either stage, or LogEvent::Empty) and emits no record.  A regex failure without
+// KeepingSourceWhenParseFail erases the event when key k's content was its only one (ShouldEraseEvent).
+template <class S>
+LC_HD uint32_t lc_delim_regex_sls_body(const LcDelimRegexSlsCfg& c, const uint8_t* base, const LcDelimRegexSlsRow& r,
+                                       S& s) {
+    LcDelimRegexStage x{c, base, r, lc_delim_regex_value(c, r.d.status, r.d.nf) != LC_DR_ABSENT,
+                        lc_regex_sls_verdict(c.x, r.status) == 0u, 0u};
+    const uint32_t n = lc_delim_sls_body(c.d, base, r.d, s, x);
+    return x.present ? n - 1 + x.m : n;
+}
+
+// The row's counter verdicts (0 / 1): the delimiter stage's successful, failed, discarded, blank, then the regex
+// stage's successful, failed (LC_REGEX_NOMATCH), key-not-found, discarded.  cnt = lc_delim_regex_sls_body's result.
+// An event the delimiter stage erased never reaches the regex stage.
+struct LcDelimRegexVerdict {
+    uint32_t ctr[8];
+};
+LC_HD LcDelimRegexVerdict lc_delim_regex_verdict(const LcDelimRegexSlsCfg& c, const LcDelimRegexSlsRow& r,
+                                                 uint32_t cnt) {
+    LcDelimRegexVerdict v;
+    const uint32_t st = r.d.status;
+    v.ctr[0] = st == 0;
+    v.ctr[1] = st != 0 && st != 2;
+    v.ctr[2] = v.ctr[1] && !c.d.keep_fail;
+    v.ctr[3] = st == 2;
+    const bool present = lc_delim_regex_value(c, st, r.d.nf) != LC_DR_ABSENT;
+    const uint32_t rv = lc_regex_sls_verdict(c.x, r.status);
+    v.ctr[5] = present && rv == 1u;
+    v.ctr[6] = !present && !v.ctr[2];
+    v.ctr[7] = present && rv != 0u && cnt == 0u;
+    v.ctr[4] = present && !v.ctr[7];
+    return v;
+}
+
+// Host side: the chain's own checks and fields, after lc_delim_sls_setup (d) and lc_regex_sls_setup (with the regex
+// stage's arguments) accepted their halves.  Returns nullptr (c->col and the *_is_k flags set), or why the chain is
+// refused: a regex SourceKey that is not one of the delimiter's keys, or a content the regex stage may write (a key,
+// RenamedSourceKey, "__raw_log__") under a name the delimiter stage may leave besides key k -- that overwrite would
+// depend on the row's shape.  Likewise ShouldEraseEvent's "_time_" + "_source_" rule on a regex failure.
+inline const char* lc_delim_regex_sls_link(const LcDelimSlsCfg& d, const char* const* dkeys, const uint32_t* dkey_lens,
+                                           const char* dsrc, uint32_t dsrc_len, const char* dren, uint32_t dren_len,
+                                           const char* const* rkeys, const uint32_t* rkey_lens, uint32_t rnkeys,
+                                           const char* rsrc, uint32_t rsrc_len, const char* rren, uint32_t rren_len,
+                                           int rkeep_fail, int rkeep_succeed, int rcopy_raw, int rwhole_line,
+                                           LcDelimRegexSlsCfg* c) {
+    auto eq = [](const char* a, uint32_t la, const char* b, uint32_t lb) {
+        return la == lb && (la == 0 || !memcmp(a, b, la));
+    };
+    auto is_skip = [&](uint32_t j) {
+        return d.mode == LC_DELIM_SLS_DISCARD && dkey_lens[j] == 1 && dkeys[j][0] == '_';
+    };
+    c->col = LC_DELIM_SLS_NONE;
+    for (uint32_t j = 0; j < d.nkeys; ++j)
+        if (!is_skip(j) && eq(dkeys[j], dkey_lens[j], rsrc, rsrc_len))
+            c->col = j;
+    if (c->col == LC_DELIM_SLS_NONE)
+        return "the regex SourceKey is not one of the delimiter's keys";
+    // a content the delimiter stage may leave under `name`, other than key k's
+    auto left = [&](const char* name, uint32_t len) {
+        uint32_t idx;
+        if (eq(name, len, rsrc, rsrc_len))
+            return false;
+        for (uint32_t j = 0; j < d.nkeys; ++j)
+            if (!is_skip(j) && eq(dkeys[j], dkey_lens[j], name, len))
+                return true;
+        return eq(name, len, dsrc, dsrc_len) || ((d.keep_fail || d.keep_succeed) && eq(name, len, dren, dren_len)) ||
+               (d.keep_fail && d.copy_raw && eq(name, len, "__raw_log__", 11)) ||
+               (d.mode != LC_DELIM_SLS_DISCARD && lc_delim_column_form(name, len, &idx));
+    };
+    bool clash = false;
+    if (rwhole_line)
+        clash = rnkeys ? left(rkeys[0], rkey_lens[0]) : left("content", 7);
+    else
+        for (uint32_t j = 0; j < rnkeys; ++j)
+            clash = clash || left(rkeys[j], rkey_lens[j]);
+    clash = clash || ((rkeep_fail || rkeep_succeed) && left(rren, rren_len)) ||
+            (rkeep_fail && rcopy_raw && left("__raw_log__", 11));
+    if (clash)
+        return "a regex key, RenamedSourceKey or __raw_log__ names a content the delimiter stage may leave besides the "
+               "regex SourceKey";
+    if (!rkeep_fail && left("_time_", 6) && left("_source_", 8))
+        return "_time_ and _source_ may both be left by the delimiter stage (the regex failure's erase rule)";
+    c->src_is_k = d.src_col == c->col;
+    c->ren_is_k = d.ren_col == c->col;
+    c->raw_is_k = eq(dkeys[c->col], dkey_lens[c->col], "__raw_log__", 11);
     return nullptr;
 }
 

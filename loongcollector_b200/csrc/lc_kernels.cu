@@ -3692,6 +3692,121 @@ void launch_delim_sls_emit(const LcDelimSlsCfg& c, const DelimSlsTables& t, cons
                                                                                  d_body_size, d_out);
 }
 
+// ---- f4, delimiter -> regex chain: the value tap (one thread per row; a row with doubled quotes in key k's column
+// copies the collapsed value to its side slot, the common row only reads its table entries) and the Log records
+// (lc_exec.cuh: lc_delim_regex_sls_body -- the size pass one thread per event, the emit pass one warp per event).
+__global__ void __launch_bounds__(256)
+    delim_regex_tap_size_kernel(LcDelimRegexSlsCfg c, DelimSlsTables t, uint64_t n, uint32_t* __restrict__ copy) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n)
+        copy[i] = lc_delim_regex_tap(c, delim_sls_row(c.d, t, nullptr, nullptr, i)).copy;
+}
+
+__global__ void __launch_bounds__(256)
+    delim_regex_tap_kernel(LcDelimRegexSlsCfg c, DelimSlsTables t, uint64_t n, const uint64_t* __restrict__ slot,
+                           uint64_t side_at, uint8_t* base, uint32_t* __restrict__ val_off,
+                           uint32_t* __restrict__ val_len) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n)
+        return;
+    const LcDelimSlsRow r = delim_sls_row(c.d, t, nullptr, nullptr, i);
+    const LcDrTap v = lc_delim_regex_tap(c, r);
+    uint32_t off = v.off;
+    if (v.copy) {
+        off = (uint32_t)(side_at + slot[i]);
+        lc_delim_regex_copy(c, base, r, base + off, v.copy);
+    }
+    val_off[i] = off;
+    val_len[i] = v.len;
+}
+
+__device__ __forceinline__ LcDelimRegexSlsRow delim_regex_sls_row(const LcDelimRegexSlsCfg& c,
+                                                                  const DelimRegexSlsTables& t, const uint32_t* ev_time,
+                                                                  const uint32_t* ev_ns, uint64_t i) {
+    LcDelimRegexSlsRow r;
+    r.d = delim_sls_row(c.d, t.d, ev_time, ev_ns, i);
+    r.vo = t.val_off[i];
+    r.vl = t.val_len[i];
+    r.status = t.status ? t.status[i] : 0u;
+    r.co = t.cap_off ? t.cap_off + i * c.x.pitch : nullptr;
+    r.cl = t.cap_len ? t.cap_len + i * c.x.pitch : nullptr;
+    return r;
+}
+
+__global__ void __launch_bounds__(256)
+    delim_regex_sls_size_kernel(LcDelimRegexSlsCfg c, DelimRegexSlsTables t, const uint32_t* __restrict__ ev_ns,
+                                uint64_t n, uint32_t* __restrict__ rec_size, uint32_t* __restrict__ body_size,
+                                unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    LcDelimRegexVerdict v = {};
+    if (i < n) {
+        const LcDelimRegexSlsRow r = delim_regex_sls_row(c, t, nullptr, ev_ns, i);
+        LcSlsCount s{0};
+        const uint32_t cnt = lc_delim_regex_sls_body(c, t.d.base, r, s);
+        const uint32_t body = cnt ? s.n : 0u;
+        rec_size[i] = cnt ? 1 + lc_varint_size(body) + body : 0u;
+        body_size[i] = body;
+        v = lc_delim_regex_verdict(c, r, cnt);
+    }
+    if (counters) { // one atomic per warp and counter
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const uint32_t w = __reduce_add_sync(0xFFFFFFFFu, v.ctr[k]);
+            if ((threadIdx.x & 31) == 0 && w)
+                atomicAdd(counters + k, (unsigned long long)w);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    delim_regex_sls_emit_kernel(LcDelimRegexSlsCfg c, DelimRegexSlsTables t, const uint32_t* __restrict__ ev_time,
+                                const uint32_t* __restrict__ ev_ns, uint64_t n, const uint64_t* __restrict__ rec_off,
+                                const uint32_t* __restrict__ body_size, uint8_t* __restrict__ out) {
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n)
+        return;
+    const uint32_t body = body_size[i];
+    if (!body)
+        return; // erased or LogEvent::Empty: no record (SLSSerializer.cpp:383-385)
+    const LcDelimRegexSlsRow r = delim_regex_sls_row(c, t, ev_time, ev_ns, i);
+    uint8_t h[6];
+    h[0] = 0x0A;
+    const uint32_t hn = 1 + lc_put_varint(h + 1, body);
+    LcSlsWrite s{out + rec_off[i], 0u, hn + body, threadIdx.x & 31, 32};
+    s.put(h, hn);
+    lc_delim_regex_sls_body(c, t.d.base, r, s);
+}
+
+void launch_delim_regex_tap_sizes(const LcDelimRegexSlsCfg& c, const DelimSlsTables& t, uint64_t n, uint32_t* d_copy,
+                                  cudaStream_t st) {
+    if (n)
+        delim_regex_tap_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, n, d_copy);
+}
+
+void launch_delim_regex_tap(const LcDelimRegexSlsCfg& c, const DelimSlsTables& t, uint64_t n, const uint64_t* d_slot,
+                            uint64_t side_at, uint8_t* d_base, uint32_t* d_val_off, uint32_t* d_val_len,
+                            cudaStream_t st) {
+    if (n)
+        delim_regex_tap_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, n, d_slot, side_at, d_base,
+                                                                             d_val_off, d_val_len);
+}
+
+void launch_delim_regex_sls_sizes(const LcDelimRegexSlsCfg& c, const DelimRegexSlsTables& t, const uint32_t* d_ev_ns,
+                                  uint64_t n, uint32_t* d_rec_size, uint32_t* d_body_size,
+                                  unsigned long long* d_counters, cudaStream_t st) {
+    if (n)
+        delim_regex_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, d_ev_ns, n, d_rec_size,
+                                                                                  d_body_size, d_counters);
+}
+
+void launch_delim_regex_sls_emit(const LcDelimRegexSlsCfg& c, const DelimRegexSlsTables& t, const uint32_t* d_ev_time,
+                                 const uint32_t* d_ev_ns, uint64_t n, const uint64_t* d_rec_off,
+                                 const uint32_t* d_body_size, uint8_t* d_out, cudaStream_t st) {
+    if (n)
+        delim_regex_sls_emit_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, t, d_ev_time, d_ev_ns, n,
+                                                                                       d_rec_off, d_body_size, d_out);
+}
+
 // ---- f4, split-fed: Log records of the pieces a splitter cuts from one source value (lc_exec.cuh: lc_span_sls_rec,
 // lc_span_sls_tile).  The size pass runs one thread per piece; the emit pass one warp per kSpanTile bytes of OUTPUT,
 // so records of 0 B and of many MiB share a launch without one warp copying a whole long record.

@@ -6,6 +6,7 @@
 
 struct LcDelimSlsCfg; // lc_exec.cuh
 struct LcRegexSlsCfg;
+struct LcDelimRegexSlsCfg;
 struct LcSpanSlsCfg;
 struct LcLz4Seq;
 struct LcLz4Chunk;
@@ -237,6 +238,31 @@ void launch_delim_sls_sizes(const LcDelimSlsCfg& c, const DelimSlsTables& t, con
 void launch_delim_sls_emit(const LcDelimSlsCfg& c, const DelimSlsTables& t, const uint32_t* d_ev_time,
                            const uint32_t* d_ev_ns, uint64_t n, const uint64_t* d_rec_off, const uint32_t* d_body_size,
                            uint8_t* d_out, cudaStream_t st);
+
+// f4, delimiter -> regex chain (lc_exec.cuh: LcDelimRegexSlsCfg).  launch_delim_regex_tap_sizes: d_copy[i] = bytes of
+// row i's side copy (0 = none).  launch_delim_regex_tap: the value table (d_val_off, d_val_len) of every row; a row
+// with a copy gets it at d_base[side_at + d_slot[i], + d_copy[i]) (d_slot = exclusive sum of d_copy).  The sizes and
+// emit passes as for launch_sls_sizes over the delimiter tables, the value table and the regex tables over it
+// (status / captures nullptr in whole-line mode); d_counters (or nullptr): u64 [8] += lc_delim_regex_verdict.
+struct DelimRegexSlsTables {
+    DelimSlsTables d;
+    const uint32_t* val_off;
+    const uint32_t* val_len;
+    const uint8_t* status;
+    const uint32_t* cap_off; // [n][pitch]
+    const uint32_t* cap_len;
+};
+void launch_delim_regex_tap_sizes(const LcDelimRegexSlsCfg& c, const DelimSlsTables& t, uint64_t n, uint32_t* d_copy,
+                                  cudaStream_t st);
+void launch_delim_regex_tap(const LcDelimRegexSlsCfg& c, const DelimSlsTables& t, uint64_t n, const uint64_t* d_slot,
+                            uint64_t side_at, uint8_t* d_base, uint32_t* d_val_off, uint32_t* d_val_len,
+                            cudaStream_t st);
+void launch_delim_regex_sls_sizes(const LcDelimRegexSlsCfg& c, const DelimRegexSlsTables& t, const uint32_t* d_ev_ns,
+                                  uint64_t n, uint32_t* d_rec_size, uint32_t* d_body_size,
+                                  unsigned long long* d_counters, cudaStream_t st);
+void launch_delim_regex_sls_emit(const LcDelimRegexSlsCfg& c, const DelimRegexSlsTables& t, const uint32_t* d_ev_time,
+                                 const uint32_t* d_ev_ns, uint64_t n, const uint64_t* d_rec_off,
+                                 const uint32_t* d_body_size, uint8_t* d_out, cudaStream_t st);
 
 // f4, split-fed: Log records of the pieces of one source value (lc_exec.cuh: LcSpanSlsCfg, keys on the device).
 // rec_size[k] = bytes of piece k's record (never 0); the emit pass writes the `total` bytes from the record offsets,

@@ -2186,6 +2186,127 @@ bool ProcessorParseDelimiterNative::SerializeSlsImpl(PipelineEventGroup& group, 
     return rawSize ? ok : FinishSls(ser, n, ctr[2], need, res, tail, out, err);
 }
 
+bool ProcessorParseDelimiterNative::SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                                                 bool enableNs, std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+}
+
+bool ProcessorParseDelimiterNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                                                    bool enableNs, std::string& block, uint64_t& rawSize,
+                                                    std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+}
+
+// out = the wire bytes (rawSize null) or their LZ4 block (rawSize = their size)
+bool ProcessorParseDelimiterNative::ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                                                      bool enableNs, std::string& out, uint64_t* rawSize,
+                                                      std::string& err) {
+    SLSEventGroupSerializer ser;
+    ser.mEnableTimestampNanosecond = enableNs;
+    std::vector<const char*> kp, rkp;
+    std::vector<uint32_t> kl, rkl;
+    size_t keyBytes = 0;
+    for (const auto& k : mKeys) {
+        kp.push_back(k.data());
+        kl.push_back((uint32_t)k.size());
+        keyBytes += k.size();
+    }
+    for (const auto& k : next.mKeys) {
+        rkp.push_back(k.data());
+        rkl.push_back((uint32_t)k.size());
+        keyBytes += k.size();
+    }
+    const std::string& renamed = mCommonParserOptions.mRenamedSourceKey;
+    const std::string& rrenamed = next.mCommonParserOptions.mRenamedSourceKey;
+    const CommonParserOptions& ro = next.mCommonParserOptions;
+    // the chain's own checks (lc_delim_regex_sls_link), on top of this processor's (mDeviceSls)
+    bool accepted = false;
+    if (mDeviceSls) {
+        std::vector<uint8_t> kb(keyBytes + mSourceKey.size() + renamed.size() + 12);
+        std::vector<uint32_t> at(mKeys.size() + 4), plan(3 * next.mKeys.size() + 12);
+        LcDelimRegexSlsCfg c;
+        accepted =
+            !lc_delim_sls_setup(reinterpret_cast<const uint8_t*>(mSeparator.data()), (uint32_t)mSeparator.size(),
+                                (uint8_t)mQuote, mOverflowedFieldsTreatment == OverflowedFieldsTreatment::EXTEND,
+                                mExtractingPartialFields, kp.data(), kl.data(), (uint32_t)mKeys.size(),
+                                mSourceKey.data(), (uint32_t)mSourceKey.size(), renamed.data(),
+                                (uint32_t)renamed.size(), mCommonParserOptions.mKeepingSourceWhenParseFail,
+                                mCommonParserOptions.mKeepingSourceWhenParseSucceed,
+                                mCommonParserOptions.mCopingRawLog, (uint32_t)mKeys.size() + 16, &c.d, kb.data(),
+                                at.data()) &&
+            !lc_regex_sls_setup(rkp.data(), rkl.data(), (uint32_t)next.mKeys.size(), next.mSourceKey.data(),
+                                (uint32_t)next.mSourceKey.size(), rrenamed.data(), (uint32_t)rrenamed.size(),
+                                ro.mKeepingSourceWhenParseFail, ro.mKeepingSourceWhenParseSucceed, ro.mCopingRawLog,
+                                next.mIsWholeLineMode, 0, &c.x, plan.data()) &&
+            !lc_delim_regex_sls_link(c.d, kp.data(), kl.data(), mSourceKey.data(), (uint32_t)mSourceKey.size(),
+                                     renamed.data(), (uint32_t)renamed.size(), rkp.data(), rkl.data(),
+                                     (uint32_t)next.mKeys.size(), next.mSourceKey.data(),
+                                     (uint32_t)next.mSourceKey.size(), rrenamed.data(), (uint32_t)rrenamed.size(),
+                                     ro.mKeepingSourceWhenParseFail, ro.mKeepingSourceWhenParseSucceed,
+                                     ro.mCopingRawLog, next.mIsWholeLineMode, &c);
+    }
+    if (!accepted || !IsFlatSlsGroup(group, mSourceKey)) {
+        Process(group);
+        next.Process(group);
+        if (!rawSize)
+            return ser.Serialize(group, out, err);
+        std::string raw;
+        const bool ok = ser.Serialize(group, raw, err);
+        return CompressSls(ok, raw, out, *rawSize, err);
+    }
+    // every event is SourceKey -> line: both stages and the serialiser in one device pass
+    const size_t n = group.GetEvents().size();
+    FlatBatch batch;
+    std::vector<uint32_t> evTime, evNs;
+    GatherFlatSls(group, enableNs, batch, evTime, evNs);
+    std::string res;
+    uint64_t need = 0, ctr[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    const std::string tail = SlsGroupTail(group);
+    const size_t estimate =
+        (size_t)(2 * batch.baseLen + n * (64 + keyBytes + renamed.size() + rrenamed.size()) + 64);
+    // the arguments both device calls share, up to whole_line
+    auto args = [&](auto fn, auto... rest) {
+        return fn(Engine(), next.mIsWholeLineMode ? nullptr : next.mReg.get(), batch.base, batch.baseLen,
+                  batch.off.data(), batch.len.data(), n, evTime.data(), evNs.data(), mAllowingShortenedFields,
+                  (uint32_t)mKeys.size() + 16, reinterpret_cast<const uint8_t*>(mSeparator.data()),
+                  (uint32_t)mSeparator.size(), (uint8_t)mQuote,
+                  mOverflowedFieldsTreatment == OverflowedFieldsTreatment::EXTEND, mExtractingPartialFields,
+                  kp.data(), kl.data(), (uint32_t)mKeys.size(), mSourceKey.data(), (uint32_t)mSourceKey.size(),
+                  renamed.data(), (uint32_t)renamed.size(), mCommonParserOptions.mKeepingSourceWhenParseFail,
+                  mCommonParserOptions.mKeepingSourceWhenParseSucceed, mCommonParserOptions.mCopingRawLog,
+                  rkp.data(), rkl.data(), (uint32_t)next.mKeys.size(), next.mSourceKey.data(),
+                  (uint32_t)next.mSourceKey.size(), rrenamed.data(), (uint32_t)rrenamed.size(),
+                  ro.mKeepingSourceWhenParseFail, ro.mKeepingSourceWhenParseSucceed, ro.mCopingRawLog,
+                  next.mIsWholeLineMode, rest...);
+    };
+    uint64_t erased = 0; // events either stage erased
+    bool ok;
+    if (rawSize) {
+        ok = RunSlsLz4DevicePass(
+            [&](uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw) {
+                const int rc = args(lc_delim_regex_parse_sls_lz4, reinterpret_cast<const uint8_t*>(tail.data()),
+                                    (uint64_t)tail.size(), o, cap, len, raw, ctr);
+                erased = ctr[2] + ctr[7];
+                return rc;
+            },
+            estimate + tail.size(), ser, n, erased, tail.size(), out, *rawSize, err, "lc_delim_regex_parse_sls_lz4");
+    } else {
+        RunSlsDevicePass(
+            [&](uint8_t* o, uint64_t cap, uint64_t* len) { return args(lc_delim_regex_parse_sls, o, cap, len, ctr); },
+            estimate, tail.size(), ser.mMaxSendLogGroupSize, res, need, "lc_delim_regex_parse_sls");
+        erased = ctr[2] + ctr[7];
+    }
+    // the counters both Process calls would have moved (a blank value counts as out_failed, :220-242)
+    mOutSuccessfulEventsTotal.Add(ctr[0]);
+    mOutFailedEventsTotal.Add(ctr[1] + ctr[3]);
+    mDiscardedEventsTotal.Add(ctr[2]);
+    next.mOutSuccessfulEventsTotal.Add(ctr[4]);
+    next.mOutFailedEventsTotal.Add(ctr[5]);
+    next.mOutKeyNotFoundEventsTotal.Add(ctr[6]);
+    next.mDiscardedEventsTotal.Add(ctr[7]);
+    return rawSize ? ok : FinishSls(ser, n, erased, need, res, tail, out, err);
+}
+
 bool ProcessorParseRegexNative::SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out,
                                              std::string& err) {
     return SerializeSlsImpl(group, enableNs, out, nullptr, err);

@@ -210,6 +210,7 @@ private:
     void EpilogueGroup(PipelineEventGroup& group, uint64_t firstEv, const struct ThreadScratch& sc, uint32_t G,
                        LocalCounters& c) const;
     void AddCounters(const LocalCounters& c);
+    friend class ProcessorParseDelimiterNative; // the delimiter -> regex chain's SerializeSls
     bool mSourceKeyOverwritten = false;
     bool mIsWholeLineMode = false;
     bool mKeysDistinct = false; // no key repeats: an event that holds only the source key takes the parsed fields as
@@ -248,6 +249,16 @@ public:
     // SerializeSls followed by LZ4Compressor::Compress, as for ProcessorParseRegexNative (lc_delim_parse_sls_lz4).
     bool SerializeSlsLz4(PipelineEventGroup& group, bool enableNs, std::string& block, uint64_t& rawSize,
                          std::string& err);
+    // Process(group), then next.Process(group) (next: the regex processor behind this one in the pipeline, parsing one
+    // of this processor's keys), then SLSEventGroupSerializer::Serialize: the same bytes or error message, and the same
+    // counter updates on both processors.  On a flat group without log.file.offset metadata and a chain
+    // lc_delim_regex_parse_sls accepts, both stages run in one device pass and only the wire bytes come back; the
+    // group's events are left as they were.  Otherwise the three calls run.
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs, std::string& out,
+                      std::string& err);
+    // The same followed by LZ4Compressor::Compress, as SerializeSlsLz4 (lc_delim_regex_parse_sls_lz4).
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs, std::string& block,
+                         uint64_t& rawSize, std::string& err);
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
@@ -255,6 +266,8 @@ protected:
 private:
     bool SerializeSlsImpl(PipelineEventGroup& group, bool enableNs, std::string& out, uint64_t* rawSize,
                           std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs,
+                           std::string& out, uint64_t* rawSize, std::string& err);
     bool mSourceKeyOverwritten = false;
     bool mDeviceSls = false; // the configuration passes lc_delim_parse_sls's checks
 };
