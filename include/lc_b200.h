@@ -386,6 +386,73 @@ int lc_multiline_split_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, con
                            uint32_t time, uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
                            uint64_t* n_events, uint64_t counters[3]);
 
+/* ---- f4: the split -> regex chain (ProcessorSplitLogStringNative or ProcessorSplitMultilineLogStringNative, then
+ * ProcessorParseRegexNative with the same SourceKey -- BASELINE configs C2 / C3 on file input) to the SLS wire format.
+ * The source event is flat: source_key -> the value, with its position src_pos, time and time_ns (LC_SLS_NO_NS = no
+ * Time_ns).  Piece k enters the regex stage as [source_key -> piece] or, when offset_key != NULL (log.file.offset
+ * metadata; an empty key is still a key), [source_key -> piece, offset_key -> decimal(src_pos + off[k])].  The regex
+ * stage then runs as for lc_sls_serialize_regex_dev (keys .. whole_line), on that event: a regex key equal to
+ * offset_key overwrites the digits in place; renamed_key or "__raw_log__" equal to offset_key is not added (the key is
+ * present); a failed piece without keep_fail is erased (ShouldEraseEvent, CommonParserOptions.cpp:107-110).
+ * counters[3] (may be NULL) = ProcessorParseRegexNative's out_successful, out_failed (LC_REGEX_NOMATCH) and discarded.
+ * Refused with LC_ERR_INVALID_ARG: offset_key equal to source_key, and lc_sls_serialize_regex_dev's refusals.
+ * LC_ERR_TOO_LARGE when src_len plus the key bytes reach 4 GiB, or a record would.
+ *
+ * lc_sls_serialize_split_regex_dev: from the DEVICE piece tables of one lc_split_lines_dev / lc_multiline_split_dev
+ * call over d_src[0, src_len) and the DEVICE tables of lc_regex_parse_dev over those pieces (d_status, [n][row_pitch]
+ * d_cap_off / d_cap_len; NULL in whole-line mode).  d_out receives the bytes; *out_len (host) their count;
+ * LC_ERR_CAPACITY if > out_cap (nothing written, *out_len and counters set). */
+int lc_sls_serialize_split_regex_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+                                     const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                     const uint32_t* d_cap_off, const uint32_t* d_cap_len, uint32_t row_pitch,
+                                     const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                                     const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                                     uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                                     int whole_line, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+                                     uint32_t time, uint32_t time_ns, uint8_t* d_out, uint64_t out_cap,
+                                     uint64_t* out_len, uint64_t counters[3]);
+
+/* The same with a HOST source value: upload it once, split it on the device (lc_split_lines / lc_multiline_split
+ * rules), run lc_regex_parse_dev over the pieces (re may be NULL in whole-line mode), serialise, and bring back only
+ * the wire bytes.  *n_events (may be NULL) = number of pieces; the multiline calls add the splitter's counters to
+ * ml_counters[3] (may be NULL) as lc_multiline_split does.  *out_len, *n_events and the counters are set on LC_OK and
+ * on LC_ERR_CAPACITY.  The _lz4 variants put tail[0, tail_len) behind the records and return ONE LZ4 block, as
+ * lc_regex_parse_sls_lz4 does (*raw_len = records + tail bytes). */
+int lc_split_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                             uint8_t split_char, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                             const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                             uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, int whole_line,
+                             const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+                             uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                             uint64_t counters[3]);
+int lc_split_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                 uint8_t split_char, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                                 const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                                 uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                                 int whole_line, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+                                 uint32_t time, uint32_t time_ns, const uint8_t* tail, uint64_t tail_len,
+                                 uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+                                 uint64_t* n_events, uint64_t counters[3]);
+int lc_multiline_split_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                       const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                       int discard_unmatched, const char* const* keys, const uint32_t* key_lens,
+                                       uint32_t nkeys, const char* source_key, uint32_t source_key_len,
+                                       const char* renamed_key, uint32_t renamed_key_len, int keep_fail,
+                                       int keep_succeed, int copy_raw, int whole_line, const char* offset_key,
+                                       uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                       uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                       uint64_t counters[3], uint64_t ml_counters[3]);
+int lc_multiline_split_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                           const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                           int discard_unmatched, const char* const* keys, const uint32_t* key_lens,
+                                           uint32_t nkeys, const char* source_key, uint32_t source_key_len,
+                                           const char* renamed_key, uint32_t renamed_key_len, int keep_fail,
+                                           int keep_succeed, int copy_raw, int whole_line, const char* offset_key,
+                                           uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                           const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+                                           uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                                           uint64_t counters[3], uint64_t ml_counters[3]);
+
 /* lc_regex_parse_sls / lc_delim_parse_sls finished as the SLS flusher finishes a group: the records, followed by
  * tail[0, tail_len) (the group-level fields: topic, source, machine uuid, tags), become ONE LZ4 block (the block format
  * of lc_lz4_compress_dev) and only the block comes back.  *raw_len = records + tail bytes (x-log-bodyrawsize),

@@ -1747,12 +1747,31 @@ int lc_sls_serialize_logs(lc_engine_t* e, const uint8_t* base, uint64_t base_len
 // ------------------------------------------------------------------------------------------------ processor -> SLS
 namespace {
 
-// Serialise from device tables (lc_sls_serialize_delim_dev / _regex_dev / _parsed_dev): `sizes(rec_size, body_size,
-// d_counters)` queues the size pass, an exclusive sum gives the record offsets, `emit(rec_off, body_size, d_out)`
-// queues the emit pass.  counters (host, or nullptr) receive the ncounters device counters of the size pass.
+// The fused LZ4 calls (lc_regex_parse_sls_lz4, lc_delim_parse_sls_lz4): the group-level fields that follow the
+// records, and where the records' size plus theirs goes
+struct Lz4Tail {
+    const uint8_t* tail;
+    uint64_t len;
+    uint64_t* raw_len;
+};
+int lz4_one_block(lc_engine_t* e, const char* what, const uint8_t* d_src, uint64_t raw, uint8_t* out, uint64_t out_cap,
+                  uint64_t* out_len);
+
+// Where serialize_sls_dev's records go besides d_out, and a counter that refuses the call
+struct SlsTo {
+    uint8_t* host = nullptr;    // d_out == nullptr: the records are staged in `lab` and copied back here
+    const Lz4Tail* z = nullptr; // records ‖ z->tail become one LZ4 block, copied back to `host`
+    int too_large = -1;         // counter k > 0: a record would reach 4 GiB, LC_ERR_TOO_LARGE
+};
+
+// Serialise from device tables (lc_sls_serialize_delim_dev / _regex_dev / _parsed_dev / _split_regex_dev and the
+// split -> regex host calls): `sizes(rec_size, body_size, d_counters)` queues the size pass, an exclusive sum gives the
+// record offsets, `emit(rec_off, body_size, d_out)` queues the emit pass.  counters (host, or nullptr) receive the
+// ncounters device counters of the size pass.  `to` (host copy, LZ4 block, refusing counter) as SlsTo says; with z,
+// out_cap and *out_len are the block's.
 template <class Sizes, class Emit>
 int serialize_sls_dev(lc_engine_t* e, const char* what, uint64_t n, uint32_t ncounters, Sizes sizes, Emit emit,
-                      uint8_t* d_out, uint64_t out_cap, uint64_t* out_len, uint64_t* counters) {
+                      uint8_t* d_out, uint64_t out_cap, uint64_t* out_len, uint64_t* counters, const SlsTo& to = {}) {
     CU_TRY(e->lab_sizes.ensure(n * 4));
     CU_TRY(e->cnt.ensure(n * 4));
     CU_TRY(e->lab_off.ensure(n * 8));
@@ -1780,29 +1799,42 @@ int serialize_sls_dev(lc_engine_t* e, const char* what, uint64_t n, uint32_t nco
     CU_TRY(cudaStreamSynchronize(e->stream));
     for (uint32_t k = 0; d_ctr && k < ncounters; ++k)
         counters[k] = ctr[k];
-    *out_len = hs->total;
-    if (hs->total > out_cap)
+    if (to.too_large >= 0 && ctr[to.too_large])
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": a record would reach 4 GiB");
+    const uint64_t total = hs->total;
+    if (to.z) {
+        const uint64_t raw = total + to.z->len;
+        *to.z->raw_len = raw;
+        if (raw > LC_LZ4_MAX_INPUT)
+            return fail(LC_ERR_TOO_LARGE, std::string(what) + ": records and tail are larger than LZ4_MAX_INPUT_SIZE");
+        CU_TRY(e->lab.ensure(raw + 16));
+        if (total) {
+            emit(e->lab_off.as<uint64_t>(), e->cnt.as<uint32_t>(), e->lab.as<uint8_t>());
+            e->launches++;
+            CU_TRY(cudaGetLastError());
+        }
+        if (to.z->len)
+            CU_TRY(cudaMemcpyAsync(e->lab.as<uint8_t>() + total, to.z->tail, to.z->len, cudaMemcpyHostToDevice,
+                                   e->stream));
+        return lz4_one_block(e, what, e->lab.as<uint8_t>(), raw, to.host, out_cap, out_len);
+    }
+    *out_len = total;
+    if (total > out_cap)
         return fail(LC_ERR_CAPACITY, std::string(what) + ": output capacity too small");
-    if (hs->total == 0)
+    if (total == 0)
         return LC_OK;
-    if (!d_out)
+    if (!d_out && !to.host)
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
-    emit(e->lab_off.as<uint64_t>(), e->cnt.as<uint32_t>(), d_out);
+    if (!d_out)
+        CU_TRY(e->lab.ensure(total));
+    emit(e->lab_off.as<uint64_t>(), e->cnt.as<uint32_t>(), d_out ? d_out : e->lab.as<uint8_t>());
     e->launches++;
     CU_TRY(cudaGetLastError());
+    if (!d_out)
+        CU_TRY(cudaMemcpyAsync(to.host, e->lab.p, total, cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(cudaStreamSynchronize(e->stream));
     return LC_OK;
 }
-
-// The fused LZ4 calls (lc_regex_parse_sls_lz4, lc_delim_parse_sls_lz4): the group-level fields that follow the
-// records, and where the records' size plus theirs goes
-struct Lz4Tail {
-    const uint8_t* tail;
-    uint64_t len;
-    uint64_t* raw_len;
-};
-int lz4_one_block(lc_engine_t* e, const char* what, const uint8_t* d_src, uint64_t raw, uint8_t* out, uint64_t out_cap,
-                  uint64_t* out_len);
 
 // a fused call without events: the block of the tail alone
 int lz4_tail_only(lc_engine_t* e, const char* what, const Lz4Tail& z, uint8_t* out, uint64_t out_cap,
@@ -2719,6 +2751,238 @@ int lc_multiline_split_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, con
     return split_sls_host(e, "lc_multiline_split_sls", buf, len, split, key, key_len, offset_key, offset_key_len,
                           src_pos, time, time_ns, out, out_cap, out_len, n_events);
 }
+
+} // extern "C"
+
+// ------------------------------------------------------------------------------------------------ split -> regex -> SLS
+// The regex stage's configuration and the offset content of the split events (CHAIN_PARAMS's regex half, plus
+// offset_key -- NULL = no log.file.offset metadata -- and the source event's position, time and ns)
+#define SPLIT_REGEX_PARAMS                                                                                             \
+    const char *const *keys, const uint32_t *key_lens, uint32_t nkeys, const char *source_key,                         \
+        uint32_t source_key_len, const char *renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed,   \
+        int copy_raw, int whole_line, const char *offset_key, uint32_t offset_key_len, uint64_t src_pos,              \
+        uint32_t time, uint32_t time_ns
+#define SPLIT_REGEX_ARGS                                                                                               \
+    keys, key_lens, nkeys, source_key, source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed,          \
+        copy_raw, whole_line, offset_key, offset_key_len, src_pos, time, time_ns
+
+namespace {
+
+// lc_split_regex_sls_setup's plans over the key table keys..., SourceKey, RenamedSourceKey, "__raw_log__", "content",
+// offset_key, staged on the device (`sls_plan`, which neither splitter nor the regex stage uses).  Every single
+// content then stays below 4 GiB; a record that would not is caught by the size pass.
+int split_regex_sls_config(lc_engine_t* e, const char* what, uint64_t src_len, SPLIT_REGEX_PARAMS, uint32_t pitch,
+                           LcSplitRegexSlsCfg* c) {
+    if ((nkeys && (!keys || !key_lens)) || (source_key_len && !source_key) || (renamed_key_len && !renamed_key))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    uint64_t kbytes = (uint64_t)source_key_len + renamed_key_len + (offset_key ? offset_key_len : 0u) + 18;
+    for (uint32_t k = 0; k < nkeys; ++k) {
+        if (key_lens[k] && !keys[k])
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+        kbytes += key_lens[k];
+    }
+    if (src_len + kbytes + 96 > 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": source value and keys must stay below 4 GiB");
+    std::vector<uint32_t> plan(3 * (size_t)nkeys + 24);
+    const char* why = lc_split_regex_sls_setup(keys, key_lens, nkeys, source_key, source_key_len, renamed_key,
+                                               renamed_key_len, offset_key, offset_key_len, keep_fail, keep_succeed,
+                                               copy_raw, whole_line, pitch, src_pos, time, time_ns, c, plan.data());
+    if (why)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    std::vector<const char*> strings(keys, keys + nkeys);
+    std::vector<uint32_t> lens(key_lens, key_lens + nkeys);
+    strings.insert(strings.end(), {source_key, renamed_key, "__raw_log__", "content", offset_key});
+    lens.insert(lens.end(), {source_key_len, renamed_key_len, 11u, 7u, offset_key ? offset_key_len : 0u});
+    return stage_regex_sls(e, what, plan.data(), strings.data(), lens.data(), nkeys + 5, &c->x);
+}
+
+// The size pass and the emit of the chain over n pieces (serialize_sls_dev): into d_out (the device-fed call), or
+// back to the host buffer out, or -- with z -- records ‖ tail as one LZ4 block.  counters[3] = successful, failed,
+// discarded; set whenever the size pass ran.
+int split_regex_sls_run(lc_engine_t* e, const char* what, const LcSplitRegexSlsCfg& c, const lck::RegexSlsTables& t,
+                        uint64_t n, uint8_t* d_out, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                        uint64_t counters[3], const Lz4Tail* z) {
+    uint64_t ctr[4] = {0, 0, 0, 0}; // + pieces whose record would reach 4 GiB
+    SlsTo to;
+    to.host = out;
+    to.z = z;
+    to.too_large = 3;
+    const int rc = serialize_sls_dev(
+        e, what, n, 4,
+        [&](uint32_t* rec, uint32_t* body, unsigned long long* d_ctr) {
+            lck::launch_split_regex_sls_sizes(c, t, n, rec, body, d_ctr, e->stream);
+        },
+        [&](const uint64_t* rec_off, const uint32_t* body, uint8_t* dst) {
+            lck::launch_split_regex_sls_emit(c, t, n, rec_off, body, dst, e->stream);
+        },
+        d_out, out_cap, out_len, ctr, to);
+    memcpy(counters, ctr, 3 * sizeof(uint64_t));
+    return rc;
+}
+
+// Host-buffer split + regex + serialise (lc_split_regex_parse_sls and the multiline / LZ4 siblings): the source goes
+// up once into `in`, `split(&n)` cuts it into the piece tables out_a / out_b (and out_c flags), the regex stage runs
+// over them into dr_status / dr_cap_off / dr_cap_len, and only the wire bytes (or their LZ4 block) come back.
+template <class Split>
+int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                         Split split, SPLIT_REGEX_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                         uint64_t* n_events, uint64_t counters[3], const Lz4Tail* z) {
+    if (!e || (!re && !whole_line) || !out_len || (len && !buf) || (z && (!z->raw_len || (z->len && !z->tail))))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (n_events)
+        *n_events = 0;
+    uint64_t ctr[3] = {0, 0, 0};
+    if (counters)
+        memset(counters, 0, 3 * sizeof(uint64_t));
+    if (z)
+        *z->raw_len = 0;
+    int rc = whole_line ? (int)LC_OK : check_regex_usable(re, what);
+    if (rc)
+        return rc;
+    if (len >= 0xFFFFFFF0ull)
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB per call");
+    rc = bind(e);
+    if (rc)
+        return rc;
+    const uint32_t G = whole_line ? 0u : re->res.ngroups;
+    LcSplitRegexSlsCfg c;
+    rc = split_regex_sls_config(e, what, len, SPLIT_REGEX_ARGS, G, &c);
+    if (rc)
+        return rc;
+    uint64_t n = 0;
+    if (len) {
+        CU_TRY(e->in.ensure(len + 16));
+        CU_TRY(e->out_a.ensure((len + 1) * 4));
+        CU_TRY(e->out_b.ensure((len + 1) * 4));
+        CU_TRY(e->out_c.ensure(len + 1));
+        CU_TRY(cudaMemcpyAsync(e->in.p, buf, len, cudaMemcpyHostToDevice, e->stream));
+        rc = split(&n);
+        if (rc)
+            return rc;
+    }
+    if (n_events)
+        *n_events = n;
+    if (n == 0)
+        return z ? lz4_tail_only(e, what, *z, out, out_cap, out_len) : (int)LC_OK;
+    if (n * (uint64_t)G >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^32 captures per call");
+    const bool caps = !whole_line && nkeys && nkeys <= G;
+    if (!whole_line) {
+        CU_TRY(e->dr_status.ensure(n));
+        CU_TRY(e->dr_cap_off.ensure(n * G * 4 + 4));
+        CU_TRY(e->dr_cap_len.ensure(n * G * 4 + 4));
+        rc = regex_parse_dev_impl(e, re, e->in.as<uint8_t>(), len, len, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), 1, n, nkeys, e->dr_status.as<uint8_t>(),
+                                  e->dr_cap_off.as<uint32_t>(), e->dr_cap_len.as<uint32_t>(), false);
+        if (rc)
+            return rc;
+    }
+    const lck::RegexSlsTables t{e->in.as<uint8_t>(), e->out_a.as<uint32_t>(), e->out_b.as<uint32_t>(),
+                                whole_line ? nullptr : e->dr_status.as<uint8_t>(),
+                                caps ? e->dr_cap_off.as<uint32_t>() : nullptr,
+                                caps ? e->dr_cap_len.as<uint32_t>() : nullptr};
+    rc = split_regex_sls_run(e, what, c, t, n, nullptr, out, out_cap, out_len, ctr, z);
+    if (counters)
+        memcpy(counters, ctr, sizeof ctr);
+    return rc;
+}
+
+template <class Split>
+int split_regex_lz4_host(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                         Split split, SPLIT_REGEX_PARAMS, const uint8_t* tail, uint64_t tail_len, uint8_t* out,
+                         uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                         uint64_t counters[3]) {
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return split_regex_sls_host(e, what, re, buf, len, split, SPLIT_REGEX_ARGS, out, out_cap, out_len, n_events,
+                                counters, &z);
+}
+
+} // namespace
+
+extern "C" {
+
+int lc_sls_serialize_split_regex_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+                                     const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                     const uint32_t* d_cap_off, const uint32_t* d_cap_len, uint32_t row_pitch,
+                                     SPLIT_REGEX_PARAMS, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len,
+                                     uint64_t counters[3]) {
+    static const char* what = "lc_sls_serialize_split_regex_dev";
+    const bool caps = !whole_line && nkeys && nkeys <= row_pitch; // the parsed plan reads the capture tables
+    if (!e || !out_len || (n && (!d_src || !d_off || !d_len)) || (n && !whole_line && !d_status) ||
+        (n && caps && (!d_cap_off || !d_cap_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (counters)
+        memset(counters, 0, 3 * sizeof(uint64_t));
+    if (src_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)row_pitch >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 pieces and < 2^32 captures per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcSplitRegexSlsCfg c;
+    rc = split_regex_sls_config(e, what, src_len, SPLIT_REGEX_ARGS, row_pitch, &c);
+    if (rc || n == 0)
+        return rc;
+    const lck::RegexSlsTables t{d_src, d_off, d_len, whole_line ? nullptr : d_status, caps ? d_cap_off : nullptr,
+                                caps ? d_cap_len : nullptr};
+    uint64_t ctr[3] = {0, 0, 0};
+    rc = split_regex_sls_run(e, what, c, t, n, d_out, nullptr, out_cap, out_len, ctr, nullptr);
+    if (counters)
+        memcpy(counters, ctr, sizeof ctr);
+    return rc;
+}
+
+int lc_split_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                             uint8_t split_char, SPLIT_REGEX_PARAMS, uint8_t* out, uint64_t out_cap,
+                             uint64_t* out_len, uint64_t* n_events, uint64_t counters[3]) {
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_regex_sls_host(e, "lc_split_regex_parse_sls", re, buf, len, split, SPLIT_REGEX_ARGS, out, out_cap,
+                                out_len, n_events, counters, nullptr);
+}
+
+int lc_split_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                 uint8_t split_char, SPLIT_REGEX_PARAMS, const uint8_t* tail, uint64_t tail_len,
+                                 uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+                                 uint64_t* n_events, uint64_t counters[3]) {
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_regex_lz4_host(e, "lc_split_regex_parse_sls_lz4", re, buf, len, split, SPLIT_REGEX_ARGS, tail,
+                                tail_len, out, out_cap, out_len, raw_len, n_events, counters);
+}
+
+// (the multiline splitter's own counters[3] are added to ml_counters as lc_multiline_split_dev adds them)
+#define ML_SPLIT                                                                                                       \
+    [&](uint64_t* n) {                                                                                                 \
+        return lc_multiline_split_dev(e, e->in.as<uint8_t>(), len, start, cont, end, discard_unmatched,               \
+                                      e->out_a.as<uint32_t>(), e->out_b.as<uint32_t>(), e->out_c.as<uint8_t>(), len,  \
+                                      n, ml_counters);                                                                 \
+    }
+
+int lc_multiline_split_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                       const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                       int discard_unmatched, SPLIT_REGEX_PARAMS, uint8_t* out, uint64_t out_cap,
+                                       uint64_t* out_len, uint64_t* n_events, uint64_t counters[3],
+                                       uint64_t ml_counters[3]) {
+    return split_regex_sls_host(e, "lc_multiline_split_regex_parse_sls", re, buf, len, ML_SPLIT, SPLIT_REGEX_ARGS,
+                                out, out_cap, out_len, n_events, counters, nullptr);
+}
+
+int lc_multiline_split_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                           const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                           int discard_unmatched, SPLIT_REGEX_PARAMS, const uint8_t* tail,
+                                           uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                                           uint64_t* raw_len, uint64_t* n_events, uint64_t counters[3],
+                                           uint64_t ml_counters[3]) {
+    return split_regex_lz4_host(e, "lc_multiline_split_regex_parse_sls_lz4", re, buf, len, ML_SPLIT,
+                                SPLIT_REGEX_ARGS, tail, tail_len, out, out_cap, out_len, raw_len, n_events, counters);
+}
+#undef ML_SPLIT
 
 } // extern "C"
 

@@ -1196,7 +1196,8 @@ inline const char* lc_delim_sls_setup(const uint8_t* sep, uint32_t sep_len, uint
 // the configuration once into two content plans (lc_regex_sls_setup) and the device walks the plan of each row.  The
 // same body function serves the counting and the writing pass (sinks LcSlsCount / LcSlsWrite above).
 
-#define LC_REGEX_SLS_LINE 0xFFFFFFFFu // value source of a plan entry: the whole line (else capture j)
+#define LC_REGEX_SLS_LINE 0xFFFFFFFFu   // value source of a plan entry: the whole line (else capture j)
+#define LC_REGEX_SLS_DIGITS 0xFFFFFFFEu // ... the split piece's file offset in decimal (lc_regex_sls_plans only)
 
 // Plan entry e = (plan[2e] = key id, plan[2e + 1] = capture index or LC_REGEX_SLS_LINE), key id k naming the key
 // bytes [key_at[k], key_at[k + 1]) of `keys`.  Entries [0, n_ok) are the plan of parsed rows, [n_ok, n_ok + n_fail)
@@ -1288,20 +1289,32 @@ inline void lc_sls_key_table(const char* const* strings, const uint32_t* lens, u
 //   failed: delete(SourceKey); with KeepingSourceWhenParseFail RenamedSourceKey -> line, then "__raw_log__" -> line
 //           with CopingRawLog, each only if that key is not live; without it the event is empty and erased
 // so the kernels need no branch per quirk.
-inline const char* lc_regex_sls_setup(const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+//
+// lc_regex_sls_plans is the same with an optional offset content (has_offset): the event starts as [SourceKey -> line,
+// offset_key -> LC_REGEX_SLS_DIGITS] and the key table gains offset_key as id nkeys + 4; `plan` then needs
+// 3 * nkeys + 24 words.  A regex key, RenamedSourceKey or "__raw_log__" equal to offset_key lands on that content like
+// on any other, and a failed row without KeepingSourceWhenParseFail is erased although the offset content is left
+// (ShouldEraseEvent, CommonParserOptions.cpp:107-110).  Without it the plans are lc_regex_sls_setup's.
+inline const char* lc_regex_sls_plans(const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
                                       const char* source_key, uint32_t source_len, const char* renamed_key,
-                                      uint32_t renamed_len, int keep_fail, int keep_succeed, int copy_raw,
+                                      uint32_t renamed_len, int has_offset, const char* offset_key,
+                                      uint32_t offset_len, int keep_fail, int keep_succeed, int copy_raw,
                                       int whole_line, uint32_t pitch, LcRegexSlsCfg* c, uint32_t* plan) {
-    if ((nkeys && (!keys || !key_lens)) || (source_len && !source_key) || (renamed_len && !renamed_key) || !c || !plan)
+    if ((nkeys && (!keys || !key_lens)) || (source_len && !source_key) || (renamed_len && !renamed_key) ||
+        (has_offset && offset_len && !offset_key) || !c || !plan)
         return "bad arguments";
     for (uint32_t k = 0; k < nkeys; ++k)
         if (key_lens[k] && !keys[k])
             return "bad arguments";
-    const uint32_t K_SRC = nkeys, K_REN = nkeys + 1, K_RAW = nkeys + 2, K_CONTENT = nkeys + 3;
+    const uint32_t K_SRC = nkeys, K_REN = nkeys + 1, K_RAW = nkeys + 2, K_CONTENT = nkeys + 3, K_OFF = nkeys + 4;
     auto str = [&](uint32_t k, uint32_t* l) -> const char* {
         if (k < nkeys) {
             *l = key_lens[k];
             return keys[k];
+        }
+        if (k == K_OFF) {
+            *l = offset_len;
+            return offset_key;
         }
         *l = k == K_SRC ? source_len : k == K_REN ? renamed_len : k == K_RAW ? 11u : 7u;
         return k == K_SRC ? source_key : k == K_REN ? renamed_key : k == K_RAW ? "__raw_log__" : "content";
@@ -1355,9 +1368,14 @@ inline const char* lc_regex_sls_setup(const char* const* keys, const uint32_t* k
     for (uint32_t k = 0; k < nkeys; ++k)
         src_overwritten = src_overwritten || same(k, K_SRC);
     memset(c, 0, sizeof *c);
+    // the event as the processor receives it
+    auto start = [&]() {
+        list[0] = K_SRC, list[1] = LC_REGEX_SLS_LINE, list[2] = 1u;
+        list[3] = K_OFF, list[4] = LC_REGEX_SLS_DIGITS, list[5] = 1u;
+        len = has_offset ? 2u : 1u;
+    };
     // parsed rows
-    list[0] = K_SRC, list[1] = LC_REGEX_SLS_LINE, list[2] = 1u;
-    len = 1;
+    start();
     if (whole_line)
         set(nkeys ? 0u : K_CONTENT, LC_REGEX_SLS_LINE);
     else
@@ -1373,8 +1391,7 @@ inline const char* lc_regex_sls_setup(const char* const* keys, const uint32_t* k
     list = plan + 2 * c->n_ok;
     len = 0;
     if (!whole_line) {
-        list[0] = K_SRC, list[1] = LC_REGEX_SLS_LINE, list[2] = 1u;
-        len = 1;
+        start();
         del(K_SRC);
         if (keep_fail) {
             add_absent(K_REN);
@@ -1382,12 +1399,20 @@ inline const char* lc_regex_sls_setup(const char* const* keys, const uint32_t* k
                 add_absent(K_RAW);
         }
     }
-    c->n_fail = finish();
+    c->n_fail = keep_fail ? finish() : 0u; // erased: empty, or only the offset content left
     c->pitch = pitch;
     c->whole_line = whole_line != 0;
     c->ok_fits = whole_line || nkeys <= pitch;
     c->keep_fail = keep_fail != 0;
     return nullptr;
+}
+
+inline const char* lc_regex_sls_setup(const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                                      const char* source_key, uint32_t source_len, const char* renamed_key,
+                                      uint32_t renamed_len, int keep_fail, int keep_succeed, int copy_raw,
+                                      int whole_line, uint32_t pitch, LcRegexSlsCfg* c, uint32_t* plan) {
+    return lc_regex_sls_plans(keys, key_lens, nkeys, source_key, source_len, renamed_key, renamed_len, 0, nullptr, 0u,
+                              keep_fail, keep_succeed, copy_raw, whole_line, pitch, c, plan);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1845,6 +1870,121 @@ LC_HD void lc_span_sls_tile(const LcSpanSlsCfg& c, const uint64_t* rec_off, uint
         if (a < z)
             lc_copy_span(o + a, c.src + off + (a - vs), z - a, lo, hi, lane, nlanes);
     }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, split -> regex chain: the Log record of piece k that ProcessorSplitLogStringNative /
+// ProcessorSplitMultilineLogStringNative followed by ProcessorParseRegexNative (same SourceKey) leave behind, written
+// straight from the piece tables of the splitter and the regex tables of lc_regex_parse_dev over those pieces.  The
+// piece enters the regex stage as [SourceKey -> piece] or, with log.file.offset metadata, [SourceKey -> piece,
+// offset_key -> decimal(src_pos + off[k])]; lc_regex_sls_plans compiles the configuration into the content plans over
+// "the piece", "capture j" and "the piece's offset digits", so the rows need no branch per quirk.
+struct LcSplitRegexSlsCfg {
+    LcRegexSlsCfg x;  // the plans (lc_regex_sls_plans), key table keys..., SourceKey, RenamedSourceKey, "__raw_log__",
+                      // "content", offset_key
+    uint64_t src_pos; // the source event's file offset
+    uint32_t time;    // the source event's time, as the split events inherit it
+    uint32_t has_ns, ns;
+};
+
+// One piece: src[po, + plen) and its row of the regex tables (offsets into src).
+struct LcSplitRegexSlsRow {
+    uint32_t po, plen;
+    uint32_t status;
+    const uint32_t* co;
+    const uint32_t* cl;
+};
+
+// the nd decimal digits of v into sink s: counting sinks count them, a writing sink's lanes write one digit each
+template <class S>
+LC_HD void lc_sls_digits(S& s, uint64_t, uint32_t nd) {
+    s.put(nullptr, nd);
+}
+LC_HD void lc_sls_digits(LcSlsWrite& s, uint64_t v, uint32_t nd) {
+    for (uint32_t j = s.lane; j < nd; j += s.nlanes)
+        if (s.at + j < s.lim)
+            s.out[s.at + j] = lc_dec_digit(v, j, nd);
+    s.at += nd;
+}
+
+// The body of the piece's Log record -- Time, the contents of its plan, Time_ns -- into sink s (LcSlsCount /
+// LcSlsWrite / LcSlsCount64).  Returns the number of contents; 0 = erased or empty, no record.
+template <class S>
+LC_HD uint32_t lc_split_regex_sls_body(const LcSplitRegexSlsCfg& c, const uint8_t* src, const LcSplitRegexSlsRow& r,
+                                       S& s) {
+    {
+        uint8_t h[6];
+        h[0] = 0x08;
+        const uint32_t n = 1 + lc_put_varint(h + 1, c.time < (1u << 28) ? (1u << 28) : c.time); // always 5 bytes
+        s.put(h, n);
+    }
+    const bool ok = lc_regex_sls_verdict(c.x, r.status) == 0u;
+    const uint32_t* e = c.x.plan + (ok ? 0u : 2u * c.x.n_ok);
+    const uint32_t m = ok ? c.x.n_ok : c.x.n_fail;
+    const uint64_t pos = c.src_pos + r.po;
+    const uint32_t nd = lc_dec_digits(pos);
+    for (uint32_t k = 0; k < m; ++k) {
+        const uint32_t kid = e[2 * k], vs = e[2 * k + 1];
+        const uint8_t* key = c.x.keys + c.x.key_at[kid];
+        const uint32_t kl = c.x.key_at[kid + 1] - c.x.key_at[kid];
+        const bool digits = vs == LC_REGEX_SLS_DIGITS, line = vs == LC_REGEX_SLS_LINE;
+        const uint32_t vl = digits ? nd : line ? r.plen : r.cl[vs];
+        lc_sls_pair_open(s, key, kl, vl);
+        if (digits)
+            lc_sls_digits(s, pos, nd);
+        else
+            s.copy(src + (line ? r.po : r.co[vs]), vl);
+    }
+    if (c.has_ns) {
+        const uint8_t h[5] = {0x25, (uint8_t)c.ns, (uint8_t)(c.ns >> 8), (uint8_t)(c.ns >> 16), (uint8_t)(c.ns >> 24)};
+        s.put(h, 5);
+    }
+    return m;
+}
+
+// counting sink of the size pass in 64 bits: a body of 2^32 bytes or more is refused instead of wrapping
+struct LcSlsCount64 {
+    uint64_t n;
+    LC_HD void put(const uint8_t*, uint32_t k) { n += k; }
+    LC_HD void copy(const uint8_t*, uint32_t k) { n += k; }
+};
+
+// The piece's counter verdicts (0 / 1): ProcessorParseRegexNative's out_successful (every piece not erased),
+// out_failed (LC_REGEX_NOMATCH only) and discarded.  A split event always holds SourceKey, so no key-not-found.
+struct LcSplitRegexVerdict {
+    uint32_t ok, failed, erased;
+};
+LC_HD LcSplitRegexVerdict lc_split_regex_verdict(const LcSplitRegexSlsCfg& c, uint32_t status) {
+    const uint32_t v = lc_regex_sls_verdict(c.x, status);
+    const uint32_t kept = v == 0u || c.x.keep_fail;
+    return {kept, v == 1u ? 1u : 0u, kept ? 0u : 1u};
+}
+
+// Host side: the configuration of the chain.  offset_key == nullptr: no log.file.offset metadata.  `plan` needs
+// 3 * nkeys + 24 words.  Returns nullptr, or why the chain is refused: lc_regex_sls_setup's refusals, and an offset
+// key equal to SourceKey (the split would replace the piece by its digits, and the regex would parse those).
+inline const char* lc_split_regex_sls_setup(const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                                            const char* source_key, uint32_t source_len, const char* renamed_key,
+                                            uint32_t renamed_len, const char* offset_key, uint32_t offset_len,
+                                            int keep_fail, int keep_succeed, int copy_raw, int whole_line,
+                                            uint32_t pitch, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                            LcSplitRegexSlsCfg* c, uint32_t* plan) {
+    if (!c)
+        return "bad arguments";
+    if (offset_key && offset_len == source_len && (offset_len == 0 || (source_key && !memcmp(offset_key, source_key,
+                                                                                               offset_len))))
+        return "the offset key equals SourceKey";
+    memset(c, 0, sizeof *c);
+    const char* why = lc_regex_sls_plans(keys, key_lens, nkeys, source_key, source_len, renamed_key, renamed_len,
+                                         offset_key != nullptr, offset_key, offset_len, keep_fail, keep_succeed,
+                                         copy_raw, whole_line, pitch, &c->x, plan);
+    if (why)
+        return why;
+    c->src_pos = src_pos;
+    c->time = time;
+    c->has_ns = time_ns != 0xFFFFFFFFu;
+    c->ns = c->has_ns ? time_ns : 0u;
+    return nullptr;
 }
 
 // ------------------------------------------------------------------------------------------------------------

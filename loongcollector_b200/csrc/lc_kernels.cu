@@ -3602,6 +3602,87 @@ void launch_regex_sls_emit(const LcRegexSlsCfg& c, const RegexSlsTables& t, cons
                                                                                  d_body_size, d_out);
 }
 
+// ---- f4, split -> regex chain: Log records of the pieces a splitter cut and a ProcessorParseRegexNative parsed,
+// straight from the piece tables and the regex tables over them (lc_exec.cuh: lc_split_regex_sls_body) -- the size
+// pass one thread per piece, the emit pass one warp per piece.  counters: u64 [4] += successful, failed, discarded,
+// pieces whose record would reach 4 GiB (their size is left 0 and the call is refused).
+__device__ __forceinline__ LcSplitRegexSlsRow split_regex_sls_row(const LcSplitRegexSlsCfg& c, const RegexSlsTables& t,
+                                                                  uint64_t i) {
+    LcSplitRegexSlsRow r;
+    r.po = t.ev_off[i];
+    r.plen = t.ev_len[i];
+    r.status = c.x.whole_line ? 0u : t.status[i];
+    r.co = t.cap_off ? t.cap_off + i * c.x.pitch : nullptr;
+    r.cl = t.cap_len ? t.cap_len + i * c.x.pitch : nullptr;
+    return r;
+}
+
+__global__ void __launch_bounds__(256)
+    split_regex_sls_size_kernel(LcSplitRegexSlsCfg c, RegexSlsTables t, uint64_t n, uint32_t* __restrict__ rec_size,
+                                uint32_t* __restrict__ body_size, unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    LcSplitRegexVerdict v{0u, 0u, 0u};
+    uint32_t big = 0;
+    if (i < n) {
+        const LcSplitRegexSlsRow r = split_regex_sls_row(c, t, i);
+        LcSlsCount64 s{0};
+        const uint32_t cnt = lc_split_regex_sls_body(c, t.base, r, s);
+        big = s.n + 16 > 0xFFFFFFFFull;
+        const uint32_t body = cnt && !big ? (uint32_t)s.n : 0u;
+        rec_size[i] = body ? 1 + lc_varint_size(body) + body : 0u;
+        body_size[i] = body;
+        v = lc_split_regex_verdict(c, r.status);
+    }
+    // one atomic per warp and counter
+    const uint32_t ok = __reduce_add_sync(0xFFFFFFFFu, v.ok), failed = __reduce_add_sync(0xFFFFFFFFu, v.failed),
+                   erased = __reduce_add_sync(0xFFFFFFFFu, v.erased);
+    big = __reduce_add_sync(0xFFFFFFFFu, big);
+    if ((threadIdx.x & 31) == 0) {
+        if (ok)
+            atomicAdd(counters + 0, (unsigned long long)ok);
+        if (failed)
+            atomicAdd(counters + 1, (unsigned long long)failed);
+        if (erased)
+            atomicAdd(counters + 2, (unsigned long long)erased);
+        if (big)
+            atomicAdd(counters + 3, (unsigned long long)big);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    split_regex_sls_emit_kernel(LcSplitRegexSlsCfg c, RegexSlsTables t, uint64_t n, const uint64_t* __restrict__ rec_off,
+                                const uint32_t* __restrict__ body_size, uint8_t* __restrict__ out) {
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n)
+        return;
+    const uint32_t body = body_size[i];
+    if (!body)
+        return; // erased or LogEvent::Empty: no record
+    const LcSplitRegexSlsRow r = split_regex_sls_row(c, t, i);
+    uint8_t h[6];
+    h[0] = 0x0A;
+    const uint32_t hn = 1 + lc_put_varint(h + 1, body);
+    LcSlsWrite s{out + rec_off[i], 0u, hn + body, threadIdx.x & 31, 32};
+    s.put(h, hn);
+    lc_split_regex_sls_body(c, t.base, r, s);
+}
+
+void launch_split_regex_sls_sizes(const LcSplitRegexSlsCfg& c, const RegexSlsTables& t, uint64_t n,
+                                  uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                  cudaStream_t st) {
+    if (n)
+        split_regex_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_size, d_body_size,
+                                                                                  d_counters);
+}
+
+void launch_split_regex_sls_emit(const LcSplitRegexSlsCfg& c, const RegexSlsTables& t, uint64_t n,
+                                 const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                 cudaStream_t st) {
+    if (n)
+        split_regex_sls_emit_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_off, d_body_size,
+                                                                                       d_out);
+}
+
 // ---- f4, delimiter-fed: Log records of the events a ProcessorParseDelimiterNative leaves behind, straight from the
 // delimiter stage's tables.  Both passes run the same per-row function (lc_exec.cuh: lc_delim_sls_body) -- the size
 // pass with a counting sink, one thread per event; the emit pass with a writing sink, one warp per event.

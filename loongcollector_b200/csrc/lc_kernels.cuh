@@ -8,6 +8,7 @@ struct LcDelimSlsCfg; // lc_exec.cuh
 struct LcRegexSlsCfg;
 struct LcDelimRegexSlsCfg;
 struct LcSpanSlsCfg;
+struct LcSplitRegexSlsCfg;
 struct LcLz4Seq;
 struct LcLz4Chunk;
 
@@ -218,6 +219,17 @@ void launch_regex_sls_sizes(const LcRegexSlsCfg& c, const RegexSlsTables& t, con
 void launch_regex_sls_emit(const LcRegexSlsCfg& c, const RegexSlsTables& t, const uint32_t* d_ev_time,
                            const uint32_t* d_ev_ns, uint64_t n, const uint64_t* d_rec_off, const uint32_t* d_body_size,
                            uint8_t* d_out, cudaStream_t st);
+
+// f4, split -> regex chain: Log records of the pieces t.ev_off / t.ev_len of the source value t.base, parsed into the
+// regex tables of t (lc_exec.cuh: LcSplitRegexSlsCfg, plans and key strings on the device).  Sizes as for
+// launch_sls_sizes; d_counters: u64 [4] += successful, failed (LC_REGEX_NOMATCH), discarded pieces, and pieces whose
+// record would reach 4 GiB.
+void launch_split_regex_sls_sizes(const LcSplitRegexSlsCfg& c, const RegexSlsTables& t, uint64_t n,
+                                  uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                  cudaStream_t st);
+void launch_split_regex_sls_emit(const LcSplitRegexSlsCfg& c, const RegexSlsTables& t, uint64_t n,
+                                 const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                 cudaStream_t st);
 
 // f4, delimiter-fed: Log records from the delimiter stage's result tables (launch_delim) + the configuration of
 // lc_exec.cuh (LcDelimSlsCfg, key strings on the device).  Sizes as for launch_sls_sizes; d_counters (or nullptr):

@@ -1887,7 +1887,7 @@ bool CompressSls(bool ok, std::string& raw, std::string& block, uint64_t& rawSiz
 // `estimate` first and by the exact block size when that was short (unless the group is over the size limit anyway).
 // Then SLSEventGroupSerializer::Serialize's checks, in its order, on the raw size.
 template <class Call>
-bool RunSlsLz4DevicePass(Call call, size_t estimate, const SLSEventGroupSerializer& ser, uint64_t n,
+bool RunSlsLz4DevicePass(Call call, size_t estimate, const SLSEventGroupSerializer& ser, const uint64_t& n,
                          const uint64_t& discarded, size_t tailSize, std::string& block, uint64_t& rawSize,
                          std::string& err, const char* what) {
     uint64_t blen = 0, raw = 0;
@@ -1921,10 +1921,10 @@ bool RunSlsLz4DevicePass(Call call, size_t estimate, const SLSEventGroupSerializ
 // the records are concatenated in event order; counters[3] += the ctr of each source event's last call.  The records
 // are what CreateNewEvent builds (ProcessorSplitLogStringNative.cpp:131-161): RAW events serialise as "content" ->
 // piece; LOG events as SourceKey -> piece plus, with log.file.offset metadata, that key -> the piece's file offset.
-// An empty value emits nothing.
+// An empty value emits nothing.  counters[3..6) are a chained regex stage's (successful, failed, discarded).
 template <class Call>
 bool SplitSerializeSls(PipelineEventGroup& group, bool enableNs, const std::string& sourceKey, bool raw, Call call,
-                       const char* what, std::string& out, std::string& err, uint64_t counters[3]) {
+                       const char* what, std::string& out, std::string& err, uint64_t counters[6]) {
     SLSEventGroupSerializer ser;
     ser.mEnableTimestampNanosecond = enableNs;
     static const std::string kRawKey = "content"; // DEFAULT_CONTENT_KEY (SLSSerializer.cpp:366-374)
@@ -1944,10 +1944,10 @@ bool SplitSerializeSls(PipelineEventGroup& group, bool enableNs, const std::stri
             continue;
         const uint32_t ns =
             enableNs && src.GetTimestampNanosecond() ? src.GetTimestampNanosecond().value() : LC_SLS_NO_NS;
-        uint64_t need = 0, nev = 0, ctr[3];
+        uint64_t need = 0, nev = 0, ctr[6];
         RunSlsDevicePass(
             [&](uint8_t* o, uint64_t cap, uint64_t* len) {
-                ctr[0] = ctr[1] = ctr[2] = 0; // (a second, exactly sized call must not count the lines twice)
+                memset(ctr, 0, sizeof ctr); // (a second, exactly sized call must not count the lines twice)
                 return call(val, key, hasOffset ? &okey : nullptr, src.GetPosition().first,
                             (uint32_t)src.GetTimestamp(), ns, o, cap, len, &nev, ctr);
             },
@@ -1957,10 +1957,114 @@ bool SplitSerializeSls(PipelineEventGroup& group, bool enableNs, const std::stri
         // (else the group is over the size limit: the sizes still add up for the error message)
         total += need;
         nEvents += nev;
-        for (int k = 0; k < 3; ++k)
+        for (int k = 0; k < 6; ++k)
             counters[k] += ctr[k];
     }
-    return FinishSls(ser, nEvents, 0, total, res, tail, out, err);
+    return FinishSls(ser, nEvents, counters[5], total, res, tail, out, err);
+}
+} // namespace
+
+// The regex stage of the split -> regex chain: a ProcessorParseRegexNative's configuration as the chain calls take it
+// (SPLIT_REGEX_STAGE_ARGS), the host check of lc_split_regex_sls_setup, and the counters Process would move.
+struct SplitRegexStage {
+    ProcessorParseRegexNative& r;
+    std::vector<const char*> kp;
+    std::vector<uint32_t> kl;
+    const lc_regex_t* re;
+    bool wholeLine;
+    explicit SplitRegexStage(ProcessorParseRegexNative& next)
+        : r(next), re(next.mIsWholeLineMode ? nullptr : next.mReg.get()), wholeLine(next.mIsWholeLineMode) {
+        for (const auto& k : r.mKeys) {
+            kp.push_back(k.data());
+            kl.push_back((uint32_t)k.size());
+        }
+    }
+    const std::string& Renamed() const { return r.mCommonParserOptions.mRenamedSourceKey; }
+    const CommonParserOptions& Opt() const { return r.mCommonParserOptions; }
+    // whether the chain's device calls take this stage behind a splitter reading sourceKey
+    bool Accepts(const std::string& sourceKey, const StringView* okey) const {
+        if (r.mSourceKey != sourceKey)
+            return false;
+        std::vector<uint32_t> plan(3 * r.mKeys.size() + 24);
+        LcSplitRegexSlsCfg c;
+        return !lc_split_regex_sls_setup(kp.data(), kl.data(), (uint32_t)r.mKeys.size(), r.mSourceKey.data(),
+                                         (uint32_t)r.mSourceKey.size(), Renamed().data(), (uint32_t)Renamed().size(),
+                                         okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u,
+                                         Opt().mKeepingSourceWhenParseFail, Opt().mKeepingSourceWhenParseSucceed,
+                                         Opt().mCopingRawLog, wholeLine, 0, 0, 0, LC_SLS_NO_NS, &c, plan.data());
+    }
+    void Add(const uint64_t ctr[3]) const {
+        r.mOutSuccessfulEventsTotal.Add(ctr[0]);
+        r.mOutFailedEventsTotal.Add(ctr[1]);
+        r.mDiscardedEventsTotal.Add(ctr[2]);
+    }
+};
+#define SPLIT_REGEX_STAGE_ARGS(x)                                                                                      \
+    (x).kp.data(), (x).kl.data(), (uint32_t)(x).kp.size(), (x).r.mSourceKey.data(), (uint32_t)(x).r.mSourceKey.size(), \
+        (x).Renamed().data(), (uint32_t)(x).Renamed().size(), (x).Opt().mKeepingSourceWhenParseFail,                    \
+        (x).Opt().mKeepingSourceWhenParseSucceed, (x).Opt().mCopingRawLog, (x).wholeLine
+
+namespace {
+// The split -> regex chain of either splitter: `process(group)` is the splitter's Process; the device calls are
+// sls(val, okey, pos, time, ns, out, cap, &len, &nev, rctr, sctr) and lz4(val, okey, pos, time, ns, tail, tailLen,
+// out, cap, &len, &raw, &nev, rctr, sctr) (rctr[3] = the regex stage's counters, sctr[3] = the splitter's).
+// sctr_total[3] += the splitter's counters of every device call.  rawSize null: out = the wire bytes; else out = their
+// LZ4 block and *rawSize their size.
+template <class ProcessFn, class Sls, class Lz4>
+bool SplitRegexChainSls(PipelineEventGroup& group, const SplitRegexStage& x, const std::string& sourceKey,
+                        bool rawContent, bool enableNs, std::string& out, uint64_t* rawSize, std::string& err,
+                        ProcessFn process, Sls sls, Lz4 lz4, const char* what, const char* lzwhat,
+                        uint64_t sctrTotal[3]) {
+    SLSEventGroupSerializer ser;
+    ser.mEnableTimestampNanosecond = enableNs;
+    const bool hasOffset = group.HasMetadata(EventGroupMetaKey::LOG_FILE_OFFSET_KEY);
+    StringView okey = hasOffset ? group.GetMetadata(EventGroupMetaKey::LOG_FILE_OFFSET_KEY) : StringView();
+    if (hasOffset && !okey.data())
+        okey = StringView(""); // an empty key is still a key: the C-ABI reads NULL as "no offset key"
+    const StringView* okp = hasOffset ? &okey : nullptr;
+    if (rawContent || !IsFlatGroup(group, sourceKey) || !x.Accepts(sourceKey, okp)) {
+        process(group);
+        x.r.Process(group);
+        if (!rawSize)
+            return ser.Serialize(group, out, err);
+        std::string raw;
+        const bool ok = ser.Serialize(group, raw, err);
+        return CompressSls(ok, raw, out, *rawSize, err);
+    }
+    const EventsContainer& events = group.GetEvents();
+    if (rawSize && events.size() == 1 && !events[0].Cast<LogEvent>().FirstLive()->first.second.empty()) {
+        // the reader's case: one chunk, split, parsed, serialised and compressed on the device
+        const LogEvent& src = events[0].Cast<LogEvent>();
+        const StringView val = src.FirstLive()->first.second;
+        const uint32_t ns =
+            enableNs && src.GetTimestampNanosecond() ? src.GetTimestampNanosecond().value() : LC_SLS_NO_NS;
+        const std::string tail = SlsGroupTail(group);
+        uint64_t nev = 0, rctr[3] = {0, 0, 0}, sctr[3] = {0, 0, 0};
+        const bool ok = RunSlsLz4DevicePass(
+            [&](uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw) {
+                memset(rctr, 0, sizeof rctr);
+                memset(sctr, 0, sizeof sctr);
+                return lz4(val, okp, src.GetPosition().first, (uint32_t)src.GetTimestamp(), ns,
+                           reinterpret_cast<const uint8_t*>(tail.data()), (uint64_t)tail.size(), o, cap, len, raw,
+                           &nev, rctr, sctr);
+            },
+            2 * val.size() + 4096 + tail.size(), ser, nev, rctr[2], tail.size(), out, *rawSize, err, lzwhat);
+        x.Add(rctr);
+        for (int k = 0; k < 3; ++k)
+            sctrTotal[k] += sctr[k];
+        return ok;
+    }
+    auto call = [&](StringView val, const std::string&, const StringView* ok, uint64_t pos, uint32_t time, uint32_t ns,
+                    uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* ctr) {
+        return sls(val, ok, pos, time, ns, o, cap, len, nev, ctr + 3, ctr);
+    };
+    uint64_t ctr[6] = {0, 0, 0, 0, 0, 0};
+    std::string raw;
+    const bool ok = SplitSerializeSls(group, enableNs, sourceKey, false, call, what, rawSize ? raw : out, err, ctr);
+    x.Add(ctr + 3);
+    for (int k = 0; k < 3; ++k)
+        sctrTotal[k] += ctr[k];
+    return rawSize ? CompressSls(ok, raw, out, *rawSize, err) : ok;
 }
 } // namespace
 
@@ -2086,7 +2190,7 @@ bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, bool
                             key.data(), (uint32_t)key.size(), okey ? okey->data() : nullptr,
                             okey ? (uint32_t)okey->size() : 0u, pos, time, ns, o, cap, len, nev);
     };
-    uint64_t unused[3] = {0, 0, 0};
+    uint64_t unused[6] = {0, 0, 0, 0, 0, 0};
     return SplitSerializeSls(group, enableNs, mSourceKey, mEnableRawContent, call, "lc_split_sls", out, err, unused);
 }
 
@@ -2107,9 +2211,90 @@ bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& gr
                                       o, cap, len, nev, ctr);
     };
     // matched_events, input lines, unmatched lines: moved as Process moves them (:82-84,106-107)
-    uint64_t ctr[3] = {0, 0, 0};
+    uint64_t ctr[6] = {0, 0, 0, 0, 0, 0};
     const bool ok = SplitSerializeSls(group, enableNs, mSourceKey, mEnableRawContent, call, "lc_multiline_split_sls",
                                       out, err, ctr);
+    mMatchedEventsTotal.Add(ctr[0]);
+    mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
+    mUnmatchedLinesTotal.Add(ctr[2]);
+    return ok;
+}
+
+bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                                                 bool enableNs, std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                                                    bool enableNs, std::string& block, uint64_t& rawSize,
+                                                    std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitLogStringNative::ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                                                      bool enableNs, std::string& out, uint64_t* rawSize,
+                                                      std::string& err) {
+    const SplitRegexStage x(next);
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        return lc_split_regex_parse_sls(Engine(), x.re, src(val), val.size(), (uint8_t)mSplitChar,
+                                        SPLIT_REGEX_STAGE_ARGS(x), okey ? okey->data() : nullptr,
+                                        okey ? (uint32_t)okey->size() : 0u, pos, time, ns, o, cap, len, nev, rctr);
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        return lc_split_regex_parse_sls_lz4(Engine(), x.re, src(val), val.size(), (uint8_t)mSplitChar,
+                                            SPLIT_REGEX_STAGE_ARGS(x), okey ? okey->data() : nullptr,
+                                            okey ? (uint32_t)okey->size() : 0u, pos, time, ns, tail, tailLen, o, cap,
+                                            len, raw, nev, rctr);
+    };
+    uint64_t unused[3] = {0, 0, 0};
+    return SplitRegexChainSls(
+        group, x, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_split_regex_parse_sls",
+        "lc_split_regex_parse_sls_lz4", unused);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                                                          bool enableNs, std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSlsLz4(PipelineEventGroup& group,
+                                                             ProcessorParseRegexNative& next, bool enableNs,
+                                                             std::string& block, uint64_t& rawSize, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGroup& group,
+                                                               ProcessorParseRegexNative& next, bool enableNs,
+                                                               std::string& out, uint64_t* rawSize, std::string& err) {
+    const SplitRegexStage x(next);
+    const bool discard = mMultiline.mUnmatchedContentTreatment == MultilineOptions::UnmatchedContentTreatment::DISCARD;
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        return lc_multiline_split_regex_parse_sls(Engine(), x.re, src(val), val.size(), mStart.get(),
+                                                  mContinue.get(), mEnd.get(), discard, SPLIT_REGEX_STAGE_ARGS(x),
+                                                  okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u,
+                                                  pos, time, ns, o, cap, len, nev, rctr, sctr);
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        return lc_multiline_split_regex_parse_sls_lz4(
+            Engine(), x.re, src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
+            SPLIT_REGEX_STAGE_ARGS(x), okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos, time,
+            ns, tail, tailLen, o, cap, len, raw, nev, rctr, sctr);
+    };
+    // matched_events, input lines, unmatched lines: moved as Process moves them (:82-84,106-107)
+    uint64_t ctr[3] = {0, 0, 0};
+    const bool ok = SplitRegexChainSls(
+        group, x, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_multiline_split_regex_parse_sls",
+        "lc_multiline_split_regex_parse_sls_lz4", ctr);
     mMatchedEventsTotal.Add(ctr[0]);
     mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
     mUnmatchedLinesTotal.Add(ctr[2]);

@@ -112,6 +112,8 @@ private:
     lc_regex_t* mRe = nullptr;
 };
 
+class ProcessorParseRegexNative;
+
 class ProcessorSplitLogStringNative : public Processor {
 public:
     static const std::string sName;
@@ -127,9 +129,25 @@ public:
     // A group whose events are all LogEvents {SourceKey -> value} is split and serialised on the device, one source
     // event per call, and only the wire bytes come back; any other group runs Process + Serialize.
     bool SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out, std::string& err);
+    // Process(group), then next.Process(group) (next: the regex processor behind this one, reading SourceKey), then
+    // SLSEventGroupSerializer::Serialize: the same bytes or error message, and the same counter updates on both
+    // processors.  On a flat group without EnableRawContent, whose regex SourceKey is this SourceKey and whose
+    // configuration lc_split_regex_parse_sls accepts, each source event is split, parsed and serialised in one device
+    // pass (log.file.offset metadata included) and only the wire bytes come back; the group's events are left as they
+    // were.  Otherwise the three calls run.
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs, std::string& out,
+                      std::string& err);
+    // The same followed by LZ4Compressor::Compress.  A device-path group of one source event is compressed on the
+    // device (lc_split_regex_parse_sls_lz4); other groups compress SerializeSls's bytes.
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs, std::string& block,
+                         uint64_t& rawSize, std::string& err);
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
+
+private:
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs,
+                           std::string& out, uint64_t* rawSize, std::string& err);
 };
 
 class ProcessorSplitMultilineLogStringNative : public Processor {
@@ -148,12 +166,19 @@ public:
     // A group whose events are all LogEvents {SourceKey -> value} is split and serialised on the device, one source
     // event per call, and only the wire bytes come back; any other group runs Process + Serialize.
     bool SerializeSls(PipelineEventGroup& group, bool enableNs, std::string& out, std::string& err);
+    // The split -> regex chain, as ProcessorSplitLogStringNative's (lc_multiline_split_regex_parse_sls[_lz4]).
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs, std::string& out,
+                      std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs, std::string& block,
+                         uint64_t& rawSize, std::string& err);
     Counter mMatchedEventsTotal, mMatchedLinesTotal, mUnmatchedLinesTotal;
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs,
+                           std::string& out, uint64_t* rawSize, std::string& err);
     CompiledRegex mStart, mContinue, mEnd;
 };
 
@@ -211,6 +236,7 @@ private:
                        LocalCounters& c) const;
     void AddCounters(const LocalCounters& c);
     friend class ProcessorParseDelimiterNative; // the delimiter -> regex chain's SerializeSls
+    friend struct SplitRegexStage;              // the split -> regex chain's
     bool mSourceKeyOverwritten = false;
     bool mIsWholeLineMode = false;
     bool mKeysDistinct = false; // no key repeats: an event that holds only the source key takes the parsed fields as

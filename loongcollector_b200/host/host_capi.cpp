@@ -238,10 +238,19 @@ char* lc_host_chain_serialize_sls(lc_host_processor_t* delim, lc_host_processor_
     if (raw_len_out)
         *raw_len_out = 0;
     try {
-        auto* d = dynamic_cast<ProcessorParseDelimiterNative*>(delim->proc.get());
+        Processor* d = delim->proc.get();
         auto* r = dynamic_cast<ProcessorParseRegexNative*>(regex->proc.get());
-        if (!d || !r)
-            throw std::runtime_error("not a processor_parse_delimiter_native and a processor_parse_regex_native");
+        auto* pd = dynamic_cast<ProcessorParseDelimiterNative*>(d);
+        auto* ps = dynamic_cast<ProcessorSplitLogStringNative*>(d);
+        auto* pm = dynamic_cast<ProcessorSplitMultilineLogStringNative*>(d);
+        if (!(pd || ps || pm) || !r)
+            throw std::runtime_error("not a processor_parse_delimiter_native or a splitter, and a "
+                                     "processor_parse_regex_native");
+        // the chain's SerializeSls / SerializeSlsLz4 on whichever processor comes first
+        auto chain = [&](auto* p, PipelineEventGroup& g, std::string& res, uint64_t& raw, std::string& err) {
+            return mode == 2 ? p->SerializeSlsLz4(g, *r, enable_ns != 0, res, raw, err)
+                             : p->SerializeSls(g, *r, enable_ns != 0, res, err);
+        };
         PipelineEventGroup group(std::make_shared<SourceBuffer>());
         if (!group.FromJsonString(group_json ? group_json : "null"))
             throw std::runtime_error("group JSON does not parse");
@@ -255,10 +264,10 @@ char* lc_host_chain_serialize_sls(lc_host_processor_t* delim, lc_host_processor_
             SLSEventGroupSerializer ser;
             ser.mEnableTimestampNanosecond = enable_ns != 0;
             ok = ser.Serialize(group, res, err);
-        } else if (mode == 2) {
-            ok = d->SerializeSlsLz4(group, *r, enable_ns != 0, res, raw, err);
         } else {
-            ok = d->SerializeSls(group, *r, enable_ns != 0, res, err);
+            ok = pd   ? chain(pd, group, res, raw, err)
+                 : ps ? chain(ps, group, res, raw, err)
+                      : chain(pm, group, res, raw, err);
         }
         if (d->EngineErrors() + r->EngineErrors() != errs)
             throw std::runtime_error("engine error inside Process: " + d->LastError() + r->LastError());
