@@ -453,6 +453,82 @@ int lc_multiline_split_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re,
                                            uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
                                            uint64_t counters[3], uint64_t ml_counters[3]);
 
+/* ---- f4: the split -> regex -> filter chain (the above, then ProcessorFilterNative / processor_filter_regex_native;
+ * the pipeline of the reference's file-to-blackhole benchmark) to the SLS wire format.  The filter sees the event the
+ * regex stage left behind: a leaf is regex_match of its key's value there, false when the key is absent
+ * (ProcessorFilterNative.cpp:459-486); keys are compared as bytes.  prog is a postfix program: an entry < nleaves
+ * pushes that leaf, LC_FILTER_NOT pops one value and pushes its negation, LC_FILTER_AND / LC_FILTER_OR pop two and
+ * push the result; it must leave exactly one value.  nprog == 0 is BYPASS mode (every event kept; regs may be NULL).
+ * Otherwise (RULE / EXPRESSION mode) an event without contents is removed whatever the leaves say (:83-117).  The
+ * filter keeps event order and moves none of the regex stage's counters.  DiscardingNonUTF8 is not supported.
+ * Refused with LC_ERR_INVALID_ARG: more than LC_FILTER_MAX_LEAVES leaves or LC_FILTER_MAX_PROG entries, a malformed
+ * program (an unknown entry, a pop of an empty stack, more than 32 values on the stack, not one value at the end), a
+ * NULL leaf regex in RULE / EXPRESSION mode.  LC_ERR_TOO_LARGE also when some leaf reads the offset digits and the
+ * chunk has 2^32 / 20 pieces or more. */
+#define LC_FILTER_MAX_LEAVES 32
+#define LC_FILTER_MAX_PROG 128
+#define LC_FILTER_NOT 0xFFFFFFFDu
+#define LC_FILTER_AND 0xFFFFFFFEu
+#define LC_FILTER_OR 0xFFFFFFFFu
+typedef struct lc_filter_desc {
+    uint32_t nleaves;
+    const char* const* keys; /* key of leaf l: keys[l][0, key_lens[l]) */
+    const uint32_t* key_lens;
+    const lc_regex_t* const* regs; /* regex of leaf l, matched against the whole value */
+    uint32_t nprog;
+    const uint32_t* prog;
+} lc_filter_desc_t;
+
+/* Each takes its unfiltered sibling's arguments plus the filter, and counters[4] (may be NULL) = the regex stage's
+ * three, then the events the filter removed.  Sizing, capacity, 4 GiB, LZ4 and tail rules are the siblings'; a chunk
+ * whose pieces are all removed gives 0 bytes (the LZ4 calls: the block of the tail alone). */
+int lc_sls_serialize_split_regex_filter_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len,
+                                            const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+                                            const uint8_t* d_status, const uint32_t* d_cap_off,
+                                            const uint32_t* d_cap_len, uint32_t row_pitch, const char* const* keys,
+                                            const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+                                            uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+                                            int keep_fail, int keep_succeed, int copy_raw, int whole_line,
+                                            const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+                                            uint32_t time, uint32_t time_ns, const lc_filter_desc_t* filter,
+                                            uint8_t* d_out, uint64_t out_cap, uint64_t* out_len,
+                                            uint64_t counters[4]);
+int lc_split_regex_filter_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                    uint8_t split_char, const char* const* keys, const uint32_t* key_lens,
+                                    uint32_t nkeys, const char* source_key, uint32_t source_key_len,
+                                    const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed,
+                                    int copy_raw, int whole_line, const char* offset_key, uint32_t offset_key_len,
+                                    uint64_t src_pos, uint32_t time, uint32_t time_ns, const lc_filter_desc_t* filter,
+                                    uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                    uint64_t counters[4]);
+int lc_split_regex_filter_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                        uint8_t split_char, const char* const* keys, const uint32_t* key_lens,
+                                        uint32_t nkeys, const char* source_key, uint32_t source_key_len,
+                                        const char* renamed_key, uint32_t renamed_key_len, int keep_fail,
+                                        int keep_succeed, int copy_raw, int whole_line, const char* offset_key,
+                                        uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                        const lc_filter_desc_t* filter, const uint8_t* tail, uint64_t tail_len,
+                                        uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+                                        uint64_t* n_events, uint64_t counters[4]);
+int lc_multiline_split_regex_filter_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                              const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                              int discard_unmatched, const char* const* keys, const uint32_t* key_lens,
+                                              uint32_t nkeys, const char* source_key, uint32_t source_key_len,
+                                              const char* renamed_key, uint32_t renamed_key_len, int keep_fail,
+                                              int keep_succeed, int copy_raw, int whole_line, const char* offset_key,
+                                              uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+                                              uint32_t time_ns, const lc_filter_desc_t* filter, uint8_t* out,
+                                              uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                              uint64_t counters[4], uint64_t ml_counters[3]);
+int lc_multiline_split_regex_filter_parse_sls_lz4(
+    lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+    const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, const char* const* keys,
+    const uint32_t* key_lens, uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+    uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, int whole_line, const char* offset_key,
+    uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns, const lc_filter_desc_t* filter,
+    const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+    uint64_t* n_events, uint64_t counters[4], uint64_t ml_counters[3]);
+
 /* lc_regex_parse_sls / lc_delim_parse_sls finished as the SLS flusher finishes a group: the records, followed by
  * tail[0, tail_len) (the group-level fields: topic, source, machine uuid, tags), become ONE LZ4 block (the block format
  * of lc_lz4_compress_dev) and only the block comes back.  *raw_len = records + tail bytes (x-log-bodyrawsize),

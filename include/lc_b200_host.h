@@ -61,6 +61,14 @@ char* lc_host_chain_serialize_sls(lc_host_processor_t* delim, lc_host_processor_
                                   int enable_ns, int mode, unsigned long long* len_out, unsigned long long* raw_len_out,
                                   char** err_out, char** fail_out);
 
+/* The split -> regex -> filter chain on the group described by group_json: split (either splitter), then regex (a
+ * "processor_parse_regex_native" reading the splitter's SourceKey), then filter (a "processor_filter_regex_native").
+ * mode 0: split's SerializeSls(group, regex, filter); mode 1: Process x 3 + SLSEventGroupSerializer::Serialize on the
+ * same in-memory group; mode 2: SerializeSlsLz4(group, regex, filter).  Returns as lc_host_chain_serialize_sls. */
+char* lc_host_chain3_serialize_sls(lc_host_processor_t* split, lc_host_processor_t* regex, lc_host_processor_t* filter,
+                                   const char* group_json, int enable_ns, int mode, unsigned long long* len_out,
+                                   unsigned long long* raw_len_out, char** err_out, char** fail_out);
+
 /* LZ4Compressor::Compress (core/common/compression/LZ4Compressor.cpp:25-44), GPU-backed: the n inputs
  * (data[k], len[k]) in one device call, one LZ4 block each.  Returns the malloc'd blocks back to back, their total
  * length and blk_len[k]; or NULL + *err_out = the compressor's error message ("input size is incorrect") or an engine

@@ -121,6 +121,17 @@ def lib():
         [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
     L.lc_multiline_split_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sls_cfg + [i32] + \
         sr_tail + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
+    # the split -> regex -> filter chain: the siblings' arguments with the filter behind time_ns
+    L.lc_sls_serialize_split_regex_filter_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32] + sls_cfg + \
+        [i32] + sr_tail + [vp, vp, u64, C.POINTER(u64), vp]
+    L.lc_split_regex_filter_parse_sls.argtypes = [vp, vp, vp, u64, u8] + sls_cfg + [i32] + sr_tail + \
+        [vp, vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_split_regex_filter_parse_sls_lz4.argtypes = [vp, vp, vp, u64, u8] + sls_cfg + [i32] + sr_tail + \
+        [vp, vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_multiline_split_regex_filter_parse_sls.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sls_cfg + [i32] + \
+        sr_tail + [vp, vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
+    L.lc_multiline_split_regex_filter_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sls_cfg + \
+        [i32] + sr_tail + [vp, vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
     _LIB = L
     return L
 
@@ -185,6 +196,41 @@ class Regex:
 
 def _rh(r):
     return r._h if r is not None else None
+
+
+LC_FILTER_NOT, LC_FILTER_AND, LC_FILTER_OR = 0xFFFFFFFD, 0xFFFFFFFE, 0xFFFFFFFF
+_FILTER_OPS = {"not": LC_FILTER_NOT, "and": LC_FILTER_AND, "or": LC_FILTER_OR}
+
+
+class _FilterDesc(C.Structure):
+    _fields_ = [("nleaves", C.c_uint32), ("keys", C.c_void_p), ("key_lens", C.c_void_p), ("regs", C.c_void_p),
+                ("nprog", C.c_uint32), ("prog", C.c_void_p)]
+
+
+class Filter:
+    """A processor_filter_regex_native rule as the split -> regex -> filter calls take it (lc_filter_desc_t).
+    leaves: [(key bytes, Regex or None)]; prog: postfix program, each entry a leaf index or "not" / "and" / "or" (or
+    the LC_FILTER_* codes, or any int, to exercise the refusals).  An empty prog is BYPASS mode."""
+
+    def __init__(self, leaves, prog):
+        self.leaves = list(leaves)
+        self._karr = (C.c_char_p * max(len(self.leaves), 1))(*[k for k, _ in self.leaves])
+        self._kl = np.array([len(k) for k, _ in self.leaves] or [0], np.uint32)
+        self._regs = (C.c_void_p * max(len(self.leaves), 1))(*[_rh(r) for _, r in self.leaves])
+        self._prog = np.array([_FILTER_OPS[x] if isinstance(x, str) else x for x in prog] or [0], np.uint32)
+        self.desc = _FilterDesc(len(self.leaves), C.cast(self._karr, C.c_void_p), _p(self._kl),
+                                C.cast(self._regs, C.c_void_p), len(prog), _p(self._prog))
+
+    @staticmethod
+    def rule(pairs):
+        """RULE mode: every (key, Regex) must hold"""
+        prog = [0] if pairs else []
+        for i in range(1, len(pairs)):
+            prog += [i, "and"]
+        return Filter(pairs, prog)
+
+    def ptr(self):
+        return C.cast(C.pointer(self.desc), C.c_void_p)
 
 
 class Engine:
@@ -699,10 +745,10 @@ class Engine:
         return int(need.value), ctr
 
     def _split_regex(self, fn, rx, buf, extra, keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw,
-                     whole_line, offset_key, src_pos, time, time_ns, out_cap, ml, tail):
+                     whole_line, offset_key, src_pos, time, time_ns, out_cap, ml, tail, filt=None):
         """one host-buffer split -> regex call, sized by an estimate first and by the exact size when that was short;
-        tail None: the wire bytes, else records ‖ tail as one LZ4 block.  Returns (bytes, raw_len, n_events,
-        counters[3], ml_counters[3] or None)"""
+        tail None: the wire bytes, else records ‖ tail as one LZ4 block.  filt (a Filter): the _filter_ call, with
+        counters[4].  Returns (bytes, raw_len, n_events, counters[3] or [4], ml_counters[3] or None)"""
         a = _u8(buf)
         _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
         tl = None if tail is None else np.frombuffer(bytes(tail), np.uint8)
@@ -711,11 +757,12 @@ class Engine:
         for _ in range(2):
             out = np.empty(max(cap, 1), np.uint8)
             need, raw, nev = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
-            ctr, mctr = np.zeros(3, np.uint64), np.zeros(3, np.uint64)
+            ctr, mctr = np.zeros(3 if filt is None else 4, np.uint64), np.zeros(3, np.uint64)
             z = [] if tl is None else [_p(tl) if tl.size else None, tl.size]
             outs = [_p(out), cap, C.byref(need)] + ([] if tl is None else [C.byref(raw)]) + [C.byref(nev), _p(ctr)]
+            f = [] if filt is None else [filt.ptr()]
             rc = fn(self._h, _rh(rx), _p(a), a.size, *extra, *cfg, int(bool(whole_line)),
-                    *self._sr_tail(offset_key, src_pos, time, time_ns), *z, *outs, *([_p(mctr)] if ml else []))
+                    *self._sr_tail(offset_key, src_pos, time, time_ns), *f, *z, *outs, *([_p(mctr)] if ml else []))
             if rc == LC_ERR_CAPACITY and out_cap is None:
                 cap = int(need.value)
                 continue
@@ -765,6 +812,71 @@ class Engine:
             lib().lc_multiline_split_regex_parse_sls_lz4, rx, buf,
             [_rh(start), _rh(cont), _rh(end), int(bool(discard))], keys, source_key, renamed_key, keep_fail,
             keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, True, tail)
+
+    def sls_serialize_split_regex_filter_dev(self, d_src, src_len, d_off, d_len, n, d_status, d_cap_off, d_cap_len,
+                                             row_pitch, keys, source_key, filt, renamed_key=None, keep_fail=False,
+                                             keep_succeed=False, copy_raw=False, whole_line=False, offset_key=None,
+                                             src_pos=0, time=0, time_ns=None, d_out=None, out_cap=0):
+        """sls_serialize_split_regex_dev with the Filter filt behind the regex stage
+        (lc_sls_serialize_split_regex_filter_dev).  Returns (byte count, counters[4] = successful, failed, discarded,
+        removed by the filter); with d_out None the byte count needed."""
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        need = C.c_uint64(0)
+        ctr = np.zeros(4, np.uint64)
+        rc = lib().lc_sls_serialize_split_regex_filter_dev(self._h, _p(d_src), src_len, _p(d_off), _p(d_len), n,
+                                                           _p(d_status), _p(d_cap_off), _p(d_cap_len), row_pitch,
+                                                           *cfg, int(bool(whole_line)),
+                                                           *self._sr_tail(offset_key, src_pos, time, time_ns),
+                                                           filt.ptr(), _p(d_out), out_cap, C.byref(need), _p(ctr))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value), ctr  # a sizing query
+        _check(rc)
+        return int(need.value), ctr
+
+    def split_regex_filter_parse_sls(self, rx, buf, split_char, keys, source_key, filt, renamed_key=None,
+                                     keep_fail=False, keep_succeed=False, copy_raw=False, whole_line=False,
+                                     offset_key=None, src_pos=0, time=0, time_ns=None, out_cap=None):
+        """split_regex_parse_sls with the Filter filt (lc_split_regex_filter_parse_sls).  Returns (bytes, number of
+        pieces, counters[4])."""
+        data, _raw, nev, ctr, _m = self._split_regex(
+            lib().lc_split_regex_filter_parse_sls, rx, buf, [split_char], keys, source_key, renamed_key, keep_fail,
+            keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, False, None, filt)
+        return data, nev, ctr
+
+    def split_regex_filter_parse_sls_lz4(self, rx, buf, split_char, keys, source_key, filt, renamed_key=None,
+                                         keep_fail=False, keep_succeed=False, copy_raw=False, whole_line=False,
+                                         offset_key=None, src_pos=0, time=0, time_ns=None, tail=b"", out_cap=None):
+        """split_regex_filter_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_split_regex_filter_parse_sls_lz4).  Returns (block, raw_len, number of pieces, counters[4])."""
+        data, raw, nev, ctr, _m = self._split_regex(
+            lib().lc_split_regex_filter_parse_sls_lz4, rx, buf, [split_char], keys, source_key, renamed_key,
+            keep_fail, keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, False, tail,
+            filt)
+        return data, raw, nev, ctr
+
+    def multiline_split_regex_filter_parse_sls(self, rx, buf, start, cont, end, discard, keys, source_key, filt,
+                                               renamed_key=None, keep_fail=False, keep_succeed=False, copy_raw=False,
+                                               whole_line=False, offset_key=None, src_pos=0, time=0, time_ns=None,
+                                               out_cap=None):
+        """The same with the multiline splitter (lc_multiline_split_regex_filter_parse_sls).  Returns (bytes, number
+        of events, counters[4], splitter counters[3])."""
+        data, _raw, nev, ctr, mctr = self._split_regex(
+            lib().lc_multiline_split_regex_filter_parse_sls, rx, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], keys, source_key, renamed_key, keep_fail,
+            keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, True, None, filt)
+        return data, nev, ctr, mctr
+
+    def multiline_split_regex_filter_parse_sls_lz4(self, rx, buf, start, cont, end, discard, keys, source_key, filt,
+                                                   renamed_key=None, keep_fail=False, keep_succeed=False,
+                                                   copy_raw=False, whole_line=False, offset_key=None, src_pos=0,
+                                                   time=0, time_ns=None, tail=b"", out_cap=None):
+        """multiline_split_regex_filter_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_multiline_split_regex_filter_parse_sls_lz4).  Returns (block, raw_len, number of events, counters[4],
+        splitter counters[3])."""
+        return self._split_regex(
+            lib().lc_multiline_split_regex_filter_parse_sls_lz4, rx, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], keys, source_key, renamed_key, keep_fail,
+            keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, True, tail, filt)
 
     def lz4_compress_dev(self, d_in, nseg, d_seg_off, d_seg_len, d_out=None, out_cap=0, d_blk_off=None,
                          d_blk_len=None):
@@ -969,6 +1081,36 @@ def host_chain_serialize_sls(delim, regex, group, enable_ns=False, mode=0):
     n, raw = C.c_ulonglong(0), C.c_ulonglong(0)
     out = L.lc_host_chain_serialize_sls(delim._h, regex._h, json.dumps(group).encode("utf-8"), int(bool(enable_ns)),
                                         mode, C.byref(n), C.byref(raw), C.byref(err), C.byref(fail))
+    if fail.value:
+        msg = C.string_at(fail.value).decode()
+        L.lc_host_string_free(fail)
+        raise LcError(LC_ERR_CUDA, msg)
+    if not out:
+        msg = C.string_at(err.value).decode() if err.value else "unknown error"
+        if err.value:
+            L.lc_host_string_free(err)
+        return None, 0, msg
+    data = C.string_at(out, n.value)
+    L.lc_host_string_free(out)
+    return data, int(raw.value), None
+
+
+def host_chain3_serialize_sls(split, regex, filt, group, enable_ns=False, mode=0):
+    """The split -> regex -> filter chain of three HostProcessors on a JSON group (lc_host_chain3_serialize_sls).
+    mode 0: split's SerializeSls(group, regex, filter); 1: Process x 3 + Serialize; 2: SerializeSlsLz4.  Returns (bytes,
+    raw_len, None) or (None, 0, error)."""
+    import json
+    L = lib()
+    L.lc_host_chain3_serialize_sls.restype = C.c_void_p
+    L.lc_host_chain3_serialize_sls.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_char_p, C.c_int, C.c_int,
+                                               C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong),
+                                               C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+    L.lc_host_string_free.argtypes = [C.c_void_p]
+    err, fail = C.c_void_p(), C.c_void_p()
+    n, raw = C.c_ulonglong(0), C.c_ulonglong(0)
+    out = L.lc_host_chain3_serialize_sls(split._h, regex._h, filt._h, json.dumps(group).encode("utf-8"),
+                                         int(bool(enable_ns)), mode, C.byref(n), C.byref(raw), C.byref(err),
+                                         C.byref(fail))
     if fail.value:
         msg = C.string_at(fail.value).decode()
         L.lc_host_string_free(fail)

@@ -105,6 +105,10 @@ struct lc_engine {
     // delimiter -> regex -> SLS chain: the delimiter's key strings, the value table, the regex tables over it, side-copy
     // sizes and slots, the per-chunk scan descriptors of the tap; no stage of the chain uses them for anything else
     DevBuf dr_keys, dr_val_off, dr_val_len, dr_status, dr_cap_off, dr_cap_len, dr_copy, dr_slot, dr_desc;
+    // split -> regex -> filter chain: one leaf's value tables, the match bytes of every leaf, the offset-digit scratch,
+    // the removed-piece counter and the keep bytes; the chain's piece and regex tables live elsewhere (in, out_a,
+    // out_b, out_c, dr_*), and so does the scratch of the boolean match (out_d, out_e, lab*, order, desc)
+    DevBuf fl_tab, fl_match, fl_dig, fl_keep;
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
     std::unordered_map<uint64_t, void*> blobs; // regex id * 4 + layout -> device blob
@@ -319,7 +323,7 @@ void lc_engine_destroy(lc_engine_t* e) {
                       &e->lab_off, &e->lab, &e->order, &e->desc, &e->small, &e->split_scratch, &e->sls_plan,
                       &e->z_seq, &e->z_info, &e->z_size, &e->z_first, &e->z_choff, &e->z_tab, &e->z_out,
                       &e->dr_keys, &e->dr_val_off, &e->dr_val_len, &e->dr_status, &e->dr_cap_off, &e->dr_cap_len,
-                      &e->dr_copy, &e->dr_slot, &e->dr_desc};
+                      &e->dr_copy, &e->dr_slot, &e->dr_desc, &e->fl_tab, &e->fl_match, &e->fl_dig, &e->fl_keep};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -2755,6 +2759,10 @@ int lc_multiline_split_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, con
 } // extern "C"
 
 // ------------------------------------------------------------------------------------------------ split -> regex -> SLS
+static_assert(LC_FILTER_MAX_LEAVES == LC_FILTER_SLS_LEAVES && LC_FILTER_MAX_PROG == LC_FILTER_SLS_PROG &&
+                  LC_FILTER_NOT == LC_FILTER_SLS_NOT && LC_FILTER_AND == LC_FILTER_SLS_AND &&
+                  LC_FILTER_OR == LC_FILTER_SLS_OR,
+              "lc_b200.h and lc_exec.cuh disagree on the filter program");
 // The regex stage's configuration and the offset content of the split events (CHAIN_PARAMS's regex half, plus
 // offset_key -- NULL = no log.file.offset metadata -- and the source event's position, time and ns)
 #define SPLIT_REGEX_PARAMS                                                                                             \
@@ -2770,9 +2778,10 @@ namespace {
 
 // lc_split_regex_sls_setup's plans over the key table keys..., SourceKey, RenamedSourceKey, "__raw_log__", "content",
 // offset_key, staged on the device (`sls_plan`, which neither splitter nor the regex stage uses).  Every single
-// content then stays below 4 GiB; a record that would not is caught by the size pass.
+// content then stays below 4 GiB; a record that would not is caught by the size pass.  With fd, the filter behind the
+// chain is checked and resolved against those plans into *f (lc_filter_sls_setup).
 int split_regex_sls_config(lc_engine_t* e, const char* what, uint64_t src_len, SPLIT_REGEX_PARAMS, uint32_t pitch,
-                           LcSplitRegexSlsCfg* c) {
+                           LcSplitRegexSlsCfg* c, const lc_filter_desc_t* fd = nullptr, LcFilterSlsCfg* f = nullptr) {
     if ((nkeys && (!keys || !key_lens)) || (source_key_len && !source_key) || (renamed_key_len && !renamed_key))
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
     uint64_t kbytes = (uint64_t)source_key_len + renamed_key_len + (offset_key ? offset_key_len : 0u) + 18;
@@ -2793,7 +2802,71 @@ int split_regex_sls_config(lc_engine_t* e, const char* what, uint64_t src_len, S
     std::vector<uint32_t> lens(key_lens, key_lens + nkeys);
     strings.insert(strings.end(), {source_key, renamed_key, "__raw_log__", "content", offset_key});
     lens.insert(lens.end(), {source_key_len, renamed_key_len, 11u, 7u, offset_key ? offset_key_len : 0u});
+    if (fd) {
+        why = lc_filter_sls_setup(plan.data(), c->x.n_ok, c->x.n_fail, strings.data(), lens.data(), fd->nleaves,
+                                  fd->keys, fd->key_lens, fd->nprog, fd->prog, f);
+        if (why)
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+        for (uint32_t l = 0; fd->nprog && l < fd->nleaves; ++l) {
+            if (!fd->regs || !fd->regs[l])
+                return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+            const int rc = check_regex_usable(fd->regs[l], what);
+            if (rc)
+                return rc;
+        }
+    }
     return stage_regex_sls(e, what, plan.data(), strings.data(), lens.data(), nkeys + 5, &c->x);
+}
+
+// The filter over the n pieces of t: leaf by leaf, the tap and the boolean match over the source value (and over the
+// digit scratch when the leaf reads the offset digits), then the keep bytes and the removed count.  *keep = the keep
+// bytes (nullptr in BYPASS mode); *d_removed = the device counter of removed pieces (read after the size pass).
+int filter_sls_run(lc_engine_t* e, const char* what, const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f,
+                   const lc_filter_desc_t* fd, const lck::RegexSlsTables& t, uint64_t n, uint64_t src_len,
+                   const uint8_t** keep, const uint64_t** d_removed) {
+    *keep = nullptr;
+    *d_removed = nullptr;
+    if (f.nprog == 0 || n == 0)
+        return LC_OK;
+    const uint64_t nl = f.nleaves, dig_bytes = f.any_digits ? n * LC_FILTER_SLS_DIGIT_PITCH : 0;
+    if (dig_bytes + 16 >= 0xFFFFFFF0ull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": the offset digits of the pieces must stay below 4 GiB");
+    CU_TRY(e->fl_tab.ensure(n * 16));
+    CU_TRY(e->fl_match.ensure(nl * n * (f.any_digits ? 2 : 1) + 1));
+    CU_TRY(e->fl_keep.ensure(n + 16));
+    if (f.any_digits)
+        CU_TRY(e->fl_dig.ensure(dig_bytes + 16));
+    uint32_t* off = e->fl_tab.as<uint32_t>();
+    uint32_t *len = off + n, *doff = off + 2 * n, *dlen = off + 3 * n;
+    uint8_t* m = e->fl_match.as<uint8_t>();
+    uint64_t* removed = e->fl_keep.as<uint64_t>();
+    CU_TRY(cudaMemsetAsync(removed, 0, 8, e->stream));
+    for (uint32_t l = 0; l < f.nleaves; ++l) {
+        bool src = false, dig = false;
+        for (int v = 0; v < 2; ++v) {
+            dig = dig || f.src[l][v] == LC_REGEX_SLS_DIGITS;
+            src = src || (f.src[l][v] != LC_REGEX_SLS_DIGITS && f.src[l][v] != LC_FILTER_SLS_ABSENT);
+        }
+        if (!src && !dig)
+            continue; // absent everywhere: the leaf never holds
+        lck::launch_filter_tap(c, f, l, t, n, off, len, dig ? doff : nullptr, dlen, e->fl_dig.as<uint8_t>(),
+                               e->stream);
+        e->launches++;
+        CU_TRY(cudaGetLastError());
+        int rc = src ? lc_regex_match_dev(e, fd->regs[l], t.base, src_len, off, len, n, m + l * n) : (int)LC_OK;
+        if (!rc && dig)
+            rc = lc_regex_match_dev(e, fd->regs[l], e->fl_dig.as<uint8_t>(), dig_bytes, doff, dlen, n,
+                                    m + (nl + l) * n);
+        if (rc)
+            return rc;
+    }
+    uint8_t* k = e->fl_keep.as<uint8_t>() + 16;
+    lck::launch_filter_eval(c, f, t.status, n, m, k, reinterpret_cast<unsigned long long*>(removed), e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    *keep = k;
+    *d_removed = removed;
+    return LC_OK;
 }
 
 // The size pass and the emit of the chain over n pieces (serialize_sls_dev): into d_out (the device-fed call), or
@@ -2801,7 +2874,7 @@ int split_regex_sls_config(lc_engine_t* e, const char* what, uint64_t src_len, S
 // discarded; set whenever the size pass ran.
 int split_regex_sls_run(lc_engine_t* e, const char* what, const LcSplitRegexSlsCfg& c, const lck::RegexSlsTables& t,
                         uint64_t n, uint8_t* d_out, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
-                        uint64_t counters[3], const Lz4Tail* z) {
+                        uint64_t counters[3], const Lz4Tail* z, const uint8_t* keep = nullptr) {
     uint64_t ctr[4] = {0, 0, 0, 0}; // + pieces whose record would reach 4 GiB
     SlsTo to;
     to.host = out;
@@ -2810,7 +2883,7 @@ int split_regex_sls_run(lc_engine_t* e, const char* what, const LcSplitRegexSlsC
     const int rc = serialize_sls_dev(
         e, what, n, 4,
         [&](uint32_t* rec, uint32_t* body, unsigned long long* d_ctr) {
-            lck::launch_split_regex_sls_sizes(c, t, n, rec, body, d_ctr, e->stream);
+            lck::launch_split_regex_sls_sizes(c, t, n, keep, rec, body, d_ctr, e->stream);
         },
         [&](const uint64_t* rec_off, const uint32_t* body, uint8_t* dst) {
             lck::launch_split_regex_sls_emit(c, t, n, rec_off, body, dst, e->stream);
@@ -2822,19 +2895,22 @@ int split_regex_sls_run(lc_engine_t* e, const char* what, const LcSplitRegexSlsC
 
 // Host-buffer split + regex + serialise (lc_split_regex_parse_sls and the multiline / LZ4 siblings): the source goes
 // up once into `in`, `split(&n)` cuts it into the piece tables out_a / out_b (and out_c flags), the regex stage runs
-// over them into dr_status / dr_cap_off / dr_cap_len, and only the wire bytes (or their LZ4 block) come back.
+// over them into dr_status / dr_cap_off / dr_cap_len, and only the wire bytes (or their LZ4 block) come back.  With
+// fd (the _filter_ calls), the filter runs between the regex stage and the size pass and counters has a 4th entry.
 template <class Split>
 int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
                          Split split, SPLIT_REGEX_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
-                         uint64_t* n_events, uint64_t counters[3], const Lz4Tail* z) {
+                         uint64_t* n_events, uint64_t counters[3], const Lz4Tail* z,
+                         const lc_filter_desc_t* fd = nullptr) {
     if (!e || (!re && !whole_line) || !out_len || (len && !buf) || (z && (!z->raw_len || (z->len && !z->tail))))
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
     *out_len = 0;
     if (n_events)
         *n_events = 0;
-    uint64_t ctr[3] = {0, 0, 0};
+    uint64_t ctr[4] = {0, 0, 0, 0};
+    const size_t nctr = fd ? 4 : 3;
     if (counters)
-        memset(counters, 0, 3 * sizeof(uint64_t));
+        memset(counters, 0, nctr * sizeof(uint64_t));
     if (z)
         *z->raw_len = 0;
     int rc = whole_line ? (int)LC_OK : check_regex_usable(re, what);
@@ -2847,7 +2923,8 @@ int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re,
         return rc;
     const uint32_t G = whole_line ? 0u : re->res.ngroups;
     LcSplitRegexSlsCfg c;
-    rc = split_regex_sls_config(e, what, len, SPLIT_REGEX_ARGS, G, &c);
+    LcFilterSlsCfg f;
+    rc = split_regex_sls_config(e, what, len, SPLIT_REGEX_ARGS, G, &c, fd, &f);
     if (rc)
         return rc;
     uint64_t n = 0;
@@ -2882,9 +2959,20 @@ int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re,
                                 whole_line ? nullptr : e->dr_status.as<uint8_t>(),
                                 caps ? e->dr_cap_off.as<uint32_t>() : nullptr,
                                 caps ? e->dr_cap_len.as<uint32_t>() : nullptr};
-    rc = split_regex_sls_run(e, what, c, t, n, nullptr, out, out_cap, out_len, ctr, z);
+    const uint8_t* keep = nullptr;
+    const uint64_t* d_removed = nullptr;
+    if (fd) {
+        rc = filter_sls_run(e, what, c, f, fd, t, n, len, &keep, &d_removed);
+        if (rc)
+            return rc;
+    }
+    rc = split_regex_sls_run(e, what, c, t, n, nullptr, out, out_cap, out_len, ctr, z, keep);
+    if (d_removed && (rc == LC_OK || rc == LC_ERR_CAPACITY)) {
+        CU_TRY(cudaMemcpyAsync(&ctr[3], d_removed, 8, cudaMemcpyDeviceToHost, e->stream));
+        CU_TRY(cudaStreamSynchronize(e->stream));
+    }
     if (counters)
-        memcpy(counters, ctr, sizeof ctr);
+        memcpy(counters, ctr, nctr * sizeof(uint64_t));
     return rc;
 }
 
@@ -2892,10 +2980,54 @@ template <class Split>
 int split_regex_lz4_host(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
                          Split split, SPLIT_REGEX_PARAMS, const uint8_t* tail, uint64_t tail_len, uint8_t* out,
                          uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
-                         uint64_t counters[3]) {
+                         uint64_t counters[3], const lc_filter_desc_t* fd = nullptr) {
     const Lz4Tail z{tail, tail_len, raw_len};
     return split_regex_sls_host(e, what, re, buf, len, split, SPLIT_REGEX_ARGS, out, out_cap, out_len, n_events,
-                                counters, &z);
+                                counters, &z, fd);
+}
+
+// lc_sls_serialize_split_regex_dev and its _filter_ sibling (fd; counters then has a 4th entry)
+int split_regex_sls_dev(lc_engine_t* e, const char* what, const uint8_t* d_src, uint64_t src_len,
+                        const uint32_t* d_off, const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                        const uint32_t* d_cap_off, const uint32_t* d_cap_len, uint32_t row_pitch, SPLIT_REGEX_PARAMS,
+                        const lc_filter_desc_t* fd, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len,
+                        uint64_t* counters) {
+    const bool caps = !whole_line && nkeys && nkeys <= row_pitch; // the parsed plan reads the capture tables
+    if (!e || !out_len || (n && (!d_src || !d_off || !d_len)) || (n && !whole_line && !d_status) ||
+        (n && caps && (!d_cap_off || !d_cap_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    const size_t nctr = fd ? 4 : 3;
+    if (counters)
+        memset(counters, 0, nctr * sizeof(uint64_t));
+    if (src_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)row_pitch >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 pieces and < 2^32 captures per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcSplitRegexSlsCfg c;
+    LcFilterSlsCfg f;
+    rc = split_regex_sls_config(e, what, src_len, SPLIT_REGEX_ARGS, row_pitch, &c, fd, &f);
+    if (rc || n == 0)
+        return rc;
+    const lck::RegexSlsTables t{d_src, d_off, d_len, whole_line ? nullptr : d_status, caps ? d_cap_off : nullptr,
+                                caps ? d_cap_len : nullptr};
+    const uint8_t* keep = nullptr;
+    const uint64_t* d_removed = nullptr;
+    if (fd) {
+        rc = filter_sls_run(e, what, c, f, fd, t, n, src_len, &keep, &d_removed);
+        if (rc)
+            return rc;
+    }
+    uint64_t ctr[4] = {0, 0, 0, 0};
+    rc = split_regex_sls_run(e, what, c, t, n, d_out, nullptr, out_cap, out_len, ctr, nullptr, keep);
+    if (d_removed && (rc == LC_OK || rc == LC_ERR_CAPACITY)) {
+        CU_TRY(cudaMemcpyAsync(&ctr[3], d_removed, 8, cudaMemcpyDeviceToHost, e->stream));
+        CU_TRY(cudaStreamSynchronize(e->stream));
+    }
+    if (counters)
+        memcpy(counters, ctr, nctr * sizeof(uint64_t));
+    return rc;
 }
 
 } // namespace
@@ -2907,30 +3039,22 @@ int lc_sls_serialize_split_regex_dev(lc_engine_t* e, const uint8_t* d_src, uint6
                                      const uint32_t* d_cap_off, const uint32_t* d_cap_len, uint32_t row_pitch,
                                      SPLIT_REGEX_PARAMS, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len,
                                      uint64_t counters[3]) {
-    static const char* what = "lc_sls_serialize_split_regex_dev";
-    const bool caps = !whole_line && nkeys && nkeys <= row_pitch; // the parsed plan reads the capture tables
-    if (!e || !out_len || (n && (!d_src || !d_off || !d_len)) || (n && !whole_line && !d_status) ||
-        (n && caps && (!d_cap_off || !d_cap_len)))
+    return split_regex_sls_dev(e, "lc_sls_serialize_split_regex_dev", d_src, src_len, d_off, d_len, n, d_status,
+                               d_cap_off, d_cap_len, row_pitch, SPLIT_REGEX_ARGS, nullptr, d_out, out_cap, out_len,
+                               counters);
+}
+
+int lc_sls_serialize_split_regex_filter_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len,
+                                            const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+                                            const uint8_t* d_status, const uint32_t* d_cap_off,
+                                            const uint32_t* d_cap_len, uint32_t row_pitch, SPLIT_REGEX_PARAMS,
+                                            const lc_filter_desc_t* filter, uint8_t* d_out, uint64_t out_cap,
+                                            uint64_t* out_len, uint64_t counters[4]) {
+    static const char* what = "lc_sls_serialize_split_regex_filter_dev";
+    if (!filter)
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
-    *out_len = 0;
-    if (counters)
-        memset(counters, 0, 3 * sizeof(uint64_t));
-    if (src_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)row_pitch >= (1ull << 32))
-        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 pieces and < 2^32 captures per call");
-    int rc = bind(e);
-    if (rc)
-        return rc;
-    LcSplitRegexSlsCfg c;
-    rc = split_regex_sls_config(e, what, src_len, SPLIT_REGEX_ARGS, row_pitch, &c);
-    if (rc || n == 0)
-        return rc;
-    const lck::RegexSlsTables t{d_src, d_off, d_len, whole_line ? nullptr : d_status, caps ? d_cap_off : nullptr,
-                                caps ? d_cap_len : nullptr};
-    uint64_t ctr[3] = {0, 0, 0};
-    rc = split_regex_sls_run(e, what, c, t, n, d_out, nullptr, out_cap, out_len, ctr, nullptr);
-    if (counters)
-        memcpy(counters, ctr, sizeof ctr);
-    return rc;
+    return split_regex_sls_dev(e, what, d_src, src_len, d_off, d_len, n, d_status, d_cap_off, d_cap_len, row_pitch,
+                               SPLIT_REGEX_ARGS, filter, d_out, out_cap, out_len, counters);
 }
 
 int lc_split_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
@@ -2982,6 +3106,62 @@ int lc_multiline_split_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re,
     return split_regex_lz4_host(e, "lc_multiline_split_regex_parse_sls_lz4", re, buf, len, ML_SPLIT,
                                 SPLIT_REGEX_ARGS, tail, tail_len, out, out_cap, out_len, raw_len, n_events, counters);
 }
+
+#define FILTER_CHECK(name)                                                                                             \
+    if (!filter)                                                                                                       \
+        return fail(LC_ERR_INVALID_ARG, std::string(name) + ": bad arguments");
+
+int lc_split_regex_filter_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                    uint8_t split_char, SPLIT_REGEX_PARAMS, const lc_filter_desc_t* filter,
+                                    uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                    uint64_t counters[4]) {
+    FILTER_CHECK("lc_split_regex_filter_parse_sls")
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_regex_sls_host(e, "lc_split_regex_filter_parse_sls", re, buf, len, split, SPLIT_REGEX_ARGS, out,
+                                out_cap, out_len, n_events, counters, nullptr, filter);
+}
+
+int lc_split_regex_filter_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                        uint8_t split_char, SPLIT_REGEX_PARAMS, const lc_filter_desc_t* filter,
+                                        const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+                                        uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                                        uint64_t counters[4]) {
+    FILTER_CHECK("lc_split_regex_filter_parse_sls_lz4")
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_regex_lz4_host(e, "lc_split_regex_filter_parse_sls_lz4", re, buf, len, split, SPLIT_REGEX_ARGS, tail,
+                                tail_len, out, out_cap, out_len, raw_len, n_events, counters, filter);
+}
+
+int lc_multiline_split_regex_filter_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                              const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                              int discard_unmatched, SPLIT_REGEX_PARAMS,
+                                              const lc_filter_desc_t* filter, uint8_t* out, uint64_t out_cap,
+                                              uint64_t* out_len, uint64_t* n_events, uint64_t counters[4],
+                                              uint64_t ml_counters[3]) {
+    FILTER_CHECK("lc_multiline_split_regex_filter_parse_sls")
+    return split_regex_sls_host(e, "lc_multiline_split_regex_filter_parse_sls", re, buf, len, ML_SPLIT,
+                                SPLIT_REGEX_ARGS, out, out_cap, out_len, n_events, counters, nullptr, filter);
+}
+
+int lc_multiline_split_regex_filter_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf,
+                                                  uint64_t len, const lc_regex_t* start, const lc_regex_t* cont,
+                                                  const lc_regex_t* end, int discard_unmatched, SPLIT_REGEX_PARAMS,
+                                                  const lc_filter_desc_t* filter, const uint8_t* tail,
+                                                  uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+                                                  uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                                                  uint64_t counters[4], uint64_t ml_counters[3]) {
+    FILTER_CHECK("lc_multiline_split_regex_filter_parse_sls_lz4")
+    return split_regex_lz4_host(e, "lc_multiline_split_regex_filter_parse_sls_lz4", re, buf, len, ML_SPLIT,
+                                SPLIT_REGEX_ARGS, tail, tail_len, out, out_cap, out_len, raw_len, n_events, counters,
+                                filter);
+}
+#undef FILTER_CHECK
 #undef ML_SPLIT
 
 } // extern "C"

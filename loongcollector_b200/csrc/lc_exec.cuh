@@ -1988,6 +1988,148 @@ inline const char* lc_split_regex_sls_setup(const char* const* keys, const uint3
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// f4, split -> regex -> filter chain: ProcessorFilterNative (ProcessorFilterNative.cpp:83-117,459-486) behind the
+// split -> regex chain.  The filter sees the event the regex stage left behind, so a leaf's key resolves once, on the
+// host, through that stage's two content plans to a value source per verdict (parsed / failed): capture j, the piece
+// (LC_REGEX_SLS_LINE), the piece's offset digits (LC_REGEX_SLS_DIGITS) or absent.  A leaf is regex_match of that
+// value, false when the key is absent; the leaves combine through a postfix program of not / and / or.  In RULE and
+// EXPRESSION mode (nprog > 0) an event without contents is removed whatever the leaves say; BYPASS (nprog == 0) keeps
+// every event.  The regex stage's counters are not moved: it counted every piece before the filter ran.
+
+#define LC_FILTER_SLS_LEAVES 32        // leaves per filter (lc_b200.h: LC_FILTER_MAX_LEAVES)
+#define LC_FILTER_SLS_PROG 128         // program entries per filter (lc_b200.h: LC_FILTER_MAX_PROG)
+#define LC_FILTER_SLS_ABSENT 0xFFFFFFFDu // value source of a leaf: its key is not in the event
+#define LC_FILTER_SLS_NOT 0xFFFFFFFDu  // program opcodes (lc_b200.h: LC_FILTER_NOT / _AND / _OR)
+#define LC_FILTER_SLS_AND 0xFFFFFFFEu
+#define LC_FILTER_SLS_OR 0xFFFFFFFFu
+#define LC_FILTER_SLS_DIGIT_PITCH 20u  // bytes per row of the digit scratch: the longest decimal u64
+
+struct LcFilterSlsCfg {
+    uint32_t nleaves;
+    uint32_t nprog;                        // 0: BYPASS mode, every event is kept
+    uint32_t src[LC_FILTER_SLS_LEAVES][2]; // value source of leaf l in a parsed [0] / failed [1] row
+    uint32_t empty[2];                     // the parsed / failed event has no contents
+    uint32_t any_digits;                   // some leaf reads the offset digits
+    uint8_t prog[LC_FILTER_SLS_PROG];      // leaf index, or 253 / 254 / 255 = not / and / or
+};
+
+// Host side: resolve the leaves against the chain's plans (lc_regex_sls_plans: entries [0, n_ok) parsed, then n_fail
+// failed; key id k names kstr[k] / klen[k]) and check the program.  Returns nullptr, or why the filter is refused: more
+// than LC_FILTER_SLS_LEAVES leaves or LC_FILTER_SLS_PROG entries, an entry that is neither a leaf nor an opcode, a pop
+// of an empty stack, a stack deeper than 32, or a program that does not leave exactly one value.
+inline const char* lc_filter_sls_setup(const uint32_t* plan, uint32_t n_ok, uint32_t n_fail, const char* const* kstr,
+                                       const uint32_t* klen, uint32_t nleaves, const char* const* leaf_keys,
+                                       const uint32_t* leaf_lens, uint32_t nprog, const uint32_t* prog,
+                                       LcFilterSlsCfg* f) {
+    if (!f || !plan || (nleaves && (!leaf_keys || !leaf_lens)) || (nprog && !prog))
+        return "bad arguments";
+    if (nleaves > LC_FILTER_SLS_LEAVES)
+        return "too many filter leaves";
+    if (nprog > LC_FILTER_SLS_PROG)
+        return "filter program too long";
+    memset(f, 0, sizeof *f);
+    f->nleaves = nleaves;
+    f->nprog = nprog;
+    f->empty[0] = n_ok == 0u;
+    f->empty[1] = n_fail == 0u;
+    uint32_t depth = 0;
+    for (uint32_t k = 0; k < nprog; ++k) {
+        const uint32_t op = prog[k];
+        if (op < nleaves) {
+            if (++depth > 32u)
+                return "filter program too deep";
+            f->prog[k] = (uint8_t)op;
+        } else if (op == LC_FILTER_SLS_NOT) {
+            if (depth < 1u)
+                return "malformed filter program";
+            f->prog[k] = 253;
+        } else if (op == LC_FILTER_SLS_AND || op == LC_FILTER_SLS_OR) {
+            if (depth < 2u)
+                return "malformed filter program";
+            --depth;
+            f->prog[k] = op == LC_FILTER_SLS_AND ? 254 : 255;
+        } else {
+            return "malformed filter program";
+        }
+    }
+    if (nprog && depth != 1u)
+        return "malformed filter program";
+    for (uint32_t l = 0; l < nleaves; ++l) {
+        if (leaf_lens[l] && !leaf_keys[l])
+            return "bad arguments";
+        for (uint32_t v = 0; v < 2; ++v) {
+            const uint32_t* e = plan + (v ? 2u * n_ok : 0u);
+            uint32_t s = LC_FILTER_SLS_ABSENT;
+            for (uint32_t k = 0; k < (v ? n_fail : n_ok); ++k) {
+                const uint32_t kid = e[2 * k];
+                if (klen[kid] == leaf_lens[l] && (!leaf_lens[l] || !memcmp(kstr[kid], leaf_keys[l], leaf_lens[l]))) {
+                    s = e[2 * k + 1]; // a plan's keys are unique
+                    break;
+                }
+            }
+            f->src[l][v] = s;
+            f->any_digits |= s == LC_REGEX_SLS_DIGITS;
+        }
+    }
+    return nullptr;
+}
+
+// The row's value source for leaf l: LC_FILTER_SLS_ABSENT, LC_REGEX_SLS_DIGITS, LC_REGEX_SLS_LINE or capture j.  An
+// erased row (failed without KeepingSourceWhenParseFail) never reaches the filter; its failed plan is empty.
+LC_HD uint32_t lc_filter_leaf_src(const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f, uint32_t l, uint32_t status) {
+    return f.src[l][lc_regex_sls_verdict(c.x, status) == 0u ? 0 : 1];
+}
+
+// The leaf's value in row r: *off / *len into the source value (the piece or a capture), or *len = the digit count of
+// the piece's offset.  Returns the source (absent: *off = *len = 0).
+LC_HD uint32_t lc_filter_leaf(const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f, uint32_t l,
+                              const LcSplitRegexSlsRow& r, uint32_t* off, uint32_t* len) {
+    const uint32_t s = lc_filter_leaf_src(c, f, l, r.status);
+    *off = 0;
+    *len = 0;
+    if (s == LC_REGEX_SLS_DIGITS)
+        *len = lc_dec_digits(c.src_pos + r.po);
+    else if (s == LC_REGEX_SLS_LINE)
+        *off = r.po, *len = r.plen;
+    else if (s != LC_FILTER_SLS_ABSENT)
+        *off = r.co[s], *len = r.cl[s];
+    return s;
+}
+
+// The filter's verdict on an event that reached it: 1 kept, 0 removed.  bits: bit l = leaf l held (an absent key
+// holds no leaf).  empty: the event has no contents.
+LC_HD uint32_t lc_filter_eval(const LcFilterSlsCfg& f, uint32_t bits, bool empty) {
+    if (f.nprog == 0u)
+        return 1u;
+    if (empty)
+        return 0u;
+    uint32_t st = 0, sp = 0; // the stack, bit sp - 1 on top
+    for (uint32_t k = 0; k < f.nprog; ++k) {
+        const uint32_t op = f.prog[k];
+        if (op < LC_FILTER_SLS_LEAVES) {
+            st = (st & ~(1u << sp)) | (((bits >> op) & 1u) << sp);
+            ++sp;
+        } else if (op == 253u) {
+            st ^= 1u << (sp - 1);
+        } else {
+            --sp;
+            const uint32_t a = (st >> (sp - 1)) & 1u, b = (st >> sp) & 1u;
+            const uint32_t v = op == 254u ? (a & b) : (a | b);
+            st = (st & ~(1u << (sp - 1))) | (v << (sp - 1));
+        }
+    }
+    return st & 1u;
+}
+
+// The row's verdicts behind the filter: *reached = the regex stage kept it, *empty = it has no contents.
+LC_HD void lc_filter_row_state(const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f, uint32_t status, bool* reached,
+                               bool* empty) {
+    const bool ok = lc_regex_sls_verdict(c.x, status) == 0u;
+    *reached = ok || c.x.keep_fail;
+    *empty = f.empty[ok ? 0 : 1] != 0u;
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // f4, LZ4: one LZ4 *block* (what LZ4_compress_default emits and the SLS server decodes with x-log-bodyrawsize) per
 // segment.  A segment is cut into chunks of LC_LZ4_CHUNK bytes; the bytes are a sequential function of the segment:
 //   candidate(p)  = the latest q < p with hash(q) == hash(p), kept as q mod 2^16 (so read as the q' = p - d with

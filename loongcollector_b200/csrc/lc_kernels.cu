@@ -3617,16 +3617,18 @@ __device__ __forceinline__ LcSplitRegexSlsRow split_regex_sls_row(const LcSplitR
     return r;
 }
 
+// keep (or nullptr): a filter's verdict per piece; a removed piece gets size 0 and is never counted as too large
 __global__ void __launch_bounds__(256)
-    split_regex_sls_size_kernel(LcSplitRegexSlsCfg c, RegexSlsTables t, uint64_t n, uint32_t* __restrict__ rec_size,
-                                uint32_t* __restrict__ body_size, unsigned long long* __restrict__ counters) {
+    split_regex_sls_size_kernel(LcSplitRegexSlsCfg c, RegexSlsTables t, uint64_t n, const uint8_t* __restrict__ keep,
+                                uint32_t* __restrict__ rec_size, uint32_t* __restrict__ body_size,
+                                unsigned long long* __restrict__ counters) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     LcSplitRegexVerdict v{0u, 0u, 0u};
     uint32_t big = 0;
     if (i < n) {
         const LcSplitRegexSlsRow r = split_regex_sls_row(c, t, i);
         LcSlsCount64 s{0};
-        const uint32_t cnt = lc_split_regex_sls_body(c, t.base, r, s);
+        const uint32_t cnt = keep && !keep[i] ? 0u : lc_split_regex_sls_body(c, t.base, r, s);
         big = s.n + 16 > 0xFFFFFFFFull;
         const uint32_t body = cnt && !big ? (uint32_t)s.n : 0u;
         rec_size[i] = body ? 1 + lc_varint_size(body) + body : 0u;
@@ -3668,11 +3670,80 @@ __global__ void __launch_bounds__(256)
 }
 
 void launch_split_regex_sls_sizes(const LcSplitRegexSlsCfg& c, const RegexSlsTables& t, uint64_t n,
-                                  uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
-                                  cudaStream_t st) {
+                                  const uint8_t* d_keep, uint32_t* d_rec_size, uint32_t* d_body_size,
+                                  unsigned long long* d_counters, cudaStream_t st) {
     if (n)
-        split_regex_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_size, d_body_size,
-                                                                                  d_counters);
+        split_regex_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, n, d_keep, d_rec_size,
+                                                                                  d_body_size, d_counters);
+}
+
+// ---- f4, split -> regex -> filter chain (lc_exec.cuh: lc_filter_leaf, lc_filter_eval), one thread per piece.  The
+// tap writes leaf l's values as a dense table over the source value (off / len; 0 / 0 where the value is absent or is
+// the offset digits) and, with dig, a second table over the digit scratch (row i's digits at dig + 20 i; 0 / 0 where
+// the value is not the digits), so that the boolean match runs over each base in turn.
+__global__ void __launch_bounds__(256)
+    filter_tap_kernel(LcSplitRegexSlsCfg c, LcFilterSlsCfg f, uint32_t leaf, RegexSlsTables t, uint64_t n,
+                      uint32_t* __restrict__ off, uint32_t* __restrict__ len, uint32_t* __restrict__ doff,
+                      uint32_t* __restrict__ dlen, uint8_t* __restrict__ dig) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n)
+        return;
+    const LcSplitRegexSlsRow r = split_regex_sls_row(c, t, i);
+    uint32_t o, l;
+    const uint32_t s = lc_filter_leaf(c, f, leaf, r, &o, &l);
+    const bool digits = s == LC_REGEX_SLS_DIGITS;
+    off[i] = digits ? 0u : o;
+    len[i] = digits ? 0u : l;
+    if (doff) {
+        const uint32_t at = (uint32_t)i * LC_FILTER_SLS_DIGIT_PITCH;
+        doff[i] = digits ? at : 0u;
+        dlen[i] = digits ? l : 0u;
+        const uint64_t pos = c.src_pos + r.po;
+        for (uint32_t j = 0; digits && j < l; ++j)
+            dig[at + j] = lc_dec_digit(pos, j, l);
+    }
+}
+
+// keep[i] = the filter's verdict; counters[0] += pieces the filter removed (one atomic per warp).  m: the match bytes,
+// [l * n + i] over the source value and, with f.any_digits, [(nleaves + l) * n + i] over the digit scratch.
+__global__ void __launch_bounds__(256)
+    filter_eval_kernel(LcSplitRegexSlsCfg c, LcFilterSlsCfg f, const uint8_t* __restrict__ status, uint64_t n,
+                       const uint8_t* __restrict__ m, uint8_t* __restrict__ keep,
+                       unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t removed = 0;
+    if (i < n) {
+        const uint32_t st = c.x.whole_line ? 0u : status[i];
+        bool reached, empty;
+        lc_filter_row_state(c, f, st, &reached, &empty);
+        uint32_t bits = 0;
+        for (uint32_t l = 0; l < f.nleaves; ++l) {
+            const uint32_t s = lc_filter_leaf_src(c, f, l, st);
+            if (s != LC_FILTER_SLS_ABSENT)
+                bits |= (uint32_t)m[(uint64_t)(s == LC_REGEX_SLS_DIGITS ? f.nleaves + l : l) * n + i] << l;
+        }
+        const uint32_t k = reached ? lc_filter_eval(f, bits, empty) : 0u;
+        keep[i] = (uint8_t)k;
+        removed = reached && !k;
+    }
+    removed = __reduce_add_sync(0xFFFFFFFFu, removed);
+    if ((threadIdx.x & 31) == 0 && removed)
+        atomicAdd(counters, (unsigned long long)removed);
+}
+
+void launch_filter_tap(const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f, uint32_t leaf, const RegexSlsTables& t,
+                       uint64_t n, uint32_t* d_off, uint32_t* d_len, uint32_t* d_doff, uint32_t* d_dlen,
+                       uint8_t* d_dig, cudaStream_t st) {
+    if (n)
+        filter_tap_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, f, leaf, t, n, d_off, d_len, d_doff, d_dlen,
+                                                                        d_dig);
+}
+
+void launch_filter_eval(const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f, const uint8_t* d_status, uint64_t n,
+                        const uint8_t* d_match, uint8_t* d_keep, unsigned long long* d_counters, cudaStream_t st) {
+    if (n)
+        filter_eval_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, f, d_status, n, d_match, d_keep,
+                                                                         d_counters);
 }
 
 void launch_split_regex_sls_emit(const LcSplitRegexSlsCfg& c, const RegexSlsTables& t, uint64_t n,

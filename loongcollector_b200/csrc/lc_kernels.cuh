@@ -9,6 +9,7 @@ struct LcRegexSlsCfg;
 struct LcDelimRegexSlsCfg;
 struct LcSpanSlsCfg;
 struct LcSplitRegexSlsCfg;
+struct LcFilterSlsCfg;
 struct LcLz4Seq;
 struct LcLz4Chunk;
 
@@ -223,10 +224,20 @@ void launch_regex_sls_emit(const LcRegexSlsCfg& c, const RegexSlsTables& t, cons
 // f4, split -> regex chain: Log records of the pieces t.ev_off / t.ev_len of the source value t.base, parsed into the
 // regex tables of t (lc_exec.cuh: LcSplitRegexSlsCfg, plans and key strings on the device).  Sizes as for
 // launch_sls_sizes; d_counters: u64 [4] += successful, failed (LC_REGEX_NOMATCH), discarded pieces, and pieces whose
-// record would reach 4 GiB.
+// record would reach 4 GiB.  d_keep (or nullptr): a filter's verdict per piece (launch_filter_eval); a removed piece
+// has no record.
 void launch_split_regex_sls_sizes(const LcSplitRegexSlsCfg& c, const RegexSlsTables& t, uint64_t n,
-                                  uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
-                                  cudaStream_t st);
+                                  const uint8_t* d_keep, uint32_t* d_rec_size, uint32_t* d_body_size,
+                                  unsigned long long* d_counters, cudaStream_t st);
+// f4, split -> regex -> filter chain (lc_exec.cuh: LcFilterSlsCfg).  launch_filter_tap: leaf's values as a dense
+// (d_off, d_len) table over t.base and, with d_doff, a (d_doff, d_dlen) table over the digit scratch d_dig (20 bytes
+// per piece).  launch_filter_eval: d_keep[i] = the filter's verdict from the match bytes d_match (lc_regex_match_dev
+// over those tables, [l * n + i] and, with digits, [(nleaves + l) * n + i]); d_counters: u64 [1] += removed pieces.
+void launch_filter_tap(const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f, uint32_t leaf, const RegexSlsTables& t,
+                       uint64_t n, uint32_t* d_off, uint32_t* d_len, uint32_t* d_doff, uint32_t* d_dlen,
+                       uint8_t* d_dig, cudaStream_t st);
+void launch_filter_eval(const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f, const uint8_t* d_status, uint64_t n,
+                        const uint8_t* d_match, uint8_t* d_keep, unsigned long long* d_counters, cudaStream_t st);
 void launch_split_regex_sls_emit(const LcSplitRegexSlsCfg& c, const RegexSlsTables& t, uint64_t n,
                                  const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
                                  cudaStream_t st);

@@ -1285,6 +1285,59 @@ bool ProcessorFilterNative::Init(const Json::Value& config) {
             mFilterMode = Mode::RULE_MODE;
     }
     GetBool(config, "DiscardingNonUTF8", mDiscardingNonUTF8);
+    BuildDeviceFilter();
+    return true;
+}
+
+void ProcessorFilterNative::BuildDeviceFilter() {
+    mDevKeys.clear();
+    mDevKeyLens.clear();
+    mDevRegs.clear();
+    mDevProg.clear();
+    for (const Leaf& l : mLeaves) {
+        mDevKeys.push_back(l.key.data());
+        mDevKeyLens.push_back((uint32_t)l.key.size());
+        mDevRegs.push_back(l.reg->get());
+    }
+    uint32_t depth = 0, maxDepth = 0;
+    auto push = [&](uint32_t op) {
+        mDevProg.push_back(op);
+        depth = op < LC_FILTER_NOT ? depth + 1 : op == LC_FILTER_NOT ? depth : depth - 1;
+        maxDepth = depth > maxDepth ? depth : maxDepth;
+    };
+    if (mFilterMode == Mode::RULE_MODE) {
+        for (size_t li = 0; li < mLeaves.size(); ++li) {
+            push((uint32_t)li);
+            if (li)
+                push(LC_FILTER_AND);
+        }
+    } else if (mFilterMode == Mode::EXPRESSION_MODE) {
+        auto post = [&](auto&& self, int node) -> void {
+            const Node& n = mNodes[node];
+            if (n.op == 0) {
+                push((uint32_t)n.leaf);
+                return;
+            }
+            self(self, n.left);
+            if (n.op != 1)
+                self(self, n.right);
+            push(n.op == 1 ? LC_FILTER_NOT : n.op == 2 ? LC_FILTER_AND : LC_FILTER_OR);
+        };
+        post(post, mRoot);
+    }
+    mDeviceOk = !mDiscardingNonUTF8 && mLeaves.size() <= LC_FILTER_MAX_LEAVES &&
+                mDevProg.size() <= LC_FILTER_MAX_PROG && maxDepth <= 32;
+}
+
+bool ProcessorFilterNative::DeviceFilter(lc_filter_desc_t* d) const {
+    if (!mDeviceOk)
+        return false;
+    d->nleaves = (uint32_t)mLeaves.size();
+    d->keys = mDevKeys.data();
+    d->key_lens = mDevKeyLens.data();
+    d->regs = mDevRegs.data();
+    d->nprog = (uint32_t)mDevProg.size();
+    d->prog = mDevProg.data();
     return true;
 }
 
@@ -1921,10 +1974,11 @@ bool RunSlsLz4DevicePass(Call call, size_t estimate, const SLSEventGroupSerializ
 // the records are concatenated in event order; counters[3] += the ctr of each source event's last call.  The records
 // are what CreateNewEvent builds (ProcessorSplitLogStringNative.cpp:131-161): RAW events serialise as "content" ->
 // piece; LOG events as SourceKey -> piece plus, with log.file.offset metadata, that key -> the piece's file offset.
-// An empty value emits nothing.  counters[3..6) are a chained regex stage's (successful, failed, discarded).
+// An empty value emits nothing.  counters[3..6) are a chained regex stage's (successful, failed, discarded),
+// counters[6] the events a filter behind it removed.
 template <class Call>
 bool SplitSerializeSls(PipelineEventGroup& group, bool enableNs, const std::string& sourceKey, bool raw, Call call,
-                       const char* what, std::string& out, std::string& err, uint64_t counters[6]) {
+                       const char* what, std::string& out, std::string& err, uint64_t counters[7]) {
     SLSEventGroupSerializer ser;
     ser.mEnableTimestampNanosecond = enableNs;
     static const std::string kRawKey = "content"; // DEFAULT_CONTENT_KEY (SLSSerializer.cpp:366-374)
@@ -1944,7 +1998,7 @@ bool SplitSerializeSls(PipelineEventGroup& group, bool enableNs, const std::stri
             continue;
         const uint32_t ns =
             enableNs && src.GetTimestampNanosecond() ? src.GetTimestampNanosecond().value() : LC_SLS_NO_NS;
-        uint64_t need = 0, nev = 0, ctr[6];
+        uint64_t need = 0, nev = 0, ctr[7];
         RunSlsDevicePass(
             [&](uint8_t* o, uint64_t cap, uint64_t* len) {
                 memset(ctr, 0, sizeof ctr); // (a second, exactly sized call must not count the lines twice)
@@ -1957,10 +2011,10 @@ bool SplitSerializeSls(PipelineEventGroup& group, bool enableNs, const std::stri
         // (else the group is over the size limit: the sizes still add up for the error message)
         total += need;
         nEvents += nev;
-        for (int k = 0; k < 6; ++k)
+        for (int k = 0; k < 7; ++k)
             counters[k] += ctr[k];
     }
-    return FinishSls(ser, nEvents, counters[5], total, res, tail, out, err);
+    return FinishSls(ser, nEvents, counters[5] + counters[6], total, res, tail, out, err);
 }
 } // namespace
 
@@ -2007,14 +2061,15 @@ struct SplitRegexStage {
 namespace {
 // The split -> regex chain of either splitter: `process(group)` is the splitter's Process; the device calls are
 // sls(val, okey, pos, time, ns, out, cap, &len, &nev, rctr, sctr) and lz4(val, okey, pos, time, ns, tail, tailLen,
-// out, cap, &len, &raw, &nev, rctr, sctr) (rctr[3] = the regex stage's counters, sctr[3] = the splitter's).
-// sctr_total[3] += the splitter's counters of every device call.  rawSize null: out = the wire bytes; else out = their
-// LZ4 block and *rawSize their size.
+// out, cap, &len, &raw, &nev, rctr, sctr) (rctr[4] = the regex stage's counters and the filter's removed events,
+// sctr[3] = the splitter's).  filter (or nullptr): the filter behind the regex stage, whose rule the device calls take
+// when filterOk.  sctr_total[3] += the splitter's counters of every device call.  rawSize null: out = the wire bytes;
+// else out = their LZ4 block and *rawSize their size.
 template <class ProcessFn, class Sls, class Lz4>
-bool SplitRegexChainSls(PipelineEventGroup& group, const SplitRegexStage& x, const std::string& sourceKey,
-                        bool rawContent, bool enableNs, std::string& out, uint64_t* rawSize, std::string& err,
-                        ProcessFn process, Sls sls, Lz4 lz4, const char* what, const char* lzwhat,
-                        uint64_t sctrTotal[3]) {
+bool SplitRegexChainSls(PipelineEventGroup& group, const SplitRegexStage& x, ProcessorFilterNative* filter,
+                        bool filterOk, const std::string& sourceKey, bool rawContent, bool enableNs, std::string& out,
+                        uint64_t* rawSize, std::string& err, ProcessFn process, Sls sls, Lz4 lz4, const char* what,
+                        const char* lzwhat, uint64_t sctrTotal[3]) {
     SLSEventGroupSerializer ser;
     ser.mEnableTimestampNanosecond = enableNs;
     const bool hasOffset = group.HasMetadata(EventGroupMetaKey::LOG_FILE_OFFSET_KEY);
@@ -2022,9 +2077,11 @@ bool SplitRegexChainSls(PipelineEventGroup& group, const SplitRegexStage& x, con
     if (hasOffset && !okey.data())
         okey = StringView(""); // an empty key is still a key: the C-ABI reads NULL as "no offset key"
     const StringView* okp = hasOffset ? &okey : nullptr;
-    if (rawContent || !IsFlatGroup(group, sourceKey) || !x.Accepts(sourceKey, okp)) {
+    if (rawContent || !IsFlatGroup(group, sourceKey) || !x.Accepts(sourceKey, okp) || (filter && !filterOk)) {
         process(group);
         x.r.Process(group);
+        if (filter)
+            filter->Process(group);
         if (!rawSize)
             return ser.Serialize(group, out, err);
         std::string raw;
@@ -2039,16 +2096,18 @@ bool SplitRegexChainSls(PipelineEventGroup& group, const SplitRegexStage& x, con
         const uint32_t ns =
             enableNs && src.GetTimestampNanosecond() ? src.GetTimestampNanosecond().value() : LC_SLS_NO_NS;
         const std::string tail = SlsGroupTail(group);
-        uint64_t nev = 0, rctr[3] = {0, 0, 0}, sctr[3] = {0, 0, 0};
+        uint64_t nev = 0, gone = 0, rctr[4] = {0, 0, 0, 0}, sctr[3] = {0, 0, 0};
         const bool ok = RunSlsLz4DevicePass(
             [&](uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw) {
                 memset(rctr, 0, sizeof rctr);
                 memset(sctr, 0, sizeof sctr);
-                return lz4(val, okp, src.GetPosition().first, (uint32_t)src.GetTimestamp(), ns,
-                           reinterpret_cast<const uint8_t*>(tail.data()), (uint64_t)tail.size(), o, cap, len, raw,
-                           &nev, rctr, sctr);
+                const int rc = lz4(val, okp, src.GetPosition().first, (uint32_t)src.GetTimestamp(), ns,
+                                   reinterpret_cast<const uint8_t*>(tail.data()), (uint64_t)tail.size(), o, cap, len,
+                                   raw, &nev, rctr, sctr);
+                gone = rctr[2] + rctr[3]; // erased by the regex stage or removed by the filter
+                return rc;
             },
-            2 * val.size() + 4096 + tail.size(), ser, nev, rctr[2], tail.size(), out, *rawSize, err, lzwhat);
+            2 * val.size() + 4096 + tail.size(), ser, nev, gone, tail.size(), out, *rawSize, err, lzwhat);
         x.Add(rctr);
         for (int k = 0; k < 3; ++k)
             sctrTotal[k] += sctr[k];
@@ -2058,7 +2117,7 @@ bool SplitRegexChainSls(PipelineEventGroup& group, const SplitRegexStage& x, con
                     uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* ctr) {
         return sls(val, ok, pos, time, ns, o, cap, len, nev, ctr + 3, ctr);
     };
-    uint64_t ctr[6] = {0, 0, 0, 0, 0, 0};
+    uint64_t ctr[7] = {0, 0, 0, 0, 0, 0, 0};
     std::string raw;
     const bool ok = SplitSerializeSls(group, enableNs, sourceKey, false, call, what, rawSize ? raw : out, err, ctr);
     x.Add(ctr + 3);
@@ -2190,7 +2249,7 @@ bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, bool
                             key.data(), (uint32_t)key.size(), okey ? okey->data() : nullptr,
                             okey ? (uint32_t)okey->size() : 0u, pos, time, ns, o, cap, len, nev);
     };
-    uint64_t unused[6] = {0, 0, 0, 0, 0, 0};
+    uint64_t unused[7] = {0, 0, 0, 0, 0, 0, 0};
     return SplitSerializeSls(group, enableNs, mSourceKey, mEnableRawContent, call, "lc_split_sls", out, err, unused);
 }
 
@@ -2211,7 +2270,7 @@ bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& gr
                                       o, cap, len, nev, ctr);
     };
     // matched_events, input lines, unmatched lines: moved as Process moves them (:82-84,106-107)
-    uint64_t ctr[6] = {0, 0, 0, 0, 0, 0};
+    uint64_t ctr[7] = {0, 0, 0, 0, 0, 0, 0};
     const bool ok = SplitSerializeSls(group, enableNs, mSourceKey, mEnableRawContent, call, "lc_multiline_split_sls",
                                       out, err, ctr);
     mMatchedEventsTotal.Add(ctr[0]);
@@ -2222,79 +2281,131 @@ bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& gr
 
 bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
                                                  bool enableNs, std::string& out, std::string& err) {
-    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+    return ChainSerializeSls(group, next, nullptr, enableNs, out, nullptr, err);
 }
 
 bool ProcessorSplitLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next,
                                                     bool enableNs, std::string& block, uint64_t& rawSize,
                                                     std::string& err) {
-    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+    return ChainSerializeSls(group, next, nullptr, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                                                 ProcessorFilterNative& filter, bool enableNs, std::string& out,
+                                                 std::string& err) {
+    return ChainSerializeSls(group, next, &filter, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                                                    ProcessorFilterNative& filter, bool enableNs, std::string& block,
+                                                    uint64_t& rawSize, std::string& err) {
+    return ChainSerializeSls(group, next, &filter, enableNs, block, &rawSize, err);
 }
 
 bool ProcessorSplitLogStringNative::ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
-                                                      bool enableNs, std::string& out, uint64_t* rawSize,
-                                                      std::string& err) {
+                                                      ProcessorFilterNative* filter, bool enableNs, std::string& out,
+                                                      uint64_t* rawSize, std::string& err) {
     const SplitRegexStage x(next);
+    lc_filter_desc_t fd{};
+    const bool filterOk = filter && filter->DeviceFilter(&fd);
     auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
     auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
                    uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t*) {
-        return lc_split_regex_parse_sls(Engine(), x.re, src(val), val.size(), (uint8_t)mSplitChar,
-                                        SPLIT_REGEX_STAGE_ARGS(x), okey ? okey->data() : nullptr,
-                                        okey ? (uint32_t)okey->size() : 0u, pos, time, ns, o, cap, len, nev, rctr);
+        const char* ok = okey ? okey->data() : nullptr;
+        const uint32_t okl = okey ? (uint32_t)okey->size() : 0u;
+        return filter ? lc_split_regex_filter_parse_sls(Engine(), x.re, src(val), val.size(), (uint8_t)mSplitChar,
+                                                        SPLIT_REGEX_STAGE_ARGS(x), ok, okl, pos, time, ns, &fd, o, cap,
+                                                        len, nev, rctr)
+                      : lc_split_regex_parse_sls(Engine(), x.re, src(val), val.size(), (uint8_t)mSplitChar,
+                                                 SPLIT_REGEX_STAGE_ARGS(x), ok, okl, pos, time, ns, o, cap, len, nev,
+                                                 rctr);
     };
     auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
                    const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
                    uint64_t* nev, uint64_t* rctr, uint64_t*) {
-        return lc_split_regex_parse_sls_lz4(Engine(), x.re, src(val), val.size(), (uint8_t)mSplitChar,
-                                            SPLIT_REGEX_STAGE_ARGS(x), okey ? okey->data() : nullptr,
-                                            okey ? (uint32_t)okey->size() : 0u, pos, time, ns, tail, tailLen, o, cap,
-                                            len, raw, nev, rctr);
+        const char* ok = okey ? okey->data() : nullptr;
+        const uint32_t okl = okey ? (uint32_t)okey->size() : 0u;
+        return filter ? lc_split_regex_filter_parse_sls_lz4(Engine(), x.re, src(val), val.size(), (uint8_t)mSplitChar,
+                                                            SPLIT_REGEX_STAGE_ARGS(x), ok, okl, pos, time, ns, &fd,
+                                                            tail, tailLen, o, cap, len, raw, nev, rctr)
+                      : lc_split_regex_parse_sls_lz4(Engine(), x.re, src(val), val.size(), (uint8_t)mSplitChar,
+                                                     SPLIT_REGEX_STAGE_ARGS(x), ok, okl, pos, time, ns, tail, tailLen,
+                                                     o, cap, len, raw, nev, rctr);
     };
     uint64_t unused[3] = {0, 0, 0};
     return SplitRegexChainSls(
-        group, x, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
-        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_split_regex_parse_sls",
-        "lc_split_regex_parse_sls_lz4", unused);
+        group, x, filter, filterOk, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4,
+        filter ? "lc_split_regex_filter_parse_sls" : "lc_split_regex_parse_sls",
+        filter ? "lc_split_regex_filter_parse_sls_lz4" : "lc_split_regex_parse_sls_lz4", unused);
 }
 
 bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
                                                           bool enableNs, std::string& out, std::string& err) {
-    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+    return ChainSerializeSls(group, next, nullptr, enableNs, out, nullptr, err);
 }
 
 bool ProcessorSplitMultilineLogStringNative::SerializeSlsLz4(PipelineEventGroup& group,
                                                              ProcessorParseRegexNative& next, bool enableNs,
                                                              std::string& block, uint64_t& rawSize, std::string& err) {
-    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+    return ChainSerializeSls(group, next, nullptr, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                                                          ProcessorFilterNative& filter, bool enableNs,
+                                                          std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, &filter, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSlsLz4(PipelineEventGroup& group,
+                                                             ProcessorParseRegexNative& next,
+                                                             ProcessorFilterNative& filter, bool enableNs,
+                                                             std::string& block, uint64_t& rawSize, std::string& err) {
+    return ChainSerializeSls(group, next, &filter, enableNs, block, &rawSize, err);
 }
 
 bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGroup& group,
-                                                               ProcessorParseRegexNative& next, bool enableNs,
+                                                               ProcessorParseRegexNative& next,
+                                                               ProcessorFilterNative* filter, bool enableNs,
                                                                std::string& out, uint64_t* rawSize, std::string& err) {
     const SplitRegexStage x(next);
+    lc_filter_desc_t fd{};
+    const bool filterOk = filter && filter->DeviceFilter(&fd);
     const bool discard = mMultiline.mUnmatchedContentTreatment == MultilineOptions::UnmatchedContentTreatment::DISCARD;
     auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
     auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
                    uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
-        return lc_multiline_split_regex_parse_sls(Engine(), x.re, src(val), val.size(), mStart.get(),
-                                                  mContinue.get(), mEnd.get(), discard, SPLIT_REGEX_STAGE_ARGS(x),
-                                                  okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u,
-                                                  pos, time, ns, o, cap, len, nev, rctr, sctr);
+        const char* ok = okey ? okey->data() : nullptr;
+        const uint32_t okl = okey ? (uint32_t)okey->size() : 0u;
+        return filter ? lc_multiline_split_regex_filter_parse_sls(
+                            Engine(), x.re, src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
+                            SPLIT_REGEX_STAGE_ARGS(x), ok, okl, pos, time, ns, &fd, o, cap, len, nev, rctr, sctr)
+                      : lc_multiline_split_regex_parse_sls(Engine(), x.re, src(val), val.size(), mStart.get(),
+                                                           mContinue.get(), mEnd.get(), discard,
+                                                           SPLIT_REGEX_STAGE_ARGS(x), ok, okl, pos, time, ns, o, cap,
+                                                           len, nev, rctr, sctr);
     };
     auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
                    const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
                    uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
-        return lc_multiline_split_regex_parse_sls_lz4(
-            Engine(), x.re, src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
-            SPLIT_REGEX_STAGE_ARGS(x), okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos, time,
-            ns, tail, tailLen, o, cap, len, raw, nev, rctr, sctr);
+        const char* ok = okey ? okey->data() : nullptr;
+        const uint32_t okl = okey ? (uint32_t)okey->size() : 0u;
+        return filter ? lc_multiline_split_regex_filter_parse_sls_lz4(
+                            Engine(), x.re, src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
+                            SPLIT_REGEX_STAGE_ARGS(x), ok, okl, pos, time, ns, &fd, tail, tailLen, o, cap, len, raw,
+                            nev, rctr, sctr)
+                      : lc_multiline_split_regex_parse_sls_lz4(
+                            Engine(), x.re, src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
+                            SPLIT_REGEX_STAGE_ARGS(x), ok, okl, pos, time, ns, tail, tailLen, o, cap, len, raw, nev,
+                            rctr, sctr);
     };
     // matched_events, input lines, unmatched lines: moved as Process moves them (:82-84,106-107)
     uint64_t ctr[3] = {0, 0, 0};
     const bool ok = SplitRegexChainSls(
-        group, x, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
-        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_multiline_split_regex_parse_sls",
-        "lc_multiline_split_regex_parse_sls_lz4", ctr);
+        group, x, filter, filterOk, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4,
+        filter ? "lc_multiline_split_regex_filter_parse_sls" : "lc_multiline_split_regex_parse_sls",
+        filter ? "lc_multiline_split_regex_filter_parse_sls_lz4" : "lc_multiline_split_regex_parse_sls_lz4", ctr);
     mMatchedEventsTotal.Add(ctr[0]);
     mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
     mUnmatchedLinesTotal.Add(ctr[2]);

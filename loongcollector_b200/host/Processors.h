@@ -113,6 +113,7 @@ private:
 };
 
 class ProcessorParseRegexNative;
+class ProcessorFilterNative;
 
 class ProcessorSplitLogStringNative : public Processor {
 public:
@@ -141,13 +142,21 @@ public:
     // device (lc_split_regex_parse_sls_lz4); other groups compress SerializeSls's bytes.
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs, std::string& block,
                          uint64_t& rawSize, std::string& err);
+    // Process(group), next.Process(group), filter.Process(group) (filter: the processor_filter_regex_native behind
+    // next), then SLSEventGroupSerializer::Serialize: the same bytes or error message, and the same counter updates.
+    // The device path (lc_split_regex_filter_parse_sls[_lz4]) applies under SerializeSls(group, next)'s conditions when
+    // filter.DeviceFilter accepts the rule; otherwise the four calls run.
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative& filter,
+                      bool enableNs, std::string& out, std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative& filter,
+                         bool enableNs, std::string& block, uint64_t& rawSize, std::string& err);
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
-    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs,
-                           std::string& out, uint64_t* rawSize, std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative* filter,
+                           bool enableNs, std::string& out, uint64_t* rawSize, std::string& err);
 };
 
 class ProcessorSplitMultilineLogStringNative : public Processor {
@@ -171,14 +180,20 @@ public:
                       std::string& err);
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs, std::string& block,
                          uint64_t& rawSize, std::string& err);
+    // The split -> regex -> filter chain, as ProcessorSplitLogStringNative's
+    // (lc_multiline_split_regex_filter_parse_sls[_lz4]).
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative& filter,
+                      bool enableNs, std::string& out, std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative& filter,
+                         bool enableNs, std::string& block, uint64_t& rawSize, std::string& err);
     Counter mMatchedEventsTotal, mMatchedLinesTotal, mUnmatchedLinesTotal;
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
-    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs,
-                           std::string& out, uint64_t* rawSize, std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative* filter,
+                           bool enableNs, std::string& out, uint64_t* rawSize, std::string& err);
     CompiledRegex mStart, mContinue, mEnd;
 };
 
@@ -311,6 +326,11 @@ public:
     using Processor::Process;
     bool mDiscardingNonUTF8 = false;
     ~ProcessorFilterNative() override;
+    // The rule as the split -> regex -> filter device calls take it: RULE and Include mode the leaves ANDed in their
+    // evaluation order, EXPRESSION mode the postfix program of the tree, BYPASS the empty program.  *d points into
+    // this object.  False when the device calls cannot reproduce the rule: DiscardingNonUTF8, more leaves or program
+    // entries than lc_b200.h allows, or a stack deeper than 32.
+    bool DeviceFilter(lc_filter_desc_t* d) const;
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
@@ -332,6 +352,13 @@ private:
     std::vector<Leaf> mLeaves;
     std::vector<Node> mNodes;
     int mRoot = -1;
+    // DeviceFilter's description, built by Init
+    void BuildDeviceFilter();
+    bool mDeviceOk = false;
+    std::vector<const char*> mDevKeys;
+    std::vector<uint32_t> mDevKeyLens;
+    std::vector<const lc_regex_t*> mDevRegs;
+    std::vector<uint32_t> mDevProg;
 };
 
 // Second "next" row (SURVEY.md 8f): merges already-split LogEvents of a group back into records -- by the docker

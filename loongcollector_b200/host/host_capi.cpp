@@ -291,6 +291,70 @@ char* lc_host_chain_serialize_sls(lc_host_processor_t* delim, lc_host_processor_
     }
 }
 
+char* lc_host_chain3_serialize_sls(lc_host_processor_t* split, lc_host_processor_t* regex, lc_host_processor_t* filter,
+                                   const char* group_json, int enable_ns, int mode, unsigned long long* len_out,
+                                   unsigned long long* raw_len_out, char** err_out, char** fail_out) {
+    if (err_out)
+        *err_out = nullptr;
+    if (fail_out)
+        *fail_out = nullptr;
+    if (len_out)
+        *len_out = 0;
+    if (raw_len_out)
+        *raw_len_out = 0;
+    try {
+        Processor* d = split->proc.get();
+        auto* r = dynamic_cast<ProcessorParseRegexNative*>(regex->proc.get());
+        auto* f = dynamic_cast<ProcessorFilterNative*>(filter->proc.get());
+        auto* ps = dynamic_cast<ProcessorSplitLogStringNative*>(d);
+        auto* pm = dynamic_cast<ProcessorSplitMultilineLogStringNative*>(d);
+        if (!(ps || pm) || !r || !f)
+            throw std::runtime_error("not a splitter, a processor_parse_regex_native and a "
+                                     "processor_filter_regex_native");
+        auto chain = [&](auto* p, PipelineEventGroup& g, std::string& res, uint64_t& raw, std::string& err) {
+            return mode == 2 ? p->SerializeSlsLz4(g, *r, *f, enable_ns != 0, res, raw, err)
+                             : p->SerializeSls(g, *r, *f, enable_ns != 0, res, err);
+        };
+        PipelineEventGroup group(std::make_shared<SourceBuffer>());
+        if (!group.FromJsonString(group_json ? group_json : "null"))
+            throw std::runtime_error("group JSON does not parse");
+        const uint64_t errs = d->EngineErrors() + r->EngineErrors() + f->EngineErrors();
+        std::string res, err;
+        uint64_t raw = 0;
+        bool ok;
+        if (mode == 1) {
+            d->Process(group);
+            r->Process(group);
+            f->Process(group);
+            SLSEventGroupSerializer ser;
+            ser.mEnableTimestampNanosecond = enable_ns != 0;
+            ok = ser.Serialize(group, res, err);
+        } else {
+            ok = ps ? chain(ps, group, res, raw, err) : chain(pm, group, res, raw, err);
+        }
+        if (d->EngineErrors() + r->EngineErrors() + f->EngineErrors() != errs)
+            throw std::runtime_error("engine error inside Process: " + d->LastError() + r->LastError() +
+                                     f->LastError());
+        if (!ok) {
+            if (err_out)
+                *err_out = dup(err);
+            return nullptr;
+        }
+        char* out = (char*)malloc(res.size() + 1);
+        memcpy(out, res.data(), res.size());
+        out[res.size()] = 0;
+        if (len_out)
+            *len_out = res.size();
+        if (raw_len_out)
+            *raw_len_out = raw;
+        return out;
+    } catch (const std::exception& e) {
+        if (fail_out)
+            *fail_out = dup(std::string("chain3 SerializeSls threw: ") + e.what());
+        return nullptr;
+    }
+}
+
 char* lc_host_lz4_compress(const char* const* data, const unsigned long long* len, unsigned long long n,
                            unsigned long long* len_out, unsigned long long* blk_len, char** err_out) {
     if (err_out)
