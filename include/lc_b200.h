@@ -453,8 +453,82 @@ int lc_multiline_split_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re,
                                            uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
                                            uint64_t counters[3], uint64_t ml_counters[3]);
 
-/* ---- f4: the split -> regex -> filter chain (the above, then ProcessorFilterNative / processor_filter_regex_native;
- * the pipeline of the reference's file-to-blackhole benchmark) to the SLS wire format.  The filter sees the event the
+/* ---- f4: the split -> delimiter chain (ProcessorSplitLogStringNative or ProcessorSplitMultilineLogStringNative, then
+ * ProcessorParseDelimiterNative with the same SourceKey -- BASELINE config C4 on file input) to the SLS wire format.
+ * The source event is flat, as for the split -> regex chain, and piece k enters the delimiter stage as [source_key ->
+ * piece] or, when offset_key != NULL, [source_key -> piece, offset_key -> decimal(src_pos + off[k])].  The delimiter
+ * stage then runs as for lc_sls_serialize_delim_dev (sep .. copy_raw) on that event, and SetContentNoCopy replaces in
+ * place, so a record's contents are: source_key's (the column keyed source_key, or deleted), the offset content (the
+ * column keyed offset_key -- not written again in column order -- or the digits when the row failed, is too short to
+ * reach it, or skips it as a discarded "_"), the other columns in column order, then renamed_key / "__raw_log__"
+ * unless one of them is offset_key (the key is present).  A blank or empty piece is left untouched; a failed piece
+ * without keep_fail keeps only the offset content and is erased (ShouldEraseEvent).  counters[4] (may be NULL) =
+ * successful, failed, discarded, blank, as lc_delim_parse_sls counts them (out_failed = failed + blank).  Refused with
+ * LC_ERR_INVALID_ARG: offset_key equal to source_key; unless discard, an offset_key of the form __column<digits>__
+ * (a generated overflow key could collide with it on some rows); and lc_sls_serialize_delim_dev's refusals.
+ * LC_ERR_TOO_LARGE when src_len reaches 0xFFFFFFF0, n reaches 2^30 or n * max_fields 2^32, or a record would reach
+ * 4 GiB.
+ *
+ * lc_sls_serialize_split_delim_dev: from the DEVICE piece tables of one lc_split_lines_dev / lc_multiline_split_dev
+ * call over d_src[0, src_len) and the DEVICE tables of lc_delim_parse_dev over those pieces (d_status, d_nfields,
+ * [n][max_fields] d_f_off / d_f_len / d_f_dq).  d_out receives the bytes; *out_len (host) their count;
+ * LC_ERR_CAPACITY if > out_cap (nothing written, *out_len and counters set). */
+int lc_sls_serialize_split_delim_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+                                     const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                     const uint32_t* d_nfields, const uint32_t* d_f_off, const uint32_t* d_f_len,
+                                     const uint32_t* d_f_dq, uint32_t max_fields, const uint8_t* sep, uint32_t sep_len,
+                                     uint8_t quote, int extend, int discard, const char* const* keys,
+                                     const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+                                     uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+                                     int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+                                     uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                     uint8_t* d_out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[4]);
+
+/* The same with a HOST source value: upload it once, split it on the device, run lc_delim_parse_dev over the pieces
+ * (allow_short, max_fields as for lc_delim_parse_sls), serialise, and bring back only the wire bytes; *n_events,
+ * ml_counters, the _lz4 variants and which outputs are set on LC_ERR_CAPACITY as for lc_split_regex_parse_sls. */
+int lc_split_delim_parse_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, uint8_t split_char, const uint8_t* sep,
+                             uint32_t sep_len, uint8_t quote, int extend, int discard, int allow_short,
+                             uint32_t max_fields, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                             const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                             uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                             const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+                             uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                             uint64_t counters[4]);
+int lc_split_delim_parse_sls_lz4(lc_engine_t* e, const uint8_t* buf, uint64_t len, uint8_t split_char,
+                                 const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard,
+                                 int allow_short, uint32_t max_fields, const char* const* keys,
+                                 const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+                                 uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+                                 int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+                                 uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                 const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+                                 uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events, uint64_t counters[4]);
+int lc_multiline_split_delim_parse_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+                                       const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched,
+                                       const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard,
+                                       int allow_short, uint32_t max_fields, const char* const* keys,
+                                       const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+                                       uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+                                       int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+                                       uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                       uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                       uint64_t counters[4], uint64_t ml_counters[3]);
+int lc_multiline_split_delim_parse_sls_lz4(lc_engine_t* e, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+                                           const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched,
+                                           const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend,
+                                           int discard, int allow_short, uint32_t max_fields, const char* const* keys,
+                                           const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+                                           uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+                                           int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+                                           uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                           const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+                                           uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                                           uint64_t counters[4], uint64_t ml_counters[3]);
+
+/* ---- f4: the split -> regex -> filter chain (the split -> regex chain, then ProcessorFilterNative /
+ * processor_filter_regex_native; the pipeline of the reference's file-to-blackhole benchmark) to the SLS wire format.
+ * The filter sees the event the
  * regex stage left behind: a leaf is regex_match of its key's value there, false when the key is absent
  * (ProcessorFilterNative.cpp:459-486); keys are compared as bytes.  prog is a postfix program: an entry < nleaves
  * pushes that leaf, LC_FILTER_NOT pops one value and pushes its negation, LC_FILTER_AND / LC_FILTER_OR pop two and

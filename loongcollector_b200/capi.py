@@ -132,6 +132,18 @@ def lib():
         sr_tail + [vp, vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
     L.lc_multiline_split_regex_filter_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sls_cfg + \
         [i32] + sr_tail + [vp, vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
+    # the split -> delimiter chain: the delimiter's arguments (sep .. copy_raw), then the split -> regex tail
+    sd_cfg = [vp, u32, u8, i32, i32, i32, u32]  # sep .. max_fields of the host-buffer calls
+    L.lc_sls_serialize_split_delim_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, vp, u32, vp, u32, u8,
+                                                   i32, i32] + sls_cfg + sr_tail + [vp, u64, C.POINTER(u64), vp]
+    L.lc_split_delim_parse_sls.argtypes = [vp, vp, u64, u8] + sd_cfg + sls_cfg + sr_tail + \
+        [vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_split_delim_parse_sls_lz4.argtypes = [vp, vp, u64, u8] + sd_cfg + sls_cfg + sr_tail + \
+        [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_multiline_split_delim_parse_sls.argtypes = [vp, vp, u64, vp, vp, vp, i32] + sd_cfg + sls_cfg + sr_tail + \
+        [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
+    L.lc_multiline_split_delim_parse_sls_lz4.argtypes = [vp, vp, u64, vp, vp, vp, i32] + sd_cfg + sls_cfg + \
+        sr_tail + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
     _LIB = L
     return L
 
@@ -878,6 +890,106 @@ class Engine:
             [_rh(start), _rh(cont), _rh(end), int(bool(discard))], keys, source_key, renamed_key, keep_fail,
             keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, True, tail, filt)
 
+    def sls_serialize_split_delim_dev(self, d_src, src_len, d_off, d_len, n, d_status, d_nf, d_fo, d_fl, d_fd,
+                                      max_fields, sep: bytes, quote, treatment, keys, source_key, renamed_key=None,
+                                      keep_fail=False, keep_succeed=False, copy_raw=False, offset_key=None, src_pos=0,
+                                      time=0, time_ns=None, d_out=None, out_cap=0):
+        """Wire bytes of the split -> delimiter chain from the device piece tables of one split_lines_dev /
+        multiline_split_dev call and the device tables of delim_parse_dev over those pieces (treatment: "extend" /
+        "keep" / "discard"; lc_sls_serialize_split_delim_dev).  Returns (byte count written to d_out, counters[4] =
+        successful, failed, discarded, blank); with d_out None the byte count needed."""
+        sp = np.frombuffer(sep, np.uint8)
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        need = C.c_uint64(0)
+        ctr = np.zeros(4, np.uint64)
+        rc = lib().lc_sls_serialize_split_delim_dev(self._h, _p(d_src), src_len, _p(d_off), _p(d_len), n,
+                                                    _p(d_status), _p(d_nf), _p(d_fo), _p(d_fl), _p(d_fd), max_fields,
+                                                    _p(sp), len(sep), quote, int(treatment == "extend"),
+                                                    int(treatment == "discard"), *cfg,
+                                                    *self._sr_tail(offset_key, src_pos, time, time_ns), _p(d_out),
+                                                    out_cap, C.byref(need), _p(ctr))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value), ctr  # a sizing query
+        _check(rc)
+        return int(need.value), ctr
+
+    def _split_delim(self, fn, buf, extra, sep, quote, treatment, keys, source_key, renamed_key, keep_fail,
+                     keep_succeed, copy_raw, allow_short, max_fields, offset_key, src_pos, time, time_ns, out_cap, ml,
+                     tail):
+        """one host-buffer split -> delimiter call, sized by an estimate first and by the exact size when that was
+        short; tail None: the wire bytes, else records ‖ tail as one LZ4 block.  Returns (bytes, raw_len, n_events,
+        counters[4], ml_counters[3] or None)"""
+        a = _u8(buf)
+        sp = np.frombuffer(sep, np.uint8)
+        mf = int(max_fields if max_fields is not None else len(keys) + 16)
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        dcfg = [_p(sp), len(sep), quote, int(treatment == "extend"), int(treatment == "discard"),
+                int(bool(allow_short)), mf]
+        tl = None if tail is None else np.frombuffer(bytes(tail), np.uint8)
+        est = 2 * a.size + 4096 + (0 if tl is None else tl.size)
+        cap = int(out_cap if out_cap is not None else est + est // 255 + 16)
+        for _ in range(2):
+            out = np.empty(max(cap, 1), np.uint8)
+            need, raw, nev = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+            ctr, mctr = np.zeros(4, np.uint64), np.zeros(3, np.uint64)
+            z = [] if tl is None else [_p(tl) if tl.size else None, tl.size]
+            outs = [_p(out), cap, C.byref(need)] + ([] if tl is None else [C.byref(raw)]) + [C.byref(nev), _p(ctr)]
+            rc = fn(self._h, _p(a), a.size, *extra, *dcfg, *cfg, *self._sr_tail(offset_key, src_pos, time, time_ns),
+                    *z, *outs, *([_p(mctr)] if ml else []))
+            if rc == LC_ERR_CAPACITY and out_cap is None:
+                cap = int(need.value)
+                continue
+            _check(rc)
+            return bytes(out[:need.value]), int(raw.value), int(nev.value), ctr, (mctr if ml else None)
+        _check(rc)
+
+    def split_delim_parse_sls(self, buf, split_char, sep: bytes, quote, treatment, keys, source_key, renamed_key=None,
+                              keep_fail=False, keep_succeed=False, copy_raw=False, allow_short=True, max_fields=None,
+                              offset_key=None, src_pos=0, time=0, time_ns=None, out_cap=None):
+        """Host source value in: split, delimiter, wire bytes out (lc_split_delim_parse_sls).  Returns (bytes, number
+        of pieces, counters[4] = successful, failed, discarded, blank)."""
+        data, _raw, nev, ctr, _m = self._split_delim(
+            lib().lc_split_delim_parse_sls, buf, [split_char], sep, quote, treatment, keys, source_key, renamed_key,
+            keep_fail, keep_succeed, copy_raw, allow_short, max_fields, offset_key, src_pos, time, time_ns, out_cap,
+            False, None)
+        return data, nev, ctr
+
+    def split_delim_parse_sls_lz4(self, buf, split_char, sep: bytes, quote, treatment, keys, source_key,
+                                  renamed_key=None, keep_fail=False, keep_succeed=False, copy_raw=False,
+                                  allow_short=True, max_fields=None, offset_key=None, src_pos=0, time=0, time_ns=None,
+                                  tail=b"", out_cap=None):
+        """split_delim_parse_sls's records followed by `tail` as ONE LZ4 block (lc_split_delim_parse_sls_lz4).
+        Returns (block, raw_len, number of pieces, counters[4])."""
+        data, raw, nev, ctr, _m = self._split_delim(
+            lib().lc_split_delim_parse_sls_lz4, buf, [split_char], sep, quote, treatment, keys, source_key,
+            renamed_key, keep_fail, keep_succeed, copy_raw, allow_short, max_fields, offset_key, src_pos, time,
+            time_ns, out_cap, False, tail)
+        return data, raw, nev, ctr
+
+    def multiline_split_delim_parse_sls(self, buf, start, cont, end, discard, sep: bytes, quote, treatment, keys,
+                                        source_key, renamed_key=None, keep_fail=False, keep_succeed=False,
+                                        copy_raw=False, allow_short=True, max_fields=None, offset_key=None, src_pos=0,
+                                        time=0, time_ns=None, out_cap=None):
+        """The same with the multiline splitter (lc_multiline_split_delim_parse_sls).  Returns (bytes, number of
+        events, counters[4], splitter counters[3] = matched_events, input_lines, unmatched_lines)."""
+        data, _raw, nev, ctr, mctr = self._split_delim(
+            lib().lc_multiline_split_delim_parse_sls, buf, [_rh(start), _rh(cont), _rh(end), int(bool(discard))], sep,
+            quote, treatment, keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw, allow_short,
+            max_fields, offset_key, src_pos, time, time_ns, out_cap, True, None)
+        return data, nev, ctr, mctr
+
+    def multiline_split_delim_parse_sls_lz4(self, buf, start, cont, end, discard, sep: bytes, quote, treatment, keys,
+                                            source_key, renamed_key=None, keep_fail=False, keep_succeed=False,
+                                            copy_raw=False, allow_short=True, max_fields=None, offset_key=None,
+                                            src_pos=0, time=0, time_ns=None, tail=b"", out_cap=None):
+        """multiline_split_delim_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_multiline_split_delim_parse_sls_lz4).  Returns (block, raw_len, number of events, counters[4], splitter
+        counters[3])."""
+        return self._split_delim(
+            lib().lc_multiline_split_delim_parse_sls_lz4, buf, [_rh(start), _rh(cont), _rh(end), int(bool(discard))],
+            sep, quote, treatment, keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw, allow_short,
+            max_fields, offset_key, src_pos, time, time_ns, out_cap, True, tail)
+
     def lz4_compress_dev(self, d_in, nseg, d_seg_off, d_seg_len, d_out=None, out_cap=0, d_blk_off=None,
                          d_blk_len=None):
         """One LZ4 block per device segment d_in[d_seg_off[g], + d_seg_len[g]) (u64 / u32 tables), packed in d_out
@@ -1066,8 +1178,8 @@ class HostProcessor:
 
 
 def host_chain_serialize_sls(delim, regex, group, enable_ns=False, mode=0):
-    """The delimiter -> regex or split -> regex chain of two HostProcessors on a JSON group
-    (lc_host_chain_serialize_sls; delim may be either splitter).  mode 0:
+    """The delimiter -> regex, split -> regex or split -> delimiter chain of two HostProcessors on a JSON group
+    (lc_host_chain_serialize_sls; delim may be either splitter, and regex a delimiter behind a splitter).  mode 0:
     delim's SerializeSls(group, regex); 1: Process + Process + Serialize; 2: SerializeSlsLz4.  Returns (bytes, raw_len,
     None) or (None, 0, error)."""
     import json

@@ -2893,27 +2893,24 @@ int split_regex_sls_run(lc_engine_t* e, const char* what, const LcSplitRegexSlsC
     return rc;
 }
 
-// Host-buffer split + regex + serialise (lc_split_regex_parse_sls and the multiline / LZ4 siblings): the source goes
-// up once into `in`, `split(&n)` cuts it into the piece tables out_a / out_b (and out_c flags), the regex stage runs
-// over them into dr_status / dr_cap_off / dr_cap_len, and only the wire bytes (or their LZ4 block) come back.  With
-// fd (the _filter_ calls), the filter runs between the regex stage and the size pass and counters has a 4th entry.
-template <class Split>
-int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
-                         Split split, SPLIT_REGEX_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
-                         uint64_t* n_events, uint64_t counters[3], const Lz4Tail* z,
-                         const lc_filter_desc_t* fd = nullptr) {
-    if (!e || (!re && !whole_line) || !out_len || (len && !buf) || (z && (!z->raw_len || (z->len && !z->tail))))
+// Host-buffer split + parse + serialise (the split -> regex and split -> delimiter calls): the source goes up once into
+// `in`, `split(&n)` cuts it into the piece tables out_a / out_b (and out_c flags), then the parse stage and the
+// serialiser run over them and only the wire bytes (or, with z, records ‖ tail as one LZ4 block) come back.  The
+// stage's part: stage_args = its own arguments are usable; begin() = its checks before the engine is bound (it zeroes
+// its counters); config() = its configuration, staged on the device before the split; run(n) = parse, size pass and
+// emit over the n > 0 pieces.
+template <class Split, class Begin, class Config, class Run>
+int split_chain_sls_host(lc_engine_t* e, const char* what, const uint8_t* buf, uint64_t len, Split split,
+                         bool stage_args, Begin begin, Config config, Run run, uint8_t* out, uint64_t out_cap,
+                         uint64_t* out_len, uint64_t* n_events, const Lz4Tail* z) {
+    if (!e || !stage_args || !out_len || (len && !buf) || (z && (!z->raw_len || (z->len && !z->tail))))
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
     *out_len = 0;
     if (n_events)
         *n_events = 0;
-    uint64_t ctr[4] = {0, 0, 0, 0};
-    const size_t nctr = fd ? 4 : 3;
-    if (counters)
-        memset(counters, 0, nctr * sizeof(uint64_t));
     if (z)
         *z->raw_len = 0;
-    int rc = whole_line ? (int)LC_OK : check_regex_usable(re, what);
+    int rc = begin();
     if (rc)
         return rc;
     if (len >= 0xFFFFFFF0ull)
@@ -2921,10 +2918,7 @@ int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re,
     rc = bind(e);
     if (rc)
         return rc;
-    const uint32_t G = whole_line ? 0u : re->res.ngroups;
-    LcSplitRegexSlsCfg c;
-    LcFilterSlsCfg f;
-    rc = split_regex_sls_config(e, what, len, SPLIT_REGEX_ARGS, G, &c, fd, &f);
+    rc = config();
     if (rc)
         return rc;
     uint64_t n = 0;
@@ -2942,6 +2936,18 @@ int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re,
         *n_events = n;
     if (n == 0)
         return z ? lz4_tail_only(e, what, *z, out, out_cap, out_len) : (int)LC_OK;
+    return run(n);
+}
+
+// The regex stage of the split -> regex calls (split_regex_sls_host) over the n pieces: the regex tables go to
+// dr_status / dr_cap_off / dr_cap_len; with fd (the _filter_ calls), the filter runs between the regex stage and the
+// size pass and counters has a 4th entry.
+int split_regex_sls_stage(lc_engine_t* e, const char* what, const lc_regex_t* re, uint64_t len, uint64_t n, uint32_t G,
+                          uint32_t nkeys, int whole_line, const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f,
+                          const lc_filter_desc_t* fd, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                          size_t nctr, uint64_t* counters, const Lz4Tail* z) {
+    uint64_t ctr[4] = {0, 0, 0, 0};
+    int rc;
     if (n * (uint64_t)G >= (1ull << 32))
         return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^32 captures per call");
     const bool caps = !whole_line && nkeys && nkeys <= G;
@@ -2974,6 +2980,33 @@ int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re,
     if (counters)
         memcpy(counters, ctr, nctr * sizeof(uint64_t));
     return rc;
+}
+
+// Host-buffer split + regex + serialise (lc_split_regex_parse_sls and the multiline / LZ4 siblings)
+template <class Split>
+int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                         Split split, SPLIT_REGEX_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                         uint64_t* n_events, uint64_t counters[3], const Lz4Tail* z,
+                         const lc_filter_desc_t* fd = nullptr) {
+    const size_t nctr = fd ? 4 : 3;
+    uint32_t G = 0;
+    LcSplitRegexSlsCfg c;
+    LcFilterSlsCfg f;
+    auto begin = [&]() {
+        if (counters)
+            memset(counters, 0, nctr * sizeof(uint64_t));
+        return whole_line ? (int)LC_OK : check_regex_usable(re, what);
+    };
+    auto config = [&]() {
+        G = whole_line ? 0u : re->res.ngroups;
+        return split_regex_sls_config(e, what, len, SPLIT_REGEX_ARGS, G, &c, fd, &f);
+    };
+    auto run = [&](uint64_t n) {
+        return split_regex_sls_stage(e, what, re, len, n, G, nkeys, whole_line, c, f, fd, out, out_cap, out_len, nctr,
+                                     counters, z);
+    };
+    return split_chain_sls_host(e, what, buf, len, split, re || whole_line, begin, config, run, out, out_cap,
+                                out_len, n_events, z);
 }
 
 template <class Split>
@@ -3162,6 +3195,196 @@ int lc_multiline_split_regex_filter_parse_sls_lz4(lc_engine_t* e, const lc_regex
                                 filter);
 }
 #undef FILTER_CHECK
+
+} // extern "C"
+
+// ------------------------------------------------------------------------------------ split -> delimiter -> SLS
+// The delimiter stage's key configuration (lc_sls_serialize_delim_dev's keys .. copy_raw) and the offset content of the
+// split events (offset_key -- NULL = no log.file.offset metadata -- and the source event's position, time and ns)
+#define DELIM_KEY_PARAMS                                                                                               \
+    const char *const *keys, const uint32_t *key_lens, uint32_t nkeys, const char *source_key,                         \
+        uint32_t source_key_len, const char *renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed,   \
+        int copy_raw
+#define DELIM_KEY_ARGS                                                                                                 \
+    keys, key_lens, nkeys, source_key, source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed, copy_raw
+#define OFFSET_PARAMS const char *offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns
+#define OFFSET_ARGS offset_key, offset_key_len, src_pos, time, time_ns
+// the host-buffer calls' delimiter arguments (lc_delim_parse_sls's sep .. copy_raw) and the offset content
+#define SPLIT_DELIM_PARAMS                                                                                             \
+    const uint8_t *sep, uint32_t sep_len, uint8_t quote, int extend, int discard, int allow_short,                     \
+        uint32_t max_fields, DELIM_KEY_PARAMS, OFFSET_PARAMS
+#define SPLIT_DELIM_ARGS sep, sep_len, quote, extend, discard, allow_short, max_fields, DELIM_KEY_ARGS, OFFSET_ARGS
+
+namespace {
+
+// lc_delim_sls_setup + lc_split_delim_sls_link: the delimiter's key strings are staged in `dr_keys`, the offset key in
+// `sls_plan`; neither splitter, nor lc_delim_parse_dev, nor the serialiser uses them.
+int split_delim_sls_config(lc_engine_t* e, const char* what, uint32_t max_fields, const uint8_t* sep,
+                           uint32_t sep_len, uint8_t quote, int extend, int discard, DELIM_KEY_PARAMS, OFFSET_PARAMS,
+                           LcSplitDelimSlsCfg* c) {
+    LcDelimSlsCfg d;
+    int rc = delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, DELIM_KEY_ARGS, &d,
+                              &e->dr_keys);
+    if (rc)
+        return rc;
+    const char* why = lc_split_delim_sls_link(d, keys, key_lens, source_key, source_key_len, renamed_key,
+                                              renamed_key_len, offset_key, offset_key_len, src_pos, time, time_ns, c);
+    if (why)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    if (offset_key) {
+        CU_TRY(e->sls_plan.ensure(offset_key_len + 16));
+        if (offset_key_len) {
+            CU_TRY(cudaMemcpyAsync(e->sls_plan.p, offset_key, offset_key_len, cudaMemcpyHostToDevice, e->stream));
+            // (pageable source: its bytes must be on the device before it dies)
+            CU_TRY(cudaStreamSynchronize(e->stream));
+        }
+        c->okey = e->sls_plan.as<uint8_t>();
+    }
+    return LC_OK;
+}
+
+// The size pass and the emit of the chain over the n pieces of t (serialize_sls_dev): into d_out (the device-fed
+// call), or back to the host buffer out, or -- with z -- records ‖ tail as one LZ4 block.  counters[4] (or nullptr) =
+// successful, failed, discarded, blank; set whenever the size pass ran.
+int split_delim_sls_run(lc_engine_t* e, const char* what, const LcSplitDelimSlsCfg& c, const lck::DelimSlsTables& t,
+                        uint64_t n, uint8_t* d_out, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                        uint64_t* counters, const Lz4Tail* z) {
+    uint64_t ctr[5] = {0, 0, 0, 0, 0}; // + pieces whose record would reach 4 GiB
+    SlsTo to;
+    to.host = out;
+    to.z = z;
+    to.too_large = 4;
+    const int rc = serialize_sls_dev(
+        e, what, n, 5,
+        [&](uint32_t* rec, uint32_t* body, unsigned long long* d_ctr) {
+            lck::launch_split_delim_sls_sizes(c, t, n, rec, body, d_ctr, e->stream);
+        },
+        [&](const uint64_t* rec_off, const uint32_t* body, uint8_t* dst) {
+            lck::launch_split_delim_sls_emit(c, t, n, rec_off, body, dst, e->stream);
+        },
+        d_out, out_cap, out_len, ctr, to);
+    if (counters)
+        memcpy(counters, ctr, 4 * sizeof(uint64_t));
+    return rc;
+}
+
+// Host-buffer split + delimiter + serialise (lc_split_delim_parse_sls and the multiline / LZ4 siblings, through
+// split_chain_sls_host).  Workspace: the source in `in`, the piece tables in out_a / out_b (out_c: the multiline
+// flags), the delimiter tables in dr_status (status), dr_val_off (column counts), out_d / out_e / dr_cap_off (f_off /
+// f_len / f_dq, [n][max_fields]), the key strings in dr_keys and sls_plan.  The splitters, lc_delim_parse_dev (its
+// tiled kernel stages in shared memory) and the serialiser (lab_sizes, cnt, lab_off, state, desc, lab, z_*) use none
+// of the others'.
+template <class Split>
+int split_delim_sls_host(lc_engine_t* e, const char* what, const uint8_t* buf, uint64_t len, Split split,
+                         SPLIT_DELIM_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                         uint64_t counters[4], const Lz4Tail* z) {
+    LcSplitDelimSlsCfg c;
+    auto begin = [&]() {
+        if (counters)
+            memset(counters, 0, 4 * sizeof(uint64_t));
+        return (int)LC_OK;
+    };
+    auto config = [&]() {
+        return split_delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, DELIM_KEY_ARGS,
+                                      OFFSET_ARGS, &c);
+    };
+    auto run = [&](uint64_t n) {
+        if (n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32))
+            return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^30 pieces and < 2^32 columns per call");
+        const uint64_t fbytes = n * max_fields * 4;
+        CU_TRY(e->dr_status.ensure(n));
+        CU_TRY(e->dr_val_off.ensure(n * 4));
+        CU_TRY(e->out_d.ensure(fbytes));
+        CU_TRY(e->out_e.ensure(fbytes));
+        CU_TRY(e->dr_cap_off.ensure(fbytes));
+        const lck::DelimSlsTables t{e->in.as<uint8_t>(),         e->out_a.as<uint32_t>(),
+                                    e->out_b.as<uint32_t>(),     e->dr_status.as<uint8_t>(),
+                                    e->dr_val_off.as<uint32_t>(), e->out_d.as<uint32_t>(),
+                                    e->out_e.as<uint32_t>(),     e->dr_cap_off.as<uint32_t>()};
+        int rc = lc_delim_parse_dev(e, t.base, len, t.ev_off, t.ev_len, n, sep, sep_len, quote, nkeys, extend,
+                                    allow_short, max_fields, e->dr_status.as<uint8_t>(),
+                                    e->dr_val_off.as<uint32_t>(), e->out_d.as<uint32_t>(), e->out_e.as<uint32_t>(),
+                                    e->dr_cap_off.as<uint32_t>());
+        if (rc)
+            return rc;
+        return split_delim_sls_run(e, what, c, t, n, nullptr, out, out_cap, out_len, counters, z);
+    };
+    return split_chain_sls_host(e, what, buf, len, split, sep != nullptr, begin, config, run, out, out_cap, out_len,
+                                n_events, z);
+}
+
+} // namespace
+
+extern "C" {
+
+int lc_sls_serialize_split_delim_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+                                     const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                     const uint32_t* d_nfields, const uint32_t* d_f_off, const uint32_t* d_f_len,
+                                     const uint32_t* d_f_dq, uint32_t max_fields, const uint8_t* sep, uint32_t sep_len,
+                                     uint8_t quote, int extend, int discard, DELIM_KEY_PARAMS, OFFSET_PARAMS,
+                                     uint8_t* d_out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[4]) {
+    static const char* what = "lc_sls_serialize_split_delim_dev";
+    if (!e || !out_len || (n && (!d_src || !d_off || !d_len || !d_status || !d_nfields || !d_f_off || !d_f_len ||
+                                 !d_f_dq)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (counters)
+        memset(counters, 0, 4 * sizeof(uint64_t));
+    if (src_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 pieces and < 2^32 columns per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcSplitDelimSlsCfg c;
+    rc = split_delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, DELIM_KEY_ARGS, OFFSET_ARGS,
+                                &c);
+    if (rc || n == 0)
+        return rc;
+    const lck::DelimSlsTables t{d_src, d_off, d_len, d_status, d_nfields, d_f_off, d_f_len, d_f_dq};
+    return split_delim_sls_run(e, what, c, t, n, d_out, nullptr, out_cap, out_len, counters, nullptr);
+}
+
+int lc_split_delim_parse_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, uint8_t split_char,
+                             SPLIT_DELIM_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                             uint64_t* n_events, uint64_t counters[4]) {
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_delim_sls_host(e, "lc_split_delim_parse_sls", buf, len, split, SPLIT_DELIM_ARGS, out, out_cap,
+                                out_len, n_events, counters, nullptr);
+}
+
+int lc_split_delim_parse_sls_lz4(lc_engine_t* e, const uint8_t* buf, uint64_t len, uint8_t split_char,
+                                 SPLIT_DELIM_PARAMS, const uint8_t* tail, uint64_t tail_len, uint8_t* out,
+                                 uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                                 uint64_t counters[4]) {
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return split_delim_sls_host(e, "lc_split_delim_parse_sls_lz4", buf, len, split, SPLIT_DELIM_ARGS, out, out_cap,
+                                out_len, n_events, counters, &z);
+}
+
+int lc_multiline_split_delim_parse_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+                                       const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched,
+                                       SPLIT_DELIM_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                                       uint64_t* n_events, uint64_t counters[4], uint64_t ml_counters[3]) {
+    return split_delim_sls_host(e, "lc_multiline_split_delim_parse_sls", buf, len, ML_SPLIT, SPLIT_DELIM_ARGS, out,
+                                out_cap, out_len, n_events, counters, nullptr);
+}
+
+int lc_multiline_split_delim_parse_sls_lz4(lc_engine_t* e, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+                                           const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched,
+                                           SPLIT_DELIM_PARAMS, const uint8_t* tail, uint64_t tail_len, uint8_t* out,
+                                           uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+                                           uint64_t* n_events, uint64_t counters[4], uint64_t ml_counters[3]) {
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return split_delim_sls_host(e, "lc_multiline_split_delim_parse_sls_lz4", buf, len, ML_SPLIT, SPLIT_DELIM_ARGS,
+                                out, out_cap, out_len, n_events, counters, &z);
+}
 #undef ML_SPLIT
 
 } // extern "C"

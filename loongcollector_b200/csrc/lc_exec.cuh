@@ -978,12 +978,22 @@ LC_HD void lc_delim_sls_columns(const LcDelimSlsCfg& c, const uint8_t* base, con
 // kid = the key id of the content: key j < nkeys, or nkeys + 0 / 1 / 2 = SourceKey / RenamedSourceKey / "__raw_log__"
 // -- and when x owns it, x.in_place(s) is written in its place instead; x.tail(s) runs after the contents, before
 // Time_ns.  The count returned is the delimiter stage's, owned content included.
+// A content the event holds before the delimiter runs, after SourceKey (the split's offset content), is x's slot: on
+// every row that is not erased the body writes column x.slot_col() there when the row parsed and reaches it (that
+// column is then not written in column order), else x.slot(s) -- which returns whether it wrote a content.
+// x.slot_holds(kid): the slot's key is RenamedSourceKey / "__raw_log__" (kid), which AddLog(..., false) then skips.
 struct LcDelimNoChain {
     LC_HD bool own(uint32_t) const { return false; }
     template <class S>
     LC_HD void in_place(S&) {}
     template <class S>
     LC_HD void tail(S&) {}
+    LC_HD uint32_t slot_col() const { return LC_DELIM_SLS_NONE; }
+    LC_HD bool slot_holds(uint32_t) const { return false; }
+    template <class S>
+    LC_HD bool slot(S&) {
+        return false;
+    }
 };
 
 template <class S, class X>
@@ -1014,12 +1024,26 @@ LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, co
         else
             s.copy(base + off, len);
     };
+    const uint32_t xcol = x.slot_col();
+    auto slot = [&](bool parsed) {
+        if (parsed && xcol < r.nf) { // xcol < nkeys < max_fields: always in the table
+            const uint32_t dq = c.use_quote ? r.fd[xcol] : 0u;
+            lc_sls_pair_open(s, kp(xcol), kl(xcol), r.fl[xcol] - dq);
+            value(r.fo[xcol], r.fl[xcol], dq);
+            ++cnt;
+        } else if (x.slot(s)) {
+            ++cnt;
+        }
+    };
     if (r.status == 2) { // LC_DELIM_BLANK
         whole_line(K_SRC);
+        slot(false);
     } else if (r.status != 0) { // LC_DELIM_PARSE_FAIL / LC_DELIM_COLUMNS
         if (c.keep_fail) {
-            whole_line(K_REN);
-            if (c.copy_raw && !c.ren_is_raw)
+            slot(false);
+            if (!x.slot_holds(K_REN))
+                whole_line(K_REN);
+            if (c.copy_raw && !c.ren_is_raw && !x.slot_holds(K_RAW))
                 whole_line(K_RAW);
         }
     } else {
@@ -1039,12 +1063,13 @@ LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, co
                 whole_line(K_SRC);
             }
         }
+        slot(true);
         const bool joined = c.mode == LC_DELIM_SLS_KEEP && c.use_quote;
         const uint32_t jend = c.mode == LC_DELIM_SLS_EXTEND                 ? 0xFFFFFFFFu
                               : (c.mode == LC_DELIM_SLS_KEEP && !joined) ? nk + 1 // the split's remainder column
                                                                           : nk;
         auto col = [&](uint32_t j, uint32_t off, uint32_t len, uint32_t dq) {
-            if (j == c.src_col)
+            if (j == c.src_col || j == xcol)
                 return;
             if (!c.use_quote)
                 dq = 0;
@@ -1082,7 +1107,8 @@ LC_HD uint32_t lc_delim_sls_body(const LcDelimSlsCfg& c, const uint8_t* base, co
             const bool present =
                 (c.ren_is_src && c.src_overwritten) || (c.ren_col != LC_DELIM_SLS_NONE && c.ren_col < nf) ||
                 (c.ren_xcol != LC_DELIM_SLS_NONE && c.ren_xcol >= nk && c.ren_xcol < nf &&
-                 (c.mode == LC_DELIM_SLS_EXTEND || (c.mode == LC_DELIM_SLS_KEEP && c.ren_xcol == nk)));
+                 (c.mode == LC_DELIM_SLS_EXTEND || (c.mode == LC_DELIM_SLS_KEEP && c.ren_xcol == nk))) ||
+                x.slot_holds(K_REN);
             if (!present)
                 whole_line(K_REN);
         }
@@ -1482,8 +1508,8 @@ struct LcDelimRegexSlsRow {
     const uint32_t* cl;
 };
 
-// the regex stage as the delimiter body's chained stage (LcDelimNoChain's interface)
-struct LcDelimRegexStage {
+// the regex stage as the delimiter body's chained stage (LcDelimNoChain's interface; no slot)
+struct LcDelimRegexStage : LcDelimNoChain {
     const LcDelimRegexSlsCfg& c;
     const uint8_t* base;
     const LcDelimRegexSlsRow& r;
@@ -1524,7 +1550,7 @@ struct LcDelimRegexStage {
 template <class S>
 LC_HD uint32_t lc_delim_regex_sls_body(const LcDelimRegexSlsCfg& c, const uint8_t* base, const LcDelimRegexSlsRow& r,
                                        S& s) {
-    LcDelimRegexStage x{c, base, r, lc_delim_regex_value(c, r.d.status, r.d.nf) != LC_DR_ABSENT,
+    LcDelimRegexStage x{{}, c, base, r, lc_delim_regex_value(c, r.d.status, r.d.nf) != LC_DR_ABSENT,
                         lc_regex_sls_verdict(c.x, r.status) == 0u, 0u};
     const uint32_t n = lc_delim_sls_body(c.d, base, r.d, s, x);
     return x.present ? n - 1 + x.m : n;
@@ -1947,6 +1973,7 @@ struct LcSlsCount64 {
     uint64_t n;
     LC_HD void put(const uint8_t*, uint32_t k) { n += k; }
     LC_HD void copy(const uint8_t*, uint32_t k) { n += k; }
+    LC_HD void unquote(const uint8_t*, uint32_t, uint32_t out_n, uint8_t) { n += out_n; }
 };
 
 // The piece's counter verdicts (0 / 1): ProcessorParseRegexNative's out_successful (every piece not erased),
@@ -1980,6 +2007,107 @@ inline const char* lc_split_regex_sls_setup(const char* const* keys, const uint3
                                          copy_raw, whole_line, pitch, &c->x, plan);
     if (why)
         return why;
+    c->src_pos = src_pos;
+    c->time = time;
+    c->has_ns = time_ns != 0xFFFFFFFFu;
+    c->ns = c->has_ns ? time_ns : 0u;
+    return nullptr;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, split -> delimiter chain: the Log record of piece k that ProcessorSplitLogStringNative /
+// ProcessorSplitMultilineLogStringNative followed by ProcessorParseDelimiterNative (same SourceKey) leave behind,
+// written straight from the piece tables of the splitter and the delimiter tables of lc_delim_parse_dev over those
+// pieces.  The piece enters the delimiter stage as [SourceKey -> piece] or, with log.file.offset metadata,
+// [SourceKey -> piece, offset_key -> decimal(src_pos + off[k])].  The record is the delimiter's body
+// (lc_delim_sls_body) with the offset content as its chained stage's slot: SetContentNoCopy replaces in place, so the
+// contents come out as SourceKey's, the offset slot (the column keyed offset_key when the row parsed and reaches it,
+// else the digits), the other columns in column order, then RenamedSourceKey / "__raw_log__" unless one of them is the
+// offset key.  A blank row is left untouched; a failed row without KeepingSourceWhenParseFail keeps only the offset
+// content and is erased (ShouldEraseEvent), so the rows erased and the four counters are those of the delimiter stage
+// alone.
+struct LcSplitDelimSlsCfg {
+    LcDelimSlsCfg d;     // the delimiter stage (lc_delim_sls_setup)
+    const uint8_t* okey; // device copy of the offset key
+    uint32_t oklen;
+    uint32_t has_offset;
+    uint32_t off_col;          // the column keyed offset_key (not a skipped "_"), or NONE
+    uint32_t ren_is_off;       // RenamedSourceKey == offset_key
+    uint32_t raw_is_off;       // "__raw_log__" == offset_key
+    uint64_t src_pos;          // the source event's file offset
+    uint32_t time;             // the source event's time, as the split events inherit it
+    uint32_t has_ns, ns;
+};
+
+// the offset content as the delimiter body's chained stage (LcDelimNoChain's interface)
+struct LcSplitDelimStage : LcDelimNoChain {
+    const LcSplitDelimSlsCfg& c;
+    uint64_t pos; // src_pos + the piece's offset
+    LC_HD uint32_t slot_col() const { return c.off_col; }
+    LC_HD bool slot_holds(uint32_t kid) const {
+        return (kid == c.d.nkeys + 1 && c.ren_is_off) || (kid == c.d.nkeys + 2 && c.raw_is_off);
+    }
+    template <class S>
+    LC_HD bool slot(S& s) {
+        if (!c.has_offset)
+            return false;
+        const uint32_t nd = lc_dec_digits(pos);
+        lc_sls_pair_open(s, c.okey, c.oklen, nd);
+        lc_sls_digits(s, pos, nd);
+        return true;
+    }
+};
+
+// The body of the piece's Log record into sink s (LcSlsCount64 / LcSlsWrite); r = the piece (eo, elen: its offset and
+// length in src) and its row of the delimiter tables, with the source event's time and ns.  Returns the number of
+// contents; 0 = erased, no record.
+template <class S>
+LC_HD uint32_t lc_split_delim_sls_body(const LcSplitDelimSlsCfg& c, const uint8_t* src, const LcDelimSlsRow& r,
+                                       S& s) {
+    LcSplitDelimStage x{{}, c, c.src_pos + r.eo};
+    return lc_delim_sls_body(c.d, src, r, s, x);
+}
+
+// The row's counter verdicts (0 / 1), as lc_delim_parse_sls counts them: successful, failed, discarded, blank.
+struct LcDelimSlsVerdict {
+    uint32_t ok, failed, erased, blank;
+};
+LC_HD LcDelimSlsVerdict lc_delim_sls_verdict(const LcDelimSlsCfg& c, uint32_t status) {
+    const uint32_t ok = status == 0, blank = status == 2, failed = !ok && !blank;
+    return {ok, failed, failed && !c.keep_fail ? 1u : 0u, blank};
+}
+
+// Host side: the chain's own checks and fields, after lc_delim_sls_setup accepted the delimiter stage (d, with the
+// same keys, SourceKey and RenamedSourceKey).  offset_key == nullptr: no log.file.offset metadata.  Returns nullptr, or
+// why the chain is refused: an offset key equal to SourceKey (the split would replace the piece by its digits, and the
+// delimiter would parse those), or -- unless overflow columns are discarded -- an offset key of the form
+// __column<digits>__, which a generated overflow key could overwrite on some rows and not on others.
+inline const char* lc_split_delim_sls_link(const LcDelimSlsCfg& d, const char* const* keys, const uint32_t* key_lens,
+                                           const char* source_key, uint32_t source_len, const char* renamed_key,
+                                           uint32_t renamed_len, const char* offset_key, uint32_t offset_len,
+                                           uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                           LcSplitDelimSlsCfg* c) {
+    auto eq = [](const char* a, uint32_t la, const char* b, uint32_t lb) {
+        return la == lb && (la == 0 || !memcmp(a, b, la));
+    };
+    memset(c, 0, sizeof *c);
+    c->d = d;
+    c->off_col = LC_DELIM_SLS_NONE;
+    if (offset_key) {
+        uint32_t idx;
+        if (eq(offset_key, offset_len, source_key, source_len))
+            return "the offset key equals SourceKey";
+        if (d.mode != LC_DELIM_SLS_DISCARD && lc_delim_column_form(offset_key, offset_len, &idx))
+            return "an offset key of the form __column<digits>__ collides with the generated overflow keys";
+        c->has_offset = 1;
+        c->oklen = offset_len;
+        for (uint32_t k = 0; k < d.nkeys; ++k)
+            if (eq(keys[k], key_lens[k], offset_key, offset_len) &&
+                !(d.mode == LC_DELIM_SLS_DISCARD && key_lens[k] == 1 && keys[k][0] == '_'))
+                c->off_col = k;
+        c->ren_is_off = eq(renamed_key, renamed_len, offset_key, offset_len);
+        c->raw_is_off = eq("__raw_log__", 11, offset_key, offset_len);
+    }
     c->src_pos = src_pos;
     c->time = time;
     c->has_ns = time_ns != 0xFFFFFFFFu;

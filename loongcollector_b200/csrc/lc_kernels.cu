@@ -3959,6 +3959,89 @@ void launch_delim_regex_sls_emit(const LcDelimRegexSlsCfg& c, const DelimRegexSl
                                                                                        d_rec_off, d_body_size, d_out);
 }
 
+// ---- f4, split -> delimiter chain: Log records of the pieces a splitter cut and a ProcessorParseDelimiterNative
+// parsed, straight from the piece tables and the delimiter tables over them (lc_exec.cuh: lc_split_delim_sls_body) --
+// the size pass one thread per piece, the emit pass one warp per piece.  counters: u64 [5] += successful, failed,
+// discarded, blank, pieces whose record would reach 4 GiB (their size is left 0 and the call is refused).
+__device__ __forceinline__ LcDelimSlsRow split_delim_sls_row(const LcSplitDelimSlsCfg& c, const DelimSlsTables& t,
+                                                             uint64_t i) {
+    LcDelimSlsRow r;
+    r.eo = t.ev_off[i];
+    r.elen = t.ev_len[i];
+    r.status = t.status[i];
+    r.nf = t.nfields[i];
+    r.fo = t.f_off + i * c.d.max_fields;
+    r.fl = t.f_len + i * c.d.max_fields;
+    r.fd = t.f_dq + i * c.d.max_fields;
+    r.time = c.time;
+    r.has_ns = c.has_ns;
+    r.ns = c.ns;
+    return r;
+}
+
+__global__ void __launch_bounds__(256)
+    split_delim_sls_size_kernel(LcSplitDelimSlsCfg c, DelimSlsTables t, uint64_t n, uint32_t* __restrict__ rec_size,
+                                uint32_t* __restrict__ body_size, unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    LcDelimSlsVerdict v{0u, 0u, 0u, 0u};
+    uint32_t big = 0;
+    if (i < n) {
+        const LcDelimSlsRow r = split_delim_sls_row(c, t, i);
+        LcSlsCount64 s{0};
+        const uint32_t cnt = lc_split_delim_sls_body(c, t.base, r, s);
+        big = s.n + 16 > 0xFFFFFFFFull;
+        const uint32_t body = cnt && !big ? (uint32_t)s.n : 0u;
+        rec_size[i] = body ? 1 + lc_varint_size(body) + body : 0u;
+        body_size[i] = body;
+        v = lc_delim_sls_verdict(c.d, r.status);
+    }
+    // one atomic per warp and counter
+    const uint32_t w[5] = {__reduce_add_sync(0xFFFFFFFFu, v.ok), __reduce_add_sync(0xFFFFFFFFu, v.failed),
+                           __reduce_add_sync(0xFFFFFFFFu, v.erased), __reduce_add_sync(0xFFFFFFFFu, v.blank),
+                           __reduce_add_sync(0xFFFFFFFFu, big)};
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int k = 0; k < 5; ++k)
+            if (w[k])
+                atomicAdd(counters + k, (unsigned long long)w[k]);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    split_delim_sls_emit_kernel(LcSplitDelimSlsCfg c, DelimSlsTables t, uint64_t n,
+                                const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ body_size,
+                                uint8_t* __restrict__ out) {
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n)
+        return;
+    const uint32_t body = body_size[i];
+    if (!body)
+        return; // erased: no record
+    const LcDelimSlsRow r = split_delim_sls_row(c, t, i);
+    uint8_t h[6];
+    h[0] = 0x0A;
+    const uint32_t hn = 1 + lc_put_varint(h + 1, body);
+    LcSlsWrite s{out + rec_off[i], 0u, hn + body, threadIdx.x & 31, 32};
+    s.put(h, hn);
+    lc_split_delim_sls_body(c, t.base, r, s);
+}
+
+void launch_split_delim_sls_sizes(const LcSplitDelimSlsCfg& c, const DelimSlsTables& t, uint64_t n,
+                                  uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                  cudaStream_t st) {
+    if (n)
+        split_delim_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_size, d_body_size,
+                                                                                  d_counters);
+}
+
+void launch_split_delim_sls_emit(const LcSplitDelimSlsCfg& c, const DelimSlsTables& t, uint64_t n,
+                                 const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                 cudaStream_t st) {
+    if (n)
+        split_delim_sls_emit_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_off, d_body_size,
+                                                                                       d_out);
+}
+
 // ---- f4, split-fed: Log records of the pieces a splitter cuts from one source value (lc_exec.cuh: lc_span_sls_rec,
 // lc_span_sls_tile).  The size pass runs one thread per piece; the emit pass one warp per kSpanTile bytes of OUTPUT,
 // so records of 0 B and of many MiB share a launch without one warp copying a whole long record.

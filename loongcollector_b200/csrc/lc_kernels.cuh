@@ -9,6 +9,7 @@ struct LcRegexSlsCfg;
 struct LcDelimRegexSlsCfg;
 struct LcSpanSlsCfg;
 struct LcSplitRegexSlsCfg;
+struct LcSplitDelimSlsCfg;
 struct LcFilterSlsCfg;
 struct LcLz4Seq;
 struct LcLz4Chunk;
@@ -286,6 +287,16 @@ void launch_delim_regex_sls_sizes(const LcDelimRegexSlsCfg& c, const DelimRegexS
 void launch_delim_regex_sls_emit(const LcDelimRegexSlsCfg& c, const DelimRegexSlsTables& t, const uint32_t* d_ev_time,
                                  const uint32_t* d_ev_ns, uint64_t n, const uint64_t* d_rec_off,
                                  const uint32_t* d_body_size, uint8_t* d_out, cudaStream_t st);
+
+// f4, split -> delimiter chain (lc_exec.cuh: LcSplitDelimSlsCfg): the sizes and emit passes as for launch_sls_sizes
+// over the piece tables (t.ev_off / t.ev_len over t.base = the source value) and the delimiter tables over them;
+// d_counters: u64 [5] += successful, failed, discarded, blank, pieces whose record would reach 4 GiB.
+void launch_split_delim_sls_sizes(const LcSplitDelimSlsCfg& c, const DelimSlsTables& t, uint64_t n,
+                                  uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                  cudaStream_t st);
+void launch_split_delim_sls_emit(const LcSplitDelimSlsCfg& c, const DelimSlsTables& t, uint64_t n,
+                                 const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                 cudaStream_t st);
 
 // f4, split-fed: Log records of the pieces of one source value (lc_exec.cuh: LcSpanSlsCfg, keys on the device).
 // rec_size[k] = bytes of piece k's record (never 0); the emit pass writes the `total` bytes from the record offsets,

@@ -2052,21 +2052,86 @@ struct SplitRegexStage {
         r.mOutFailedEventsTotal.Add(ctr[1]);
         r.mDiscardedEventsTotal.Add(ctr[2]);
     }
+    void Process(PipelineEventGroup& group) const { r.Process(group); }
 };
 #define SPLIT_REGEX_STAGE_ARGS(x)                                                                                      \
     (x).kp.data(), (x).kl.data(), (uint32_t)(x).kp.size(), (x).r.mSourceKey.data(), (uint32_t)(x).r.mSourceKey.size(), \
         (x).Renamed().data(), (uint32_t)(x).Renamed().size(), (x).Opt().mKeepingSourceWhenParseFail,                    \
         (x).Opt().mKeepingSourceWhenParseSucceed, (x).Opt().mCopingRawLog, (x).wholeLine
 
+// The delimiter stage of the split -> delimiter chain: a ProcessorParseDelimiterNative's configuration as the chain
+// calls take it (SPLIT_DELIM_STAGE_ARGS), the host checks of lc_delim_sls_setup + lc_split_delim_sls_link, and the
+// counters Process would move.
+struct SplitDelimStage {
+    ProcessorParseDelimiterNative& d;
+    std::vector<const char*> kp;
+    std::vector<uint32_t> kl;
+    explicit SplitDelimStage(ProcessorParseDelimiterNative& next) : d(next) {
+        for (const auto& k : d.mKeys) {
+            kp.push_back(k.data());
+            kl.push_back((uint32_t)k.size());
+        }
+    }
+    const std::string& Renamed() const { return d.mCommonParserOptions.mRenamedSourceKey; }
+    const CommonParserOptions& Opt() const { return d.mCommonParserOptions; }
+    const uint8_t* Sep() const { return reinterpret_cast<const uint8_t*>(d.mSeparator.data()); }
+    bool Extend() const {
+        return d.mOverflowedFieldsTreatment == ProcessorParseDelimiterNative::OverflowedFieldsTreatment::EXTEND;
+    }
+    uint32_t MaxFields() const { return (uint32_t)d.mKeys.size() + 16; }
+    // whether the chain's device calls take this stage behind a splitter reading sourceKey
+    bool Accepts(const std::string& sourceKey, const StringView* okey) const {
+        if (!d.mDeviceSls || d.mSourceKey != sourceKey)
+            return false;
+        size_t keyBytes = d.mSourceKey.size() + Renamed().size() + 12;
+        for (const auto& k : d.mKeys)
+            keyBytes += k.size();
+        std::vector<uint8_t> kb(keyBytes);
+        std::vector<uint32_t> at(d.mKeys.size() + 4);
+        LcDelimSlsCfg dc;
+        LcSplitDelimSlsCfg c;
+        return !lc_delim_sls_setup(Sep(), (uint32_t)d.mSeparator.size(), (uint8_t)d.mQuote, Extend(),
+                                   d.mExtractingPartialFields, kp.data(), kl.data(), (uint32_t)kp.size(),
+                                   d.mSourceKey.data(), (uint32_t)d.mSourceKey.size(), Renamed().data(),
+                                   (uint32_t)Renamed().size(), Opt().mKeepingSourceWhenParseFail,
+                                   Opt().mKeepingSourceWhenParseSucceed, Opt().mCopingRawLog, MaxFields(), &dc,
+                                   kb.data(), at.data()) &&
+               !lc_split_delim_sls_link(dc, kp.data(), kl.data(), d.mSourceKey.data(), (uint32_t)d.mSourceKey.size(),
+                                        Renamed().data(), (uint32_t)Renamed().size(), okey ? okey->data() : nullptr,
+                                        okey ? (uint32_t)okey->size() : 0u, 0, 0, LC_SLS_NO_NS, &c);
+    }
+    // the device calls' counters[4] (successful, failed, discarded, blank) as the chain driver takes a stage's:
+    // successful, out_failed (a blank value counts as failed, :220-242), discarded, removed by a filter (none)
+    static void Fold(const uint64_t c4[4], uint64_t rctr[4]) {
+        rctr[0] = c4[0];
+        rctr[1] = c4[1] + c4[3];
+        rctr[2] = c4[2];
+        rctr[3] = 0;
+    }
+    void Add(const uint64_t ctr[3]) const {
+        d.mOutSuccessfulEventsTotal.Add(ctr[0]);
+        d.mOutFailedEventsTotal.Add(ctr[1]);
+        d.mDiscardedEventsTotal.Add(ctr[2]);
+    }
+    void Process(PipelineEventGroup& group) const { d.Process(group); }
+};
+#define SPLIT_DELIM_STAGE_ARGS(x)                                                                                      \
+    (x).Sep(), (uint32_t)(x).d.mSeparator.size(), (uint8_t)(x).d.mQuote, (x).Extend(),                                 \
+        (x).d.mExtractingPartialFields, (x).d.mAllowingShortenedFields, (x).MaxFields(), (x).kp.data(),             \
+        (x).kl.data(), (uint32_t)(x).kp.size(), (x).d.mSourceKey.data(), (uint32_t)(x).d.mSourceKey.size(),           \
+        (x).Renamed().data(), (uint32_t)(x).Renamed().size(), (x).Opt().mKeepingSourceWhenParseFail,                    \
+        (x).Opt().mKeepingSourceWhenParseSucceed, (x).Opt().mCopingRawLog
+
 namespace {
-// The split -> regex chain of either splitter: `process(group)` is the splitter's Process; the device calls are
-// sls(val, okey, pos, time, ns, out, cap, &len, &nev, rctr, sctr) and lz4(val, okey, pos, time, ns, tail, tailLen,
-// out, cap, &len, &raw, &nev, rctr, sctr) (rctr[4] = the regex stage's counters and the filter's removed events,
-// sctr[3] = the splitter's).  filter (or nullptr): the filter behind the regex stage, whose rule the device calls take
-// when filterOk.  sctr_total[3] += the splitter's counters of every device call.  rawSize null: out = the wire bytes;
-// else out = their LZ4 block and *rawSize their size.
-template <class ProcessFn, class Sls, class Lz4>
-bool SplitRegexChainSls(PipelineEventGroup& group, const SplitRegexStage& x, ProcessorFilterNative* filter,
+// The split -> parse chain of either splitter, with the parse stage x (SplitRegexStage, SplitDelimStage):
+// `process(group)` is the splitter's Process; the device calls are sls(val, okey, pos, time, ns, out, cap, &len, &nev,
+// rctr, sctr) and lz4(val, okey, pos, time, ns, tail, tailLen, out, cap, &len, &raw, &nev, rctr, sctr) (rctr[4] = the
+// stage's counters as x.Add takes them and the events a filter removed, sctr[3] = the splitter's).  filter (or
+// nullptr): the filter behind the regex stage, whose rule the device calls take when filterOk.  sctr_total[3] += the
+// splitter's counters of every device call.  rawSize null: out = the wire bytes; else out = their LZ4 block and
+// *rawSize their size.
+template <class Stage, class ProcessFn, class Sls, class Lz4>
+bool SplitRegexChainSls(PipelineEventGroup& group, const Stage& x, ProcessorFilterNative* filter,
                         bool filterOk, const std::string& sourceKey, bool rawContent, bool enableNs, std::string& out,
                         uint64_t* rawSize, std::string& err, ProcessFn process, Sls sls, Lz4 lz4, const char* what,
                         const char* lzwhat, uint64_t sctrTotal[3]) {
@@ -2079,7 +2144,7 @@ bool SplitRegexChainSls(PipelineEventGroup& group, const SplitRegexStage& x, Pro
     const StringView* okp = hasOffset ? &okey : nullptr;
     if (rawContent || !IsFlatGroup(group, sourceKey) || !x.Accepts(sourceKey, okp) || (filter && !filterOk)) {
         process(group);
-        x.r.Process(group);
+        x.Process(group);
         if (filter)
             filter->Process(group);
         if (!rawSize)
@@ -2406,6 +2471,101 @@ bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGrou
         [&](PipelineEventGroup& g) { Process(g); }, sls, lz4,
         filter ? "lc_multiline_split_regex_filter_parse_sls" : "lc_multiline_split_regex_parse_sls",
         filter ? "lc_multiline_split_regex_filter_parse_sls_lz4" : "lc_multiline_split_regex_parse_sls_lz4", ctr);
+    mMatchedEventsTotal.Add(ctr[0]);
+    mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
+    mUnmatchedLinesTotal.Add(ctr[2]);
+    return ok;
+}
+
+bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                                                 bool enableNs, std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                                                    bool enableNs, std::string& block, uint64_t& rawSize,
+                                                    std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitLogStringNative::ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                                                      bool enableNs, std::string& out, uint64_t* rawSize,
+                                                      std::string& err) {
+    const SplitDelimStage x(next);
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c4[4] = {0, 0, 0, 0};
+        const int rc = lc_split_delim_parse_sls(Engine(), src(val), val.size(), (uint8_t)mSplitChar,
+                                                SPLIT_DELIM_STAGE_ARGS(x), okey ? okey->data() : nullptr,
+                                                okey ? (uint32_t)okey->size() : 0u, pos, time, ns, o, cap, len, nev,
+                                                c4);
+        SplitDelimStage::Fold(c4, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c4[4] = {0, 0, 0, 0};
+        const int rc = lc_split_delim_parse_sls_lz4(Engine(), src(val), val.size(), (uint8_t)mSplitChar,
+                                                    SPLIT_DELIM_STAGE_ARGS(x), okey ? okey->data() : nullptr,
+                                                    okey ? (uint32_t)okey->size() : 0u, pos, time, ns, tail, tailLen,
+                                                    o, cap, len, raw, nev, c4);
+        SplitDelimStage::Fold(c4, rctr);
+        return rc;
+    };
+    uint64_t unused[3] = {0, 0, 0};
+    return SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_split_delim_parse_sls",
+        "lc_split_delim_parse_sls_lz4", unused);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& group,
+                                                          ProcessorParseDelimiterNative& next, bool enableNs,
+                                                          std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSlsLz4(PipelineEventGroup& group,
+                                                             ProcessorParseDelimiterNative& next, bool enableNs,
+                                                             std::string& block, uint64_t& rawSize, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGroup& group,
+                                                               ProcessorParseDelimiterNative& next, bool enableNs,
+                                                               std::string& out, uint64_t* rawSize, std::string& err) {
+    const SplitDelimStage x(next);
+    const bool discard = mMultiline.mUnmatchedContentTreatment == MultilineOptions::UnmatchedContentTreatment::DISCARD;
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c4[4] = {0, 0, 0, 0};
+        const int rc = lc_multiline_split_delim_parse_sls(
+            Engine(), src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
+            SPLIT_DELIM_STAGE_ARGS(x), okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos, time,
+            ns, o, cap, len, nev, c4, sctr);
+        SplitDelimStage::Fold(c4, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c4[4] = {0, 0, 0, 0};
+        const int rc = lc_multiline_split_delim_parse_sls_lz4(
+            Engine(), src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
+            SPLIT_DELIM_STAGE_ARGS(x), okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos, time,
+            ns, tail, tailLen, o, cap, len, raw, nev, c4, sctr);
+        SplitDelimStage::Fold(c4, rctr);
+        return rc;
+    };
+    // matched_events, input lines, unmatched lines: moved as Process moves them (:82-84,106-107)
+    uint64_t ctr[3] = {0, 0, 0};
+    const bool ok = SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_multiline_split_delim_parse_sls",
+        "lc_multiline_split_delim_parse_sls_lz4", ctr);
     mMatchedEventsTotal.Add(ctr[0]);
     mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
     mUnmatchedLinesTotal.Add(ctr[2]);

@@ -113,6 +113,7 @@ private:
 };
 
 class ProcessorParseRegexNative;
+class ProcessorParseDelimiterNative;
 class ProcessorFilterNative;
 
 class ProcessorSplitLogStringNative : public Processor {
@@ -150,6 +151,18 @@ public:
                       bool enableNs, std::string& out, std::string& err);
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative& filter,
                          bool enableNs, std::string& block, uint64_t& rawSize, std::string& err);
+    // Process(group), then next.Process(group) (next: the delimiter processor behind this one, reading SourceKey), then
+    // SLSEventGroupSerializer::Serialize: the same bytes or error message, and the same counter updates on both
+    // processors.  On a flat group without EnableRawContent, whose delimiter SourceKey is this SourceKey and whose
+    // configuration lc_split_delim_parse_sls accepts, each source event is split, parsed and serialised in one device
+    // pass (log.file.offset metadata included) and only the wire bytes come back; the group's events are left as they
+    // were.  Otherwise the three calls run.
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs, std::string& out,
+                      std::string& err);
+    // The same followed by LZ4Compressor::Compress.  A device-path group of one source event is compressed on the
+    // device (lc_split_delim_parse_sls_lz4); other groups compress SerializeSls's bytes.
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
+                         std::string& block, uint64_t& rawSize, std::string& err);
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
@@ -157,6 +170,8 @@ protected:
 private:
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative* filter,
                            bool enableNs, std::string& out, uint64_t* rawSize, std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
+                           std::string& out, uint64_t* rawSize, std::string& err);
 };
 
 class ProcessorSplitMultilineLogStringNative : public Processor {
@@ -186,6 +201,11 @@ public:
                       bool enableNs, std::string& out, std::string& err);
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative& filter,
                          bool enableNs, std::string& block, uint64_t& rawSize, std::string& err);
+    // The split -> delimiter chain, as ProcessorSplitLogStringNative's (lc_multiline_split_delim_parse_sls[_lz4]).
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs, std::string& out,
+                      std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
+                         std::string& block, uint64_t& rawSize, std::string& err);
     Counter mMatchedEventsTotal, mMatchedLinesTotal, mUnmatchedLinesTotal;
 
 protected:
@@ -194,6 +214,8 @@ protected:
 private:
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative* filter,
                            bool enableNs, std::string& out, uint64_t* rawSize, std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
+                           std::string& out, uint64_t* rawSize, std::string& err);
     CompiledRegex mStart, mContinue, mEnd;
 };
 
@@ -309,6 +331,7 @@ private:
                           std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs,
                            std::string& out, uint64_t* rawSize, std::string& err);
+    friend struct SplitDelimStage; // the split -> delimiter chain's SerializeSls
     bool mSourceKeyOverwritten = false;
     bool mDeviceSls = false; // the configuration passes lc_delim_parse_sls's checks
 };

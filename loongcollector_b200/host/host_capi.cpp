@@ -6,6 +6,7 @@
 #include <memory>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/lc_b200_host.h"
@@ -239,38 +240,47 @@ char* lc_host_chain_serialize_sls(lc_host_processor_t* delim, lc_host_processor_
         *raw_len_out = 0;
     try {
         Processor* d = delim->proc.get();
-        auto* r = dynamic_cast<ProcessorParseRegexNative*>(regex->proc.get());
+        Processor* second = regex->proc.get();
+        auto* r = dynamic_cast<ProcessorParseRegexNative*>(second);
         auto* pd = dynamic_cast<ProcessorParseDelimiterNative*>(d);
         auto* ps = dynamic_cast<ProcessorSplitLogStringNative*>(d);
         auto* pm = dynamic_cast<ProcessorSplitMultilineLogStringNative*>(d);
-        if (!(pd || ps || pm) || !r)
+        auto* sd = (ps || pm) ? dynamic_cast<ProcessorParseDelimiterNative*>(second) : nullptr;
+        if (!((pd || ps || pm) && r) && !sd)
             throw std::runtime_error("not a processor_parse_delimiter_native or a splitter, and a "
-                                     "processor_parse_regex_native");
-        // the chain's SerializeSls / SerializeSlsLz4 on whichever processor comes first
-        auto chain = [&](auto* p, PipelineEventGroup& g, std::string& res, uint64_t& raw, std::string& err) {
-            return mode == 2 ? p->SerializeSlsLz4(g, *r, enable_ns != 0, res, raw, err)
-                             : p->SerializeSls(g, *r, enable_ns != 0, res, err);
+                                     "processor_parse_regex_native; nor a splitter and a "
+                                     "processor_parse_delimiter_native");
+        // the chain's SerializeSls / SerializeSlsLz4 on whichever processor comes first, with the second as next
+        auto chain = [&](auto* p, auto& next, PipelineEventGroup& g, std::string& res, uint64_t& raw,
+                         std::string& err) {
+            return mode == 2 ? p->SerializeSlsLz4(g, next, enable_ns != 0, res, raw, err)
+                             : p->SerializeSls(g, next, enable_ns != 0, res, err);
+        };
+        auto first = [&](auto& next, PipelineEventGroup& g, std::string& res, uint64_t& raw, std::string& err) {
+            if constexpr (std::is_same_v<std::decay_t<decltype(next)>, ProcessorParseRegexNative>) {
+                if (pd)
+                    return chain(pd, next, g, res, raw, err);
+            }
+            return ps ? chain(ps, next, g, res, raw, err) : chain(pm, next, g, res, raw, err);
         };
         PipelineEventGroup group(std::make_shared<SourceBuffer>());
         if (!group.FromJsonString(group_json ? group_json : "null"))
             throw std::runtime_error("group JSON does not parse");
-        const uint64_t errs = d->EngineErrors() + r->EngineErrors();
+        const uint64_t errs = d->EngineErrors() + second->EngineErrors();
         std::string res, err;
         uint64_t raw = 0;
         bool ok;
         if (mode == 1) {
             d->Process(group);
-            r->Process(group);
+            second->Process(group);
             SLSEventGroupSerializer ser;
             ser.mEnableTimestampNanosecond = enable_ns != 0;
             ok = ser.Serialize(group, res, err);
         } else {
-            ok = pd   ? chain(pd, group, res, raw, err)
-                 : ps ? chain(ps, group, res, raw, err)
-                      : chain(pm, group, res, raw, err);
+            ok = r ? first(*r, group, res, raw, err) : first(*sd, group, res, raw, err);
         }
-        if (d->EngineErrors() + r->EngineErrors() != errs)
-            throw std::runtime_error("engine error inside Process: " + d->LastError() + r->LastError());
+        if (d->EngineErrors() + second->EngineErrors() != errs)
+            throw std::runtime_error("engine error inside Process: " + d->LastError() + second->LastError());
         if (!ok) {
             if (err_out)
                 *err_out = dup(err);
