@@ -727,6 +727,26 @@ int lc_lz4_compress_dev(lc_engine_t* e, const uint8_t* d_in, uint64_t nseg, cons
 int lc_lz4_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr, const uint32_t* seg_len,
                     uint8_t* out, uint64_t out_cap, uint64_t* blk_off, uint32_t* blk_len, uint64_t* out_len);
 
+/* zstd compression of serialised groups (FlusherSLS's CompressType "zstd", ZstdCompressor::Compress = ZSTD_compress
+ * at level 1): segment g = d_in[d_seg_off[g], + d_seg_len[g]) becomes one complete zstd *frame* (RFC 8878), the frames
+ * packed back to back in d_out: frame g = d_out[d_frm_off[g], + d_frm_len[g]).  The bytes are deterministic; they
+ * need not equal libzstd's.  Frame header: Single_Segment_Flag set, Frame_Content_Size present, no checksum, no
+ * dictionary; an empty segment is exactly 28 b5 2f fd 20 00 01 00 00.  Blocks hold at most 128 KiB of the segment,
+ * and a block that would not shrink is stored Raw, so a frame is never larger than ZSTD_compressBound(n).  Matches are
+ * those of the LZ4 compressor's parse pass (offsets up to 65 535); literals are Huffman-coded, sequences use the
+ * predefined FSE tables (the layout is pinned in lc_exec.cuh).  *out_len (host) = the total; if it exceeds out_cap,
+ * LC_ERR_CAPACITY and nothing is written.  A segment over LZ4_MAX_INPUT_SIZE (0x7E000000, the limit of the shared
+ * parse pass) is refused with LC_ERR_TOO_LARGE.  Workspace: the LZ4 call's, plus 128 KiB per block of 128 KiB. */
+int lc_zstd_compress_dev(lc_engine_t* e, const uint8_t* d_in, uint64_t nseg, const uint64_t* d_seg_off,
+                         const uint32_t* d_seg_len, uint8_t* d_out, uint64_t out_cap, uint64_t* d_frm_off,
+                         uint32_t* d_frm_len, uint64_t* out_len);
+
+/* The same with HOST segments seg_ptr[g][0, seg_len[g]): they go up in groups of whole segments while earlier groups
+ * are parsed, and only the frames come back (out, frm_off, frm_len on the host).  *out_len is set on LC_OK and on
+ * LC_ERR_CAPACITY. */
+int lc_zstd_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr, const uint32_t* seg_len,
+                     uint8_t* out, uint64_t out_cap, uint64_t* frm_off, uint32_t* frm_len, uint64_t* out_len);
+
 #ifdef __cplusplus
 }
 #endif

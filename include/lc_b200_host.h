@@ -78,6 +78,11 @@ char* lc_host_chain3_serialize_sls(lc_host_processor_t* split, lc_host_processor
 char* lc_host_lz4_compress(const char* const* data, const unsigned long long* len, unsigned long long n,
                            unsigned long long* len_out, unsigned long long* blk_len, char** err_out);
 
+/* ZstdCompressor::Compress (core/common/compression/ZstdCompressor.cpp), GPU-backed, the twin of lc_host_lz4_compress:
+ * the n inputs in one device call, one zstd frame each, back to back (frm_len[k]); or NULL + *err_out. */
+char* lc_host_zstd_compress(const char* const* data, const unsigned long long* len, unsigned long long n,
+                            unsigned long long* len_out, unsigned long long* frm_len, char** err_out);
+
 /* Loads a dynamic plugin the way the agent does (dlopen, dlsym("processor_interface"), version == 100 --
  * PluginRegistry.cpp:255-275) and drives it like DynamicCProcessorProxy (.cpp:21-36): init(ins, &config, &context),
  * process(plugin_state, &group), finalize(plugin_state).  Returns the processed group's JSON ("null" when group_json

@@ -97,6 +97,8 @@ def lib():
                                                                                          C.POINTER(u64), vp]
     L.lc_lz4_compress_dev.argtypes = [vp, vp, u64, vp, vp, vp, u64, vp, vp, C.POINTER(u64)]
     L.lc_lz4_compress.argtypes = [vp, u64, vp, vp, vp, u64, vp, vp, C.POINTER(u64)]
+    L.lc_zstd_compress_dev.argtypes = [vp, vp, u64, vp, vp, vp, u64, vp, vp, C.POINTER(u64)]
+    L.lc_zstd_compress.argtypes = [vp, u64, vp, vp, vp, u64, vp, vp, C.POINTER(u64)]
     L.lc_delim_parse_sls_lz4.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32, u8, i32, i32, i32, u32] + \
         sls_cfg + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
     L.lc_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp] + sls_cfg + \
@@ -1017,6 +1019,33 @@ class Engine:
                                      _p(blen), C.byref(need)))
         return [bytes(out[int(o):int(o) + int(ln)]) for o, ln in zip(boff[:n], blen[:n])]
 
+    def zstd_compress_dev(self, d_in, nseg, d_seg_off, d_seg_len, d_out=None, out_cap=0, d_frm_off=None,
+                          d_frm_len=None):
+        """One zstd frame per device segment d_in[d_seg_off[g], + d_seg_len[g]) (u64 / u32 tables), packed in d_out
+        with the table d_frm_off (u64) / d_frm_len (u32) (lc_zstd_compress_dev).  Returns the byte count written to
+        d_out, or with d_out None the byte count needed."""
+        need = C.c_uint64(0)
+        rc = lib().lc_zstd_compress_dev(self._h, _p(d_in), nseg, _p(d_seg_off), _p(d_seg_len), _p(d_out), out_cap,
+                                        _p(d_frm_off), _p(d_frm_len), C.byref(need))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value)  # a sizing query
+        _check(rc)
+        return int(need.value)
+
+    def zstd_compress(self, segments, out_cap=None):
+        """Host segments (bytes-like) in, one zstd frame each out (lc_zstd_compress).  Returns the list of frames."""
+        segs = [_u8(s) for s in segments]
+        n = len(segs)
+        ptrs = (C.c_void_p * max(n, 1))(*[s.ctypes.data for s in segs])
+        lens = np.array([s.size for s in segs] or [0], np.uint32)
+        cap = int(out_cap if out_cap is not None else sum(zstd_bound(int(x)) for x in lens[:n]))
+        out = np.empty(max(cap, 1), np.uint8)
+        foff, flen = np.zeros(max(n, 1), np.uint64), np.zeros(max(n, 1), np.uint32)
+        need = C.c_uint64(0)
+        _check(lib().lc_zstd_compress(self._h, n, C.cast(ptrs, C.c_void_p), _p(lens), _p(out), cap, _p(foff),
+                                      _p(flen), C.byref(need)))
+        return [bytes(out[int(o):int(o) + int(ln)]) for o, ln in zip(foff[:n], flen[:n])]
+
     def split_lines_dev(self, d_buf, length, split_char, d_off, d_len, cap):
         n = C.c_uint64(0)
         _check(lib().lc_split_lines_dev(self._h, _p(d_buf), length, split_char, _p(d_off), _p(d_len), cap,
@@ -1263,6 +1292,40 @@ def host_lz4_compress(inputs):
     for k in range(n):
         res.append(data[o:o + int(blen[k])])
         o += int(blen[k])
+    return res, None
+
+
+def zstd_bound(n):
+    """ZSTD_compressBound(n): the largest frame lc_zstd_compress[_dev] makes of n bytes."""
+    return n + (n >> 8) + (((128 << 10) - n) >> 11 if n < (128 << 10) else 0)
+
+
+def host_zstd_compress(inputs):
+    """The host layer's GPU-backed ZstdCompressor::Compress over a list of byte strings in one device call
+    (lc_host_zstd_compress): (list of frames, None) or (None, error)."""
+    L = lib()
+    L.lc_host_zstd_compress.restype = C.c_void_p
+    L.lc_host_zstd_compress.argtypes = [C.c_void_p, C.c_void_p, C.c_ulonglong, C.POINTER(C.c_ulonglong), C.c_void_p,
+                                        C.POINTER(C.c_void_p)]
+    L.lc_host_string_free.argtypes = [C.c_void_p]
+    bufs = [bytes(x) for x in inputs]
+    n = len(bufs)
+    ptrs = (C.c_char_p * max(n, 1))(*bufs)
+    lens = np.array([len(b) for b in bufs] or [0], np.uint64)
+    flen = np.zeros(max(n, 1), np.uint64)
+    total, err = C.c_ulonglong(0), C.c_void_p()
+    out = L.lc_host_zstd_compress(C.cast(ptrs, C.c_void_p), _p(lens), n, C.byref(total), _p(flen), C.byref(err))
+    if not out:
+        msg = C.string_at(err.value).decode() if err.value else "unknown error"
+        if err.value:
+            L.lc_host_string_free(err)
+        return None, msg
+    data = C.string_at(out, total.value)
+    L.lc_host_string_free(out)
+    res, o = [], 0
+    for k in range(n):
+        res.append(data[o:o + int(flen[k])])
+        o += int(flen[k])
     return res, None
 
 

@@ -102,6 +102,9 @@ struct lc_engine {
     // LZ4 compressor: sequences, chunk summaries, chunk sizes / anchors, chunk and block offsets, host-call tables and
     // output; no parse or SLS stage uses them
     DevBuf z_seq, z_info, z_size, z_first, z_choff, z_tab, z_out;
+    // zstd compressor (behind the LZ4 parse pass): per-segment first block, per-block body sizes and frame bytes,
+    // block offsets, one LC_ZSTD_BLOCK slot per block for its compressed body
+    DevBuf zs_first, zs_size, zs_off, zs_slot;
     // delimiter -> regex -> SLS chain: the delimiter's key strings, the value table, the regex tables over it, side-copy
     // sizes and slots, the per-chunk scan descriptors of the tap; no stage of the chain uses them for anything else
     DevBuf dr_keys, dr_val_off, dr_val_len, dr_status, dr_cap_off, dr_cap_len, dr_copy, dr_slot, dr_desc;
@@ -322,6 +325,7 @@ void lc_engine_destroy(lc_engine_t* e) {
                       &e->lines_off, &e->lines_len, &e->flags, &e->state, &e->cnt, &e->pos, &e->lab_sizes,
                       &e->lab_off, &e->lab, &e->order, &e->desc, &e->small, &e->split_scratch, &e->sls_plan,
                       &e->z_seq, &e->z_info, &e->z_size, &e->z_first, &e->z_choff, &e->z_tab, &e->z_out,
+                      &e->zs_first, &e->zs_size, &e->zs_off, &e->zs_slot,
                       &e->dr_keys, &e->dr_val_off, &e->dr_val_len, &e->dr_status, &e->dr_cap_off, &e->dr_cap_len,
                       &e->dr_copy, &e->dr_slot, &e->dr_desc, &e->fl_tab, &e->fl_match, &e->fl_dig, &e->fl_keep};
     for (DevBuf* b : bufs)
@@ -3491,50 +3495,38 @@ int lz4_one_block(lc_engine_t* e, const char* what, const uint8_t* d_src, uint64
     return LC_OK;
 }
 
-} // namespace
-
-extern "C" {
-
-int lc_lz4_compress_dev(lc_engine_t* e, const uint8_t* d_in, uint64_t nseg, const uint64_t* d_seg_off,
-                        const uint32_t* d_seg_len, uint8_t* d_out, uint64_t out_cap, uint64_t* d_blk_off,
-                        uint32_t* d_blk_len, uint64_t* out_len) {
-    static const char* what = "lc_lz4_compress_dev";
-    if (!e || !out_len || (nseg && (!d_in || !d_seg_off || !d_seg_len)))
-        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
-    *out_len = 0;
-    if (nseg == 0)
-        return LC_OK;
-    if (nseg >= (1ull << 32))
+// The parse pass over device segments (lc_lz4_compress_dev, lc_zstd_compress_dev; g.in, g.seg_off, g.seg_len and
+// g.nseg >= 1 set): the chunk tables, then every chunk's matches.
+int parse_dev(lc_engine_t* e, const char* what, lck::Lz4Segs& g) {
+    if (g.nseg >= (1ull << 32))
         return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^32 segments per call");
     int rc = bind(e);
     if (rc)
         return rc;
-    lck::Lz4Segs g{d_in, d_seg_off, d_seg_len, nullptr, nseg, 0};
     rc = lz4_chunk_tables(e, what, g, nullptr, 0);
     if (rc)
         return rc;
     lck::launch_lz4_parse(g, 0, g.nchunks, e->z_seq.as<LcLz4Seq>(), e->z_info.as<LcLz4Chunk>(), e->stream);
     e->launches++;
     CU_TRY(cudaGetLastError());
-    // without an output (a sizing query) every total is over capacity: blocks are at least one byte
-    rc = lz4_finish(e, what, g, d_out, d_out && d_blk_off && d_blk_len ? out_cap : 0, d_blk_off, d_blk_len, out_len);
-    if (rc)
-        return rc;
-    CU_TRY(cudaStreamSynchronize(e->stream));
     return LC_OK;
 }
 
-int lc_lz4_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr, const uint32_t* seg_len,
-                    uint8_t* out, uint64_t out_cap, uint64_t* blk_off, uint32_t* blk_len, uint64_t* out_len) {
-    static const char* what = "lc_lz4_compress";
-    if (!e || !out_len || (nseg && (!seg_ptr || !seg_len || !blk_off || !blk_len)))
-        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
-    *out_len = 0;
-    if (nseg == 0)
-        return LC_OK;
+int drain_copies(lc_engine_t* e, int code) {
+    cudaStreamSynchronize(e->s_h2d);
+    cudaStreamSynchronize(e->stream);
+    return code;
+}
+
+// The parse pass over nseg >= 1 HOST segments (lc_lz4_compress, lc_zstd_compress): they are packed at 16-byte aligned
+// offsets of the engine's input buffer (g), going up in groups of whole segments on the copy stream while each landed
+// group's chunks are parsed.  *d_off / *d_len: room for the per-segment output table.  A failure after the first
+// upload returns through drain_copies().
+int parse_host(lc_engine_t* e, const char* what, uint64_t nseg, const uint8_t* const* seg_ptr, const uint32_t* seg_len,
+               lck::Lz4Segs& g, uint64_t** d_off, uint32_t** d_len) {
     if (nseg >= (1ull << 32))
         return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^32 segments per call");
-    // the segments are packed at 16-byte aligned offsets of the engine's input buffer; the chunk table is built here
+    // the chunk table is built here
     std::vector<uint64_t> soff(nseg), first(nseg);
     uint64_t total_in = 0, nchunks = 0;
     for (uint64_t k = 0; k < nseg; ++k) {
@@ -3553,16 +3545,15 @@ int lc_lz4_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr
     CU_TRY(e->in.ensure(total_in + 16));
     CU_TRY(e->z_tab.ensure(nseg * 24));
     uint64_t* d_soff = e->z_tab.as<uint64_t>();
-    uint64_t* d_boff = d_soff + nseg;
-    uint32_t* d_slen = reinterpret_cast<uint32_t*>(d_boff + nseg);
-    uint32_t* d_blen = d_slen + nseg;
+    *d_off = d_soff + nseg;
+    uint32_t* d_slen = reinterpret_cast<uint32_t*>(*d_off + nseg);
+    *d_len = d_slen + nseg;
     CU_TRY(cudaMemcpyAsync(d_soff, soff.data(), nseg * 8, cudaMemcpyHostToDevice, e->stream));
     CU_TRY(cudaMemcpyAsync(d_slen, seg_len, nseg * 4, cudaMemcpyHostToDevice, e->stream));
-    lck::Lz4Segs g{e->in.as<uint8_t>(), d_soff, d_slen, nullptr, nseg, 0};
+    g = lck::Lz4Segs{e->in.as<uint8_t>(), d_soff, d_slen, nullptr, nseg, 0};
     rc = lz4_chunk_tables(e, what, g, first.data(), nchunks);
     if (rc)
         return rc;
-    // groups of whole segments go up on the copy stream; each group's chunks are parsed as soon as it has landed
     const uint64_t kGroupBytes = 32ull << 20;
     uint64_t ngroups = (total_in + kGroupBytes - 1) / kGroupBytes;
     ngroups = ngroups < 1 ? 1 : ngroups > 64 ? 64 : ngroups;
@@ -3571,14 +3562,9 @@ int lc_lz4_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr
     rc = ensure_copy_streams(e, (int)ngroups);
     if (rc)
         return rc;
-    auto drain = [&](int code) {
-        cudaStreamSynchronize(e->s_h2d);
-        cudaStreamSynchronize(e->stream);
-        return code;
-    };
     if (cudaEventRecord(e->ev_comp[0], e->stream) != cudaSuccess ||
         cudaStreamWaitEvent(e->s_h2d, e->ev_comp[0], 0) != cudaSuccess)
-        return drain(fail(LC_ERR_CUDA, "stream ordering failed"));
+        return drain_copies(e, fail(LC_ERR_CUDA, "stream ordering failed"));
     uint8_t* d_in = e->in.as<uint8_t>();
     uint64_t s0 = 0;
     for (uint64_t c = 0; c < ngroups; ++c) {
@@ -3589,10 +3575,10 @@ int lc_lz4_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr
         for (uint64_t k = s0; k < s1; ++k)
             if (seg_len[k] && cudaMemcpyAsync(d_in + soff[k], seg_ptr[k], seg_len[k], cudaMemcpyHostToDevice,
                                               e->s_h2d) != cudaSuccess)
-                return drain(fail(LC_ERR_CUDA, std::string(what) + ": upload failed"));
+                return drain_copies(e, fail(LC_ERR_CUDA, std::string(what) + ": upload failed"));
         if (cudaEventRecord(e->ev_h2d[c], e->s_h2d) != cudaSuccess ||
             cudaStreamWaitEvent(e->stream, e->ev_h2d[c], 0) != cudaSuccess)
-            return drain(fail(LC_ERR_CUDA, "stream ordering failed"));
+            return drain_copies(e, fail(LC_ERR_CUDA, "stream ordering failed"));
         const uint64_t k1 = s1 < nseg ? first[s1] : nchunks;
         lck::launch_lz4_parse(g, s0 < nseg ? first[s0] : nchunks, k1, e->z_seq.as<LcLz4Seq>(),
                               e->z_info.as<LcLz4Chunk>(), e->stream);
@@ -3600,17 +3586,165 @@ int lc_lz4_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr
         s0 = s1;
     }
     if (cudaGetLastError() != cudaSuccess)
-        return drain(fail(LC_ERR_CUDA, std::string(what) + ": parse launch failed"));
-    rc = lz4_finish(e, what, g, nullptr, out_cap, d_boff, d_blen, out_len);
-    if (rc)
-        return drain(rc);
-    if (*out_len && !out)
-        return drain(fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments"));
-    CU_TRY(cudaMemcpyAsync(out, e->z_out.p, *out_len, cudaMemcpyDeviceToHost, e->stream));
-    CU_TRY(cudaMemcpyAsync(blk_off, d_boff, nseg * 8, cudaMemcpyDeviceToHost, e->stream));
-    CU_TRY(cudaMemcpyAsync(blk_len, d_blen, nseg * 4, cudaMemcpyDeviceToHost, e->stream));
+        return drain_copies(e, fail(LC_ERR_CUDA, std::string(what) + ": parse launch failed"));
+    return LC_OK;
+}
+
+// The host calls' ending: the output (in z_out) and the per-segment table back to the host.
+int copy_back(lc_engine_t* e, const char* what, uint64_t nseg, uint8_t* out, uint64_t* off, uint32_t* len,
+              const uint64_t* d_off, const uint32_t* d_len, uint64_t out_len) {
+    if (out_len && !out)
+        return drain_copies(e, fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments"));
+    CU_TRY(cudaMemcpyAsync(out, e->z_out.p, out_len, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(off, d_off, nseg * 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(len, d_len, nseg * 4, cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(cudaStreamSynchronize(e->stream));
     return LC_OK;
+}
+
+// After the parse pass: the zstd block table (bfirst_host / nblocks from the host, or counted here), every block's
+// body in its slot, the frame offsets, and (when the total fits out_cap) the frames at d_out and the per-segment
+// table.  *out_len = the total on LC_OK and on LC_ERR_CAPACITY.  d_out == nullptr: the engine's z_out.
+int zstd_finish(lc_engine_t* e, const char* what, const lck::Lz4Segs& g, const uint64_t* bfirst_host, uint64_t nblocks,
+                uint8_t* d_out, uint64_t out_cap, uint64_t* d_frm_off, uint32_t* d_frm_len, uint64_t* out_len) {
+    Small* ds = e->small.as<Small>();
+    Small* hs = (Small*)e->h_small;
+    CU_TRY(e->zs_first.ensure(g.nseg * 8 + 8));
+    uint64_t* d_bfirst = e->zs_first.as<uint64_t>();
+    uint64_t* desc;
+    int rc;
+    if (bfirst_host) {
+        CU_TRY(cudaMemcpyAsync(d_bfirst, bfirst_host, g.nseg * 8, cudaMemcpyHostToDevice, e->stream));
+    } else {
+        CU_TRY(e->zs_size.ensure(g.nseg * 4 + 4));
+        rc = prep_desc(e, lck::scan_tiles(g.nseg), &desc);
+        if (rc)
+            return rc;
+        lck::launch_zstd_nblocks(g.seg_len, g.nseg, e->zs_size.as<uint32_t>(), e->stream);
+        lck::launch_exclusive_sum(e->zs_size.as<uint32_t>(), g.nseg, d_bfirst, &ds->total, desc, &ds->tickets[2],
+                                  e->stream);
+        e->launches += 2;
+        CU_TRY(cudaGetLastError());
+        CU_TRY(cudaMemcpyAsync(&hs->total, &ds->total, 8, cudaMemcpyDeviceToHost, e->stream));
+        CU_TRY(cudaStreamSynchronize(e->stream));
+        nblocks = hs->total;
+    }
+    CU_TRY(e->zs_size.ensure(nblocks * 8));
+    CU_TRY(e->zs_off.ensure(nblocks * 8 + 8));
+    CU_TRY(e->zs_slot.ensure(nblocks * LC_ZSTD_BLOCK));
+    uint32_t* d_body = e->zs_size.as<uint32_t>();
+    uint32_t* d_esz = d_body + nblocks;
+    lck::launch_zstd_blocks(g, d_bfirst, nblocks, e->z_seq.as<LcLz4Seq>(), e->z_info.as<LcLz4Chunk>(),
+                            e->zs_slot.as<uint8_t>(), d_body, d_esz, e->stream);
+    rc = prep_desc(e, lck::scan_tiles(nblocks), &desc);
+    if (rc)
+        return rc;
+    lck::launch_exclusive_sum(d_esz, nblocks, e->zs_off.as<uint64_t>(), &ds->total, desc, &ds->tickets[2], e->stream);
+    e->launches += 2;
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(&hs->total, &ds->total, 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    *out_len = hs->total;
+    if (hs->total > out_cap)
+        return fail(LC_ERR_CAPACITY, std::string(what) + ": output capacity too small");
+    if (!d_out) {
+        CU_TRY(e->z_out.ensure(hs->total));
+        d_out = e->z_out.as<uint8_t>();
+    }
+    lck::launch_zstd_emit(g, d_bfirst, nblocks, e->zs_slot.as<uint8_t>(), d_body, e->zs_off.as<uint64_t>(), &ds->total,
+                          d_out, d_frm_off, d_frm_len, e->stream);
+    e->launches += 2;
+    CU_TRY(cudaGetLastError());
+    return LC_OK;
+}
+
+} // namespace
+
+extern "C" {
+
+int lc_lz4_compress_dev(lc_engine_t* e, const uint8_t* d_in, uint64_t nseg, const uint64_t* d_seg_off,
+                        const uint32_t* d_seg_len, uint8_t* d_out, uint64_t out_cap, uint64_t* d_blk_off,
+                        uint32_t* d_blk_len, uint64_t* out_len) {
+    static const char* what = "lc_lz4_compress_dev";
+    if (!e || !out_len || (nseg && (!d_in || !d_seg_off || !d_seg_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (nseg == 0)
+        return LC_OK;
+    lck::Lz4Segs g{d_in, d_seg_off, d_seg_len, nullptr, nseg, 0};
+    int rc = parse_dev(e, what, g);
+    if (rc)
+        return rc;
+    // without an output (a sizing query) every total is over capacity: blocks are at least one byte
+    rc = lz4_finish(e, what, g, d_out, d_out && d_blk_off && d_blk_len ? out_cap : 0, d_blk_off, d_blk_len, out_len);
+    if (rc)
+        return rc;
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    return LC_OK;
+}
+
+int lc_lz4_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr, const uint32_t* seg_len,
+                    uint8_t* out, uint64_t out_cap, uint64_t* blk_off, uint32_t* blk_len, uint64_t* out_len) {
+    static const char* what = "lc_lz4_compress";
+    if (!e || !out_len || (nseg && (!seg_ptr || !seg_len || !blk_off || !blk_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (nseg == 0)
+        return LC_OK;
+    lck::Lz4Segs g;
+    uint64_t* d_boff;
+    uint32_t* d_blen;
+    int rc = parse_host(e, what, nseg, seg_ptr, seg_len, g, &d_boff, &d_blen);
+    if (rc)
+        return rc;
+    rc = lz4_finish(e, what, g, nullptr, out_cap, d_boff, d_blen, out_len);
+    return rc ? drain_copies(e, rc) : copy_back(e, what, nseg, out, blk_off, blk_len, d_boff, d_blen, *out_len);
+}
+
+int lc_zstd_compress_dev(lc_engine_t* e, const uint8_t* d_in, uint64_t nseg, const uint64_t* d_seg_off,
+                         const uint32_t* d_seg_len, uint8_t* d_out, uint64_t out_cap, uint64_t* d_frm_off,
+                         uint32_t* d_frm_len, uint64_t* out_len) {
+    static const char* what = "lc_zstd_compress_dev";
+    if (!e || !out_len || (nseg && (!d_in || !d_seg_off || !d_seg_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (nseg == 0)
+        return LC_OK;
+    lck::Lz4Segs g{d_in, d_seg_off, d_seg_len, nullptr, nseg, 0};
+    int rc = parse_dev(e, what, g);
+    if (rc)
+        return rc;
+    // without an output (a sizing query) every total is over capacity: frames are at least 9 bytes
+    rc = zstd_finish(e, what, g, nullptr, 0, d_out, d_out && d_frm_off && d_frm_len ? out_cap : 0, d_frm_off,
+                     d_frm_len, out_len);
+    if (rc)
+        return rc;
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    return LC_OK;
+}
+
+int lc_zstd_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr, const uint32_t* seg_len,
+                     uint8_t* out, uint64_t out_cap, uint64_t* frm_off, uint32_t* frm_len, uint64_t* out_len) {
+    static const char* what = "lc_zstd_compress";
+    if (!e || !out_len || (nseg && (!seg_ptr || !seg_len || !frm_off || !frm_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (nseg == 0)
+        return LC_OK;
+    lck::Lz4Segs g;
+    uint64_t* d_foff;
+    uint32_t* d_flen;
+    int rc = parse_host(e, what, nseg, seg_ptr, seg_len, g, &d_foff, &d_flen);
+    if (rc)
+        return rc;
+    std::vector<uint64_t> bfirst(nseg);
+    uint64_t nblocks = 0;
+    for (uint64_t k = 0; k < nseg; ++k) {
+        bfirst[k] = nblocks;
+        nblocks += lc_zstd_nblocks(seg_len[k]);
+    }
+    rc = zstd_finish(e, what, g, bfirst.data(), nblocks, nullptr, out_cap, d_foff, d_flen, out_len);
+    return rc ? drain_copies(e, rc) : copy_back(e, what, nseg, out, frm_off, frm_len, d_foff, d_flen, *out_len);
 }
 
 } // extern "C"

@@ -2498,3 +2498,734 @@ LC_HD void lc_lz4_emit_chunk(const uint8_t* s, uint32_t n, uint32_t c0, const Lc
     if (last)
         lc_lz4_put_seq(s, a, n - a, 0, 0, o, lane, W);
 }
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, zstd: one zstd *frame* (RFC 8878) per segment, for FlusherSLS's CompressType "zstd" (ZstdCompressor =
+// ZSTD_compress).  The bytes are a sequential function of the segment s[0, n); they need not equal libzstd's.
+//   frame      = magic 28 b5 2f fd; a Frame_Header_Descriptor with Single_Segment_Flag = 1, no checksum and no
+//                dictionary; Frame_Content_Size in 1 byte (n < 256, FCS flag 0), 2 bytes (n < 65792, flag 1, n - 256) or
+//                4 bytes (flag 2); then the blocks.  An empty segment is one empty Raw block: 28 b5 2f fd 20 00 01 00 00.
+//   blocks     = LC_ZSTD_BLOCK (128 KiB) bytes of the segment each, the last one shorter.  A block whose compressed
+//                body would not be smaller than its bytes is a Raw block; RLE blocks are not used.
+//   sequences  = the matches lc_lz4_parse_chunk finds in the block's two LZ4 chunks (they end inside their chunk, so
+//                inside the block), each a new offset: Offset_Value = distance + 3, never a repeat offset.
+//                Literals_Length = the bytes since the block's previous match (or its start): literal runs are cut at
+//                block boundaries, and the bytes after the last match are the block's trailing literals.  LL, OF and ML
+//                use the predefined distributions (Symbol_Compression_Modes = 0); each FSE state starts at the lowest
+//                decoding state of its symbol.  A block without a match has Number_of_Sequences = 0.
+//   literals   = RLE for one distinct byte; Raw for fewer than LC_ZSTD_MIN_HUF literals or when Huffman would not be
+//                smaller; else Huffman_Compressed in 4 streams, with the code of lc_zstd_huf_lengths (at most
+//                LC_ZSTD_HUF_MAX bits).  Its weights are described with FSE (accuracy log LC_ZSTD_WLOG, counts of
+//                lc_zstd_wnorm) or in the direct 4-bit form, whichever is smaller (the direct form on a tie); with
+//                neither possible the literals go Raw.
+// A block is built by W lanes (lc_zstd_block): a warp on the device (W = 32), any W on the host (tests/emul), with the
+// same bytes.  Its literals are gathered behind each chunk's matches in the LZ4 sequence scratch, which has room for
+// them: a chunk of c bytes with L literals has at most (c - L) / 4 matches of 8 bytes, and 2 (c - L) + L <= 2 c.
+#define LC_ZSTD_BLOCK (2u * LC_LZ4_CHUNK) // segment bytes per block: two LZ4 chunks
+#define LC_ZSTD_MIN_HUF 64u               // fewer literals are not Huffman-coded (4 streams need at least 6)
+#define LC_ZSTD_HUF_MAX 11u               // longest Huffman code
+#define LC_ZSTD_WLOG 6u                   // accuracy log of the FSE weight description
+#define LC_ZSTD_RAW 0u                    // literal modes (Literals_Block_Type)
+#define LC_ZSTD_RLE 1u
+#define LC_ZSTD_HUF 2u
+
+LC_HD uint32_t lc_zstd_nblocks(uint32_t n) { return n ? (n + LC_ZSTD_BLOCK - 1) / LC_ZSTD_BLOCK : 1u; }
+LC_HD uint32_t lc_zstd_fcs_bytes(uint32_t n) { return n < 256 ? 1u : n < 65536 + 256 ? 2u : 4u; }
+LC_HD uint32_t lc_zstd_hdr(uint32_t n) { return 5 + lc_zstd_fcs_bytes(n); } // magic, descriptor, content size
+LC_HD uint64_t lc_zstd_bound(uint64_t n) {                                    // ZSTD_compressBound
+    return n + (n >> 8) + (n < (128u << 10) ? ((128u << 10) - n) >> 11 : 0u);
+}
+
+LC_HD uint32_t lc_popc(uint32_t m) {
+#if defined(__CUDA_ARCH__)
+    return __popc(m);
+#else
+    return __builtin_popcount(m);
+#endif
+}
+LC_HD uint32_t lc_bits(uint32_t k) { return k >= 32 ? 0xFFFFFFFFu : (1u << k) - 1u; } // the k low bits
+LC_HD void lc_or32(uint32_t* p, uint32_t v) {
+#if defined(__CUDA_ARCH__)
+    atomicOr(p, v);
+#else
+    *p |= v;
+#endif
+}
+LC_HD void lc_add32(uint32_t* p, uint32_t v) {
+#if defined(__CUDA_ARCH__)
+    atomicAdd(p, v);
+#else
+    *p += v;
+#endif
+}
+
+// OR of v[0, W) (all lanes call it)
+LC_HD uint32_t lc_warp_or(const uint32_t* v, uint32_t lane, uint32_t W) {
+#if defined(__CUDA_ARCH__)
+    (void)W;
+    return __reduce_or_sync(0xFFFFFFFFu, v[lane]);
+#else
+    (void)lane;
+    uint32_t m = 0;
+    for (uint32_t j = 0; j < W; ++j)
+        m |= v[j];
+    return m;
+#endif
+}
+
+// v[0, W) -> its exclusive prefix sums, in place; returns the total (all lanes call it)
+LC_HD uint32_t lc_warp_exscan(uint32_t* v, uint32_t lane, uint32_t W) {
+#if defined(__CUDA_ARCH__)
+    (void)W;
+    const uint32_t x = v[lane];
+    uint32_t s = x;
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, s, d);
+        if (lane >= d)
+            s += y;
+    }
+    v[lane] = s - x;
+    return __shfl_sync(0xFFFFFFFFu, s, 31);
+#else
+    (void)lane;
+    uint32_t s = 0;
+    for (uint32_t j = 0; j < W; ++j) {
+        const uint32_t x = v[j];
+        v[j] = s;
+        s += x;
+    }
+    return s;
+#endif
+}
+
+// Forward bit writer, least significant bit first (every zstd bitstream and the FSE table description).  Bytes at
+// and past `cap` are counted in n but not written.
+struct LcBitW {
+    uint8_t* o;
+    uint32_t n, cap, nb;
+    uint64_t acc;
+};
+LC_HD void lc_bw_put(LcBitW& b, uint32_t v, uint32_t nbits) { // nbits <= 24
+    b.acc |= (uint64_t)v << b.nb;
+    b.nb += nbits;
+    while (b.nb >= 8) {
+        if (b.n < b.cap)
+            b.o[b.n] = (uint8_t)b.acc;
+        ++b.n;
+        b.acc >>= 8;
+        b.nb -= 8;
+    }
+}
+LC_HD void lc_bw_align(LcBitW& b) { // zero bits up to the next byte
+    if (b.nb)
+        lc_bw_put(b, 0, 8 - b.nb);
+}
+LC_HD void lc_bw_close(LcBitW& b) { // a backward-read bitstream ends with a 1 bit, then zeros to the byte
+    lc_bw_put(b, 1, 1);
+    lc_bw_align(b);
+}
+
+// An FSE table of accuracy log al: the decoding spread sym[] and, per symbol s, its decoding states in increasing
+// order st[cum[s], cum[s + 1]).
+struct LcFse {
+    uint16_t cum[54];
+    uint8_t st[64];
+    uint8_t sym[64];
+    uint32_t al;
+};
+
+// normalised count of symbol s (-1 = "less than 1"): the predefined LL (tab 0), ML (1) and OF (2) distributions
+// (RFC 8878 3.1.1.3.2.2), or wn[s] (tab 3)
+LC_HD int lc_zstd_norm(uint32_t tab, const int16_t* wn, uint32_t s) {
+    if (tab == 0)
+        return s == 0 ? 4 : s == 1 ? 3 : s <= 12 ? 2 : s <= 15 ? 1 : s <= 24 ? 2 : s == 25 ? 3 : s == 26 ? 2 : s <= 31 ? 1 : -1;
+    if (tab == 1)
+        return s == 0 ? 1 : s == 1 ? 4 : s == 2 ? 3 : s <= 8 ? 2 : s <= 45 ? 1 : -1;
+    if (tab == 2)
+        return s <= 5 ? 1 : s <= 8 ? 2 : s <= 23 ? 1 : -1;
+    return wn[s];
+}
+
+// one lane builds t for the nsym symbols of table `tab` (FSE_buildDTable's spread)
+LC_HD void lc_fse_build(uint32_t tab, const int16_t* wn, uint32_t nsym, uint32_t al, LcFse& t) {
+    const uint32_t T = 1u << al, step = (T >> 1) + (T >> 3) + 3;
+    uint32_t high = T - 1, pos = 0;
+    t.al = al;
+    t.cum[0] = 0;
+    for (uint32_t s = 0; s < nsym; ++s) {
+        const int c = lc_zstd_norm(tab, wn, s);
+        if (c == -1)
+            t.sym[high--] = (uint8_t)s;
+        t.cum[s + 1] = (uint16_t)(t.cum[s] + (c < 0 ? 1 : c));
+    }
+    for (uint32_t s = 0; s < nsym; ++s)
+        for (int i = 0, c = lc_zstd_norm(tab, wn, s); i < c; ++i) {
+            t.sym[pos] = (uint8_t)s;
+            do
+                pos = (pos + step) & (T - 1);
+            while (pos > high);
+        }
+    for (uint32_t u = 0; u < T; ++u) // cum[s] runs to cum[s + 1] ...
+        t.st[t.cum[t.sym[u]]++] = (uint8_t)u;
+    for (uint32_t s = nsym; s > 0; --s) // ... and is put back
+        t.cum[s] = t.cum[s - 1];
+    t.cum[0] = 0;
+}
+
+// The encoder's first state for symbol s, and one encoding step: from state S (the next symbol's) to a state of s,
+// writing the bits the decoder reads to get from there back to S.
+LC_HD uint32_t lc_fse_init(const LcFse& t, uint32_t s) { return t.st[t.cum[s]]; }
+LC_HD uint32_t lc_fse_enc(const LcFse& t, uint32_t S, uint32_t s, LcBitW& b) {
+    const uint32_t c = t.cum[s + 1] - t.cum[s], V = S + (1u << t.al);
+    uint32_t nb = lc_hi_bit(V) - lc_hi_bit(2 * c - 1);
+    if ((V >> nb) >= 2 * c)
+        ++nb;
+    lc_bw_put(b, V & lc_bits(nb), nb);
+    return t.st[t.cum[s] + (V >> nb) - c];
+}
+
+// The FSE table description (FSE_writeNCount) of norm[0, nsym), accuracy log al.
+LC_HD void lc_fse_ncount(const int16_t* norm, uint32_t nsym, uint32_t al, LcBitW& b) {
+    lc_bw_put(b, al - 5, 4);
+    int remaining = (1 << al) + 1, threshold = 1 << al;
+    uint32_t nbits = al + 1, s = 0;
+    bool prev0 = false;
+    while (s < nsym && remaining > 1) {
+        if (prev0) {
+            uint32_t start = s;
+            while (!norm[s])
+                ++s;
+            for (; s >= start + 24; start += 24)
+                lc_bw_put(b, 0xFFFFu, 16);
+            for (; s >= start + 3; start += 3)
+                lc_bw_put(b, 3, 2);
+            lc_bw_put(b, s - start, 2);
+        }
+        int count = norm[s++];
+        const int max = (2 * threshold - 1) - remaining;
+        remaining -= count < 0 ? -count : count;
+        ++count;
+        if (count >= threshold)
+            count += max;
+        lc_bw_put(b, (uint32_t)count, nbits - (count < max));
+        prev0 = count == 1;
+        while (remaining < threshold) {
+            --nbits;
+            threshold >>= 1;
+        }
+    }
+    lc_bw_align(b);
+}
+
+// FSE counts of the weight description: c[v] weights of value v < nv among nw, at least 2 distinct values.  Each count
+// is at most half the table, so that every decoding state reads at least one bit: the two-state weight decoder then
+// stops after exactly nw weights.
+LC_HD void lc_zstd_wnorm(const uint32_t* c, uint32_t nv, uint32_t nw, int16_t* norm) {
+    const int T = 1 << LC_ZSTD_WLOG;
+    int sum = 0;
+    for (uint32_t v = 0; v < nv; ++v) {
+        int x = (int)((uint64_t)c[v] * T / nw);
+        x = c[v] && x < 1 ? 1 : x > T / 2 ? T / 2 : x;
+        norm[v] = (int16_t)x;
+        sum += x;
+    }
+    while (sum > T) { // the largest count gives one
+        uint32_t best = nv;
+        for (uint32_t v = 0; v < nv; ++v)
+            if (norm[v] > 1 && (best == nv || norm[v] > norm[best]))
+                best = v;
+        --norm[best];
+        --sum;
+    }
+    while (sum < T) { // the most frequent value below half the table takes one
+        uint32_t best = nv;
+        for (uint32_t v = 0; v < nv; ++v)
+            if (c[v] && norm[v] < T / 2 && (best == nv || c[v] > c[best]))
+                best = v;
+        ++norm[best];
+        ++sum;
+    }
+}
+
+struct LcZstdWarp { // per-warp scratch of the block pass (shared memory on the device)
+    uint32_t hist[256];         // literal counts
+    uint32_t ncnt[512];         // Huffman node counts (leaves in `order`, then internal nodes)
+    uint16_t npar[512];         // Huffman node parents, then depths
+    uint16_t code[256];         // Huffman code of each byte
+    uint8_t len[256];           // its length (0: absent)
+    uint8_t order[256];         // the bytes present, by increasing (count, byte)
+    uint32_t st[16];            // bit staging of a Huffman stream
+    uint32_t v[32], u[32];      // per-lane values
+    uint32_t nl[16];            // codes per length, then the next code of each length
+    uint32_t res[4];            // lane 0's results for the warp
+    uint32_t wc[16];            // weight value counts
+    int16_t wn[16];             // their FSE counts
+    uint8_t wdesc[128];         // the Huffman tree description
+    LcFse ll, ml, of, wf;       // predefined sequence tables, weight table
+};
+
+// Huffman code lengths (one lane) of the m >= 2 bytes order[0, m) with counts hist[]: a Huffman tree over the leaves in
+// increasing order (a leaf before an internal node of the same count), depths over LC_ZSTD_HUF_MAX cut to it, then the
+// Kraft sum repaired: the least frequent codes shorter than the limit grow until the code fits, and the most frequent
+// codes shrink while it stays within.  Returns the longest length; the code is complete.
+LC_HD uint32_t lc_zstd_huf_lengths(LcZstdWarp& w, uint32_t m) {
+    const uint32_t M = LC_ZSTD_HUF_MAX, full = 1u << M;
+    for (uint32_t i = 0; i < m; ++i)
+        w.ncnt[i] = w.hist[w.order[i]];
+    uint32_t li = 0, ii = m;
+    for (uint32_t nn = m; nn < 2 * m - 1; ++nn) {
+        uint32_t a[2];
+        for (uint32_t k = 0; k < 2; ++k)
+            a[k] = li < m && (ii >= nn || w.ncnt[li] <= w.ncnt[ii]) ? li++ : ii++;
+        w.ncnt[nn] = w.ncnt[a[0]] + w.ncnt[a[1]];
+        w.npar[a[0]] = w.npar[a[1]] = (uint16_t)nn;
+    }
+    w.npar[2 * m - 2] = 0;
+    for (uint32_t i = 2 * m - 2; i-- > 0;)
+        w.npar[i] = (uint16_t)(w.npar[w.npar[i]] + 1);
+    uint32_t K = 0; // Kraft sum in units of 2^-M
+    for (uint32_t i = 0; i < m; ++i) {
+        const uint32_t d = w.npar[i] < M ? w.npar[i] : M;
+        w.len[w.order[i]] = (uint8_t)d;
+        K += 1u << (M - d);
+    }
+    for (uint32_t i = 0; K > full;) {
+        uint8_t& L = w.len[w.order[i]];
+        if (L >= M) {
+            ++i;
+            continue;
+        }
+        K -= 1u << (M - 1 - L);
+        ++L;
+    }
+    while (K < full)
+        for (uint32_t i = m; i-- > 0 && K < full;) {
+            uint8_t& L = w.len[w.order[i]];
+            while (L > 1 && K + (1u << (M - L)) <= full) {
+                K += 1u << (M - L);
+                --L;
+            }
+        }
+    uint32_t lmax = 0;
+    for (uint32_t i = 0; i < m; ++i)
+        lmax = w.len[w.order[i]] > lmax ? w.len[w.order[i]] : lmax;
+    return lmax;
+}
+
+// Canonical codes of the lengths (one lane): by decreasing length, then increasing byte, from code 0 (RFC 8878
+// 4.2.1.3).  Then the tree description of the weights of bytes [0, maxs) in w.wdesc (the weight of byte maxs is
+// implied); returns its size, or 0 when neither form can hold it.
+LC_HD uint32_t lc_zstd_huf_table(LcZstdWarp& w, uint32_t lmax, uint32_t maxs) {
+    for (uint32_t L = 0; L < 16; ++L)
+        w.nl[L] = 0;
+    for (uint32_t s = 0; s <= maxs; ++s)
+        ++w.nl[w.len[s]];
+    uint32_t next = 0;
+    for (uint32_t L = lmax; L >= 1; --L) { // nl[L] becomes the first code of length L
+        const uint32_t c = w.nl[L];
+        w.nl[L] = next;
+        next = (next + c) >> 1;
+    }
+    for (uint32_t s = 0; s <= maxs; ++s)
+        if (w.len[s])
+            w.code[s] = (uint16_t)w.nl[w.len[s]]++;
+    // weights: lmax + 1 - length (0 for an absent byte)
+    const uint32_t N = maxs;
+    uint32_t nv = 0, distinct = 0;
+    for (uint32_t v = 0; v < 16; ++v)
+        w.wc[v] = 0;
+    for (uint32_t s = 0; s < N; ++s) {
+        const uint32_t wt = w.len[s] ? lmax + 1 - w.len[s] : 0u;
+        distinct += !w.wc[wt]++;
+        nv = wt + 1 > nv ? wt + 1 : nv;
+    }
+    const uint32_t direct = N <= 128 ? 1 + (N + 1) / 2 : 0u;
+    uint32_t fse = 0;
+    if (distinct >= 2) {
+        lc_zstd_wnorm(w.wc, nv, N, w.wn);
+        lc_fse_build(3, w.wn, nv, LC_ZSTD_WLOG, w.wf);
+        LcBitW b{w.wdesc + 1, 0, 127, 0, 0};
+        lc_fse_ncount(w.wn, nv, LC_ZSTD_WLOG, b);
+        // two interleaved states: even weights on the first, odd on the second, encoded from the end
+        uint32_t X[2];
+        const auto wt = [&](uint32_t s) { return w.len[s] ? lmax + 1 - w.len[s] : 0u; };
+        X[(N - 1) & 1] = lc_fse_init(w.wf, wt(N - 1));
+        X[(N - 2) & 1] = lc_fse_init(w.wf, wt(N - 2));
+        for (uint32_t i = N - 2; i-- > 0;)
+            X[i & 1] = lc_fse_enc(w.wf, X[i & 1], wt(i), b);
+        lc_bw_put(b, X[1], LC_ZSTD_WLOG);
+        lc_bw_put(b, X[0], LC_ZSTD_WLOG);
+        lc_bw_close(b);
+        fse = b.n <= 127 ? 1 + b.n : 0u;
+    }
+    if (fse && (!direct || fse < direct)) {
+        w.wdesc[0] = (uint8_t)(fse - 1);
+        return fse;
+    }
+    if (!direct)
+        return 0;
+    w.wdesc[0] = (uint8_t)(127 + N);
+    for (uint32_t j = 0; 2 * j < N; ++j) {
+        const uint32_t a = w.len[2 * j] ? lmax + 1 - w.len[2 * j] : 0u;
+        const uint32_t c = 2 * j + 1 < N && w.len[2 * j + 1] ? lmax + 1 - w.len[2 * j + 1] : 0u;
+        w.wdesc[1 + j] = (uint8_t)(a << 4 | c);
+    }
+    return direct;
+}
+
+// sequence codes (RFC 8878 3.1.1.3.2.1): literal length ll, match length code of mb = ml - 3
+LC_HD uint32_t lc_zstd_llc(uint32_t ll) {
+    return ll < 16 ? ll : ll < 24 ? 16 + ((ll - 16) >> 1) : ll < 32 ? 20 + ((ll - 24) >> 2) : ll < 48 ? 22 + ((ll - 32) >> 3) : ll < 64 ? 24 : lc_hi_bit(ll) + 19;
+}
+LC_HD uint32_t lc_zstd_llbase(uint32_t c) {
+    return c < 16 ? c : c < 20 ? 16 + 2 * (c - 16) : c < 22 ? 24 + 4 * (c - 20) : c < 24 ? 32 + 8 * (c - 22) : c == 24 ? 48 : 1u << (c - 19);
+}
+LC_HD uint32_t lc_zstd_llbits(uint32_t c) { return c < 16 ? 0 : c < 20 ? 1 : c < 22 ? 2 : c < 24 ? 3 : c == 24 ? 4 : c - 19; }
+LC_HD uint32_t lc_zstd_mlc(uint32_t mb) {
+    return mb < 32 ? mb : mb < 40 ? 32 + ((mb - 32) >> 1) : mb < 48 ? 36 + ((mb - 40) >> 2) : mb < 64 ? 38 + ((mb - 48) >> 3) : mb < 96 ? 40 + ((mb - 64) >> 4) : mb < 128 ? 42 : lc_hi_bit(mb) + 36;
+}
+LC_HD uint32_t lc_zstd_mlbase(uint32_t c) {
+    return c < 32 ? c : c < 36 ? 32 + 2 * (c - 32) : c < 38 ? 40 + 4 * (c - 36) : c < 40 ? 48 + 8 * (c - 38) : c < 42 ? 64 + 16 * (c - 40) : c == 42 ? 96 : 1u << (c - 36);
+}
+LC_HD uint32_t lc_zstd_mlbits(uint32_t c) { return c < 32 ? 0 : c < 36 ? 1 : c < 38 ? 2 : c < 40 ? 3 : c < 42 ? 4 : c == 42 ? 5 : c - 36; }
+
+// One block: segment bytes s[b0, b1) (b1 - b0 <= LC_ZSTD_BLOCK), the matches of its first chunk seq[0][0, nseq[0]) and
+// of its second seq[1][0, nseq[1]) (seq[1] == nullptr: one chunk).  Each chunk's literals go to its scratch behind its
+// matches.
+struct LcZstdBlk {
+    const uint8_t* s;
+    uint32_t b0, b1;
+    LcLz4Seq* seq[2];
+    uint32_t nseq[2];
+};
+
+// match i of the block: position p, distance d, length ml
+LC_HD void lc_zstd_match(const LcZstdBlk& b, uint32_t i, uint32_t& p, uint32_t& d, uint32_t& ml) {
+    const uint32_t c = i >= b.nseq[0];
+    const LcLz4Seq q = b.seq[c][i - (c ? b.nseq[0] : 0u)];
+    p = b.b0 + c * LC_LZ4_CHUNK + (q.a & 0xFFFFu);
+    d = q.a >> 16;
+    ml = q.b;
+}
+// literal i of the block (l0 = literals of the first chunk)
+LC_HD uint8_t lc_zstd_lit(const LcZstdBlk& b, uint32_t l0, uint32_t i) {
+    return i < l0 ? reinterpret_cast<const uint8_t*>(b.seq[0] + b.nseq[0])[i]
+                  : reinterpret_cast<const uint8_t*>(b.seq[1] + b.nseq[1])[i - l0];
+}
+
+// Literals section header of a Raw / RLE (mode) or Huffman section of r literals (c = compressed size)
+LC_HD uint32_t lc_zstd_lhdr(uint32_t mode, uint32_t r, uint32_t c) {
+    if (mode != LC_ZSTD_HUF)
+        return r < 32 ? 1u : r < 4096 ? 2u : 3u;
+    return r < 1024 && c < 1024 ? 3u : r < 16384 && c < 16384 ? 4u : 5u;
+}
+LC_HD void lc_zstd_put_lhdr(uint8_t* o, uint32_t mode, uint32_t r, uint32_t c) {
+    const uint32_t h = lc_zstd_lhdr(mode, r, c);
+    uint64_t v;
+    if (mode != LC_ZSTD_HUF)
+        v = h == 1 ? mode | r << 3 : h == 2 ? mode | 1u << 2 | r << 4 : mode | 3u << 2 | r << 4;
+    else
+        v = h == 3 ? mode | 1u << 2 | r << 4 | (uint64_t)c << 14
+            : h == 4 ? mode | 2u << 2 | r << 4 | (uint64_t)c << 18
+                     : mode | 3u << 2 | r << 4 | (uint64_t)c << 22;
+    for (uint32_t j = 0; j < h; ++j)
+        o[j] = (uint8_t)(v >> (8 * j));
+}
+
+// One Huffman stream of literals [a, e) of the block at o: the literals from the last to the first, each code at the
+// bit offset its lanes find by a prefix sum, then the closing 1 bit.
+LC_HD void lc_zstd_huf_stream(const LcZstdBlk& b, uint32_t l0, uint32_t a, uint32_t e, uint8_t* o, LcZstdWarp& w,
+                              uint32_t lane, uint32_t W) {
+    uint32_t pos = 0, base = 0; // bits written; bit of w.st[0] (a multiple of 32)
+    LC_LANES(l) {
+        for (uint32_t j = l; j < 16; j += W)
+            w.st[j] = 0;
+    }
+    LC_WARP_SYNC();
+    while (e > a) {
+        const uint32_t cnt = e - a < W ? e - a : W;
+        LC_LANES(l) {
+            const uint32_t ch = l < cnt ? lc_zstd_lit(b, l0, e - 1 - l) : 0u;
+            w.u[l] = ch;
+            w.v[l] = l < cnt ? w.len[ch] : 0u;
+        }
+        LC_WARP_SYNC();
+        const uint32_t tot = lc_warp_exscan(w.v, lane, W);
+        LC_WARP_SYNC();
+        LC_LANES(l) {
+            if (l < cnt) {
+                const uint32_t P = pos - base + w.v[l], ch = w.u[l], c = w.code[ch];
+                lc_or32(&w.st[P >> 5], c << (P & 31));
+                if ((P & 31) + w.len[ch] > 32)
+                    lc_or32(&w.st[(P >> 5) + 1], c >> (32 - (P & 31)));
+            }
+        }
+        LC_WARP_SYNC();
+        pos += tot;
+        e -= cnt;
+        const uint32_t nw = (pos - base) >> 5; // complete words
+        LC_LANES(l) {
+            for (uint32_t j = l; j < 4 * nw; j += W)
+                o[(base >> 3) + j] = (uint8_t)(w.st[j >> 2] >> (8 * (j & 3)));
+        }
+        const uint32_t carry = w.st[nw];
+        LC_WARP_SYNC();
+        LC_LANES(l) {
+            for (uint32_t j = l; j < 16; j += W)
+                w.st[j] = j ? 0u : carry;
+        }
+        LC_WARP_SYNC();
+        base += nw << 5;
+    }
+    if (lane == 0)
+        w.st[(pos - base) >> 5] |= 1u << ((pos - base) & 31);
+    LC_WARP_SYNC();
+    const uint32_t nbytes = (pos + 8) >> 3;
+    LC_LANES(l) {
+        for (uint32_t j = (base >> 3) + l; j < nbytes; j += W)
+            o[j] = (uint8_t)(w.st[(j - (base >> 3)) >> 2] >> (8 * (j & 3)));
+    }
+    LC_WARP_SYNC();
+}
+
+// One lane: the sequences section of the block's ns matches at b.o[n, cap) (b.n = its start).
+LC_HD void lc_zstd_sequences(const LcZstdBlk& b, uint32_t ns, const LcZstdWarp& w, LcBitW& bw) {
+    if (ns < 128) {
+        lc_bw_put(bw, ns, 8);
+    } else if (ns < 0x7F00) {
+        lc_bw_put(bw, (ns >> 8) + 128, 8);
+        lc_bw_put(bw, ns & 0xFF, 8);
+    } else {
+        lc_bw_put(bw, 255, 8);
+        lc_bw_put(bw, ns - 0x7F00, 16);
+    }
+    if (!ns)
+        return;
+    lc_bw_put(bw, 0, 8); // Symbol_Compression_Modes: predefined LL, OF and ML
+    uint32_t sll = 0, sof = 0, sml = 0, p, d, ml;
+    lc_zstd_match(b, ns - 1, p, d, ml);
+    for (uint32_t i = ns; i-- > 0;) {
+        uint32_t pp = b.b0, pd = 0, pml = 0;
+        if (i) {
+            lc_zstd_match(b, i - 1, pp, pd, pml);
+            pp += pml;
+        }
+        const uint32_t ll = p - pp, mb = ml - 3, ov = d + 3;
+        const uint32_t llc = lc_zstd_llc(ll), mlc = lc_zstd_mlc(mb), ofc = lc_hi_bit(ov);
+        if (i + 1 == ns) {
+            sll = lc_fse_init(w.ll, llc);
+            sof = lc_fse_init(w.of, ofc);
+            sml = lc_fse_init(w.ml, mlc);
+        } else {
+            sof = lc_fse_enc(w.of, sof, ofc, bw);
+            sml = lc_fse_enc(w.ml, sml, mlc, bw);
+            sll = lc_fse_enc(w.ll, sll, llc, bw);
+        }
+        lc_bw_put(bw, ll - lc_zstd_llbase(llc), lc_zstd_llbits(llc));
+        lc_bw_put(bw, mb - lc_zstd_mlbase(mlc), lc_zstd_mlbits(mlc));
+        lc_bw_put(bw, ov - (1u << ofc), ofc);
+        if (i) {
+            p = pp - pml;
+            d = pd;
+            ml = pml;
+        }
+    }
+    lc_bw_put(bw, sml, 6);
+    lc_bw_put(bw, sof, 5);
+    lc_bw_put(bw, sll, 6);
+    lc_bw_close(bw);
+}
+
+// Block pass: the compressed body of block b at o[0, b.b1 - b.b0) when it is smaller than the block's bytes; returns
+// its size, or 0 for a Raw block (o then holds scratch).
+LC_HD uint32_t lc_zstd_block(const LcZstdBlk& b, uint8_t* o, LcZstdWarp& w, uint32_t lane, uint32_t W) {
+    const uint32_t raw = b.b1 - b.b0;
+    if (raw == 0)
+        return 0;
+    if (lane == 0) {
+        lc_fse_build(0, nullptr, 36, 6, w.ll);
+        lc_fse_build(1, nullptr, 53, 6, w.ml);
+        lc_fse_build(2, nullptr, 29, 5, w.of);
+    }
+    LC_LANES(l) {
+        for (uint32_t i = l; i < 256; i += W)
+            w.hist[i] = 0;
+    }
+    LC_WARP_SYNC();
+    // 1. each chunk's literals behind its matches, W positions at a time, and their histogram
+    uint32_t nlit[2] = {0, 0};
+    for (uint32_t c = 0; c < 2 && b.seq[c]; ++c) {
+        const uint32_t c0 = b.b0 + c * LC_LZ4_CHUNK, c1 = b.b1 - c0 < LC_LZ4_CHUNK ? b.b1 : c0 + LC_LZ4_CHUNK;
+        const LcLz4Seq* q = b.seq[c];
+        uint8_t* lit = reinterpret_cast<uint8_t*>(b.seq[c] + b.nseq[c]);
+        uint32_t m = 0, k = 0; // matches that end before x, literals before x
+        for (uint32_t x = c0; x < c1; x += W) {
+            const uint32_t x1 = c1 - x < W ? c1 : x + W;
+            LC_LANES(l) { // lane l: the coverage of [x, x1) by match m + l, and whether it ends there
+                uint32_t cov = 0, end = 0;
+                if (m + l < b.nseq[c]) {
+                    const LcLz4Seq z = q[m + l];
+                    const uint32_t ms = c0 + (z.a & 0xFFFFu), me = ms + z.b;
+                    const uint32_t lo = ms > x ? ms : x, hi = me < x1 ? me : x1;
+                    cov = lo < hi ? lc_bits(hi - lo) << (lo - x) : 0u;
+                    end = me <= x1;
+                }
+                w.v[l] = cov;
+                w.u[l] = end;
+            }
+            LC_WARP_SYNC();
+            const uint32_t litm = ~lc_warp_or(w.v, lane, W) & lc_bits(x1 - x);
+            const uint32_t ends = lc_lz4_ballot(w.u, lane, W);
+            LC_WARP_SYNC();
+            LC_LANES(l) {
+                if ((litm >> l) & 1) {
+                    const uint8_t ch = b.s[x + l];
+                    lit[k + lc_popc(litm & lc_bits(l))] = ch;
+                    lc_add32(&w.hist[ch], 1);
+                }
+            }
+            k += lc_popc(litm);
+            m += lc_popc(ends);
+        }
+        nlit[c] = k;
+    }
+    LC_WARP_SYNC();
+    const uint32_t l0 = nlit[0], R = nlit[0] + nlit[1];
+    // 2. the bytes present by increasing (count, byte), for the Huffman tree
+    if (R >= LC_ZSTD_MIN_HUF) {
+        LC_LANES(l) {
+            for (uint32_t s = l; s < 256; s += W) {
+                const uint32_t cs = w.hist[s];
+                if (!cs)
+                    continue;
+                uint32_t r = 0;
+                for (uint32_t t = 0; t < 256; ++t)
+                    r += w.hist[t] && (w.hist[t] < cs || (w.hist[t] == cs && t < s));
+                w.order[r] = (uint8_t)s;
+            }
+        }
+        LC_WARP_SYNC();
+    }
+    // 3. one lane: the literal mode, the code and its description
+    if (lane == 0) {
+        uint32_t m = 0, maxs = 0;
+        for (uint32_t s = 0; s < 256; ++s) {
+            w.len[s] = 0;
+            if (w.hist[s]) {
+                ++m;
+                maxs = s;
+            }
+        }
+        uint32_t mode = m == 1 ? LC_ZSTD_RLE : LC_ZSTD_RAW, dl = 0;
+        if (m >= 2 && R >= LC_ZSTD_MIN_HUF) {
+            dl = lc_zstd_huf_table(w, lc_zstd_huf_lengths(w, m), maxs);
+            mode = dl ? LC_ZSTD_HUF : mode;
+        }
+        w.res[0] = mode;
+        w.res[1] = dl;
+        w.res[2] = maxs;
+    }
+    LC_WARP_SYNC();
+    uint32_t mode = w.res[0];
+    const uint32_t dl = w.res[1], q4 = (R + 3) / 4;
+    uint32_t sbytes[4] = {0, 0, 0, 0}, csize = 0;
+    if (mode == LC_ZSTD_HUF) {
+        csize = dl + 6;
+        for (uint32_t k = 0; k < 4; ++k) {
+            const uint32_t a = k * q4, e = k == 3 ? R : a + q4;
+            LC_LANES(l) {
+                uint32_t bits = 0;
+                for (uint32_t i = a + l; i < e; i += W)
+                    bits += w.len[lc_zstd_lit(b, l0, i)];
+                w.v[l] = bits;
+            }
+            LC_WARP_SYNC();
+            sbytes[k] = lc_warp_exscan(w.v, lane, W) / 8 + 1;
+            LC_WARP_SYNC();
+            csize += sbytes[k];
+        }
+        if (lc_zstd_lhdr(mode, R, csize) + csize >= lc_zstd_lhdr(LC_ZSTD_RAW, R, 0) + R)
+            mode = LC_ZSTD_RAW;
+    }
+    const uint32_t lh = lc_zstd_lhdr(mode, R, csize);
+    const uint32_t lsize = lh + (mode == LC_ZSTD_HUF ? csize : mode == LC_ZSTD_RLE ? 1 : R);
+    if (lsize + 1 >= raw) // the sequences section takes at least one byte
+        return 0;
+    // 4. the literals section
+    if (lane == 0) {
+        lc_zstd_put_lhdr(o, mode, R, csize);
+        if (mode == LC_ZSTD_RLE)
+            o[lh] = (uint8_t)w.res[2];
+        if (mode == LC_ZSTD_HUF)
+            for (uint32_t k = 0; k < 3; ++k) {
+                o[lh + dl + 2 * k] = (uint8_t)sbytes[k];
+                o[lh + dl + 2 * k + 1] = (uint8_t)(sbytes[k] >> 8);
+            }
+    }
+    if (mode == LC_ZSTD_RAW) {
+        LC_LANES(l) {
+            for (uint32_t i = l; i < R; i += W)
+                o[lh + i] = lc_zstd_lit(b, l0, i);
+        }
+    } else if (mode == LC_ZSTD_HUF) {
+        LC_LANES(l) {
+            for (uint32_t j = l; j < dl; j += W)
+                o[lh + j] = w.wdesc[j];
+        }
+        uint8_t* so = o + lh + dl + 6;
+        for (uint32_t k = 0; k < 4; ++k) {
+            lc_zstd_huf_stream(b, l0, k * q4, k == 3 ? R : (k + 1) * q4, so, w, lane, W);
+            so += sbytes[k];
+        }
+    }
+    LC_WARP_SYNC();
+    // 5. one lane: the sequences section, abandoned when the body reaches the block's size
+    if (lane == 0) {
+        LcBitW bw{o, lsize, raw - 1, 0, 0};
+        lc_zstd_sequences(b, b.nseq[0] + b.nseq[1], w, bw);
+        w.res[3] = bw.n <= bw.cap ? bw.n : 0u;
+    }
+    LC_WARP_SYNC();
+    return w.res[3];
+}
+
+// frame header of an n-byte segment at o[0, lc_zstd_hdr(n))
+LC_HD void lc_zstd_put_hdr(uint32_t n, uint8_t* o) {
+    const uint32_t f = lc_zstd_fcs_bytes(n), v = f == 2 ? n - 256 : n;
+    o[0] = 0x28;
+    o[1] = 0xB5;
+    o[2] = 0x2F;
+    o[3] = 0xFD;
+    o[4] = (uint8_t)((f == 1 ? 0u : f == 2 ? 1u : 2u) << 6 | 0x20);
+    for (uint32_t j = 0; j < f; ++j)
+        o[5 + j] = (uint8_t)(v >> (8 * j));
+}
+
+// bytes of block j of an n-byte segment in its frame (the frame header with block 0), body = lc_zstd_block's result
+LC_HD uint32_t lc_zstd_emit_size(uint32_t n, uint32_t j, uint32_t body) {
+    const uint32_t b0 = j * LC_ZSTD_BLOCK, b1 = n - b0 < LC_ZSTD_BLOCK ? n : b0 + LC_ZSTD_BLOCK;
+    return (j ? 0u : lc_zstd_hdr(n)) + 3 + (body ? body : b1 - b0);
+}
+
+// Emit pass of block j of the segment s[0, n) at o: (block 0) the frame header, the block header, then the body from
+// the block's slot or (Raw) the segment.
+LC_HD void lc_zstd_emit_block(const uint8_t* s, uint32_t n, uint32_t j, const uint8_t* slot, uint32_t body, uint8_t* o,
+                              uint32_t lane, uint32_t W) {
+    const uint32_t b0 = j * LC_ZSTD_BLOCK, b1 = n - b0 < LC_ZSTD_BLOCK ? n : b0 + LC_ZSTD_BLOCK;
+    if (!j) {
+        if (lane == 0)
+            lc_zstd_put_hdr(n, o);
+        o += lc_zstd_hdr(n);
+    }
+    const uint32_t size = body ? body : b1 - b0, h = (b1 == n) | (body ? 2u : 0u) << 1 | size << 3;
+    if (lane == 0) {
+        o[0] = (uint8_t)h;
+        o[1] = (uint8_t)(h >> 8);
+        o[2] = (uint8_t)(h >> 16);
+    }
+    const uint8_t* src = body ? slot : s + b0;
+    LC_LANES(l) {
+        for (uint32_t i = l; i < size; i += W)
+            o[3 + i] = src[i];
+    }
+}

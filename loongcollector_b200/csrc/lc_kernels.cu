@@ -4191,4 +4191,90 @@ void launch_lz4_emit(const Lz4Segs& g, const LcLz4Seq* d_seq, const LcLz4Chunk* 
         g.in, g.seg_off, g.seg_len, g.first, g.nseg, g.nchunks, d_seq, d_info, d_anchor, d_choff, d_out);
 }
 
+// ---- f4, zstd: one frame per segment (lc_exec.cuh: lc_zstd_block, lc_zstd_emit_block) over the matches of the LZ4
+// parse pass.  The block pass runs one warp per 128 KiB block, the emit pass one warp per block.
+constexpr int kZstdWarps = 4; // warps per block of the zstd block and emit kernels
+
+__global__ void __launch_bounds__(256)
+    zstd_nblocks_kernel(const uint32_t* __restrict__ seg_len, uint64_t nseg, uint32_t* __restrict__ nblk) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < nseg)
+        nblk[g] = lc_zstd_nblocks(seg_len[g]);
+}
+
+__global__ void __launch_bounds__(32 * kZstdWarps)
+    zstd_block_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ seg_off,
+                      const uint32_t* __restrict__ seg_len, const uint64_t* __restrict__ first,
+                      const uint64_t* __restrict__ bfirst, uint64_t nseg, uint64_t nblocks, LcLz4Seq* seq,
+                      const LcLz4Chunk* __restrict__ info, uint8_t* __restrict__ slot, uint32_t* __restrict__ body,
+                      uint32_t* __restrict__ esz) {
+    __shared__ LcZstdWarp s_w[kZstdWarps];
+    const uint32_t wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint64_t k = (uint64_t)blockIdx.x * kZstdWarps + wid;
+    if (k >= nblocks)
+        return;
+    const uint64_t g = lc_span_sls_find(bfirst, nseg, k);
+    const uint32_t n = seg_len[g], j = (uint32_t)(k - bfirst[g]), b0 = j * LC_ZSTD_BLOCK;
+    const uint64_t c = first[g] + 2 * j;
+    LcZstdBlk b{in + seg_off[g], b0, n - b0 < LC_ZSTD_BLOCK ? n : b0 + LC_ZSTD_BLOCK, {seq + c * LC_LZ4_SEQ_CAP, nullptr},
+                {info[c].nseq, 0}};
+    if (b.b1 - b.b0 > LC_LZ4_CHUNK) {
+        b.seq[1] = seq + (c + 1) * LC_LZ4_SEQ_CAP;
+        b.nseq[1] = info[c + 1].nseq;
+    }
+    const uint32_t z = lc_zstd_block(b, slot + k * LC_ZSTD_BLOCK, s_w[wid], lane, 32);
+    if (lane == 0) {
+        body[k] = z;
+        esz[k] = lc_zstd_emit_size(n, j, z);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    zstd_frames_kernel(const uint64_t* __restrict__ bfirst, const uint64_t* __restrict__ boff,
+                       const uint64_t* __restrict__ total, uint64_t nseg, uint64_t* __restrict__ frm_off,
+                       uint32_t* __restrict__ frm_len) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= nseg)
+        return;
+    const uint64_t a = boff[bfirst[g]], e = g + 1 < nseg ? boff[bfirst[g + 1]] : *total;
+    frm_off[g] = a;
+    frm_len[g] = (uint32_t)(e - a);
+}
+
+__global__ void __launch_bounds__(32 * kZstdWarps)
+    zstd_emit_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ seg_off,
+                     const uint32_t* __restrict__ seg_len, const uint64_t* __restrict__ bfirst, uint64_t nseg,
+                     uint64_t nblocks, const uint8_t* __restrict__ slot, const uint32_t* __restrict__ body,
+                     const uint64_t* __restrict__ boff, uint8_t* __restrict__ out) {
+    const uint64_t k = (uint64_t)blockIdx.x * kZstdWarps + (threadIdx.x >> 5);
+    if (k >= nblocks)
+        return;
+    const uint64_t g = lc_span_sls_find(bfirst, nseg, k);
+    lc_zstd_emit_block(in + seg_off[g], seg_len[g], (uint32_t)(k - bfirst[g]), slot + k * LC_ZSTD_BLOCK, body[k],
+                       out + boff[k], threadIdx.x & 31, 32);
+}
+
+void launch_zstd_nblocks(const uint32_t* d_seg_len, uint64_t nseg, uint32_t* d_nblk, cudaStream_t st) {
+    if (nseg)
+        zstd_nblocks_kernel<<<(unsigned)((nseg + 255) / 256), 256, 0, st>>>(d_seg_len, nseg, d_nblk);
+}
+
+void launch_zstd_blocks(const Lz4Segs& g, const uint64_t* d_bfirst, uint64_t nblocks, LcLz4Seq* d_seq,
+                        const LcLz4Chunk* d_info, uint8_t* d_slot, uint32_t* d_body, uint32_t* d_esz, cudaStream_t st) {
+    if (nblocks)
+        zstd_block_kernel<<<(unsigned)((nblocks + kZstdWarps - 1) / kZstdWarps), 32 * kZstdWarps, 0, st>>>(
+            g.in, g.seg_off, g.seg_len, g.first, d_bfirst, g.nseg, nblocks, d_seq, d_info, d_slot, d_body, d_esz);
+}
+
+void launch_zstd_emit(const Lz4Segs& g, const uint64_t* d_bfirst, uint64_t nblocks, const uint8_t* d_slot,
+                      const uint32_t* d_body, const uint64_t* d_boff, const uint64_t* d_total, uint8_t* d_out,
+                      uint64_t* d_frm_off, uint32_t* d_frm_len, cudaStream_t st) {
+    if (!g.nseg)
+        return;
+    zstd_frames_kernel<<<(unsigned)((g.nseg + 255) / 256), 256, 0, st>>>(d_bfirst, d_boff, d_total, g.nseg, d_frm_off,
+                                                                          d_frm_len);
+    zstd_emit_kernel<<<(unsigned)((nblocks + kZstdWarps - 1) / kZstdWarps), 32 * kZstdWarps, 0, st>>>(
+        g.in, g.seg_off, g.seg_len, d_bfirst, g.nseg, nblocks, d_slot, d_body, d_boff, d_out);
+}
+
 } // namespace lck

@@ -329,4 +329,17 @@ void launch_lz4_emit(const Lz4Segs& g, const LcLz4Seq* d_seq, const LcLz4Chunk* 
                      const uint64_t* d_choff, const uint64_t* d_total, uint8_t* d_out, uint64_t* d_blk_off,
                      uint32_t* d_blk_len, cudaStream_t st);
 
+// f4, zstd: one zstd frame per segment (lc_exec.cuh), over the matches launch_lz4_parse left in d_seq (every chunk of
+// the segments in g).  Block k of LC_ZSTD_BLOCK bytes belongs to the segment g with bfirst[g] <= k < bfirst[g + 1]
+// (bfirst = exclusive sum of lc_zstd_nblocks per segment, which launch_zstd_nblocks writes).
+// launch_zstd_blocks: the compressed body of each block in its slot (d_slot + k * LC_ZSTD_BLOCK), d_body[k] = its size
+// or 0 (Raw), d_esz[k] = the block's bytes in its frame; its literals go to the scratch behind each chunk's matches.
+// After an exclusive sum of d_esz (d_boff, *d_total), launch_zstd_emit writes the frames and the per-segment table.
+void launch_zstd_nblocks(const uint32_t* d_seg_len, uint64_t nseg, uint32_t* d_nblk, cudaStream_t st);
+void launch_zstd_blocks(const Lz4Segs& g, const uint64_t* d_bfirst, uint64_t nblocks, LcLz4Seq* d_seq,
+                        const LcLz4Chunk* d_info, uint8_t* d_slot, uint32_t* d_body, uint32_t* d_esz, cudaStream_t st);
+void launch_zstd_emit(const Lz4Segs& g, const uint64_t* d_bfirst, uint64_t nblocks, const uint8_t* d_slot,
+                      const uint32_t* d_body, const uint64_t* d_boff, const uint64_t* d_total, uint8_t* d_out,
+                      uint64_t* d_frm_off, uint32_t* d_frm_len, cudaStream_t st);
+
 } // namespace lck

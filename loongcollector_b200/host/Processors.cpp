@@ -2871,6 +2871,47 @@ bool LZ4Compressor::Compress(const std::vector<std::string>& inputs, std::vector
     return true;
 }
 
+bool ZstdCompressor::Compress(const std::string& input, std::string& output, std::string& errorMsg) {
+    std::vector<std::string> out;
+    if (!Compress(std::vector<std::string>{input}, out, errorMsg))
+        return false;
+    output.swap(out[0]);
+    return true;
+}
+
+bool ZstdCompressor::Compress(const std::vector<std::string>& inputs, std::vector<std::string>& outputs,
+                              std::string& errorMsg) {
+    (void)mCompressionLevel;
+    std::vector<const uint8_t*> ptr;
+    std::vector<uint32_t> len;
+    uint64_t cap = 0;
+    for (const std::string& in : inputs) {
+        // the device parse pass takes at most LZ4_MAX_INPUT_SIZE bytes per input; ZSTD_compress's message for an
+        // input it cannot take
+        if (in.size() > LC_LZ4_MAX_INPUT) {
+            errorMsg = "Src size is incorrect";
+            return false;
+        }
+        ptr.push_back(reinterpret_cast<const uint8_t*>(in.data()));
+        len.push_back((uint32_t)in.size());
+        cap += lc_zstd_bound(in.size());
+    }
+    outputs.clear();
+    if (inputs.empty())
+        return true;
+    std::string all(cap, '\0');
+    std::vector<uint64_t> foff(inputs.size());
+    std::vector<uint32_t> flen(inputs.size());
+    uint64_t total = 0;
+    Check(lc_zstd_compress(Engine(), inputs.size(), ptr.data(), len.data(), reinterpret_cast<uint8_t*>(&all[0]), cap,
+                           foff.data(), flen.data(), &total),
+          "lc_zstd_compress");
+    outputs.reserve(inputs.size());
+    for (size_t k = 0; k < inputs.size(); ++k)
+        outputs.emplace_back(all, foff[k], flen[k]);
+    return true;
+}
+
 Processor* CreateProcessor(const std::string& type) {
     if (type == ProcessorMergeMultilineLogNative::sName)
         return new ProcessorMergeMultilineLogNative;

@@ -441,6 +441,26 @@ public:
     bool Compress(const std::vector<std::string>& inputs, std::vector<std::string>& outputs, std::string& errorMsg);
 };
 
+// core/common/compression/CompressType.h
+enum class CompressType { NONE, LZ4, ZSTD };
+
+// FlusherSLS's other compressor, CompressType "zstd" (core/common/compression/ZstdCompressor.cpp: ZSTD_compress at
+// the configured level) on the GPU: one zstd frame per input (lc_zstd_compress).  The frames are valid zstd frames of
+// the input, not libzstd's exact bytes.  The level is accepted for the reference's constructor and does not change the
+// bytes: there is one device encoder, whose ratio lies between libzstd's levels -1 and 1 (DESIGN.md §5).  As for
+// LZ4Compressor, the batched overload compresses many serialised groups in one device call.
+class ZstdCompressor {
+public:
+    explicit ZstdCompressor(CompressType type, int32_t level = 1) : mType(type), mCompressionLevel(level) {}
+    bool Compress(const std::string& input, std::string& output, std::string& errorMsg);
+    bool Compress(const std::vector<std::string>& inputs, std::vector<std::string>& outputs, std::string& errorMsg);
+    CompressType GetCompressType() const { return mType; }
+
+private:
+    CompressType mType;
+    int32_t mCompressionLevel;
+};
+
 // Factory by plugin type name (the names the reference registers, PluginRegistry.cpp:183-200).
 Processor* CreateProcessor(const std::string& type);
 

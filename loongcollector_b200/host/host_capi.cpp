@@ -399,6 +399,40 @@ char* lc_host_lz4_compress(const char* const* data, const unsigned long long* le
     }
 }
 
+char* lc_host_zstd_compress(const char* const* data, const unsigned long long* len, unsigned long long n,
+                            unsigned long long* len_out, unsigned long long* frm_len, char** err_out) {
+    if (err_out)
+        *err_out = nullptr;
+    if (len_out)
+        *len_out = 0;
+    try {
+        std::vector<std::string> in, out;
+        for (unsigned long long k = 0; k < n; ++k)
+            in.emplace_back(data[k], len[k]);
+        std::string err;
+        ZstdCompressor c(CompressType::ZSTD);
+        if (!c.Compress(in, out, err)) {
+            if (err_out)
+                *err_out = dup(err);
+            return nullptr;
+        }
+        std::string all;
+        for (unsigned long long k = 0; k < n; ++k) {
+            frm_len[k] = out[k].size();
+            all += out[k];
+        }
+        char* res = (char*)malloc(all.size() + 1);
+        memcpy(res, all.data(), all.size());
+        if (len_out)
+            *len_out = all.size();
+        return res;
+    } catch (const std::exception& e) {
+        if (err_out)
+            *err_out = dup(std::string("ZstdCompressor::Compress threw: ") + e.what());
+        return nullptr;
+    }
+}
+
 // What PluginRegistry::LoadProcessorPlugin + DynamicCProcessorProxy do with a dynamic plugin
 // (PluginRegistry.cpp:218-275, DynamicCProcessorProxy.cpp:21-36), step by step, on the plugin at so_path.
 char* lc_host_dynamic_plugin_roundtrip(const char* so_path, const char* config_json, const char* group_json,
