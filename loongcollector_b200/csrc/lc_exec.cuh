@@ -314,18 +314,23 @@ LC_HD LcTdfaView lc_tdfa_view(const void* blob) {
     return v;
 }
 
-// does the 16-byte chunk w[0..3] hold one of the exit bytes of skip word sk (LC_TDFA_SKIP set)?
+// does the 16-byte chunk w[0..3] hold one of the exit bytes of skip word sk (LC_TDFA_SKIP set)?  Branch-free: both
+// exit slots are always tested (a one-exit state repeats its byte in the second, lc_tables.h), a zero-exit state is
+// masked at the end.
 LC_HD bool lc_tdfa_chunk_has_exit(uint32_t sk, const uint32_t w[4]) {
-    const uint32_t n = (sk >> 16) & 3u;
+#ifdef __CUDA_ARCH__
+    const uint32_t e0 = __byte_perm(sk, 0, 0x0000), e1 = __byte_perm(sk, 0, 0x1111);
+#else
+    const uint32_t e0 = (sk & 0xFFu) * 0x01010101u, e1 = ((sk >> 8) & 0xFFu) * 0x01010101u;
+#endif
     uint32_t hit = 0;
-    for (uint32_t k = 0; k < n; ++k) {
-        const uint32_t splat = ((sk >> (8 * k)) & 0xFFu) * 0x01010101u;
-        for (int j = 0; j < 4; ++j) {
-            const uint32_t x = w[j] ^ splat;
-            hit |= (x - 0x01010101u) & ~x & 0x80808080u; // some byte of x is zero
-        }
+    for (int j = 0; j < 4; ++j) {
+        const uint32_t x0 = w[j] ^ e0, x1 = w[j] ^ e1;
+        hit = ((x0 - 0x01010101u) & ~x0) | hit;
+        hit = ((x1 - 0x01010101u) & ~x1) | hit;
     }
-    return hit != 0;
+    // (x - 0x01010101) & ~x & 0x80808080 is nonzero iff some byte of x is zero
+    return (hit & 0x80808080u) != 0 && (sk & 0x30000u) != 0;
 }
 
 // RegT = uint16_t (events shorter than 65535 bytes: the shared-memory register files of the kernels) or uint32_t

@@ -1553,13 +1553,22 @@ int launch_regex_fast2(const void* d_blob, uint32_t blob_bytes, bool multi, bool
 // Why: with one line per lane, a per-lane 16-byte LDG touches 32 different 128-byte lines, i.e. 32 L1 tag
 // wavefronts for 512 bytes -- measured to cost more than the automaton's own look-ups.  Here the warp fetches its
 // 32 lines COOPERATIVELY: one cp.async (LDGSTS) instruction moves 4 full 128-byte lines (8 lanes x 16 B each, 4
-// wavefronts) straight into a per-warp staging tile laid out [chunk][(line + chunk) mod 32] in 16-byte units; the
-// rotation makes both the 16-byte async writes and the later per-lane LDS.128 reads bank-conflict free.  Lanes
-// then consume their own line from the tile.  All hot-loop accesses use 32-bit shared-window addresses: the class
+// wavefronts) straight into a per-warp staging tile (tile_slot): line j of the warp owns the 128-byte row j, so every
+// global line of an LDGSTS lands in one shared-memory row, and its 8 chunks are permuted by j inside the row, so that
+// the per-lane LDS.128 reads of one chunk column stay bank-conflict free.  Lanes then consume their own line from
+// the tile.  All hot-loop accesses use 32-bit shared-window addresses: the class
 // table sits on a 256-byte boundary (address = PRMT(byte, base)), and the pair table's row offsets are rebased to
 // absolute addresses while the automaton is staged, so a pair step is
 //   PRMT PRMT LDS.U8 LDS.U8 IMAD LEA LDS LOP  + two predicated STS.U16 for capture boundaries.
 #define LCT_STAGE_CHUNKS 8u /* 16-byte chunks per line per stage: 128 B = one L1 line per 8-lane group */
+
+// The one place that knows the staging tile's layout: shared address of chunk q of line j (only q mod 8 counts) in
+// the 4 KB tile at `tile` (128-byte aligned).  Row j holds line j, chunk q in 16-byte unit (q ^ j) mod 8: the 8 lanes
+// that copy one global line write one row, and the 8 lanes 8g..8g+7 that read one chunk column hit 8 distinct bank
+// quads.  Since only j mod 8 enters the permutation, tile_slot(tile + 1024 * g, r, q) == tile_slot(tile, 8 * g + r, q).
+__device__ __forceinline__ uint32_t tile_slot(uint32_t tile, uint32_t j, uint32_t q) {
+    return tile + (j << 7) + (((q ^ j) & 7u) << 4);
+}
 
 __device__ __forceinline__ uint32_t lds_u8(uint32_t a) {
     uint32_t v;
@@ -1597,8 +1606,12 @@ __device__ __forceinline__ void sts_u16(uint32_t a, uint32_t v) {
 __device__ __forceinline__ void sts_u64(uint32_t a, uint32_t x, uint32_t y) {
     asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(a), "r"(x), "r"(y) : "memory");
 }
-__device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+// 16-byte cp.async if i < n.  The predicate lives inside the asm, so that the compiler forms the addresses once for
+// all copies of a stage instead of sinking their arithmetic into one branch per copy.
+__device__ __forceinline__ void cp_async_16_if_lt(uint32_t dst, const void* src, uint32_t i, uint32_t n) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.lt.u32 p, %2, %3;\n\t@p cp.async.cg.shared.global [%0], [%1], 16;\n\t}"
+                 ::"r"(dst), "l"(src), "r"(i), "r"(n)
+                 : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() {
     asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
@@ -1686,8 +1699,10 @@ __device__ __noinline__ uint32_t tdfa_partial_chunk(const LcTdfaView v, const Td
 }
 
 // (Tile fill alternatives measured on C2 and dropped as slower: cp.async.ca instead of .cg; LDG.128 into registers
-// followed by STS.128 -- 8x fewer shared-memory wavefronts than LDGSTS, which writes one 16-byte wavefront per lane --
-// but the loads stall the issuing warp and the extra live registers spill under the 64-register cap.)
+// followed by STS.128 -- the loads stall the issuing warp and the extra live registers spill under the 64-register
+// cap.  The shared-memory side of LDGSTS is cheap only when the 8 lanes of one global line write one 128-byte row:
+// with the earlier [chunk][line ^ chunk] tile, where every lane of an LDGSTS wrote a row of its own, the fill alone
+// (tools/tile_fill_probe.py, C2's 4 Mi x 256 B lines in HBM) took 1.39-1.59x as long as with tile_slot's layout.)
 //
 // The warp's 32 lines (one per lane; line = frame of `len` bytes starting `mis` bytes into its first 16-byte chunk,
 // chunk list published in the warp's info slots as {first chunk index, chunk count}) walk through automaton `t`
@@ -1695,20 +1710,32 @@ __device__ __noinline__ uint32_t tdfa_partial_chunk(const LcTdfaView v, const Td
 // Lanes whose `row` is `dead` on entry (or becomes dead) only help fetching.  Returns the final row.
 struct TdfaLoader {
     const uint4* gbase16; // 16-byte aligned base of the arena
-    uint32_t ld_q;        // loader role: chunk column of lines ld_L0 + r (r = 0..7)
+    uint32_t ld_q;        // loader role: chunk column of lines ld_L0 + r (r = 0..7), ld_L0 = (lane >> 3) * 8
     uint32_t ld_info;     // info slots of those lines
-    uint32_t ld_dst;      // tile slot of (chunk ld_q, line ld_L0)
-    uint32_t tile_abs;    // this warp's 4 KB tile
-    uint32_t rd_lane16;   // lane << 4
-    // cooperative fetch of chunks s0..s0+7 of the warp's 32 lines: instruction r moves lines r, r+8, r+16, r+24
+    uint32_t ld_rows;     // tile + ld_L0 * 128: tile_slot(ld_rows, r, q) is the slot of chunk q of line ld_L0 + r
+    uint32_t tile_abs;    // this warp's 4 KB tile (128-byte aligned)
+    uint32_t lane;
+    __device__ __forceinline__ void init(const uint8_t* base, uint32_t info_abs, uint32_t tile, uint32_t ln) {
+        gbase16 = reinterpret_cast<const uint4*>((uintptr_t)base & ~(uintptr_t)15);
+        ld_q = ln & 7;
+        ld_info = info_abs + (ln >> 3) * 64;
+        ld_rows = tile + (ln >> 3) * 1024;
+        tile_abs = tile;
+        lane = ln;
+    }
+    // shared address of chunk k of this lane's own line
+    __device__ __forceinline__ uint32_t own(uint32_t k) const { return tile_slot(tile_abs, lane, k); }
+    // cooperative fetch of chunks s0..s0+7 of the warp's 32 lines: instruction r moves lines r, r+8, r+16, r+24.
+    // The 8 info loads go first, so that the copies do not wait on them one by one.
     __device__ __forceinline__ void stage(uint32_t s0) {
         const uint32_t cidx = s0 + ld_q;
+        uint2 inf[8];
 #pragma unroll
-        for (uint32_t r = 0; r < 8; ++r) {
-            const uint2 inf = lds_u64_v(ld_info + r * 8);
-            if (cidx < inf.y)
-                cp_async_16(ld_dst + ((r ^ ld_q) << 4), gbase16 + inf.x + cidx);
-        }
+        for (uint32_t r = 0; r < 8; ++r)
+            inf[r] = lds_u64_v(ld_info + r * 8);
+#pragma unroll
+        for (uint32_t r = 0; r < 8; ++r) // (chunk indices of the arena fit 32 bits: g0 is one)
+            cp_async_16_if_lt(tile_slot(ld_rows, r, ld_q), gbase16 + (inf[r].x + cidx), cidx, inf[r].y);
         cp_async_wait_all();
         __syncwarp();
     }
@@ -1724,18 +1751,16 @@ __device__ __forceinline__ uint32_t tdfa_walk_lines(const LcTdfaView& v, const T
     const uint32_t k_tail = len ? (Q - 1) >> 4 : 0;
     const bool has_head = len && !(kf_lo == 0 && kf_hi > 0);        // chunk 0 is not fully paired
     const bool has_tail = len && k_tail >= kf_hi && !(has_head && k_tail == 0);
-    const uint32_t tile_abs = L.tile_abs, rd_lane16 = L.rd_lane16;
     for (uint32_t s0 = 0; s0 < max_nch; s0 += LCT_STAGE_CHUNKS) {
         L.stage(s0); // chunks s0..s0+7 of the warp's 32 lines are in the tile when this returns
         // ---- every lane walks its own line through the tile
         if (row != dead) {
             if (has_head && s0 == 0)
-                row = tdfa_partial_chunk(v, t, row, tile_abs + rd_lane16, 0, mis, len, regs_m2, rg, sink);
+                row = tdfa_partial_chunk(v, t, row, L.own(0), 0, mis, len, regs_m2, rg, sink);
             const uint32_t ka = kf_lo > s0 ? kf_lo : s0;
             const uint32_t kb = kf_hi < s0 + LCT_STAGE_CHUNKS ? kf_hi : s0 + LCT_STAGE_CHUNKS;
             for (uint32_t k = ka; k < kb; ++k) {
-                const uint32_t q = k & 7;
-                const uint4 vv = lds_u128_v(tile_abs + (q << 9) + (rd_lane16 ^ (q << 4)));
+                const uint4 vv = lds_u128_v(L.own(k));
                 {
                     // run skipping: inside [^"]* / .* / after the line has died the state maps every byte but (at
                     // most) two back to itself without touching a register -- a chunk without those bytes is a no-op
@@ -1761,11 +1786,8 @@ __device__ __forceinline__ uint32_t tdfa_walk_lines(const LcTdfaView& v, const T
                 if (SLOW && row == sink) // some step set several registers: redo this chunk step by step
                     row = t.t2 + t.row_bytes * tdfa_chunk_slow(v, __umulhi(row_in - t.t2, t.inv_row), vv, pos0, rg);
             }
-            if (has_tail && k_tail - s0 < LCT_STAGE_CHUNKS) {
-                const uint32_t q = k_tail & 7;
-                row = tdfa_partial_chunk(v, t, row, tile_abs + (q << 9) + (rd_lane16 ^ (q << 4)), k_tail * 16, mis,
-                                         len, regs_m2, rg, sink);
-            }
+            if (has_tail && k_tail - s0 < LCT_STAGE_CHUNKS)
+                row = tdfa_partial_chunk(v, t, row, L.own(k_tail), k_tail * 16, mis, len, regs_m2, rg, sink);
         }
         __syncwarp();
     }
@@ -1807,8 +1829,8 @@ __global__ void __launch_bounds__(1024, 1)
                              uint32_t reg_pitch /* halfwords */, unsigned long long* next_batch, uint32_t* overflow,
                              const uint32_t* __restrict__ order, const uint32_t* __restrict__ order_flag) {
     extern __shared__ uint4 smem[];
-    // carve-out: [pad][class table, 256 B @ 256-aligned][blob][16 B][register files][line info: warps x 32 x 8 B]
-    // [tiles: warps x 4 KB]
+    // carve-out: [pad][class table, 256 B @ 256-aligned][blob][16 B][register files][pad to 128 B]
+    // [line info: warps x 32 x 8 B][tiles: warps x 4 KB, 128-byte aligned rows (tile_slot)]
     const uint32_t s0abs = (uint32_t)__cvta_generic_to_shared(smem);
     const uint32_t cls_abs = (s0abs + 255u) & ~255u;
     uint8_t* g_cls = reinterpret_cast<uint8_t*>(smem) + (cls_abs - s0abs);
@@ -1831,7 +1853,8 @@ __global__ void __launch_bounds__(1024, 1)
     uint16_t* regs = wregs + (size_t)lane * reg_pitch;
     const uint32_t regs_abs = (uint32_t)__cvta_generic_to_shared(regs);
     const uint32_t regs_m2 = regs_abs - 2;
-    const uint32_t aux_abs = (uint32_t)__cvta_generic_to_shared(g_regs0 + (size_t)blockDim.x * reg_pitch * 2);
+    const uint32_t aux_abs = ((uint32_t)__cvta_generic_to_shared(g_regs0 + (size_t)blockDim.x * reg_pitch * 2) + 127u) &
+                             ~127u;
     const uint32_t info_abs = aux_abs + wid * 256;
     const uint32_t tile_abs = aux_abs + nwarps * 256 + wid * (LCT_STAGE_CHUNKS * 512);
     // bounce the class-table address through shared memory so that it lives in a per-thread register: with a
@@ -1844,16 +1867,8 @@ __global__ void __launch_bounds__(1024, 1)
     uint16_t* rg = regs;
     if (order && order_flag && *order_flag == 0) // the length pre-pass found a uniform batch: natural order
         order = nullptr;
-    // loader role of this lane: chunk column q of lines L0 + r (r = 0..7); tile slot of (chunk q, line) is
-    // q * 512 + ((line ^ q) << 4): the XOR keeps the 8 writers of a line and the 32 readers of a row on distinct banks
     TdfaLoader L;
-    L.gbase16 = reinterpret_cast<const uint4*>((uintptr_t)base & ~(uintptr_t)15);
-    L.ld_q = lane & 7;
-    const uint32_t ld_L0 = (lane >> 3) * 8;
-    L.ld_info = info_abs + ld_L0 * 8;
-    L.ld_dst = tile_abs + (L.ld_q << 9) + (ld_L0 << 4);
-    L.tile_abs = tile_abs;
-    L.rd_lane16 = lane << 4;
+    L.init(base, info_abs, tile_abs, lane);
     for (;;) {
         unsigned long long batch = 0;
         if (lane == 0)
@@ -2019,7 +2034,9 @@ __global__ void __launch_bounds__(1024, 1)
     uint16_t* regs = wregs + (size_t)lane * reg_pitch;
     const uint32_t regs_abs = (uint32_t)__cvta_generic_to_shared(regs);
     const uint32_t regs_m2 = regs_abs - 2;
-    const uint32_t aux_abs = (uint32_t)__cvta_generic_to_shared(g_regs0 + (size_t)blockDim.x * reg_pitch * 2);
+    // line info and tiles behind the register files, 128-byte aligned (tile_slot)
+    const uint32_t aux_abs = ((uint32_t)__cvta_generic_to_shared(g_regs0 + (size_t)blockDim.x * reg_pitch * 2) + 127u) &
+                             ~127u;
     const uint32_t info_abs = aux_abs + wid * 256;
     const uint32_t tile_abs = aux_abs + nwarps * 256 + wid * (LCT_STAGE_CHUNKS * 512);
     const uint32_t pats_abs = (uint32_t)__cvta_generic_to_shared(pats);
@@ -2027,13 +2044,7 @@ __global__ void __launch_bounds__(1024, 1)
     if (order && order_flag && *order_flag == 0)
         order = nullptr;
     TdfaLoader L;
-    L.gbase16 = reinterpret_cast<const uint4*>((uintptr_t)base & ~(uintptr_t)15);
-    L.ld_q = lane & 7;
-    const uint32_t ld_L0 = (lane >> 3) * 8;
-    L.ld_info = info_abs + ld_L0 * 8;
-    L.ld_dst = tile_abs + (L.ld_q << 9) + (ld_L0 << 4);
-    L.tile_abs = tile_abs;
-    L.rd_lane16 = lane << 4;
+    L.init(base, info_abs, tile_abs, lane);
     for (;;) {
         unsigned long long batch = 0;
         if (lane == 0)
@@ -3215,12 +3226,13 @@ __global__ void __launch_bounds__(128)
 
 // ---- tiled variant for the quote FSM (the common configuration) -----------------------------------------------------
 // Same structure as the staged regex kernel: persistent warps claim 32-line batches, fetch the lines COOPERATIVELY
-// (cp.async, 4 full 128-byte segments per instruction, [chunk][line ^ chunk] tile) instead of every lane pulling its
+// (TdfaLoader: cp.async, 4 full 128-byte segments per instruction, tile_slot layout) instead of every lane pulling its
 // own line with LDG.128 (32 different 128-byte lines per instruction), and each lane then streams its line out of the
 // tile through the resumable run-skipping FSM (lc_delim_chunk).  Only the trimmed range is fetched: the lane first looks
 // at the last 16 bytes of its line for trailing blanks / CRs (:226-238); leading blanks are skipped in the stream.
 // Field records are assembled in the per-warp row block in shared memory and leave as coalesced 128-byte stores, as
-// in delim_kernel<true>.  Shared memory per warp: 256 B line info + 4 KB tile + 3 x 32 x (max_fields | 1) words.
+// in delim_kernel<true>.  Shared memory per warp: 256 B line info + 4 KB tile + 3 x 32 x (max_fields | 1) words, plus
+// 128 B per block to align the tiles.
 __global__ void __launch_bounds__(1024, 1)
     delim_tiled_kernel(DelimConfig cfg, const uint8_t* __restrict__ base, const uint32_t* __restrict__ ev_off,
                        const uint32_t* __restrict__ ev_len, uint64_t n, uint8_t* __restrict__ status,
@@ -3232,23 +3244,19 @@ __global__ void __launch_bounds__(1024, 1)
     // pitch MF), so that they leave -- zero padding included -- as plain 16-byte vector copies
     const uint32_t MF = cfg.max_fields;
     const uint32_t blk_words = 32 * MF, blk_pad = (blk_words + 3u) & ~3u; // words per table block (16-byte multiple)
-    const uint32_t s0abs = (uint32_t)__cvta_generic_to_shared(smem);
+    // line info and tiles from the first 128-byte boundary of the window (tile_slot), the row blocks behind them
+    const uint32_t raw_abs = (uint32_t)__cvta_generic_to_shared(smem), s0abs = (raw_abs + 127u) & ~127u;
     const uint32_t info_abs = s0abs + wid * 256;
     const uint32_t tile_abs = s0abs + nwarps * 256 + wid * (LCT_STAGE_CHUNKS * 512);
-    uint32_t* wrows = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(smem) + (size_t)nwarps * (256 + 4096)) +
+    uint32_t* wrows = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(smem) + (s0abs - raw_abs) +
+                                                  (size_t)nwarps * (256 + 4096)) +
                       (size_t)wid * 3 * blk_pad;
     uint32_t* fo = wrows + lane * MF;
     uint32_t* fl = fo + blk_pad;
     uint32_t* fd = fl + blk_pad;
     const uint32_t base_mis = (uint32_t)((uintptr_t)base & 15);
     TdfaLoader L;
-    L.gbase16 = reinterpret_cast<const uint4*>((uintptr_t)base & ~(uintptr_t)15);
-    L.ld_q = lane & 7;
-    const uint32_t ld_L0 = (lane >> 3) * 8;
-    L.ld_info = info_abs + ld_L0 * 8;
-    L.ld_dst = tile_abs + (L.ld_q << 9) + (ld_L0 << 4);
-    L.tile_abs = tile_abs;
-    L.rd_lane16 = lane << 4;
+    L.init(base, info_abs, tile_abs, lane);
     const uint32_t sep_splat = cfg.sep[0] * 0x01010101u, quote_splat = cfg.quote * 0x01010101u;
     for (;;) {
         unsigned long long batch = 0;
@@ -3319,9 +3327,8 @@ __global__ void __launch_bounds__(1024, 1)
             if (parse && ok && !slow) {
                 const uint32_t kb = nch < s0 + LCT_STAGE_CHUNKS ? nch : s0 + LCT_STAGE_CHUNKS;
                 for (uint32_t k = s0; k < kb; k += 2) { // 32 bytes per step (the second chunk may lie behind the record)
-                    const uint32_t q = k & 7;
-                    const uint4 v0 = lds_u128_v(tile_abs + (q << 9) + (L.rd_lane16 ^ (q << 4)));
-                    const uint4 v1 = lds_u128_v(tile_abs + ((q + 1) << 9) + (L.rd_lane16 ^ ((q + 1) << 4)));
+                    const uint4 v0 = lds_u128_v(L.own(k));
+                    const uint4 v1 = lds_u128_v(L.own(k + 1));
                     const uint32_t q0 = k * 16;
                     if (!started) {
                         // leading ' ' (:233-238): the first byte that is not a blank starts the record
@@ -3441,9 +3448,9 @@ void launch_delim(const DelimConfig& cfg, const uint8_t* d_base, const uint32_t*
         cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         const size_t per_warp = 256 + 4096 + (size_t)3 * ((32 * cfg.max_fields + 3u) & ~3u) * 4;
-        uint32_t warps = (uint32_t)std::min<size_t>(32, (size_t)smem_max / per_warp);
+        uint32_t warps = (uint32_t)std::min<size_t>(32, ((size_t)smem_max - 128) / per_warp);
         if (warps >= 8) {
-            const size_t smem = per_warp * warps;
+            const size_t smem = per_warp * warps + 128;
             cudaFuncSetAttribute(delim_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             const uint64_t need = (n + warps * 32 - 1) / (warps * 32);
             const unsigned g = (unsigned)std::min<uint64_t>(need, (uint64_t)sms);

@@ -93,10 +93,11 @@ int launch_regex_fast2(const void* d_blob, uint32_t blob_bytes, bool multi, bool
 // a3 single-pass tagged-DFA path (LcTdfaHeader): no labels; per thread only nregs u16 registers in shared memory.
 // Events of 65535 bytes or more raise *d_overflow and are left to launch_regex_tdfa_long (32-bit slots).
 // Lines are fetched cooperatively (cp.async, 4 full 128-byte lines per instruction) into a per-warp 4 KB tile;
-// carve-out = 512 B (aligned class table) + blob + register files + 256 B line info and 4 KB tile per warp
+// carve-out = 512 B (aligned class table) + blob + register files + 128 B (alignment of the tiles) + 256 B line
+// info and 4 KB tile per warp
 inline uint32_t tdfa_reg_pitch(uint32_t nregs) { return (((nregs + 1) / 2) | 1u) * 2; } // halfwords; odd WORD pitch
 inline size_t tdfa_staged_smem_bytes(uint32_t blob_bytes, uint32_t nregs, uint32_t threads) {
-    return 512 + (size_t)blob_bytes + 16 + (size_t)threads * tdfa_reg_pitch(nregs) * 2 +
+    return 512 + (size_t)blob_bytes + 16 + (size_t)threads * tdfa_reg_pitch(nregs) * 2 + 128 +
            (size_t)(threads / 32) * (256 + 4096);
 }
 int launch_regex_tdfa_staged(const void* d_blob, uint32_t blob_bytes, bool slow, uint32_t nregs, const uint8_t* d_base,
@@ -121,7 +122,7 @@ inline size_t tdfa_multi_table_bytes(const TdfaMultiArgs& a) {
     return t;
 }
 inline size_t tdfa_multi_smem_bytes(const TdfaMultiArgs& a, uint32_t max_nregs, uint32_t threads) {
-    return tdfa_multi_table_bytes(a) + 16 + (size_t)threads * tdfa_reg_pitch(max_nregs) * 2 +
+    return tdfa_multi_table_bytes(a) + 16 + (size_t)threads * tdfa_reg_pitch(max_nregs) * 2 + 128 +
            (size_t)(threads / 32) * (256 + 4096);
 }
 int launch_regex_tdfa_multi(const TdfaMultiArgs& a, uint32_t p_base, bool resume, bool slow, uint32_t max_nregs,

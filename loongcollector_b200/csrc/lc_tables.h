@@ -172,7 +172,8 @@ struct LcFast2Header {
 //   skip  u32 [nstates+1]          run skipping: a state that every byte except at most two "exit" bytes maps back to
 //                                  itself without touching a register (the inside of [^"]*, .*, the dead state) can
 //                                  jump over a whole 16-byte chunk that holds none of its exit bytes.
-//                                  0 = not skippable; else LC_TDFA_SKIP | nexits << 16 | exit2 << 8 | exit1.
+//                                  0 = not skippable; else LC_TDFA_SKIP | nexits << 16 | exit2 << 8 | exit1, with
+//                                  exit2 = exit1 when nexits = 1.
 #define LC_TDFA_MAGIC 0x4C435444u /* 'LCTD' */
 #define LC_TDFA_SLOW 0x00800000u
 #define LC_TDFA_SRC_POS 0xFFu

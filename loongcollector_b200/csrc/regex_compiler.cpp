@@ -1954,6 +1954,8 @@ CompileResult compile_regex(const char* pattern, size_t len, size_t max_table_by
                         ++nexit;
                     }
                 }
+                if (nexit == 1)
+                    ex[1] = ex[0]; // the exit test always checks both slots
                 if (nexit <= 2)
                     skip[s] = LC_TDFA_SKIP | nexit << 16 | ex[1] << 8 | ex[0];
             }
