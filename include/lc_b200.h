@@ -711,6 +711,92 @@ int lc_delim_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uin
                                  uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
                                  uint64_t* raw_len, uint64_t counters[8]);
 
+/* ---- f4: the split -> delimiter -> regex chain (ProcessorSplitLogStringNative or
+ * ProcessorSplitMultilineLogStringNative, then ProcessorParseDelimiterNative with the same SourceKey, then
+ * ProcessorParseRegexNative reading one of the delimiter's keys -- BASELINE config C4 on file input) to the SLS wire
+ * format.  The source event is flat, and piece k enters the chain as [source_key -> piece] or, when offset_key !=
+ * NULL, [source_key -> piece, offset_key -> decimal(src_pos + off[k])].
+ *   - The delimiter stage (sep .. copy_raw) runs as for lc_sls_serialize_split_delim_dev: the offset content follows
+ *     source_key's and holds the column keyed offset_key when the row parsed and reaches it, else the digits; a blank
+ *     piece is left untouched; a failed piece without keep_fail is erased.
+ *   - The regex stage (rkeys .. whole_line) then runs as for lc_sls_serialize_delim_regex_dev: it reads key k's value
+ *     (column k unquoted, the whole line, or none), deletes key k's content in place or overwrites it by a regex key
+ *     equal to k, and its other contents follow the delimiter's.
+ *   - A regex failure without rkeep_fail erases the piece when no content is left, or only the offset content
+ *     (ShouldEraseEvent); the regex stage's discarded counter counts it.
+ * counters[8] (may be NULL) as lc_sls_serialize_delim_regex_dev's.  Refused with LC_ERR_INVALID_ARG: what
+ * lc_sls_serialize_split_delim_dev or lc_sls_serialize_delim_regex_dev refuses; an offset_key equal to rsource_key;
+ * a regex key, rrenamed_key or "__raw_log__" equal to offset_key (the offset content counts as one more content the
+ * delimiter stage leaves besides key k's, also for the "_time_" / "_source_" rule).
+ *
+ * lc_sls_serialize_split_delim_regex_dev: from the DEVICE piece tables of one lc_split_lines_dev /
+ * lc_multiline_split_dev call over d_src[0, src_len), the delimiter tables of lc_delim_parse_dev over those pieces,
+ * the value table of lc_delim_regex_tap_dev over the same tables (its side copies behind src_len in d_src) and the
+ * regex tables of lc_regex_parse_dev over the values (NULL in whole-line mode).  d_out receives the bytes; *out_len
+ * (host) their count; LC_ERR_CAPACITY if > out_cap (nothing written, *out_len and counters set).  LC_ERR_TOO_LARGE
+ * when src_len reaches 0xFFFFFFF0, n reaches 2^30, n * max_fields or n * row_pitch 2^32, or a record would reach
+ * 4 GiB. */
+int lc_sls_serialize_split_delim_regex_dev(
+    lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+    const uint8_t* d_status, const uint32_t* d_nfields, const uint32_t* d_f_off, const uint32_t* d_f_len,
+    const uint32_t* d_f_dq, uint32_t max_fields, const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend,
+    int discard, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+    uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed,
+    int copy_raw, const char* const* rkeys, const uint32_t* rkey_lens, uint32_t rnkeys, const char* rsource_key,
+    uint32_t rsource_key_len, const char* rrenamed_key, uint32_t rrenamed_key_len, int rkeep_fail, int rkeep_succeed,
+    int rcopy_raw, int whole_line, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+    uint32_t time_ns, const uint32_t* d_val_off, const uint32_t* d_val_len, const uint8_t* d_re_status,
+    const uint32_t* d_cap_off, const uint32_t* d_cap_len, uint32_t row_pitch, uint8_t* d_out, uint64_t out_cap,
+    uint64_t* out_len, uint64_t counters[8]);
+
+/* The same with a HOST source value: upload it once, split it on the device, run lc_delim_parse_dev over the pieces
+ * (allow_short, max_fields as for lc_delim_parse_sls), the value tap, the regex stage over the values (re may be NULL
+ * in whole-line mode), serialise, and bring back only the wire bytes; *n_events, ml_counters, the _lz4 variants and
+ * which outputs are set on LC_ERR_CAPACITY as for lc_split_regex_parse_sls.  The side copies go behind the source on
+ * the device: LC_ERR_TOO_LARGE, before anything is allocated, when align16(len) + len reaches 4 GiB; and past the
+ * piece, column and capture limits of lc_split_delim_parse_sls / lc_split_regex_parse_sls. */
+int lc_split_delim_regex_parse_sls(
+    lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len, uint8_t split_char, int allow_short,
+    uint32_t max_fields, const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard,
+    const char* const* keys, const uint32_t* key_lens, uint32_t nkeys, const char* source_key, uint32_t source_key_len,
+    const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+    const char* const* rkeys, const uint32_t* rkey_lens, uint32_t rnkeys, const char* rsource_key,
+    uint32_t rsource_key_len, const char* rrenamed_key, uint32_t rrenamed_key_len, int rkeep_fail, int rkeep_succeed,
+    int rcopy_raw, int whole_line, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+    uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events, uint64_t counters[8]);
+int lc_split_delim_regex_parse_sls_lz4(
+    lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len, uint8_t split_char, int allow_short,
+    uint32_t max_fields, const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard,
+    const char* const* keys, const uint32_t* key_lens, uint32_t nkeys, const char* source_key, uint32_t source_key_len,
+    const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+    const char* const* rkeys, const uint32_t* rkey_lens, uint32_t rnkeys, const char* rsource_key,
+    uint32_t rsource_key_len, const char* rrenamed_key, uint32_t rrenamed_key_len, int rkeep_fail, int rkeep_succeed,
+    int rcopy_raw, int whole_line, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+    uint32_t time_ns, const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+    uint64_t* raw_len, uint64_t* n_events, uint64_t counters[8]);
+int lc_multiline_split_delim_regex_parse_sls(
+    lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+    const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, int allow_short, uint32_t max_fields,
+    const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard, const char* const* keys,
+    const uint32_t* key_lens, uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+    uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, const char* const* rkeys,
+    const uint32_t* rkey_lens, uint32_t rnkeys, const char* rsource_key, uint32_t rsource_key_len,
+    const char* rrenamed_key, uint32_t rrenamed_key_len, int rkeep_fail, int rkeep_succeed, int rcopy_raw,
+    int whole_line, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+    uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events, uint64_t counters[8],
+    uint64_t ml_counters[3]);
+int lc_multiline_split_delim_regex_parse_sls_lz4(
+    lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+    const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, int allow_short, uint32_t max_fields,
+    const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend, int discard, const char* const* keys,
+    const uint32_t* key_lens, uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+    uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, const char* const* rkeys,
+    const uint32_t* rkey_lens, uint32_t rnkeys, const char* rsource_key, uint32_t rsource_key_len,
+    const char* rrenamed_key, uint32_t rrenamed_key_len, int rkeep_fail, int rkeep_succeed, int rcopy_raw,
+    int whole_line, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+    const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+    uint64_t* n_events, uint64_t counters[8], uint64_t ml_counters[3]);
+
 /* LZ4 compression of serialised groups (FlusherSLS's default compressor, LZ4Compressor::Compress =
  * LZ4_compress_default): segment g = d_in[d_seg_off[g], + d_seg_len[g]) becomes one LZ4 *block* (not a frame), the
  * blocks packed back to back in d_out: block g = d_out[d_blk_off[g], + d_blk_len[g]).  The bytes are deterministic;

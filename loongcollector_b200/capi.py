@@ -146,6 +146,18 @@ def lib():
         [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
     L.lc_multiline_split_delim_parse_sls_lz4.argtypes = [vp, vp, u64, vp, vp, vp, i32] + sd_cfg + sls_cfg + \
         sr_tail + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
+    # the split -> delimiter -> regex chain: allow_short, max_fields, both stages' arguments, the split -> regex tail
+    sdr_cfg = [i32, u32] + chain_cfg + sr_tail
+    L.lc_sls_serialize_split_delim_regex_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, vp, u32] + \
+        chain_cfg + sr_tail + [vp, vp, vp, vp, vp, u32, vp, u64, C.POINTER(u64), vp]
+    L.lc_split_delim_regex_parse_sls.argtypes = [vp, vp, vp, u64, u8] + sdr_cfg + \
+        [vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_split_delim_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, u8] + sdr_cfg + \
+        [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_multiline_split_delim_regex_parse_sls.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sdr_cfg + \
+        [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
+    L.lc_multiline_split_delim_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sdr_cfg + \
+        [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
     _LIB = L
     return L
 
@@ -992,6 +1004,95 @@ class Engine:
             sep, quote, treatment, keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw, allow_short,
             max_fields, offset_key, src_pos, time, time_ns, out_cap, True, tail)
 
+    def sls_serialize_split_delim_regex_dev(self, d_src, src_len, d_off, d_len, n, d_status, d_nf, d_fo, d_fl, d_fd,
+                                            max_fields, delim, regex, d_val_off, d_val_len, d_re_status, d_cap_off,
+                                            d_cap_len, row_pitch, offset_key=None, src_pos=0, time=0, time_ns=None,
+                                            d_out=None, out_cap=0):
+        """Wire bytes of the split -> delimiter -> regex chain from the device piece tables of one split_lines_dev /
+        multiline_split_dev call, the device tables of delim_parse_dev over those pieces, the value table of
+        delim_regex_tap_dev over the same tables and the regex tables over the values (delim, regex: as for
+        sls_serialize_delim_regex_dev; lc_sls_serialize_split_delim_regex_dev).  Returns (byte count written to d_out,
+        counters[8]); with d_out None the byte count needed."""
+        _keep, cfg = self._chain_cfg(delim, regex)
+        need = C.c_uint64(0)
+        ctr = np.zeros(8, np.uint64)
+        rc = lib().lc_sls_serialize_split_delim_regex_dev(
+            self._h, _p(d_src), src_len, _p(d_off), _p(d_len), n, _p(d_status), _p(d_nf), _p(d_fo), _p(d_fl),
+            _p(d_fd), max_fields, *cfg, *self._sr_tail(offset_key, src_pos, time, time_ns), _p(d_val_off),
+            _p(d_val_len), _p(d_re_status), _p(d_cap_off), _p(d_cap_len), row_pitch, _p(d_out), out_cap,
+            C.byref(need), _p(ctr))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value), ctr  # a sizing query
+        _check(rc)
+        return int(need.value), ctr
+
+    def _split_delim_regex(self, fn, rx, buf, extra, delim, regex, allow_short, max_fields, offset_key, src_pos, time,
+                           time_ns, out_cap, ml, tail):
+        """one host-buffer split -> delimiter -> regex call, sized by an estimate first and by the exact size when that
+        was short; tail None: the wire bytes, else records ‖ tail as one LZ4 block.  Returns (bytes, raw_len,
+        n_events, counters[8], ml_counters[3] or None)"""
+        a = _u8(buf)
+        mf = int(max_fields if max_fields is not None else len(delim["keys"]) + 16)
+        _keep, cfg = self._chain_cfg(delim, regex)
+        tl = None if tail is None else np.frombuffer(bytes(tail), np.uint8)
+        est = 2 * a.size + 4096 + (0 if tl is None else tl.size)
+        cap = int(out_cap if out_cap is not None else est + est // 255 + 16)
+        for _ in range(2):
+            out = np.empty(max(cap, 1), np.uint8)
+            need, raw, nev = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+            ctr, mctr = np.zeros(8, np.uint64), np.zeros(3, np.uint64)
+            z = [] if tl is None else [_p(tl) if tl.size else None, tl.size]
+            outs = [_p(out), cap, C.byref(need)] + ([] if tl is None else [C.byref(raw)]) + [C.byref(nev), _p(ctr)]
+            rc = fn(self._h, _rh(rx), _p(a), a.size, *extra, int(bool(allow_short)), mf, *cfg,
+                    *self._sr_tail(offset_key, src_pos, time, time_ns), *z, *outs, *([_p(mctr)] if ml else []))
+            if rc == LC_ERR_CAPACITY and out_cap is None:
+                cap = int(need.value)
+                continue
+            _check(rc)
+            return bytes(out[:need.value]), int(raw.value), int(nev.value), ctr, (mctr if ml else None)
+        _check(rc)
+
+    def split_delim_regex_parse_sls(self, rx, buf, split_char, delim, regex, allow_short=True, max_fields=None,
+                                    offset_key=None, src_pos=0, time=0, time_ns=None, out_cap=None):
+        """Host source value in: split, delimiter, regex on one of its keys, wire bytes out
+        (lc_split_delim_regex_parse_sls; rx may be None in whole-line mode; delim, regex as for
+        sls_serialize_delim_regex_dev).  Returns (bytes, number of pieces, counters[8])."""
+        data, _raw, nev, ctr, _m = self._split_delim_regex(
+            lib().lc_split_delim_regex_parse_sls, rx, buf, [split_char], delim, regex, allow_short, max_fields,
+            offset_key, src_pos, time, time_ns, out_cap, False, None)
+        return data, nev, ctr
+
+    def split_delim_regex_parse_sls_lz4(self, rx, buf, split_char, delim, regex, allow_short=True, max_fields=None,
+                                        offset_key=None, src_pos=0, time=0, time_ns=None, tail=b"", out_cap=None):
+        """split_delim_regex_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_split_delim_regex_parse_sls_lz4).  Returns (block, raw_len, number of pieces, counters[8])."""
+        data, raw, nev, ctr, _m = self._split_delim_regex(
+            lib().lc_split_delim_regex_parse_sls_lz4, rx, buf, [split_char], delim, regex, allow_short, max_fields,
+            offset_key, src_pos, time, time_ns, out_cap, False, tail)
+        return data, raw, nev, ctr
+
+    def multiline_split_delim_regex_parse_sls(self, rx, buf, start, cont, end, discard, delim, regex,
+                                              allow_short=True, max_fields=None, offset_key=None, src_pos=0, time=0,
+                                              time_ns=None, out_cap=None):
+        """The same with the multiline splitter (lc_multiline_split_delim_regex_parse_sls).  Returns (bytes, number
+        of events, counters[8], splitter counters[3] = matched_events, input_lines, unmatched_lines)."""
+        data, _raw, nev, ctr, mctr = self._split_delim_regex(
+            lib().lc_multiline_split_delim_regex_parse_sls, rx, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], delim, regex, allow_short, max_fields, offset_key,
+            src_pos, time, time_ns, out_cap, True, None)
+        return data, nev, ctr, mctr
+
+    def multiline_split_delim_regex_parse_sls_lz4(self, rx, buf, start, cont, end, discard, delim, regex,
+                                                  allow_short=True, max_fields=None, offset_key=None, src_pos=0,
+                                                  time=0, time_ns=None, tail=b"", out_cap=None):
+        """multiline_split_delim_regex_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_multiline_split_delim_regex_parse_sls_lz4).  Returns (block, raw_len, number of events, counters[8],
+        splitter counters[3])."""
+        return self._split_delim_regex(
+            lib().lc_multiline_split_delim_regex_parse_sls_lz4, rx, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], delim, regex, allow_short, max_fields, offset_key,
+            src_pos, time, time_ns, out_cap, True, tail)
+
     def lz4_compress_dev(self, d_in, nseg, d_seg_off, d_seg_len, d_out=None, out_cap=0, d_blk_off=None,
                          d_blk_len=None):
         """One LZ4 block per device segment d_in[d_seg_off[g], + d_seg_len[g]) (u64 / u32 tables), packed in d_out
@@ -1239,7 +1340,8 @@ def host_chain_serialize_sls(delim, regex, group, enable_ns=False, mode=0):
 def host_chain3_serialize_sls(split, regex, filt, group, enable_ns=False, mode=0):
     """The split -> regex -> filter chain of three HostProcessors on a JSON group (lc_host_chain3_serialize_sls).
     mode 0: split's SerializeSls(group, regex, filter); 1: Process x 3 + Serialize; 2: SerializeSlsLz4.  Returns (bytes,
-    raw_len, None) or (None, 0, error)."""
+    raw_len, None) or (None, 0, error).  The split -> delimiter -> regex chain goes through the same call, with a
+    delimiter processor as `regex` and a regex processor as `filt`."""
     import json
     L = lib()
     L.lc_host_chain3_serialize_sls.restype = C.c_void_p

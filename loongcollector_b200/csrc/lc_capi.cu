@@ -112,6 +112,9 @@ struct lc_engine {
     // the removed-piece counter and the keep bytes; the chain's piece and regex tables live elsewhere (in, out_a,
     // out_b, out_c, dr_*), and so does the scratch of the boolean match (out_d, out_e, lab*, order, desc)
     DevBuf fl_tab, fl_match, fl_dig, fl_keep;
+    // split -> delimiter -> regex chain: the delimiter tables over the pieces (status, column counts, f_off, f_len,
+    // f_dq) and the offset key; its value, regex and tap tables are the dr_* of the delimiter -> regex chain
+    DevBuf sdr_status, sdr_nf, sdr_f_off, sdr_f_len, sdr_f_dq, sdr_okey;
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
     std::unordered_map<uint64_t, void*> blobs; // regex id * 4 + layout -> device blob
@@ -327,7 +330,8 @@ void lc_engine_destroy(lc_engine_t* e) {
                       &e->z_seq, &e->z_info, &e->z_size, &e->z_first, &e->z_choff, &e->z_tab, &e->z_out,
                       &e->zs_first, &e->zs_size, &e->zs_off, &e->zs_slot,
                       &e->dr_keys, &e->dr_val_off, &e->dr_val_len, &e->dr_status, &e->dr_cap_off, &e->dr_cap_len,
-                      &e->dr_copy, &e->dr_slot, &e->dr_desc, &e->fl_tab, &e->fl_match, &e->fl_dig, &e->fl_keep};
+                      &e->dr_copy, &e->dr_slot, &e->dr_desc, &e->fl_tab, &e->fl_match, &e->fl_dig, &e->fl_keep,
+                      &e->sdr_status, &e->sdr_nf, &e->sdr_f_off, &e->sdr_f_len, &e->sdr_f_dq, &e->sdr_okey};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -1801,7 +1805,7 @@ int serialize_sls_dev(lc_engine_t* e, const char* what, uint64_t n, uint32_t nco
     e->launches += 2;
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(&hs->total, &ds->total, 8, cudaMemcpyDeviceToHost, e->stream));
-    unsigned long long ctr[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    unsigned long long ctr[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     if (d_ctr)
         CU_TRY(cudaMemcpyAsync(ctr, d_ctr, ncounters * sizeof(unsigned long long), cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(cudaStreamSynchronize(e->stream));
@@ -3389,7 +3393,256 @@ int lc_multiline_split_delim_parse_sls_lz4(lc_engine_t* e, const uint8_t* buf, u
     return split_delim_sls_host(e, "lc_multiline_split_delim_parse_sls_lz4", buf, len, ML_SPLIT, SPLIT_DELIM_ARGS,
                                 out, out_cap, out_len, n_events, counters, &z);
 }
+} // extern "C"
+
+// ------------------------------------------------------------------------------ split -> delimiter -> regex -> SLS
+namespace {
+
+// lc_delim_sls_setup + lc_regex_sls_setup + lc_split_delim_regex_sls_link: the delimiter's key strings are staged in
+// `dr_keys`, the regex plans in `sls_plan` and the offset key in `sdr_okey`.  pitch = the regex tables' row pitch.
+int split_delim_regex_config(lc_engine_t* e, const char* what, uint32_t max_fields, CHAIN_PARAMS, OFFSET_PARAMS,
+                             uint32_t pitch, LcSplitDelimRegexSlsCfg* c) {
+    memset(c, 0, sizeof *c);
+    int rc = delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, keys, key_lens, nkeys,
+                              source_key, source_key_len, renamed_key, renamed_key_len, keep_fail, keep_succeed,
+                              copy_raw, &c->r.d, &e->dr_keys);
+    if (rc)
+        return rc;
+    rc = regex_sls_config(e, what, rkeys, rkey_lens, rnkeys, rsource_key, rsource_key_len, rrenamed_key,
+                          rrenamed_key_len, rkeep_fail, rkeep_succeed, rcopy_raw, whole_line, pitch, &c->r.x);
+    if (rc)
+        return rc;
+    const char* why = lc_split_delim_regex_sls_link(keys, key_lens, source_key, source_key_len, renamed_key,
+                                                    renamed_key_len, rkeys, rkey_lens, rnkeys, rsource_key,
+                                                    rsource_key_len, rrenamed_key, rrenamed_key_len, rkeep_fail,
+                                                    rkeep_succeed, rcopy_raw, whole_line, OFFSET_ARGS, c);
+    if (why)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    if (offset_key) {
+        CU_TRY(e->sdr_okey.ensure(offset_key_len + 16));
+        if (offset_key_len) {
+            CU_TRY(cudaMemcpyAsync(e->sdr_okey.p, offset_key, offset_key_len, cudaMemcpyHostToDevice, e->stream));
+            // (pageable source: its bytes must be on the device before it dies)
+            CU_TRY(cudaStreamSynchronize(e->stream));
+        }
+        c->s.okey = e->sdr_okey.as<uint8_t>();
+    }
+    return LC_OK;
+}
+
+// The size pass and the emit of the chain over the n pieces of t (serialize_sls_dev): into d_out (the device-fed
+// call), or back to the host buffer out, or -- with z -- records ‖ tail as one LZ4 block.  counters[8] (or nullptr) as
+// lc_delim_regex_verdict orders them; set whenever the size pass ran.
+int split_delim_regex_sls_run(lc_engine_t* e, const char* what, const LcSplitDelimRegexSlsCfg& c,
+                              const lck::DelimRegexSlsTables& t, uint64_t n, uint8_t* d_out, uint8_t* out,
+                              uint64_t out_cap, uint64_t* out_len, uint64_t* counters, const Lz4Tail* z) {
+    uint64_t ctr[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; // + pieces whose record would reach 4 GiB
+    SlsTo to;
+    to.host = out;
+    to.z = z;
+    to.too_large = 8;
+    const int rc = serialize_sls_dev(
+        e, what, n, 9,
+        [&](uint32_t* rec, uint32_t* body, unsigned long long* d_ctr) {
+            lck::launch_split_delim_regex_sls_sizes(c, t, n, rec, body, d_ctr, e->stream);
+        },
+        [&](const uint64_t* rec_off, const uint32_t* body, uint8_t* dst) {
+            lck::launch_split_delim_regex_sls_emit(c, t, n, rec_off, body, dst, e->stream);
+        },
+        d_out, out_cap, out_len, ctr, to);
+    if (counters)
+        memcpy(counters, ctr, 8 * sizeof(uint64_t));
+    return rc;
+}
+
+// Host-buffer split + delimiter + tap + regex + serialise (lc_split_delim_regex_parse_sls and the multiline / LZ4
+// siblings, through split_chain_sls_host).  Workspace:
+//   in                      the source [0, len), then the tap's side copies from align16(len): a copy is never longer
+//                           than its piece and the pieces do not overlap, so len bytes hold them all
+//   out_a / out_b (out_c)   the piece tables (the multiline flags)
+//   sdr_status, sdr_nf,     the delimiter tables over the pieces (status, column counts, [n][max_fields] f_off /
+//   sdr_f_off / _len / _dq  f_len / f_dq); the split -> delimiter chain's dr_status / dr_val_off / out_d / out_e /
+//                           dr_cap_off are the value and regex tables or the regex stage's scratch here
+//   dr_val_off / dr_val_len the value table (the tap), dr_copy / dr_slot / dr_desc its sizes, slots and scan
+//   dr_status, dr_cap_off / dr_cap_len   the regex tables over the values
+//   dr_keys, sls_plan, sdr_okey          the delimiter's key strings, the regex plans, the offset key
+// The splitters, lc_delim_parse_dev (its tiled kernel stages in shared memory), the regex stage (order, lab*, desc,
+// small; out_d / out_e only for a match without captures) and the serialiser (lab_sizes, cnt, lab_off, state, desc,
+// lab, z_*) use none of the others'.
+template <class Split>
+int split_delim_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* buf,
+                               uint64_t len, Split split, int allow_short, uint32_t max_fields, CHAIN_PARAMS,
+                               OFFSET_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                               uint64_t counters[8], const Lz4Tail* z) {
+    const uint64_t side_at = (len + 15) & ~15ull, arena = side_at + len;
+    uint32_t G = 0;
+    LcSplitDelimRegexSlsCfg c;
+    auto begin = [&]() {
+        if (counters)
+            memset(counters, 0, 8 * sizeof(uint64_t));
+        if (arena + 16 >= 0xFFFFFFF0ull)
+            return fail(LC_ERR_TOO_LARGE, std::string(what) + ": the source and its side copies must stay below 4 GiB");
+        return whole_line ? (int)LC_OK : check_regex_usable(re, what);
+    };
+    auto config = [&]() {
+        G = whole_line ? 0u : re->res.ngroups;
+        const int rc = split_delim_regex_config(e, what, max_fields, CHAIN_ARGS, OFFSET_ARGS, G, &c);
+        if (rc)
+            return rc;
+        CU_TRY(e->in.ensure(arena + 16)); // before the upload: `in` does not keep its bytes when it grows
+        return (int)LC_OK;
+    };
+    auto run = [&](uint64_t n) {
+        if (n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32) || n * (uint64_t)G >= (1ull << 32))
+            return fail(LC_ERR_TOO_LARGE,
+                        std::string(what) + ": < 2^30 pieces, < 2^32 columns and < 2^32 captures per call");
+        const uint64_t fbytes = n * max_fields * 4, dwords = lck::scan_tiles(n) + 3;
+        CU_TRY(e->sdr_status.ensure(n));
+        CU_TRY(e->sdr_nf.ensure(n * 4));
+        CU_TRY(e->sdr_f_off.ensure(fbytes));
+        CU_TRY(e->sdr_f_len.ensure(fbytes));
+        CU_TRY(e->sdr_f_dq.ensure(fbytes));
+        CU_TRY(e->dr_val_off.ensure(n * 4));
+        CU_TRY(e->dr_val_len.ensure(n * 4));
+        CU_TRY(e->dr_copy.ensure(n * 4));
+        CU_TRY(e->dr_slot.ensure(n * 8));
+        CU_TRY(e->dr_desc.ensure(dwords * 8));
+        CU_TRY(cudaMemsetAsync(e->dr_desc.p, 0, dwords * 8, e->stream));
+        uint8_t* base = e->in.as<uint8_t>();
+        const lck::DelimSlsTables dt{base,
+                                     e->out_a.as<uint32_t>(),
+                                     e->out_b.as<uint32_t>(),
+                                     e->sdr_status.as<uint8_t>(),
+                                     e->sdr_nf.as<uint32_t>(),
+                                     e->sdr_f_off.as<uint32_t>(),
+                                     e->sdr_f_len.as<uint32_t>(),
+                                     e->sdr_f_dq.as<uint32_t>()};
+        int rc = lc_delim_parse_dev(e, base, len, dt.ev_off, dt.ev_len, n, sep, sep_len, quote, nkeys, extend,
+                                    allow_short, max_fields, e->sdr_status.as<uint8_t>(), e->sdr_nf.as<uint32_t>(),
+                                    e->sdr_f_off.as<uint32_t>(), e->sdr_f_len.as<uint32_t>(),
+                                    e->sdr_f_dq.as<uint32_t>());
+        if (rc)
+            return rc;
+        queue_tap(e, c.r, dt, n, side_at, base, e->dr_copy.as<uint32_t>(), e->dr_slot.as<uint64_t>(),
+                  e->dr_desc.as<uint64_t>(), e->dr_val_off.as<uint32_t>(), e->dr_val_len.as<uint32_t>());
+        CU_TRY(cudaGetLastError());
+        const bool caps = !whole_line && rnkeys && rnkeys <= G;
+        if (!whole_line) {
+            CU_TRY(e->dr_status.ensure(n));
+            CU_TRY(e->dr_cap_off.ensure(n * G * 4 + 4));
+            CU_TRY(e->dr_cap_len.ensure(n * G * 4 + 4));
+            // (the values lie in the pieces or their side copies: len bytes at most)
+            rc = regex_parse_dev_impl(e, re, base, arena, len, e->dr_val_off.as<uint32_t>(),
+                                      e->dr_val_len.as<uint32_t>(), 1, n, rnkeys, e->dr_status.as<uint8_t>(),
+                                      e->dr_cap_off.as<uint32_t>(), e->dr_cap_len.as<uint32_t>(), false);
+            if (rc)
+                return rc;
+        }
+        const lck::DelimRegexSlsTables t{dt,
+                                         e->dr_val_off.as<uint32_t>(),
+                                         e->dr_val_len.as<uint32_t>(),
+                                         whole_line ? nullptr : e->dr_status.as<uint8_t>(),
+                                         caps ? e->dr_cap_off.as<uint32_t>() : nullptr,
+                                         caps ? e->dr_cap_len.as<uint32_t>() : nullptr};
+        return split_delim_regex_sls_run(e, what, c, t, n, nullptr, out, out_cap, out_len, counters, z);
+    };
+    return split_chain_sls_host(e, what, buf, len, split, (re || whole_line) && sep != nullptr, begin, config, run,
+                                out, out_cap, out_len, n_events, z);
+}
+
+} // namespace
+
+// the host-buffer calls' stage arguments: the delimiter's allow_short / max_fields and both stages' (CHAIN_PARAMS),
+// then the offset content
+#define SPLIT_DELIM_REGEX_PARAMS int allow_short, uint32_t max_fields, CHAIN_PARAMS, OFFSET_PARAMS
+#define SPLIT_DELIM_REGEX_ARGS allow_short, max_fields, CHAIN_ARGS, OFFSET_ARGS
+
+extern "C" {
+
+int lc_sls_serialize_split_delim_regex_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len,
+                                           const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+                                           const uint8_t* d_status, const uint32_t* d_nfields, const uint32_t* d_f_off,
+                                           const uint32_t* d_f_len, const uint32_t* d_f_dq, uint32_t max_fields,
+                                           CHAIN_PARAMS, OFFSET_PARAMS, const uint32_t* d_val_off,
+                                           const uint32_t* d_val_len, const uint8_t* d_re_status,
+                                           const uint32_t* d_cap_off, const uint32_t* d_cap_len, uint32_t row_pitch,
+                                           uint8_t* d_out, uint64_t out_cap, uint64_t* out_len,
+                                           uint64_t counters[8]) {
+    static const char* what = "lc_sls_serialize_split_delim_regex_dev";
+    const bool caps = !whole_line && rnkeys && rnkeys <= row_pitch; // the parsed plan reads the capture tables
+    if (!e || !out_len || (n && (!d_src || !d_off || !d_len || !d_status || !d_nfields || !d_f_off || !d_f_len ||
+                                 !d_f_dq || !d_val_off || !d_val_len)) ||
+        (n && !whole_line && !d_re_status) || (n && caps && (!d_cap_off || !d_cap_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (counters)
+        memset(counters, 0, 8 * sizeof(uint64_t));
+    if (src_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32) ||
+        n * (uint64_t)row_pitch >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 pieces, < 2^32 columns and < 2^32 captures "
+                                      "per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcSplitDelimRegexSlsCfg c;
+    rc = split_delim_regex_config(e, what, max_fields, CHAIN_ARGS, OFFSET_ARGS, row_pitch, &c);
+    if (rc || n == 0)
+        return rc;
+    const lck::DelimRegexSlsTables t{{d_src, d_off, d_len, d_status, d_nfields, d_f_off, d_f_len, d_f_dq},
+                                     d_val_off,
+                                     d_val_len,
+                                     whole_line ? nullptr : d_re_status,
+                                     caps ? d_cap_off : nullptr,
+                                     caps ? d_cap_len : nullptr};
+    return split_delim_regex_sls_run(e, what, c, t, n, d_out, nullptr, out_cap, out_len, counters, nullptr);
+}
+
+int lc_split_delim_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                   uint8_t split_char, SPLIT_DELIM_REGEX_PARAMS, uint8_t* out, uint64_t out_cap,
+                                   uint64_t* out_len, uint64_t* n_events, uint64_t counters[8]) {
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_delim_regex_sls_host(e, "lc_split_delim_regex_parse_sls", re, buf, len, split,
+                                      SPLIT_DELIM_REGEX_ARGS, out, out_cap, out_len, n_events, counters, nullptr);
+}
+
+int lc_split_delim_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                       uint8_t split_char, SPLIT_DELIM_REGEX_PARAMS, const uint8_t* tail,
+                                       uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                                       uint64_t* raw_len, uint64_t* n_events, uint64_t counters[8]) {
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return split_delim_regex_sls_host(e, "lc_split_delim_regex_parse_sls_lz4", re, buf, len, split,
+                                      SPLIT_DELIM_REGEX_ARGS, out, out_cap, out_len, n_events, counters, &z);
+}
+
+int lc_multiline_split_delim_regex_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                             const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                             int discard_unmatched, SPLIT_DELIM_REGEX_PARAMS, uint8_t* out,
+                                             uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                             uint64_t counters[8], uint64_t ml_counters[3]) {
+    return split_delim_regex_sls_host(e, "lc_multiline_split_delim_regex_parse_sls", re, buf, len, ML_SPLIT,
+                                      SPLIT_DELIM_REGEX_ARGS, out, out_cap, out_len, n_events, counters, nullptr);
+}
+
+int lc_multiline_split_delim_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf,
+                                                 uint64_t len, const lc_regex_t* start, const lc_regex_t* cont,
+                                                 const lc_regex_t* end, int discard_unmatched,
+                                                 SPLIT_DELIM_REGEX_PARAMS, const uint8_t* tail, uint64_t tail_len,
+                                                 uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+                                                 uint64_t* n_events, uint64_t counters[8], uint64_t ml_counters[3]) {
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return split_delim_regex_sls_host(e, "lc_multiline_split_delim_regex_parse_sls_lz4", re, buf, len, ML_SPLIT,
+                                      SPLIT_DELIM_REGEX_ARGS, out, out_cap, out_len, n_events, counters, &z);
+}
 #undef ML_SPLIT
+#undef SPLIT_DELIM_REGEX_PARAMS
+#undef SPLIT_DELIM_REGEX_ARGS
 
 } // extern "C"
 

@@ -1588,13 +1588,15 @@ LC_HD LcDelimRegexVerdict lc_delim_regex_verdict(const LcDelimRegexSlsCfg& c, co
 // stage's arguments) accepted their halves.  Returns nullptr (c->col and the *_is_k flags set), or why the chain is
 // refused: a regex SourceKey that is not one of the delimiter's keys, or a content the regex stage may write (a key,
 // RenamedSourceKey, "__raw_log__") under a name the delimiter stage may leave besides key k -- that overwrite would
-// depend on the row's shape.  Likewise ShouldEraseEvent's "_time_" + "_source_" rule on a regex failure.
+// depend on the row's shape.  Likewise ShouldEraseEvent's "_time_" + "_source_" rule on a regex failure.  okey (or
+// nullptr): a content the event held before the delimiter stage ran (the split's offset content), which the delimiter
+// stage leaves on every row it does not erase.
 inline const char* lc_delim_regex_sls_link(const LcDelimSlsCfg& d, const char* const* dkeys, const uint32_t* dkey_lens,
                                            const char* dsrc, uint32_t dsrc_len, const char* dren, uint32_t dren_len,
                                            const char* const* rkeys, const uint32_t* rkey_lens, uint32_t rnkeys,
                                            const char* rsrc, uint32_t rsrc_len, const char* rren, uint32_t rren_len,
                                            int rkeep_fail, int rkeep_succeed, int rcopy_raw, int rwhole_line,
-                                           LcDelimRegexSlsCfg* c) {
+                                           LcDelimRegexSlsCfg* c, const char* okey = nullptr, uint32_t okey_len = 0) {
     auto eq = [](const char* a, uint32_t la, const char* b, uint32_t lb) {
         return la == lb && (la == 0 || !memcmp(a, b, la));
     };
@@ -1617,7 +1619,8 @@ inline const char* lc_delim_regex_sls_link(const LcDelimSlsCfg& d, const char* c
                 return true;
         return eq(name, len, dsrc, dsrc_len) || ((d.keep_fail || d.keep_succeed) && eq(name, len, dren, dren_len)) ||
                (d.keep_fail && d.copy_raw && eq(name, len, "__raw_log__", 11)) ||
-               (d.mode != LC_DELIM_SLS_DISCARD && lc_delim_column_form(name, len, &idx));
+               (d.mode != LC_DELIM_SLS_DISCARD && lc_delim_column_form(name, len, &idx)) ||
+               (okey && eq(name, len, okey, okey_len));
     };
     bool clash = false;
     if (rwhole_line)
@@ -2118,6 +2121,85 @@ inline const char* lc_split_delim_sls_link(const LcDelimSlsCfg& d, const char* c
     c->has_ns = time_ns != 0xFFFFFFFFu;
     c->ns = c->has_ns ? time_ns : 0u;
     return nullptr;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, split -> delimiter -> regex chain: the Log record of piece k that a splitter, ProcessorParseDelimiterNative (the
+// splitter's SourceKey) and ProcessorParseRegexNative (SourceKey = key k of the delimiter) leave behind, written
+// straight from the piece tables, the delimiter tables over the pieces, the value table of the tap over those
+// (lc_delim_regex_tap, unchanged: the piece tables are its event table) and the regex tables over the values.
+//   - The piece enters as [SourceKey -> piece, offset_key -> decimal(src_pos + off[k])], or without the offset content
+//     when there is no log.file.offset metadata.
+//   - The delimiter stage runs as in the split -> delimiter chain: the offset slot follows SourceKey's content and holds
+//     the column keyed offset_key when the row parsed and reaches it, else the digits; a blank piece is left
+//     untouched; a failed piece without KeepingSourceWhenParseFail is erased.
+//   - The regex stage runs as in the delimiter -> regex chain: it reads key k's value by lc_delim_regex_value's rule,
+//     deletes key k's content in place (or overwrites it with a regex key equal to k) and appends the rest of its plan
+//     after the delimiter's contents.
+//   - ShouldEraseEvent (CommonParserOptions.cpp:99-117): a regex failure without the regex stage's
+//     KeepingSourceWhenParseFail erases the event when nothing is left, or when the offset content is all that is left.
+// lc_split_delim_regex_sls_link refuses an offset key equal to key k (on a row too short to reach column k the slot
+// would hold the digits under key k, and the regex would read them), and any regex content named like the offset key.
+struct LcSplitDelimRegexSlsCfg {
+    LcDelimRegexSlsCfg r; // the delimiter and regex stages (the tap's configuration)
+    LcSplitDelimSlsCfg s; // the offset content and the source event's time (s.d == r.d)
+};
+
+// both chained stages at once: the regex stage's own / in_place / tail and the split stage's slot
+struct LcSplitDelimRegexStage : LcDelimRegexStage {
+    LcSplitDelimStage o;
+    LC_HD uint32_t slot_col() const { return o.slot_col(); }
+    LC_HD bool slot_holds(uint32_t kid) const { return o.slot_holds(kid); }
+    template <class S>
+    LC_HD bool slot(S& s) {
+        return o.slot(s);
+    }
+};
+
+// The body of the piece's Log record into sink s (LcSlsCount64 / LcSlsWrite); r.d = the piece and its delimiter row
+// (with the source event's time and ns), the rest its value and regex row.  Returns the number of contents; 0 = erased.
+template <class S>
+LC_HD uint32_t lc_split_delim_regex_sls_body(const LcSplitDelimRegexSlsCfg& c, const uint8_t* src,
+                                             const LcDelimRegexSlsRow& r, S& s) {
+    LcSplitDelimRegexStage x{{{}, c.r, src, r, lc_delim_regex_value(c.r, r.d.status, r.d.nf) != LC_DR_ABSENT,
+                              lc_regex_sls_verdict(c.r.x, r.status) == 0u, 0u},
+                             {{}, c.s, c.s.src_pos + r.d.eo}};
+    const uint32_t n = lc_delim_sls_body(c.r.d, src, r.d, s, x);
+    if (!x.present)
+        return n;
+    // A present value means the delimiter stage kept the row, so the slot holds the offset content whenever there is
+    // one; a failed regex stage without KeepingSourceWhenParseFail appends nothing.
+    const uint32_t left = n - 1 + x.m;
+    return left == 1 && c.s.has_offset && !x.ok && !c.r.x.keep_fail ? 0u : left;
+}
+
+// The piece's counter verdicts: lc_delim_regex_verdict's 8, with cnt = lc_split_delim_regex_sls_body's result.
+LC_HD LcDelimRegexVerdict lc_split_delim_regex_verdict(const LcSplitDelimRegexSlsCfg& c, const LcDelimRegexSlsRow& r,
+                                                       uint32_t cnt) {
+    return lc_delim_regex_verdict(c.r, r, cnt);
+}
+
+// Host side: the chain's checks and fields, after lc_delim_sls_setup (c->r.d) and lc_regex_sls_setup (c->r.x, SourceKey
+// = rsrc) accepted their halves: lc_split_delim_sls_link, then an offset key equal to the regex SourceKey is refused,
+// then lc_delim_regex_sls_link with the offset content as one more content the delimiter stage leaves besides key k
+// (which also puts the offset key under its "_time_" / "_source_" rule).  Returns nullptr, or why the chain is refused.
+inline const char* lc_split_delim_regex_sls_link(const char* const* dkeys, const uint32_t* dkey_lens,
+                                                 const char* dsrc, uint32_t dsrc_len, const char* dren,
+                                                 uint32_t dren_len, const char* const* rkeys,
+                                                 const uint32_t* rkey_lens, uint32_t rnkeys, const char* rsrc,
+                                                 uint32_t rsrc_len, const char* rren, uint32_t rren_len,
+                                                 int rkeep_fail, int rkeep_succeed, int rcopy_raw, int rwhole_line,
+                                                 const char* offset_key, uint32_t offset_len, uint64_t src_pos,
+                                                 uint32_t time, uint32_t time_ns, LcSplitDelimRegexSlsCfg* c) {
+    const char* why = lc_split_delim_sls_link(c->r.d, dkeys, dkey_lens, dsrc, dsrc_len, dren, dren_len, offset_key,
+                                              offset_len, src_pos, time, time_ns, &c->s);
+    if (why)
+        return why;
+    if (offset_key && offset_len == rsrc_len && (rsrc_len == 0 || !memcmp(offset_key, rsrc, rsrc_len)))
+        return "the offset key equals the regex SourceKey";
+    return lc_delim_regex_sls_link(c->r.d, dkeys, dkey_lens, dsrc, dsrc_len, dren, dren_len, rkeys, rkey_lens, rnkeys,
+                                   rsrc, rsrc_len, rren, rren_len, rkeep_fail, rkeep_succeed, rcopy_raw, rwhole_line,
+                                   &c->r, offset_key, offset_len);
 }
 
 // ------------------------------------------------------------------------------------------------------------

@@ -4049,6 +4049,84 @@ void launch_split_delim_sls_emit(const LcSplitDelimSlsCfg& c, const DelimSlsTabl
                                                                                        d_out);
 }
 
+// ---- f4, split -> delimiter -> regex chain: Log records of the pieces a splitter cut, a ProcessorParseDelimiterNative
+// parsed and a ProcessorParseRegexNative parsed one column of (lc_exec.cuh: lc_split_delim_regex_sls_body), from the
+// piece, delimiter, value and regex tables -- the size pass one thread per piece, the emit pass one warp per piece.
+// counters: u64 [9] += lc_delim_regex_verdict's 8, pieces whose record would reach 4 GiB (their size is left 0 and the
+// call is refused).
+__device__ __forceinline__ LcDelimRegexSlsRow split_delim_regex_sls_row(const LcSplitDelimRegexSlsCfg& c,
+                                                                        const DelimRegexSlsTables& t, uint64_t i) {
+    LcDelimRegexSlsRow r;
+    r.d = split_delim_sls_row(c.s, t.d, i);
+    r.vo = t.val_off[i];
+    r.vl = t.val_len[i];
+    r.status = t.status ? t.status[i] : 0u;
+    r.co = t.cap_off ? t.cap_off + i * c.r.x.pitch : nullptr;
+    r.cl = t.cap_len ? t.cap_len + i * c.r.x.pitch : nullptr;
+    return r;
+}
+
+__global__ void __launch_bounds__(256)
+    split_delim_regex_sls_size_kernel(LcSplitDelimRegexSlsCfg c, DelimRegexSlsTables t, uint64_t n,
+                                      uint32_t* __restrict__ rec_size, uint32_t* __restrict__ body_size,
+                                      unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    LcDelimRegexVerdict v = {};
+    uint32_t big = 0;
+    if (i < n) {
+        const LcDelimRegexSlsRow r = split_delim_regex_sls_row(c, t, i);
+        LcSlsCount64 s{0};
+        const uint32_t cnt = lc_split_delim_regex_sls_body(c, t.d.base, r, s);
+        big = s.n + 16 > 0xFFFFFFFFull;
+        const uint32_t body = cnt && !big ? (uint32_t)s.n : 0u;
+        rec_size[i] = body ? 1 + lc_varint_size(body) + body : 0u;
+        body_size[i] = body;
+        v = lc_split_delim_regex_verdict(c, r, cnt);
+    }
+    // one atomic per warp and counter
+#pragma unroll
+    for (int k = 0; k < 9; ++k) {
+        const uint32_t w = __reduce_add_sync(0xFFFFFFFFu, k < 8 ? v.ctr[k] : big);
+        if ((threadIdx.x & 31) == 0 && w)
+            atomicAdd(counters + k, (unsigned long long)w);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    split_delim_regex_sls_emit_kernel(LcSplitDelimRegexSlsCfg c, DelimRegexSlsTables t, uint64_t n,
+                                      const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ body_size,
+                                      uint8_t* __restrict__ out) {
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n)
+        return;
+    const uint32_t body = body_size[i];
+    if (!body)
+        return; // erased: no record
+    const LcDelimRegexSlsRow r = split_delim_regex_sls_row(c, t, i);
+    uint8_t h[6];
+    h[0] = 0x0A;
+    const uint32_t hn = 1 + lc_put_varint(h + 1, body);
+    LcSlsWrite s{out + rec_off[i], 0u, hn + body, threadIdx.x & 31, 32};
+    s.put(h, hn);
+    lc_split_delim_regex_sls_body(c, t.d.base, r, s);
+}
+
+void launch_split_delim_regex_sls_sizes(const LcSplitDelimRegexSlsCfg& c, const DelimRegexSlsTables& t, uint64_t n,
+                                        uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                        cudaStream_t st) {
+    if (n)
+        split_delim_regex_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_size,
+                                                                                        d_body_size, d_counters);
+}
+
+void launch_split_delim_regex_sls_emit(const LcSplitDelimRegexSlsCfg& c, const DelimRegexSlsTables& t, uint64_t n,
+                                       const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                       cudaStream_t st) {
+    if (n)
+        split_delim_regex_sls_emit_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_off,
+                                                                                             d_body_size, d_out);
+}
+
 // ---- f4, split-fed: Log records of the pieces a splitter cuts from one source value (lc_exec.cuh: lc_span_sls_rec,
 // lc_span_sls_tile).  The size pass runs one thread per piece; the emit pass one warp per kSpanTile bytes of OUTPUT,
 // so records of 0 B and of many MiB share a launch without one warp copying a whole long record.

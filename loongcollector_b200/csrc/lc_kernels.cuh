@@ -10,6 +10,7 @@ struct LcDelimRegexSlsCfg;
 struct LcSpanSlsCfg;
 struct LcSplitRegexSlsCfg;
 struct LcSplitDelimSlsCfg;
+struct LcSplitDelimRegexSlsCfg;
 struct LcFilterSlsCfg;
 struct LcLz4Seq;
 struct LcLz4Chunk;
@@ -298,6 +299,17 @@ void launch_split_delim_sls_sizes(const LcSplitDelimSlsCfg& c, const DelimSlsTab
 void launch_split_delim_sls_emit(const LcSplitDelimSlsCfg& c, const DelimSlsTables& t, uint64_t n,
                                  const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
                                  cudaStream_t st);
+
+// f4, split -> delimiter -> regex chain (lc_exec.cuh: LcSplitDelimRegexSlsCfg): the sizes and emit passes over the
+// piece tables (t.d.ev_off / t.d.ev_len over t.d.base = the source value, with its side copies), the delimiter tables
+// over them, the value table of the tap and the regex tables over the values; d_counters: u64 [9] +=
+// lc_delim_regex_verdict's 8, pieces whose record would reach 4 GiB.
+void launch_split_delim_regex_sls_sizes(const LcSplitDelimRegexSlsCfg& c, const DelimRegexSlsTables& t, uint64_t n,
+                                        uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                        cudaStream_t st);
+void launch_split_delim_regex_sls_emit(const LcSplitDelimRegexSlsCfg& c, const DelimRegexSlsTables& t, uint64_t n,
+                                       const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                       cudaStream_t st);
 
 // f4, split-fed: Log records of the pieces of one source value (lc_exec.cuh: LcSpanSlsCfg, keys on the device).
 // rec_size[k] = bytes of piece k's record (never 0); the emit pass writes the `total` bytes from the record offsets,

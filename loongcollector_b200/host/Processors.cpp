@@ -1974,11 +1974,11 @@ bool RunSlsLz4DevicePass(Call call, size_t estimate, const SLSEventGroupSerializ
 // the records are concatenated in event order; counters[3] += the ctr of each source event's last call.  The records
 // are what CreateNewEvent builds (ProcessorSplitLogStringNative.cpp:131-161): RAW events serialise as "content" ->
 // piece; LOG events as SourceKey -> piece plus, with log.file.offset metadata, that key -> the piece's file offset.
-// An empty value emits nothing.  counters[3..6) are a chained regex stage's (successful, failed, discarded),
-// counters[6] the events a filter behind it removed.
-template <class Call>
+// An empty value emits nothing.  counters[3..N) are a chained stage's as SplitRegexChainSls lays them out: counters[5]
+// + counters[6] are the events it erased or a filter behind it removed.
+template <size_t N, class Call>
 bool SplitSerializeSls(PipelineEventGroup& group, bool enableNs, const std::string& sourceKey, bool raw, Call call,
-                       const char* what, std::string& out, std::string& err, uint64_t counters[7]) {
+                       const char* what, std::string& out, std::string& err, uint64_t (&counters)[N]) {
     SLSEventGroupSerializer ser;
     ser.mEnableTimestampNanosecond = enableNs;
     static const std::string kRawKey = "content"; // DEFAULT_CONTENT_KEY (SLSSerializer.cpp:366-374)
@@ -1998,7 +1998,7 @@ bool SplitSerializeSls(PipelineEventGroup& group, bool enableNs, const std::stri
             continue;
         const uint32_t ns =
             enableNs && src.GetTimestampNanosecond() ? src.GetTimestampNanosecond().value() : LC_SLS_NO_NS;
-        uint64_t need = 0, nev = 0, ctr[7];
+        uint64_t need = 0, nev = 0, ctr[N];
         RunSlsDevicePass(
             [&](uint8_t* o, uint64_t cap, uint64_t* len) {
                 memset(ctr, 0, sizeof ctr); // (a second, exactly sized call must not count the lines twice)
@@ -2011,7 +2011,7 @@ bool SplitSerializeSls(PipelineEventGroup& group, bool enableNs, const std::stri
         // (else the group is over the size limit: the sizes still add up for the error message)
         total += need;
         nEvents += nev;
-        for (int k = 0; k < 7; ++k)
+        for (size_t k = 0; k < N; ++k)
             counters[k] += ctr[k];
     }
     return FinishSls(ser, nEvents, counters[5] + counters[6], total, res, tail, out, err);
@@ -2122,11 +2122,93 @@ struct SplitDelimStage {
         (x).Renamed().data(), (uint32_t)(x).Renamed().size(), (x).Opt().mKeepingSourceWhenParseFail,                    \
         (x).Opt().mKeepingSourceWhenParseSucceed, (x).Opt().mCopingRawLog
 
+// The delimiter and regex stages of the split -> delimiter -> regex chain: the delimiter stage as SplitDelimStage has
+// it, the regex stage's configuration as the chain calls take it (SPLIT_DELIM_REGEX_STAGE_ARGS), the host checks of
+// lc_delim_sls_setup + lc_regex_sls_setup + lc_split_delim_regex_sls_link, and the counters both Process calls would
+// move.
+struct SplitDelimRegexStage {
+    SplitDelimStage d;
+    ProcessorParseRegexNative& r;
+    std::vector<const char*> kp;
+    std::vector<uint32_t> kl;
+    const lc_regex_t* re;
+    bool wholeLine;
+    SplitDelimRegexStage(ProcessorParseDelimiterNative& delim, ProcessorParseRegexNative& regex)
+        : d(delim), r(regex), re(regex.mIsWholeLineMode ? nullptr : regex.mReg.get()),
+          wholeLine(regex.mIsWholeLineMode) {
+        for (const auto& k : r.mKeys) {
+            kp.push_back(k.data());
+            kl.push_back((uint32_t)k.size());
+        }
+    }
+    const std::string& Renamed() const { return r.mCommonParserOptions.mRenamedSourceKey; }
+    const CommonParserOptions& Opt() const { return r.mCommonParserOptions; }
+    // whether the chain's device calls take both stages behind a splitter reading sourceKey
+    bool Accepts(const std::string& sourceKey, const StringView* okey) const {
+        const ProcessorParseDelimiterNative& p = d.d;
+        if (!p.mDeviceSls || p.mSourceKey != sourceKey)
+            return false;
+        size_t keyBytes = p.mSourceKey.size() + d.Renamed().size() + 12;
+        for (const auto& k : p.mKeys)
+            keyBytes += k.size();
+        std::vector<uint8_t> kb(keyBytes);
+        std::vector<uint32_t> at(p.mKeys.size() + 4), plan(3 * r.mKeys.size() + 12);
+        LcSplitDelimRegexSlsCfg c;
+        memset(&c, 0, sizeof c);
+        return !lc_delim_sls_setup(d.Sep(), (uint32_t)p.mSeparator.size(), (uint8_t)p.mQuote, d.Extend(),
+                                   p.mExtractingPartialFields, d.kp.data(), d.kl.data(), (uint32_t)d.kp.size(),
+                                   p.mSourceKey.data(), (uint32_t)p.mSourceKey.size(), d.Renamed().data(),
+                                   (uint32_t)d.Renamed().size(), d.Opt().mKeepingSourceWhenParseFail,
+                                   d.Opt().mKeepingSourceWhenParseSucceed, d.Opt().mCopingRawLog, d.MaxFields(),
+                                   &c.r.d, kb.data(), at.data()) &&
+               !lc_regex_sls_setup(kp.data(), kl.data(), (uint32_t)kp.size(), r.mSourceKey.data(),
+                                   (uint32_t)r.mSourceKey.size(), Renamed().data(), (uint32_t)Renamed().size(),
+                                   Opt().mKeepingSourceWhenParseFail, Opt().mKeepingSourceWhenParseSucceed,
+                                   Opt().mCopingRawLog, wholeLine, 0, &c.r.x, plan.data()) &&
+               !lc_split_delim_regex_sls_link(
+                   d.kp.data(), d.kl.data(), p.mSourceKey.data(), (uint32_t)p.mSourceKey.size(), d.Renamed().data(),
+                   (uint32_t)d.Renamed().size(), kp.data(), kl.data(), (uint32_t)kp.size(), r.mSourceKey.data(),
+                   (uint32_t)r.mSourceKey.size(), Renamed().data(), (uint32_t)Renamed().size(),
+                   Opt().mKeepingSourceWhenParseFail, Opt().mKeepingSourceWhenParseSucceed, Opt().mCopingRawLog,
+                   wholeLine, okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, 0, 0, LC_SLS_NO_NS,
+                   &c);
+    }
+    // the device calls' counters[8] as the chain driver takes a stage's: the delimiter's successful, out_failed (a
+    // blank value counts as failed, :220-242) and discarded, the regex stage's discarded (so that [2] + [3] are the
+    // events the chain erased), successful, out_failed and out_key_not_found
+    static void Fold(const uint64_t c8[8], uint64_t rctr[8]) {
+        const uint64_t f[8] = {c8[0], c8[1] + c8[3], c8[2], c8[7], c8[4], c8[5], c8[6], 0};
+        memcpy(rctr, f, sizeof f);
+    }
+    void Add(const uint64_t ctr[7]) const {
+        d.Add(ctr);
+        r.mDiscardedEventsTotal.Add(ctr[3]);
+        r.mOutSuccessfulEventsTotal.Add(ctr[4]);
+        r.mOutFailedEventsTotal.Add(ctr[5]);
+        r.mOutKeyNotFoundEventsTotal.Add(ctr[6]);
+    }
+    void Process(PipelineEventGroup& group) const {
+        d.Process(group);
+        r.Process(group);
+    }
+};
+// the chain calls' arguments after the source value and the splitter's: allow_short, max_fields, then both stages'
+#define SPLIT_DELIM_REGEX_STAGE_ARGS(x)                                                                                \
+    (x).d.d.mAllowingShortenedFields, (x).d.MaxFields(), (x).d.Sep(), (uint32_t)(x).d.d.mSeparator.size(),             \
+        (uint8_t)(x).d.d.mQuote, (x).d.Extend(), (x).d.d.mExtractingPartialFields, (x).d.kp.data(), (x).d.kl.data(),   \
+        (uint32_t)(x).d.kp.size(), (x).d.d.mSourceKey.data(), (uint32_t)(x).d.d.mSourceKey.size(),                     \
+        (x).d.Renamed().data(), (uint32_t)(x).d.Renamed().size(), (x).d.Opt().mKeepingSourceWhenParseFail,              \
+        (x).d.Opt().mKeepingSourceWhenParseSucceed, (x).d.Opt().mCopingRawLog, (x).kp.data(), (x).kl.data(),          \
+        (uint32_t)(x).kp.size(), (x).r.mSourceKey.data(), (uint32_t)(x).r.mSourceKey.size(), (x).Renamed().data(),     \
+        (uint32_t)(x).Renamed().size(), (x).Opt().mKeepingSourceWhenParseFail,                                          \
+        (x).Opt().mKeepingSourceWhenParseSucceed, (x).Opt().mCopingRawLog, (x).wholeLine
+
 namespace {
-// The split -> parse chain of either splitter, with the parse stage x (SplitRegexStage, SplitDelimStage):
-// `process(group)` is the splitter's Process; the device calls are sls(val, okey, pos, time, ns, out, cap, &len, &nev,
-// rctr, sctr) and lz4(val, okey, pos, time, ns, tail, tailLen, out, cap, &len, &raw, &nev, rctr, sctr) (rctr[4] = the
-// stage's counters as x.Add takes them and the events a filter removed, sctr[3] = the splitter's).  filter (or
+// The split -> parse chain of either splitter, with the parse stage x (SplitRegexStage, SplitDelimStage,
+// SplitDelimRegexStage): `process(group)` is the splitter's Process; the device calls are sls(val, okey, pos, time, ns,
+// out, cap, &len, &nev, rctr, sctr) and lz4(val, okey, pos, time, ns, tail, tailLen, out, cap, &len, &raw, &nev, rctr,
+// sctr) (rctr[8] = the stage's counters as x.Add takes them, rctr[2] + rctr[3] = the events it erased or a filter
+// behind it removed; sctr[3] = the splitter's).  filter (or
 // nullptr): the filter behind the regex stage, whose rule the device calls take when filterOk.  sctr_total[3] += the
 // splitter's counters of every device call.  rawSize null: out = the wire bytes; else out = their LZ4 block and
 // *rawSize their size.
@@ -2161,7 +2243,7 @@ bool SplitRegexChainSls(PipelineEventGroup& group, const Stage& x, ProcessorFilt
         const uint32_t ns =
             enableNs && src.GetTimestampNanosecond() ? src.GetTimestampNanosecond().value() : LC_SLS_NO_NS;
         const std::string tail = SlsGroupTail(group);
-        uint64_t nev = 0, gone = 0, rctr[4] = {0, 0, 0, 0}, sctr[3] = {0, 0, 0};
+        uint64_t nev = 0, gone = 0, rctr[8] = {0, 0, 0, 0, 0, 0, 0, 0}, sctr[3] = {0, 0, 0};
         const bool ok = RunSlsLz4DevicePass(
             [&](uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw) {
                 memset(rctr, 0, sizeof rctr);
@@ -2169,7 +2251,7 @@ bool SplitRegexChainSls(PipelineEventGroup& group, const Stage& x, ProcessorFilt
                 const int rc = lz4(val, okp, src.GetPosition().first, (uint32_t)src.GetTimestamp(), ns,
                                    reinterpret_cast<const uint8_t*>(tail.data()), (uint64_t)tail.size(), o, cap, len,
                                    raw, &nev, rctr, sctr);
-                gone = rctr[2] + rctr[3]; // erased by the regex stage or removed by the filter
+                gone = rctr[2] + rctr[3]; // erased by the stage or removed by the filter
                 return rc;
             },
             2 * val.size() + 4096 + tail.size(), ser, nev, gone, tail.size(), out, *rawSize, err, lzwhat);
@@ -2182,7 +2264,7 @@ bool SplitRegexChainSls(PipelineEventGroup& group, const Stage& x, ProcessorFilt
                     uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* ctr) {
         return sls(val, ok, pos, time, ns, o, cap, len, nev, ctr + 3, ctr);
     };
-    uint64_t ctr[7] = {0, 0, 0, 0, 0, 0, 0};
+    uint64_t ctr[11] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     std::string raw;
     const bool ok = SplitSerializeSls(group, enableNs, sourceKey, false, call, what, rawSize ? raw : out, err, ctr);
     x.Add(ctr + 3);
@@ -2566,6 +2648,105 @@ bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGrou
         group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
         [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_multiline_split_delim_parse_sls",
         "lc_multiline_split_delim_parse_sls_lz4", ctr);
+    mMatchedEventsTotal.Add(ctr[0]);
+    mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
+    mUnmatchedLinesTotal.Add(ctr[2]);
+    return ok;
+}
+
+bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                                                 ProcessorParseRegexNative& regex, bool enableNs, std::string& out,
+                                                 std::string& err) {
+    return ChainSerializeSls(group, next, regex, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                                                    ProcessorParseRegexNative& regex, bool enableNs,
+                                                    std::string& block, uint64_t& rawSize, std::string& err) {
+    return ChainSerializeSls(group, next, regex, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitLogStringNative::ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                                                      ProcessorParseRegexNative& regex, bool enableNs,
+                                                      std::string& out, uint64_t* rawSize, std::string& err) {
+    const SplitDelimRegexStage x(next, regex);
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_split_delim_regex_parse_sls(Engine(), x.re, src(val), val.size(), (uint8_t)mSplitChar,
+                                                      SPLIT_DELIM_REGEX_STAGE_ARGS(x), okey ? okey->data() : nullptr,
+                                                      okey ? (uint32_t)okey->size() : 0u, pos, time, ns, o, cap, len,
+                                                      nev, c8);
+        SplitDelimRegexStage::Fold(c8, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_split_delim_regex_parse_sls_lz4(
+            Engine(), x.re, src(val), val.size(), (uint8_t)mSplitChar, SPLIT_DELIM_REGEX_STAGE_ARGS(x),
+            okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos, time, ns, tail, tailLen, o, cap,
+            len, raw, nev, c8);
+        SplitDelimRegexStage::Fold(c8, rctr);
+        return rc;
+    };
+    uint64_t unused[3] = {0, 0, 0};
+    return SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_split_delim_regex_parse_sls",
+        "lc_split_delim_regex_parse_sls_lz4", unused);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& group,
+                                                          ProcessorParseDelimiterNative& next,
+                                                          ProcessorParseRegexNative& regex, bool enableNs,
+                                                          std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, regex, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSlsLz4(PipelineEventGroup& group,
+                                                             ProcessorParseDelimiterNative& next,
+                                                             ProcessorParseRegexNative& regex, bool enableNs,
+                                                             std::string& block, uint64_t& rawSize, std::string& err) {
+    return ChainSerializeSls(group, next, regex, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGroup& group,
+                                                               ProcessorParseDelimiterNative& next,
+                                                               ProcessorParseRegexNative& regex, bool enableNs,
+                                                               std::string& out, uint64_t* rawSize, std::string& err) {
+    const SplitDelimRegexStage x(next, regex);
+    const bool discard = mMultiline.mUnmatchedContentTreatment == MultilineOptions::UnmatchedContentTreatment::DISCARD;
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_multiline_split_delim_regex_parse_sls(
+            Engine(), x.re, src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
+            SPLIT_DELIM_REGEX_STAGE_ARGS(x), okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos,
+            time, ns, o, cap, len, nev, c8, sctr);
+        SplitDelimRegexStage::Fold(c8, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_multiline_split_delim_regex_parse_sls_lz4(
+            Engine(), x.re, src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
+            SPLIT_DELIM_REGEX_STAGE_ARGS(x), okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos,
+            time, ns, tail, tailLen, o, cap, len, raw, nev, c8, sctr);
+        SplitDelimRegexStage::Fold(c8, rctr);
+        return rc;
+    };
+    // matched_events, input lines, unmatched lines: moved as Process moves them (:82-84,106-107)
+    uint64_t ctr[3] = {0, 0, 0};
+    const bool ok = SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_multiline_split_delim_regex_parse_sls",
+        "lc_multiline_split_delim_regex_parse_sls_lz4", ctr);
     mMatchedEventsTotal.Add(ctr[0]);
     mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
     mUnmatchedLinesTotal.Add(ctr[2]);

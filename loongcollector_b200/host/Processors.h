@@ -163,6 +163,20 @@ public:
     // device (lc_split_delim_parse_sls_lz4); other groups compress SerializeSls's bytes.
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
                          std::string& block, uint64_t& rawSize, std::string& err);
+    // The split -> delimiter -> regex chain: Process(group), next.Process(group), regex.Process(group) (regex reading
+    // one of next's keys), then SLSEventGroupSerializer::Serialize: the same bytes or error message, and the same
+    // counter updates on all three processors.  On a flat group without EnableRawContent, whose delimiter SourceKey is
+    // this SourceKey, whose regex SourceKey is one of the delimiter's keys and whose configuration
+    // lc_split_delim_regex_parse_sls accepts, each source event is split, parsed by both stages and serialised in one
+    // device pass (log.file.offset metadata included) and only the wire bytes come back; the group's events are left as
+    // they were.  Otherwise the four calls run.
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, ProcessorParseRegexNative& regex,
+                      bool enableNs, std::string& out, std::string& err);
+    // The same followed by LZ4Compressor::Compress.  A device-path group of one source event is compressed on the
+    // device (lc_split_delim_regex_parse_sls_lz4); other groups compress SerializeSls's bytes.
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                         ProcessorParseRegexNative& regex, bool enableNs, std::string& block, uint64_t& rawSize,
+                         std::string& err);
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
@@ -172,6 +186,9 @@ private:
                            bool enableNs, std::string& out, uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
                            std::string& out, uint64_t* rawSize, std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                           ProcessorParseRegexNative& regex, bool enableNs, std::string& out, uint64_t* rawSize,
+                           std::string& err);
 };
 
 class ProcessorSplitMultilineLogStringNative : public Processor {
@@ -206,6 +223,13 @@ public:
                       std::string& err);
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
                          std::string& block, uint64_t& rawSize, std::string& err);
+    // The split -> delimiter -> regex chain, as ProcessorSplitLogStringNative's
+    // (lc_multiline_split_delim_regex_parse_sls[_lz4]).
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, ProcessorParseRegexNative& regex,
+                      bool enableNs, std::string& out, std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                         ProcessorParseRegexNative& regex, bool enableNs, std::string& block, uint64_t& rawSize,
+                         std::string& err);
     Counter mMatchedEventsTotal, mMatchedLinesTotal, mUnmatchedLinesTotal;
 
 protected:
@@ -216,6 +240,9 @@ private:
                            bool enableNs, std::string& out, uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
                            std::string& out, uint64_t* rawSize, std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                           ProcessorParseRegexNative& regex, bool enableNs, std::string& out, uint64_t* rawSize,
+                           std::string& err);
     CompiledRegex mStart, mContinue, mEnd;
 };
 
@@ -274,6 +301,7 @@ private:
     void AddCounters(const LocalCounters& c);
     friend class ProcessorParseDelimiterNative; // the delimiter -> regex chain's SerializeSls
     friend struct SplitRegexStage;              // the split -> regex chain's
+    friend struct SplitDelimRegexStage;         // the split -> delimiter -> regex chain's
     bool mSourceKeyOverwritten = false;
     bool mIsWholeLineMode = false;
     bool mKeysDistinct = false; // no key repeats: an event that holds only the source key takes the parsed fields as
@@ -331,7 +359,8 @@ private:
                           std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, bool enableNs,
                            std::string& out, uint64_t* rawSize, std::string& err);
-    friend struct SplitDelimStage; // the split -> delimiter chain's SerializeSls
+    friend struct SplitDelimStage;      // the split -> delimiter chain's SerializeSls
+    friend struct SplitDelimRegexStage; // the split -> delimiter -> regex chain's
     bool mSourceKeyOverwritten = false;
     bool mDeviceSls = false; // the configuration passes lc_delim_parse_sls's checks
 };

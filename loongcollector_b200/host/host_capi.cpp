@@ -313,38 +313,47 @@ char* lc_host_chain3_serialize_sls(lc_host_processor_t* split, lc_host_processor
     if (raw_len_out)
         *raw_len_out = 0;
     try {
+        // (splitter, regex, filter) or (splitter, delimiter, regex)
         Processor* d = split->proc.get();
-        auto* r = dynamic_cast<ProcessorParseRegexNative*>(regex->proc.get());
-        auto* f = dynamic_cast<ProcessorFilterNative*>(filter->proc.get());
+        Processor* b = regex->proc.get();
+        Processor* c = filter->proc.get();
+        auto* r = dynamic_cast<ProcessorParseRegexNative*>(b);
+        auto* f = dynamic_cast<ProcessorFilterNative*>(c);
+        auto* dl = dynamic_cast<ProcessorParseDelimiterNative*>(b);
+        auto* dr = dynamic_cast<ProcessorParseRegexNative*>(c);
         auto* ps = dynamic_cast<ProcessorSplitLogStringNative*>(d);
         auto* pm = dynamic_cast<ProcessorSplitMultilineLogStringNative*>(d);
-        if (!(ps || pm) || !r || !f)
-            throw std::runtime_error("not a splitter, a processor_parse_regex_native and a "
-                                     "processor_filter_regex_native");
+        if (!(ps || pm) || !((r && f) || (dl && dr)))
+            throw std::runtime_error("not a splitter followed by a processor_parse_regex_native and a "
+                                     "processor_filter_regex_native, or by a processor_parse_delimiter_native and a "
+                                     "processor_parse_regex_native");
         auto chain = [&](auto* p, PipelineEventGroup& g, std::string& res, uint64_t& raw, std::string& err) {
+            if (dl)
+                return mode == 2 ? p->SerializeSlsLz4(g, *dl, *dr, enable_ns != 0, res, raw, err)
+                                 : p->SerializeSls(g, *dl, *dr, enable_ns != 0, res, err);
             return mode == 2 ? p->SerializeSlsLz4(g, *r, *f, enable_ns != 0, res, raw, err)
                              : p->SerializeSls(g, *r, *f, enable_ns != 0, res, err);
         };
         PipelineEventGroup group(std::make_shared<SourceBuffer>());
         if (!group.FromJsonString(group_json ? group_json : "null"))
             throw std::runtime_error("group JSON does not parse");
-        const uint64_t errs = d->EngineErrors() + r->EngineErrors() + f->EngineErrors();
+        const uint64_t errs = d->EngineErrors() + b->EngineErrors() + c->EngineErrors();
         std::string res, err;
         uint64_t raw = 0;
         bool ok;
         if (mode == 1) {
             d->Process(group);
-            r->Process(group);
-            f->Process(group);
+            b->Process(group);
+            c->Process(group);
             SLSEventGroupSerializer ser;
             ser.mEnableTimestampNanosecond = enable_ns != 0;
             ok = ser.Serialize(group, res, err);
         } else {
             ok = ps ? chain(ps, group, res, raw, err) : chain(pm, group, res, raw, err);
         }
-        if (d->EngineErrors() + r->EngineErrors() + f->EngineErrors() != errs)
-            throw std::runtime_error("engine error inside Process: " + d->LastError() + r->LastError() +
-                                     f->LastError());
+        if (d->EngineErrors() + b->EngineErrors() + c->EngineErrors() != errs)
+            throw std::runtime_error("engine error inside Process: " + d->LastError() + b->LastError() +
+                                     c->LastError());
         if (!ok) {
             if (err_out)
                 *err_out = dup(err);
