@@ -833,6 +833,54 @@ int lc_zstd_compress_dev(lc_engine_t* e, const uint8_t* d_in, uint64_t nseg, con
 int lc_zstd_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_ptr, const uint32_t* seg_len,
                      uint8_t* out, uint64_t out_cap, uint64_t* frm_off, uint32_t* frm_len, uint64_t* out_len);
 
+/* ---- ProcessorParseTimestampNative (ProcessorParseTimestampNative.cpp:100-235, Strptime TimeUtil.cpp:112-160,
+ *      strptime_ns Strptime.cpp)
+ * lc_timestamp_compile is Init: SourceFormat becomes a device program; source_year is SourceYear (-1 unset, 0 deduce
+ * the year from "now" as DeduceYear does, > 0 that year); tz_adjust is mLogTimeZoneOffsetSecond (SourceTimezone's
+ * offset minus the local one, ParseLogTimeZoneOffsetSecond), subtracted after every successful full parse.  The
+ * process's local zone is probed with mktime here (a per-year table of its standard and daylight offsets), so the
+ * kernels need no tzdata; compile again after the zone changes.  Refused with LC_ERR_INVALID_ARG (message in
+ * lc_last_error): %c, %x and %X (the locale's formats), a NUL byte inside the format, and a format of more than 96
+ * directives and literal bytes.  Every other strptime_ns directive runs as the reference runs it: %Z consumes GMT or
+ * UTC and nothing else; unknown conversions and %s inside a longer format fail every value.
+ *
+ * lc_timestamp_parse[_dev]: event i's value is base[ev_off[i], + ev_len[i]); ev_len[i] == LC_TS_NO_KEY means the
+ * event has no SourceKey.  Events [grp[g], grp[g + 1]) form group g (grp has ngroups + 1 entries, grp[0] = 0 and
+ * grp[ngroups] = n); ParseLogTime's second-level cache starts empty in every group and events keep their order in it.
+ * now is time(NULL) of the call (the reference reads it per event); discard_interval >= 0 discards an event whose time
+ * is more than that many seconds behind now (ilogtail_discard_old_data with ilogtail_discard_interval, 43200 by default;
+ * pass -1 for one-time pipelines or with the flag off); a time <= 0 is always discarded.
+ * Per event: status[i] as LC_TS_*; sec[i] / nsec[i] the time the event gets (SetTimestamp) for LC_TS_OK and the one
+ * it would have got for LC_TS_DISCARDED, 0 for the other statuses.  counters[5] = key_not_found, out_failed, history_failure, discarded,
+ * out_successful.  A value is read over [off, off + len) followed by NUL bytes: the reference hands strptime a
+ * StringView that need not be terminated, so the two agree whenever the value is terminated.
+ * The _dev calls take device tables and write d_counters (u64[5], device) without waiting for the device; the first
+ * call of a compiled format on an engine also uploads its program from host memory. */
+#define LC_TS_OK 0
+#define LC_TS_NOT_FOUND 1  /* no SourceKey: out_key_not_found++, event kept */
+#define LC_TS_FAILED 2     /* parse failure: out_failed++, event kept with its time unchanged */
+#define LC_TS_DISCARDED 3  /* time <= 0 or too old: history_failure++, discarded++, event erased */
+#define LC_TS_NO_KEY 0xFFFFFFFFu
+typedef struct lc_timestamp lc_timestamp_t;
+int lc_timestamp_compile(const char* format, size_t len, int32_t source_year, int32_t tz_adjust,
+                         lc_timestamp_t** out);
+void lc_timestamp_free(lc_timestamp_t* t);
+int lc_timestamp_parse(lc_engine_t* e, const lc_timestamp_t* ts, const uint8_t* base, uint64_t base_len,
+                       const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* grp,
+                       uint64_t ngroups, int64_t now, int32_t discard_interval, int64_t* sec, uint32_t* nsec,
+                       uint8_t* status, uint64_t* counters);
+int lc_timestamp_parse_dev(lc_engine_t* e, const lc_timestamp_t* ts, const uint8_t* d_base, uint64_t base_len,
+                           const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, const uint32_t* d_grp,
+                           uint64_t ngroups, int64_t now, int32_t discard_interval, int64_t* d_sec, uint32_t* d_nsec,
+                           uint8_t* d_status, uint64_t* d_counters);
+/* The same over capture column k of one lc_regex_parse_dev result (d_rx_status, [n][row_pitch] d_cap_off / d_cap_len),
+ * read in place: a row the regex did not parse (status != LC_REGEX_OK) has no value (LC_TS_NOT_FOUND). */
+int lc_timestamp_parse_capture_dev(lc_engine_t* e, const lc_timestamp_t* ts, const uint8_t* d_base, uint64_t base_len,
+                                   const uint8_t* d_rx_status, const uint32_t* d_cap_off, const uint32_t* d_cap_len,
+                                   uint32_t row_pitch, uint32_t k, uint64_t n, const uint32_t* d_grp,
+                                   uint64_t ngroups, int64_t now, int32_t discard_interval, int64_t* d_sec,
+                                   uint32_t* d_nsec, uint8_t* d_status, uint64_t* d_counters);
+
 #ifdef __cplusplus
 }
 #endif

@@ -22,6 +22,11 @@ void lc_host_processor_destroy(lc_host_processor_t* p);
 /* Runs Processor::Process(PipelineEventGroup&) on the group described by group_json and returns the group's
  * ToJsonString(enable_event_meta) ("null" for an empty group) as a malloc'd string; NULL + *err_out on error. */
 char* lc_host_processor_process(lc_host_processor_t* p, const char* group_json, int enable_event_meta, char** err_out);
+/* Runs Processor::Process(std::vector<PipelineEventGroup>&) -- one call for all groups, as a pipeline hands them over
+ * -- on the JSON array of groups groups_json and returns the array of their ToJson(enable_event_meta) as a malloc'd
+ * string; NULL + *err_out on error. */
+char* lc_host_processor_process_groups(lc_host_processor_t* p, const char* groups_json, int enable_event_meta,
+                                       char** err_out);
 /* {"counter": value, ...} with the reference's counter meanings. */
 char* lc_host_processor_counters(const lc_host_processor_t* p);
 void lc_host_string_free(char* s);

@@ -99,6 +99,12 @@ def lib():
     L.lc_lz4_compress.argtypes = [vp, u64, vp, vp, vp, u64, vp, vp, C.POINTER(u64)]
     L.lc_zstd_compress_dev.argtypes = [vp, vp, u64, vp, vp, vp, u64, vp, vp, C.POINTER(u64)]
     L.lc_zstd_compress.argtypes = [vp, u64, vp, vp, vp, u64, vp, vp, C.POINTER(u64)]
+    L.lc_timestamp_compile.argtypes = [C.c_char_p, C.c_size_t, i32, i32, C.POINTER(vp)]
+    L.lc_timestamp_free.argtypes = [vp]
+    ts_tail = [vp, u64, C.c_int64, i32, vp, vp, vp, vp]  # grp .. counters
+    L.lc_timestamp_parse.argtypes = [vp, vp, vp, u64, vp, vp, u64] + ts_tail
+    L.lc_timestamp_parse_dev.argtypes = [vp, vp, vp, u64, vp, vp, u64] + ts_tail
+    L.lc_timestamp_parse_capture_dev.argtypes = [vp, vp, vp, u64, vp, vp, vp, u32, u32, u64] + ts_tail
     L.lc_delim_parse_sls_lz4.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32, u8, i32, i32, i32, u32] + \
         sls_cfg + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
     L.lc_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp] + sls_cfg + \
@@ -216,6 +222,35 @@ class Regex:
         try:
             if self._h:
                 lib().lc_regex_free(self._h)
+        except Exception:
+            pass
+
+
+LC_TS_OK, LC_TS_NOT_FOUND, LC_TS_FAILED, LC_TS_DISCARDED = 0, 1, 2, 3
+LC_TS_NO_KEY = 0xFFFFFFFF
+
+
+class Timestamp:
+    """Compiled SourceFormat of ProcessorParseTimestampNative (lc_timestamp_compile): SourceYear (-1 unset, 0 deduce,
+    > 0 that year) and the timezone adjustment (mLogTimeZoneOffsetSecond) are fixed here, and so is the process's
+    local zone."""
+
+    def __init__(self, fmt, source_year=-1, tz_adjust=0):
+        if isinstance(fmt, str):
+            fmt = fmt.encode("utf-8")
+        self.format = fmt
+        h = C.c_void_p()
+        L = lib()
+        rc = L.lc_timestamp_compile(fmt, len(fmt), int(source_year), int(tz_adjust), C.byref(h))
+        self._h = h
+        if rc != LC_OK:
+            self._h = None
+            raise LcError(rc, L.lc_last_error().decode())
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib().lc_timestamp_free(self._h)
         except Exception:
             pass
 
@@ -1153,6 +1188,34 @@ class Engine:
                                         C.byref(n)))
         return n.value
 
+    def timestamp_parse(self, ts, base, ev_off, ev_len, grp, now, discard_interval=43200):
+        """ProcessorParseTimestampNative over host buffers (lc_timestamp_parse): ev_len LC_TS_NO_KEY = no SourceKey,
+        grp = group starts plus n.  Returns (status u8, sec i64, nsec u32, counters u64[5])."""
+        a = _u8(base)
+        ev_off = np.ascontiguousarray(ev_off, np.uint32)
+        ev_len = np.ascontiguousarray(ev_len, np.uint32)
+        grp = np.ascontiguousarray(grp, np.uint32)
+        n = ev_off.size
+        st, sec, ns = np.empty(n, np.uint8), np.empty(n, np.int64), np.empty(n, np.uint32)
+        cnt = np.zeros(5, np.uint64)
+        _check(lib().lc_timestamp_parse(self._h, ts._h, _p(a), a.size, _p(ev_off), _p(ev_len), n, _p(grp),
+                                        max(grp.size - 1, 0), int(now), int(discard_interval), _p(sec), _p(ns),
+                                        _p(st), _p(cnt)))
+        return st, sec, ns, cnt
+
+    def timestamp_parse_dev(self, ts, d_base, base_len, d_ev_off, d_ev_len, n, d_grp, ngroups, now, discard_interval,
+                            d_sec, d_nsec, d_status, d_counters):
+        _check(lib().lc_timestamp_parse_dev(self._h, ts._h, _p(d_base), base_len, _p(d_ev_off), _p(d_ev_len), n,
+                                            _p(d_grp), ngroups, int(now), int(discard_interval), _p(d_sec), _p(d_nsec),
+                                            _p(d_status), _p(d_counters)))
+
+    def timestamp_parse_capture_dev(self, ts, d_base, base_len, d_rx_status, d_cap_off, d_cap_len, row_pitch, k, n,
+                                    d_grp, ngroups, now, discard_interval, d_sec, d_nsec, d_status, d_counters):
+        _check(lib().lc_timestamp_parse_capture_dev(self._h, ts._h, _p(d_base), base_len, _p(d_rx_status),
+                                                    _p(d_cap_off), _p(d_cap_len), row_pitch, k, n, _p(d_grp), ngroups,
+                                                    int(now), int(discard_interval), _p(d_sec), _p(d_nsec),
+                                                    _p(d_status), _p(d_counters)))
+
     def regex_parse_dev(self, rx, d_base, base_len, d_ev_off, d_ev_len, n, nkeys, d_status, d_cap_off, d_cap_len):
         _check(lib().lc_regex_parse_dev(self._h, rx._h, _p(d_base), base_len, _p(d_ev_off), _p(d_ev_len), n, nkeys,
                                         _p(d_status), _p(d_cap_off), _p(d_cap_len)))
@@ -1205,6 +1268,8 @@ class HostProcessor:
         L.lc_host_processor_destroy.argtypes = [C.c_void_p]
         L.lc_host_processor_process.restype = C.c_void_p
         L.lc_host_processor_process.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_void_p)]
+        L.lc_host_processor_process_groups.restype = C.c_void_p
+        L.lc_host_processor_process_groups.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.POINTER(C.c_void_p)]
         L.lc_host_processor_counters.restype = C.c_void_p
         L.lc_host_processor_counters.argtypes = [C.c_void_p]
         L.lc_host_string_free.argtypes = [C.c_void_p]
@@ -1224,6 +1289,22 @@ class HostProcessor:
         err = C.c_void_p()
         out = L.lc_host_processor_process(self._h, json.dumps(group).encode("utf-8"), int(enable_event_meta),
                                           C.byref(err))
+        if not out:
+            msg = C.string_at(err.value).decode() if err.value else "unknown error"
+            if err.value:
+                L.lc_host_string_free(err)
+            raise LcError(LC_ERR_CUDA, msg)
+        s = C.string_at(out).decode("utf-8")
+        L.lc_host_string_free(out)
+        return json.loads(s)
+
+    def process_groups(self, groups, enable_event_meta=True):
+        """Processor::Process(std::vector<PipelineEventGroup>&) on a list of groups in one call.  Returns the list."""
+        import json
+        L = lib()
+        err = C.c_void_p()
+        out = L.lc_host_processor_process_groups(self._h, json.dumps(groups).encode("utf-8"), int(enable_event_meta),
+                                                 C.byref(err))
         if not out:
             msg = C.string_at(err.value).decode() if err.value else "unknown error"
             if err.value:

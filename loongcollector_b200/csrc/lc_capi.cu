@@ -115,6 +115,10 @@ struct lc_engine {
     // split -> delimiter -> regex chain: the delimiter tables over the pieces (status, column counts, f_off, f_len,
     // f_dq) and the offset key; its value, regex and tap tables are the dr_* of the delimiter -> regex chain
     DevBuf sdr_status, sdr_nf, sdr_f_off, sdr_f_len, sdr_f_dq, sdr_okey;
+    // timestamp parse: the LcTsConf of the program ts_conf_id (uploaded on its first call here), the full-parse
+    // results, the host call's counters
+    DevBuf ts_conf, ts_full, ts_cnt;
+    uint64_t ts_conf_id = 0;
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
     std::unordered_map<uint64_t, void*> blobs; // regex id * 4 + layout -> device blob
@@ -331,7 +335,8 @@ void lc_engine_destroy(lc_engine_t* e) {
                       &e->zs_first, &e->zs_size, &e->zs_off, &e->zs_slot,
                       &e->dr_keys, &e->dr_val_off, &e->dr_val_len, &e->dr_status, &e->dr_cap_off, &e->dr_cap_len,
                       &e->dr_copy, &e->dr_slot, &e->dr_desc, &e->fl_tab, &e->fl_match, &e->fl_dig, &e->fl_keep,
-                      &e->sdr_status, &e->sdr_nf, &e->sdr_f_off, &e->sdr_f_len, &e->sdr_f_dq, &e->sdr_okey};
+                      &e->sdr_status, &e->sdr_nf, &e->sdr_f_off, &e->sdr_f_len, &e->sdr_f_dq, &e->sdr_okey,
+                      &e->ts_conf, &e->ts_full, &e->ts_cnt};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -4001,3 +4006,148 @@ int lc_zstd_compress(lc_engine_t* e, uint64_t nseg, const uint8_t* const* seg_pt
 }
 
 } // extern "C"
+
+// ------------------------------------------------------------------------------------------------ timestamp parse
+struct lc_timestamp {
+    uint64_t id;
+    LcTsConf conf;
+};
+
+int lc_timestamp_compile(const char* format, size_t len, int32_t source_year, int32_t tz_adjust,
+                         lc_timestamp_t** out) {
+    if (!out || (!format && len))
+        return fail(LC_ERR_INVALID_ARG, "lc_timestamp_compile: bad arguments");
+    *out = nullptr;
+    lc_timestamp* t = new (std::nothrow) lc_timestamp;
+    if (!t)
+        return fail(LC_ERR_INVALID_ARG, "out of host memory");
+    memset(&t->conf, 0, sizeof t->conf);
+    const char* err = nullptr;
+    if (lc_ts_compile(format ? format : "", len, t->conf, &err) != 0) {
+        delete t;
+        return fail(LC_ERR_INVALID_ARG, std::string("lc_timestamp_compile: ") + err);
+    }
+    t->conf.source_year = source_year;
+    t->conf.adjust = tz_adjust;
+    lc_ts_probe_zone(t->conf);
+    t->id = g_regex_ids.fetch_add(1);
+    *out = t;
+    return LC_OK;
+}
+
+void lc_timestamp_free(lc_timestamp_t* t) { delete t; }
+
+namespace {
+
+// both passes over the value table `sp`; d_counters (u64[5], device) are written
+int ts_run(lc_engine_t* e, const lc_timestamp_t* ts, const uint8_t* d_base, const LcTsSpans& sp, uint64_t n,
+           const uint32_t* d_grp, uint64_t ngroups, int64_t now, int32_t discard_interval, int64_t* d_sec,
+           uint32_t* d_nsec, uint8_t* d_status, uint64_t* d_counters) {
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcTsNow t;
+    t.now = now;
+    const time_t tn = (time_t)now;
+    struct tm lt;
+    memset(&lt, 0, sizeof lt);
+    localtime_r(&tn, &lt);
+    t.year = lt.tm_year;
+    t.mon = lt.tm_mon;
+    t.mday = lt.tm_mday;
+    t.discard_interval = discard_interval;
+    if (e->ts_conf_id != ts->id) {
+        CU_TRY(e->ts_conf.ensure(sizeof(LcTsConf)));
+        CU_TRY(cudaMemcpyAsync(e->ts_conf.p, &ts->conf, sizeof(LcTsConf), cudaMemcpyHostToDevice, e->stream));
+        e->ts_conf_id = ts->id;
+    }
+    CU_TRY(cudaMemsetAsync(d_counters, 0, 5 * sizeof(uint64_t), e->stream));
+    if (n) {
+        CU_TRY(e->ts_full.ensure(n * sizeof(LcTsFull)));
+        lck::launch_ts_full(e->ts_conf.as<LcTsConf>(), t, d_base, sp, n, e->ts_full.as<LcTsFull>(), e->stream);
+        lck::launch_ts_resolve(e->ts_conf.as<LcTsConf>(), t, d_base, sp, e->ts_full.as<LcTsFull>(), d_grp, ngroups, d_sec,
+                               d_nsec, d_status, reinterpret_cast<unsigned long long*>(d_counters), e->stream);
+        e->launches += 2;
+    }
+    CU_TRY(cudaGetLastError());
+    return LC_OK;
+}
+
+} // namespace
+
+int lc_timestamp_parse_dev(lc_engine_t* e, const lc_timestamp_t* ts, const uint8_t* d_base, uint64_t base_len,
+                           const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, const uint32_t* d_grp,
+                           uint64_t ngroups, int64_t now, int32_t discard_interval, int64_t* d_sec, uint32_t* d_nsec,
+                           uint8_t* d_status, uint64_t* d_counters) {
+    if (!e || !ts || !d_counters || (n && (!d_base || !d_ev_off || !d_ev_len || !d_grp || !ngroups || !d_sec ||
+                                           !d_nsec || !d_status)))
+        return fail(LC_ERR_INVALID_ARG, "lc_timestamp_parse_dev: bad arguments");
+    if (base_len >= 0xFFFFFFF0ull || n >= 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE, "lc_timestamp_parse_dev: buffer must be < 4 GiB and < 2^32 events per call");
+    return ts_run(e, ts, d_base, LcTsSpans{d_ev_off, d_ev_len, nullptr, 1}, n, d_grp, ngroups, now,
+                  discard_interval, d_sec, d_nsec, d_status, d_counters);
+}
+
+int lc_timestamp_parse_capture_dev(lc_engine_t* e, const lc_timestamp_t* ts, const uint8_t* d_base, uint64_t base_len,
+                                   const uint8_t* d_rx_status, const uint32_t* d_cap_off, const uint32_t* d_cap_len,
+                                   uint32_t row_pitch, uint32_t k, uint64_t n, const uint32_t* d_grp,
+                                   uint64_t ngroups, int64_t now, int32_t discard_interval, int64_t* d_sec,
+                                   uint32_t* d_nsec, uint8_t* d_status, uint64_t* d_counters) {
+    if (!e || !ts || !d_counters || k >= row_pitch ||
+        (n && (!d_base || !d_rx_status || !d_cap_off || !d_cap_len || !d_grp || !ngroups || !d_sec || !d_nsec ||
+               !d_status)))
+        return fail(LC_ERR_INVALID_ARG, "lc_timestamp_parse_capture_dev: bad arguments");
+    if (base_len >= 0xFFFFFFF0ull || n >= 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE,
+                    "lc_timestamp_parse_capture_dev: buffer must be < 4 GiB and < 2^32 events per call");
+    return ts_run(e, ts, d_base, LcTsSpans{d_cap_off + k, d_cap_len + k, d_rx_status, row_pitch}, n, d_grp, ngroups,
+                  now, discard_interval, d_sec, d_nsec, d_status, d_counters);
+}
+
+int lc_timestamp_parse(lc_engine_t* e, const lc_timestamp_t* ts, const uint8_t* base, uint64_t base_len,
+                       const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* grp,
+                       uint64_t ngroups, int64_t now, int32_t discard_interval, int64_t* sec, uint32_t* nsec,
+                       uint8_t* status, uint64_t* counters) {
+    static const char* what = "lc_timestamp_parse";
+    if (!e || !ts || !counters || (n && (!base || !ev_off || !ev_len || !grp || !ngroups || !sec || !nsec || !status)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    if (base_len >= 0xFFFFFFF0ull || n >= 0xFFFFFFFFull || ngroups >= 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": buffer must be < 4 GiB and < 2^32 events per call");
+    memset(counters, 0, 5 * sizeof(uint64_t));
+    if (n == 0)
+        return LC_OK;
+    if (grp[0] != 0 || grp[ngroups] != n)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": groups must cover the events");
+    for (uint64_t g = 0; g < ngroups; ++g)
+        if (grp[g + 1] < grp[g])
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": group starts must not decrease");
+    for (uint64_t i = 0; i < n; ++i)
+        if (ev_len[i] != LC_TS_NO_KEY && (uint64_t)ev_off[i] + ev_len[i] > base_len)
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": event outside the buffer");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    CU_TRY(e->in.ensure(base_len + 16));
+    CU_TRY(e->ev_off.ensure(n * 4));
+    CU_TRY(e->ev_len.ensure(n * 4));
+    CU_TRY(e->lines_off.ensure((ngroups + 1) * 4));
+    CU_TRY(e->out_a.ensure(n * 8));
+    CU_TRY(e->out_b.ensure(n * 4));
+    CU_TRY(e->out_c.ensure(n));
+    CU_TRY(e->ts_cnt.ensure(5 * sizeof(uint64_t)));
+    CU_TRY(cudaMemcpyAsync(e->in.p, base, base_len, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(e->ev_off.p, ev_off, n * 4, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(e->ev_len.p, ev_len, n * 4, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(e->lines_off.p, grp, (ngroups + 1) * 4, cudaMemcpyHostToDevice, e->stream));
+    rc = ts_run(e, ts, e->in.as<uint8_t>(), LcTsSpans{e->ev_off.as<uint32_t>(), e->ev_len.as<uint32_t>(), nullptr, 1},
+                n, e->lines_off.as<uint32_t>(), ngroups, now, discard_interval, e->out_a.as<int64_t>(),
+                e->out_b.as<uint32_t>(), e->out_c.as<uint8_t>(), e->ts_cnt.as<uint64_t>());
+    if (rc)
+        return rc;
+    CU_TRY(cudaMemcpyAsync(sec, e->out_a.p, n * 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(nsec, e->out_b.p, n * 4, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(status, e->out_c.p, n, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(counters, e->ts_cnt.p, 5 * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    return LC_OK;
+}

@@ -7,6 +7,7 @@
 #pragma once
 #include <stdint.h>
 #include <string.h>
+#include <time.h>
 
 #include "lc_tables.h"
 
@@ -3314,5 +3315,773 @@ LC_HD void lc_zstd_emit_block(const uint8_t* s, uint32_t n, uint32_t j, const ui
     LC_LANES(l) {
         for (uint32_t i = l; i < size; i += W)
             o[3 + i] = src[i];
+    }
+}
+
+// ================================================================================================ timestamp parse
+// ProcessorParseTimestampNative (ProcessorParseTimestampNative.cpp:100-235) over Strptime (TimeUtil.cpp:112-160) and
+// strptime_ns (Strptime.cpp), in two passes:
+//   - lc_ts_full: one lane per event runs the compiled format over the value: the full parse's outcome, Strptime's
+//     tv_sec (mktime of the partially filled tm, written even when the parse fails), tv_nsec and the cache key length.
+//   - lc_ts_resolve: one warp per group applies ParseLogTime's second-level cache, a sequential state reset at the start
+//     of every group, 32 events per step; then the verdict of ProcessEvent.
+// The format is compiled on the host (lc_ts_compile) into a short program of LcTsOp.  The strptime_ns directives are
+// run as written for the C locale; %c, %x and %X (the "locale's format" conversions) are refused.  %Z with a zone
+// name other than GMT / UTC consumes nothing, as strptime_ns does on Linux.
+// mktime is restated over a per-year table of the process zone's (standard, daylight) offsets, probed with mktime on
+// the host (lc_ts_probe_zone): glibc's mktime honours tm_isdst = 0 / 1 with the zone's standard / daylight offset.
+// Bounds: a value is read over [off, off + len) followed by NUL bytes; the reference hands strptime a StringView that
+// need not be NUL-terminated, so the two agree whenever the value is terminated.
+#define LC_TS_MAX_OPS 96
+#define LC_TS_Y0 1800
+#define LC_TS_NYEARS 500
+#define LC_TS_NO_KEY 0xFFFFFFFFu  // ev_len of an event without SourceKey
+#define LC_TS_KFAIL 0xFFFFFFFFu   // LcTsFull::klen of a failed full parse
+#define LC_TS_MIN_YEAR (-2147483647 - 1)
+
+#define LC_TS_ST_OK 0
+#define LC_TS_ST_NOT_FOUND 1
+#define LC_TS_ST_FAILED 2
+#define LC_TS_ST_DISCARDED 3
+
+// counters[5]: ProcessorParseTimestampNative's metrics in this order
+#define LC_TS_C_KEY_NOT_FOUND 0
+#define LC_TS_C_OUT_FAILED 1
+#define LC_TS_C_HISTORY_FAILURE 2
+#define LC_TS_C_DISCARDED 3
+#define LC_TS_C_OUT_SUCCESSFUL 4
+
+enum LcTsOpCode : uint8_t {
+    LC_TSO_WS,       // white space in the format, %n, %t: eat isspace
+    LC_TSO_LIT,      // literal byte (also %%)
+    LC_TSO_FAIL,     // return NULL (unknown conversion, %s inside a format, an alternative modifier not allowed)
+    LC_TSO_RESET_NS, // start of %D %F %R %r %T: the recursive strptime_ns call zeroes the nanoseconds
+    LC_TSO_WDAY_NAME, LC_TSO_MON_NAME, LC_TSO_CENTURY, LC_TSO_MDAY, LC_TSO_NSEC, LC_TSO_HOUR24, LC_TSO_HOUR12,
+    LC_TSO_YDAY, LC_TSO_MIN, LC_TSO_MON, LC_TSO_AMPM, LC_TSO_SEC, LC_TSO_WEEK, LC_TSO_WDAY0, LC_TSO_WDAY1,
+    LC_TSO_YEAR2_ISO, LC_TSO_YEAR_ISO, LC_TSO_YEAR, LC_TSO_YEAR2, LC_TSO_ZONE_NAME, LC_TSO_ZONE_OFF,
+};
+#define LC_TSF_FAIL_AFTER 1u // the conversion runs, then the directive's LEGAL_ALT returns NULL
+#define LC_TSF_INNER 2u      // %y inside %D: the recursive call's own split_year
+
+struct LcTsOp {
+    uint8_t code, flags, ch, pad;
+};
+
+#define LC_TSM_HAVE_F 1u  // strstr(format, "%f")
+#define LC_TSM_END_F 2u   // ... and it is the last two bytes
+#define LC_TSM_EPOCH 4u   // format == "%s"
+#define LC_TSM_F_ONLY 8u  // format == "%f": Strptime returns before mktime
+
+struct LcTsConf {
+    LcTsOp ops[LC_TS_MAX_OPS];
+    uint32_t nops, mode;
+    int32_t source_year;  // SourceYear (-1 unset, 0 deduce from now, > 0 that year)
+    int32_t adjust;       // mLogTimeZoneOffsetSecond, subtracted after a successful full parse
+    int32_t std_off[LC_TS_NYEARS], dst_off[LC_TS_NYEARS]; // seconds east of UTC, year LC_TS_Y0 + k
+};
+
+struct LcTsNow {  // what a call reads of "now"
+    int64_t now;  // time(NULL)
+    int32_t year, mon, mday; // localtime_r(now): tm_year, tm_mon, tm_mday (DeduceYear)
+    int32_t discard_interval; // ilogtail_discard_interval, < 0 = no history discard (flag off, one-time pipeline)
+};
+
+// Host: SourceFormat -> program.  Returns 0, or -1 with *err set for a directive the program cannot run.
+inline int lc_ts_compile(const char* fmt, size_t len, LcTsConf& c, const char** err) {
+    c.nops = 0;
+    c.mode = 0;
+    if (memchr(fmt, 0, len)) {
+        *err = "SourceFormat: a NUL byte inside the format";
+        return -1;
+    }
+    const size_t flen = len;
+    for (size_t i = 0; i + 1 < flen; ++i)
+        if (fmt[i] == '%' && fmt[i + 1] == 'f') {
+            c.mode |= LC_TSM_HAVE_F | (i + 2 == flen ? LC_TSM_END_F : 0u);
+            break;
+        }
+    if (flen == 2 && fmt[0] == '%' && fmt[1] == 's') {
+        c.mode |= LC_TSM_EPOCH;
+        return 0;
+    }
+    if (flen == 2 && fmt[0] == '%' && fmt[1] == 'f')
+        c.mode |= LC_TSM_F_ONLY;
+    auto emit = [&](uint8_t code, uint8_t flags = 0, uint8_t ch = 0) -> bool {
+        if (c.nops >= LC_TS_MAX_OPS)
+            return false;
+        c.ops[c.nops++] = LcTsOp{code, flags, ch, 0};
+        return true;
+    };
+    auto inner = [&](const char* s) -> bool { // the recursive call of %D %F %R %r %T
+        bool ok = emit(LC_TSO_RESET_NS);
+        for (; *s && ok; ++s) {
+            if (*s == ' ')
+                ok = emit(LC_TSO_WS);
+            else if (*s != '%')
+                ok = emit(LC_TSO_LIT, 0, (uint8_t)*s);
+            else {
+                const char d = *++s;
+                const uint8_t code = d == 'm'   ? LC_TSO_MON
+                                     : d == 'd' ? LC_TSO_MDAY
+                                     : d == 'y' ? LC_TSO_YEAR2
+                                     : d == 'Y' ? LC_TSO_YEAR
+                                     : d == 'H' ? LC_TSO_HOUR24
+                                     : d == 'I' ? LC_TSO_HOUR12
+                                     : d == 'M' ? LC_TSO_MIN
+                                     : d == 'S' ? LC_TSO_SEC
+                                                : LC_TSO_AMPM;
+                ok = emit(code, d == 'y' ? LC_TSF_INNER : 0u);
+            }
+        }
+        return ok;
+    };
+    size_t i = 0;
+    while (i < flen) {
+        const unsigned char ch = (unsigned char)fmt[i++];
+        if (ch == ' ' || (ch >= 9 && ch <= 13)) {
+            if (!emit(LC_TSO_WS))
+                goto too_long;
+            continue;
+        }
+        if (ch != '%') {
+            if (!emit(LC_TSO_LIT, 0, ch))
+                goto too_long;
+            continue;
+        }
+        unsigned alt = 0;
+        for (;;) {
+            const char d = i < flen ? fmt[i++] : '\0';
+            // LEGAL_ALT(x) before the conversion fails -> FAIL; after it -> FAIL_AFTER
+            auto conv = [&](uint8_t code, unsigned legal) -> bool {
+                return emit(code, (alt & ~legal) ? LC_TSF_FAIL_AFTER : 0u);
+            };
+            bool ok = true;
+            switch (d) {
+            case '%':
+                ok = alt ? emit(LC_TSO_FAIL) : emit(LC_TSO_LIT, 0, '%');
+                break;
+            case 'E':
+            case 'O':
+                if (alt) {
+                    ok = emit(LC_TSO_FAIL);
+                    break;
+                }
+                alt = d == 'E' ? 1u : 2u;
+                continue;
+            case 'c':
+            case 'x':
+            case 'X':
+                *err = "SourceFormat: %c, %x and %X (the locale's formats) are not supported on the device";
+                return -1;
+            case 'D': ok = alt ? emit(LC_TSO_FAIL) : inner("%m/%d/%y"); break;
+            case 'F': ok = alt ? emit(LC_TSO_FAIL) : inner("%Y-%m-%d"); break;
+            case 'R': ok = alt ? emit(LC_TSO_FAIL) : inner("%H:%M"); break;
+            case 'r': ok = alt ? emit(LC_TSO_FAIL) : inner("%I:%M:%S %p"); break;
+            case 'T': ok = alt ? emit(LC_TSO_FAIL) : inner("%H:%M:%S"); break;
+            case 'A': case 'a': ok = conv(LC_TSO_WDAY_NAME, 0); break;
+            case 'B': case 'b': case 'h': ok = conv(LC_TSO_MON_NAME, 0); break;
+            case 'C': ok = conv(LC_TSO_CENTURY, 1); break;
+            case 'd': case 'e': ok = conv(LC_TSO_MDAY, 2); break;
+            case 'f': ok = conv(LC_TSO_NSEC, 2); break;
+            case 'k': ok = alt ? emit(LC_TSO_FAIL) : conv(LC_TSO_HOUR24, 2); break;
+            case 'H': ok = conv(LC_TSO_HOUR24, 2); break;
+            case 'l': ok = alt ? emit(LC_TSO_FAIL) : conv(LC_TSO_HOUR12, 2); break;
+            case 'I': ok = conv(LC_TSO_HOUR12, 2); break;
+            case 'j': ok = conv(LC_TSO_YDAY, 0); break;
+            case 'M': ok = conv(LC_TSO_MIN, 2); break;
+            case 'm': ok = conv(LC_TSO_MON, 2); break;
+            case 'p': ok = conv(LC_TSO_AMPM, 0); break;
+            case 'S': ok = conv(LC_TSO_SEC, 2); break;
+            case 'U': case 'W': ok = conv(LC_TSO_WEEK, 2); break;
+            case 'V': ok = emit(LC_TSO_WEEK); break;
+            case 'w': ok = conv(LC_TSO_WDAY0, 2); break;
+            case 'u': ok = conv(LC_TSO_WDAY1, 2); break;
+            case 'g': ok = emit(LC_TSO_YEAR2_ISO); break;
+            case 'G': ok = emit(LC_TSO_YEAR_ISO); break;
+            case 'Y': ok = conv(LC_TSO_YEAR, 1); break;
+            case 'y': ok = emit(LC_TSO_YEAR2); break;
+            case 'Z': ok = emit(LC_TSO_ZONE_NAME); break;
+            case 'z': ok = emit(LC_TSO_ZONE_OFF); break;
+            case 'n': case 't': ok = alt ? emit(LC_TSO_FAIL) : emit(LC_TSO_WS); break;
+            default: ok = emit(LC_TSO_FAIL); break; // unknown conversion, %s inside a format, a trailing '%'
+            }
+            if (!ok)
+                goto too_long;
+            if (d == '\0')
+                return 0; // strptime_ns returns NULL before it reads past the format's end
+            break;
+        }
+    }
+    return 0;
+too_long:
+    *err = "SourceFormat: more directives than the device program holds";
+    return -1;
+}
+
+LC_HD int64_t lc_ts_days_from_civil(int64_t y, uint32_t m, uint32_t d) { // proleptic Gregorian, m 1..12
+    y -= m <= 2;
+    const int64_t era = (y >= 0 ? y : y - 399) / 400;
+    const uint32_t yoe = (uint32_t)(y - era * 400);
+    const uint32_t doy = (153 * (m + (m > 2 ? -3 : 9)) + 2) / 5 + d - 1;
+    const uint32_t doe = yoe * 365 + yoe / 4 - yoe / 100 + doy;
+    return era * 146097 + (int64_t)doe - 719468;
+}
+
+LC_HD int64_t lc_ts_year_of_days(int64_t z) { // civil year of day z since 1970-01-01
+    z += 719468;
+    const int64_t era = (z >= 0 ? z : z - 146096) / 146097;
+    const uint32_t doe = (uint32_t)(z - era * 146097);
+    const uint32_t yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;
+    const uint32_t doy = doe - (365 * yoe + yoe / 4 - yoe / 100);
+    const uint32_t mp = (5 * doy + 2) / 153;
+    return (int64_t)yoe + era * 400 + (mp >= 10);
+}
+
+struct LcTsTm {
+    int sec, min, hour, mday, mon, year, isdst;
+};
+
+// mktime of a tm whose fields are in the ranges the parser leaves (mon 0..11, mday 0..31, sec 0..61).  glibc computes
+// in 64 bits, so a year that was never set (tm_year = INT_MIN) gives a time far in the past, and -1 only when the
+// normalised date leaves the range of tm_year.
+LC_HD int64_t lc_ts_mktime(const LcTsConf& c, const LcTsTm& t) {
+    const int64_t days = lc_ts_days_from_civil((int64_t)t.year + 1900, (uint32_t)t.mon + 1, 1) + t.mday - 1;
+    const int64_t local = days * 86400 + t.hour * 3600 + t.min * 60 + t.sec;
+    const int64_t d = local >= 0 ? local / 86400 : (local - 86399) / 86400;
+    const int64_t y = lc_ts_year_of_days(d);
+    if (y - 1900 < (int64_t)LC_TS_MIN_YEAR)
+        return -1; // the normalised tm_year does not fit an int (a never-set year with tm_mday 0): EOVERFLOW
+    int64_t k = y - LC_TS_Y0;
+    k = k < 0 ? 0 : (k >= LC_TS_NYEARS ? LC_TS_NYEARS - 1 : k);
+    return local - (t.isdst ? c.dst_off[k] : c.std_off[k]);
+}
+
+struct LcTsIn { // the value: bytes past len read as NUL
+    const uint8_t* s;
+    uint32_t n;
+    LC_HD uint32_t at(uint32_t p) const { return p < n ? s[p] : 0u; }
+};
+
+LC_HD bool lc_ts_space(uint32_t ch) { return ch == ' ' || (ch >= 9 && ch <= 13); }
+LC_HD bool lc_ts_digit(uint32_t ch) { return ch - '0' < 10u; }
+
+// conv_num: false = NULL (dest untouched)
+LC_HD bool lc_ts_num(const LcTsIn& in, uint32_t& p, int& dest, uint32_t llim, uint32_t ulim) {
+    uint32_t ch = in.at(p), result = 0, rulim = ulim;
+    if (!lc_ts_digit(ch))
+        return false;
+    do {
+        result = result * 10 + (ch - '0');
+        rulim /= 10;
+        ch = in.at(++p);
+    } while (result * 10 <= ulim && rulim && lc_ts_digit(ch));
+    if (result < llim || result > ulim)
+        return false;
+    dest = (int)result;
+    return true;
+}
+
+// conv_nanosecond: unsigned 32-bit arithmetic, as the reference's
+LC_HD bool lc_ts_nsec(const LcTsIn& in, uint32_t& p, uint32_t& dest, int& nlen) {
+    uint32_t ch = in.at(p), result = 0;
+    if (!lc_ts_digit(ch))
+        return false;
+    const uint32_t start = p;
+    int digits = 0;
+    do {
+        result = result * 10 + (ch - '0');
+        ++digits;
+        ch = in.at(++p);
+    } while (lc_ts_digit(ch));
+    for (int i = 0; i < 9 - digits; i++)
+        result *= 10;
+    dest = result;
+    nlen = (int)(p - start);
+    return true;
+}
+
+LC_HD const char* lc_ts_name(uint32_t table, uint32_t i) {
+    switch (table * 16 + i) {
+    case 0: return "Sunday"; case 1: return "Monday"; case 2: return "Tuesday"; case 3: return "Wednesday";
+    case 4: return "Thursday"; case 5: return "Friday"; case 6: return "Saturday";
+    case 16: return "Sun"; case 17: return "Mon"; case 18: return "Tue"; case 19: return "Wed"; case 20: return "Thu";
+    case 21: return "Fri"; case 22: return "Sat";
+    case 32: return "January"; case 33: return "February"; case 34: return "March"; case 35: return "April";
+    case 36: return "May"; case 37: return "June"; case 38: return "July"; case 39: return "August";
+    case 40: return "September"; case 41: return "October"; case 42: return "November"; case 43: return "December";
+    case 48: return "Jan"; case 49: return "Feb"; case 50: return "Mar"; case 51: return "Apr"; case 52: return "May";
+    case 53: return "Jun"; case 54: return "Jul"; case 55: return "Aug"; case 56: return "Sep"; case 57: return "Oct";
+    case 58: return "Nov"; case 59: return "Dec";
+    case 64: return "AM"; case 65: return "PM";
+    case 80: return "EST"; case 81: return "CST"; case 82: return "MST"; case 83: return "PST";
+    case 96: return "EDT"; case 97: return "CDT"; case 98: return "MDT"; case 99: return "PDT";
+    case 112: return "GMT"; case 113: return "UTC";
+    default: return "";
+    }
+}
+
+LC_HD uint32_t lc_ts_lower(uint32_t ch) { return ch - 'A' < 26u ? ch + 32 : ch; }
+
+// strncasecmp(name, bp, strlen(name)) == 0
+LC_HD bool lc_ts_name_at(const LcTsIn& in, uint32_t p, const char* name, uint32_t& len) {
+    uint32_t k = 0;
+    for (; name[k]; ++k)
+        if (lc_ts_lower((uint8_t)name[k]) != lc_ts_lower(in.at(p + k)))
+            return false;
+    len = k;
+    return true;
+}
+
+// find_string over table `full` (and then `abbr` when abbr >= 0) of c names
+LC_HD bool lc_ts_find(const LcTsIn& in, uint32_t& p, int& tgt, uint32_t full, int abbr, uint32_t c) {
+    for (int t = (int)full; t >= 0; t = t == (int)full ? abbr : -1) {
+        for (uint32_t i = 0; i < c; i++) {
+            uint32_t len;
+            if (lc_ts_name_at(in, p, lc_ts_name((uint32_t)t, i), len)) {
+                tgt = (int)i;
+                p += len;
+                return true;
+            }
+        }
+    }
+    return false;
+}
+
+struct LcTsFull { // per-event result of the full parse
+    int64_t raw;   // Strptime's tv_sec (for a "%f" format: unchanged, 0 here; see lc_ts_resolve)
+    uint32_t nsec; // tv_nsec of a successful parse
+    uint32_t klen; // cache key length of a successful parse, LC_TS_KFAIL when it failed
+};
+
+// %s (Strptime.cpp:85-112): strtoll, at most 10 digits of seconds, the following digits as %f
+LC_HD bool lc_ts_epoch(const LcTsIn& in, int64_t& secs, uint32_t& nsec, int& nlen) {
+    uint32_t p = 0;
+    while (lc_ts_space(in.at(p)))
+        ++p;
+    const bool neg = in.at(p) == '-';
+    if (in.at(p) == '-' || in.at(p) == '+')
+        ++p;
+    uint64_t acc = 0;
+    bool over = false;
+    const uint64_t lim = neg ? 9223372036854775808ull : 9223372036854775807ull;
+    while (lc_ts_digit(in.at(p))) {
+        const uint32_t dg = in.at(p++) - '0';
+        if (!over && acc > (lim - dg) / 10)
+            over = true;
+        if (!over)
+            acc = acc * 10 + dg;
+    }
+    if (over)
+        acc = lim;
+    int64_t n = neg ? (int64_t)(0 - acc) : (int64_t)acc;
+    uint32_t blen = n < 0 ? 1 : 0; // std::to_string(n).length()
+    for (uint64_t a = acc;; a /= 10) {
+        ++blen;
+        if (a < 10)
+            break;
+    }
+    const uint32_t slen = blen >= 10 ? 10 : blen;
+    for (uint32_t i = 0; i < blen - slen; ++i)
+        n /= 10;
+    if (n == 0)
+        return false;
+    secs = n;
+    nsec = 0;
+    nlen = 0;
+    uint32_t q = slen;
+    uint32_t ns;
+    int nl;
+    if (lc_ts_nsec(in, q, ns, nl)) {
+        nsec = ns;
+        nlen = nl;
+    }
+    return true;
+}
+
+// Strptime(value, SourceFormat, &logTime, nanosecondLength, SourceYear) with logTime = {0, 0}
+LC_HD LcTsFull lc_ts_full(const LcTsConf& c, const LcTsNow& now, const uint8_t* s, uint32_t n) {
+    const LcTsIn in{s, n};
+    LcTsTm tm{0, 0, 0, 0, 0, LC_TS_MIN_YEAR, 0};
+    uint32_t nsec = 0;
+    int nlen = -1;
+    bool ok = true;
+    int64_t epoch = 0;
+    bool have_epoch = false;
+    if (c.mode & LC_TSM_EPOCH) {
+        ok = lc_ts_epoch(in, epoch, nsec, nlen);
+        have_epoch = ok; // localtime_r then mktime gives the seconds back
+    } else {
+        uint32_t p = 0;
+        int split = 0;
+        for (uint32_t k = 0; k < c.nops && ok; ++k) {
+            const LcTsOp op = c.ops[k];
+            int i = 0;
+            bool r = true; // bp != NULL after the conversion
+            switch (op.code) {
+            case LC_TSO_WS:
+                while (lc_ts_space(in.at(p)))
+                    ++p;
+                break;
+            case LC_TSO_LIT:
+                r = in.at(p++) == op.ch;
+                break;
+            case LC_TSO_FAIL: r = false; break;
+            case LC_TSO_RESET_NS: nsec = 0; break;
+            case LC_TSO_WDAY_NAME: { int w; r = lc_ts_find(in, p, w, 0, 1, 7); break; }
+            case LC_TSO_MON_NAME: r = lc_ts_find(in, p, tm.mon, 2, 3, 12); break;
+            case LC_TSO_CENTURY:
+                i = 20;
+                r = lc_ts_num(in, p, i, 0, 99);
+                i = i * 100 - 1900;
+                if (split)
+                    i += tm.year % 100;
+                split = 1;
+                tm.year = i;
+                break;
+            case LC_TSO_MDAY: r = lc_ts_num(in, p, tm.mday, 1, 31); break;
+            case LC_TSO_NSEC: r = lc_ts_nsec(in, p, nsec, nlen); break;
+            case LC_TSO_HOUR24: r = lc_ts_num(in, p, tm.hour, 0, 23); break;
+            case LC_TSO_HOUR12:
+                r = lc_ts_num(in, p, tm.hour, 1, 12);
+                if (tm.hour == 12)
+                    tm.hour = 0;
+                break;
+            case LC_TSO_YDAY: i = 1; r = lc_ts_num(in, p, i, 1, 366); break;
+            case LC_TSO_MIN: r = lc_ts_num(in, p, tm.min, 0, 59); break;
+            case LC_TSO_MON:
+                i = 1;
+                r = lc_ts_num(in, p, i, 1, 12);
+                tm.mon = i - 1;
+                break;
+            case LC_TSO_AMPM:
+                r = lc_ts_find(in, p, i, 4, -1, 2);
+                if (tm.hour > 11) {
+                    ok = false;
+                    continue;
+                }
+                tm.hour += i * 12;
+                break;
+            case LC_TSO_SEC: r = lc_ts_num(in, p, tm.sec, 0, 61); break;
+            case LC_TSO_WEEK: r = lc_ts_num(in, p, i, 0, 53); break;
+            case LC_TSO_WDAY0: r = lc_ts_num(in, p, i, 0, 6); break;
+            case LC_TSO_WDAY1: i = 1; r = lc_ts_num(in, p, i, 1, 7); break;
+            case LC_TSO_YEAR2_ISO: r = lc_ts_num(in, p, i, 0, 99); break;
+            case LC_TSO_YEAR_ISO:
+                do
+                    ++p;
+                while (lc_ts_digit(in.at(p)));
+                break;
+            case LC_TSO_YEAR:
+                i = 1900;
+                r = lc_ts_num(in, p, i, 0, 9999);
+                tm.year = i - 1900;
+                break;
+            case LC_TSO_YEAR2:
+                r = lc_ts_num(in, p, i, 0, 99);
+                if (split && !(op.flags & LC_TSF_INNER))
+                    i += (tm.year / 100) * 100;
+                else {
+                    if (!(op.flags & LC_TSF_INNER))
+                        split = 1;
+                    i = i <= 68 ? i + 2000 - 1900 : i + 1900 - 1900;
+                }
+                tm.year = i;
+                break;
+            case LC_TSO_ZONE_NAME: {
+                uint32_t len;
+                if (lc_ts_name_at(in, p, "GMT", len) || lc_ts_name_at(in, p, "UTC", len)) {
+                    tm.isdst = 0;
+                    p += 3;
+                }
+                break;
+            }
+            case LC_TSO_ZONE_OFF: {
+                while (lc_ts_space(in.at(p)))
+                    ++p;
+                const uint32_t ch = in.at(p++);
+                if (ch == 'G' || ch == 'U' || ch == 'Z') {
+                    if ((ch == 'G' && in.at(p++) != 'M') || (ch != 'Z' && in.at(p++) != 'T')) {
+                        ok = false;
+                        continue;
+                    }
+                    tm.isdst = 0;
+                    break;
+                }
+                if (ch != '+' && ch != '-') {
+                    --p;
+                    int z;
+                    if (lc_ts_find(in, p, z, 5, -1, 4))
+                        break;
+                    if (lc_ts_find(in, p, z, 6, -1, 4)) {
+                        tm.isdst = 1;
+                        break;
+                    }
+                    const uint32_t b = in.at(p);
+                    if ((b >= 'A' && b <= 'I') || (b >= 'L' && b <= 'Y')) {
+                        ++p;
+                        break;
+                    }
+                    ok = false;
+                    continue;
+                }
+                int offs = 0, d = 0;
+                while (d < 4) {
+                    if (lc_ts_digit(in.at(p))) {
+                        offs = offs * 10 + (int)(in.at(p++) - '0');
+                        d++;
+                        continue;
+                    }
+                    if (d == 2 && in.at(p) == ':') {
+                        p++;
+                        continue;
+                    }
+                    break;
+                }
+                if (d != 2 && (d != 4 || offs % 100 >= 60)) {
+                    ok = false;
+                    continue;
+                }
+                tm.isdst = 0;
+                break;
+            }
+            }
+            if (!r || (op.flags & LC_TSF_FAIL_AFTER))
+                ok = false;
+        }
+    }
+    LcTsFull f{0, nsec, ok ? (nlen < 0 ? n : n - (uint32_t)nlen) : LC_TS_KFAIL};
+    if (c.mode & LC_TSM_F_ONLY)
+        return f;
+    if (have_epoch) {
+        f.raw = epoch;
+        return f;
+    }
+    if (c.source_year >= 0 && tm.year == LC_TS_MIN_YEAR) {
+        if (c.source_year > 0)
+            tm.year = c.source_year - 1900;
+        else if (tm.mon == 0 && tm.mday == 1 && now.mon == 11 && now.mday == 31) // DeduceYear
+            tm.year = now.year + 1;
+        else if (tm.mon == 11 && tm.mday == 31 && now.mon == 0 && now.mday == 1)
+            tm.year = now.year - 1;
+        else
+            tm.year = now.year;
+    }
+    f.raw = lc_ts_mktime(c, tm);
+    return f;
+}
+
+LC_HD uint32_t lc_ts_popc(uint32_t m) {
+#if defined(__CUDA_ARCH__)
+    return (uint32_t)__popc(m);
+#else
+    return (uint32_t)__builtin_popcount(m);
+#endif
+}
+
+// Where event i's value is: a dense (off, len) table (len LC_TS_NO_KEY = no SourceKey), or capture column k of a
+// regex result (st != NULL: off / len point at column k of [n][pitch] tables; a row not parsed has no value).
+struct LcTsSpans {
+    const uint32_t* off;
+    const uint32_t* len;
+    const uint8_t* st;
+    uint32_t pitch;
+    LC_HD bool get(uint64_t i, uint32_t& o, uint32_t& l) const {
+        if (st) {
+            if (st[i] != 0)
+                return false;
+            o = off[i * pitch];
+            l = len[i * pitch];
+            return true;
+        }
+        l = len[i];
+        if (l == LC_TS_NO_KEY)
+            return false;
+        o = off[i];
+        return true;
+    }
+};
+
+struct LcTsWarp { // per-warp scratch of the resolution pass (shared memory on the device)
+    uint32_t v[32];   // per-lane ballot predicate
+    uint32_t off[32]; // the step's values
+    uint32_t len[32];
+    uint32_t klen[32]; // LcTsFull of the step's events
+    uint32_t fns[32];
+    int64_t raw[32];
+};
+
+// IsPrefixString(value, key): false for an empty key
+LC_HD bool lc_ts_prefix(const uint8_t* base, uint32_t a, uint32_t alen, uint32_t k, uint32_t klen) {
+    if (klen == 0 || alen < klen)
+        return false;
+    for (uint32_t i = 0; i < klen; ++i)
+        if (base[a + i] != base[k + i])
+            return false;
+    return true;
+}
+
+LC_HD uint32_t lc_ts_below(uint32_t l) { return l >= 32 ? 0xFFFFFFFFu : (1u << l) - 1u; }
+
+// ParseLogTime's second-level cache and ProcessEvent's verdict over the events [e0, e1) of one group, W lanes,
+// 32 events per step.  Each lane tests its value against the cache key the step starts with (hx) and against the key
+// of the nearest earlier event of the step whose full parse succeeded (hp); the masks then tell which events miss
+// (a miss with a successful full parse moves the cache), as far as the step can know them: it ends at the first
+// event that hits a key set inside the step and would have to be compared with a key that is not its predecessor's.
+// A hit inherits tv_sec from the last full parse of the group, successful or not.  cnt[5] += the counters.
+LC_HD void lc_ts_resolve(const LcTsConf& c, const LcTsNow& now, const uint8_t* base, const LcTsSpans& sp, const LcTsFull* full,
+                         uint64_t e0, uint64_t e1, int64_t* sec, uint32_t* nsec, uint8_t* status, uint64_t* cnt,
+                         LcTsWarp& w, uint32_t lane, uint32_t W) {
+    const bool cacheable = !(c.mode & LC_TSM_HAVE_F) || (c.mode & LC_TSM_END_F);
+    bool have_key = false;
+    uint32_t key_off = 0, key_len = 0;
+    int64_t state = 0; // logTime.tv_sec
+    for (uint64_t b = e0; b < e1;) {
+        const uint32_t nv = e1 - b < W ? (uint32_t)(e1 - b) : W;
+        LC_LANES(l) {
+            uint32_t o = 0, ln = 0;
+            const bool pres = l < nv && sp.get(b + l, o, ln);
+            const LcTsFull f = pres ? full[b + l] : LcTsFull{0, 0, LC_TS_KFAIL};
+            w.off[l] = o;
+            w.len[l] = pres ? ln : LC_TS_NO_KEY;
+            w.klen[l] = f.klen;
+            w.fns[l] = f.nsec;
+            w.raw[l] = f.raw;
+        }
+        LC_WARP_SYNC();
+        LC_LANES(l) { w.v[l] = w.len[l] != LC_TS_NO_KEY; }
+        const uint32_t pm = lc_lz4_ballot(w.v, lane, W);
+        LC_LANES(l) { w.v[l] = w.len[l] != LC_TS_NO_KEY && w.klen[l] != LC_TS_KFAIL; }
+        const uint32_t okm = lc_lz4_ballot(w.v, lane, W);
+        LC_LANES(l) {
+            w.v[l] = cacheable && have_key && w.len[l] != LC_TS_NO_KEY &&
+                     lc_ts_prefix(base, w.off[l], w.len[l], key_off, key_len);
+        }
+        const uint32_t hxm = lc_lz4_ballot(w.v, lane, W);
+        LC_LANES(l) {
+            const uint32_t before = okm & lc_ts_below(l);
+            const uint32_t p = before ? lc_hi_bit(before) : 0u;
+            w.v[l] = cacheable && before && w.len[l] != LC_TS_NO_KEY &&
+                     lc_ts_prefix(base, w.off[l], w.len[l], w.off[p], w.klen[p]);
+        }
+        const uint32_t hpm = lc_lz4_ballot(w.v, lane, W);
+        // which events of the step hit, and how far the step can tell
+        const uint32_t valid = lc_ts_below(nv);
+        uint32_t hitm = 0, pos = 0;
+        int owner = -1;
+        while (cacheable && pos < nv) {
+            const uint32_t rng = valid & ~lc_ts_below(pos);
+            if (owner < 0) {
+                const uint32_t mv = okm & ~hxm & rng;
+                if (!mv) {
+                    hitm |= hxm & rng;
+                    pos = nv;
+                    break;
+                }
+                const uint32_t m = lc_lo_bit(mv);
+                hitm |= hxm & rng & lc_ts_below(m);
+                owner = (int)m;
+                pos = m + 1;
+            } else {
+                const uint32_t nx = okm & rng;
+                if (!nx) {
+                    hitm |= hpm & rng;
+                    pos = nv;
+                    break;
+                }
+                const uint32_t m = lc_lo_bit(nx);
+                hitm |= hpm & rng & lc_ts_below(m + 1);
+                pos = m + 1;
+                if ((hpm >> m) & 1u)
+                    break; // m hits the owner's key, so the events after it are compared with m's key: next step
+                owner = (int)m;
+            }
+        }
+        if (!cacheable)
+            pos = nv;
+        const uint32_t res = lc_ts_below(pos);
+        const uint32_t missm = pm & ~hitm & res, okmiss = okm & missm;
+        const int64_t state0 = state;
+        // tv_sec left by the full parse of miss lane j
+        auto after = [&](uint32_t j) -> int64_t {
+            if (c.mode & LC_TSM_F_ONLY)
+                return state0 - (int64_t)c.adjust * (int64_t)lc_ts_popc(okmiss & lc_ts_below(j + 1));
+            return w.klen[j] != LC_TS_KFAIL ? w.raw[j] - c.adjust : w.raw[j];
+        };
+        LC_LANES(l) {
+            if (l < pos) {
+                uint8_t st;
+                int64_t s = 0;
+                uint32_t ns = 0;
+                if (w.len[l] == LC_TS_NO_KEY) {
+                    st = LC_TS_ST_NOT_FOUND;
+                    cnt[LC_TS_C_KEY_NOT_FOUND]++;
+                } else {
+                    bool ok;
+                    if ((hitm >> l) & 1u) {
+                        const uint32_t lm = missm & lc_ts_below(l), lo = okmiss & lc_ts_below(l);
+                        s = lm ? after(lc_hi_bit(lm)) : state0;
+                        const uint32_t kl = lo ? w.klen[lc_hi_bit(lo)] : key_len;
+                        ok = true;
+                        if ((c.mode & LC_TSM_END_F) || ((c.mode & LC_TSM_EPOCH) && w.len[l] > kl)) {
+                            const LcTsIn in{base + w.off[l] + kl, w.len[l] - kl};
+                            uint32_t q = 0;
+                            int nl;
+                            ok = lc_ts_nsec(in, q, ns, nl);
+                            if (!ok)
+                                ns = 0;
+                        }
+                    } else {
+                        ok = w.klen[l] != LC_TS_KFAIL;
+                        s = after(l);
+                        ns = w.fns[l];
+                    }
+                    if (!ok) {
+                        s = 0;
+                        ns = 0;
+                        st = LC_TS_ST_FAILED;
+                        cnt[LC_TS_C_OUT_FAILED]++;
+                    } else if (s <= 0 || (now.discard_interval >= 0 && now.now - s > (int64_t)now.discard_interval)) {
+                        st = LC_TS_ST_DISCARDED;
+                        cnt[LC_TS_C_HISTORY_FAILURE]++;
+                        cnt[LC_TS_C_DISCARDED]++;
+                    } else {
+                        st = LC_TS_ST_OK;
+                        cnt[LC_TS_C_OUT_SUCCESSFUL]++;
+                    }
+                }
+                sec[b + l] = s;
+                nsec[b + l] = ns;
+                status[b + l] = st;
+            }
+        }
+        if (okmiss) {
+            const uint32_t j = lc_hi_bit(okmiss);
+            have_key = true;
+            key_off = w.off[j];
+            key_len = w.klen[j];
+        }
+        if (missm)
+            state = after(lc_hi_bit(missm));
+        LC_WARP_SYNC();
+        b += pos;
+    }
+}
+
+// Host, at Init: the process zone's offsets for tm_isdst = 0 and 1, per year, as mktime applies them (probed at
+// July 1st, 12:00 of each year).
+inline void lc_ts_probe_zone(LcTsConf& c) {
+    for (int k = 0; k < LC_TS_NYEARS; ++k) {
+        const int64_t local = lc_ts_days_from_civil(LC_TS_Y0 + k, 7, 1) * 86400 + 43200;
+        for (int d = 0; d < 2; ++d) {
+            struct tm t;
+            memset(&t, 0, sizeof t);
+            t.tm_year = LC_TS_Y0 + k - 1900;
+            t.tm_mon = 6;
+            t.tm_mday = 1;
+            t.tm_hour = 12;
+            t.tm_isdst = d;
+            const int64_t off = local - (int64_t)mktime(&t);
+            (d ? c.dst_off : c.std_off)[k] = (int32_t)off;
+        }
     }
 }

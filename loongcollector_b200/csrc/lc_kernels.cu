@@ -4362,4 +4362,50 @@ void launch_zstd_emit(const Lz4Segs& g, const uint64_t* d_bfirst, uint64_t nbloc
         g.in, g.seg_off, g.seg_len, d_bfirst, g.nseg, nblocks, d_slot, d_body, d_boff, d_out);
 }
 
+// ---------------------------------------------------------------------------------------------- timestamp parse
+__global__ void __launch_bounds__(256)
+    ts_full_kernel(const LcTsConf* __restrict__ conf, LcTsNow now, const uint8_t* __restrict__ base, LcTsSpans sp,
+                   uint64_t n, LcTsFull* __restrict__ full) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t o, l;
+    if (i >= n || !sp.get(i, o, l))
+        return;
+    full[i] = lc_ts_full(*conf, now, base + o, l);
+}
+
+constexpr int kTsWarps = 4;
+
+__global__ void __launch_bounds__(32 * kTsWarps)
+    ts_resolve_kernel(const LcTsConf* __restrict__ conf, LcTsNow now, const uint8_t* __restrict__ base, LcTsSpans sp,
+                      const LcTsFull* __restrict__ full, const uint32_t* __restrict__ grp, uint64_t ngroups,
+                      int64_t* __restrict__ sec, uint32_t* __restrict__ nsec, uint8_t* __restrict__ status,
+                      unsigned long long* __restrict__ counters) {
+    __shared__ LcTsWarp ws[kTsWarps];
+    const uint32_t wi = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint64_t cnt[5] = {0, 0, 0, 0, 0};
+    for (uint64_t g = (uint64_t)blockIdx.x * kTsWarps + wi; g < ngroups; g += (uint64_t)gridDim.x * kTsWarps)
+        lc_ts_resolve(*conf, now, base, sp, full, grp[g], grp[g + 1], sec, nsec, status, cnt, ws[wi], lane, 32);
+    for (int k = 0; k < 5; ++k) {
+        const uint32_t t = __reduce_add_sync(0xFFFFFFFFu, (uint32_t)cnt[k]);
+        if (lane == 0 && t)
+            atomicAdd(&counters[k], (unsigned long long)t);
+    }
+}
+
+void launch_ts_full(const LcTsConf* d_conf, const LcTsNow& now, const uint8_t* d_base, const LcTsSpans& sp, uint64_t n,
+                    LcTsFull* d_full, cudaStream_t st) {
+    if (n)
+        ts_full_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_conf, now, d_base, sp, n, d_full);
+}
+
+void launch_ts_resolve(const LcTsConf* d_conf, const LcTsNow& now, const uint8_t* d_base, const LcTsSpans& sp, const LcTsFull* d_full,
+                       const uint32_t* d_grp, uint64_t ngroups, int64_t* d_sec, uint32_t* d_nsec, uint8_t* d_status,
+                       unsigned long long* d_counters, cudaStream_t st) {
+    if (!ngroups)
+        return;
+    const uint64_t blocks = (ngroups + kTsWarps - 1) / kTsWarps;
+    ts_resolve_kernel<<<(unsigned)(blocks < (1u << 20) ? blocks : (1u << 20)), 32 * kTsWarps, 0, st>>>(
+        d_conf, now, d_base, sp, d_full, d_grp, ngroups, d_sec, d_nsec, d_status, d_counters);
+}
+
 } // namespace lck

@@ -13,6 +13,10 @@ struct LcSplitDelimSlsCfg;
 struct LcSplitDelimRegexSlsCfg;
 struct LcFilterSlsCfg;
 struct LcLz4Seq;
+struct LcTsConf;
+struct LcTsNow;
+struct LcTsSpans;
+struct LcTsFull;
 struct LcLz4Chunk;
 
 namespace lck {
@@ -354,5 +358,14 @@ void launch_zstd_blocks(const Lz4Segs& g, const uint64_t* d_bfirst, uint64_t nbl
 void launch_zstd_emit(const Lz4Segs& g, const uint64_t* d_bfirst, uint64_t nblocks, const uint8_t* d_slot,
                       const uint32_t* d_body, const uint64_t* d_boff, const uint64_t* d_total, uint8_t* d_out,
                       uint64_t* d_frm_off, uint32_t* d_frm_len, cudaStream_t st);
+
+// ProcessorParseTimestampNative (lc_exec.cuh): launch_ts_full runs the compiled format over every event with a value
+// (one thread per event, d_full[i]); launch_ts_resolve applies the second-level cache and the verdict, one warp per
+// group (events [d_grp[g], d_grp[g + 1])), and adds the five counters to d_counters (u64, zeroed by the caller).
+void launch_ts_full(const LcTsConf* d_conf, const LcTsNow& now, const uint8_t* d_base, const LcTsSpans& sp, uint64_t n,
+                    LcTsFull* d_full, cudaStream_t st);
+void launch_ts_resolve(const LcTsConf* d_conf, const LcTsNow& now, const uint8_t* d_base, const LcTsSpans& sp, const LcTsFull* d_full,
+                       const uint32_t* d_grp, uint64_t ngroups, int64_t* d_sec, uint32_t* d_nsec, uint8_t* d_status,
+                       unsigned long long* d_counters, cudaStream_t st);
 
 } // namespace lck

@@ -3093,7 +3093,156 @@ bool ZstdCompressor::Compress(const std::vector<std::string>& inputs, std::vecto
     return true;
 }
 
+// ------------------------------------------------------------------------------------ ProcessorParseTimestampNative
+const std::string ProcessorParseTimestampNative::sName = "processor_parse_timestamp_native";
+
+namespace {
+
+// ParseTimeZoneOffsetSecond (TimeUtil.cpp:372-391): "GMT+08:00" -> seconds east
+bool ParseGmtOffset(const std::string& tz, int& sec) {
+    if (tz.size() != 9 || tz[6] != ':' || (tz[3] != '+' && tz[3] != '-') || tz.compare(0, 3, "GMT") != 0)
+        return false;
+    auto num = [](const std::string& s, int& v) {
+        if (s.empty() || !isdigit((unsigned char)s[0]))
+            return false;
+        v = 0;
+        for (char c : s) {
+            if (!isdigit((unsigned char)c))
+                return false;
+            v = v * 10 + (c - '0');
+        }
+        return true;
+    };
+    int h, m;
+    if (!num(tz.substr(4, 2), h) || !num(tz.substr(7, 2), m))
+        return false;
+    sec = h * 3600 + m * 60;
+    if (tz[3] == '-')
+        sec = -sec;
+    return true;
+}
+
+int LocalGmtOffset() { // GetLocalTimeZoneOffsetSecond (TimeUtil.cpp:72-79)
+    time_t now = time(nullptr);
+    struct tm t;
+    memset(&t, 0, sizeof t);
+    localtime_r(&now, &t);
+    return (int)t.tm_gmtoff;
+}
+
+} // namespace
+
+bool ProcessorParseTimestampNative::Init(const Json::Value& config) {
+    mWarnings.clear();
+    if (!GetString(config, "SourceKey", mSourceKey) || mSourceKey.empty())
+        return Fail("mandatory string param SourceKey is missing");
+    if (!GetString(config, "SourceFormat", mSourceFormat) || mSourceFormat.empty())
+        return Fail("mandatory string param SourceFormat is missing");
+    mLogTimeZoneOffsetSecond = 0;
+    if (config.isMember("SourceTimezone") && !config["SourceTimezone"].isString()) {
+        mWarnings.push_back("optional string param SourceTimezone is not of type string");
+    } else if (GetString(config, "SourceTimezone", mSourceTimezone) && !mSourceTimezone.empty()) {
+        int tz = 0;
+        if (ParseGmtOffset(mSourceTimezone, tz))
+            mLogTimeZoneOffsetSecond = tz - LocalGmtOffset();
+        else
+            mWarnings.push_back("string param SourceTimezone is not valid");
+    }
+    if (config.isMember("SourceYear")) {
+        if (config["SourceYear"].isInt())
+            mSourceYear = config["SourceYear"].asInt();
+        else
+            mWarnings.push_back("optional int param SourceYear is not of type int");
+    }
+    lc_timestamp_free(mProgram);
+    mProgram = nullptr;
+    if (lc_timestamp_compile(mSourceFormat.data(), mSourceFormat.size(), mSourceYear, mLogTimeZoneOffsetSecond,
+                             &mProgram) != LC_OK)
+        return Fail(std::string("string param SourceFormat is not supported: ") + lc_last_error());
+    return true;
+}
+
+void ProcessorParseTimestampNative::Process(PipelineEventGroup& group) {
+    std::vector<PipelineEventGroup> one;
+    one.emplace_back(std::move(group));
+    Process(one);
+    group = std::move(one[0]);
+}
+
+void ProcessorParseTimestampNative::Process(std::vector<PipelineEventGroup>& groups) {
+    if (!mProgram)
+        return;
+    // values of every group back to back, one event table, group starts
+    std::string bytes;
+    std::vector<uint32_t> off, len, grp{0};
+    for (auto& g : groups) {
+        for (PipelineEventPtr& e : g.MutableEvents()) {
+            const LogEvent* ev = IsSupportedEvent(e) ? &e.Cast<LogEvent>() : nullptr;
+            if (ev && ev->HasContent(mSourceKey)) {
+                const StringView v = ev->GetContent(mSourceKey);
+                off.push_back((uint32_t)bytes.size());
+                len.push_back((uint32_t)v.size());
+                bytes.append(v.data(), v.size());
+            } else {
+                off.push_back(0);
+                len.push_back(LC_TS_NO_KEY);
+            }
+        }
+        grp.push_back((uint32_t)off.size());
+    }
+    const uint64_t n = off.size();
+    if (n == 0)
+        return;
+    std::vector<int64_t> sec(n);
+    std::vector<uint32_t> nsec(n);
+    std::vector<uint8_t> status(n);
+    uint64_t cnt[5];
+    try {
+        Check(lc_timestamp_parse(Engine(), mProgram, reinterpret_cast<const uint8_t*>(bytes.data()), bytes.size(),
+                                 off.data(), len.data(), n, grp.data(), groups.size(), (int64_t)time(nullptr),
+                                 mDiscardOldData ? mDiscardInterval : -1, sec.data(), nsec.data(), status.data(), cnt),
+              "lc_timestamp_parse");
+    } catch (const std::exception& ex) {
+        EngineFailed(ex.what());
+        return;
+    }
+    uint64_t i = 0;
+    uint64_t unsupported = 0;
+    for (auto& g : groups) {
+        EventsContainer& events = g.MutableEvents();
+        size_t wIdx = 0;
+        for (size_t rIdx = 0; rIdx < events.size(); ++rIdx, ++i) {
+            if (!IsSupportedEvent(events[rIdx])) {
+                unsupported++; // counted as key_not_found by the device: ProcessEvent counts it out_failed
+            } else if (status[i] == LC_TS_DISCARDED) {
+                continue;
+            } else if (status[i] == LC_TS_OK) {
+                events[rIdx].Cast<LogEvent>().SetTimestamp(sec[i], nsec[i]);
+            }
+            if (wIdx != rIdx)
+                events[wIdx] = std::move(events[rIdx]);
+            ++wIdx;
+        }
+        events.resize(wIdx);
+    }
+    mOutKeyNotFoundEventsTotal.Add(cnt[0] - unsupported);
+    mOutFailedEventsTotal.Add(cnt[1] + unsupported);
+    mHistoryFailureTotal.Add(cnt[2]);
+    mDiscardedEventsTotal.Add(cnt[3]);
+    mOutSuccessfulEventsTotal.Add(cnt[4]);
+}
+
+std::vector<std::pair<std::string, uint64_t>> ProcessorParseTimestampNative::Counters() const {
+    return {{"discarded", mDiscardedEventsTotal.GetValue()},
+            {"out_failed", mOutFailedEventsTotal.GetValue()},
+            {"out_key_not_found", mOutKeyNotFoundEventsTotal.GetValue()},
+            {"out_successful", mOutSuccessfulEventsTotal.GetValue()},
+            {"history_failure", mHistoryFailureTotal.GetValue()}};
+}
+
 Processor* CreateProcessor(const std::string& type) {
+    if (type == ProcessorParseTimestampNative::sName)
+        return new ProcessorParseTimestampNative;
     if (type == ProcessorMergeMultilineLogNative::sName)
         return new ProcessorMergeMultilineLogNative;
     if (type == ProcessorFilterNative::sName)

@@ -368,6 +368,37 @@ private:
 // First "next" row (SURVEY.md 8f): regex include / exclude filter.  Every regex leaf of the rule / expression is
 // evaluated for the whole group with one batched boolean regex_match on the GPU; the and/or/not tree and the
 // non-UTF8 blanking stay on the host.  core/plugin/processor/ProcessorFilterNative.cpp:30-275,380-488
+// processor_parse_timestamp_native (ProcessorParseTimestampNative.cpp:30-235): the groups of one call go to the device
+// in one lc_timestamp_parse call (the full parse and the second-level cache run there, the cache starting empty in
+// every group); the host sets the times, erases the discarded events (rIdx / wIdx) and adds the counters.
+// Init also fails where the device program refuses SourceFormat (%c, %x, %X: LastError() says so); there is no CPU
+// fallback.  "now" is read once per call, where the reference calls time(NULL) per event.
+class ProcessorParseTimestampNative : public Processor {
+public:
+    static const std::string sName;
+    const std::string& Name() const override { return sName; }
+    ~ProcessorParseTimestampNative() override { lc_timestamp_free(mProgram); }
+    bool Init(const Json::Value& config) override;
+    void Process(PipelineEventGroup& group) override;
+    void Process(std::vector<PipelineEventGroup>& groups) override;
+    std::vector<std::pair<std::string, uint64_t>> Counters() const override;
+    std::string mSourceKey, mSourceFormat, mSourceTimezone;
+    int32_t mSourceYear = -1;
+    int32_t mLogTimeZoneOffsetSecond = 0;
+    // ilogtail_discard_old_data (on by default; off for one-time pipelines) and ilogtail_discard_interval
+    bool mDiscardOldData = true;
+    int32_t mDiscardInterval = 43200;
+    std::vector<std::string> mWarnings; // the reference's PARAM_WARNING_* messages of the last Init
+    Counter mDiscardedEventsTotal, mOutFailedEventsTotal, mOutKeyNotFoundEventsTotal, mOutSuccessfulEventsTotal,
+        mHistoryFailureTotal;
+
+protected:
+    bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
+
+private:
+    lc_timestamp_t* mProgram = nullptr;
+};
+
 class ProcessorFilterNative : public Processor {
 public:
     static const std::string sName;

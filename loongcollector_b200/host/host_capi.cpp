@@ -82,6 +82,37 @@ char* lc_host_processor_process(lc_host_processor_t* p, const char* group_json, 
     }
 }
 
+char* lc_host_processor_process_groups(lc_host_processor_t* p, const char* groups_json, int enable_event_meta,
+                                       char** err_out) {
+    if (err_out)
+        *err_out = nullptr;
+    try {
+        Json::Value arr;
+        std::string err;
+        const char* gj = groups_json ? groups_json : "[]";
+        if (!Json::Value::parse(gj, gj + strlen(gj), arr, err) || !arr.isArray())
+            throw std::runtime_error("groups JSON is not an array");
+        std::vector<PipelineEventGroup> groups;
+        for (size_t k = 0; k < arr.size(); ++k) {
+            groups.emplace_back(std::make_shared<SourceBuffer>());
+            if (!groups.back().FromJson(arr[k]))
+                throw std::runtime_error("group JSON does not parse");
+        }
+        const uint64_t errs = p->proc->EngineErrors();
+        p->proc->Process(groups);
+        if (p->proc->EngineErrors() != errs)
+            throw std::runtime_error("engine error inside Process: " + p->proc->LastError());
+        Json::Value out(Json::arrayValue);
+        for (auto& g : groups)
+            out.append(g.ToJson(enable_event_meta != 0));
+        return dup(out.toString());
+    } catch (const std::exception& e) {
+        if (err_out)
+            *err_out = dup(e.what());
+        return nullptr;
+    }
+}
+
 char* lc_host_processor_counters(const lc_host_processor_t* p) {
     Json::Value v(Json::objectValue);
     for (auto& kv : p->proc->Counters())
