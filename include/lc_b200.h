@@ -603,6 +603,90 @@ int lc_multiline_split_regex_filter_parse_sls_lz4(
     const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
     uint64_t* n_events, uint64_t counters[4], uint64_t ml_counters[3]);
 
+/* ---- f4: the split -> regex -> timestamp chain (the split -> regex chain, then ProcessorParseTimestampNative with
+ * SourceKey tkey, ProcessorParseTimestampNative.cpp:100-179; the processor documentation's nginx pipeline) to the SLS
+ * wire format.  Pieces and the regex stage are exactly the split -> regex chain's (same arguments, offset metadata,
+ * refusals and erase rule).  The row rule:
+ *   - The timestamp stage sees the pieces the regex stage kept, in piece order, as ONE group (the second-level cache
+ *     starts empty per call).  A piece the regex stage erased is no event of the stage: no counter, no cache step.
+ *   - Its value is what the regex stage left under tkey: a capture (with repeated keys the plan's winner), the piece
+ *     (KeepingSourceWhenParseSucceed, or a kept failure under SourceKey / RenamedSourceKey / "__raw_log__"), or
+ *     nothing (LC_TS_NOT_FOUND).  A tkey that holds the offset digits (tkey equal to offset_key) is refused with
+ *     LC_ERR_INVALID_ARG.  The value is read over [off, off + len) followed by NUL bytes, as lc_timestamp_parse reads.
+ *   - LC_TS_OK: the record's Time is the parsed seconds truncated to 32 bits (raised to at least 2^28 as every
+ *     record's); with enable_ns (mEnableTimestampNanosecond) Time_ns is the parsed nanoseconds, even 0 and even when
+ *     the source event had none.  LC_TS_NOT_FOUND, LC_TS_FAILED: the source event's time / time_ns.  LC_TS_DISCARDED:
+ *     no record.
+ *   - time_ns is the source event's Time_ns as the serialiser writes it, so it must agree with enable_ns: a time_ns
+ *     other than LC_SLS_NO_NS with enable_ns == 0 is refused with LC_ERR_INVALID_ARG (the records that keep the source
+ *     time would carry Time_ns and the parsed ones would not).
+ *   - counters[8] (may be NULL) = the regex stage's out_successful, out_failed, discarded, then the timestamp stage's
+ *     key_not_found, out_failed, history_failure, discarded, out_successful.
+ *
+ * lc_split_regex_timestamp_tap_dev: from the DEVICE piece and regex tables (as for lc_sls_serialize_split_regex_dev)
+ * and the regex stage's configuration, writes the DEVICE value table d_val_off / d_val_len[n] over d_src that
+ * lc_timestamp_parse_dev takes with one group (ev_len LC_TS_NO_KEY: erased by the regex stage, or no tkey).  It
+ * queues the work on the engine's stream and returns without waiting.
+ * lc_sls_serialize_split_regex_timestamp_dev: lc_sls_serialize_split_regex_dev's arguments plus the DEVICE results
+ * of that lc_timestamp_parse_dev call (d_ts_status, d_ts_sec, d_ts_nsec) and enable_ns.  Sizing query, capacity and
+ * 4 GiB rules are the sibling's. */
+struct lc_timestamp; /* lc_timestamp_t, compiled by lc_timestamp_compile below */
+int lc_split_regex_timestamp_tap_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+                                     const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                     const uint32_t* d_cap_off, const uint32_t* d_cap_len, uint32_t row_pitch,
+                                     const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                                     const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                                     uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                                     int whole_line, const char* offset_key, uint32_t offset_key_len,
+                                     const char* tkey, uint32_t tkey_len, uint32_t* d_val_off, uint32_t* d_val_len);
+int lc_sls_serialize_split_regex_timestamp_dev(
+    lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+    const uint8_t* d_status, const uint32_t* d_cap_off, const uint32_t* d_cap_len, uint32_t row_pitch,
+    const char* const* keys, const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+    uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed,
+    int copy_raw, int whole_line, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+    uint32_t time_ns, const uint8_t* d_ts_status, const int64_t* d_ts_sec, const uint32_t* d_ts_nsec, int enable_ns,
+    uint8_t* d_out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[8]);
+
+/* The same with a HOST source value: upload it once, split, regex, tap, both timestamp passes (ts compiled by
+ * lc_timestamp_compile; now = time(NULL) of the call, discard_interval as for lc_timestamp_parse, -1 = no history
+ * discard), size and emit (and LZ4), and bring back only the bytes.  *n_events, ml_counters, LZ4, the tail and the
+ * capacity as for lc_split_regex_parse_sls.  A chunk whose pieces are all erased or discarded gives 0 bytes (the LZ4
+ * calls: the block of the tail alone). */
+int lc_split_regex_timestamp_parse_sls(
+    lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len, uint8_t split_char,
+    const char* const* keys, const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+    uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed,
+    int copy_raw, int whole_line, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+    uint32_t time_ns, const char* tkey, uint32_t tkey_len, const struct lc_timestamp* ts, int64_t now,
+    int32_t discard_interval, int enable_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+    uint64_t counters[8]);
+int lc_split_regex_timestamp_parse_sls_lz4(
+    lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len, uint8_t split_char,
+    const char* const* keys, const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+    uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed,
+    int copy_raw, int whole_line, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+    uint32_t time_ns, const char* tkey, uint32_t tkey_len, const struct lc_timestamp* ts, int64_t now,
+    int32_t discard_interval, int enable_ns, const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+    uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events, uint64_t counters[8]);
+int lc_multiline_split_regex_timestamp_parse_sls(
+    lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+    const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, const char* const* keys,
+    const uint32_t* key_lens, uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+    uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, int whole_line, const char* offset_key,
+    uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns, const char* tkey, uint32_t tkey_len,
+    const struct lc_timestamp* ts, int64_t now, int32_t discard_interval, int enable_ns, uint8_t* out, uint64_t out_cap,
+    uint64_t* out_len, uint64_t* n_events, uint64_t counters[8], uint64_t ml_counters[3]);
+int lc_multiline_split_regex_timestamp_parse_sls_lz4(
+    lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+    const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, const char* const* keys,
+    const uint32_t* key_lens, uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+    uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, int whole_line, const char* offset_key,
+    uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns, const char* tkey, uint32_t tkey_len,
+    const struct lc_timestamp* ts, int64_t now, int32_t discard_interval, int enable_ns, const uint8_t* tail,
+    uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+    uint64_t counters[8], uint64_t ml_counters[3]);
+
 /* lc_regex_parse_sls / lc_delim_parse_sls finished as the SLS flusher finishes a group: the records, followed by
  * tail[0, tail_len) (the group-level fields: topic, source, machine uuid, tags), become ONE LZ4 block (the block format
  * of lc_lz4_compress_dev) and only the block comes back.  *raw_len = records + tail bytes (x-log-bodyrawsize),

@@ -140,6 +140,20 @@ def lib():
         sr_tail + [vp, vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
     L.lc_multiline_split_regex_filter_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sls_cfg + \
         [i32] + sr_tail + [vp, vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
+    # the split -> regex -> timestamp chain: the siblings' arguments with the timestamp stage behind time_ns
+    ts_cfg = [C.c_char_p, u32, vp, C.c_int64, i32, i32]  # tkey, tkey_len, ts, now, discard_interval, enable_ns
+    L.lc_split_regex_timestamp_tap_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32] + sls_cfg + \
+        [i32, C.c_char_p, u32, C.c_char_p, u32, vp, vp]
+    L.lc_sls_serialize_split_regex_timestamp_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32] + sls_cfg + \
+        [i32] + sr_tail + [vp, vp, vp, i32, vp, u64, C.POINTER(u64), vp]
+    L.lc_split_regex_timestamp_parse_sls.argtypes = [vp, vp, vp, u64, u8] + sls_cfg + [i32] + sr_tail + ts_cfg + \
+        [vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_split_regex_timestamp_parse_sls_lz4.argtypes = [vp, vp, vp, u64, u8] + sls_cfg + [i32] + sr_tail + \
+        ts_cfg + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_multiline_split_regex_timestamp_parse_sls.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sls_cfg + \
+        [i32] + sr_tail + ts_cfg + [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
+    L.lc_multiline_split_regex_timestamp_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sls_cfg + \
+        [i32] + sr_tail + ts_cfg + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
     # the split -> delimiter chain: the delimiter's arguments (sep .. copy_raw), then the split -> regex tail
     sd_cfg = [vp, u32, u8, i32, i32, i32, u32]  # sep .. max_fields of the host-buffer calls
     L.lc_sls_serialize_split_delim_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, vp, u32, vp, u32, u8,
@@ -806,10 +820,11 @@ class Engine:
         return int(need.value), ctr
 
     def _split_regex(self, fn, rx, buf, extra, keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw,
-                     whole_line, offset_key, src_pos, time, time_ns, out_cap, ml, tail, filt=None):
+                     whole_line, offset_key, src_pos, time, time_ns, out_cap, ml, tail, filt=None, tsx=None):
         """one host-buffer split -> regex call, sized by an estimate first and by the exact size when that was short;
         tail None: the wire bytes, else records ‖ tail as one LZ4 block.  filt (a Filter): the _filter_ call, with
-        counters[4].  Returns (bytes, raw_len, n_events, counters[3] or [4], ml_counters[3] or None)"""
+        counters[4]; tsx (_ts_args): the _timestamp_ call, with counters[8].  Returns (bytes, raw_len, n_events,
+        counters[3], [4] or [8], ml_counters[3] or None)"""
         a = _u8(buf)
         _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
         tl = None if tail is None else np.frombuffer(bytes(tail), np.uint8)
@@ -818,10 +833,10 @@ class Engine:
         for _ in range(2):
             out = np.empty(max(cap, 1), np.uint8)
             need, raw, nev = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
-            ctr, mctr = np.zeros(3 if filt is None else 4, np.uint64), np.zeros(3, np.uint64)
+            ctr, mctr = np.zeros(8 if tsx else 3 if filt is None else 4, np.uint64), np.zeros(3, np.uint64)
             z = [] if tl is None else [_p(tl) if tl.size else None, tl.size]
             outs = [_p(out), cap, C.byref(need)] + ([] if tl is None else [C.byref(raw)]) + [C.byref(nev), _p(ctr)]
-            f = [] if filt is None else [filt.ptr()]
+            f = ([] if filt is None else [filt.ptr()]) + (tsx or [])
             rc = fn(self._h, _rh(rx), _p(a), a.size, *extra, *cfg, int(bool(whole_line)),
                     *self._sr_tail(offset_key, src_pos, time, time_ns), *f, *z, *outs, *([_p(mctr)] if ml else []))
             if rc == LC_ERR_CAPACITY and out_cap is None:
@@ -938,6 +953,99 @@ class Engine:
             lib().lc_multiline_split_regex_filter_parse_sls_lz4, rx, buf,
             [_rh(start), _rh(cont), _rh(end), int(bool(discard))], keys, source_key, renamed_key, keep_fail,
             keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, True, tail, filt)
+
+    @staticmethod
+    def _ts_args(tkey, ts, now, discard_interval, enable_ns):
+        """the timestamp stage of the split -> regex -> timestamp calls: SourceKey tkey (bytes), the compiled
+        Timestamp ts, now (time(NULL)), discard_interval (-1 = no history discard), enable_ns"""
+        return [tkey, len(tkey), ts._h, int(now), int(discard_interval), int(bool(enable_ns))]
+
+    def split_regex_timestamp_tap_dev(self, d_src, src_len, d_off, d_len, n, d_status, d_cap_off, d_cap_len,
+                                      row_pitch, keys, source_key, tkey, d_val_off, d_val_len, renamed_key=None,
+                                      keep_fail=False, keep_succeed=False, copy_raw=False, whole_line=False,
+                                      offset_key=None):
+        """The timestamp stage's value table (d_val_off, d_val_len; LC_TS_NO_KEY = no value) from the device piece
+        and regex tables of the split -> regex chain (lc_split_regex_timestamp_tap_dev); queued, not waited for."""
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        _check(lib().lc_split_regex_timestamp_tap_dev(
+            self._h, _p(d_src), src_len, _p(d_off), _p(d_len), n, _p(d_status), _p(d_cap_off), _p(d_cap_len),
+            row_pitch, *cfg, int(bool(whole_line)), *self._sr_tail(offset_key, 0, 0, None)[:2], tkey, len(tkey),
+            _p(d_val_off), _p(d_val_len)))
+
+    def sls_serialize_split_regex_timestamp_dev(self, d_src, src_len, d_off, d_len, n, d_status, d_cap_off,
+                                                d_cap_len, row_pitch, keys, source_key, d_ts_status, d_ts_sec,
+                                                d_ts_nsec, enable_ns=False, renamed_key=None, keep_fail=False,
+                                                keep_succeed=False, copy_raw=False, whole_line=False, offset_key=None,
+                                                src_pos=0, time=0, time_ns=None, d_out=None, out_cap=0):
+        """sls_serialize_split_regex_dev with each record's time from the device results of timestamp_parse_dev over
+        the tap's value table (lc_sls_serialize_split_regex_timestamp_dev).  Returns (byte count, counters[8] = the
+        regex stage's three, then key_not_found, out_failed, history_failure, discarded, out_successful); with d_out
+        None the byte count needed."""
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        need = C.c_uint64(0)
+        ctr = np.zeros(8, np.uint64)
+        rc = lib().lc_sls_serialize_split_regex_timestamp_dev(
+            self._h, _p(d_src), src_len, _p(d_off), _p(d_len), n, _p(d_status), _p(d_cap_off), _p(d_cap_len),
+            row_pitch, *cfg, int(bool(whole_line)), *self._sr_tail(offset_key, src_pos, time, time_ns),
+            _p(d_ts_status), _p(d_ts_sec), _p(d_ts_nsec), int(bool(enable_ns)), _p(d_out), out_cap, C.byref(need),
+            _p(ctr))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value), ctr  # a sizing query
+        _check(rc)
+        return int(need.value), ctr
+
+    def split_regex_timestamp_parse_sls(self, rx, buf, split_char, keys, source_key, tkey, ts, now,
+                                        discard_interval=-1, enable_ns=False, renamed_key=None, keep_fail=False,
+                                        keep_succeed=False, copy_raw=False, whole_line=False, offset_key=None,
+                                        src_pos=0, time=0, time_ns=None, out_cap=None):
+        """split_regex_parse_sls with ProcessorParseTimestampNative (SourceKey tkey, the compiled Timestamp ts)
+        behind the regex stage (lc_split_regex_timestamp_parse_sls).  Returns (bytes, number of pieces,
+        counters[8])."""
+        data, _raw, nev, ctr, _m = self._split_regex(
+            lib().lc_split_regex_timestamp_parse_sls, rx, buf, [split_char], keys, source_key, renamed_key,
+            keep_fail, keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, False, None,
+            None, self._ts_args(tkey, ts, now, discard_interval, enable_ns))
+        return data, nev, ctr
+
+    def split_regex_timestamp_parse_sls_lz4(self, rx, buf, split_char, keys, source_key, tkey, ts, now,
+                                            discard_interval=-1, enable_ns=False, renamed_key=None, keep_fail=False,
+                                            keep_succeed=False, copy_raw=False, whole_line=False, offset_key=None,
+                                            src_pos=0, time=0, time_ns=None, tail=b"", out_cap=None):
+        """split_regex_timestamp_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_split_regex_timestamp_parse_sls_lz4).  Returns (block, raw_len, number of pieces, counters[8])."""
+        data, raw, nev, ctr, _m = self._split_regex(
+            lib().lc_split_regex_timestamp_parse_sls_lz4, rx, buf, [split_char], keys, source_key, renamed_key,
+            keep_fail, keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, False, tail,
+            None, self._ts_args(tkey, ts, now, discard_interval, enable_ns))
+        return data, raw, nev, ctr
+
+    def multiline_split_regex_timestamp_parse_sls(self, rx, buf, start, cont, end, discard, keys, source_key, tkey,
+                                                  ts, now, discard_interval=-1, enable_ns=False, renamed_key=None,
+                                                  keep_fail=False, keep_succeed=False, copy_raw=False,
+                                                  whole_line=False, offset_key=None, src_pos=0, time=0, time_ns=None,
+                                                  out_cap=None):
+        """The same with the multiline splitter (lc_multiline_split_regex_timestamp_parse_sls).  Returns (bytes,
+        number of events, counters[8], splitter counters[3])."""
+        data, _raw, nev, ctr, mctr = self._split_regex(
+            lib().lc_multiline_split_regex_timestamp_parse_sls, rx, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], keys, source_key, renamed_key, keep_fail,
+            keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, True, None, None,
+            self._ts_args(tkey, ts, now, discard_interval, enable_ns))
+        return data, nev, ctr, mctr
+
+    def multiline_split_regex_timestamp_parse_sls_lz4(self, rx, buf, start, cont, end, discard, keys, source_key,
+                                                      tkey, ts, now, discard_interval=-1, enable_ns=False,
+                                                      renamed_key=None, keep_fail=False, keep_succeed=False,
+                                                      copy_raw=False, whole_line=False, offset_key=None, src_pos=0,
+                                                      time=0, time_ns=None, tail=b"", out_cap=None):
+        """multiline_split_regex_timestamp_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_multiline_split_regex_timestamp_parse_sls_lz4).  Returns (block, raw_len, number of events, counters[8],
+        splitter counters[3])."""
+        return self._split_regex(
+            lib().lc_multiline_split_regex_timestamp_parse_sls_lz4, rx, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], keys, source_key, renamed_key, keep_fail,
+            keep_succeed, copy_raw, whole_line, offset_key, src_pos, time, time_ns, out_cap, True, tail, None,
+            self._ts_args(tkey, ts, now, discard_interval, enable_ns))
 
     def sls_serialize_split_delim_dev(self, d_src, src_len, d_off, d_len, n, d_status, d_nf, d_fo, d_fl, d_fd,
                                       max_fields, sep: bytes, quote, treatment, keys, source_key, renamed_key=None,
@@ -1422,7 +1530,8 @@ def host_chain3_serialize_sls(split, regex, filt, group, enable_ns=False, mode=0
     """The split -> regex -> filter chain of three HostProcessors on a JSON group (lc_host_chain3_serialize_sls).
     mode 0: split's SerializeSls(group, regex, filter); 1: Process x 3 + Serialize; 2: SerializeSlsLz4.  Returns (bytes,
     raw_len, None) or (None, 0, error).  The split -> delimiter -> regex chain goes through the same call, with a
-    delimiter processor as `regex` and a regex processor as `filt`."""
+    delimiter processor as `regex` and a regex processor as `filt`; so does the split -> regex -> timestamp chain, with
+    a timestamp processor as `filt`."""
     import json
     L = lib()
     L.lc_host_chain3_serialize_sls.restype = C.c_void_p

@@ -119,6 +119,9 @@ struct lc_engine {
     // results, the host call's counters
     DevBuf ts_conf, ts_full, ts_cnt;
     uint64_t ts_conf_id = 0;
+    // split -> regex -> timestamp chain: the tap's value table and group starts, the timestamp tables over the pieces;
+    // the chain's piece and regex tables are the split -> regex chain's (in, out_a, out_b, dr_*)
+    DevBuf st_val, st_sec, st_nsec, st_status;
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
     std::unordered_map<uint64_t, void*> blobs; // regex id * 4 + layout -> device blob
@@ -336,7 +339,7 @@ void lc_engine_destroy(lc_engine_t* e) {
                       &e->dr_keys, &e->dr_val_off, &e->dr_val_len, &e->dr_status, &e->dr_cap_off, &e->dr_cap_len,
                       &e->dr_copy, &e->dr_slot, &e->dr_desc, &e->fl_tab, &e->fl_match, &e->fl_dig, &e->fl_keep,
                       &e->sdr_status, &e->sdr_nf, &e->sdr_f_off, &e->sdr_f_len, &e->sdr_f_dq, &e->sdr_okey,
-                      &e->ts_conf, &e->ts_full, &e->ts_cnt};
+                      &e->ts_conf, &e->ts_full, &e->ts_cnt, &e->st_val, &e->st_sec, &e->st_nsec, &e->st_status};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -2789,12 +2792,29 @@ static_assert(LC_FILTER_MAX_LEAVES == LC_FILTER_SLS_LEAVES && LC_FILTER_MAX_PROG
 
 namespace {
 
+// The timestamp stage of the split -> regex -> timestamp calls: its SourceKey, the compiled SourceFormat, the call's
+// time(NULL), the history discard (-1 = none) and mEnableTimestampNanosecond
+struct TsArgs {
+    const char* tkey;
+    uint32_t tkey_len;
+    const lc_timestamp_t* ts;
+    int64_t now;
+    int32_t discard_interval;
+    int enable_ns;
+};
+
+int ts_run(lc_engine_t* e, const lc_timestamp_t* ts, const uint8_t* d_base, const LcTsSpans& sp, uint64_t n,
+           const uint32_t* d_grp, uint64_t ngroups, int64_t now, int32_t discard_interval, int64_t* d_sec,
+           uint32_t* d_nsec, uint8_t* d_status, uint64_t* d_counters);
+
 // lc_split_regex_sls_setup's plans over the key table keys..., SourceKey, RenamedSourceKey, "__raw_log__", "content",
 // offset_key, staged on the device (`sls_plan`, which neither splitter nor the regex stage uses).  Every single
 // content then stays below 4 GiB; a record that would not is caught by the size pass.  With fd, the filter behind the
-// chain is checked and resolved against those plans into *f (lc_filter_sls_setup).
+// chain is checked and resolved against those plans into *f (lc_filter_sls_setup); with tkey (the timestamp calls),
+// the timestamp stage's SourceKey into *tc (lc_split_regex_ts_setup).
 int split_regex_sls_config(lc_engine_t* e, const char* what, uint64_t src_len, SPLIT_REGEX_PARAMS, uint32_t pitch,
-                           LcSplitRegexSlsCfg* c, const lc_filter_desc_t* fd = nullptr, LcFilterSlsCfg* f = nullptr) {
+                           LcSplitRegexSlsCfg* c, const lc_filter_desc_t* fd = nullptr, LcFilterSlsCfg* f = nullptr,
+                           const TsArgs* ta = nullptr, LcSplitRegexTsCfg* tc = nullptr) {
     if ((nkeys && (!keys || !key_lens)) || (source_key_len && !source_key) || (renamed_key_len && !renamed_key))
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
     uint64_t kbytes = (uint64_t)source_key_len + renamed_key_len + (offset_key ? offset_key_len : 0u) + 18;
@@ -2811,10 +2831,10 @@ int split_regex_sls_config(lc_engine_t* e, const char* what, uint64_t src_len, S
                                                copy_raw, whole_line, pitch, src_pos, time, time_ns, c, plan.data());
     if (why)
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
-    std::vector<const char*> strings(keys, keys + nkeys);
-    std::vector<uint32_t> lens(key_lens, key_lens + nkeys);
-    strings.insert(strings.end(), {source_key, renamed_key, "__raw_log__", "content", offset_key});
-    lens.insert(lens.end(), {source_key_len, renamed_key_len, 11u, 7u, offset_key ? offset_key_len : 0u});
+    std::vector<const char*> strings(nkeys + LC_SPLIT_REGEX_SLS_NSTR);
+    std::vector<uint32_t> lens(nkeys + LC_SPLIT_REGEX_SLS_NSTR);
+    lc_split_regex_sls_strings(keys, key_lens, nkeys, source_key, source_key_len, renamed_key, renamed_key_len,
+                               offset_key, offset_key_len, strings.data(), lens.data());
     if (fd) {
         why = lc_filter_sls_setup(plan.data(), c->x.n_ok, c->x.n_fail, strings.data(), lens.data(), fd->nleaves,
                                   fd->keys, fd->key_lens, fd->nprog, fd->prog, f);
@@ -2828,7 +2848,37 @@ int split_regex_sls_config(lc_engine_t* e, const char* what, uint64_t src_len, S
                 return rc;
         }
     }
-    return stage_regex_sls(e, what, plan.data(), strings.data(), lens.data(), nkeys + 5, &c->x);
+    if (ta) {
+        why = lc_split_regex_ts_setup(*c, plan.data(), strings.data(), lens.data(), ta->tkey, ta->tkey_len,
+                                      ta->enable_ns, tc);
+        if (why)
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    }
+    return stage_regex_sls(e, what, plan.data(), strings.data(), lens.data(), nkeys + LC_SPLIT_REGEX_SLS_NSTR, &c->x);
+}
+
+// The split -> regex -> timestamp chain's tap and timestamp passes over the n pieces of t: the value table into
+// st_val, then lc_timestamp_parse_dev's two passes with the whole source value as one group into *ts (st_status,
+// st_sec, st_nsec).  The stage's counters are the size pass's, so the passes' own go to ts_cnt unread.
+int split_regex_ts_run(lc_engine_t* e, const LcSplitRegexSlsCfg& c, const LcSplitRegexTsCfg& tc, const TsArgs& ta,
+                       const lck::RegexSlsTables& t, uint64_t n, lck::TsRowTables* ts) {
+    CU_TRY(e->st_val.ensure(n * 8 + 8));
+    CU_TRY(e->st_sec.ensure(n * 8));
+    CU_TRY(e->st_nsec.ensure(n * 4));
+    CU_TRY(e->st_status.ensure(n));
+    CU_TRY(e->ts_cnt.ensure(5 * sizeof(uint64_t)));
+    uint32_t* off = e->st_val.as<uint32_t>();
+    uint32_t *len = off + n, *grp = off + 2 * n;
+    const uint32_t g[2] = {0u, (uint32_t)n};
+    CU_TRY(cudaMemcpyAsync(grp, g, sizeof g, cudaMemcpyHostToDevice, e->stream));
+    lck::launch_split_regex_ts_tap(c, tc, t, n, off, len, e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    const int rc = ts_run(e, ta.ts, t.base, LcTsSpans{off, len, nullptr, 1}, n, grp, 1, ta.now, ta.discard_interval,
+                          e->st_sec.as<int64_t>(), e->st_nsec.as<uint32_t>(), e->st_status.as<uint8_t>(),
+                          e->ts_cnt.as<uint64_t>());
+    *ts = lck::TsRowTables{e->st_status.as<uint8_t>(), e->st_sec.as<int64_t>(), e->st_nsec.as<uint32_t>()};
+    return rc;
 }
 
 // The filter over the n pieces of t: leaf by leaf, the tap and the boolean match over the source value (and over the
@@ -2884,25 +2934,34 @@ int filter_sls_run(lc_engine_t* e, const char* what, const LcSplitRegexSlsCfg& c
 
 // The size pass and the emit of the chain over n pieces (serialize_sls_dev): into d_out (the device-fed call), or
 // back to the host buffer out, or -- with z -- records ‖ tail as one LZ4 block.  counters[3] = successful, failed,
-// discarded; set whenever the size pass ran.
+// discarded; set whenever the size pass ran.  With tc (the timestamp calls), each record's time comes from the
+// timestamp tables ts and counters has LC_SRTS_COUNTERS entries.
 int split_regex_sls_run(lc_engine_t* e, const char* what, const LcSplitRegexSlsCfg& c, const lck::RegexSlsTables& t,
                         uint64_t n, uint8_t* d_out, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
-                        uint64_t counters[3], const Lz4Tail* z, const uint8_t* keep = nullptr) {
-    uint64_t ctr[4] = {0, 0, 0, 0}; // + pieces whose record would reach 4 GiB
+                        uint64_t* counters, const Lz4Tail* z, const uint8_t* keep = nullptr,
+                        const LcSplitRegexTsCfg* tc = nullptr, const lck::TsRowTables* ts = nullptr) {
+    const uint32_t nstage = tc ? LC_SRTS_COUNTERS : 3u;
+    uint64_t ctr[LC_SRTS_COUNTERS + 1] = {0}; // + pieces whose record would reach 4 GiB
     SlsTo to;
     to.host = out;
     to.z = z;
-    to.too_large = 3;
+    to.too_large = (int)nstage;
     const int rc = serialize_sls_dev(
-        e, what, n, 4,
+        e, what, n, nstage + 1,
         [&](uint32_t* rec, uint32_t* body, unsigned long long* d_ctr) {
-            lck::launch_split_regex_sls_sizes(c, t, n, keep, rec, body, d_ctr, e->stream);
+            if (tc)
+                lck::launch_split_regex_ts_sls_sizes(c, *tc, t, *ts, n, rec, body, d_ctr, e->stream);
+            else
+                lck::launch_split_regex_sls_sizes(c, t, n, keep, rec, body, d_ctr, e->stream);
         },
         [&](const uint64_t* rec_off, const uint32_t* body, uint8_t* dst) {
-            lck::launch_split_regex_sls_emit(c, t, n, rec_off, body, dst, e->stream);
+            if (tc)
+                lck::launch_split_regex_ts_sls_emit(c, *tc, t, *ts, n, rec_off, body, dst, e->stream);
+            else
+                lck::launch_split_regex_sls_emit(c, t, n, rec_off, body, dst, e->stream);
         },
         d_out, out_cap, out_len, ctr, to);
-    memcpy(counters, ctr, 3 * sizeof(uint64_t));
+    memcpy(counters, ctr, nstage * sizeof(uint64_t));
     return rc;
 }
 
@@ -2954,12 +3013,14 @@ int split_chain_sls_host(lc_engine_t* e, const char* what, const uint8_t* buf, u
 
 // The regex stage of the split -> regex calls (split_regex_sls_host) over the n pieces: the regex tables go to
 // dr_status / dr_cap_off / dr_cap_len; with fd (the _filter_ calls), the filter runs between the regex stage and the
-// size pass and counters has a 4th entry.
+// size pass and counters has a 4th entry; with ta (the _timestamp_ calls), the tap and the timestamp passes run there
+// and counters has LC_SRTS_COUNTERS entries.
 int split_regex_sls_stage(lc_engine_t* e, const char* what, const lc_regex_t* re, uint64_t len, uint64_t n, uint32_t G,
                           uint32_t nkeys, int whole_line, const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f,
                           const lc_filter_desc_t* fd, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
-                          size_t nctr, uint64_t* counters, const Lz4Tail* z) {
-    uint64_t ctr[4] = {0, 0, 0, 0};
+                          size_t nctr, uint64_t* counters, const Lz4Tail* z, const TsArgs* ta = nullptr,
+                          const LcSplitRegexTsCfg* tc = nullptr) {
+    uint64_t ctr[LC_SRTS_COUNTERS] = {0};
     int rc;
     if (n * (uint64_t)G >= (1ull << 32))
         return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^32 captures per call");
@@ -2985,7 +3046,13 @@ int split_regex_sls_stage(lc_engine_t* e, const char* what, const lc_regex_t* re
         if (rc)
             return rc;
     }
-    rc = split_regex_sls_run(e, what, c, t, n, nullptr, out, out_cap, out_len, ctr, z, keep);
+    lck::TsRowTables ts{};
+    if (ta) {
+        rc = split_regex_ts_run(e, c, *tc, *ta, t, n, &ts);
+        if (rc)
+            return rc;
+    }
+    rc = split_regex_sls_run(e, what, c, t, n, nullptr, out, out_cap, out_len, ctr, z, keep, ta ? tc : nullptr, &ts);
     if (d_removed && (rc == LC_OK || rc == LC_ERR_CAPACITY)) {
         CU_TRY(cudaMemcpyAsync(&ctr[3], d_removed, 8, cudaMemcpyDeviceToHost, e->stream));
         CU_TRY(cudaStreamSynchronize(e->stream));
@@ -2999,12 +3066,13 @@ int split_regex_sls_stage(lc_engine_t* e, const char* what, const lc_regex_t* re
 template <class Split>
 int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
                          Split split, SPLIT_REGEX_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
-                         uint64_t* n_events, uint64_t counters[3], const Lz4Tail* z,
-                         const lc_filter_desc_t* fd = nullptr) {
-    const size_t nctr = fd ? 4 : 3;
+                         uint64_t* n_events, uint64_t* counters, const Lz4Tail* z,
+                         const lc_filter_desc_t* fd = nullptr, const TsArgs* ta = nullptr) {
+    const size_t nctr = fd ? 4 : ta ? LC_SRTS_COUNTERS : 3;
     uint32_t G = 0;
     LcSplitRegexSlsCfg c;
     LcFilterSlsCfg f;
+    LcSplitRegexTsCfg tc;
     auto begin = [&]() {
         if (counters)
             memset(counters, 0, nctr * sizeof(uint64_t));
@@ -3012,38 +3080,40 @@ int split_regex_sls_host(lc_engine_t* e, const char* what, const lc_regex_t* re,
     };
     auto config = [&]() {
         G = whole_line ? 0u : re->res.ngroups;
-        return split_regex_sls_config(e, what, len, SPLIT_REGEX_ARGS, G, &c, fd, &f);
+        return split_regex_sls_config(e, what, len, SPLIT_REGEX_ARGS, G, &c, fd, &f, ta, &tc);
     };
     auto run = [&](uint64_t n) {
         return split_regex_sls_stage(e, what, re, len, n, G, nkeys, whole_line, c, f, fd, out, out_cap, out_len, nctr,
-                                     counters, z);
+                                     counters, z, ta, &tc);
     };
-    return split_chain_sls_host(e, what, buf, len, split, re || whole_line, begin, config, run, out, out_cap,
-                                out_len, n_events, z);
+    return split_chain_sls_host(e, what, buf, len, split, (re || whole_line) && (!ta || ta->ts), begin, config, run,
+                                out, out_cap, out_len, n_events, z);
 }
 
 template <class Split>
 int split_regex_lz4_host(lc_engine_t* e, const char* what, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
                          Split split, SPLIT_REGEX_PARAMS, const uint8_t* tail, uint64_t tail_len, uint8_t* out,
                          uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
-                         uint64_t counters[3], const lc_filter_desc_t* fd = nullptr) {
+                         uint64_t* counters, const lc_filter_desc_t* fd = nullptr, const TsArgs* ta = nullptr) {
     const Lz4Tail z{tail, tail_len, raw_len};
     return split_regex_sls_host(e, what, re, buf, len, split, SPLIT_REGEX_ARGS, out, out_cap, out_len, n_events,
-                                counters, &z, fd);
+                                counters, &z, fd, ta);
 }
 
-// lc_sls_serialize_split_regex_dev and its _filter_ sibling (fd; counters then has a 4th entry)
+// lc_sls_serialize_split_regex_dev and its _filter_ sibling (fd; counters then has a 4th entry) and _timestamp_
+// sibling (tc, ts: the timestamp tables; counters then has LC_SRTS_COUNTERS entries)
 int split_regex_sls_dev(lc_engine_t* e, const char* what, const uint8_t* d_src, uint64_t src_len,
                         const uint32_t* d_off, const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
                         const uint32_t* d_cap_off, const uint32_t* d_cap_len, uint32_t row_pitch, SPLIT_REGEX_PARAMS,
                         const lc_filter_desc_t* fd, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len,
-                        uint64_t* counters) {
+                        uint64_t* counters, const LcSplitRegexTsCfg* tc = nullptr,
+                        const lck::TsRowTables* ts = nullptr) {
     const bool caps = !whole_line && nkeys && nkeys <= row_pitch; // the parsed plan reads the capture tables
     if (!e || !out_len || (n && (!d_src || !d_off || !d_len)) || (n && !whole_line && !d_status) ||
-        (n && caps && (!d_cap_off || !d_cap_len)))
+        (n && caps && (!d_cap_off || !d_cap_len)) || (n && tc && (!ts->status || !ts->sec || !ts->nsec)))
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
     *out_len = 0;
-    const size_t nctr = fd ? 4 : 3;
+    const size_t nctr = fd ? 4 : tc ? LC_SRTS_COUNTERS : 3;
     if (counters)
         memset(counters, 0, nctr * sizeof(uint64_t));
     if (src_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)row_pitch >= (1ull << 32))
@@ -3054,8 +3124,13 @@ int split_regex_sls_dev(lc_engine_t* e, const char* what, const uint8_t* d_src, 
     LcSplitRegexSlsCfg c;
     LcFilterSlsCfg f;
     rc = split_regex_sls_config(e, what, src_len, SPLIT_REGEX_ARGS, row_pitch, &c, fd, &f);
-    if (rc || n == 0)
+    if (rc)
         return rc;
+    const char* why = tc ? lc_split_regex_ts_ns_check(c, (int)tc->enable_ns) : nullptr;
+    if (why)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    if (n == 0)
+        return LC_OK;
     const lck::RegexSlsTables t{d_src, d_off, d_len, whole_line ? nullptr : d_status, caps ? d_cap_off : nullptr,
                                 caps ? d_cap_len : nullptr};
     const uint8_t* keep = nullptr;
@@ -3065,8 +3140,8 @@ int split_regex_sls_dev(lc_engine_t* e, const char* what, const uint8_t* d_src, 
         if (rc)
             return rc;
     }
-    uint64_t ctr[4] = {0, 0, 0, 0};
-    rc = split_regex_sls_run(e, what, c, t, n, d_out, nullptr, out_cap, out_len, ctr, nullptr, keep);
+    uint64_t ctr[LC_SRTS_COUNTERS] = {0};
+    rc = split_regex_sls_run(e, what, c, t, n, d_out, nullptr, out_cap, out_len, ctr, nullptr, keep, tc, ts);
     if (d_removed && (rc == LC_OK || rc == LC_ERR_CAPACITY)) {
         CU_TRY(cudaMemcpyAsync(&ctr[3], d_removed, 8, cudaMemcpyDeviceToHost, e->stream));
         CU_TRY(cudaStreamSynchronize(e->stream));
@@ -3208,6 +3283,110 @@ int lc_multiline_split_regex_filter_parse_sls_lz4(lc_engine_t* e, const lc_regex
                                 filter);
 }
 #undef FILTER_CHECK
+
+int lc_split_regex_timestamp_tap_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+                                     const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                     const uint32_t* d_cap_off, const uint32_t* d_cap_len, uint32_t row_pitch,
+                                     const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                                     const char* source_key, uint32_t source_key_len, const char* renamed_key,
+                                     uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                                     int whole_line, const char* offset_key, uint32_t offset_key_len,
+                                     const char* tkey, uint32_t tkey_len, uint32_t* d_val_off, uint32_t* d_val_len) {
+    static const char* what = "lc_split_regex_timestamp_tap_dev";
+    const bool caps = !whole_line && nkeys && nkeys <= row_pitch;
+    if (!e || (n && (!d_src || !d_off || !d_len || !d_val_off || !d_val_len)) || (n && !whole_line && !d_status) ||
+        (n && caps && (!d_cap_off || !d_cap_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    if (src_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)row_pitch >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 pieces and < 2^32 captures per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    const uint64_t src_pos = 0;
+    const uint32_t time = 0, time_ns = LC_SLS_NO_NS;
+    const TsArgs ta{tkey, tkey_len, nullptr, 0, -1, 0};
+    LcSplitRegexSlsCfg c;
+    LcSplitRegexTsCfg tc;
+    rc = split_regex_sls_config(e, what, src_len, SPLIT_REGEX_ARGS, row_pitch, &c, nullptr, nullptr, &ta, &tc);
+    if (rc || n == 0)
+        return rc;
+    const lck::RegexSlsTables t{d_src, d_off, d_len, whole_line ? nullptr : d_status, caps ? d_cap_off : nullptr,
+                                caps ? d_cap_len : nullptr};
+    lck::launch_split_regex_ts_tap(c, tc, t, n, d_val_off, d_val_len, e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    return LC_OK;
+}
+
+int lc_sls_serialize_split_regex_timestamp_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len,
+                                               const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+                                               const uint8_t* d_status, const uint32_t* d_cap_off,
+                                               const uint32_t* d_cap_len, uint32_t row_pitch, SPLIT_REGEX_PARAMS,
+                                               const uint8_t* d_ts_status, const int64_t* d_ts_sec,
+                                               const uint32_t* d_ts_nsec, int enable_ns, uint8_t* d_out,
+                                               uint64_t out_cap, uint64_t* out_len, uint64_t counters[8]) {
+    const LcSplitRegexTsCfg tc{{LC_FILTER_SLS_ABSENT, LC_FILTER_SLS_ABSENT}, enable_ns != 0 ? 1u : 0u};
+    const lck::TsRowTables ts{d_ts_status, d_ts_sec, d_ts_nsec};
+    return split_regex_sls_dev(e, "lc_sls_serialize_split_regex_timestamp_dev", d_src, src_len, d_off, d_len, n,
+                               d_status, d_cap_off, d_cap_len, row_pitch, SPLIT_REGEX_ARGS, nullptr, d_out, out_cap,
+                               out_len, counters, &tc, &ts);
+}
+
+#define TS_ARGS_OF_CALL const TsArgs ta{tkey, tkey_len, ts, now, discard_interval, enable_ns};
+
+int lc_split_regex_timestamp_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                       uint8_t split_char, SPLIT_REGEX_PARAMS, const char* tkey, uint32_t tkey_len,
+                                       const lc_timestamp_t* ts, int64_t now, int32_t discard_interval, int enable_ns,
+                                       uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                       uint64_t counters[8]) {
+    TS_ARGS_OF_CALL
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_regex_sls_host(e, "lc_split_regex_timestamp_parse_sls", re, buf, len, split, SPLIT_REGEX_ARGS, out,
+                                out_cap, out_len, n_events, counters, nullptr, nullptr, &ta);
+}
+
+int lc_split_regex_timestamp_parse_sls_lz4(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len,
+                                           uint8_t split_char, SPLIT_REGEX_PARAMS, const char* tkey,
+                                           uint32_t tkey_len, const lc_timestamp_t* ts, int64_t now,
+                                           int32_t discard_interval, int enable_ns, const uint8_t* tail,
+                                           uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                                           uint64_t* raw_len, uint64_t* n_events, uint64_t counters[8]) {
+    TS_ARGS_OF_CALL
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_regex_lz4_host(e, "lc_split_regex_timestamp_parse_sls_lz4", re, buf, len, split, SPLIT_REGEX_ARGS,
+                                tail, tail_len, out, out_cap, out_len, raw_len, n_events, counters, nullptr, &ta);
+}
+
+int lc_multiline_split_regex_timestamp_parse_sls(lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf,
+                                                 uint64_t len, const lc_regex_t* start, const lc_regex_t* cont,
+                                                 const lc_regex_t* end, int discard_unmatched, SPLIT_REGEX_PARAMS,
+                                                 const char* tkey, uint32_t tkey_len, const lc_timestamp_t* ts,
+                                                 int64_t now, int32_t discard_interval, int enable_ns, uint8_t* out,
+                                                 uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                                 uint64_t counters[8], uint64_t ml_counters[3]) {
+    TS_ARGS_OF_CALL
+    return split_regex_sls_host(e, "lc_multiline_split_regex_timestamp_parse_sls", re, buf, len, ML_SPLIT,
+                                SPLIT_REGEX_ARGS, out, out_cap, out_len, n_events, counters, nullptr, nullptr, &ta);
+}
+
+int lc_multiline_split_regex_timestamp_parse_sls_lz4(
+    lc_engine_t* e, const lc_regex_t* re, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+    const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, SPLIT_REGEX_PARAMS, const char* tkey,
+    uint32_t tkey_len, const lc_timestamp_t* ts, int64_t now, int32_t discard_interval, int enable_ns,
+    const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+    uint64_t* n_events, uint64_t counters[8], uint64_t ml_counters[3]) {
+    TS_ARGS_OF_CALL
+    return split_regex_lz4_host(e, "lc_multiline_split_regex_timestamp_parse_sls_lz4", re, buf, len, ML_SPLIT,
+                                SPLIT_REGEX_ARGS, tail, tail_len, out, out_cap, out_len, raw_len, n_events, counters,
+                                nullptr, &ta);
+}
+#undef TS_ARGS_OF_CALL
 
 } // extern "C"
 

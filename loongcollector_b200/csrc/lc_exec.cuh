@@ -1943,14 +1943,15 @@ LC_HD void lc_sls_digits(LcSlsWrite& s, uint64_t v, uint32_t nd) {
 }
 
 // The body of the piece's Log record -- Time, the contents of its plan, Time_ns -- into sink s (LcSlsCount /
-// LcSlsWrite / LcSlsCount64).  Returns the number of contents; 0 = erased or empty, no record.
+// LcSlsWrite / LcSlsCount64), with the record's own time and ns (has_ns = 0: no Time_ns).  Returns the number of
+// contents; 0 = erased or empty, no record.
 template <class S>
 LC_HD uint32_t lc_split_regex_sls_body(const LcSplitRegexSlsCfg& c, const uint8_t* src, const LcSplitRegexSlsRow& r,
-                                       S& s) {
+                                       uint32_t time, uint32_t has_ns, uint32_t ns, S& s) {
     {
         uint8_t h[6];
         h[0] = 0x08;
-        const uint32_t n = 1 + lc_put_varint(h + 1, c.time < (1u << 28) ? (1u << 28) : c.time); // always 5 bytes
+        const uint32_t n = 1 + lc_put_varint(h + 1, time < (1u << 28) ? (1u << 28) : time); // always 5 bytes
         s.put(h, n);
     }
     const bool ok = lc_regex_sls_verdict(c.x, r.status) == 0u;
@@ -1970,11 +1971,18 @@ LC_HD uint32_t lc_split_regex_sls_body(const LcSplitRegexSlsCfg& c, const uint8_
         else
             s.copy(src + (line ? r.po : r.co[vs]), vl);
     }
-    if (c.has_ns) {
-        const uint8_t h[5] = {0x25, (uint8_t)c.ns, (uint8_t)(c.ns >> 8), (uint8_t)(c.ns >> 16), (uint8_t)(c.ns >> 24)};
+    if (has_ns) {
+        const uint8_t h[5] = {0x25, (uint8_t)ns, (uint8_t)(ns >> 8), (uint8_t)(ns >> 16), (uint8_t)(ns >> 24)};
         s.put(h, 5);
     }
     return m;
+}
+
+// ... with the source event's time and ns, as every split piece inherits them
+template <class S>
+LC_HD uint32_t lc_split_regex_sls_body(const LcSplitRegexSlsCfg& c, const uint8_t* src, const LcSplitRegexSlsRow& r,
+                                       S& s) {
+    return lc_split_regex_sls_body(c, src, r, c.time, c.has_ns, c.ns, s);
 }
 
 // counting sink of the size pass in 64 bits: a body of 2^32 bytes or more is refused instead of wrapping
@@ -2021,6 +2029,27 @@ inline const char* lc_split_regex_sls_setup(const char* const* keys, const uint3
     c->has_ns = time_ns != 0xFFFFFFFFu;
     c->ns = c->has_ns ? time_ns : 0u;
     return nullptr;
+}
+
+// Host side: the key table the plans of lc_split_regex_sls_setup name, key id k = strings[k] / lens[k]: the regex keys,
+// then SourceKey, RenamedSourceKey, "__raw_log__", "content" and the offset key (empty when there is none).  strings
+// and lens take nkeys + LC_SPLIT_REGEX_SLS_NSTR entries.  The C-ABI stages this table on the device, and every host
+// check of a stage behind the chain (lc_filter_sls_setup, lc_split_regex_ts_setup) resolves its keys against it.
+#define LC_SPLIT_REGEX_SLS_NSTR 5
+inline void lc_split_regex_sls_strings(const char* const* keys, const uint32_t* key_lens, uint32_t nkeys,
+                                       const char* source_key, uint32_t source_len, const char* renamed_key,
+                                       uint32_t renamed_len, const char* offset_key, uint32_t offset_len,
+                                       const char** strings, uint32_t* lens) {
+    for (uint32_t k = 0; k < nkeys; ++k) {
+        strings[k] = keys[k];
+        lens[k] = key_lens[k];
+    }
+    const char* const s[LC_SPLIT_REGEX_SLS_NSTR] = {source_key, renamed_key, "__raw_log__", "content", offset_key};
+    const uint32_t l[LC_SPLIT_REGEX_SLS_NSTR] = {source_len, renamed_len, 11u, 7u, offset_key ? offset_len : 0u};
+    for (uint32_t k = 0; k < LC_SPLIT_REGEX_SLS_NSTR; ++k) {
+        strings[nkeys + k] = s[k];
+        lens[nkeys + k] = l[k];
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -2229,8 +2258,27 @@ struct LcFilterSlsCfg {
     uint8_t prog[LC_FILTER_SLS_PROG];      // leaf index, or 253 / 254 / 255 = not / and / or
 };
 
-// Host side: resolve the leaves against the chain's plans (lc_regex_sls_plans: entries [0, n_ok) parsed, then n_fail
-// failed; key id k names kstr[k] / klen[k]) and check the program.  Returns nullptr, or why the filter is refused: more
+// Host side: where `key` (key[0, len)) is in the event the regex stage leaves behind, per verdict: src[0] in a parsed
+// event, src[1] in a failed one.  Each is capture j, LC_REGEX_SLS_LINE, LC_REGEX_SLS_DIGITS or LC_FILTER_SLS_ABSENT.
+// plan: the chain's plans (lc_regex_sls_plans: entries [0, n_ok) parsed, then n_fail failed; key id k names kstr[k] /
+// klen[k]); a plan's keys are unique.
+inline void lc_regex_sls_key_src(const uint32_t* plan, uint32_t n_ok, uint32_t n_fail, const char* const* kstr,
+                                 const uint32_t* klen, const char* key, uint32_t len, uint32_t src[2]) {
+    for (uint32_t v = 0; v < 2; ++v) {
+        const uint32_t* e = plan + (v ? 2u * n_ok : 0u);
+        uint32_t s = LC_FILTER_SLS_ABSENT;
+        for (uint32_t k = 0; k < (v ? n_fail : n_ok); ++k) {
+            const uint32_t kid = e[2 * k];
+            if (klen[kid] == len && (!len || !memcmp(kstr[kid], key, len))) {
+                s = e[2 * k + 1];
+                break;
+            }
+        }
+        src[v] = s;
+    }
+}
+
+// Host side: resolve the leaves against the chain's plans (lc_regex_sls_key_src) and check the program.  Returns nullptr, or why the filter is refused: more
 // than LC_FILTER_SLS_LEAVES leaves or LC_FILTER_SLS_PROG entries, an entry that is neither a leaf nor an opcode, a pop
 // of an empty stack, a stack deeper than 32, or a program that does not leave exactly one value.
 inline const char* lc_filter_sls_setup(const uint32_t* plan, uint32_t n_ok, uint32_t n_fail, const char* const* kstr,
@@ -2273,19 +2321,9 @@ inline const char* lc_filter_sls_setup(const uint32_t* plan, uint32_t n_ok, uint
     for (uint32_t l = 0; l < nleaves; ++l) {
         if (leaf_lens[l] && !leaf_keys[l])
             return "bad arguments";
-        for (uint32_t v = 0; v < 2; ++v) {
-            const uint32_t* e = plan + (v ? 2u * n_ok : 0u);
-            uint32_t s = LC_FILTER_SLS_ABSENT;
-            for (uint32_t k = 0; k < (v ? n_fail : n_ok); ++k) {
-                const uint32_t kid = e[2 * k];
-                if (klen[kid] == leaf_lens[l] && (!leaf_lens[l] || !memcmp(kstr[kid], leaf_keys[l], leaf_lens[l]))) {
-                    s = e[2 * k + 1]; // a plan's keys are unique
-                    break;
-                }
-            }
-            f->src[l][v] = s;
-            f->any_digits |= s == LC_REGEX_SLS_DIGITS;
-        }
+        lc_regex_sls_key_src(plan, n_ok, n_fail, kstr, klen, leaf_keys[l], leaf_lens[l], f->src[l]);
+        for (uint32_t v = 0; v < 2; ++v)
+            f->any_digits |= f->src[l][v] == LC_REGEX_SLS_DIGITS;
     }
     return nullptr;
 }
@@ -4084,4 +4122,98 @@ inline void lc_ts_probe_zone(LcTsConf& c) {
             (d ? c.dst_off : c.std_off)[k] = (int32_t)off;
         }
     }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, split -> regex -> timestamp chain: ProcessorParseTimestampNative (ProcessorParseTimestampNative.cpp:100-179, the
+// SourceKey tkey) behind the split -> regex chain, whose pieces and regex stage are unchanged.
+//   - The timestamp stage sees the pieces the regex stage kept, in piece order, as one group: a piece the regex stage
+//     erased is not an event of the stage (no counter, no cache step).
+//   - Its value is what the regex stage left under tkey: resolved once, on the host, through the chain's two content
+//     plans (lc_regex_sls_key_src) to capture j, the piece, or absent (LC_TS_NOT_FOUND).  tkey holding the offset
+//     digits is refused.  Both a piece the regex erased and an absent key give the tap's value LC_TS_NO_KEY, which the
+//     cache pass skips; the counters come from the size pass, which tells the two apart.
+//   - The value is read over [off, off + len) followed by NUL bytes, as every timestamp value is.
+//   - LC_TS_OK: Time = the parsed seconds truncated to 32 bits (raised to 2^28 by the body, LogGroupSerializer.cpp:
+//     111-119) and, with enable_ns, Time_ns = the parsed nanoseconds (SetTimestamp(t, ns) engages the optional).
+//     LC_TS_NOT_FOUND / LC_TS_FAILED: the source event's time and ns.  LC_TS_DISCARDED: no record.
+struct LcSplitRegexTsCfg {
+    uint32_t src[2];    // value source of tkey in a parsed [0] / failed [1] event: capture j, LC_REGEX_SLS_LINE, or
+                        // LC_FILTER_SLS_ABSENT
+    uint32_t enable_ns; // mEnableTimestampNanosecond: a parsed time writes Time_ns
+};
+
+// counters[8] of the chain: the regex stage's three, then the timestamp stage's five in lc_timestamp_parse's order
+#define LC_SRTS_COUNTERS 8
+
+// Host side: whether the source event's Time_ns agrees with enable_ns.  time_ns is the source event's Time_ns as the
+// serialiser writes it, so a source Time_ns without enable_ns would give Time_ns to the records that keep the source
+// time and not to the parsed ones, a mix no configuration of the reference produces.  Returns nullptr, or why not.
+inline const char* lc_split_regex_ts_ns_check(const LcSplitRegexSlsCfg& c, int enable_ns) {
+    return c.has_ns && !enable_ns ? "a source time_ns needs enable_ns" : nullptr;
+}
+
+// Host side: resolve tkey (lc_regex_sls_key_src over the plans of lc_split_regex_sls_setup, which accepted c; kstr /
+// klen: lc_split_regex_sls_strings' key table) and check the source Time_ns against enable_ns.  Returns nullptr, or
+// why the chain is refused.
+inline const char* lc_split_regex_ts_setup(const LcSplitRegexSlsCfg& c, const uint32_t* plan, const char* const* kstr,
+                                           const uint32_t* klen, const char* tkey, uint32_t tkey_len, int enable_ns,
+                                           LcSplitRegexTsCfg* t) {
+    if (!t || !plan || (tkey_len && !tkey))
+        return "bad arguments";
+    const char* why = lc_split_regex_ts_ns_check(c, enable_ns);
+    if (why)
+        return why;
+    lc_regex_sls_key_src(plan, c.x.n_ok, c.x.n_fail, kstr, klen, tkey, tkey_len, t->src);
+    if (t->src[0] == LC_REGEX_SLS_DIGITS || t->src[1] == LC_REGEX_SLS_DIGITS)
+        return "the timestamp key holds the offset digits (it equals the offset key)";
+    t->enable_ns = enable_ns != 0;
+    return nullptr;
+}
+
+// The tap: row r's value for the timestamp stage, *len = LC_TS_NO_KEY when the regex stage erased the piece or left
+// no tkey.
+LC_HD void lc_split_regex_ts_value(const LcSplitRegexSlsCfg& c, const LcSplitRegexTsCfg& t,
+                                   const LcSplitRegexSlsRow& r, uint32_t* off, uint32_t* len) {
+    const uint32_t v = lc_regex_sls_verdict(c.x, r.status);
+    const uint32_t s = t.src[v == 0u ? 0 : 1];
+    *off = 0;
+    *len = LC_TS_NO_KEY;
+    if ((v != 0u && !c.x.keep_fail) || s == LC_FILTER_SLS_ABSENT)
+        return;
+    if (s == LC_REGEX_SLS_LINE)
+        *off = r.po, *len = r.plen;
+    else
+        *off = r.co[s], *len = r.cl[s];
+}
+
+// The record's time after the timestamp stage (ts: the stage's LC_TS_ST_* of the row, sec / nsec its time).
+struct LcSplitRegexTsTime {
+    uint32_t keep; // 0: LC_TS_DISCARDED, no record
+    uint32_t time, has_ns, ns;
+};
+LC_HD LcSplitRegexTsTime lc_split_regex_ts_time(const LcSplitRegexSlsCfg& c, const LcSplitRegexTsCfg& t, uint32_t ts,
+                                                int64_t sec, uint32_t nsec) {
+    if (ts == LC_TS_ST_OK)
+        return {1u, (uint32_t)sec, t.enable_ns, nsec};
+    return {ts != LC_TS_ST_DISCARDED, c.time, c.has_ns, c.ns};
+}
+
+// The row's counter verdicts as bits of the LC_SRTS_COUNTERS counters: the regex stage's (lc_split_regex_verdict),
+// then -- when the regex stage kept the piece -- the timestamp stage's key_not_found, out_failed, history_failure,
+// discarded, out_successful.
+LC_HD uint32_t lc_split_regex_ts_verdict(const LcSplitRegexSlsCfg& c, uint32_t status, uint32_t ts) {
+    const LcSplitRegexVerdict v = lc_split_regex_verdict(c, status);
+    uint32_t bits = v.ok | (v.failed << 1) | (v.erased << 2);
+    if (v.erased)
+        return bits;
+    if (ts == LC_TS_ST_NOT_FOUND)
+        bits |= 1u << (3 + LC_TS_C_KEY_NOT_FOUND);
+    else if (ts == LC_TS_ST_FAILED)
+        bits |= 1u << (3 + LC_TS_C_OUT_FAILED);
+    else if (ts == LC_TS_ST_DISCARDED)
+        bits |= (1u << (3 + LC_TS_C_HISTORY_FAILURE)) | (1u << (3 + LC_TS_C_DISCARDED));
+    else
+        bits |= 1u << (3 + LC_TS_C_OUT_SUCCESSFUL);
+    return bits;
 }

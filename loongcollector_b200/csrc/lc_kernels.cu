@@ -3761,6 +3761,94 @@ void launch_split_regex_sls_emit(const LcSplitRegexSlsCfg& c, const RegexSlsTabl
                                                                                        d_out);
 }
 
+// ---- f4, split -> regex -> timestamp chain (lc_exec.cuh: lc_split_regex_ts_value, _time, _verdict).  The tap, one
+// thread per piece, writes the dense value table the timestamp passes take; the size pass (one thread per piece) and
+// the emit pass (one warp per piece) run lc_split_regex_sls_body with each record's own time.
+__global__ void __launch_bounds__(256)
+    split_regex_ts_tap_kernel(LcSplitRegexSlsCfg c, LcSplitRegexTsCfg tc, RegexSlsTables t, uint64_t n,
+                              uint32_t* __restrict__ off, uint32_t* __restrict__ len) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n)
+        return;
+    uint32_t o, l;
+    lc_split_regex_ts_value(c, tc, split_regex_sls_row(c, t, i), &o, &l);
+    off[i] = o;
+    len[i] = l;
+}
+
+// counters: u64 [9] += the LC_SRTS_COUNTERS verdicts (one atomic per warp and counter), then pieces whose record
+// would reach 4 GiB
+__global__ void __launch_bounds__(256)
+    split_regex_ts_sls_size_kernel(LcSplitRegexSlsCfg c, LcSplitRegexTsCfg tc, RegexSlsTables t, TsRowTables ts,
+                                   uint64_t n, uint32_t* __restrict__ rec_size, uint32_t* __restrict__ body_size,
+                                   unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t bits = 0, big = 0;
+    if (i < n) {
+        const LcSplitRegexSlsRow r = split_regex_sls_row(c, t, i);
+        const uint32_t st = ts.status[i];
+        const LcSplitRegexTsTime tm = lc_split_regex_ts_time(c, tc, st, ts.sec[i], ts.nsec[i]);
+        LcSlsCount64 s{0};
+        const uint32_t cnt = tm.keep ? lc_split_regex_sls_body(c, t.base, r, tm.time, tm.has_ns, tm.ns, s) : 0u;
+        big = s.n + 16 > 0xFFFFFFFFull;
+        const uint32_t body = cnt && !big ? (uint32_t)s.n : 0u;
+        rec_size[i] = body ? 1 + lc_varint_size(body) + body : 0u;
+        body_size[i] = body;
+        bits = lc_split_regex_ts_verdict(c, r.status, st);
+    }
+#pragma unroll
+    for (uint32_t k = 0; k < LC_SRTS_COUNTERS; ++k) {
+        const uint32_t v = __reduce_add_sync(0xFFFFFFFFu, (bits >> k) & 1u);
+        if ((threadIdx.x & 31) == 0 && v)
+            atomicAdd(counters + k, (unsigned long long)v);
+    }
+    big = __reduce_add_sync(0xFFFFFFFFu, big);
+    if ((threadIdx.x & 31) == 0 && big)
+        atomicAdd(counters + LC_SRTS_COUNTERS, (unsigned long long)big);
+}
+
+__global__ void __launch_bounds__(256)
+    split_regex_ts_sls_emit_kernel(LcSplitRegexSlsCfg c, LcSplitRegexTsCfg tc, RegexSlsTables t, TsRowTables ts,
+                                   uint64_t n, const uint64_t* __restrict__ rec_off,
+                                   const uint32_t* __restrict__ body_size, uint8_t* __restrict__ out) {
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n)
+        return;
+    const uint32_t body = body_size[i];
+    if (!body)
+        return; // erased, discarded or LogEvent::Empty: no record
+    const LcSplitRegexSlsRow r = split_regex_sls_row(c, t, i);
+    const LcSplitRegexTsTime tm = lc_split_regex_ts_time(c, tc, ts.status[i], ts.sec[i], ts.nsec[i]);
+    uint8_t h[6];
+    h[0] = 0x0A;
+    const uint32_t hn = 1 + lc_put_varint(h + 1, body);
+    LcSlsWrite s{out + rec_off[i], 0u, hn + body, threadIdx.x & 31, 32};
+    s.put(h, hn);
+    lc_split_regex_sls_body(c, t.base, r, tm.time, tm.has_ns, tm.ns, s);
+}
+
+void launch_split_regex_ts_tap(const LcSplitRegexSlsCfg& c, const LcSplitRegexTsCfg& tc, const RegexSlsTables& t,
+                               uint64_t n, uint32_t* d_off, uint32_t* d_len, cudaStream_t st) {
+    if (n)
+        split_regex_ts_tap_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, tc, t, n, d_off, d_len);
+}
+
+void launch_split_regex_ts_sls_sizes(const LcSplitRegexSlsCfg& c, const LcSplitRegexTsCfg& tc, const RegexSlsTables& t,
+                                     const TsRowTables& ts, uint64_t n, uint32_t* d_rec_size, uint32_t* d_body_size,
+                                     unsigned long long* d_counters, cudaStream_t st) {
+    if (n)
+        split_regex_ts_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, tc, t, ts, n, d_rec_size,
+                                                                                     d_body_size, d_counters);
+}
+
+void launch_split_regex_ts_sls_emit(const LcSplitRegexSlsCfg& c, const LcSplitRegexTsCfg& tc, const RegexSlsTables& t,
+                                    const TsRowTables& ts, uint64_t n, const uint64_t* d_rec_off,
+                                    const uint32_t* d_body_size, uint8_t* d_out, cudaStream_t st) {
+    if (n)
+        split_regex_ts_sls_emit_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, tc, t, ts, n, d_rec_off,
+                                                                                          d_body_size, d_out);
+}
+
 // ---- f4, delimiter-fed: Log records of the events a ProcessorParseDelimiterNative leaves behind, straight from the
 // delimiter stage's tables.  Both passes run the same per-row function (lc_exec.cuh: lc_delim_sls_body) -- the size
 // pass with a counting sink, one thread per event; the emit pass with a writing sink, one warp per event.

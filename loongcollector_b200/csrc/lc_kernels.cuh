@@ -12,6 +12,7 @@ struct LcSplitRegexSlsCfg;
 struct LcSplitDelimSlsCfg;
 struct LcSplitDelimRegexSlsCfg;
 struct LcFilterSlsCfg;
+struct LcSplitRegexTsCfg;
 struct LcLz4Seq;
 struct LcTsConf;
 struct LcTsNow;
@@ -248,6 +249,24 @@ void launch_filter_eval(const LcSplitRegexSlsCfg& c, const LcFilterSlsCfg& f, co
 void launch_split_regex_sls_emit(const LcSplitRegexSlsCfg& c, const RegexSlsTables& t, uint64_t n,
                                  const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
                                  cudaStream_t st);
+// f4, split -> regex -> timestamp chain (lc_exec.cuh: LcSplitRegexTsCfg).  launch_split_regex_ts_tap: the dense value
+// table (d_off, d_len) over t.base that the timestamp passes take (LC_TS_NO_KEY: erased by the regex stage, or no
+// tkey).  The size and emit passes are launch_split_regex_sls_*'s with each record's time from the timestamp tables ts
+// (a discarded piece has no record); d_counters: u64 [9] += the chain's 8 counters (LC_SRTS_COUNTERS), then pieces
+// whose record would reach 4 GiB.
+struct TsRowTables {
+    const uint8_t* status; // LC_TS_* per piece
+    const int64_t* sec;
+    const uint32_t* nsec;
+};
+void launch_split_regex_ts_tap(const LcSplitRegexSlsCfg& c, const LcSplitRegexTsCfg& tc, const RegexSlsTables& t,
+                               uint64_t n, uint32_t* d_off, uint32_t* d_len, cudaStream_t st);
+void launch_split_regex_ts_sls_sizes(const LcSplitRegexSlsCfg& c, const LcSplitRegexTsCfg& tc, const RegexSlsTables& t,
+                                     const TsRowTables& ts, uint64_t n, uint32_t* d_rec_size, uint32_t* d_body_size,
+                                     unsigned long long* d_counters, cudaStream_t st);
+void launch_split_regex_ts_sls_emit(const LcSplitRegexSlsCfg& c, const LcSplitRegexTsCfg& tc, const RegexSlsTables& t,
+                                    const TsRowTables& ts, uint64_t n, const uint64_t* d_rec_off,
+                                    const uint32_t* d_body_size, uint8_t* d_out, cudaStream_t st);
 
 // f4, delimiter-fed: Log records from the delimiter stage's result tables (launch_delim) + the configuration of
 // lc_exec.cuh (LcDelimSlsCfg, key strings on the device).  Sizes as for launch_sls_sizes; d_counters (or nullptr):

@@ -115,6 +115,7 @@ private:
 class ProcessorParseRegexNative;
 class ProcessorParseDelimiterNative;
 class ProcessorFilterNative;
+class ProcessorParseTimestampNative;
 
 class ProcessorSplitLogStringNative : public Processor {
 public:
@@ -177,6 +178,17 @@ public:
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
                          ProcessorParseRegexNative& regex, bool enableNs, std::string& block, uint64_t& rawSize,
                          std::string& err);
+    // The split -> regex -> timestamp chain: Process(group), next.Process(group), timestamp.Process(group)
+    // (timestamp: the processor_parse_timestamp_native behind next), then SLSEventGroupSerializer::Serialize: the
+    // same bytes or error message, and the same counter updates on all three processors.  The device path
+    // (lc_split_regex_timestamp_parse_sls[_lz4]) applies under SerializeSls(group, next)'s conditions when the group
+    // holds exactly one source event (the reader's shape: the second-level cache then never has to carry across
+    // calls) and the chain accepts timestamp's SourceKey; "now" is read once per call.  Otherwise the four calls run.
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                      ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& out, std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                         ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& block,
+                         uint64_t& rawSize, std::string& err);
 
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
@@ -189,6 +201,9 @@ private:
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
                            ProcessorParseRegexNative& regex, bool enableNs, std::string& out, uint64_t* rawSize,
                            std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                           ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& out,
+                           uint64_t* rawSize, std::string& err);
 };
 
 class ProcessorSplitMultilineLogStringNative : public Processor {
@@ -230,6 +245,13 @@ public:
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
                          ProcessorParseRegexNative& regex, bool enableNs, std::string& block, uint64_t& rawSize,
                          std::string& err);
+    // The split -> regex -> timestamp chain, as ProcessorSplitLogStringNative's
+    // (lc_multiline_split_regex_timestamp_parse_sls[_lz4]).
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                      ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& out, std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                         ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& block,
+                         uint64_t& rawSize, std::string& err);
     Counter mMatchedEventsTotal, mMatchedLinesTotal, mUnmatchedLinesTotal;
 
 protected:
@@ -243,6 +265,9 @@ private:
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
                            ProcessorParseRegexNative& regex, bool enableNs, std::string& out, uint64_t* rawSize,
                            std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next,
+                           ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& out,
+                           uint64_t* rawSize, std::string& err);
     CompiledRegex mStart, mContinue, mEnd;
 };
 
@@ -396,6 +421,7 @@ protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
+    friend struct SplitRegexTsStage; // the split -> regex -> timestamp chain's SerializeSls
     lc_timestamp_t* mProgram = nullptr;
 };
 
