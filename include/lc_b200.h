@@ -965,6 +965,64 @@ int lc_timestamp_parse_capture_dev(lc_engine_t* e, const lc_timestamp_t* ts, con
                                    uint64_t ngroups, int64_t now, int32_t discard_interval, int64_t* d_sec,
                                    uint32_t* d_nsec, uint8_t* d_status, uint64_t* d_counters);
 
+/* ---- ProcessorParseApsaraNative (ProcessorParseApsaraNative.cpp: ProcessEvent 116-241, ApsaraEasyReadLogTimeParser
+ *      251-323, FindBaseFields 342-361, ParseApsaraBaseFields 433-463)
+ * lc_apsara_compile is Init: source_key is SourceKey; tz_adjust is mLogTimeZoneOffsetSecond (Timezone's offset minus
+ * the local one, ParseLogTimeZoneOffsetSecond; 0 without a valid Timezone), subtracted from every parsed
+ * "%Y-%m-%d %H:%M:%S" time and never from an epoch ("[1...]") time.  The process's local zone is probed here as
+ * lc_timestamp_compile probes it; compile again after the zone changes.
+ *
+ * lc_apsara_parse[_dev]: event i's value is base[ev_off[i], + ev_len[i]); ev_len[i] == LC_TS_NO_KEY means the event
+ * has no SourceKey.  Events [grp[g], grp[g + 1]) form group g (grp[0] = 0, grp[ngroups] = n, not decreasing); the time
+ * cache starts empty in every group and follows event order.  now is time(NULL) of the call; discard_interval >= 0
+ * discards an event whose time is more than that many seconds behind now, -1 = no such rule.
+ * Per event:
+ *   - status[i]: LC_APSARA_* in the low 3 bits; LC_APSARA_OVERWRITTEN is set on LC_APSARA_OK when a key:value key
+ *     equals SourceKey (the event keeps its SourceKey content).
+ *   - sec[i], nsec[i]: SetTimestamp's seconds and nanoseconds (micro * 1000 % 10^9) for LC_APSARA_OK, and the ones
+ *     the event would have got for LC_APSARA_DISCARDED; micro[i] is logTime_in_micro (the "microtime" content is its
+ *     "%ld" digits).  All three are 0 for the other statuses.
+ *   - first[i] .. first[i + 1]: its entries (first has n + 1 entries; only LC_APSARA_OK events have any), in append
+ *     order: the base fields (key_off one of LC_APSARA_KEY_*, key_len 0), then the key:value fields (key and value
+ *     as offsets into base).  The "microtime" content follows them and is not an entry.
+ * counters[5] = key_not_found, out_failed, history_failure, discarded, out_successful.  out_failed counts empty values
+ * and failed time parses; discarded counts only the history discards: whether a failed event is erased depends on
+ * its other contents (CommonParserOptions::ShouldEraseEvent), which the caller adds.
+ * *n_entries is the number of entries; when it exceeds entry_cap the call returns LC_ERR_CAPACITY and writes no entry
+ * (the other outputs are written), so entry_cap 0 makes a sizing query.  An event past base_len is refused with
+ * LC_ERR_INVALID_ARG (the _dev call finds it on the device, without reading it).  The time string is read as a C
+ * string and the 19-byte cache key past the end of base reads as NUL bytes (see lc_exec.cuh).
+ * The _dev call takes device tables (d_grp as above, not checked).  Unlike the other _dev calls it waits for the
+ * device before it returns: it reads the entry total on the host, and every output, the entries included, is written
+ * when it returns, so it can be read from any stream.  The host call sizes its device copy of the entries from the
+ * total, not from entry_cap. */
+#define LC_APSARA_OK 0
+#define LC_APSARA_NOT_FOUND 1 /* no SourceKey: out_key_not_found++, event kept */
+#define LC_APSARA_EMPTY 2     /* empty value: out_failed++, event kept untouched */
+#define LC_APSARA_FAILED 3    /* time parse failed or gave <= 0: out_failed++, the failure path */
+#define LC_APSARA_DISCARDED 4 /* too old: history_failure++, discarded++, event erased */
+#define LC_APSARA_OVERWRITTEN 0x80
+#define LC_APSARA_KEY_LEVEL 0xFFFFFFF0u  /* __LEVEL__ */
+#define LC_APSARA_KEY_THREAD 0xFFFFFFF1u /* __THREAD__ */
+#define LC_APSARA_KEY_FILE 0xFFFFFFF2u   /* __FILE__ */
+#define LC_APSARA_KEY_LINE 0xFFFFFFF3u   /* __LINE__ */
+typedef struct lc_apsara lc_apsara_t;
+typedef struct {
+    uint32_t key_off, key_len, val_off, val_len;
+} lc_apsara_entry_t;
+int lc_apsara_compile(const char* source_key, size_t key_len, int32_t tz_adjust, lc_apsara_t** out);
+void lc_apsara_free(lc_apsara_t* a);
+int lc_apsara_parse(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* base, uint64_t base_len,
+                    const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* grp, uint64_t ngroups,
+                    int64_t now, int32_t discard_interval, uint8_t* status, int64_t* sec, uint32_t* nsec,
+                    int64_t* micro, uint64_t* first, lc_apsara_entry_t* entries, uint64_t entry_cap,
+                    uint64_t* n_entries, uint64_t* counters);
+int lc_apsara_parse_dev(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* d_base, uint64_t base_len,
+                        const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, const uint32_t* d_grp,
+                        uint64_t ngroups, int64_t now, int32_t discard_interval, uint8_t* d_status, int64_t* d_sec,
+                        uint32_t* d_nsec, int64_t* d_micro, uint64_t* d_first, lc_apsara_entry_t* d_entries,
+                        uint64_t entry_cap, uint64_t* n_entries, uint64_t* d_counters);
+
 #ifdef __cplusplus
 }
 #endif

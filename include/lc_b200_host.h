@@ -29,6 +29,10 @@ char* lc_host_processor_process_groups(lc_host_processor_t* p, const char* group
                                        char** err_out);
 /* {"counter": value, ...} with the reference's counter meanings. */
 char* lc_host_processor_counters(const lc_host_processor_t* p);
+/* The process-wide flags ilogtail_discard_old_data / ilogtail_discard_interval as the time-parsing processors
+ * (processor_parse_timestamp_native, processor_parse_apsara_native) read them: on with 43200 s by default, off for
+ * one-time pipelines.  Returns 0, or -1 for another processor. */
+int lc_host_processor_set_discard_old_data(lc_host_processor_t* p, int enabled, int32_t interval);
 void lc_host_string_free(char* s);
 
 /* SLSEventGroupSerializer::Serialize (core/collection_pipeline/serializer/SLSSerializer.cpp:162-252) of the LOG or RAW

@@ -105,6 +105,11 @@ def lib():
     L.lc_timestamp_parse.argtypes = [vp, vp, vp, u64, vp, vp, u64] + ts_tail
     L.lc_timestamp_parse_dev.argtypes = [vp, vp, vp, u64, vp, vp, u64] + ts_tail
     L.lc_timestamp_parse_capture_dev.argtypes = [vp, vp, vp, u64, vp, vp, vp, u32, u32, u64] + ts_tail
+    L.lc_apsara_compile.argtypes = [C.c_char_p, C.c_size_t, i32, C.POINTER(vp)]
+    L.lc_apsara_free.argtypes = [vp]
+    ap_args = [vp, vp, vp, u64, vp, vp, u64, vp, u64, C.c_int64, i32, vp, vp, vp, vp, vp, vp, u64, C.POINTER(u64), vp]
+    L.lc_apsara_parse.argtypes = ap_args
+    L.lc_apsara_parse_dev.argtypes = ap_args
     L.lc_delim_parse_sls_lz4.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32, u8, i32, i32, i32, u32] + \
         sls_cfg + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
     L.lc_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp] + sls_cfg + \
@@ -267,6 +272,36 @@ class Timestamp:
                 lib().lc_timestamp_free(self._h)
         except Exception:
             pass
+
+
+class Apsara:
+    """ProcessorParseApsaraNative's Init (lc_apsara_compile): SourceKey and the timezone adjustment
+    (mLogTimeZoneOffsetSecond) are fixed here, and so is the process's local zone."""
+
+    def __init__(self, source_key, tz_adjust=0):
+        if isinstance(source_key, str):
+            source_key = source_key.encode("utf-8")
+        h = C.c_void_p()
+        L = lib()
+        rc = L.lc_apsara_compile(source_key, len(source_key), int(tz_adjust), C.byref(h))
+        self._h = h
+        if rc != LC_OK:
+            self._h = None
+            raise LcError(rc, L.lc_last_error().decode())
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib().lc_apsara_free(self._h)
+        except Exception:
+            pass
+
+
+# lc_apsara_parse's status values and base-field keys
+LC_APSARA_OK, LC_APSARA_NOT_FOUND, LC_APSARA_EMPTY, LC_APSARA_FAILED, LC_APSARA_DISCARDED = 0, 1, 2, 3, 4
+LC_APSARA_OVERWRITTEN = 0x80
+LC_APSARA_KEY_LEVEL = 0xFFFFFFF0
+APSARA_BASE_KEYS = (b"__LEVEL__", b"__THREAD__", b"__FILE__", b"__LINE__")
 
 
 def _rh(r):
@@ -1311,6 +1346,44 @@ class Engine:
                                         _p(st), _p(cnt)))
         return st, sec, ns, cnt
 
+    def apsara_parse(self, ap, base, ev_off, ev_len, grp, now, discard_interval=43200, entry_cap=None):
+        """ProcessorParseApsaraNative over host buffers (lc_apsara_parse): ev_len LC_TS_NO_KEY = no SourceKey, grp =
+        group starts plus n.  entry_cap None sizes the entries with a first call.  Returns (status u8, sec i64,
+        nsec u32, micro i64, first u64[n + 1], entries u32[m, 4], counters u64[5])."""
+        a = _u8(base)
+        ev_off = np.ascontiguousarray(ev_off, np.uint32)
+        ev_len = np.ascontiguousarray(ev_len, np.uint32)
+        grp = np.ascontiguousarray(grp, np.uint32)
+        n = ev_off.size
+        st, sec, ns = np.empty(n, np.uint8), np.empty(n, np.int64), np.empty(n, np.uint32)
+        us, first = np.empty(n, np.int64), np.empty(n + 1, np.uint64)
+        cnt = np.zeros(5, np.uint64)
+        m = C.c_uint64(0)
+
+        def call(cap, ent):
+            return lib().lc_apsara_parse(self._h, ap._h, _p(a), a.size, _p(ev_off), _p(ev_len), n, _p(grp),
+                                         max(grp.size - 1, 0), int(now), int(discard_interval), _p(st), _p(sec),
+                                         _p(ns), _p(us), _p(first), _p(ent), cap, C.byref(m), _p(cnt))
+        if entry_cap is None:
+            rc = call(0, np.zeros((1, 4), np.uint32))
+            if rc not in (LC_OK, LC_ERR_CAPACITY):
+                _check(rc)
+            entry_cap = m.value
+        ent = np.zeros((max(int(entry_cap), 1), 4), np.uint32)
+        _check(call(int(entry_cap), ent))
+        return st, sec, ns, us, first, ent[:m.value], cnt
+
+    def apsara_parse_dev(self, ap, d_base, base_len, d_ev_off, d_ev_len, n, d_grp, ngroups, now, discard_interval,
+                         d_status, d_sec, d_nsec, d_micro, d_first, d_entries, entry_cap, d_counters):
+        """lc_apsara_parse_dev over device tables; waits for the device.  Returns the entry count (raises LcError
+        with LC_ERR_CAPACITY when it exceeds entry_cap; no entry is written then)."""
+        m = C.c_uint64(0)
+        _check(lib().lc_apsara_parse_dev(self._h, ap._h, _p(d_base), base_len, _p(d_ev_off), _p(d_ev_len), n,
+                                         _p(d_grp), ngroups, int(now), int(discard_interval), _p(d_status), _p(d_sec),
+                                         _p(d_nsec), _p(d_micro), _p(d_first), _p(d_entries), entry_cap, C.byref(m),
+                                         _p(d_counters)))
+        return m.value
+
     def timestamp_parse_dev(self, ts, d_base, base_len, d_ev_off, d_ev_len, n, d_grp, ngroups, now, discard_interval,
                             d_sec, d_nsec, d_status, d_counters):
         _check(lib().lc_timestamp_parse_dev(self._h, ts._h, _p(d_base), base_len, _p(d_ev_off), _p(d_ev_len), n,
@@ -1421,6 +1494,13 @@ class HostProcessor:
         s = C.string_at(out).decode("utf-8")
         L.lc_host_string_free(out)
         return json.loads(s)
+
+    def set_discard_old_data(self, enabled, interval=43200):
+        """ilogtail_discard_old_data / ilogtail_discard_interval of a time-parsing processor"""
+        L = lib()
+        L.lc_host_processor_set_discard_old_data.argtypes = [C.c_void_p, C.c_int, C.c_int32]
+        if L.lc_host_processor_set_discard_old_data(self._h, int(bool(enabled)), int(interval)) != 0:
+            raise ValueError("not a time-parsing processor")
 
     def counters(self):
         import json

@@ -122,6 +122,11 @@ struct lc_engine {
     // split -> regex -> timestamp chain: the tap's value table and group starts, the timestamp tables over the pieces;
     // the chain's piece and regex tables are the split -> regex chain's (in, out_a, out_b, dr_*)
     DevBuf st_val, st_sec, st_nsec, st_status;
+    // Apsara parse: the handle ap_conf_id's zone table and SourceKey, the scan results, the entry counts, the
+    // counters and the out-of-range flag; the host call's copies of its outputs
+    DevBuf ap_conf, ap_ev, ap_nent, ap_small;
+    uint64_t ap_conf_id = 0;
+    DevBuf ap_status, ap_sec, ap_nsec, ap_micro, ap_first, ap_ent;
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
     std::unordered_map<uint64_t, void*> blobs; // regex id * 4 + layout -> device blob
@@ -339,7 +344,9 @@ void lc_engine_destroy(lc_engine_t* e) {
                       &e->dr_keys, &e->dr_val_off, &e->dr_val_len, &e->dr_status, &e->dr_cap_off, &e->dr_cap_len,
                       &e->dr_copy, &e->dr_slot, &e->dr_desc, &e->fl_tab, &e->fl_match, &e->fl_dig, &e->fl_keep,
                       &e->sdr_status, &e->sdr_nf, &e->sdr_f_off, &e->sdr_f_len, &e->sdr_f_dq, &e->sdr_okey,
-                      &e->ts_conf, &e->ts_full, &e->ts_cnt, &e->st_val, &e->st_sec, &e->st_nsec, &e->st_status};
+                      &e->ts_conf, &e->ts_full, &e->ts_cnt, &e->st_val, &e->st_sec, &e->st_nsec, &e->st_status,
+                      &e->ap_conf, &e->ap_ev, &e->ap_nent, &e->ap_small, &e->ap_status, &e->ap_sec, &e->ap_nsec,
+                      &e->ap_micro, &e->ap_first, &e->ap_ent};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -4329,4 +4336,199 @@ int lc_timestamp_parse(lc_engine_t* e, const lc_timestamp_t* ts, const uint8_t* 
     CU_TRY(cudaMemcpyAsync(counters, e->ts_cnt.p, 5 * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(cudaStreamSynchronize(e->stream));
     return LC_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ Apsara parse
+struct lc_apsara {
+    uint64_t id;
+    LcTsConf conf; // adjust and the zone table; the format program is not used
+    std::string skey;
+};
+
+int lc_apsara_compile(const char* source_key, size_t key_len, int32_t tz_adjust, lc_apsara_t** out) {
+    if (!out || (!source_key && key_len) || key_len >= 0xFFFFFFFFull)
+        return fail(LC_ERR_INVALID_ARG, "lc_apsara_compile: bad arguments");
+    *out = nullptr;
+    lc_apsara* a = new (std::nothrow) lc_apsara;
+    if (!a)
+        return fail(LC_ERR_INVALID_ARG, "out of host memory");
+    memset(&a->conf, 0, sizeof a->conf);
+    a->conf.adjust = tz_adjust;
+    lc_ts_probe_zone(a->conf);
+    a->skey.assign(source_key ? source_key : "", key_len);
+    a->id = g_regex_ids.fetch_add(1);
+    *out = a;
+    return LC_OK;
+}
+
+void lc_apsara_free(lc_apsara_t* a) { delete a; }
+
+static_assert(sizeof(lc_apsara_entry_t) == sizeof(LcApEntry), "entry layout");
+
+namespace {
+
+// The scan, resolve and count passes (on the caller's device tables) up to the entry total, which *n_entries receives
+// after a wait for the device.  An event past base_len gives LC_ERR_INVALID_ARG.
+int ap_count(lc_engine_t* e, const lc_apsara_t* ap, const char* what, const uint8_t* d_base, uint64_t base_len,
+             const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, const uint32_t* d_grp, uint64_t ngroups,
+             int64_t now, int32_t discard_interval, uint8_t* d_status, int64_t* d_sec, uint32_t* d_nsec,
+             int64_t* d_micro, uint64_t* d_first, uint64_t* n_entries, uint64_t* d_counters) {
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    *n_entries = 0;
+    CU_TRY(cudaMemsetAsync(d_counters, 0, 5 * sizeof(uint64_t), e->stream));
+    if (n == 0) {
+        CU_TRY(cudaMemsetAsync(d_first, 0, 8, e->stream));
+        CU_TRY(cudaStreamSynchronize(e->stream));
+        return LC_OK;
+    }
+    LcTsNow t;
+    memset(&t, 0, sizeof t);
+    t.now = now;
+    t.discard_interval = discard_interval;
+    if (e->ap_conf_id != ap->id) {
+        CU_TRY(e->ap_conf.ensure(sizeof(LcTsConf) + ap->skey.size() + 1));
+        CU_TRY(cudaMemcpyAsync(e->ap_conf.p, &ap->conf, sizeof(LcTsConf), cudaMemcpyHostToDevice, e->stream));
+        if (!ap->skey.empty())
+            CU_TRY(cudaMemcpyAsync(e->ap_conf.as<uint8_t>() + sizeof(LcTsConf), ap->skey.data(), ap->skey.size(),
+                                   cudaMemcpyHostToDevice, e->stream));
+        e->ap_conf_id = ap->id;
+    }
+    CU_TRY(e->ap_ev.ensure(n * sizeof(LcApEv)));
+    CU_TRY(e->ap_nent.ensure(n * 4));
+    CU_TRY(e->ap_small.ensure(16));
+    CU_TRY(cudaMemsetAsync(e->ap_small.p, 0, 16, e->stream));
+    uint32_t* d_bad = e->ap_small.as<uint32_t>();
+    const LcTsConf* d_conf = e->ap_conf.as<LcTsConf>();
+    lck::launch_ap_scan(d_conf, d_base, base_len, d_ev_off, d_ev_len, n, e->ap_conf.as<uint8_t>() + sizeof(LcTsConf),
+                        (uint32_t)ap->skey.size(), e->ap_ev.as<LcApEv>(), d_bad, e->stream);
+    lck::launch_ap_resolve(t, e->ap_ev.as<LcApEv>(), d_grp, ngroups, d_status, d_sec, d_nsec, d_micro,
+                           e->ap_nent.as<uint32_t>(), reinterpret_cast<unsigned long long*>(d_counters), e->stream);
+    uint64_t* desc;
+    rc = prep_desc(e, lck::scan_tiles(n), &desc);
+    if (rc)
+        return rc;
+    lck::launch_exclusive_sum(e->ap_nent.as<uint32_t>(), n, d_first, d_first + n, desc, &e->small.as<Small>()->tickets[2],
+                              e->stream);
+    e->launches += 3;
+    CU_TRY(cudaGetLastError());
+    uint32_t bad = 0;
+    CU_TRY(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(n_entries, d_first + n, 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    if (bad) {
+        *n_entries = 0;
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": event outside the buffer");
+    }
+    return LC_OK;
+}
+
+// The emit pass of ap_count's events into d_entries (room for the total); queued, not waited for.
+int ap_emit(lc_engine_t* e, const uint8_t* d_base, const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n,
+            const uint8_t* d_status, const uint64_t* d_first, lc_apsara_entry_t* d_entries) {
+    lck::launch_ap_emit(d_base, d_ev_off, d_ev_len, d_status, n, d_first, reinterpret_cast<LcApEntry*>(d_entries),
+                        e->stream);
+    e->launches += 1;
+    CU_TRY(cudaGetLastError());
+    return LC_OK;
+}
+
+} // namespace
+
+int lc_apsara_parse_dev(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* d_base, uint64_t base_len,
+                        const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, const uint32_t* d_grp,
+                        uint64_t ngroups, int64_t now, int32_t discard_interval, uint8_t* d_status, int64_t* d_sec,
+                        uint32_t* d_nsec, int64_t* d_micro, uint64_t* d_first, lc_apsara_entry_t* d_entries,
+                        uint64_t entry_cap, uint64_t* n_entries, uint64_t* d_counters) {
+    static const char* what = "lc_apsara_parse_dev";
+    if (!e || !ap || !d_counters || !n_entries || !d_first || (entry_cap && !d_entries) ||
+        (n && (!d_base || !d_ev_off || !d_ev_len || !d_grp || !ngroups || !d_status || !d_sec || !d_nsec ||
+               !d_micro)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    if (base_len >= 0xFFFFFFF0ull || n >= 0xFFFFFFFFull || ngroups >= 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": buffer must be < 4 GiB and < 2^32 events per call");
+    int rc = ap_count(e, ap, what, d_base, base_len, d_ev_off, d_ev_len, n, d_grp, ngroups, now, discard_interval,
+                      d_status, d_sec, d_nsec, d_micro, d_first, n_entries, d_counters);
+    if (rc)
+        return rc;
+    if (*n_entries > entry_cap)
+        return fail(LC_ERR_CAPACITY, std::string(what) + ": entry capacity too small");
+    if (*n_entries) {
+        rc = ap_emit(e, d_base, d_ev_off, d_ev_len, n, d_status, d_first, d_entries);
+        if (rc)
+            return rc;
+        CU_TRY(cudaStreamSynchronize(e->stream));
+    }
+    return LC_OK;
+}
+
+int lc_apsara_parse(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* base, uint64_t base_len,
+                    const uint32_t* ev_off, const uint32_t* ev_len, uint64_t n, const uint32_t* grp, uint64_t ngroups,
+                    int64_t now, int32_t discard_interval, uint8_t* status, int64_t* sec, uint32_t* nsec,
+                    int64_t* micro, uint64_t* first, lc_apsara_entry_t* entries, uint64_t entry_cap,
+                    uint64_t* n_entries, uint64_t* counters) {
+    static const char* what = "lc_apsara_parse";
+    if (!e || !ap || !counters || !n_entries || !first || (entry_cap && !entries) ||
+        (n && (!base || !ev_off || !ev_len || !grp || !ngroups || !status || !sec || !nsec || !micro)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    if (base_len >= 0xFFFFFFF0ull || n >= 0xFFFFFFFFull || ngroups >= 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": buffer must be < 4 GiB and < 2^32 events per call");
+    memset(counters, 0, 5 * sizeof(uint64_t));
+    *n_entries = 0;
+    first[0] = 0;
+    if (n == 0)
+        return LC_OK;
+    if (grp[0] != 0 || grp[ngroups] != n)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": groups must cover the events");
+    for (uint64_t g = 0; g < ngroups; ++g)
+        if (grp[g + 1] < grp[g])
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": group starts must not decrease");
+    for (uint64_t i = 0; i < n; ++i)
+        if (ev_len[i] != LC_AP_NO_KEY && (uint64_t)ev_off[i] + ev_len[i] > base_len)
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": event outside the buffer");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    CU_TRY(e->in.ensure(base_len + 16));
+    CU_TRY(e->ev_off.ensure(n * 4));
+    CU_TRY(e->ev_len.ensure(n * 4));
+    CU_TRY(e->lines_off.ensure((ngroups + 1) * 4));
+    CU_TRY(e->ap_status.ensure(n));
+    CU_TRY(e->ap_sec.ensure(n * 8));
+    CU_TRY(e->ap_nsec.ensure(n * 4));
+    CU_TRY(e->ap_micro.ensure(n * 8));
+    CU_TRY(e->ap_first.ensure((n + 1) * 8));
+    CU_TRY(e->ts_cnt.ensure(5 * sizeof(uint64_t)));
+    if (base_len)
+        CU_TRY(cudaMemcpyAsync(e->in.p, base, base_len, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(e->ev_off.p, ev_off, n * 4, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(e->ev_len.p, ev_len, n * 4, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(e->lines_off.p, grp, (ngroups + 1) * 4, cudaMemcpyHostToDevice, e->stream));
+    rc = ap_count(e, ap, what, e->in.as<uint8_t>(), base_len, e->ev_off.as<uint32_t>(), e->ev_len.as<uint32_t>(), n,
+                  e->lines_off.as<uint32_t>(), ngroups, now, discard_interval, e->ap_status.as<uint8_t>(),
+                  e->ap_sec.as<int64_t>(), e->ap_nsec.as<uint32_t>(), e->ap_micro.as<int64_t>(),
+                  e->ap_first.as<uint64_t>(), n_entries, e->ts_cnt.as<uint64_t>());
+    if (rc)
+        return rc;
+    const uint64_t m = *n_entries;
+    if (m > entry_cap) {
+        rc = fail(LC_ERR_CAPACITY, std::string(what) + ": entry capacity too small");
+    } else if (m) {
+        // the device entries are sized from the count, not from entry_cap
+        CU_TRY(e->ap_ent.ensure(m * sizeof(LcApEntry)));
+        rc = ap_emit(e, e->in.as<uint8_t>(), e->ev_off.as<uint32_t>(), e->ev_len.as<uint32_t>(), n,
+                     e->ap_status.as<uint8_t>(), e->ap_first.as<uint64_t>(), e->ap_ent.as<lc_apsara_entry_t>());
+        if (rc)
+            return rc;
+        CU_TRY(cudaMemcpyAsync(entries, e->ap_ent.p, m * sizeof(LcApEntry), cudaMemcpyDeviceToHost, e->stream));
+    }
+    CU_TRY(cudaMemcpyAsync(status, e->ap_status.p, n, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(sec, e->ap_sec.p, n * 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(nsec, e->ap_nsec.p, n * 4, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(micro, e->ap_micro.p, n * 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(first, e->ap_first.p, (n + 1) * 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(counters, e->ts_cnt.p, 5 * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    return rc;
 }

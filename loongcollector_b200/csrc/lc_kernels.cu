@@ -4496,4 +4496,76 @@ void launch_ts_resolve(const LcTsConf* d_conf, const LcTsNow& now, const uint8_t
         d_conf, now, d_base, sp, d_full, d_grp, ngroups, d_sec, d_nsec, d_status, d_counters);
 }
 
+// ================================================================================================ Apsara parse
+__global__ void __launch_bounds__(256)
+    ap_scan_kernel(const LcTsConf* __restrict__ conf, const uint8_t* __restrict__ base, uint64_t base_len,
+                   const uint32_t* __restrict__ off, const uint32_t* __restrict__ len, uint64_t n,
+                   const uint8_t* __restrict__ skey, uint32_t sklen, LcApEv* __restrict__ ev, uint32_t* bad) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n)
+        return;
+    const uint32_t l = len[i], o = l == LC_AP_NO_KEY ? 0u : off[i];
+    if (l != LC_AP_NO_KEY && (uint64_t)o + l > base_len) {
+        atomicOr(bad, 1u);
+        ev[i] = LcApEv{0, 0, 0, {0, 0, 0, 0, 0}, 0, LC_AP_F_NONE, 0};
+        return;
+    }
+    ev[i] = lc_ap_scan(*conf, base, base_len, o, l, skey, sklen);
+}
+
+constexpr int kApWarps = 4;
+
+__global__ void __launch_bounds__(32 * kApWarps)
+    ap_resolve_kernel(LcTsNow now, const LcApEv* __restrict__ ev, const uint32_t* __restrict__ grp, uint64_t ngroups,
+                      uint8_t* __restrict__ status, int64_t* __restrict__ sec, uint32_t* __restrict__ nsec,
+                      int64_t* __restrict__ micro, uint32_t* __restrict__ nent,
+                      unsigned long long* __restrict__ counters) {
+    __shared__ LcApWarp ws[kApWarps];
+    const uint32_t wi = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint64_t cnt[5] = {0, 0, 0, 0, 0};
+    for (uint64_t g = (uint64_t)blockIdx.x * kApWarps + wi; g < ngroups; g += (uint64_t)gridDim.x * kApWarps)
+        lc_ap_resolve(now, ev, grp[g], grp[g + 1], status, sec, nsec, micro, nent, cnt, ws[wi], lane, 32);
+    for (int k = 0; k < 5; ++k) {
+        const uint32_t t = __reduce_add_sync(0xFFFFFFFFu, (uint32_t)cnt[k]);
+        if (lane == 0 && t)
+            atomicAdd(&counters[k], (unsigned long long)t);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    ap_emit_kernel(const uint8_t* __restrict__ base, const uint32_t* __restrict__ off,
+                   const uint32_t* __restrict__ len, const uint8_t* __restrict__ status, uint64_t n,
+                   const uint64_t* __restrict__ first, LcApEntry* __restrict__ entries) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || (status[i] & 7u) != LC_AP_ST_OK)
+        return;
+    LcApEmit em{entries + first[i], off[i]};
+    lc_ap_fields(base + off[i], len[i], em);
+}
+
+void launch_ap_scan(const LcTsConf* d_conf, const uint8_t* d_base, uint64_t base_len, const uint32_t* d_off,
+                    const uint32_t* d_len, uint64_t n, const uint8_t* d_skey, uint32_t sklen, LcApEv* d_ev,
+                    uint32_t* d_bad, cudaStream_t st) {
+    if (n)
+        ap_scan_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_conf, d_base, base_len, d_off, d_len, n, d_skey,
+                                                                     sklen, d_ev, d_bad);
+}
+
+void launch_ap_resolve(const LcTsNow& now, const LcApEv* d_ev, const uint32_t* d_grp, uint64_t ngroups,
+                       uint8_t* d_status, int64_t* d_sec, uint32_t* d_nsec, int64_t* d_micro, uint32_t* d_nent,
+                       unsigned long long* d_counters, cudaStream_t st) {
+    if (!ngroups)
+        return;
+    const uint64_t blocks = (ngroups + kApWarps - 1) / kApWarps;
+    ap_resolve_kernel<<<(unsigned)(blocks < (1u << 20) ? blocks : (1u << 20)), 32 * kApWarps, 0, st>>>(
+        now, d_ev, d_grp, ngroups, d_status, d_sec, d_nsec, d_micro, d_nent, d_counters);
+}
+
+void launch_ap_emit(const uint8_t* d_base, const uint32_t* d_off, const uint32_t* d_len, const uint8_t* d_status,
+                    uint64_t n, const uint64_t* d_first, LcApEntry* d_entries, cudaStream_t st) {
+    if (n)
+        ap_emit_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_base, d_off, d_len, d_status, n, d_first,
+                                                                     d_entries);
+}
+
 } // namespace lck

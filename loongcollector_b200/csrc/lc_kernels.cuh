@@ -18,6 +18,8 @@ struct LcTsConf;
 struct LcTsNow;
 struct LcTsSpans;
 struct LcTsFull;
+struct LcApEv;
+struct LcApEntry;
 struct LcLz4Chunk;
 
 namespace lck {
@@ -386,5 +388,18 @@ void launch_ts_full(const LcTsConf* d_conf, const LcTsNow& now, const uint8_t* d
 void launch_ts_resolve(const LcTsConf* d_conf, const LcTsNow& now, const uint8_t* d_base, const LcTsSpans& sp, const LcTsFull* d_full,
                        const uint32_t* d_grp, uint64_t ngroups, int64_t* d_sec, uint32_t* d_nsec, uint8_t* d_status,
                        unsigned long long* d_counters, cudaStream_t st);
+
+// ProcessorParseApsaraNative (lc_exec.cuh): launch_ap_scan reads each event's time form, full parse, hit
+// nanoseconds, cache key and entry count (one thread per event; *d_bad |= 1 for an event past base_len, which is not
+// read); launch_ap_resolve applies the time cache and the verdicts, one warp per group, and writes each event's entry
+// count (0 unless parsed); after an exclusive sum of those counts (d_first), launch_ap_emit writes the entries.
+void launch_ap_scan(const LcTsConf* d_conf, const uint8_t* d_base, uint64_t base_len, const uint32_t* d_off,
+                    const uint32_t* d_len, uint64_t n, const uint8_t* d_skey, uint32_t sklen, LcApEv* d_ev,
+                    uint32_t* d_bad, cudaStream_t st);
+void launch_ap_resolve(const LcTsNow& now, const LcApEv* d_ev, const uint32_t* d_grp, uint64_t ngroups,
+                       uint8_t* d_status, int64_t* d_sec, uint32_t* d_nsec, int64_t* d_micro, uint32_t* d_nent,
+                       unsigned long long* d_counters, cudaStream_t st);
+void launch_ap_emit(const uint8_t* d_base, const uint32_t* d_off, const uint32_t* d_len, const uint8_t* d_status,
+                    uint64_t n, const uint64_t* d_first, LcApEntry* d_entries, cudaStream_t st);
 
 } // namespace lck

@@ -3401,7 +3401,162 @@ std::vector<std::pair<std::string, uint64_t>> ProcessorParseTimestampNative::Cou
             {"history_failure", mHistoryFailureTotal.GetValue()}};
 }
 
+// ------------------------------------------------------------------------------------- ProcessorParseApsaraNative
+const std::string ProcessorParseApsaraNative::sName = "processor_parse_apsara_native";
+
+bool ProcessorParseApsaraNative::Init(const Json::Value& config) {
+    mWarnings.clear();
+    if (!GetString(config, "SourceKey", mSourceKey))
+        return Fail("mandatory string param SourceKey is missing");
+    mLogTimeZoneOffsetSecond = 0;
+    mTimezone.clear();
+    if (config.isMember("Timezone") && !config["Timezone"].isString()) {
+        mWarnings.push_back("optional string param Timezone is not of type string");
+    } else if (GetString(config, "Timezone", mTimezone) && !mTimezone.empty()) {
+        int tz = 0;
+        if (ParseGmtOffset(mTimezone, tz))
+            mLogTimeZoneOffsetSecond = tz - LocalGmtOffset();
+        else
+            mWarnings.push_back("string param Timezone is not valid");
+    }
+    if (!mCommonParserOptions.Init(config))
+        return false;
+    lc_apsara_free(mProgram);
+    mProgram = nullptr;
+    if (lc_apsara_compile(mSourceKey.data(), mSourceKey.size(), mLogTimeZoneOffsetSecond, &mProgram) != LC_OK)
+        return Fail(std::string("lc_apsara_compile: ") + lc_last_error());
+    return true;
+}
+
+void ProcessorParseApsaraNative::Process(PipelineEventGroup& group) {
+    std::vector<PipelineEventGroup> one;
+    one.emplace_back(std::move(group));
+    Process(one);
+    group = std::move(one[0]);
+}
+
+void ProcessorParseApsaraNative::Process(std::vector<PipelineEventGroup>& groups) {
+    static const std::string kKeys[4] = {"__LEVEL__", "__THREAD__", "__FILE__", "__LINE__"};
+    static const std::string kMicro = "microtime";
+    if (!mProgram)
+        return;
+    // values of every group back to back, one event table, group starts
+    std::string bytes;
+    std::vector<uint32_t> off, len, grp{0};
+    for (auto& g : groups) {
+        for (PipelineEventPtr& e : g.MutableEvents()) {
+            const LogEvent* ev = IsSupportedEvent(e) ? &e.Cast<LogEvent>() : nullptr;
+            if (ev && ev->HasContent(mSourceKey)) {
+                const StringView v = ev->GetContent(mSourceKey);
+                off.push_back((uint32_t)bytes.size());
+                len.push_back((uint32_t)v.size());
+                bytes.append(v.data(), v.size());
+            } else {
+                off.push_back(0);
+                len.push_back(LC_TS_NO_KEY);
+            }
+        }
+        grp.push_back((uint32_t)off.size());
+    }
+    const uint64_t n = off.size();
+    if (n == 0)
+        return;
+    std::vector<int64_t> sec(n), micro(n);
+    std::vector<uint32_t> nsec(n);
+    std::vector<uint8_t> status(n);
+    std::vector<uint64_t> first(n + 1);
+    std::vector<lc_apsara_entry_t> ent(n * 8);
+    uint64_t cnt[5], nent = 0;
+    try {
+        for (;;) {
+            const int rc = lc_apsara_parse(Engine(), mProgram, reinterpret_cast<const uint8_t*>(bytes.data()),
+                                           bytes.size(), off.data(), len.data(), n, grp.data(), groups.size(),
+                                           (int64_t)time(nullptr), mDiscardOldData ? mDiscardInterval : -1,
+                                           status.data(), sec.data(), nsec.data(), micro.data(), first.data(),
+                                           ent.data(), ent.size(), &nent, cnt);
+            if (rc != LC_ERR_CAPACITY) {
+                Check(rc, "lc_apsara_parse");
+                break;
+            }
+            ent.resize(nent);
+        }
+    } catch (const std::exception& ex) {
+        EngineFailed(ex.what());
+        return;
+    }
+    uint64_t i = 0, unsupported = 0, erased = 0;
+    for (auto& g : groups) {
+        EventsContainer& events = g.MutableEvents();
+        SourceBuffer& sb = *g.GetSourceBuffer();
+        const StringBuffer renamed = sb.CopyString(mCommonParserOptions.mRenamedSourceKey);
+        const StringView rkey(renamed.data, renamed.size);
+        auto addIfAbsent = [](LogEvent& ev, StringView k, StringView v) {
+            if (!ev.HasContent(k))
+                ev.AppendContentNoCopy(k, v);
+        };
+        size_t wIdx = 0;
+        for (size_t rIdx = 0; rIdx < events.size(); ++rIdx, ++i) {
+            const uint32_t st = status[i] & 7u;
+            if (!IsSupportedEvent(events[rIdx])) {
+                unsupported++; // counted as key_not_found by the device: ProcessEvent counts it out_failed
+            } else if (st == LC_APSARA_DISCARDED) {
+                continue;
+            } else if (st == LC_APSARA_FAILED || st == LC_APSARA_OK) {
+                LogEvent& ev = events[rIdx].Cast<LogEvent>();
+                const StringView v = ev.GetContent(mSourceKey);
+                const bool ok = st == LC_APSARA_OK;
+                if (ok) {
+                    ev.SetTimestamp(sec[i], nsec[i]);
+                    for (uint64_t k = first[i]; k < first[i + 1]; ++k) {
+                        const lc_apsara_entry_t& x = ent[k];
+                        const StringView val(v.data() + (x.val_off - off[i]), x.val_len);
+                        if (x.key_off >= LC_APSARA_KEY_LEVEL)
+                            ev.AppendContentNoCopy(kKeys[x.key_off - LC_APSARA_KEY_LEVEL], val);
+                        else
+                            ev.AppendContentNoCopy(StringView(v.data() + (x.key_off - off[i]), x.key_len), val);
+                    }
+                    const StringBuffer us = sb.CopyString(std::to_string(micro[i]));
+                    ev.AppendContentNoCopy(kMicro, StringView(us.data, us.size));
+                    if (!(status[i] & LC_APSARA_OVERWRITTEN))
+                        ev.DelContent(mSourceKey);
+                    if (mCommonParserOptions.ShouldAddSourceContent(true))
+                        addIfAbsent(ev, rkey, v);
+                } else {
+                    ev.DelContent(mSourceKey);
+                    if (mCommonParserOptions.ShouldAddSourceContent(false))
+                        addIfAbsent(ev, rkey, v);
+                    if (mCommonParserOptions.ShouldAddLegacyUnmatchedRawLog(false))
+                        addIfAbsent(ev, CommonParserOptions::legacyUnmatchedRawLogKey, v);
+                    if (mCommonParserOptions.ShouldEraseEvent(false, ev, g.GetAllMetadata())) {
+                        erased++;
+                        continue;
+                    }
+                }
+            }
+            if (wIdx != rIdx)
+                events[wIdx] = std::move(events[rIdx]);
+            ++wIdx;
+        }
+        events.resize(wIdx);
+    }
+    mOutKeyNotFoundEventsTotal.Add(cnt[0] - unsupported);
+    mOutFailedEventsTotal.Add(cnt[1] + unsupported);
+    mHistoryFailureTotal.Add(cnt[2]);
+    mDiscardedEventsTotal.Add(cnt[3] + erased);
+    mOutSuccessfulEventsTotal.Add(cnt[4]);
+}
+
+std::vector<std::pair<std::string, uint64_t>> ProcessorParseApsaraNative::Counters() const {
+    return {{"discarded", mDiscardedEventsTotal.GetValue()},
+            {"out_failed", mOutFailedEventsTotal.GetValue()},
+            {"out_key_not_found", mOutKeyNotFoundEventsTotal.GetValue()},
+            {"out_successful", mOutSuccessfulEventsTotal.GetValue()},
+            {"history_failure", mHistoryFailureTotal.GetValue()}};
+}
+
 Processor* CreateProcessor(const std::string& type) {
+    if (type == ProcessorParseApsaraNative::sName)
+        return new ProcessorParseApsaraNative;
     if (type == ProcessorParseTimestampNative::sName)
         return new ProcessorParseTimestampNative;
     if (type == ProcessorMergeMultilineLogNative::sName)

@@ -116,6 +116,7 @@ class ProcessorParseRegexNative;
 class ProcessorParseDelimiterNative;
 class ProcessorFilterNative;
 class ProcessorParseTimestampNative;
+class ProcessorParseApsaraNative;
 
 class ProcessorSplitLogStringNative : public Processor {
 public:
@@ -423,6 +424,37 @@ protected:
 private:
     friend struct SplitRegexTsStage; // the split -> regex -> timestamp chain's SerializeSls
     lc_timestamp_t* mProgram = nullptr;
+};
+
+// processor_parse_apsara_native (ProcessorParseApsaraNative.cpp:37-473): the groups of one call go to the device in
+// one lc_apsara_parse call (the time parse, the time cache, the base and key:value field scans run there, the cache
+// starting empty in every group); the host appends the entries and "microtime" (AppendContentNoCopy, no
+// de-duplication), applies CommonParserOptions, erases events and adds the counters.  "now" is read once per call,
+// where the reference calls time(NULL) per event.
+class ProcessorParseApsaraNative : public Processor {
+public:
+    static const std::string sName;
+    const std::string& Name() const override { return sName; }
+    ~ProcessorParseApsaraNative() override { lc_apsara_free(mProgram); }
+    bool Init(const Json::Value& config) override;
+    void Process(PipelineEventGroup& group) override;
+    void Process(std::vector<PipelineEventGroup>& groups) override;
+    std::vector<std::pair<std::string, uint64_t>> Counters() const override;
+    std::string mSourceKey, mTimezone;
+    int32_t mLogTimeZoneOffsetSecond = 0;
+    CommonParserOptions mCommonParserOptions;
+    // ilogtail_discard_old_data (on by default; off for one-time pipelines) and ilogtail_discard_interval
+    bool mDiscardOldData = true;
+    int32_t mDiscardInterval = 43200;
+    std::vector<std::string> mWarnings; // the reference's PARAM_WARNING_* messages of the last Init
+    Counter mDiscardedEventsTotal, mOutFailedEventsTotal, mOutKeyNotFoundEventsTotal, mOutSuccessfulEventsTotal,
+        mHistoryFailureTotal;
+
+protected:
+    bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
+
+private:
+    lc_apsara_t* mProgram = nullptr;
 };
 
 class ProcessorFilterNative : public Processor {

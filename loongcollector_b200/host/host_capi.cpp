@@ -120,6 +120,20 @@ char* lc_host_processor_counters(const lc_host_processor_t* p) {
     return dup(v.toString());
 }
 
+int lc_host_processor_set_discard_old_data(lc_host_processor_t* p, int enabled, int32_t interval) {
+    if (auto* t = dynamic_cast<ProcessorParseTimestampNative*>(p->proc.get())) {
+        t->mDiscardOldData = enabled != 0;
+        t->mDiscardInterval = interval;
+        return 0;
+    }
+    if (auto* a = dynamic_cast<ProcessorParseApsaraNative*>(p->proc.get())) {
+        a->mDiscardOldData = enabled != 0;
+        a->mDiscardInterval = interval;
+        return 0;
+    }
+    return -1;
+}
+
 void lc_host_string_free(char* s) { free(s); }
 
 char* lc_host_sls_serialize(const char* group_json, int enable_ns, unsigned long long* len_out, char** err_out) {

@@ -250,3 +250,47 @@ def csv_pool(n, seed=DEFAULT_SEED, pool=16384):
             cells.append(c)
         lines.append((",".join(cells) + "\n").encode("ascii"))
     return lines
+
+
+def apsara_lines(n, seed=DEFAULT_SEED, t0=1700000000, groups_of=1024):
+    """n Apsara log lines: "[YYYY-mm-dd HH:MM:SS.ffffff]" in runs of the same second (so the time cache hits), about
+    1 % "[<epoch micros>]" lines and 0.5 % malformed heads; 2-4 base fields in varying order, 2-8 key:value fields,
+    80 B - 2 KB.  Returns (buf u8, off u32, len u32, grp u32): one group per groups_of lines."""
+    import time as _time
+    rng = random.Random(seed)
+    parts, off, ln, pos = [], np.empty(n, np.uint32), np.empty(n, np.uint32), 0
+    sec, run = t0, 0
+    for i in range(n):
+        if run == 0:
+            sec += rng.randrange(1, 3)
+            run = rng.randrange(1, 64)
+        run -= 1
+        x = rng.random()
+        if x < 0.01:
+            head = b"[%d%06d]" % (sec, rng.randrange(10 ** 6))
+        elif x < 0.015:
+            head = rng.choice([b"[2024-13-01 00:00:00]", b"2024-01-01 00:00:00", b"[2024-01-01 00"])
+        else:
+            head = b"[" + _time.strftime("%Y-%m-%d %H:%M:%S", _time.gmtime(sec)).encode() + \
+                b".%06d]" % rng.randrange(10 ** 6)
+        base = [b"[" + rng.choice([b"INFO", b"WARNING", b"ERROR", b"DEBUG"]) + b"]",
+                b"[%d]" % rng.randrange(1, 99999), b"[src/%s.cpp:%d]" % (_rand_word(rng, 8).encode(), rng.randrange(9999)),
+                b"[" + _rand_word(rng, 6).encode() + b"]"]
+        rng.shuffle(base)
+        fields = [head] + base[:rng.randint(2, 4)]
+        target = rng.randint(80, 2048)
+        nkv = rng.randint(2, 8)
+        per = max(1, (target - sum(len(f) + 1 for f in fields)) // nkv - 8)
+        for k in range(nkv):
+            fields.append(b"%s:%s" % (_rand_word(rng, rng.randint(3, 10)).encode(),
+                                      _rand_word(rng, rng.randint(1, per)).encode()))
+        line = b"\t".join(fields)
+        off[i], ln[i] = pos, len(line)
+        parts.append(line)
+        pos += len(line)
+    grp = np.arange(0, n + groups_of, groups_of, dtype=np.uint64)
+    grp = np.minimum(grp, n).astype(np.uint32)
+    grp = np.unique(grp)
+    if grp[-1] != n or grp.size == 1:
+        grp = np.append(grp, np.uint32(n))
+    return np.frombuffer(b"".join(parts), np.uint8), off, ln, grp
