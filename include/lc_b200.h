@@ -39,6 +39,7 @@ extern "C" {
 #define LC_ERR_REGEX_UNSUPPORTED 4 /* valid for boost but outside the automaton subset (back-refs, look-behind, multi-byte look-ahead...) */
 #define LC_ERR_CAPACITY 5      /* caller-provided output capacity too small; *n_out holds the needed count */
 #define LC_ERR_TOO_LARGE 6     /* buffer >= 4 GiB or >= 2^30 lines in one call */
+#define LC_ERR_INTERNAL 7      /* a device pass would have written past its own output range; nothing was */
 
 /* per-event status of lc_regex_parse (ProcessorParseRegexNative.cpp:186-253) */
 #define LC_REGEX_OK 0
@@ -1022,6 +1023,73 @@ int lc_apsara_parse_dev(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* d_
                         uint64_t ngroups, int64_t now, int32_t discard_interval, uint8_t* d_status, int64_t* d_sec,
                         uint32_t* d_nsec, int64_t* d_micro, uint64_t* d_first, lc_apsara_entry_t* d_entries,
                         uint64_t entry_cap, uint64_t* n_entries, uint64_t* d_counters);
+
+/* ---- ProcessorParseJsonNative (ProcessorParseJsonNative.cpp: ProcessEvent, JsonLogLineParserSimdJson,
+ *      OptimizedValueToStringBuffer, ProcessNumberValueOptimized)
+ * lc_json_compile is Init: source_key is SourceKey.  lc_json_parse[_dev]: event i's value is base[ev_off[i], +
+ * ev_len[i]); ev_len[i] == LC_TS_NO_KEY means the event has no SourceKey.  No state crosses events, so there is no
+ * group table.
+ *
+ * Verdict (pinned; the reference's default build parses with simdjson's on-demand API, the other build with
+ * rapidjson, neither of which is linked here).  An event parses when its value is strict RFC 8259 JSON whose root is
+ * an object: valid UTF-8 everywhere, no raw control bytes in strings, only valid escapes, \u surrogates in pairs,
+ * numbers of the JSON grammar (no leading zeros, no '+', no NaN / Infinity), nesting depth (the root object is depth
+ * 1) at most 1024 as simdjson's default limit, whitespace around the root object.  The document ends at the root's
+ * closing brace; after it (and whitespace) a NUL byte ends the input and what follows it is ignored, as in both
+ * reference paths (the reference's TestMultipleLines depends on it); any other byte fails the event.  Where
+ * simdjson's lazy on-demand API accepts input this rule rejects -- malformed nested values such as {"a":[1,,2]},
+ * trailing garbage, "tru" atoms -- the event fails here; rapidjson fails these inputs too.
+ *
+ * Rendering (pinned to the simdjson path):
+ *   string          its unescaped bytes (\u0000 is a NUL byte, a surrogate pair 4 bytes of UTF-8)
+ *   true / false    verbatim;  null: empty
+ *   object / array  the source text from its opening to its matching closing bracket, inner whitespace kept
+ *   integer         (no '.', no exponent) with '-': "%" PRId64 when it fits int64 ("-0" is "0"), else empty;
+ *                   without '-': "%" PRIu64 when it fits uint64, else empty
+ *   other numbers   std::to_string(double) = "%f" of the correctly rounded double (round half to even on the
+ *                   sixth decimal); a double that overflows renders empty, one that underflows "0.000000" with its
+ *                   sign
+ * The empty renderings of out-of-range integers and overflowing doubles follow from the reference code and
+ * simdjson's documented range errors; they are not confirmed by a run.  An empty rendering keeps the member.
+ * Keys are unescaped; a key equal to SourceKey sets LC_JSON_OVERWRITTEN.
+ *
+ * Outputs:
+ *   - status[i]: LC_JSON_* in the low bits, LC_JSON_OVERWRITTEN with LC_JSON_OK.
+ *   - first[i] .. first[i + 1]: event i's entries (first has n + 1 words; only LC_JSON_OK events have any): the
+ *     top-level members in document order, duplicates included (the caller applies them with overwrite, as
+ *     AddLog(key, value, event) does).  An entry's key_off / val_off is an offset into base, or, with LC_JSON_ARENA
+ *     set, (offset | LC_JSON_ARENA) into the arena.  The arena holds only bytes that are not in base: keys and
+ *     strings with escapes, and every "%f" rendering, in document order, event after event.  Everything else is a
+ *     span of base: strings without escapes (without their quotes), integers ("-0" points at its "0"), true /
+ *     false, nested values.  An empty rendering is val_len 0 with val_off at the value's first byte.
+ *   - counters[3] = key_not_found, out_failed, ok (events that parsed).  out_failed counts parse failures, not
+ *     empty values (LC_JSON_EMPTY takes the failure path uncounted, as the reference does).
+ * *n_entries and *arena_bytes are the totals; when either exceeds its cap the call returns LC_ERR_CAPACITY and writes
+ * no entry and no arena byte (the other outputs are written), so caps of 0 make a sizing query.  An event past
+ * base_len (ev_off + ev_len computed in 64 bits) is refused with LC_ERR_INVALID_ARG; the _dev call finds it on the
+ * device without reading it.  base_len or an arena total of 2^31 or more is refused with LC_ERR_TOO_LARGE.
+ * LC_ERR_INTERNAL reports an emit pass that would have left its event's ranges (nothing was written past them).
+ * The _dev call takes device tables and, like lc_apsara_parse_dev, waits for the device before it returns. */
+#define LC_JSON_OK 0
+#define LC_JSON_NOT_FOUND 1 /* no SourceKey: out_key_not_found++, event kept */
+#define LC_JSON_EMPTY 2     /* empty value: the failure path, not counted */
+#define LC_JSON_FAILED 3    /* not a JSON object by the rule above: out_failed++, the failure path */
+#define LC_JSON_OVERWRITTEN 0x80
+#define LC_JSON_ARENA 0x80000000u
+typedef struct lc_json lc_json_t;
+typedef struct {
+    uint32_t key_off, key_len, val_off, val_len;
+} lc_json_entry_t;
+int lc_json_compile(const char* source_key, size_t key_len, lc_json_t** out);
+void lc_json_free(lc_json_t* js);
+int lc_json_parse(lc_engine_t* e, const lc_json_t* js, const uint8_t* base, uint64_t base_len, const uint32_t* ev_off,
+                  const uint32_t* ev_len, uint64_t n, uint8_t* status, uint64_t* first, lc_json_entry_t* entries,
+                  uint64_t entry_cap, uint64_t* n_entries, uint8_t* arena, uint64_t arena_cap, uint64_t* arena_bytes,
+                  uint64_t* counters);
+int lc_json_parse_dev(lc_engine_t* e, const lc_json_t* js, const uint8_t* d_base, uint64_t base_len,
+                      const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, uint8_t* d_status,
+                      uint64_t* d_first, lc_json_entry_t* d_entries, uint64_t entry_cap, uint64_t* n_entries,
+                      uint8_t* d_arena, uint64_t arena_cap, uint64_t* arena_bytes, uint64_t* d_counters);
 
 #ifdef __cplusplus
 }

@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libloongcollector_b200.so")
 SOURCES = ["regex_compiler.cpp", "lc_kernels.cu", "lc_capi.cu"]
-HEADERS = ["lc_tables.h", "lc_exec.cuh", "lc_scan.cuh", "lc_kernels.cuh", "regex_compiler.h",
+HEADERS = ["lc_tables.h", "lc_json_pow5.h", "lc_exec.cuh", "lc_scan.cuh", "lc_kernels.cuh", "regex_compiler.h",
            os.path.join("..", "..", "include", "lc_b200.h")]
 HOST_DIR = os.path.join(HERE, "host")
 

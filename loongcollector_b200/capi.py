@@ -110,6 +110,11 @@ def lib():
     ap_args = [vp, vp, vp, u64, vp, vp, u64, vp, u64, C.c_int64, i32, vp, vp, vp, vp, vp, vp, u64, C.POINTER(u64), vp]
     L.lc_apsara_parse.argtypes = ap_args
     L.lc_apsara_parse_dev.argtypes = ap_args
+    L.lc_json_compile.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(vp)]
+    L.lc_json_free.argtypes = [vp]
+    js_args = [vp, vp, vp, u64, vp, vp, u64, vp, vp, vp, u64, C.POINTER(u64), vp, u64, C.POINTER(u64), vp]
+    L.lc_json_parse.argtypes = js_args
+    L.lc_json_parse_dev.argtypes = js_args
     L.lc_delim_parse_sls_lz4.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32, u8, i32, i32, i32, u32] + \
         sls_cfg + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
     L.lc_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp] + sls_cfg + \
@@ -302,6 +307,34 @@ LC_APSARA_OK, LC_APSARA_NOT_FOUND, LC_APSARA_EMPTY, LC_APSARA_FAILED, LC_APSARA_
 LC_APSARA_OVERWRITTEN = 0x80
 LC_APSARA_KEY_LEVEL = 0xFFFFFFF0
 APSARA_BASE_KEYS = (b"__LEVEL__", b"__THREAD__", b"__FILE__", b"__LINE__")
+
+
+class Json:
+    """ProcessorParseJsonNative's Init (lc_json_compile): SourceKey is fixed here."""
+
+    def __init__(self, source_key):
+        if isinstance(source_key, str):
+            source_key = source_key.encode("utf-8")
+        h = C.c_void_p()
+        L = lib()
+        rc = L.lc_json_compile(source_key, len(source_key), C.byref(h))
+        self._h = h
+        if rc != LC_OK:
+            self._h = None
+            raise LcError(rc, L.lc_last_error().decode())
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib().lc_json_free(self._h)
+        except Exception:
+            pass
+
+
+# lc_json_parse's status values and arena tag
+LC_JSON_OK, LC_JSON_NOT_FOUND, LC_JSON_EMPTY, LC_JSON_FAILED, LC_JSON_OVERWRITTEN = 0, 1, 2, 3, 0x80
+LC_JSON_ARENA = 0x80000000
+LC_ERR_INTERNAL = 7
 
 
 def _rh(r):
@@ -1383,6 +1416,41 @@ class Engine:
                                          _p(d_nsec), _p(d_micro), _p(d_first), _p(d_entries), entry_cap, C.byref(m),
                                          _p(d_counters)))
         return m.value
+
+    def json_parse(self, js, base, ev_off, ev_len, entry_cap=None, arena_cap=None):
+        """ProcessorParseJsonNative over host buffers (lc_json_parse): ev_len LC_TS_NO_KEY = no SourceKey.  Caps of
+        None size the outputs with a first call.  Returns (status u8, first u64[n + 1], entries u32[m, 4], arena bytes,
+        counters u64[3])."""
+        a = _u8(base)
+        ev_off = np.ascontiguousarray(ev_off, np.uint32)
+        ev_len = np.ascontiguousarray(ev_len, np.uint32)
+        n = ev_off.size
+        st, first, cnt = np.empty(n, np.uint8), np.empty(n + 1, np.uint64), np.zeros(3, np.uint64)
+        m, ab = C.c_uint64(0), C.c_uint64(0)
+
+        def call(ecap, ent, acap, ar):
+            return lib().lc_json_parse(self._h, js._h, _p(a), a.size, _p(ev_off), _p(ev_len), n, _p(st), _p(first),
+                                       _p(ent), ecap, C.byref(m), _p(ar), acap, C.byref(ab), _p(cnt))
+        if entry_cap is None or arena_cap is None:
+            rc = call(0, np.zeros((1, 4), np.uint32), 0, np.zeros(1, np.uint8))
+            if rc not in (LC_OK, LC_ERR_CAPACITY):
+                _check(rc)
+            entry_cap = m.value if entry_cap is None else entry_cap
+            arena_cap = ab.value if arena_cap is None else arena_cap
+        ent = np.zeros((max(int(entry_cap), 1), 4), np.uint32)
+        ar = np.zeros(max(int(arena_cap), 1), np.uint8)
+        _check(call(int(entry_cap), ent, int(arena_cap), ar))
+        return st, first, ent[:m.value], ar[:ab.value].tobytes(), cnt
+
+    def json_parse_dev(self, js, d_base, base_len, d_ev_off, d_ev_len, n, d_status, d_first, d_entries, entry_cap,
+                       d_arena, arena_cap, d_counters):
+        """lc_json_parse_dev over device tables; waits for the device.  Returns (entry count, arena bytes); raises
+        LcError with LC_ERR_CAPACITY when either exceeds its cap (nothing is written to the entries or the arena)."""
+        m, ab = C.c_uint64(0), C.c_uint64(0)
+        _check(lib().lc_json_parse_dev(self._h, js._h, _p(d_base), base_len, _p(d_ev_off), _p(d_ev_len), n,
+                                       _p(d_status), _p(d_first), _p(d_entries), entry_cap, C.byref(m), _p(d_arena),
+                                       arena_cap, C.byref(ab), _p(d_counters)))
+        return m.value, ab.value
 
     def timestamp_parse_dev(self, ts, d_base, base_len, d_ev_off, d_ev_len, n, d_grp, ngroups, now, discard_interval,
                             d_sec, d_nsec, d_status, d_counters):

@@ -127,6 +127,11 @@ struct lc_engine {
     DevBuf ap_conf, ap_ev, ap_nent, ap_small;
     uint64_t ap_conf_id = 0;
     DevBuf ap_status, ap_sec, ap_nsec, ap_micro, ap_first, ap_ent;
+    // JSON parse: SourceKey (js_conf_id's), the counts, the slow flags and list, the arena starts, the flags; the host
+    // call's copies of its outputs
+    DevBuf js_conf, js_nent, js_narena, js_slow, js_list, js_afirst, js_small, js_pow5;
+    uint64_t js_conf_id = 0;
+    DevBuf js_status, js_first, js_ent, js_arena, js_cnt;
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
     std::unordered_map<uint64_t, void*> blobs; // regex id * 4 + layout -> device blob
@@ -346,7 +351,9 @@ void lc_engine_destroy(lc_engine_t* e) {
                       &e->sdr_status, &e->sdr_nf, &e->sdr_f_off, &e->sdr_f_len, &e->sdr_f_dq, &e->sdr_okey,
                       &e->ts_conf, &e->ts_full, &e->ts_cnt, &e->st_val, &e->st_sec, &e->st_nsec, &e->st_status,
                       &e->ap_conf, &e->ap_ev, &e->ap_nent, &e->ap_small, &e->ap_status, &e->ap_sec, &e->ap_nsec,
-                      &e->ap_micro, &e->ap_first, &e->ap_ent};
+                      &e->ap_micro, &e->ap_first, &e->ap_ent, &e->js_conf, &e->js_nent, &e->js_narena,
+                      &e->js_slow, &e->js_list, &e->js_afirst, &e->js_small, &e->js_status, &e->js_first, &e->js_ent,
+                      &e->js_arena, &e->js_cnt, &e->js_pow5};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -4529,6 +4536,207 @@ int lc_apsara_parse(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* base, 
     CU_TRY(cudaMemcpyAsync(micro, e->ap_micro.p, n * 8, cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(cudaMemcpyAsync(first, e->ap_first.p, (n + 1) * 8, cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(cudaMemcpyAsync(counters, e->ts_cnt.p, 5 * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ JSON parse
+struct lc_json {
+    uint64_t id;
+    std::string skey;
+};
+
+int lc_json_compile(const char* source_key, size_t key_len, lc_json_t** out) {
+    if (!out || (!source_key && key_len) || key_len >= 0xFFFFFFFFull)
+        return fail(LC_ERR_INVALID_ARG, "lc_json_compile: bad arguments");
+    *out = nullptr;
+    lc_json* j = new (std::nothrow) lc_json;
+    if (!j)
+        return fail(LC_ERR_INVALID_ARG, "out of host memory");
+    j->skey.assign(source_key ? source_key : "", key_len);
+    j->id = g_regex_ids.fetch_add(1);
+    *out = j;
+    return LC_OK;
+}
+
+void lc_json_free(lc_json_t* j) { delete j; }
+
+static_assert(sizeof(lc_json_entry_t) == sizeof(LcJsonEntry), "entry layout");
+
+namespace {
+
+// The count passes (fast, then slow over the events the fast walk gave up on) and both exclusive sums, on the caller's
+// device tables, up to the totals, which the host receives after a wait for the device.
+int js_count(lc_engine_t* e, const lc_json_t* js, const char* what, const uint8_t* d_base, uint64_t base_len,
+             const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, uint8_t* d_status, uint64_t* d_first,
+             uint64_t* n_entries, uint64_t* arena_bytes, uint64_t* d_counters) {
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    *n_entries = *arena_bytes = 0;
+    CU_TRY(cudaMemsetAsync(d_counters, 0, 3 * sizeof(uint64_t), e->stream));
+    if (n == 0) {
+        CU_TRY(cudaMemsetAsync(d_first, 0, 8, e->stream));
+        CU_TRY(cudaStreamSynchronize(e->stream));
+        return LC_OK;
+    }
+    if (!e->js_pow5.p) { // the Eisel-Lemire table, uploaded once per engine
+        CU_TRY(e->js_pow5.ensure(sizeof lc_json_pow5));
+        CU_TRY(cudaMemcpyAsync(e->js_pow5.p, lc_json_pow5, sizeof lc_json_pow5, cudaMemcpyHostToDevice, e->stream));
+    }
+    if (e->js_conf_id != js->id) {
+        CU_TRY(e->js_conf.ensure(js->skey.size() + 1));
+        if (!js->skey.empty())
+            CU_TRY(cudaMemcpyAsync(e->js_conf.p, js->skey.data(), js->skey.size(), cudaMemcpyHostToDevice, e->stream));
+        e->js_conf_id = js->id;
+    }
+    CU_TRY(e->js_nent.ensure(n * 4));
+    CU_TRY(e->js_narena.ensure(n * 4));
+    CU_TRY(e->js_slow.ensure(n));
+    CU_TRY(e->js_list.ensure(n * 4));
+    CU_TRY(e->js_afirst.ensure((n + 1) * 8));
+    CU_TRY(e->js_small.ensure(16));
+    CU_TRY(cudaMemsetAsync(e->js_small.p, 0, 16, e->stream));
+    uint32_t* d_bad = e->js_small.as<uint32_t>();
+    uint32_t* d_nslow = d_bad + 1;
+    const uint8_t* d_skey = e->js_conf.as<uint8_t>();
+    const uint32_t sklen = (uint32_t)js->skey.size();
+    auto* cnt = reinterpret_cast<unsigned long long*>(d_counters);
+    const uint64_t* d_pow5 = e->js_pow5.as<uint64_t>();
+    lck::launch_json_count(d_base, base_len, d_ev_off, d_ev_len, n, d_skey, sklen, d_pow5, d_status, e->js_nent.as<uint32_t>(),
+                           e->js_narena.as<uint32_t>(), e->js_slow.as<uint8_t>(), e->js_list.as<uint32_t>(), d_nslow,
+                           d_bad, cnt, e->stream);
+    lck::launch_json_count_slow(d_base, d_ev_off, d_ev_len, d_skey, sklen, d_pow5, e->js_list.as<uint32_t>(), d_nslow,
+                                d_status, e->js_nent.as<uint32_t>(), e->js_narena.as<uint32_t>(), cnt, e->stream);
+    const size_t tiles = lck::scan_tiles(n);
+    uint64_t* desc;
+    rc = prep_desc(e, 2 * tiles + 1, &desc);
+    if (rc)
+        return rc;
+    lck::launch_exclusive_sum(e->js_nent.as<uint32_t>(), n, d_first, d_first + n, desc, &e->small.as<Small>()->tickets[2],
+                              e->stream);
+    lck::launch_exclusive_sum(e->js_narena.as<uint32_t>(), n, e->js_afirst.as<uint64_t>(),
+                              e->js_afirst.as<uint64_t>() + n, desc + tiles + 1, &e->small.as<Small>()->tickets[3],
+                              e->stream);
+    e->launches += 4;
+    CU_TRY(cudaGetLastError());
+    uint32_t bad = 0;
+    CU_TRY(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(n_entries, d_first + n, 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(arena_bytes, e->js_afirst.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    if (bad) {
+        *n_entries = *arena_bytes = 0;
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": event outside the buffer");
+    }
+    if (*arena_bytes >= LC_JSON_ARENA)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": the arena would reach 2 GiB");
+    return LC_OK;
+}
+
+// The emit passes of js_count's events into d_entries / d_arena (room for both totals), waited for; LC_ERR_INTERNAL
+// when an event would have left its ranges.
+int js_emit(lc_engine_t* e, const lc_json_t* js, const char* what, const uint8_t* d_base, const uint32_t* d_ev_off,
+            const uint32_t* d_ev_len, uint64_t n, const uint8_t* d_status, const uint64_t* d_first,
+            lc_json_entry_t* d_entries, uint8_t* d_arena) {
+    uint32_t* d_bad = e->js_small.as<uint32_t>();
+    const uint8_t* d_skey = e->js_conf.as<uint8_t>();
+    const uint32_t sklen = (uint32_t)js->skey.size();
+    auto* ent = reinterpret_cast<LcJsonEntry*>(d_entries);
+    const uint64_t* d_pow5 = e->js_pow5.as<uint64_t>();
+    lck::launch_json_emit(d_base, d_ev_off, d_ev_len, n, d_skey, sklen, d_pow5, d_status, e->js_slow.as<uint8_t>(), d_first,
+                          e->js_afirst.as<uint64_t>(), ent, d_arena, d_bad, e->stream);
+    lck::launch_json_emit_slow(d_base, d_ev_off, d_ev_len, d_skey, sklen, d_pow5, d_status, e->js_list.as<uint32_t>(),
+                               d_bad + 1, d_first, e->js_afirst.as<uint64_t>(), ent, d_arena, d_bad, e->stream);
+    e->launches += 2;
+    CU_TRY(cudaGetLastError());
+    uint32_t bad = 0;
+    CU_TRY(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    if (bad)
+        return fail(LC_ERR_INTERNAL, std::string(what) + ": an emit pass would have left its event's output range");
+    return LC_OK;
+}
+
+} // namespace
+
+int lc_json_parse_dev(lc_engine_t* e, const lc_json_t* js, const uint8_t* d_base, uint64_t base_len,
+                      const uint32_t* d_ev_off, const uint32_t* d_ev_len, uint64_t n, uint8_t* d_status,
+                      uint64_t* d_first, lc_json_entry_t* d_entries, uint64_t entry_cap, uint64_t* n_entries,
+                      uint8_t* d_arena, uint64_t arena_cap, uint64_t* arena_bytes, uint64_t* d_counters) {
+    static const char* what = "lc_json_parse_dev";
+    if (!e || !js || !d_counters || !n_entries || !arena_bytes || !d_first || (entry_cap && !d_entries) ||
+        (arena_cap && !d_arena) || (n && (!d_base || !d_ev_off || !d_ev_len || !d_status)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    if (base_len >= LC_JSON_ARENA || n >= 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": buffer must be < 2 GiB and < 2^32 events per call");
+    int rc = js_count(e, js, what, d_base, base_len, d_ev_off, d_ev_len, n, d_status, d_first, n_entries, arena_bytes,
+                      d_counters);
+    if (rc)
+        return rc;
+    if (*n_entries > entry_cap || *arena_bytes > arena_cap)
+        return fail(LC_ERR_CAPACITY, std::string(what) + ": entry or arena capacity too small");
+    if (*n_entries)
+        return js_emit(e, js, what, d_base, d_ev_off, d_ev_len, n, d_status, d_first, d_entries, d_arena);
+    return LC_OK;
+}
+
+int lc_json_parse(lc_engine_t* e, const lc_json_t* js, const uint8_t* base, uint64_t base_len, const uint32_t* ev_off,
+                  const uint32_t* ev_len, uint64_t n, uint8_t* status, uint64_t* first, lc_json_entry_t* entries,
+                  uint64_t entry_cap, uint64_t* n_entries, uint8_t* arena, uint64_t arena_cap, uint64_t* arena_bytes,
+                  uint64_t* counters) {
+    static const char* what = "lc_json_parse";
+    if (!e || !js || !counters || !n_entries || !arena_bytes || !first || (entry_cap && !entries) ||
+        (arena_cap && !arena) || (n && (!base || !ev_off || !ev_len || !status)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    if (base_len >= LC_JSON_ARENA || n >= 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": buffer must be < 2 GiB and < 2^32 events per call");
+    memset(counters, 0, 3 * sizeof(uint64_t));
+    *n_entries = *arena_bytes = 0;
+    first[0] = 0;
+    if (n == 0)
+        return LC_OK;
+    for (uint64_t i = 0; i < n; ++i)
+        if (ev_len[i] != LC_JSON_NO_KEY && (uint64_t)ev_off[i] + ev_len[i] > base_len)
+            return fail(LC_ERR_INVALID_ARG, std::string(what) + ": event outside the buffer");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    CU_TRY(e->in.ensure(base_len + 16));
+    CU_TRY(e->ev_off.ensure(n * 4));
+    CU_TRY(e->ev_len.ensure(n * 4));
+    CU_TRY(e->js_status.ensure(n));
+    CU_TRY(e->js_first.ensure((n + 1) * 8));
+    CU_TRY(e->js_cnt.ensure(3 * sizeof(uint64_t)));
+    if (base_len)
+        CU_TRY(cudaMemcpyAsync(e->in.p, base, base_len, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(e->ev_off.p, ev_off, n * 4, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(cudaMemcpyAsync(e->ev_len.p, ev_len, n * 4, cudaMemcpyHostToDevice, e->stream));
+    const uint8_t* d_base = e->in.as<uint8_t>();
+    rc = js_count(e, js, what, d_base, base_len, e->ev_off.as<uint32_t>(), e->ev_len.as<uint32_t>(), n,
+                  e->js_status.as<uint8_t>(), e->js_first.as<uint64_t>(), n_entries, arena_bytes,
+                  e->js_cnt.as<uint64_t>());
+    if (rc)
+        return rc;
+    const uint64_t m = *n_entries, a = *arena_bytes;
+    if (m > entry_cap || a > arena_cap) {
+        rc = fail(LC_ERR_CAPACITY, std::string(what) + ": entry or arena capacity too small");
+    } else if (m) {
+        // the device copies are sized from the totals, not from the caps
+        CU_TRY(e->js_ent.ensure(m * sizeof(LcJsonEntry)));
+        CU_TRY(e->js_arena.ensure(a + 1));
+        rc = js_emit(e, js, what, d_base, e->ev_off.as<uint32_t>(), e->ev_len.as<uint32_t>(), n,
+                     e->js_status.as<uint8_t>(), e->js_first.as<uint64_t>(), e->js_ent.as<lc_json_entry_t>(),
+                     e->js_arena.as<uint8_t>());
+        if (rc)
+            return rc;
+        CU_TRY(cudaMemcpyAsync(entries, e->js_ent.p, m * sizeof(LcJsonEntry), cudaMemcpyDeviceToHost, e->stream));
+        if (a)
+            CU_TRY(cudaMemcpyAsync(arena, e->js_arena.p, a, cudaMemcpyDeviceToHost, e->stream));
+    }
+    CU_TRY(cudaMemcpyAsync(status, e->js_status.p, n, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(first, e->js_first.p, (n + 1) * 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaMemcpyAsync(counters, e->js_cnt.p, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(cudaStreamSynchronize(e->stream));
     return rc;
 }

@@ -4543,3 +4543,980 @@ LC_HD void lc_ap_resolve(const LcTsNow& now, const LcApEv* ev, uint64_t e0, uint
         LC_WARP_SYNC();
     }
 }
+
+// ================================================================================================ JSON parse
+// ProcessorParseJsonNative (ProcessorParseJsonNative.cpp: ProcessEvent, JsonLogLineParserSimdJson,
+// OptimizedValueToStringBuffer, ProcessNumberValueOptimized).  The rules are pinned in include/lc_b200.h above
+// lc_json_parse.  One thread walks one event: lc_json_walk validates the whole document (strict RFC 8259, root object,
+// depth <= 1024, valid UTF-8, paired surrogates, a NUL byte after the root ends the input) and produces its top-level
+// members.  The count pass and the emit pass run the same walk (EMIT false / true), so their sizes agree.
+//
+// SLOW = false is the fast instantiation: nesting up to LC_JSON_FAST_DEPTH in a 64-bit register, floats of at most
+// 19 significant digits through one exact operation (mantissa <= 2^53, |decimal exponent| <= 22) or else the
+// Eisel-Lemire step over a 128-bit power-of-five table in global memory, "%f" of |x| < 2^64 in 64/128-bit integers.  Anything else returns LC_JSON_W_SLOW and the event goes to the SLOW = true
+// instantiation: nesting up to 1024 on a bit stack in local memory, exact decimal-to-double conversion of any length
+// (800 significant digits and a sticky digit, decided by big-integer comparison with the halfway points), "%f" of
+// integer parts of any size.  Reads stay inside the event; writes go only to the event's entry and arena ranges, and
+// a write past either sets `over` instead.
+#include "lc_json_pow5.h" // the Eisel-Lemire table; the device walks read the engine's copy through LcJsonOut::pow5
+
+#define LC_JSON_NO_KEY 0xFFFFFFFFu
+#define LC_JSON_ST_OK 0u
+#define LC_JSON_ST_NOT_FOUND 1u
+#define LC_JSON_ST_EMPTY 2u
+#define LC_JSON_ST_FAILED 3u
+#define LC_JSON_ST_OVER 0x80u
+#define LC_JSON_ARENA 0x80000000u // tag bit of an offset into the arena (otherwise an offset into base)
+#define LC_JSON_FAST_DEPTH 64u
+#define LC_JSON_MAX_DEPTH 1024u
+#define LC_JSON_MAX_DIGITS 800
+#define LC_JSON_BIG_LIMBS 144 // 4608 bits: both sides of a halfway-point comparison fit (< 3800 bits)
+
+enum : uint32_t { LC_JSON_W_OK = 0, LC_JSON_W_FAIL = 1, LC_JSON_W_SLOW = 2 };
+
+struct LcJsonEntry {
+    uint32_t key_off, key_len, val_off, val_len;
+};
+
+// Where a walk's output goes.  The count pass (EMIT false) only sums nent and narena; the emit pass writes entry k to
+// ent[k] and arena byte j to arena[j] when they are inside [0, ent_cap) / [0, arena_cap), and sets over otherwise.
+template <bool EMIT>
+struct LcJsonOut {
+    const uint64_t* pow5; // lc_json_pow5 (host) or its device copy
+    LcJsonEntry* ent;
+    uint8_t* arena;
+    uint32_t ent_cap, arena_cap;
+    uint32_t base_off;  // the event's offset in base
+    uint32_t arena_off; // the event's first arena byte in the arena
+    uint32_t nent, narena;
+    bool over, skey_hit;
+    LC_HD void put(uint32_t j, uint32_t c) {
+        if constexpr (EMIT) {
+            if (j < arena_cap)
+                arena[j] = (uint8_t)c;
+            else
+                over = true;
+        }
+    }
+    LC_HD void entry(uint32_t ko, uint32_t kl, uint32_t vo, uint32_t vl) {
+        if constexpr (EMIT) {
+            if (nent < ent_cap)
+                ent[nent] = LcJsonEntry{ko, kl, vo, vl};
+            else
+                over = true;
+        }
+        ++nent;
+    }
+    LC_HD void grow(uint32_t k) { // narena stays <= 2^31 (the call refuses totals that reach the tag bit)
+        narena += k;
+        if (narena > LC_JSON_ARENA)
+            narena = LC_JSON_ARENA;
+    }
+};
+
+LC_HD uint64_t lc_js_bits(double x) {
+#if defined(__CUDA_ARCH__)
+    return (uint64_t)__double_as_longlong(x);
+#else
+    uint64_t u;
+    memcpy(&u, &x, 8);
+    return u;
+#endif
+}
+
+LC_HD double lc_js_dbl(uint64_t u) {
+#if defined(__CUDA_ARCH__)
+    return __longlong_as_double((long long)u);
+#else
+    double x;
+    memcpy(&x, &u, 8);
+    return x;
+#endif
+}
+
+LC_HD uint32_t lc_js_ws(const uint8_t* s, uint32_t n, uint32_t p) {
+    while (p < n && (s[p] == ' ' || s[p] == '\t' || s[p] == '\n' || s[p] == '\r'))
+        ++p;
+    return p;
+}
+
+LC_HD bool lc_js_digit(const uint8_t* s, uint32_t n, uint32_t p) { return p < n && s[p] >= '0' && s[p] <= '9'; }
+
+// the 4 hex digits at s[p..p+4) as a value, -1 when they are not 4 hex digits inside the event
+LC_HD int32_t lc_js_hex4(const uint8_t* s, uint32_t n, uint32_t p) {
+    if (p > n || n - p < 4)
+        return -1;
+    int32_t v = 0;
+    for (uint32_t k = 0; k < 4; ++k) {
+        const uint32_t c = s[p + k];
+        uint32_t d;
+        if (c >= '0' && c <= '9')
+            d = c - '0';
+        else if ((c | 0x20u) >= 'a' && (c | 0x20u) <= 'f')
+            d = (c | 0x20u) - 'a' + 10;
+        else
+            return -1;
+        v = v * 16 + (int32_t)d;
+    }
+    return v;
+}
+
+// length of the valid UTF-8 sequence (2..4 bytes) that starts with the byte >= 0x80 at s[p], 0 when it is not valid
+// (overlong forms, surrogates and code points past U+10FFFF are not valid)
+LC_HD uint32_t lc_js_utf8_len(const uint8_t* s, uint32_t n, uint32_t p) {
+    const uint32_t c = s[p];
+    uint32_t k, lo = 0x80, hi = 0xBF;
+    if (c < 0xC2)
+        return 0;
+    if (c < 0xE0) {
+        k = 2;
+    } else if (c < 0xF0) {
+        k = 3;
+        if (c == 0xE0)
+            lo = 0xA0;
+        if (c == 0xED)
+            hi = 0x9F;
+    } else if (c < 0xF5) {
+        k = 4;
+        if (c == 0xF0)
+            lo = 0x90;
+        if (c == 0xF4)
+            hi = 0x8F;
+    } else {
+        return 0;
+    }
+    if (n - p < k)
+        return 0;
+    if (s[p + 1] < lo || s[p + 1] > hi)
+        return 0;
+    for (uint32_t j = 2; j < k; ++j)
+        if ((s[p + j] & 0xC0u) != 0x80u)
+            return 0;
+    return k;
+}
+
+struct LcJsPutNone {
+    LC_HD void operator()(uint32_t, uint32_t) {}
+};
+
+// compares the unescaped bytes with SourceKey
+struct LcJsPutCmp {
+    const uint8_t* k;
+    uint32_t kl;
+    bool eq;
+    LC_HD void operator()(uint32_t j, uint32_t c) { eq = eq && j < kl && k[j] == c; }
+};
+
+// writes the unescaped bytes to the arena at `at`
+template <bool EMIT>
+struct LcJsPutArena {
+    LcJsonOut<EMIT>* o;
+    uint32_t at;
+    LC_HD void operator()(uint32_t j, uint32_t c) { o->put(at + j, c); }
+};
+
+// The string whose opening quote is s[p - 1]: returns the position after its closing quote, 0 when it is not valid.
+// *ulen is its unescaped length, *esc whether it has an escape; put(j, byte) receives unescaped byte j.
+template <class Put>
+LC_HD uint32_t lc_js_str(const uint8_t* s, uint32_t n, uint32_t p, uint32_t* ulen, bool* esc, Put& put) {
+    uint32_t u = 0;
+    bool e = false;
+    while (p < n) {
+        const uint32_t c = s[p];
+        if (c == '"') {
+            *ulen = u;
+            *esc = e;
+            return p + 1;
+        }
+        if (c < 0x20)
+            return 0;
+        if (c == '\\') {
+            e = true;
+            if (p + 1 >= n)
+                return 0;
+            uint32_t o;
+            switch (s[p + 1]) {
+            case '"': o = '"'; break;
+            case '\\': o = '\\'; break;
+            case '/': o = '/'; break;
+            case 'b': o = 8; break;
+            case 'f': o = 12; break;
+            case 'n': o = 10; break;
+            case 'r': o = 13; break;
+            case 't': o = 9; break;
+            case 'u': {
+                int32_t cp = lc_js_hex4(s, n, p + 2);
+                if (cp < 0 || (cp >= 0xDC00 && cp <= 0xDFFF))
+                    return 0;
+                p += 6;
+                if (cp >= 0xD800 && cp <= 0xDBFF) {
+                    if (p + 1 >= n || s[p] != '\\' || s[p + 1] != 'u')
+                        return 0;
+                    const int32_t lo = lc_js_hex4(s, n, p + 2);
+                    if (lo < 0xDC00 || lo > 0xDFFF)
+                        return 0;
+                    p += 6;
+                    cp = 0x10000 + ((cp - 0xD800) << 10) + (lo - 0xDC00);
+                }
+                const uint32_t v = (uint32_t)cp;
+                if (v < 0x80) {
+                    put(u++, v);
+                } else if (v < 0x800) {
+                    put(u++, 0xC0 | (v >> 6));
+                    put(u++, 0x80 | (v & 0x3F));
+                } else if (v < 0x10000) {
+                    put(u++, 0xE0 | (v >> 12));
+                    put(u++, 0x80 | ((v >> 6) & 0x3F));
+                    put(u++, 0x80 | (v & 0x3F));
+                } else {
+                    put(u++, 0xF0 | (v >> 18));
+                    put(u++, 0x80 | ((v >> 12) & 0x3F));
+                    put(u++, 0x80 | ((v >> 6) & 0x3F));
+                    put(u++, 0x80 | (v & 0x3F));
+                }
+                continue;
+            }
+            default:
+                return 0;
+            }
+            put(u++, o);
+            p += 2;
+            continue;
+        }
+        if (c < 0x80) {
+            put(u++, c);
+            ++p;
+            continue;
+        }
+        const uint32_t k = lc_js_utf8_len(s, n, p);
+        if (!k)
+            return 0;
+        for (uint32_t j = 0; j < k; ++j)
+            put(u++, s[p + j]);
+        p += k;
+    }
+    return 0;
+}
+
+// The number at s[p] ('-' or a digit): returns the position after it, 0 when it does not follow the JSON grammar.
+// *isint: no fraction and no exponent.
+LC_HD uint32_t lc_js_num(const uint8_t* s, uint32_t n, uint32_t p, bool* isint) {
+    if (s[p] == '-')
+        ++p;
+    if (!lc_js_digit(s, n, p))
+        return 0;
+    if (s[p] == '0')
+        ++p;
+    else
+        while (lc_js_digit(s, n, p))
+            ++p;
+    bool in = true;
+    if (p < n && s[p] == '.') {
+        const uint32_t q = ++p;
+        while (lc_js_digit(s, n, p))
+            ++p;
+        if (p == q)
+            return 0;
+        in = false;
+    }
+    if (p < n && (s[p] | 0x20u) == 'e') {
+        ++p;
+        if (p < n && (s[p] == '+' || s[p] == '-'))
+            ++p;
+        const uint32_t q = p;
+        while (lc_js_digit(s, n, p))
+            ++p;
+        if (p == q)
+            return 0;
+        in = false;
+    }
+    *isint = in;
+    return p;
+}
+
+// true when the nd digits at s[p] are <= the nd digits of lim (same length)
+LC_HD bool lc_js_digits_le(const uint8_t* s, uint32_t p, const char* lim, uint32_t nd) {
+    for (uint32_t k = 0; k < nd; ++k)
+        if (s[p + k] != (uint8_t)lim[k])
+            return s[p + k] < (uint8_t)lim[k];
+    return true;
+}
+
+LC_HD void lc_js_mul128(uint64_t a, uint64_t b, uint64_t* hi, uint64_t* lo) {
+#if defined(__CUDA_ARCH__)
+    *hi = __umul64hi(a, b);
+    *lo = a * b;
+#else
+    const unsigned __int128 p = (unsigned __int128)a * b;
+    *hi = (uint64_t)(p >> 64);
+    *lo = (uint64_t)p;
+#endif
+}
+
+LC_HD uint32_t lc_js_clz64(uint64_t x) { // x != 0
+#if defined(__CUDA_ARCH__)
+    return (uint32_t)__clzll((long long)x);
+#else
+    return (uint32_t)__builtin_clzll(x);
+#endif
+}
+
+// The Eisel-Lemire step (Lemire, "Number Parsing at a Gigabyte per Second", 2021): the correctly rounded double of
+// w * 10^q (w != 0, exact) from one or two 64 x 128-bit products with the table of lc_json_pow5.h.  false when it
+// cannot decide (q outside the table, a subnormal result, or a product whose dropped bits might carry), which sends
+// the event to the slow walk.
+LC_HD bool lc_js_eisel_lemire(uint64_t w, int32_t q, bool neg, const uint64_t* pow5, double* out) {
+    if (q < LC_JSON_POW5_QMIN || q > LC_JSON_POW5_QMAX)
+        return false;
+    const uint64_t* t = pow5 + 2 * (q - LC_JSON_POW5_QMIN);
+    const uint32_t lz = lc_js_clz64(w);
+    w <<= lz;
+    uint64_t hi, lo;
+    lc_js_mul128(w, t[0], &hi, &lo);
+    if ((hi & 0x1FFull) == 0x1FFull) { // the 9 bits below the 55 kept ones may carry: add the second product
+        uint64_t hi2, lo2;
+        lc_js_mul128(w, t[1], &hi2, &lo2);
+        lo += hi2;
+        if (hi2 > lo)
+            ++hi;
+    }
+    if (lo == 0xFFFFFFFFFFFFFFFFull && (q < -27 || q > 55))
+        return false;
+    const uint32_t upper = (uint32_t)(hi >> 63);
+    uint64_t m = hi >> (upper + 9);
+    int32_t p2 = (((152170 + 65536) * q) >> 16) + 63 + (int32_t)upper - (int32_t)lz + 1023;
+    if (p2 <= 0)
+        return false; // subnormal
+    if (lo <= 1 && q >= -4 && q <= 23 && (m & 3) == 1 && (m << (upper + 9)) == hi)
+        m &= ~1ull; // an exact halfway case: round to even (down)
+    m += m & 1;
+    m >>= 1;
+    if (m >= (2ull << 52)) {
+        m = 1ull << 52;
+        ++p2;
+    }
+    if (p2 >= 0x7FF)
+        return false; // overflow: the slow walk renders it
+    *out = lc_js_dbl(((uint64_t)p2 << 52) | (m & ~(1ull << 52)) | (neg ? 0x8000000000000000ull : 0ull));
+    return true;
+}
+
+// The double of the number [a, b) when the fast instantiation can decide it: at most 19 significant digits, then
+// one correctly rounded multiplication or division by an exact power of ten (mantissa <= 2^53, decimal exponent in
+// [-22, 22]) or the Eisel-Lemire step.
+LC_HD bool lc_js_dec_fast(const uint8_t* s, uint32_t a, uint32_t b, const uint64_t* pow5, double* out) {
+    const bool neg = s[a] == '-';
+    uint32_t p = a + (neg ? 1u : 0u), nsig = 0;
+    uint64_t w = 0;
+    int32_t e10 = 0;
+    bool frac = false;
+    for (; p < b; ++p) {
+        const uint32_t c = s[p];
+        if (c == '.') {
+            frac = true;
+            continue;
+        }
+        if (c < '0' || c > '9')
+            break;
+        if (nsig || c != '0') {
+            if (nsig == 19)
+                return false;
+            w = w * 10 + (c - '0');
+            ++nsig;
+        }
+        if (frac)
+            --e10;
+    }
+    if (p < b) { // exponent
+        ++p;
+        bool eneg = false;
+        if (s[p] == '+' || s[p] == '-')
+            eneg = s[p++] == '-';
+        int32_t ev = 0;
+        for (; p < b; ++p)
+            if (ev < 100000)
+                ev = ev * 10 + (int32_t)(s[p] - '0');
+        e10 += eneg ? -ev : ev;
+    }
+    if (w == 0) {
+        *out = neg ? -0.0 : 0.0;
+        return true;
+    }
+    if (w > (1ull << 53) || e10 < -22 || e10 > 22)
+        return lc_js_eisel_lemire(w, e10, neg, pow5, out);
+    double pw = 1.0;
+    for (int32_t k = e10 < 0 ? -e10 : e10; k > 0; --k)
+        pw *= 10.0; // exact up to 1e22
+    double x = (double)w;
+    if (e10 >= 0) {
+        x *= pw;
+    } else {
+#if defined(__CUDA_ARCH__)
+        // x / pw without the division routine's call: the correctly rounded reciprocal, a quotient within one ulp
+        // and one residual step give the correctly rounded quotient (Markstein); x and pw are far from the
+        // subnormal and overflow ranges here
+        const double r = __drcp_rn(pw), q = x * r;
+        x = __fma_rn(__fma_rn(-q, pw, x), r, q);
+#else
+        x /= pw;
+#endif
+    }
+    *out = neg ? -x : x;
+    return true;
+}
+
+// ---- big integers of the slow path (little-endian 32-bit limbs)
+struct LcJsBig {
+    uint32_t n;
+    uint32_t w[LC_JSON_BIG_LIMBS];
+};
+
+LC_HD void lc_big_set(LcJsBig& x, uint64_t v) {
+    x.n = 0;
+    while (v) {
+        x.w[x.n++] = (uint32_t)v;
+        v >>= 32;
+    }
+}
+
+LC_HD void lc_big_muladd(LcJsBig& x, uint32_t m, uint32_t add) {
+    uint64_t carry = add;
+    for (uint32_t k = 0; k < x.n; ++k) {
+        const uint64_t t = (uint64_t)x.w[k] * m + carry;
+        x.w[k] = (uint32_t)t;
+        carry = t >> 32;
+    }
+    if (carry && x.n < LC_JSON_BIG_LIMBS)
+        x.w[x.n++] = (uint32_t)carry;
+}
+
+LC_HD void lc_big_mulpow10(LcJsBig& x, uint32_t e) {
+    for (; e >= 9; e -= 9)
+        lc_big_muladd(x, 1000000000u, 0);
+    uint32_t m = 1;
+    for (; e; --e)
+        m *= 10;
+    if (m > 1)
+        lc_big_muladd(x, m, 0);
+}
+
+LC_HD void lc_big_shl(LcJsBig& x, uint32_t bits) {
+    if (!x.n)
+        return;
+    const uint32_t lw = bits >> 5, b = bits & 31;
+    uint32_t nn = x.n + lw + 1;
+    if (nn > LC_JSON_BIG_LIMBS)
+        nn = LC_JSON_BIG_LIMBS;
+    for (uint32_t k = nn; k-- > 0;) {
+        const uint32_t hi = k >= lw && k - lw < x.n ? x.w[k - lw] : 0u;
+        const uint32_t lo = b && k >= lw + 1 && k - lw - 1 < x.n ? x.w[k - lw - 1] : 0u;
+        x.w[k] = b ? (hi << b) | (lo >> (32 - b)) : hi;
+    }
+    x.n = nn;
+    while (x.n && !x.w[x.n - 1])
+        --x.n;
+}
+
+LC_HD int lc_big_cmp(const LcJsBig& x, const LcJsBig& y) {
+    if (x.n != y.n)
+        return x.n < y.n ? -1 : 1;
+    for (uint32_t k = x.n; k-- > 0;)
+        if (x.w[k] != y.w[k])
+            return x.w[k] < y.w[k] ? -1 : 1;
+    return 0;
+}
+
+// x = divided by 10^9, returns the remainder
+LC_HD uint32_t lc_big_div1e9(LcJsBig& x) {
+    uint64_t r = 0;
+    for (uint32_t k = x.n; k-- > 0;) {
+        const uint64_t t = (r << 32) | x.w[k];
+        x.w[k] = (uint32_t)(t / 1000000000u);
+        r = t % 1000000000u;
+    }
+    while (x.n && !x.w[x.n - 1])
+        --x.n;
+    return (uint32_t)r;
+}
+
+// sign of D * 10^E - M * 2^t
+LC_HD int lc_js_cmp_mid(const LcJsBig& D, int32_t E, uint64_t M, int32_t t, LcJsBig& L, LcJsBig& R) {
+    L = D;
+    lc_big_set(R, M);
+    if (E >= 0)
+        lc_big_mulpow10(L, (uint32_t)E);
+    else
+        lc_big_mulpow10(R, (uint32_t)-E);
+    if (t >= 0)
+        lc_big_shl(R, (uint32_t)t);
+    else
+        lc_big_shl(L, (uint32_t)-t);
+    return lc_big_cmp(L, R);
+}
+
+// The correctly rounded double (round half to even) of the number [a, b), any number of digits: the first 800
+// significant digits and a sticky digit for the rest, a first estimate from 19 digits, then steps to the neighbour
+// while the value lies past a halfway point.  Overflow gives infinity, underflow a signed zero.
+LC_HD double lc_js_dec_slow(const uint8_t* s, uint32_t a, uint32_t b) {
+    LcJsBig D, L, R;
+    const bool neg = s[a] == '-';
+    uint32_t p = a + (neg ? 1u : 0u), nd = 0, k19 = 0;
+    uint64_t w19 = 0;
+    int64_t E = 0;
+    bool frac = false, sticky = false;
+    lc_big_set(D, 0);
+    uint32_t chunk = 0, clen = 0;
+    for (; p < b; ++p) {
+        const uint32_t c = s[p];
+        if (c == '.') {
+            frac = true;
+            continue;
+        }
+        if (c < '0' || c > '9')
+            break;
+        const uint32_t d = c - '0';
+        if (nd == 0 && d == 0) {
+            if (frac)
+                --E;
+        } else if (nd < LC_JSON_MAX_DIGITS) {
+            chunk = chunk * 10 + d;
+            if (++clen == 9) {
+                lc_big_muladd(D, 1000000000u, chunk);
+                chunk = clen = 0;
+            }
+            if (k19 < 19) {
+                w19 = w19 * 10 + d;
+                ++k19;
+            }
+            ++nd;
+            if (frac)
+                --E;
+        } else {
+            sticky = sticky || d != 0;
+            if (!frac)
+                ++E;
+        }
+    }
+    if (sticky) {
+        chunk = chunk * 10 + 1;
+        ++clen;
+        ++nd;
+        --E;
+    }
+    if (clen) {
+        uint32_t m = 1;
+        for (uint32_t j = 0; j < clen; ++j)
+            m *= 10;
+        lc_big_muladd(D, m, chunk);
+    }
+    if (p < b) {
+        ++p;
+        bool eneg = false;
+        if (s[p] == '+' || s[p] == '-')
+            eneg = s[p++] == '-';
+        int64_t ev = 0;
+        for (; p < b; ++p)
+            if (ev < 100000000)
+                ev = ev * 10 + (s[p] - '0');
+        E += eneg ? -ev : ev;
+    }
+    const double zero = neg ? -0.0 : 0.0;
+    if (nd == 0)
+        return zero;
+    const int64_t dexp = (int64_t)nd + E; // the value lies in [10^(dexp-1), 10^dexp)
+    if (dexp > 310)
+        return neg ? -lc_js_dbl(0x7FF0000000000000ull) : lc_js_dbl(0x7FF0000000000000ull);
+    if (dexp < -323)
+        return zero;
+    // estimate: the first 19 digits times a power of ten, a few ulps off
+    double x = (double)w19;
+    for (int64_t e = E + (int64_t)nd - k19; e != 0;) {
+        const int64_t st = e > 22 ? 22 : e < -22 ? -22 : e;
+        double pw = 1.0;
+        for (int64_t j = st < 0 ? -st : st; j > 0; --j)
+            pw *= 10.0;
+        x = st < 0 ? x / pw : x * pw;
+        e -= st;
+    }
+    uint64_t u = lc_js_bits(x) & 0x7FFFFFFFFFFFFFFFull;
+    if (u >= 0x7FF0000000000000ull)
+        u = 0x7FEFFFFFFFFFFFFFull;
+    const int32_t Ei = (int32_t)E;
+    for (int it = 0; it < 4096; ++it) {
+        const uint32_t be = (uint32_t)(u >> 52);
+        const uint64_t m = be ? (u & 0xFFFFFFFFFFFFFull) | (1ull << 52) : u;
+        const int32_t q = be ? (int32_t)be - 1075 : -1074;
+        // the halfway point above: (2m + 1) * 2^(q - 1)
+        int c = lc_js_cmp_mid(D, Ei, 2 * m + 1, q - 1, L, R);
+        if (c > 0 || (c == 0 && (m & 1))) {
+            if (u == 0x7FEFFFFFFFFFFFFFull) {
+                u = 0x7FF0000000000000ull;
+                break;
+            }
+            ++u;
+            continue;
+        }
+        if (u == 0)
+            break;
+        // the halfway point below; the gap below a power of two is half as wide (except at the smallest normal)
+        c = (m == (1ull << 52) && be > 1) ? lc_js_cmp_mid(D, Ei, 4 * m - 1, q - 2, L, R)
+                                          : lc_js_cmp_mid(D, Ei, 2 * m - 1, q - 1, L, R);
+        if (c < 0 || (c == 0 && (m & 1))) {
+            --u;
+            continue;
+        }
+        break;
+    }
+    return lc_js_dbl(u | (neg ? 0x8000000000000000ull : 0ull));
+}
+
+// Appends "%f" of the finite x to the arena at `at` (EMIT) and returns its length; LC_JSON_W_SLOW in *slow when the
+// fast instantiation cannot print it (|x| >= 2^64).
+template <bool SLOW, bool EMIT>
+LC_HD uint32_t lc_js_printf(double x, LcJsonOut<EMIT>& o, uint32_t at, bool* slow) {
+    const uint64_t bits = lc_js_bits(x);
+    const bool neg = bits >> 63;
+    const uint64_t u = bits & 0x7FFFFFFFFFFFFFFFull;
+    const uint32_t be = (uint32_t)(u >> 52);
+    uint32_t len = 0;
+    if (neg)
+        o.put(at + len++, '-');
+    if (be >= 1023 + 64) { // |x| >= 2^64: an integer m << q with q >= 12
+        if constexpr (!SLOW) {
+            *slow = true;
+            return 0;
+        } else {
+            LcJsBig B;
+            lc_big_set(B, (u & 0xFFFFFFFFFFFFFull) | (1ull << 52));
+            lc_big_shl(B, be - 1075);
+            uint32_t ch[40], nc = 0;
+            while (B.n && nc < 40)
+                ch[nc++] = lc_big_div1e9(B);
+            uint32_t nd = 1;
+            for (uint32_t t = ch[nc - 1]; t >= 10; t /= 10)
+                ++nd;
+            for (uint32_t j = nd, t = ch[nc - 1]; j-- > 0; t /= 10)
+                o.put(at + len + j, '0' + t % 10);
+            len += nd;
+            for (uint32_t c = nc - 1; c-- > 0;) {
+                for (uint32_t j = 9, t = ch[c]; j-- > 0; t /= 10)
+                    o.put(at + len + j, '0' + t % 10);
+                len += 9;
+            }
+            for (uint32_t j = 0; j < 7; ++j)
+                o.put(at + len++, j ? '0' : '.');
+            return len;
+        }
+    }
+    uint64_t ip = 0;
+    uint32_t f6 = 0;
+    if (u) {
+        const uint64_t m = be ? (u & 0xFFFFFFFFFFFFFull) | (1ull << 52) : u;
+        const int32_t q = be ? (int32_t)be - 1075 : -1074;
+        if (q >= 0) {
+            ip = m << q;
+        } else {
+            const uint32_t k = (uint32_t)-q;
+            const uint64_t fr = k >= 64 ? m : m & ((1ull << k) - 1);
+            ip = k >= 64 ? 0 : m >> k;
+            if (k < 75) { // fr * 10^6 < 2^73: below 2^(k-1) from k = 75 on, so it rounds to 0
+                const unsigned __int128 P = (unsigned __int128)fr * 1000000u;
+                const unsigned __int128 half = (unsigned __int128)1 << (k - 1);
+                f6 = (uint32_t)(P >> k);
+                const unsigned __int128 rem = P & ((half << 1) - 1);
+                if (rem > half || (rem == half && (f6 & 1)))
+                    ++f6;
+                if (f6 == 1000000) {
+                    f6 = 0;
+                    ++ip;
+                }
+            }
+        }
+    }
+    uint32_t nd = 1;
+    for (uint64_t t = ip; t >= 10; t /= 10)
+        ++nd;
+    uint64_t t = ip;
+    for (uint32_t j = nd; j-- > 0; t /= 10)
+        o.put(at + len + j, '0' + (uint32_t)(t % 10));
+    len += nd;
+    o.put(at + len++, '.');
+    uint32_t f = f6;
+    for (uint32_t j = 6; j-- > 0; f /= 10)
+        o.put(at + len + j, '0' + f % 10);
+    return len + 6;
+}
+
+// The bracket types of the open containers: bit k set for an object at depth k + 1 (the root object is bit 0).  The
+// fast instantiation keeps LC_JSON_FAST_DEPTH bits in a register, the slow one LC_JSON_MAX_DEPTH in local memory.
+template <bool SLOW>
+struct LcJsStack {
+    uint64_t b = 1;
+    LC_HD void set(uint32_t k, bool obj) { b = (b & ~(1ull << k)) | ((uint64_t)obj << k); }
+    LC_HD bool get(uint32_t k) const { return (b >> k) & 1u; }
+};
+template <>
+struct LcJsStack<true> {
+    uint32_t w[LC_JSON_MAX_DEPTH / 32] = {1};
+    LC_HD void set(uint32_t k, bool obj) { w[k >> 5] = (w[k >> 5] & ~(1u << (k & 31))) | ((uint32_t)obj << (k & 31)); }
+    LC_HD bool get(uint32_t k) const { return (w[k >> 5] >> (k & 31)) & 1u; }
+};
+
+// Skips the nested object or array whose opening bracket is s[p] (a member value of the root object, depth 2):
+// *end receives the position after its closing bracket.  Bit d - 1 of the stack is set for an object at depth d.
+template <bool SLOW>
+LC_HD uint32_t lc_js_skip(const uint8_t* s, uint32_t n, uint32_t p, uint32_t* end) {
+    constexpr uint32_t kMax = SLOW ? LC_JSON_MAX_DEPTH : LC_JSON_FAST_DEPTH;
+    LcJsStack<SLOW> stk;
+    uint32_t d = 1;
+    bool need = true;
+    LcJsPutNone none;
+    for (;;) {
+        if (need) {
+            p = lc_js_ws(s, n, p);
+            if (p >= n)
+                return LC_JSON_W_FAIL;
+            const uint32_t c = s[p];
+            uint32_t ul;
+            bool esc, isint;
+            if (c == '{' || c == '[') {
+                if (d == kMax)
+                    return SLOW ? LC_JSON_W_FAIL : LC_JSON_W_SLOW;
+                const bool obj = c == '{';
+                stk.set(d, obj);
+                ++d;
+                p = lc_js_ws(s, n, p + 1);
+                if (p >= n)
+                    return LC_JSON_W_FAIL;
+                if (s[p] == (obj ? '}' : ']')) {
+                    ++p;
+                    --d;
+                    need = false;
+                    continue;
+                }
+                if (obj) {
+                    if (s[p] != '"' || !(p = lc_js_str(s, n, p + 1, &ul, &esc, none)))
+                        return LC_JSON_W_FAIL;
+                    p = lc_js_ws(s, n, p);
+                    if (p >= n || s[p] != ':')
+                        return LC_JSON_W_FAIL;
+                    ++p;
+                }
+                continue;
+            }
+            if (c == '"') {
+                if (!(p = lc_js_str(s, n, p + 1, &ul, &esc, none)))
+                    return LC_JSON_W_FAIL;
+            } else if (c == 't') {
+                if (n - p < 4 || s[p + 1] != 'r' || s[p + 2] != 'u' || s[p + 3] != 'e')
+                    return LC_JSON_W_FAIL;
+                p += 4;
+            } else if (c == 'f') {
+                if (n - p < 5 || s[p + 1] != 'a' || s[p + 2] != 'l' || s[p + 3] != 's' || s[p + 4] != 'e')
+                    return LC_JSON_W_FAIL;
+                p += 5;
+            } else if (c == 'n') {
+                if (n - p < 4 || s[p + 1] != 'u' || s[p + 2] != 'l' || s[p + 3] != 'l')
+                    return LC_JSON_W_FAIL;
+                p += 4;
+            } else if (c == '-' || (c >= '0' && c <= '9')) {
+                if (!(p = lc_js_num(s, n, p, &isint)))
+                    return LC_JSON_W_FAIL;
+            } else {
+                return LC_JSON_W_FAIL;
+            }
+        }
+        // after a value inside the container at depth d
+        if (d == 1) {
+            *end = p;
+            return LC_JSON_W_OK;
+        }
+        need = true;
+        p = lc_js_ws(s, n, p);
+        if (p >= n)
+            return LC_JSON_W_FAIL;
+        const bool obj = stk.get(d - 1);
+        if (s[p] == ',') {
+            ++p;
+            if (obj) {
+                uint32_t ul;
+                bool esc;
+                p = lc_js_ws(s, n, p);
+                if (p >= n || s[p] != '"' || !(p = lc_js_str(s, n, p + 1, &ul, &esc, none)))
+                    return LC_JSON_W_FAIL;
+                p = lc_js_ws(s, n, p);
+                if (p >= n || s[p] != ':')
+                    return LC_JSON_W_FAIL;
+                ++p;
+            }
+            continue;
+        }
+        if (s[p] == (obj ? '}' : ']')) {
+            ++p;
+            --d;
+            need = false;
+            continue;
+        }
+        return LC_JSON_W_FAIL;
+    }
+}
+
+// The walk over one event's value s[0, n) (n > 0): LC_JSON_W_OK with o.nent members and o.narena arena bytes,
+// LC_JSON_W_FAIL, or LC_JSON_W_SLOW (fast instantiation only: the event needs the slow one).
+template <bool SLOW, bool EMIT>
+LC_HD uint32_t lc_json_walk(const uint8_t* s, uint32_t n, const uint8_t* skey, uint32_t sklen, LcJsonOut<EMIT>& o) {
+    LcJsPutNone none;
+    uint32_t p = lc_js_ws(s, n, 0);
+    if (p >= n || s[p] != '{')
+        return LC_JSON_W_FAIL;
+    p = lc_js_ws(s, n, p + 1);
+    if (p < n && s[p] == '}') {
+        ++p;
+    } else {
+        for (;;) {
+            if (p >= n || s[p] != '"')
+                return LC_JSON_W_FAIL;
+            // the key
+            const uint32_t k0 = p + 1;
+            uint32_t kl, vl = 0, vo;
+            bool kesc, vesc, isint;
+            LcJsPutCmp cmp{skey, sklen, true};
+            if (!(p = lc_js_str(s, n, k0, &kl, &kesc, cmp)))
+                return LC_JSON_W_FAIL;
+            if (cmp.eq && kl == sklen)
+                o.skey_hit = true;
+            uint32_t ko = o.base_off + k0;
+            if (kesc) {
+                ko = LC_JSON_ARENA | (o.arena_off + o.narena);
+                if constexpr (EMIT) {
+                    LcJsPutArena<EMIT> put{&o, o.narena};
+                    lc_js_str(s, n, k0, &kl, &kesc, put);
+                }
+                o.grow(kl);
+            }
+            p = lc_js_ws(s, n, p);
+            if (p >= n || s[p] != ':')
+                return LC_JSON_W_FAIL;
+            p = lc_js_ws(s, n, p + 1);
+            if (p >= n)
+                return LC_JSON_W_FAIL;
+            // the value
+            const uint32_t c = s[p], v0 = p;
+            vo = o.base_off + v0;
+            if (c == '"') {
+                if (!(p = lc_js_str(s, n, v0 + 1, &vl, &vesc, none)))
+                    return LC_JSON_W_FAIL;
+                vo = o.base_off + v0 + 1;
+                if (vesc) {
+                    vo = LC_JSON_ARENA | (o.arena_off + o.narena);
+                    if constexpr (EMIT) {
+                        LcJsPutArena<EMIT> put{&o, o.narena};
+                        lc_js_str(s, n, v0 + 1, &vl, &vesc, put);
+                    }
+                    o.grow(vl);
+                }
+            } else if (c == '{' || c == '[') {
+                const uint32_t r = lc_js_skip<SLOW>(s, n, p, &p);
+                if (r != LC_JSON_W_OK)
+                    return r;
+                vl = p - v0;
+            } else if (c == 't') {
+                if (n - p < 4 || s[p + 1] != 'r' || s[p + 2] != 'u' || s[p + 3] != 'e')
+                    return LC_JSON_W_FAIL;
+                p += 4;
+                vl = 4;
+            } else if (c == 'f') {
+                if (n - p < 5 || s[p + 1] != 'a' || s[p + 2] != 'l' || s[p + 3] != 's' || s[p + 4] != 'e')
+                    return LC_JSON_W_FAIL;
+                p += 5;
+                vl = 5;
+            } else if (c == 'n') {
+                if (n - p < 4 || s[p + 1] != 'u' || s[p + 2] != 'l' || s[p + 3] != 'l')
+                    return LC_JSON_W_FAIL;
+                p += 4;
+            } else if (c == '-' || (c >= '0' && c <= '9')) {
+                if (!(p = lc_js_num(s, n, p, &isint)))
+                    return LC_JSON_W_FAIL;
+                if (isint) {
+                    // "%" PRId64 / "%" PRIu64 of an integer in range is its own text, but for "-0"; else empty
+                    const bool neg = c == '-';
+                    const uint32_t d0 = v0 + (neg ? 1u : 0u), nd = p - d0;
+                    if (neg ? (nd < 19 || (nd == 19 && lc_js_digits_le(s, d0, "9223372036854775808", 19)))
+                            : (nd < 20 || (nd == 20 && lc_js_digits_le(s, d0, "18446744073709551615", 20)))) {
+                        if (neg && nd == 1 && s[d0] == '0') {
+                            vo = o.base_off + d0;
+                            vl = 1;
+                        } else {
+                            vl = p - v0;
+                        }
+                    }
+                } else {
+                    double x;
+                    if (!lc_js_dec_fast(s, v0, p, o.pow5, &x)) {
+                        if constexpr (!SLOW)
+                            return LC_JSON_W_SLOW;
+                        else
+                            x = lc_js_dec_slow(s, v0, p);
+                    }
+                    if ((lc_js_bits(x) & 0x7FFFFFFFFFFFFFFFull) < 0x7FF0000000000000ull) { // infinity renders empty
+                        bool slow = false;
+                        vl = lc_js_printf<SLOW, EMIT>(x, o, o.narena, &slow);
+                        if (slow)
+                            return LC_JSON_W_SLOW;
+                        vo = LC_JSON_ARENA | (o.arena_off + o.narena);
+                        o.grow(vl);
+                    }
+                }
+            } else {
+                return LC_JSON_W_FAIL;
+            }
+            o.entry(ko, kl, vo, vl);
+            p = lc_js_ws(s, n, p);
+            if (p < n && s[p] == ',') {
+                p = lc_js_ws(s, n, p + 1);
+                continue;
+            }
+            if (p < n && s[p] == '}') {
+                ++p;
+                break;
+            }
+            return LC_JSON_W_FAIL;
+        }
+    }
+    p = lc_js_ws(s, n, p);
+    return p < n && s[p] != 0 ? LC_JSON_W_FAIL : LC_JSON_W_OK;
+}
+
+// One event of the count pass: its status, entry count and arena bytes; *slow when the fast instantiation gave up.
+// len == LC_JSON_NO_KEY: no SourceKey; an empty value is LC_JSON_ST_EMPTY.  The caller has checked the range.
+template <bool SLOW>
+LC_HD uint32_t lc_json_count(const uint8_t* base, uint32_t off, uint32_t len, const uint8_t* skey, uint32_t sklen,
+                             const uint64_t* pow5, uint32_t* nent, uint32_t* narena, bool* slow) {
+    *nent = *narena = 0;
+    *slow = false;
+    if (len == LC_JSON_NO_KEY)
+        return LC_JSON_ST_NOT_FOUND;
+    if (len == 0)
+        return LC_JSON_ST_EMPTY;
+    LcJsonOut<false> o{pow5, nullptr, nullptr, 0, 0, off, 0, 0, 0, false, false};
+    const uint32_t r = lc_json_walk<SLOW, false>(base + off, len, skey, sklen, o);
+    if (r == LC_JSON_W_SLOW) {
+        *slow = true;
+        return LC_JSON_ST_FAILED;
+    }
+    if (r != LC_JSON_W_OK)
+        return LC_JSON_ST_FAILED;
+    *nent = o.nent;
+    *narena = o.narena;
+    return LC_JSON_ST_OK | (o.skey_hit ? LC_JSON_ST_OVER : 0u);
+}
+
+// One event of the emit pass into its ranges ent[0, ent_cap) and arena[0, arena_cap) (arena_off: the range's start in
+// the arena); false when the walk does not fill them exactly (nothing is written past them).
+template <bool SLOW>
+LC_HD bool lc_json_emit(const uint8_t* base, uint32_t off, uint32_t len, const uint8_t* skey, uint32_t sklen,
+                        const uint64_t* pow5, LcJsonEntry* ent, uint32_t ent_cap, uint8_t* arena, uint32_t arena_off, uint32_t arena_cap) {
+    LcJsonOut<true> o{pow5, ent, arena, ent_cap, arena_cap, off, arena_off, 0, 0, false, false};
+    const uint32_t r = lc_json_walk<SLOW, true>(base + off, len, skey, sklen, o);
+    return r == LC_JSON_W_OK && !o.over && o.nent == ent_cap && o.narena == arena_cap;
+}

@@ -4568,4 +4568,146 @@ void launch_ap_emit(const uint8_t* d_base, const uint32_t* d_off, const uint32_t
                                                                      d_entries);
 }
 
+// ================================================================================================ JSON parse
+// counters[3] of the JSON count passes from one warp: every lane calls it
+__device__ __forceinline__ void json_add_counters(uint32_t st, bool valid, unsigned long long* counters) {
+    const uint32_t s = st & 0x7Fu;
+    const uint32_t c0 = __reduce_add_sync(0xFFFFFFFFu, valid && s == LC_JSON_ST_NOT_FOUND ? 1u : 0u);
+    const uint32_t c1 = __reduce_add_sync(0xFFFFFFFFu, valid && s == LC_JSON_ST_FAILED ? 1u : 0u);
+    const uint32_t c2 = __reduce_add_sync(0xFFFFFFFFu, valid && s == LC_JSON_ST_OK ? 1u : 0u);
+    if ((threadIdx.x & 31) == 0) {
+        if (c0)
+            atomicAdd(&counters[0], (unsigned long long)c0);
+        if (c1)
+            atomicAdd(&counters[1], (unsigned long long)c1);
+        if (c2)
+            atomicAdd(&counters[2], (unsigned long long)c2);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    json_count_kernel(const uint8_t* __restrict__ base, uint64_t base_len, const uint32_t* __restrict__ off,
+                      const uint32_t* __restrict__ len, uint64_t n, const uint8_t* __restrict__ skey, uint32_t sklen, const uint64_t* __restrict__ pow5,
+                      uint8_t* __restrict__ status, uint32_t* __restrict__ nent, uint32_t* __restrict__ narena,
+                      uint8_t* __restrict__ slow, uint32_t* __restrict__ slow_list, uint32_t* nslow, uint32_t* bad,
+                      unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool valid = i < n;
+    uint32_t st = LC_JSON_ST_FAILED, ne = 0, na = 0;
+    bool sl = false;
+    if (valid) {
+        const uint32_t l = len[i], o = l == LC_JSON_NO_KEY ? 0u : off[i];
+        if (l != LC_JSON_NO_KEY && (uint64_t)o + l > base_len)
+            atomicOr(bad, 1u);
+        else
+            st = lc_json_count<false>(base, o, l, skey, sklen, pow5, &ne, &na, &sl);
+        if (sl)
+            slow_list[atomicAdd(nslow, 1u)] = (uint32_t)i;
+        status[i] = (uint8_t)st;
+        nent[i] = ne;
+        narena[i] = na;
+        slow[i] = sl ? 1 : 0;
+    }
+    json_add_counters(st, valid && !sl, counters);
+}
+
+__global__ void __launch_bounds__(128)
+    json_count_slow_kernel(const uint8_t* __restrict__ base, const uint32_t* __restrict__ off,
+                           const uint32_t* __restrict__ len, const uint8_t* __restrict__ skey, uint32_t sklen, const uint64_t* __restrict__ pow5,
+                           const uint32_t* __restrict__ slow_list, const uint32_t* __restrict__ nslow,
+                           uint8_t* __restrict__ status, uint32_t* __restrict__ nent, uint32_t* __restrict__ narena,
+                           unsigned long long* __restrict__ counters) {
+    const uint32_t m = *nslow, stride = gridDim.x * blockDim.x;
+    for (uint32_t j0 = blockIdx.x * blockDim.x; j0 < m; j0 += stride) {
+        const uint32_t j = j0 + threadIdx.x;
+        const bool valid = j < m;
+        uint32_t st = LC_JSON_ST_FAILED;
+        if (valid) {
+            const uint32_t i = slow_list[j];
+            uint32_t ne, na;
+            bool sl;
+            st = lc_json_count<true>(base, off[i], len[i], skey, sklen, pow5, &ne, &na, &sl);
+            status[i] = (uint8_t)st;
+            nent[i] = ne;
+            narena[i] = na;
+        }
+        json_add_counters(st, valid, counters);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    json_emit_kernel(const uint8_t* __restrict__ base, const uint32_t* __restrict__ off,
+                     const uint32_t* __restrict__ len, uint64_t n, const uint8_t* __restrict__ skey, uint32_t sklen, const uint64_t* __restrict__ pow5,
+                     const uint8_t* __restrict__ status, const uint8_t* __restrict__ slow,
+                     const uint64_t* __restrict__ first, const uint64_t* __restrict__ afirst,
+                     LcJsonEntry* __restrict__ entries, uint8_t* __restrict__ arena, uint32_t* bad) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || slow[i] || (status[i] & 0x7Fu) != LC_JSON_ST_OK)
+        return;
+    const uint64_t e0 = first[i], a0 = afirst[i];
+    if (!lc_json_emit<false>(base, off[i], len[i], skey, sklen, pow5, entries + e0, (uint32_t)(first[i + 1] - e0),
+                             arena + a0, (uint32_t)a0, (uint32_t)(afirst[i + 1] - a0)))
+        atomicOr(bad, 2u);
+}
+
+__global__ void __launch_bounds__(128)
+    json_emit_slow_kernel(const uint8_t* __restrict__ base, const uint32_t* __restrict__ off,
+                          const uint32_t* __restrict__ len, const uint8_t* __restrict__ skey, uint32_t sklen, const uint64_t* __restrict__ pow5,
+                          const uint8_t* __restrict__ status, const uint32_t* __restrict__ slow_list,
+                          const uint32_t* __restrict__ nslow, const uint64_t* __restrict__ first,
+                          const uint64_t* __restrict__ afirst, LcJsonEntry* __restrict__ entries,
+                          uint8_t* __restrict__ arena, uint32_t* bad) {
+    const uint32_t m = *nslow;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
+        const uint32_t i = slow_list[j];
+        if ((status[i] & 0x7Fu) != LC_JSON_ST_OK)
+            continue;
+        const uint64_t e0 = first[i], a0 = afirst[i];
+        if (!lc_json_emit<true>(base, off[i], len[i], skey, sklen, pow5, entries + e0, (uint32_t)(first[i + 1] - e0),
+                                arena + a0, (uint32_t)a0, (uint32_t)(afirst[i + 1] - a0)))
+            atomicOr(bad, 2u);
+    }
+}
+
+// the slow kernels run a fixed grid over the device-side count of slow events, so no host round trip is needed
+constexpr unsigned kJsonSlowBlocks = 264;
+
+void launch_json_count(const uint8_t* d_base, uint64_t base_len, const uint32_t* d_off, const uint32_t* d_len,
+                       uint64_t n, const uint8_t* d_skey, uint32_t sklen, const uint64_t* d_pow5, uint8_t* d_status, uint32_t* d_nent,
+                       uint32_t* d_narena, uint8_t* d_slow, uint32_t* d_slow_list, uint32_t* d_nslow, uint32_t* d_bad,
+                       unsigned long long* d_counters, cudaStream_t st) {
+    if (n)
+        json_count_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_base, base_len, d_off, d_len, n, d_skey,
+                                                                        sklen, d_pow5, d_status, d_nent, d_narena, d_slow,
+                                                                        d_slow_list, d_nslow, d_bad, d_counters);
+}
+
+void launch_json_count_slow(const uint8_t* d_base, const uint32_t* d_off, const uint32_t* d_len,
+                            const uint8_t* d_skey, uint32_t sklen, const uint64_t* d_pow5, const uint32_t* d_slow_list, const uint32_t* d_nslow,
+                            uint8_t* d_status, uint32_t* d_nent, uint32_t* d_narena, unsigned long long* d_counters,
+                            cudaStream_t st) {
+    json_count_slow_kernel<<<kJsonSlowBlocks, 128, 0, st>>>(d_base, d_off, d_len, d_skey, sklen, d_pow5, d_slow_list,
+                                                            d_nslow, d_status, d_nent, d_narena, d_counters);
+}
+
+void launch_json_emit(const uint8_t* d_base, const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+                      const uint8_t* d_skey, uint32_t sklen, const uint64_t* d_pow5, const uint8_t* d_status, const uint8_t* d_slow,
+                      const uint64_t* d_first, const uint64_t* d_afirst, LcJsonEntry* d_entries, uint8_t* d_arena,
+                      uint32_t* d_bad, cudaStream_t st) {
+    if (n)
+        json_emit_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_base, d_off, d_len, n, d_skey, sklen, d_pow5,
+                                                                       d_status, d_slow, d_first, d_afirst, d_entries,
+                                                                       d_arena, d_bad);
+}
+
+void launch_json_emit_slow(const uint8_t* d_base, const uint32_t* d_off, const uint32_t* d_len,
+                           const uint8_t* d_skey, uint32_t sklen, const uint64_t* d_pow5, const uint8_t* d_status,
+                           const uint32_t* d_slow_list, const uint32_t* d_nslow, const uint64_t* d_first,
+                           const uint64_t* d_afirst, LcJsonEntry* d_entries, uint8_t* d_arena, uint32_t* d_bad,
+                           cudaStream_t st) {
+    json_emit_slow_kernel<<<kJsonSlowBlocks, 128, 0, st>>>(d_base, d_off, d_len, d_skey, sklen, d_pow5, d_status,
+                                                           d_slow_list,
+                                                           d_nslow, d_first, d_afirst, d_entries, d_arena, d_bad);
+}
+
 } // namespace lck

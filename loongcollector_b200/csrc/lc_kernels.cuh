@@ -20,6 +20,7 @@ struct LcTsSpans;
 struct LcTsFull;
 struct LcApEv;
 struct LcApEntry;
+struct LcJsonEntry;
 struct LcLz4Chunk;
 
 namespace lck {
@@ -401,5 +402,29 @@ void launch_ap_resolve(const LcTsNow& now, const LcApEv* d_ev, const uint32_t* d
                        unsigned long long* d_counters, cudaStream_t st);
 void launch_ap_emit(const uint8_t* d_base, const uint32_t* d_off, const uint32_t* d_len, const uint8_t* d_status,
                     uint64_t n, const uint64_t* d_first, LcApEntry* d_entries, cudaStream_t st);
+
+// ProcessorParseJsonNative (lc_exec.cuh): launch_json_count runs the fast walk, one thread per event, and writes each
+// event's status, entry count, arena bytes and slow flag; an event the fast walk gives up on is appended to d_slow_list
+// (*d_nslow) and launch_json_count_slow finishes it over that list.  *d_bad |= 1 for an event past base_len, which is
+// not read.  counters[3] += key_not_found, out_failed, ok.  After exclusive sums of both counts (d_first, d_afirst),
+// launch_json_emit and launch_json_emit_slow write the entries and arena bytes; *d_bad |= 2 when an event would not
+// fill its ranges exactly (nothing is written past them).
+void launch_json_count(const uint8_t* d_base, uint64_t base_len, const uint32_t* d_off, const uint32_t* d_len,
+                       uint64_t n, const uint8_t* d_skey, uint32_t sklen, const uint64_t* d_pow5, uint8_t* d_status, uint32_t* d_nent,
+                       uint32_t* d_narena, uint8_t* d_slow, uint32_t* d_slow_list, uint32_t* d_nslow, uint32_t* d_bad,
+                       unsigned long long* d_counters, cudaStream_t st);
+void launch_json_count_slow(const uint8_t* d_base, const uint32_t* d_off, const uint32_t* d_len,
+                            const uint8_t* d_skey, uint32_t sklen, const uint64_t* d_pow5, const uint32_t* d_slow_list, const uint32_t* d_nslow,
+                            uint8_t* d_status, uint32_t* d_nent, uint32_t* d_narena, unsigned long long* d_counters,
+                            cudaStream_t st);
+void launch_json_emit(const uint8_t* d_base, const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+                      const uint8_t* d_skey, uint32_t sklen, const uint64_t* d_pow5, const uint8_t* d_status, const uint8_t* d_slow,
+                      const uint64_t* d_first, const uint64_t* d_afirst, LcJsonEntry* d_entries, uint8_t* d_arena,
+                      uint32_t* d_bad, cudaStream_t st);
+void launch_json_emit_slow(const uint8_t* d_base, const uint32_t* d_off, const uint32_t* d_len,
+                           const uint8_t* d_skey, uint32_t sklen, const uint64_t* d_pow5, const uint8_t* d_status,
+                           const uint32_t* d_slow_list, const uint32_t* d_nslow, const uint64_t* d_first,
+                           const uint64_t* d_afirst, LcJsonEntry* d_entries, uint8_t* d_arena, uint32_t* d_bad,
+                           cudaStream_t st);
 
 } // namespace lck

@@ -3554,7 +3554,166 @@ std::vector<std::pair<std::string, uint64_t>> ProcessorParseApsaraNative::Counte
             {"history_failure", mHistoryFailureTotal.GetValue()}};
 }
 
+// ------------------------------------------------------------------------------------- ProcessorParseJsonNative
+const std::string ProcessorParseJsonNative::sName = "processor_parse_json_native";
+
+bool ProcessorParseJsonNative::Init(const Json::Value& config) {
+    if (!GetString(config, "SourceKey", mSourceKey))
+        return Fail("mandatory string param SourceKey is missing");
+    if (!mCommonParserOptions.Init(config))
+        return false;
+    lc_json_free(mProgram);
+    mProgram = nullptr;
+    if (lc_json_compile(mSourceKey.data(), mSourceKey.size(), &mProgram) != LC_OK)
+        return Fail(std::string("lc_json_compile: ") + lc_last_error());
+    return true;
+}
+
+void ProcessorParseJsonNative::Process(PipelineEventGroup& group) {
+    std::vector<PipelineEventGroup> one;
+    one.emplace_back(std::move(group));
+    Process(one);
+    group = std::move(one[0]);
+}
+
+void ProcessorParseJsonNative::Process(std::vector<PipelineEventGroup>& groups) {
+    if (!mProgram)
+        return;
+    // one device call for all groups, cut only where the values would reach the call's 2 GiB limit (ProcessBatch
+    // cuts again where the arena would)
+    size_t g0 = 0;
+    uint64_t bytes = 0;
+    for (size_t g = 0; g < groups.size(); ++g) {
+        uint64_t b = 0;
+        for (PipelineEventPtr& e : groups[g].MutableEvents())
+            if (IsSupportedEvent(e) && e.Cast<LogEvent>().HasContent(mSourceKey))
+                b += e.Cast<LogEvent>().GetContent(mSourceKey).size();
+        if (g > g0 && bytes + b >= LC_JSON_ARENA) {
+            ProcessBatch(groups, g0, g);
+            g0 = g;
+            bytes = 0;
+        }
+        bytes += b;
+    }
+    if (g0 < groups.size())
+        ProcessBatch(groups, g0, groups.size());
+}
+
+void ProcessorParseJsonNative::ProcessBatch(std::vector<PipelineEventGroup>& groups, size_t g0, size_t g1) {
+    std::string bytes;
+    std::vector<uint32_t> off, len;
+    for (size_t g = g0; g < g1; ++g) {
+        for (PipelineEventPtr& e : groups[g].MutableEvents()) {
+            const LogEvent* ev = IsSupportedEvent(e) ? &e.Cast<LogEvent>() : nullptr;
+            if (ev && ev->HasContent(mSourceKey)) {
+                const StringView v = ev->GetContent(mSourceKey);
+                off.push_back((uint32_t)bytes.size());
+                len.push_back((uint32_t)v.size());
+                bytes.append(v.data(), v.size());
+            } else {
+                off.push_back(0);
+                len.push_back(LC_TS_NO_KEY);
+            }
+        }
+    }
+    const uint64_t n = off.size();
+    if (n == 0)
+        return;
+    std::vector<uint8_t> status(n);
+    std::vector<uint64_t> first(n + 1);
+    std::vector<lc_json_entry_t> ent(n * 8);
+    std::string arena(bytes.size() + 64, '\0');
+    uint64_t cnt[3], nent = 0, narena = 0;
+    try {
+        for (;;) {
+            const int rc = lc_json_parse(Engine(), mProgram, reinterpret_cast<const uint8_t*>(bytes.data()),
+                                         bytes.size(), off.data(), len.data(), n, status.data(), first.data(),
+                                         ent.data(), ent.size(), &nent, reinterpret_cast<uint8_t*>(&arena[0]),
+                                         arena.size(), &narena, cnt);
+            if (rc == LC_ERR_TOO_LARGE && g1 - g0 > 1) {
+                // the renderings would reach the arena's 2 GiB (a "%f" can be 60 times its source): cut the batch
+                const size_t mid = g0 + (g1 - g0) / 2;
+                ProcessBatch(groups, g0, mid);
+                ProcessBatch(groups, mid, g1);
+                return;
+            }
+            if (rc != LC_ERR_CAPACITY) {
+                Check(rc, "lc_json_parse");
+                break;
+            }
+            ent.resize(nent > ent.size() ? nent : ent.size());
+            arena.resize(narena > arena.size() ? narena : arena.size());
+        }
+    } catch (const std::exception& ex) {
+        EngineFailed(ex.what());
+        return;
+    }
+    uint64_t i = 0, unsupported = 0, erased = 0, kept = 0;
+    for (size_t g = g0; g < g1; ++g) {
+        EventsContainer& events = groups[g].MutableEvents();
+        SourceBuffer& sb = *groups[g].GetSourceBuffer();
+        const StringBuffer renamed = sb.CopyString(mCommonParserOptions.mRenamedSourceKey);
+        const StringView rkey(renamed.data, renamed.size);
+        auto addIfAbsent = [](LogEvent& ev, StringView k, StringView v) {
+            if (!ev.HasContent(k))
+                ev.AppendContentNoCopy(k, v);
+        };
+        size_t wIdx = 0;
+        for (size_t rIdx = 0; rIdx < events.size(); ++rIdx, ++i) {
+            const uint32_t st = status[i] & 0x7Fu;
+            if (!IsSupportedEvent(events[rIdx])) {
+                unsupported++; // counted as key_not_found by the device: ProcessEvent counts it out_failed
+            } else if (st != LC_JSON_NOT_FOUND) {
+                LogEvent& ev = events[rIdx].Cast<LogEvent>();
+                const StringView v = ev.GetContent(mSourceKey);
+                const bool ok = st == LC_JSON_OK;
+                if (ok) {
+                    auto view = [&](uint32_t o, uint32_t l) {
+                        if (o & LC_JSON_ARENA) {
+                            const StringBuffer b = sb.CopyString(arena.data() + (o & ~LC_JSON_ARENA), l);
+                            return StringView(b.data, b.size);
+                        }
+                        return StringView(v.data() + (o - off[i]), l);
+                    };
+                    for (uint64_t k = first[i]; k < first[i + 1]; ++k) {
+                        const lc_json_entry_t& x = ent[k];
+                        ev.SetContentNoCopy(view(x.key_off, x.key_len), view(x.val_off, x.val_len));
+                    }
+                }
+                if (!ok || !(status[i] & LC_JSON_OVERWRITTEN))
+                    ev.DelContent(mSourceKey);
+                if (mCommonParserOptions.ShouldAddSourceContent(ok))
+                    addIfAbsent(ev, rkey, v);
+                if (mCommonParserOptions.ShouldAddLegacyUnmatchedRawLog(ok))
+                    addIfAbsent(ev, CommonParserOptions::legacyUnmatchedRawLogKey, v);
+                if (mCommonParserOptions.ShouldEraseEvent(ok, ev, groups[g].GetAllMetadata())) {
+                    erased++;
+                    continue;
+                }
+                kept++;
+            }
+            if (wIdx != rIdx)
+                events[wIdx] = std::move(events[rIdx]);
+            ++wIdx;
+        }
+        events.resize(wIdx);
+    }
+    mOutKeyNotFoundEventsTotal.Add(cnt[0] - unsupported);
+    mOutFailedEventsTotal.Add(cnt[1] + unsupported);
+    mDiscardedEventsTotal.Add(erased);
+    mOutSuccessfulEventsTotal.Add(kept);
+}
+
+std::vector<std::pair<std::string, uint64_t>> ProcessorParseJsonNative::Counters() const {
+    return {{"discarded", mDiscardedEventsTotal.GetValue()},
+            {"out_failed", mOutFailedEventsTotal.GetValue()},
+            {"out_key_not_found", mOutKeyNotFoundEventsTotal.GetValue()},
+            {"out_successful", mOutSuccessfulEventsTotal.GetValue()}};
+}
+
 Processor* CreateProcessor(const std::string& type) {
+    if (type == ProcessorParseJsonNative::sName)
+        return new ProcessorParseJsonNative;
     if (type == ProcessorParseApsaraNative::sName)
         return new ProcessorParseApsaraNative;
     if (type == ProcessorParseTimestampNative::sName)

@@ -117,6 +117,7 @@ class ProcessorParseDelimiterNative;
 class ProcessorFilterNative;
 class ProcessorParseTimestampNative;
 class ProcessorParseApsaraNative;
+class ProcessorParseJsonNative;
 
 class ProcessorSplitLogStringNative : public Processor {
 public:
@@ -455,6 +456,32 @@ protected:
 
 private:
     lc_apsara_t* mProgram = nullptr;
+};
+
+// processor_parse_json_native (ProcessorParseJsonNative.cpp: ProcessEvent, JsonLogLineParserSimdJson): the groups of
+// one call go to the device in one lc_json_parse call (cut where the values or the arena would reach 2 GiB);
+// the validation and the rendering of every member run there.  The host applies the members with overwrite
+// (SetContentNoCopy, as AddLog(key, value, event) does), copies the arena bytes into the group's SourceBuffer,
+// applies CommonParserOptions, erases events and adds the counters.
+class ProcessorParseJsonNative : public Processor {
+public:
+    static const std::string sName;
+    const std::string& Name() const override { return sName; }
+    ~ProcessorParseJsonNative() override { lc_json_free(mProgram); }
+    bool Init(const Json::Value& config) override;
+    void Process(PipelineEventGroup& group) override;
+    void Process(std::vector<PipelineEventGroup>& groups) override;
+    std::vector<std::pair<std::string, uint64_t>> Counters() const override;
+    std::string mSourceKey;
+    CommonParserOptions mCommonParserOptions;
+    Counter mDiscardedEventsTotal, mOutFailedEventsTotal, mOutKeyNotFoundEventsTotal, mOutSuccessfulEventsTotal;
+
+protected:
+    bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
+
+private:
+    void ProcessBatch(std::vector<PipelineEventGroup>& groups, size_t g0, size_t g1);
+    lc_json_t* mProgram = nullptr;
 };
 
 class ProcessorFilterNative : public Processor {

@@ -294,3 +294,48 @@ def apsara_lines(n, seed=DEFAULT_SEED, t0=1700000000, groups_of=1024):
     if grp[-1] != n or grp.size == 1:
         grp = np.append(grp, np.uint32(n))
     return np.frombuffer(b"".join(parts), np.uint8), off, ln, grp
+
+
+def _json_line(rng, target):
+    """one JSON access-log object of about target bytes: 8-40 members -- strings (about 10 % with escapes), ints, one
+    or two floats (shortest round-trip doubles, small and large exponents among them), booleans and null, a nested
+    label object and an array"""
+    words = lambda k: _rand_word(rng, k)  # noqa: E731
+    m = [b'"ts":%d' % rng.randrange(1_600_000_000, 1_800_000_000),
+         b'"method":"%s"' % rng.choice([b"GET", b"POST", b"PUT", b"DELETE"]),
+         b'"status":%d' % rng.choice([200, 200, 200, 301, 404, 500]),
+         b'"latency":%s' % repr(rng.uniform(0, 5000)).encode()]  # shortest round-trip doubles, 17 digits mostly
+    if rng.random() < 0.5:
+        m.append(b'"ratio":%s' % rng.choice([b"-4.56e-3", b"0.25", b"1.5e3", b"0.0078125", b"3.14159",
+                                             repr(rng.uniform(-1, 1) * 10.0 ** rng.randint(-30, 22)).encode()]))
+    m.append(b'"ok":%s' % rng.choice([b"true", b"false"]))
+    m.append(b'"trace":null')
+    m.append(b'"labels":{"app":"%s","zone":"%s","tier":%d}' % (words(6).encode(), words(4).encode(), rng.randrange(9)))
+    m.append(b'"hops":[%s]' % b",".join(b"%d" % rng.randrange(1000) for _ in range(rng.randint(0, 6))))
+    nmem = rng.randint(8, 40)
+    while len(m) < nmem:
+        k = words(rng.randint(3, 12)).encode()
+        if rng.random() < 0.7:
+            v = words(rng.randint(1, 24)).encode()
+            if rng.random() < 0.1:
+                v += rng.choice([b"\\n", b"\\t", b'\\"', b"\\u00e9", b"\\/"]) + words(4).encode()
+            m.append(b'"%s":"%s"' % (k, v))
+        else:
+            m.append(b'"%s":%d' % (k, rng.randrange(-10 ** 9, 10 ** 12)))
+    line = b"{" + b",".join(m) + b"}"
+    if len(line) < target:  # a message member brings the object to its length
+        line = line[:-1] + b',"msg":"' + words(target - len(line) - 9).encode() + b'"}'
+    return line
+
+
+def json_lines(n, seed=DEFAULT_SEED, lo=150, hi=4096, groups_of=1024, pool=8192):
+    """n JSON access-log lines of lo - hi bytes (_json_line), sampled from a seeded pool of distinct lines.  Returns
+    (buf u8, off u32, len u32, grp u32): one group per groups_of lines."""
+    rng = random.Random(seed)
+    lines = [_json_line(rng, rng.randint(lo, hi)) + b"\n" for _ in range(min(pool, n))]
+    buf, off, ln = _assemble(lines, n, seed)
+    grp = np.minimum(np.arange(0, n + groups_of, groups_of, dtype=np.uint64), n).astype(np.uint32)
+    grp = np.unique(grp)
+    if grp[-1] != n or grp.size == 1:
+        grp = np.append(grp, np.uint32(n))
+    return buf, off, ln, grp
