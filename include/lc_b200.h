@@ -1091,6 +1091,73 @@ int lc_json_parse_dev(lc_engine_t* e, const lc_json_t* js, const uint8_t* d_base
                       uint64_t* d_first, lc_json_entry_t* d_entries, uint64_t entry_cap, uint64_t* n_entries,
                       uint8_t* d_arena, uint64_t arena_cap, uint64_t* arena_bytes, uint64_t* d_counters);
 
+/* ---- f4: the split -> JSON chain (ProcessorSplitLogStringNative or ProcessorSplitMultilineLogStringNative, then
+ * ProcessorParseJsonNative with the same SourceKey -- the reference's documented pipeline for JSON-lines files) to
+ * the SLS wire format.  The source event is flat, as for the split -> regex chain: SourceKey (js's) -> the value, with
+ * its position src_pos, time and time_ns (LC_SLS_NO_NS = no Time_ns).  Piece k enters the JSON stage as [SourceKey ->
+ * piece] or, when offset_key != NULL, [SourceKey -> piece, offset_key -> decimal(src_pos + off[k])], and the stage does
+ * what ProcessorParseJsonNative::ProcessEvent does (oracle/json_parse.py restates it).  AddLog overwrites in place, so
+ * a repeated key keeps its FIRST position and takes its LAST value; keys are equal when their rendered bytes are
+ * ("a" and "\u0061" are one key).
+ *   A piece that parses (LC_JSON_OK), contents in this order: SourceKey, only when a member has that key
+ *   (LC_JSON_OVERWRITTEN), with the last such member's value (else SourceKey is deleted); the offset content, with the
+ *   last member keyed offset_key if there is one, else the digits; every other distinct member key in order of first
+ *   occurrence, with the value of its last occurrence; with keep_succeed, renamed_key -> piece unless that key is
+ *   present (a member key, the offset key, or SourceKey while overwritten -- AddLog(..., false)).
+ *   A piece that fails (LC_JSON_FAILED, or LC_JSON_EMPTY for an empty piece): SourceKey is deleted and the offset
+ *   content stays; with keep_fail, renamed_key -> piece, and with copy_raw as well "__raw_log__" -> piece, neither
+ *   added when already present; without keep_fail the piece is erased (ShouldEraseEvent).
+ *   A piece left without contents (e.g. {} without an offset key) has no record and still counts as successful.
+ *   Every record carries the source event's time and time_ns.  renamed_key is the effective RenamedSourceKey
+ *   (SourceKey when the configuration leaves it empty).
+ * counters[3] (may be NULL) = out_successful, out_failed (LC_JSON_FAILED only) and discarded, in the split -> regex
+ * chain's order; a piece always holds SourceKey, so there is no key-not-found.  Refused with LC_ERR_INVALID_ARG: an
+ * offset_key equal to SourceKey, bad arguments.  LC_ERR_TOO_LARGE: src_len >= 2^31 (the arena bit of the entries),
+ * n >= 2^30, or a record that would reach 4 GiB.
+ *
+ * lc_sls_serialize_split_json_dev: from the DEVICE piece tables of one lc_split_lines_dev / lc_multiline_split_dev
+ * call over d_src[0, src_len) and the DEVICE tables of lc_json_parse_dev over those pieces with js (d_status, d_first,
+ * d_entries, d_arena).  d_out receives the bytes; *out_len (host) their count; LC_ERR_CAPACITY if > out_cap (nothing
+ * written, *out_len and counters set). */
+int lc_sls_serialize_split_json_dev(lc_engine_t* e, const lc_json_t* js, const uint8_t* d_src, uint64_t src_len,
+                                    const uint32_t* d_off, const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                    const uint64_t* d_first, const lc_json_entry_t* d_entries, const uint8_t* d_arena,
+                                    const char* renamed_key, uint32_t renamed_key_len, int keep_fail,
+                                    int keep_succeed, int copy_raw, const char* offset_key, uint32_t offset_key_len,
+                                    uint64_t src_pos, uint32_t time, uint32_t time_ns, uint8_t* d_out,
+                                    uint64_t out_cap, uint64_t* out_len, uint64_t counters[3]);
+
+/* The same with a HOST source value: upload it once, split it on the device, run lc_json_parse_dev's passes over the
+ * pieces, serialise, and bring back only the wire bytes; *n_events, ml_counters, the _lz4 variants and which outputs
+ * are set on LC_ERR_CAPACITY as for lc_split_regex_parse_sls.  A chunk whose pieces are all erased or empty gives 0
+ * bytes (the _lz4 calls then return the block of the tail alone). */
+int lc_split_json_parse_sls(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len, uint8_t split_char,
+                            const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed,
+                            int copy_raw, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+                            uint32_t time, uint32_t time_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                            uint64_t* n_events, uint64_t counters[3]);
+int lc_split_json_parse_sls_lz4(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                                uint8_t split_char, const char* renamed_key, uint32_t renamed_key_len, int keep_fail,
+                                int keep_succeed, int copy_raw, const char* offset_key, uint32_t offset_key_len,
+                                uint64_t src_pos, uint32_t time, uint32_t time_ns, const uint8_t* tail,
+                                uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                                uint64_t* raw_len, uint64_t* n_events, uint64_t counters[3]);
+int lc_multiline_split_json_parse_sls(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                                      const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                      int discard_unmatched, const char* renamed_key, uint32_t renamed_key_len,
+                                      int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+                                      uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                      uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                      uint64_t counters[3], uint64_t ml_counters[3]);
+int lc_multiline_split_json_parse_sls_lz4(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                                          const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                          int discard_unmatched, const char* renamed_key, uint32_t renamed_key_len,
+                                          int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+                                          uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                          const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+                                          uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                                          uint64_t counters[3], uint64_t ml_counters[3]);
+
 #ifdef __cplusplus
 }
 #endif

@@ -132,6 +132,9 @@ struct lc_engine {
     DevBuf js_conf, js_nent, js_narena, js_slow, js_list, js_afirst, js_small, js_pow5;
     uint64_t js_conf_id = 0;
     DevBuf js_status, js_first, js_ent, js_arena, js_cnt;
+    // split -> JSON -> SLS chain: the resolve's per-entry winners, per-piece records, list of pieces to sort (behind
+    // its count) and sort scratch; the chain's piece and JSON tables are in, out_a, out_b and the js_* buffers
+    DevBuf sj_win, sj_ev, sj_list, sj_sort;
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
     std::unordered_map<uint64_t, void*> blobs; // regex id * 4 + layout -> device blob
@@ -353,7 +356,7 @@ void lc_engine_destroy(lc_engine_t* e) {
                       &e->ap_conf, &e->ap_ev, &e->ap_nent, &e->ap_small, &e->ap_status, &e->ap_sec, &e->ap_nsec,
                       &e->ap_micro, &e->ap_first, &e->ap_ent, &e->js_conf, &e->js_nent, &e->js_narena,
                       &e->js_slow, &e->js_list, &e->js_afirst, &e->js_small, &e->js_status, &e->js_first, &e->js_ent,
-                      &e->js_arena, &e->js_cnt, &e->js_pow5};
+                      &e->js_arena, &e->js_cnt, &e->js_pow5, &e->sj_win, &e->sj_ev, &e->sj_list, &e->sj_sort};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -4740,3 +4743,222 @@ int lc_json_parse(lc_engine_t* e, const lc_json_t* js, const uint8_t* base, uint
     CU_TRY(cudaStreamSynchronize(e->stream));
     return rc;
 }
+
+// ------------------------------------------------------------------------------------------------ split -> JSON -> SLS
+// The JSON stage's CommonParserOptions and the offset content of the split events (offset_key NULL = no
+// log.file.offset metadata), with the source event's position, time and ns
+#define SPLIT_JSON_PARAMS                                                                                              \
+    const char *renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,                 \
+        const char *offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns
+#define SPLIT_JSON_ARGS                                                                                                \
+    renamed_key, renamed_key_len, keep_fail, keep_succeed, copy_raw, offset_key, offset_key_len, src_pos, time, time_ns
+
+namespace {
+
+// lc_split_json_sls_setup over js's SourceKey, with SourceKey, RenamedSourceKey, the offset key and "__raw_log__"
+// staged on the device (`sls_plan`, which neither splitter nor the JSON stage uses) and *c pointing at them
+int split_json_sls_config(lc_engine_t* e, const char* what, const lc_json_t* js, SPLIT_JSON_PARAMS,
+                          LcSplitJsonSlsCfg* c) {
+    if (!js || (renamed_key_len && !renamed_key) || (offset_key_len && !offset_key))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    const uint32_t oklen = offset_key ? offset_key_len : 0u;
+    if ((uint64_t)js->skey.size() + renamed_key_len + oklen + 16 > 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": keys must stay below 4 GiB");
+    const char* why = lc_split_json_sls_setup(js->skey.data(), (uint32_t)js->skey.size(), renamed_key,
+                                              renamed_key_len, offset_key, oklen, keep_fail, keep_succeed, copy_raw,
+                                              src_pos, time, time_ns, c);
+    if (why)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    std::string keys = js->skey;
+    keys.append(renamed_key ? renamed_key : "", renamed_key_len);
+    keys.append(offset_key ? offset_key : "", oklen);
+    keys.append("__raw_log__", 11);
+    CU_TRY(e->sls_plan.ensure(keys.size() + 1));
+    if (!keys.empty())
+        CU_TRY(cudaMemcpyAsync(e->sls_plan.p, keys.data(), keys.size(), cudaMemcpyHostToDevice, e->stream));
+    const uint8_t* d = e->sls_plan.as<uint8_t>();
+    c->skey = d;
+    c->rkey = d + c->sklen;
+    c->okey = d + c->sklen + c->rklen;
+    c->raw = c->okey + c->oklen;
+    return LC_OK;
+}
+
+// The resolve pass, the size pass and the emit of the chain over the n pieces of t (m entries in all; t.win and t.ev
+// are set here): into d_out (the device-fed call), or back to the host buffer out, or -- with z -- records ‖ tail as
+// one LZ4 block.  counters[3] = successful, failed, discarded; set whenever the size pass ran.
+int split_json_sls_run(lc_engine_t* e, const char* what, const LcSplitJsonSlsCfg& c, lck::SplitJsonSlsTables t,
+                       uint64_t n, uint64_t m, uint8_t* d_out, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                       uint64_t* counters, const Lz4Tail* z) {
+    CU_TRY(e->sj_win.ensure(m * 4 + 4));
+    CU_TRY(e->sj_ev.ensure(n * sizeof(LcJsonSlsEv)));
+    CU_TRY(e->sj_list.ensure(n * 4 + 4));
+    CU_TRY(e->sj_sort.ensure(3 * m * 4 + 4));
+    uint32_t* nlist = e->sj_list.as<uint32_t>();
+    CU_TRY(cudaMemsetAsync(nlist, 0, 4, e->stream));
+    t.win = e->sj_win.as<uint32_t>();
+    t.ev = e->sj_ev.as<LcJsonSlsEv>();
+    lck::launch_json_resolve(c, t, n, m, nlist + 1, nlist, e->sj_sort.as<uint32_t>(), e->stream);
+    e->launches += 2;
+    CU_TRY(cudaGetLastError());
+    uint64_t ctr[4] = {0};
+    SlsTo to;
+    to.host = out;
+    to.z = z;
+    to.too_large = 3;
+    const int rc = serialize_sls_dev(
+        e, what, n, 4,
+        [&](uint32_t* rec, uint32_t* body, unsigned long long* d_ctr) {
+            lck::launch_split_json_sls_sizes(c, t, n, rec, body, d_ctr, e->stream);
+        },
+        [&](const uint64_t* rec_off, const uint32_t* body, uint8_t* dst) {
+            lck::launch_split_json_sls_emit(c, t, n, rec_off, body, dst, e->stream);
+        },
+        d_out, out_cap, out_len, ctr, to);
+    if (counters)
+        memcpy(counters, ctr, 3 * sizeof(uint64_t));
+    return rc;
+}
+
+// Host-buffer split + JSON + serialise (lc_split_json_parse_sls and the multiline / LZ4 siblings): the JSON stage
+// runs js_count / js_emit over the pieces into the js_* buffers of lc_json_parse, then split_json_sls_run.
+template <class Split>
+int split_json_sls_host(lc_engine_t* e, const char* what, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                        Split split, SPLIT_JSON_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                        uint64_t* n_events, uint64_t* counters, const Lz4Tail* z) {
+    LcSplitJsonSlsCfg c;
+    auto begin = [&]() {
+        if (counters)
+            memset(counters, 0, 3 * sizeof(uint64_t));
+        if (len >= LC_JSON_ARENA)
+            return fail(LC_ERR_TOO_LARGE, std::string(what) + ": the source value must be < 2 GiB");
+        return (int)LC_OK;
+    };
+    auto config = [&]() { return split_json_sls_config(e, what, js, SPLIT_JSON_ARGS, &c); };
+    auto run = [&](uint64_t n) {
+        if (n >= (1ull << 30))
+            return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^30 pieces per call");
+        CU_TRY(e->js_status.ensure(n));
+        CU_TRY(e->js_first.ensure((n + 1) * 8));
+        CU_TRY(e->js_cnt.ensure(3 * sizeof(uint64_t)));
+        const uint8_t* d_src = e->in.as<uint8_t>();
+        const uint32_t *off = e->out_a.as<uint32_t>(), *ln = e->out_b.as<uint32_t>();
+        uint64_t m = 0, a = 0;
+        int rc = js_count(e, js, what, d_src, len, off, ln, n, e->js_status.as<uint8_t>(), e->js_first.as<uint64_t>(),
+                          &m, &a, e->js_cnt.as<uint64_t>());
+        if (rc)
+            return rc;
+        CU_TRY(e->js_ent.ensure(m * sizeof(LcJsonEntry) + 16));
+        CU_TRY(e->js_arena.ensure(a + 16));
+        if (m) {
+            rc = js_emit(e, js, what, d_src, off, ln, n, e->js_status.as<uint8_t>(), e->js_first.as<uint64_t>(),
+                         e->js_ent.as<lc_json_entry_t>(), e->js_arena.as<uint8_t>());
+            if (rc)
+                return rc;
+        }
+        const lck::SplitJsonSlsTables t{d_src, off, ln, e->js_status.as<uint8_t>(), e->js_first.as<uint64_t>(),
+                                        e->js_ent.as<LcJsonEntry>(), e->js_arena.as<uint8_t>(), nullptr, nullptr};
+        return split_json_sls_run(e, what, c, t, n, m, nullptr, out, out_cap, out_len, counters, z);
+    };
+    return split_chain_sls_host(e, what, buf, len, split, js != nullptr, begin, config, run, out, out_cap, out_len,
+                                n_events, z);
+}
+
+template <class Split>
+int split_json_lz4_host(lc_engine_t* e, const char* what, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                        Split split, SPLIT_JSON_PARAMS, const uint8_t* tail, uint64_t tail_len, uint8_t* out,
+                        uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                        uint64_t* counters) {
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return split_json_sls_host(e, what, js, buf, len, split, SPLIT_JSON_ARGS, out, out_cap, out_len, n_events,
+                               counters, &z);
+}
+
+} // namespace
+
+// (the multiline splitter's own counters[3] are added to ml_counters as lc_multiline_split_dev adds them)
+#define ML_SPLIT                                                                                                       \
+    [&](uint64_t* n) {                                                                                                 \
+        return lc_multiline_split_dev(e, e->in.as<uint8_t>(), len, start, cont, end, discard_unmatched,               \
+                                      e->out_a.as<uint32_t>(), e->out_b.as<uint32_t>(), e->out_c.as<uint8_t>(), len,  \
+                                      n, ml_counters);                                                                 \
+    }
+
+extern "C" {
+
+int lc_sls_serialize_split_json_dev(lc_engine_t* e, const lc_json_t* js, const uint8_t* d_src, uint64_t src_len,
+                                    const uint32_t* d_off, const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                    const uint64_t* d_first, const lc_json_entry_t* d_entries, const uint8_t* d_arena,
+                                    SPLIT_JSON_PARAMS, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len,
+                                    uint64_t counters[3]) {
+    static const char* what = "lc_sls_serialize_split_json_dev";
+    if (!e || !js || !out_len || (n && (!d_src || !d_off || !d_len || !d_status || !d_first)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (counters)
+        memset(counters, 0, 3 * sizeof(uint64_t));
+    if (src_len >= LC_JSON_ARENA || n >= (1ull << 30))
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": the source value must be < 2 GiB, < 2^30 pieces per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcSplitJsonSlsCfg c;
+    rc = split_json_sls_config(e, what, js, SPLIT_JSON_ARGS, &c);
+    if (rc || n == 0)
+        return rc;
+    uint64_t m = 0;
+    CU_TRY(cudaMemcpyAsync(&m, d_first + n, 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    if (m && (!d_entries || !d_arena))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    const lck::SplitJsonSlsTables t{d_src, d_off, d_len, d_status, d_first,
+                                    reinterpret_cast<const LcJsonEntry*>(d_entries), d_arena, nullptr, nullptr};
+    return split_json_sls_run(e, what, c, t, n, m, d_out, nullptr, out_cap, out_len, counters, nullptr);
+}
+
+int lc_split_json_parse_sls(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len, uint8_t split_char,
+                            SPLIT_JSON_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                            uint64_t counters[3]) {
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_json_sls_host(e, "lc_split_json_parse_sls", js, buf, len, split, SPLIT_JSON_ARGS, out, out_cap,
+                               out_len, n_events, counters, nullptr);
+}
+
+int lc_split_json_parse_sls_lz4(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                                uint8_t split_char, SPLIT_JSON_PARAMS, const uint8_t* tail, uint64_t tail_len,
+                                uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+                                uint64_t* n_events, uint64_t counters[3]) {
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_json_lz4_host(e, "lc_split_json_parse_sls_lz4", js, buf, len, split, SPLIT_JSON_ARGS, tail,
+                               tail_len, out, out_cap, out_len, raw_len, n_events, counters);
+}
+
+int lc_multiline_split_json_parse_sls(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                                      const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                      int discard_unmatched, SPLIT_JSON_PARAMS, uint8_t* out, uint64_t out_cap,
+                                      uint64_t* out_len, uint64_t* n_events, uint64_t counters[3],
+                                      uint64_t ml_counters[3]) {
+    return split_json_sls_host(e, "lc_multiline_split_json_parse_sls", js, buf, len, ML_SPLIT, SPLIT_JSON_ARGS, out,
+                               out_cap, out_len, n_events, counters, nullptr);
+}
+
+int lc_multiline_split_json_parse_sls_lz4(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                                          const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                          int discard_unmatched, SPLIT_JSON_PARAMS, const uint8_t* tail,
+                                          uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                                          uint64_t* raw_len, uint64_t* n_events, uint64_t counters[3],
+                                          uint64_t ml_counters[3]) {
+    return split_json_lz4_host(e, "lc_multiline_split_json_parse_sls_lz4", js, buf, len, ML_SPLIT, SPLIT_JSON_ARGS,
+                               tail, tail_len, out, out_cap, out_len, raw_len, n_events, counters);
+}
+
+} // extern "C"
+#undef ML_SPLIT
+#undef SPLIT_JSON_PARAMS
+#undef SPLIT_JSON_ARGS

@@ -5520,3 +5520,308 @@ LC_HD bool lc_json_emit(const uint8_t* base, uint32_t off, uint32_t len, const u
     const uint32_t r = lc_json_walk<SLOW, true>(base + off, len, skey, sklen, o);
     return r == LC_JSON_W_OK && !o.over && o.nent == ent_cap && o.narena == arena_cap;
 }
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, split -> JSON chain: the Log record of piece k that ProcessorSplitLogStringNative /
+// ProcessorSplitMultilineLogStringNative followed by ProcessorParseJsonNative (same SourceKey) leave behind, written
+// straight from the piece tables of the splitter and the tables of lc_json_parse_dev over those pieces.  The piece
+// enters the JSON stage as [SourceKey -> piece] or, with log.file.offset metadata, [SourceKey -> piece, offset_key ->
+// decimal(src_pos + off[k])], and AddLog overwrites in place, so the record of a parsed piece is: SourceKey (when a
+// member has it), the offset content, then every other distinct member key in order of its first occurrence, each
+// with the value of its last occurrence, then RenamedSourceKey unless that key is present.  The keys come from the
+// data, so a resolve pass finds, per event, which member emits and which value it takes (lc_json_resolve_*).
+#define LC_JSON_SLS_NONE 0xFFFFFFFFu
+#define LC_JSON_SLS_WARP 32u // events of at most this many members resolve in one warp, larger ones by sorting
+
+struct LcSplitJsonSlsCfg {
+    const uint8_t* skey; // SourceKey, RenamedSourceKey, the offset key and "__raw_log__" (device copies on the
+    const uint8_t* rkey; // device: a string literal here would add a module global and move the existing kernels'
+    const uint8_t* okey; // constant-bank address slots)
+    const uint8_t* raw;
+    uint32_t sklen, rklen, oklen;
+    uint32_t has_offset;
+    uint32_t keep_fail, keep_succeed, copy_raw;
+    uint32_t ren_is_off; // RenamedSourceKey == offset key (with offset metadata: always present)
+    uint32_t raw_is_off; // "__raw_log__" == offset key
+    uint32_t ren_is_raw; // RenamedSourceKey == "__raw_log__"
+    uint64_t src_pos;    // the source event's file offset
+    uint32_t time;       // the source event's time, as the split events inherit it
+    uint32_t has_ns, ns;
+};
+
+// What the resolve pass found about one event's members: the entry (index in the event) whose value SourceKey and the
+// offset key take (LC_JSON_SLS_NONE: no member has that key), and whether a member is keyed RenamedSourceKey.
+// "__raw_log__" is only added to failed pieces, which have no members, so it needs no flag.
+struct LcJsonSlsEv {
+    uint32_t src_win, off_win, has_ren;
+};
+
+// FNV-1a of a rendered key: the resolve compares keys only inside runs of equal hashes
+struct LcJsonKeyHash {
+    LC_HD uint32_t operator()(const uint8_t* p, uint32_t n) const {
+        uint32_t h = 2166136261u;
+        for (uint32_t i = 0; i < n; ++i)
+            h = (h ^ p[i]) * 16777619u;
+        return h;
+    }
+};
+
+// the bytes an entry offset names: the source, or (LC_JSON_ARENA) the arena
+LC_HD const uint8_t* lc_json_span(const uint8_t* src, const uint8_t* arena, uint32_t o) {
+    return o & LC_JSON_ARENA ? arena + (o & ~LC_JSON_ARENA) : src + o;
+}
+
+// <0, 0, >0: byte order, then length
+LC_HD int lc_json_key_cmp(const uint8_t* a, uint32_t al, const uint8_t* b, uint32_t bl) {
+    const uint32_t n = al < bl ? al : bl;
+    for (uint32_t i = 0; i < n; ++i)
+        if (a[i] != b[i])
+            return a[i] < b[i] ? -1 : 1;
+    return al == bl ? 0 : (al < bl ? -1 : 1);
+}
+
+// bit 0: SourceKey, bit 1: the offset key (with offset metadata), bit 2: RenamedSourceKey
+LC_HD uint32_t lc_json_sls_special(const LcSplitJsonSlsCfg& c, const uint8_t* k, uint32_t kl) {
+    return (lc_json_key_cmp(k, kl, c.skey, c.sklen) == 0 ? 1u : 0u) |
+           (c.has_offset && lc_json_key_cmp(k, kl, c.okey, c.oklen) == 0 ? 2u : 0u) |
+           (lc_json_key_cmp(k, kl, c.rkey, c.rklen) == 0 ? 4u : 0u);
+}
+
+// Per-warp workspace of lc_json_resolve_warp (shared memory on the device)
+struct LcJsonResolveWarp {
+    uint32_t h[32], lead[32], win[32], sp[32];
+};
+
+// Resolve one event of m <= 32 members e[0, m) in one warp, lane l holding member l: __match_any_sync on the key hash
+// gives each lane its candidates, and a byte compare with the earlier ones finds the first member of its key (its
+// leader); a second match on the leader gives the key's members, the last of which holds the value.  win[l] = that
+// last member at the leader of every key other than SourceKey and the offset key, else LC_JSON_SLS_NONE; *ev as
+// LcJsonSlsEv says.  Every lane calls it (the host runs the 32 lanes in turn, lc_lz4_peers standing in for the match).
+template <class H>
+LC_HD void lc_json_resolve_warp(const LcSplitJsonSlsCfg& c, const uint8_t* src, const uint8_t* arena,
+                                const LcJsonEntry* e, uint32_t m, uint32_t* win, LcJsonSlsEv* ev, LcJsonResolveWarp& w,
+                                uint32_t lane) {
+    const uint32_t W = 32;
+    (void)lane;
+    const uint32_t valid = lc_low_bits(m);
+    LC_LANES(l) {
+        w.h[l] = l < m ? H()(lc_json_span(src, arena, e[l].key_off), e[l].key_len) : 0u;
+    }
+    LC_WARP_SYNC();
+    LC_LANES(l) {
+        const uint32_t below = lc_lz4_peers(w.h, l, W) & valid & lc_low_bits(l);
+        uint32_t lead = l;
+        if (l < m) {
+            const uint8_t* k = lc_json_span(src, arena, e[l].key_off);
+            for (uint32_t b = below; b; b &= b - 1) {
+                const uint32_t j = lc_lo_bit(b);
+                if (lc_json_key_cmp(k, e[l].key_len, lc_json_span(src, arena, e[j].key_off), e[j].key_len) == 0) {
+                    lead = j;
+                    break;
+                }
+            }
+        }
+        w.lead[l] = lead;
+    }
+    LC_WARP_SYNC();
+    LC_LANES(l) {
+        const uint32_t grp = lc_lz4_peers(w.lead, l, W) & valid;
+        uint32_t wn = LC_JSON_SLS_NONE, sp = 0;
+        if (l < m && w.lead[l] == l) {
+            wn = lc_hi_bit(grp);
+            sp = lc_json_sls_special(c, lc_json_span(src, arena, e[l].key_off), e[l].key_len);
+        }
+        w.win[l] = wn;
+        w.sp[l] = sp;
+        if (l < m)
+            win[l] = sp & 3u ? LC_JSON_SLS_NONE : wn;
+    }
+    LC_WARP_SYNC();
+    LC_LANES(l) {
+        if (l == 0) {
+            LcJsonSlsEv r{LC_JSON_SLS_NONE, LC_JSON_SLS_NONE, 0u};
+            for (uint32_t j = 0; j < m; ++j) {
+                if (w.sp[j] & 1u)
+                    r.src_win = w.win[j];
+                if (w.sp[j] & 2u)
+                    r.off_win = w.win[j];
+                if (w.sp[j] & 4u)
+                    r.has_ren = 1u;
+            }
+            *ev = r;
+        }
+    }
+}
+
+// member x before member y: by key hash, then key bytes, then position
+LC_HD bool lc_json_resolve_less(const uint8_t* src, const uint8_t* arena, const LcJsonEntry* e, const uint32_t* h,
+                                uint32_t x, uint32_t y) {
+    if (h[x] != h[y])
+        return h[x] < h[y];
+    const int k = lc_json_key_cmp(lc_json_span(src, arena, e[x].key_off), e[x].key_len,
+                                  lc_json_span(src, arena, e[y].key_off), e[y].key_len);
+    return k ? k < 0 : x < y;
+}
+
+// Resolve one event of any member count in one thread, with the outputs of lc_json_resolve_warp: a bottom-up merge
+// sort of the member indices by (hash, key bytes, index) puts each key's members next to each other in document order,
+// so the first of a run is the leader and the last holds the value.  O(m log m) key comparisons whatever the hashes
+// (equal hashes only fall through to the byte compare); h, a, b: m words of scratch each.
+template <class H>
+LC_HD void lc_json_resolve_sort(const LcSplitJsonSlsCfg& c, const uint8_t* src, const uint8_t* arena,
+                                const LcJsonEntry* e, uint32_t m, uint32_t* win, LcJsonSlsEv* ev, uint32_t* h,
+                                uint32_t* a, uint32_t* b) {
+    for (uint32_t j = 0; j < m; ++j) {
+        h[j] = H()(lc_json_span(src, arena, e[j].key_off), e[j].key_len);
+        a[j] = j;
+    }
+    for (uint32_t run = 1; run < m; run *= 2) {
+        for (uint32_t lo = 0; lo < m; lo += 2 * run) {
+            const uint32_t mid = lo + run < m ? lo + run : m, hi = mid + run < m ? mid + run : m;
+            uint32_t p = lo, q = mid, o = lo;
+            while (p < mid && q < hi)
+                b[o++] = lc_json_resolve_less(src, arena, e, h, a[q], a[p]) ? a[q++] : a[p++];
+            while (p < mid)
+                b[o++] = a[p++];
+            while (q < hi)
+                b[o++] = a[q++];
+        }
+        uint32_t* t = a;
+        a = b;
+        b = t;
+    }
+    LcJsonSlsEv r{LC_JSON_SLS_NONE, LC_JSON_SLS_NONE, 0u};
+    for (uint32_t s = 0, t; s < m; s = t) {
+        const uint32_t lead = a[s];
+        const uint8_t* k = lc_json_span(src, arena, e[lead].key_off);
+        for (t = s + 1; t < m && h[a[t]] == h[lead] &&
+                        lc_json_key_cmp(lc_json_span(src, arena, e[a[t]].key_off), e[a[t]].key_len, k,
+                                        e[lead].key_len) == 0;
+             ++t)
+            win[a[t]] = LC_JSON_SLS_NONE;
+        const uint32_t wn = a[t - 1], sp = lc_json_sls_special(c, k, e[lead].key_len);
+        win[lead] = sp & 3u ? LC_JSON_SLS_NONE : wn;
+        if (sp & 1u)
+            r.src_win = wn;
+        if (sp & 2u)
+            r.off_win = wn;
+        if (sp & 4u)
+            r.has_ren = 1u;
+    }
+    *ev = r;
+}
+
+// One piece: src[po, + plen), its JSON status, its m entries e (offsets into src or the arena), the resolve's win[m]
+// and event record.
+struct LcSplitJsonSlsRow {
+    uint32_t po, plen;
+    uint32_t status;
+    const LcJsonEntry* e;
+    const uint32_t* win;
+    uint32_t m;
+    LcJsonSlsEv ev;
+};
+
+// The body of the piece's Log record -- Time, its contents, Time_ns -- into sink s (LcSlsCount64 / LcSlsWrite), with
+// the source event's time and ns.  Returns the number of contents; 0 = erased or empty, no record.
+template <class S>
+LC_HD uint32_t lc_split_json_sls_body(const LcSplitJsonSlsCfg& c, const uint8_t* src, const uint8_t* arena,
+                                      const LcSplitJsonSlsRow& r, S& s) {
+    {
+        uint8_t h[6];
+        h[0] = 0x08;
+        const uint32_t n = 1 + lc_put_varint(h + 1, c.time < (1u << 28) ? (1u << 28) : c.time); // always 5 bytes
+        s.put(h, n);
+    }
+    const uint64_t pos = c.src_pos + r.po;
+    const uint32_t nd = lc_dec_digits(pos);
+    uint32_t k = 0;
+    auto member = [&](const uint8_t* key, uint32_t kl, const LcJsonEntry& v) {
+        lc_sls_pair_open(s, key, kl, v.val_len);
+        s.copy(lc_json_span(src, arena, v.val_off), v.val_len);
+        ++k;
+    };
+    auto digits = [&]() {
+        lc_sls_pair_open(s, c.okey, c.oklen, nd);
+        lc_sls_digits(s, pos, nd);
+        ++k;
+    };
+    auto piece = [&](const uint8_t* key, uint32_t kl) {
+        lc_sls_pair_open(s, key, kl, r.plen);
+        s.copy(src + r.po, r.plen);
+        ++k;
+    };
+    if ((r.status & 0x7Fu) == LC_JSON_ST_OK) {
+        if (r.ev.src_win != LC_JSON_SLS_NONE)
+            member(c.skey, c.sklen, r.e[r.ev.src_win]);
+        if (c.has_offset) {
+            if (r.ev.off_win != LC_JSON_SLS_NONE)
+                member(c.okey, c.oklen, r.e[r.ev.off_win]);
+            else
+                digits();
+        }
+        for (uint32_t j = 0; j < r.m; ++j)
+            if (r.win[j] != LC_JSON_SLS_NONE)
+                member(lc_json_span(src, arena, r.e[j].key_off), r.e[j].key_len, r.e[r.win[j]]);
+        if (c.keep_succeed && !r.ev.has_ren && !(c.has_offset && c.ren_is_off))
+            piece(c.rkey, c.rklen);
+    } else {
+        if (!c.keep_fail)
+            return 0u; // ShouldEraseEvent: nothing but the offset content is left
+        if (c.has_offset)
+            digits();
+        if (!(c.has_offset && c.ren_is_off))
+            piece(c.rkey, c.rklen);
+        if (c.copy_raw && !(c.has_offset && c.raw_is_off) && !c.ren_is_raw)
+            piece(c.raw, 11u);
+    }
+    if (c.has_ns) {
+        const uint8_t h[5] = {0x25, (uint8_t)c.ns, (uint8_t)(c.ns >> 8), (uint8_t)(c.ns >> 16), (uint8_t)(c.ns >> 24)};
+        s.put(h, 5);
+    }
+    return k;
+}
+
+// The piece's counter verdicts (0 / 1): ProcessorParseJsonNative's out_successful (every piece not erased),
+// out_failed (LC_JSON_FAILED only) and discarded.  A split event always holds SourceKey, so no key-not-found.
+LC_HD LcSplitRegexVerdict lc_split_json_verdict(const LcSplitJsonSlsCfg& c, uint32_t status) {
+    const uint32_t st = status & 0x7Fu, kept = st == LC_JSON_ST_OK || c.keep_fail;
+    return {kept, st == LC_JSON_ST_FAILED ? 1u : 0u, kept ? 0u : 1u};
+}
+
+// Host side: the configuration of the chain, with the key pointers as given and `raw` at a host "__raw_log__" (the
+// device caller points them at its copies).
+// offset_key == nullptr: no log.file.offset metadata.  Returns nullptr, or why the chain is refused: an offset key
+// equal to SourceKey (the split would replace the piece by its digits, and the JSON stage would parse those).
+inline const char* lc_split_json_sls_setup(const char* source_key, uint32_t source_len, const char* renamed_key,
+                                           uint32_t renamed_len, const char* offset_key, uint32_t offset_len,
+                                           int keep_fail, int keep_succeed, int copy_raw, uint64_t src_pos,
+                                           uint32_t time, uint32_t time_ns, LcSplitJsonSlsCfg* c) {
+    auto eq = [](const char* a, uint32_t al, const char* b, uint32_t bl) {
+        return al == bl && (al == 0 || !memcmp(a, b, al));
+    };
+    if (!c)
+        return "bad arguments";
+    if (offset_key && eq(offset_key, offset_len, source_key, source_len))
+        return "the offset key equals SourceKey";
+    memset(c, 0, sizeof *c);
+    c->skey = reinterpret_cast<const uint8_t*>(source_key);
+    c->rkey = reinterpret_cast<const uint8_t*>(renamed_key);
+    c->okey = reinterpret_cast<const uint8_t*>(offset_key);
+    c->raw = reinterpret_cast<const uint8_t*>("__raw_log__");
+    c->sklen = source_len;
+    c->rklen = renamed_len;
+    c->oklen = offset_key ? offset_len : 0u;
+    c->has_offset = offset_key != nullptr;
+    c->keep_fail = keep_fail != 0;
+    c->keep_succeed = keep_succeed != 0;
+    c->copy_raw = copy_raw != 0;
+    c->ren_is_off = offset_key && eq(renamed_key, renamed_len, offset_key, offset_len);
+    c->raw_is_off = offset_key && eq("__raw_log__", 11, offset_key, offset_len);
+    c->ren_is_raw = eq(renamed_key, renamed_len, "__raw_log__", 11);
+    c->src_pos = src_pos;
+    c->time = time;
+    c->has_ns = time_ns != 0xFFFFFFFFu;
+    c->ns = c->has_ns ? time_ns : 0u;
+    return nullptr;
+}

@@ -4710,4 +4710,131 @@ void launch_json_emit_slow(const uint8_t* d_base, const uint32_t* d_off, const u
                                                            d_nslow, d_first, d_afirst, d_entries, d_arena, d_bad);
 }
 
+// ---- f4, split -> JSON chain (lc_exec.cuh: lc_json_resolve_*, lc_split_json_sls_body).  The resolve pass runs one warp
+// per piece; a parsed piece of more than LC_JSON_SLS_WARP members goes to the list, which json_resolve_sort_kernel
+// takes one thread per piece over a fixed grid.  The size pass runs one thread per piece, the emit pass one warp per
+// piece.  counters: u64 [4] += successful, failed, discarded, pieces whose record would reach 4 GiB.
+__device__ __forceinline__ uint32_t split_json_members(const SplitJsonSlsTables& t, uint64_t i) {
+    return (t.status[i] & 0x7Fu) == LC_JSON_ST_OK ? (uint32_t)(t.first[i + 1] - t.first[i]) : 0u;
+}
+
+__global__ void __launch_bounds__(256)
+    json_resolve_warp_kernel(LcSplitJsonSlsCfg c, SplitJsonSlsTables t, uint64_t n, uint32_t* __restrict__ list,
+                             uint32_t* nlist) {
+    __shared__ LcJsonResolveWarp ws[8];
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (i >= n)
+        return;
+    const uint32_t m = split_json_members(t, i);
+    if (m > LC_JSON_SLS_WARP) {
+        if (lane == 0)
+            list[atomicAdd(nlist, 1u)] = (uint32_t)i;
+        return;
+    }
+    const uint64_t f = t.first[i];
+    lc_json_resolve_warp<LcJsonKeyHash>(c, t.src, t.arena, t.ent + f, m, t.win + f, t.ev + i, ws[threadIdx.x >> 5],
+                                        lane);
+}
+
+__global__ void __launch_bounds__(128)
+    json_resolve_sort_kernel(LcSplitJsonSlsCfg c, SplitJsonSlsTables t, const uint32_t* __restrict__ list,
+                             const uint32_t* __restrict__ nlist, uint32_t* __restrict__ scratch, uint64_t n_entries) {
+    const uint32_t cnt = *nlist;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < cnt; j += gridDim.x * blockDim.x) {
+        const uint32_t i = list[j];
+        const uint64_t f = t.first[i];
+        lc_json_resolve_sort<LcJsonKeyHash>(c, t.src, t.arena, t.ent + f, split_json_members(t, i), t.win + f,
+                                            t.ev + i, scratch + f, scratch + n_entries + f,
+                                            scratch + 2 * n_entries + f);
+    }
+}
+
+__device__ __forceinline__ LcSplitJsonSlsRow split_json_sls_row(const SplitJsonSlsTables& t, uint64_t i) {
+    LcSplitJsonSlsRow r;
+    const uint64_t f = t.first[i];
+    r.po = t.off[i];
+    r.plen = t.len[i];
+    r.status = t.status[i];
+    r.e = t.ent + f;
+    r.win = t.win + f;
+    r.m = split_json_members(t, i);
+    r.ev = t.ev[i];
+    return r;
+}
+
+__global__ void __launch_bounds__(256)
+    split_json_sls_size_kernel(LcSplitJsonSlsCfg c, SplitJsonSlsTables t, uint64_t n, uint32_t* __restrict__ rec_size,
+                               uint32_t* __restrict__ body_size, unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    LcSplitRegexVerdict v{0u, 0u, 0u};
+    uint32_t big = 0;
+    if (i < n) {
+        const LcSplitJsonSlsRow r = split_json_sls_row(t, i);
+        LcSlsCount64 s{0};
+        const uint32_t cnt = lc_split_json_sls_body(c, t.src, t.arena, r, s);
+        big = s.n + 16 > 0xFFFFFFFFull;
+        const uint32_t body = cnt && !big ? (uint32_t)s.n : 0u;
+        rec_size[i] = body ? 1 + lc_varint_size(body) + body : 0u;
+        body_size[i] = body;
+        v = lc_split_json_verdict(c, r.status);
+    }
+    const uint32_t ok = __reduce_add_sync(0xFFFFFFFFu, v.ok), failed = __reduce_add_sync(0xFFFFFFFFu, v.failed),
+                   erased = __reduce_add_sync(0xFFFFFFFFu, v.erased);
+    big = __reduce_add_sync(0xFFFFFFFFu, big);
+    if ((threadIdx.x & 31) == 0) {
+        if (ok)
+            atomicAdd(counters + 0, (unsigned long long)ok);
+        if (failed)
+            atomicAdd(counters + 1, (unsigned long long)failed);
+        if (erased)
+            atomicAdd(counters + 2, (unsigned long long)erased);
+        if (big)
+            atomicAdd(counters + 3, (unsigned long long)big);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    split_json_sls_emit_kernel(LcSplitJsonSlsCfg c, SplitJsonSlsTables t, uint64_t n,
+                               const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ body_size,
+                               uint8_t* __restrict__ out) {
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n)
+        return;
+    const uint32_t body = body_size[i];
+    if (!body)
+        return; // erased or LogEvent::Empty: no record
+    const LcSplitJsonSlsRow r = split_json_sls_row(t, i);
+    uint8_t h[6];
+    h[0] = 0x0A;
+    const uint32_t hn = 1 + lc_put_varint(h + 1, body);
+    LcSlsWrite s{out + rec_off[i], 0u, hn + body, threadIdx.x & 31, 32};
+    s.put(h, hn);
+    lc_split_json_sls_body(c, t.src, t.arena, r, s);
+}
+
+void launch_json_resolve(const LcSplitJsonSlsCfg& c, const SplitJsonSlsTables& t, uint64_t n, uint64_t n_entries,
+                         uint32_t* d_list, uint32_t* d_nlist, uint32_t* d_scratch, cudaStream_t st) {
+    if (!n)
+        return;
+    json_resolve_warp_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, t, n, d_list, d_nlist);
+    json_resolve_sort_kernel<<<kJsonSlowBlocks, 128, 0, st>>>(c, t, d_list, d_nlist, d_scratch, n_entries);
+}
+
+void launch_split_json_sls_sizes(const LcSplitJsonSlsCfg& c, const SplitJsonSlsTables& t, uint64_t n,
+                                 uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                 cudaStream_t st) {
+    if (n)
+        split_json_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_size, d_body_size,
+                                                                                 d_counters);
+}
+
+void launch_split_json_sls_emit(const LcSplitJsonSlsCfg& c, const SplitJsonSlsTables& t, uint64_t n,
+                                const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                cudaStream_t st) {
+    if (n)
+        split_json_sls_emit_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_off, d_body_size,
+                                                                                      d_out);
+}
+
 } // namespace lck

@@ -21,6 +21,8 @@ struct LcTsFull;
 struct LcApEv;
 struct LcApEntry;
 struct LcJsonEntry;
+struct LcSplitJsonSlsCfg;
+struct LcJsonSlsEv;
 struct LcLz4Chunk;
 
 namespace lck {
@@ -426,5 +428,31 @@ void launch_json_emit_slow(const uint8_t* d_base, const uint32_t* d_off, const u
                            const uint32_t* d_slow_list, const uint32_t* d_nslow, const uint64_t* d_first,
                            const uint64_t* d_afirst, LcJsonEntry* d_entries, uint8_t* d_arena, uint32_t* d_bad,
                            cudaStream_t st);
+
+// f4, split -> JSON chain (lc_exec.cuh: LcSplitJsonSlsCfg, keys on the device): the pieces off / len of the source
+// value src, parsed by lc_json_parse_dev into status / first / ent / arena; win (one word per entry) and ev (one record
+// per piece) are the resolve pass's output.  launch_json_resolve: d_list / d_nlist take the pieces of more than
+// LC_JSON_SLS_WARP members (*d_nlist zeroed by the caller), d_scratch 3 * n_entries words.  Sizes as for
+// launch_sls_sizes; d_counters: u64 [4] += successful, failed (LC_JSON_FAILED), discarded pieces, and pieces whose
+// record would reach 4 GiB.
+struct SplitJsonSlsTables {
+    const uint8_t* src;
+    const uint32_t* off;
+    const uint32_t* len;
+    const uint8_t* status;
+    const uint64_t* first;
+    const LcJsonEntry* ent;
+    const uint8_t* arena;
+    uint32_t* win;
+    LcJsonSlsEv* ev;
+};
+void launch_json_resolve(const LcSplitJsonSlsCfg& c, const SplitJsonSlsTables& t, uint64_t n, uint64_t n_entries,
+                         uint32_t* d_list, uint32_t* d_nlist, uint32_t* d_scratch, cudaStream_t st);
+void launch_split_json_sls_sizes(const LcSplitJsonSlsCfg& c, const SplitJsonSlsTables& t, uint64_t n,
+                                 uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                 cudaStream_t st);
+void launch_split_json_sls_emit(const LcSplitJsonSlsCfg& c, const SplitJsonSlsTables& t, uint64_t n,
+                                const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                cudaStream_t st);
 
 } // namespace lck

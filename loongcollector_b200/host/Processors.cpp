@@ -3733,4 +3733,136 @@ Processor* CreateProcessor(const std::string& type) {
     return nullptr;
 }
 
+// ------------------------------------------------------------------------------------------------ split -> JSON
+// The JSON stage of the split -> JSON chain: a ProcessorParseJsonNative's configuration as the chain calls take it,
+// the host check of lc_split_json_sls_setup, and the counters Process would move.
+struct SplitJsonStage {
+    ProcessorParseJsonNative& j;
+    const std::string& Renamed() const { return j.mCommonParserOptions.mRenamedSourceKey; }
+    const CommonParserOptions& Opt() const { return j.mCommonParserOptions; }
+    const lc_json_t* Program() const { return j.mProgram; }
+    // whether the chain's device calls take this stage behind a splitter reading sourceKey
+    bool Accepts(const std::string& sourceKey, const StringView* okey) const {
+        LcSplitJsonSlsCfg c;
+        return j.mProgram && j.mSourceKey == sourceKey &&
+               !lc_split_json_sls_setup(j.mSourceKey.data(), (uint32_t)j.mSourceKey.size(), Renamed().data(),
+                                        (uint32_t)Renamed().size(), okey ? okey->data() : nullptr,
+                                        okey ? (uint32_t)okey->size() : 0u, Opt().mKeepingSourceWhenParseFail,
+                                        Opt().mKeepingSourceWhenParseSucceed, Opt().mCopingRawLog, 0, 0, LC_SLS_NO_NS,
+                                        &c);
+    }
+    // the device calls' counters[3] (successful, failed, discarded) as the chain driver takes a stage's, with none
+    // removed by a filter
+    static void Fold(const uint64_t c3[3], uint64_t rctr[4]) {
+        rctr[0] = c3[0];
+        rctr[1] = c3[1];
+        rctr[2] = c3[2];
+        rctr[3] = 0;
+    }
+    void Add(const uint64_t ctr[3]) const {
+        j.mOutSuccessfulEventsTotal.Add(ctr[0]);
+        j.mOutFailedEventsTotal.Add(ctr[1]);
+        j.mDiscardedEventsTotal.Add(ctr[2]);
+    }
+    void Process(PipelineEventGroup& group) const { j.Process(group); }
+};
+#define SPLIT_JSON_STAGE_ARGS(x)                                                                                       \
+    (x).Program(), src(val), val.size()
+#define SPLIT_JSON_STAGE_OPTS(x)                                                                                       \
+    (x).Renamed().data(), (uint32_t)(x).Renamed().size(), (x).Opt().mKeepingSourceWhenParseFail,                      \
+        (x).Opt().mKeepingSourceWhenParseSucceed, (x).Opt().mCopingRawLog, okey ? okey->data() : nullptr,            \
+        okey ? (uint32_t)okey->size() : 0u, pos, time, ns
+
+bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next,
+                                                 bool enableNs, std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseJsonNative& next,
+                                                    bool enableNs, std::string& block, uint64_t& rawSize,
+                                                    std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitLogStringNative::ChainSerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next,
+                                                      bool enableNs, std::string& out, uint64_t* rawSize,
+                                                      std::string& err) {
+    const SplitJsonStage x{next};
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c3[3] = {0, 0, 0};
+        const int rc = lc_split_json_parse_sls(Engine(), SPLIT_JSON_STAGE_ARGS(x), (uint8_t)mSplitChar,
+                                               SPLIT_JSON_STAGE_OPTS(x), o, cap, len, nev, c3);
+        SplitJsonStage::Fold(c3, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c3[3] = {0, 0, 0};
+        const int rc = lc_split_json_parse_sls_lz4(Engine(), SPLIT_JSON_STAGE_ARGS(x), (uint8_t)mSplitChar,
+                                                   SPLIT_JSON_STAGE_OPTS(x), tail, tailLen, o, cap, len, raw, nev,
+                                                   c3);
+        SplitJsonStage::Fold(c3, rctr);
+        return rc;
+    };
+    uint64_t unused[3] = {0, 0, 0};
+    return SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_split_json_parse_sls", "lc_split_json_parse_sls_lz4",
+        unused);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next,
+                                                          bool enableNs, std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseJsonNative& next,
+                                                             bool enableNs, std::string& block, uint64_t& rawSize,
+                                                             std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGroup& group,
+                                                               ProcessorParseJsonNative& next, bool enableNs,
+                                                               std::string& out, uint64_t* rawSize, std::string& err) {
+    const SplitJsonStage x{next};
+    const bool discard = mMultiline.mUnmatchedContentTreatment == MultilineOptions::UnmatchedContentTreatment::DISCARD;
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c3[3] = {0, 0, 0};
+        const int rc = lc_multiline_split_json_parse_sls(Engine(), SPLIT_JSON_STAGE_ARGS(x), mStart.get(),
+                                                         mContinue.get(), mEnd.get(), discard,
+                                                         SPLIT_JSON_STAGE_OPTS(x), o, cap, len, nev, c3, sctr);
+        SplitJsonStage::Fold(c3, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c3[3] = {0, 0, 0};
+        const int rc = lc_multiline_split_json_parse_sls_lz4(Engine(), SPLIT_JSON_STAGE_ARGS(x), mStart.get(),
+                                                             mContinue.get(), mEnd.get(), discard,
+                                                             SPLIT_JSON_STAGE_OPTS(x), tail, tailLen, o, cap, len, raw,
+                                                             nev, c3, sctr);
+        SplitJsonStage::Fold(c3, rctr);
+        return rc;
+    };
+    // matched_events, input lines, unmatched lines: moved as Process moves them (:82-84,106-107)
+    uint64_t ctr[3] = {0, 0, 0};
+    const bool ok = SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_multiline_split_json_parse_sls",
+        "lc_multiline_split_json_parse_sls_lz4", ctr);
+    mMatchedEventsTotal.Add(ctr[0]);
+    mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
+    mUnmatchedLinesTotal.Add(ctr[2]);
+    return ok;
+}
+#undef SPLIT_JSON_STAGE_ARGS
+#undef SPLIT_JSON_STAGE_OPTS
+
 } // namespace logtail

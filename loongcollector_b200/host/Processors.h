@@ -192,10 +192,24 @@ public:
                          ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& block,
                          uint64_t& rawSize, std::string& err);
 
+    // The split -> JSON chain: Process(group), then next.Process(group) (next: the processor_parse_json_native behind
+    // this one, reading SourceKey), then SLSEventGroupSerializer::Serialize: the same bytes or error message, and the
+    // same counter updates on both processors.  On a flat group without EnableRawContent, whose JSON SourceKey is this
+    // SourceKey and whose configuration lc_split_json_parse_sls accepts, each source event is split, parsed and
+    // serialised in one device pass (log.file.offset metadata included) and only the wire bytes come back; the
+    // group's events are left as they were.  Otherwise the three calls run.
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& out,
+                      std::string& err);
+    // The same followed by LZ4Compressor::Compress.  A device-path group of one source event is compressed on the
+    // device (lc_split_json_parse_sls_lz4); other groups compress SerializeSls's bytes.
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& block,
+                         uint64_t& rawSize, std::string& err);
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& out,
+                           uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative* filter,
                            bool enableNs, std::string& out, uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
@@ -256,10 +270,17 @@ public:
                          uint64_t& rawSize, std::string& err);
     Counter mMatchedEventsTotal, mMatchedLinesTotal, mUnmatchedLinesTotal;
 
+    // The split -> JSON chain, as ProcessorSplitLogStringNative's (lc_multiline_split_json_parse_sls[_lz4]).
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& out,
+                      std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& block,
+                         uint64_t& rawSize, std::string& err);
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& out,
+                           uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative* filter,
                            bool enableNs, std::string& out, uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
@@ -482,6 +503,7 @@ protected:
 private:
     void ProcessBatch(std::vector<PipelineEventGroup>& groups, size_t g0, size_t g1);
     lc_json_t* mProgram = nullptr;
+    friend struct SplitJsonStage; // the split -> JSON chain's SerializeSls
 };
 
 class ProcessorFilterNative : public Processor {

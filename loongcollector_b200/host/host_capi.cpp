@@ -291,10 +291,11 @@ char* lc_host_chain_serialize_sls(lc_host_processor_t* delim, lc_host_processor_
         auto* ps = dynamic_cast<ProcessorSplitLogStringNative*>(d);
         auto* pm = dynamic_cast<ProcessorSplitMultilineLogStringNative*>(d);
         auto* sd = (ps || pm) ? dynamic_cast<ProcessorParseDelimiterNative*>(second) : nullptr;
-        if (!((pd || ps || pm) && r) && !sd)
+        auto* sj = (ps || pm) ? dynamic_cast<ProcessorParseJsonNative*>(second) : nullptr;
+        if (!((pd || ps || pm) && r) && !sd && !sj)
             throw std::runtime_error("not a processor_parse_delimiter_native or a splitter, and a "
                                      "processor_parse_regex_native; nor a splitter and a "
-                                     "processor_parse_delimiter_native");
+                                     "processor_parse_delimiter_native or processor_parse_json_native");
         // the chain's SerializeSls / SerializeSlsLz4 on whichever processor comes first, with the second as next
         auto chain = [&](auto* p, auto& next, PipelineEventGroup& g, std::string& res, uint64_t& raw,
                          std::string& err) {
@@ -322,7 +323,9 @@ char* lc_host_chain_serialize_sls(lc_host_processor_t* delim, lc_host_processor_
             ser.mEnableTimestampNanosecond = enable_ns != 0;
             ok = ser.Serialize(group, res, err);
         } else {
-            ok = r ? first(*r, group, res, raw, err) : first(*sd, group, res, raw, err);
+            ok = r    ? first(*r, group, res, raw, err)
+                 : sd ? first(*sd, group, res, raw, err)
+                      : first(*sj, group, res, raw, err);
         }
         if (d->EngineErrors() + second->EngineErrors() != errs)
             throw std::runtime_error("engine error inside Process: " + d->LastError() + second->LastError());
