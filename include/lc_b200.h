@@ -1158,6 +1158,85 @@ int lc_multiline_split_json_parse_sls_lz4(lc_engine_t* e, const lc_json_t* js, c
                                           uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
                                           uint64_t counters[3], uint64_t ml_counters[3]);
 
+/* ---- f4: the split -> Apsara chain (ProcessorSplitLogStringNative or ProcessorSplitMultilineLogStringNative, then
+ * ProcessorParseApsaraNative with the same SourceKey -- input_file, processor_parse_apsara_native, a flusher) to the
+ * SLS wire format.  The source event is flat, as for the split -> JSON chain: SourceKey (ap's) -> the value, with its
+ * position src_pos, time and time_ns (LC_SLS_NO_NS = no Time_ns).  Piece k enters the Apsara stage as [SourceKey ->
+ * piece] or, when offset_key != NULL, [SourceKey -> piece, offset_key -> decimal(src_pos + off[k])], and the stage does
+ * what ProcessorParseApsaraNative::ProcessEvent does (oracle/apsara.py restates it) with the time cache over the
+ * pieces in order, the chunk as lc_apsara_parse_dev's base.  AppendContentNoCopy never removes a duplicate, so every
+ * field is appended, duplicates included.
+ *   A piece that parses (LC_APSARA_OK): its own time and, with enable_ns, Time_ns = its nanoseconds; contents in this
+ *   order: the piece (key SourceKey); the offset content; the base fields as found (__LEVEL__, __THREAD__, __FILE__,
+ *   __LINE__); the key:value fields in order, duplicates kept, keys equal to the offset key, a base-field name or
+ *   "microtime" included; "microtime" -> the "%ld" digits of logTime_in_micro.  Then DelContent(SourceKey) removes
+ *   the NEWEST entry keyed SourceKey -- "microtime" when SourceKey is "microtime", else the base field of that name
+ *   when there is one, else the piece -- unless a key:value key equals SourceKey (LC_APSARA_OVERWRITTEN: every
+ *   SourceKey entry stays).  With keep_succeed, renamed_key -> piece unless a content left has that key.
+ *   An empty piece (LC_APSARA_EMPTY): kept untouched, [SourceKey -> "", the offset content], the source event's time.
+ *   A piece that fails (LC_APSARA_FAILED): SourceKey is deleted and the offset content stays; with keep_fail,
+ *   renamed_key -> piece, and with copy_raw as well "__raw_log__" -> piece, neither added when already present;
+ *   without keep_fail the piece is erased (ShouldEraseEvent: nothing but the offset content is left).  The source
+ *   event's time and time_ns.
+ *   A piece too old for discard_interval (LC_APSARA_DISCARDED) is erased.
+ *   renamed_key is the effective RenamedSourceKey (SourceKey when the configuration leaves it empty).
+ * counters[5] (may be NULL) in lc_apsara_parse's order: key_not_found (0: a piece always holds SourceKey), out_failed
+ * (empty and failed pieces), history_failure, discarded (the too-old pieces and the failed pieces erased), and
+ * out_successful -- the counters ProcessorParseApsaraNative::Process moves.  Refused with LC_ERR_INVALID_ARG: an
+ * offset_key equal to SourceKey, a time_ns other than LC_SLS_NO_NS without enable_ns (the kept pieces would write
+ * Time_ns and the parsed ones not), bad arguments.  LC_ERR_TOO_LARGE: src_len >= 0xFFFFFFF0 (lc_apsara_parse_dev's
+ * offsets stay below its LC_APSARA_KEY_* tags), n >= 2^30, or a record that would reach 4 GiB.
+ *
+ * lc_sls_serialize_split_apsara_dev: from the DEVICE piece tables of one lc_split_lines_dev / lc_multiline_split_dev
+ * call over d_src[0, src_len) and the DEVICE tables of lc_apsara_parse_dev over those pieces with ap, d_src as base
+ * and one group (d_status, d_sec, d_nsec, d_micro, d_first, d_entries).  d_out receives the bytes; *out_len (host)
+ * their count; LC_ERR_CAPACITY if > out_cap (nothing written, *out_len and counters set). */
+int lc_sls_serialize_split_apsara_dev(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* d_src, uint64_t src_len,
+                                      const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+                                      const uint8_t* d_status, const int64_t* d_sec, const uint32_t* d_nsec,
+                                      const int64_t* d_micro, const uint64_t* d_first,
+                                      const lc_apsara_entry_t* d_entries, const char* renamed_key,
+                                      uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+                                      const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+                                      uint32_t time_ns, int enable_ns, uint8_t* d_out, uint64_t out_cap,
+                                      uint64_t* out_len, uint64_t counters[5]);
+
+/* The same with a HOST source value: upload it once, split it on the device, run lc_apsara_parse_dev's passes over the
+ * pieces (the chunk as one group; now = time(NULL) of the caller, discard_interval as for lc_apsara_parse, -1 = no
+ * history discard), serialise, and bring back only the wire bytes; *n_events, ml_counters, the _lz4 variants and which
+ * outputs are set on LC_ERR_CAPACITY as for lc_split_regex_parse_sls.  A chunk whose pieces are all erased gives 0
+ * bytes (the _lz4 calls then return the block of the tail alone). */
+int lc_split_apsara_parse_sls(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* buf, uint64_t len,
+                              uint8_t split_char, const char* renamed_key, uint32_t renamed_key_len, int keep_fail,
+                              int keep_succeed, int copy_raw, const char* offset_key, uint32_t offset_key_len,
+                              uint64_t src_pos, uint32_t time, uint32_t time_ns, int enable_ns, int64_t now,
+                              int32_t discard_interval, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                              uint64_t* n_events, uint64_t counters[5]);
+int lc_split_apsara_parse_sls_lz4(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* buf, uint64_t len,
+                                  uint8_t split_char, const char* renamed_key, uint32_t renamed_key_len, int keep_fail,
+                                  int keep_succeed, int copy_raw, const char* offset_key, uint32_t offset_key_len,
+                                  uint64_t src_pos, uint32_t time, uint32_t time_ns, int enable_ns, int64_t now,
+                                  int32_t discard_interval, const uint8_t* tail, uint64_t tail_len, uint8_t* out,
+                                  uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                                  uint64_t counters[5]);
+int lc_multiline_split_apsara_parse_sls(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* buf, uint64_t len,
+                                        const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                        int discard_unmatched, const char* renamed_key, uint32_t renamed_key_len,
+                                        int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+                                        uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                        int enable_ns, int64_t now, int32_t discard_interval, uint8_t* out,
+                                        uint64_t out_cap, uint64_t* out_len, uint64_t* n_events, uint64_t counters[5],
+                                        uint64_t ml_counters[3]);
+int lc_multiline_split_apsara_parse_sls_lz4(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* buf, uint64_t len,
+                                            const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                            int discard_unmatched, const char* renamed_key, uint32_t renamed_key_len,
+                                            int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+                                            uint32_t offset_key_len, uint64_t src_pos, uint32_t time,
+                                            uint32_t time_ns, int enable_ns, int64_t now, int32_t discard_interval,
+                                            const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+                                            uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                                            uint64_t counters[5], uint64_t ml_counters[3]);
+
 #ifdef __cplusplus
 }
 #endif

@@ -62,9 +62,9 @@ char* lc_host_processor_serialize_sls_lz4(lc_host_processor_t* p, const char* gr
 /* The delimiter -> regex, split -> regex or split -> delimiter chain of a pipeline on the group described by
  * group_json: delim (a "processor_parse_delimiter_native", "processor_split_string_native" or
  * "processor_split_multiline_log_string_native") followed by regex (a "processor_parse_regex_native" reading one of
- * delim's keys, or the splitter's SourceKey; behind a splitter, also a "processor_parse_delimiter_native" or a
- * "processor_parse_json_native" reading its SourceKey).  mode 0: delim's SerializeSls(group, regex); mode 1: Process + Process +
- * SLSEventGroupSerializer::Serialize on the same in-memory group (the result mode 0 must equal byte for byte); mode 2:
+ * delim's keys, or the splitter's SourceKey; behind a splitter, also a "processor_parse_delimiter_native", a
+ * "processor_parse_json_native" or a "processor_parse_apsara_native" reading its SourceKey).  mode 0: delim's
+ * SerializeSls(group, regex); mode 1: Process + Process + SLSEventGroupSerializer::Serialize on the same in-memory group (the result mode 0 must equal byte for byte); mode 2:
  * SerializeSlsLz4(group, regex), the LZ4 block with *raw_len_out = the size it decompresses to.  Returns the malloc'd
  * bytes and their length, or NULL + *err_out = the serializer's error message; NULL + *fail_out on an engine failure or
  * a bad group. */

@@ -139,6 +139,18 @@ def lib():
         [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
     L.lc_multiline_split_json_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sj_cfg + \
         [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
+    sa_cfg = [C.c_char_p, u32, i32, i32, i32] + sr_tail + [i32]  # renamed_key .. enable_ns of the split -> Apsara chain
+    sa_now = [C.c_int64, i32]  # now, discard_interval
+    L.lc_sls_serialize_split_apsara_dev.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, vp, vp] + sa_cfg + \
+        [vp, u64, C.POINTER(u64), vp]
+    L.lc_split_apsara_parse_sls.argtypes = [vp, vp, vp, u64, u8] + sa_cfg + sa_now + \
+        [vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_split_apsara_parse_sls_lz4.argtypes = [vp, vp, vp, u64, u8] + sa_cfg + sa_now + \
+        [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_multiline_split_apsara_parse_sls.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sa_cfg + sa_now + \
+        [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
+    L.lc_multiline_split_apsara_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sa_cfg + sa_now + \
+        [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
     L.lc_sls_serialize_split_regex_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, u32] + sls_cfg + [i32] + \
         sr_tail + [vp, u64, C.POINTER(u64), vp]
     L.lc_split_regex_parse_sls.argtypes = [vp, vp, vp, u64, u8] + sls_cfg + [i32] + sr_tail + \
@@ -1537,6 +1549,99 @@ class Engine:
         return self._split_json(
             lib().lc_multiline_split_json_parse_sls_lz4, js, buf, [_rh(start), _rh(cont), _rh(end), int(bool(discard))],
             renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos, time, time_ns, out_cap, True, tail)
+
+    def _sa_cfg(self, renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos, time, time_ns, enable_ns):
+        r = renamed_key or b""
+        return [r, len(r), int(bool(keep_fail)), int(bool(keep_succeed)), int(bool(copy_raw))] + \
+            self._sr_tail(offset_key, src_pos, time, time_ns) + [int(bool(enable_ns))]
+
+    def sls_serialize_split_apsara_dev(self, ap, d_src, src_len, d_off, d_len, n, d_status, d_sec, d_nsec, d_micro,
+                                       d_first, d_entries, renamed_key, keep_fail=False, keep_succeed=False,
+                                       copy_raw=False, offset_key=None, src_pos=0, time=0, time_ns=None,
+                                       enable_ns=False, d_out=None, out_cap=0):
+        """Wire bytes of the split -> Apsara chain from the device piece tables of one split_lines_dev /
+        multiline_split_dev call and the device tables of apsara_parse_dev over those pieces with ap, d_src as base and
+        one group (lc_sls_serialize_split_apsara_dev); renamed_key is the effective RenamedSourceKey.  Returns (byte
+        count written to d_out, counters[5] in lc_apsara_parse's order); with d_out None the byte count needed."""
+        need = C.c_uint64(0)
+        ctr = np.zeros(5, np.uint64)
+        rc = lib().lc_sls_serialize_split_apsara_dev(
+            self._h, ap._h, _p(d_src), src_len, _p(d_off), _p(d_len), n, _p(d_status), _p(d_sec), _p(d_nsec),
+            _p(d_micro), _p(d_first), _p(d_entries),
+            *self._sa_cfg(renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos, time, time_ns,
+                          enable_ns), _p(d_out), out_cap, C.byref(need), _p(ctr))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value), ctr  # a sizing query
+        _check(rc)
+        return int(need.value), ctr
+
+    def _split_apsara(self, fn, ap, buf, extra, renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos,
+                      time, time_ns, enable_ns, now, discard_interval, out_cap, ml, tail):
+        """one host-buffer split -> Apsara call, sized by an estimate first and by the exact size when that was short;
+        tail None: the wire bytes, else records ‖ tail as one LZ4 block.  Returns (bytes, raw_len, n_events,
+        counters[5], ml_counters[3] or None)"""
+        a = _u8(buf)
+        cfg = self._sa_cfg(renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos, time, time_ns,
+                           enable_ns) + [int(now), int(discard_interval)]
+        tl = None if tail is None else np.frombuffer(bytes(tail), np.uint8)
+        est = 2 * a.size + 4096 + (0 if tl is None else tl.size)
+        cap = int(out_cap if out_cap is not None else est + est // 255 + 16)
+        for _ in range(2):
+            out = np.empty(max(cap, 1), np.uint8)
+            need, raw, nev = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+            ctr, mctr = np.zeros(5, np.uint64), np.zeros(3, np.uint64)
+            z = [] if tl is None else [_p(tl) if tl.size else None, tl.size]
+            outs = [_p(out), cap, C.byref(need)] + ([] if tl is None else [C.byref(raw)]) + [C.byref(nev), _p(ctr)]
+            rc = fn(self._h, ap._h, _p(a), a.size, *extra, *cfg, *z, *outs, *([_p(mctr)] if ml else []))
+            if rc == LC_ERR_CAPACITY and out_cap is None:
+                cap = int(need.value)
+                continue
+            _check(rc)
+            return bytes(out[:need.value]), int(raw.value), int(nev.value), ctr, (mctr if ml else None)
+        _check(rc)
+
+    def split_apsara_parse_sls(self, ap, buf, split_char, renamed_key, keep_fail=False, keep_succeed=False,
+                               copy_raw=False, offset_key=None, src_pos=0, time=0, time_ns=None, enable_ns=False,
+                               now=0, discard_interval=-1, out_cap=None):
+        """Host source value in: split, Apsara (now, discard_interval -1 = no history discard), wire bytes out
+        (lc_split_apsara_parse_sls).  Returns (bytes, number of pieces, counters[5])."""
+        data, _raw, nev, ctr, _m = self._split_apsara(
+            lib().lc_split_apsara_parse_sls, ap, buf, [split_char], renamed_key, keep_fail, keep_succeed, copy_raw,
+            offset_key, src_pos, time, time_ns, enable_ns, now, discard_interval, out_cap, False, None)
+        return data, nev, ctr
+
+    def split_apsara_parse_sls_lz4(self, ap, buf, split_char, renamed_key, keep_fail=False, keep_succeed=False,
+                                   copy_raw=False, offset_key=None, src_pos=0, time=0, time_ns=None, enable_ns=False,
+                                   now=0, discard_interval=-1, tail=b"", out_cap=None):
+        """split_apsara_parse_sls's records followed by `tail` as ONE LZ4 block (lc_split_apsara_parse_sls_lz4).
+        Returns (block, raw_len, number of pieces, counters[5])."""
+        data, raw, nev, ctr, _m = self._split_apsara(
+            lib().lc_split_apsara_parse_sls_lz4, ap, buf, [split_char], renamed_key, keep_fail, keep_succeed,
+            copy_raw, offset_key, src_pos, time, time_ns, enable_ns, now, discard_interval, out_cap, False, tail)
+        return data, raw, nev, ctr
+
+    def multiline_split_apsara_parse_sls(self, ap, buf, start, cont, end, discard, renamed_key, keep_fail=False,
+                                         keep_succeed=False, copy_raw=False, offset_key=None, src_pos=0, time=0,
+                                         time_ns=None, enable_ns=False, now=0, discard_interval=-1, out_cap=None):
+        """The same with the multiline splitter (lc_multiline_split_apsara_parse_sls).  Returns (bytes, number of
+        events, counters[5], splitter counters[3])."""
+        data, _raw, nev, ctr, mctr = self._split_apsara(
+            lib().lc_multiline_split_apsara_parse_sls, ap, buf, [_rh(start), _rh(cont), _rh(end), int(bool(discard))],
+            renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos, time, time_ns, enable_ns, now,
+            discard_interval, out_cap, True, None)
+        return data, nev, ctr, mctr
+
+    def multiline_split_apsara_parse_sls_lz4(self, ap, buf, start, cont, end, discard, renamed_key, keep_fail=False,
+                                             keep_succeed=False, copy_raw=False, offset_key=None, src_pos=0, time=0,
+                                             time_ns=None, enable_ns=False, now=0, discard_interval=-1, tail=b"",
+                                             out_cap=None):
+        """multiline_split_apsara_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_multiline_split_apsara_parse_sls_lz4).  Returns (block, raw_len, number of events, counters[5], splitter
+        counters[3])."""
+        return self._split_apsara(
+            lib().lc_multiline_split_apsara_parse_sls_lz4, ap, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], renamed_key, keep_fail, keep_succeed, copy_raw,
+            offset_key, src_pos, time, time_ns, enable_ns, now, discard_interval, out_cap, True, tail)
 
     def json_parse_dev(self, js, d_base, base_len, d_ev_off, d_ev_len, n, d_status, d_first, d_entries, entry_cap,
                        d_arena, arena_cap, d_counters):

@@ -135,6 +135,9 @@ struct lc_engine {
     // split -> JSON -> SLS chain: the resolve's per-entry winners, per-piece records, list of pieces to sort (behind
     // its count) and sort scratch; the chain's piece and JSON tables are in, out_a, out_b and the js_* buffers
     DevBuf sj_win, sj_ev, sj_list, sj_sort;
+    // split -> Apsara -> SLS chain: its one-group table; the piece and Apsara tables are in, out_a, out_b and the ap_*
+    // buffers
+    DevBuf sa_grp;
     DevBuf small;  // tickets + counters: [0..3] u32 tickets, +16: u32 n_out, +32: u64 total, +64: u64 counters[2]
     void* h_small = nullptr; // pinned mirror of `small`
     std::unordered_map<uint64_t, void*> blobs; // regex id * 4 + layout -> device blob
@@ -356,7 +359,8 @@ void lc_engine_destroy(lc_engine_t* e) {
                       &e->ap_conf, &e->ap_ev, &e->ap_nent, &e->ap_small, &e->ap_status, &e->ap_sec, &e->ap_nsec,
                       &e->ap_micro, &e->ap_first, &e->ap_ent, &e->js_conf, &e->js_nent, &e->js_narena,
                       &e->js_slow, &e->js_list, &e->js_afirst, &e->js_small, &e->js_status, &e->js_first, &e->js_ent,
-                      &e->js_arena, &e->js_cnt, &e->js_pow5, &e->sj_win, &e->sj_ev, &e->sj_list, &e->sj_sort};
+                      &e->js_arena, &e->js_cnt, &e->js_pow5, &e->sj_win, &e->sj_ev, &e->sj_list, &e->sj_sort,
+                      &e->sa_grp};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -4962,3 +4966,229 @@ int lc_multiline_split_json_parse_sls_lz4(lc_engine_t* e, const lc_json_t* js, c
 #undef ML_SPLIT
 #undef SPLIT_JSON_PARAMS
 #undef SPLIT_JSON_ARGS
+
+// ---------------------------------------------------------------------------------------------- split -> Apsara -> SLS
+// The Apsara stage's CommonParserOptions, the offset content of the split events (offset_key NULL = no
+// log.file.offset metadata) with the source event's position, time and ns, and mEnableTimestampNanosecond
+#define SPLIT_APSARA_PARAMS                                                                                            \
+    const char *renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,                 \
+        const char *offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,           \
+        int enable_ns
+#define SPLIT_APSARA_ARGS                                                                                              \
+    renamed_key, renamed_key_len, keep_fail, keep_succeed, copy_raw, offset_key, offset_key_len, src_pos, time,       \
+        time_ns, enable_ns
+
+namespace {
+
+// lc_split_apsara_sls_setup over ap's SourceKey, with SourceKey, RenamedSourceKey, the offset key and the fixed names
+// staged on the device (`sls_plan`, which neither splitter nor the Apsara stage uses) and *c pointing at them
+int split_apsara_sls_config(lc_engine_t* e, const char* what, const lc_apsara_t* ap, SPLIT_APSARA_PARAMS,
+                            LcSplitApsaraSlsCfg* c) {
+    if (!ap || (renamed_key_len && !renamed_key) || (offset_key_len && !offset_key))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    const uint32_t oklen = offset_key ? offset_key_len : 0u;
+    if ((uint64_t)ap->skey.size() + renamed_key_len + oklen + LC_AP_SLS_NAMES_LEN + 16 > 0xFFFFFFFFull)
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": keys must stay below 4 GiB");
+    const char* why = lc_split_apsara_sls_setup(ap->skey.data(), (uint32_t)ap->skey.size(), renamed_key,
+                                                renamed_key_len, offset_key, oklen, keep_fail, keep_succeed, copy_raw,
+                                                src_pos, time, time_ns, enable_ns, c);
+    if (why)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    std::string keys = ap->skey;
+    keys.append(renamed_key ? renamed_key : "", renamed_key_len);
+    keys.append(offset_key ? offset_key : "", oklen);
+    keys.append(LC_AP_SLS_NAMES, LC_AP_SLS_NAMES_LEN);
+    CU_TRY(e->sls_plan.ensure(keys.size() + 1));
+    CU_TRY(cudaMemcpyAsync(e->sls_plan.p, keys.data(), keys.size(), cudaMemcpyHostToDevice, e->stream));
+    const uint8_t* d = e->sls_plan.as<uint8_t>();
+    c->skey = d;
+    c->rkey = d + c->sklen;
+    c->okey = d + c->sklen + c->rklen;
+    c->names = c->okey + c->oklen;
+    return LC_OK;
+}
+
+// The size pass and the emit of the chain over the n pieces of t: into d_out (the device-fed call), or back to the
+// host buffer out, or -- with z -- records ‖ tail as one LZ4 block.  counters[5] in lc_apsara_parse's order; set
+// whenever the size pass ran.
+int split_apsara_sls_run(lc_engine_t* e, const char* what, const LcSplitApsaraSlsCfg& c,
+                         const lck::SplitApsaraSlsTables& t, uint64_t n, uint8_t* d_out, uint8_t* out,
+                         uint64_t out_cap, uint64_t* out_len, uint64_t* counters, const Lz4Tail* z) {
+    uint64_t ctr[LC_AP_SLS_COUNTERS + 1] = {0}; // + pieces whose record would reach 4 GiB
+    SlsTo to;
+    to.host = out;
+    to.z = z;
+    to.too_large = LC_AP_SLS_COUNTERS;
+    const int rc = serialize_sls_dev(
+        e, what, n, LC_AP_SLS_COUNTERS + 1,
+        [&](uint32_t* rec, uint32_t* body, unsigned long long* d_ctr) {
+            lck::launch_split_apsara_sls_sizes(c, t, n, rec, body, d_ctr, e->stream);
+        },
+        [&](const uint64_t* rec_off, const uint32_t* body, uint8_t* dst) {
+            lck::launch_split_apsara_sls_emit(c, t, n, rec_off, body, dst, e->stream);
+        },
+        d_out, out_cap, out_len, ctr, to);
+    if (counters)
+        memcpy(counters, ctr, LC_AP_SLS_COUNTERS * sizeof(uint64_t));
+    return rc;
+}
+
+// Host-buffer split + Apsara + serialise (lc_split_apsara_parse_sls and the multiline / LZ4 siblings): the Apsara
+// stage runs ap_count / ap_emit over the pieces, the chunk as their base and one group, into the ap_* buffers of
+// lc_apsara_parse, then split_apsara_sls_run.  The stage's counters are the size pass's, so ap_count's own go to
+// ts_cnt unread.
+template <class Split>
+int split_apsara_sls_host(lc_engine_t* e, const char* what, const lc_apsara_t* ap, const uint8_t* buf, uint64_t len,
+                          Split split, SPLIT_APSARA_PARAMS, int64_t now, int32_t discard_interval, uint8_t* out,
+                          uint64_t out_cap, uint64_t* out_len, uint64_t* n_events, uint64_t* counters,
+                          const Lz4Tail* z) {
+    LcSplitApsaraSlsCfg c;
+    auto begin = [&]() {
+        if (counters)
+            memset(counters, 0, LC_AP_SLS_COUNTERS * sizeof(uint64_t));
+        return (int)LC_OK;
+    };
+    auto config = [&]() { return split_apsara_sls_config(e, what, ap, SPLIT_APSARA_ARGS, &c); };
+    auto run = [&](uint64_t n) {
+        if (n >= (1ull << 30))
+            return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^30 pieces per call");
+        CU_TRY(e->ap_status.ensure(n));
+        CU_TRY(e->ap_sec.ensure(n * 8));
+        CU_TRY(e->ap_nsec.ensure(n * 4));
+        CU_TRY(e->ap_micro.ensure(n * 8));
+        CU_TRY(e->ap_first.ensure((n + 1) * 8));
+        CU_TRY(e->ts_cnt.ensure(5 * sizeof(uint64_t)));
+        CU_TRY(e->sa_grp.ensure(8));
+        const uint32_t g[2] = {0u, (uint32_t)n};
+        CU_TRY(cudaMemcpyAsync(e->sa_grp.p, g, sizeof g, cudaMemcpyHostToDevice, e->stream));
+        const uint8_t* d_src = e->in.as<uint8_t>();
+        const uint32_t *off = e->out_a.as<uint32_t>(), *ln = e->out_b.as<uint32_t>();
+        uint64_t m = 0;
+        int rc = ap_count(e, ap, what, d_src, len, off, ln, n, e->sa_grp.as<uint32_t>(), 1, now, discard_interval,
+                          e->ap_status.as<uint8_t>(), e->ap_sec.as<int64_t>(), e->ap_nsec.as<uint32_t>(),
+                          e->ap_micro.as<int64_t>(), e->ap_first.as<uint64_t>(), &m, e->ts_cnt.as<uint64_t>());
+        if (rc)
+            return rc;
+        CU_TRY(e->ap_ent.ensure(m * sizeof(LcApEntry) + 16));
+        if (m) {
+            rc = ap_emit(e, d_src, off, ln, n, e->ap_status.as<uint8_t>(), e->ap_first.as<uint64_t>(),
+                         e->ap_ent.as<lc_apsara_entry_t>());
+            if (rc)
+                return rc;
+        }
+        const lck::SplitApsaraSlsTables t{d_src,
+                                          off,
+                                          ln,
+                                          e->ap_status.as<uint8_t>(),
+                                          e->ap_sec.as<int64_t>(),
+                                          e->ap_nsec.as<uint32_t>(),
+                                          e->ap_micro.as<int64_t>(),
+                                          e->ap_first.as<uint64_t>(),
+                                          e->ap_ent.as<LcApEntry>()};
+        return split_apsara_sls_run(e, what, c, t, n, nullptr, out, out_cap, out_len, counters, z);
+    };
+    return split_chain_sls_host(e, what, buf, len, split, ap != nullptr, begin, config, run, out, out_cap, out_len,
+                                n_events, z);
+}
+
+template <class Split>
+int split_apsara_lz4_host(lc_engine_t* e, const char* what, const lc_apsara_t* ap, const uint8_t* buf, uint64_t len,
+                          Split split, SPLIT_APSARA_PARAMS, int64_t now, int32_t discard_interval,
+                          const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                          uint64_t* raw_len, uint64_t* n_events, uint64_t* counters) {
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return split_apsara_sls_host(e, what, ap, buf, len, split, SPLIT_APSARA_ARGS, now, discard_interval, out, out_cap,
+                                 out_len, n_events, counters, &z);
+}
+
+} // namespace
+
+// (the multiline splitter's own counters[3] are added to ml_counters as lc_multiline_split_dev adds them)
+#define ML_SPLIT                                                                                                       \
+    [&](uint64_t* n) {                                                                                                 \
+        return lc_multiline_split_dev(e, e->in.as<uint8_t>(), len, start, cont, end, discard_unmatched,               \
+                                      e->out_a.as<uint32_t>(), e->out_b.as<uint32_t>(), e->out_c.as<uint8_t>(), len,  \
+                                      n, ml_counters);                                                                 \
+    }
+#define LINE_SPLIT                                                                                                     \
+    [&](uint64_t* n) {                                                                                                 \
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),                   \
+                                  e->out_b.as<uint32_t>(), len, n);                                                    \
+    }
+
+extern "C" {
+
+int lc_sls_serialize_split_apsara_dev(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* d_src, uint64_t src_len,
+                                      const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+                                      const uint8_t* d_status, const int64_t* d_sec, const uint32_t* d_nsec,
+                                      const int64_t* d_micro, const uint64_t* d_first,
+                                      const lc_apsara_entry_t* d_entries, SPLIT_APSARA_PARAMS, uint8_t* d_out,
+                                      uint64_t out_cap, uint64_t* out_len, uint64_t counters[5]) {
+    static const char* what = "lc_sls_serialize_split_apsara_dev";
+    if (!e || !ap || !out_len ||
+        (n && (!d_src || !d_off || !d_len || !d_status || !d_sec || !d_nsec || !d_micro || !d_first)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (counters)
+        memset(counters, 0, LC_AP_SLS_COUNTERS * sizeof(uint64_t));
+    if (src_len >= 0xFFFFFFF0ull || n >= (1ull << 30))
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": the source value must be < 4 GiB, < 2^30 pieces per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcSplitApsaraSlsCfg c;
+    rc = split_apsara_sls_config(e, what, ap, SPLIT_APSARA_ARGS, &c);
+    if (rc || n == 0)
+        return rc;
+    uint64_t m = 0;
+    CU_TRY(cudaMemcpyAsync(&m, d_first + n, 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    if (m && !d_entries)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    const lck::SplitApsaraSlsTables t{d_src,   d_off,   d_len,
+                                      d_status, d_sec,  d_nsec,
+                                      d_micro, d_first, reinterpret_cast<const LcApEntry*>(d_entries)};
+    return split_apsara_sls_run(e, what, c, t, n, d_out, nullptr, out_cap, out_len, counters, nullptr);
+}
+
+int lc_split_apsara_parse_sls(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* buf, uint64_t len,
+                              uint8_t split_char, SPLIT_APSARA_PARAMS, int64_t now, int32_t discard_interval,
+                              uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                              uint64_t counters[5]) {
+    return split_apsara_sls_host(e, "lc_split_apsara_parse_sls", ap, buf, len, LINE_SPLIT, SPLIT_APSARA_ARGS, now,
+                                 discard_interval, out, out_cap, out_len, n_events, counters, nullptr);
+}
+
+int lc_split_apsara_parse_sls_lz4(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* buf, uint64_t len,
+                                  uint8_t split_char, SPLIT_APSARA_PARAMS, int64_t now, int32_t discard_interval,
+                                  const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+                                  uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events, uint64_t counters[5]) {
+    return split_apsara_lz4_host(e, "lc_split_apsara_parse_sls_lz4", ap, buf, len, LINE_SPLIT, SPLIT_APSARA_ARGS, now,
+                                 discard_interval, tail, tail_len, out, out_cap, out_len, raw_len, n_events, counters);
+}
+
+int lc_multiline_split_apsara_parse_sls(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* buf, uint64_t len,
+                                        const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                        int discard_unmatched, SPLIT_APSARA_PARAMS, int64_t now,
+                                        int32_t discard_interval, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+                                        uint64_t* n_events, uint64_t counters[5], uint64_t ml_counters[3]) {
+    return split_apsara_sls_host(e, "lc_multiline_split_apsara_parse_sls", ap, buf, len, ML_SPLIT, SPLIT_APSARA_ARGS,
+                                 now, discard_interval, out, out_cap, out_len, n_events, counters, nullptr);
+}
+
+int lc_multiline_split_apsara_parse_sls_lz4(lc_engine_t* e, const lc_apsara_t* ap, const uint8_t* buf, uint64_t len,
+                                            const lc_regex_t* start, const lc_regex_t* cont, const lc_regex_t* end,
+                                            int discard_unmatched, SPLIT_APSARA_PARAMS, int64_t now,
+                                            int32_t discard_interval, const uint8_t* tail, uint64_t tail_len,
+                                            uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+                                            uint64_t* n_events, uint64_t counters[5], uint64_t ml_counters[3]) {
+    return split_apsara_lz4_host(e, "lc_multiline_split_apsara_parse_sls_lz4", ap, buf, len, ML_SPLIT,
+                                 SPLIT_APSARA_ARGS, now, discard_interval, tail, tail_len, out, out_cap, out_len,
+                                 raw_len, n_events, counters);
+}
+
+} // extern "C"
+#undef ML_SPLIT
+#undef LINE_SPLIT
+#undef SPLIT_APSARA_PARAMS
+#undef SPLIT_APSARA_ARGS

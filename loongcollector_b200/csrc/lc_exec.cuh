@@ -5825,3 +5825,245 @@ inline const char* lc_split_json_sls_setup(const char* source_key, uint32_t sour
     c->ns = c->has_ns ? time_ns : 0u;
     return nullptr;
 }
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, split -> Apsara chain: the Log record of piece k that ProcessorSplitLogStringNative /
+// ProcessorSplitMultilineLogStringNative followed by ProcessorParseApsaraNative (same SourceKey) leave behind, written
+// straight from the piece tables of the splitter and the tables of lc_apsara_parse_dev over those pieces (the chunk as
+// its base, one group).  The piece enters the Apsara stage as [SourceKey -> piece] or, with log.file.offset metadata,
+// [SourceKey -> piece, offset_key -> decimal(src_pos + off[k])].  AppendContentNoCopy never removes a duplicate, so the
+// record of a parsed piece is those two, the base fields, the key:value fields and "microtime" in append order, less
+// the one entry DelContent(SourceKey) removes (the newest live one with that key), plus RenamedSourceKey unless some
+// live content has that key.  The rule is pinned in include/lc_b200.h above lc_sls_serialize_split_apsara_dev.
+//
+// The fixed key names, back to back: "__raw_log__" (0, 11), "microtime" (11, 9), then the base fields' names in
+// LC_AP_K_* order.  The device reads the engine's copy through LcSplitApsaraSlsCfg::names: a string literal in device
+// code would add a module global and move the existing kernels' constant-bank address slots.
+#define LC_AP_SLS_NAMES "__raw_log__microtime__LEVEL____THREAD____FILE____LINE__"
+#define LC_AP_SLS_NAMES_LEN 55u
+#define LC_AP_SLS_NONE 0xFFu // no base field has that name
+#define LC_AP_SLS_COUNTERS 5 // lc_apsara_parse's order: key_not_found, out_failed, history_failure, discarded, ok
+
+// offset and length in LC_AP_SLS_NAMES of base field t (key_off - LC_AP_K_LEVEL)
+LC_HD uint32_t lc_ap_sls_base_at(uint32_t t) { return t == 0u ? 20u : t == 1u ? 29u : t == 2u ? 39u : 47u; }
+LC_HD uint32_t lc_ap_sls_base_len(uint32_t t) { return t == 0u ? 9u : t == 1u ? 10u : 8u; }
+
+struct LcSplitApsaraSlsCfg {
+    const uint8_t* skey;  // SourceKey, RenamedSourceKey, the offset key and LC_AP_SLS_NAMES (device copies on the
+    const uint8_t* rkey;  // device, see above)
+    const uint8_t* okey;
+    const uint8_t* names;
+    uint32_t sklen, rklen, oklen;
+    uint32_t has_offset;
+    uint32_t keep_fail, keep_succeed, copy_raw;
+    uint32_t enable_ns;  // mEnableTimestampNanosecond: a parsed piece writes its Time_ns
+    uint32_t sk_base;    // the base field named SourceKey (0..3), else LC_AP_SLS_NONE
+    uint32_t sk_micro;   // SourceKey == "microtime"
+    uint32_t rk_base;    // the base field named RenamedSourceKey, else LC_AP_SLS_NONE
+    uint32_t rk_sk;      // RenamedSourceKey == SourceKey
+    uint32_t rk_off;     // RenamedSourceKey == the offset key (with offset metadata)
+    uint32_t rk_micro;   // RenamedSourceKey == "microtime"
+    uint32_t rk_raw;     // RenamedSourceKey == "__raw_log__"
+    uint32_t raw_off;    // "__raw_log__" == the offset key (with offset metadata)
+    uint64_t src_pos;    // the source event's file offset
+    uint32_t time;       // the source event's time, as the split events inherit it
+    uint32_t has_ns, ns; // ... and its Time_ns as the serialiser writes it
+};
+
+// One piece: src[po, + plen), lc_apsara_parse_dev's status / sec / nsec / micro of it, and its m entries e (offsets
+// into src; only a parsed piece has any).
+struct LcSplitApsaraSlsRow {
+    uint32_t po, plen;
+    uint32_t status;
+    int64_t sec;
+    uint32_t nsec;
+    int64_t micro;
+    const LcApEntry* e;
+    uint32_t m;
+};
+
+// whether a base field of the piece has tag t (the base fields come first, at most four)
+LC_HD bool lc_ap_sls_has_base(const LcSplitApsaraSlsRow& r, uint32_t t) {
+    for (uint32_t j = 0; j < r.m && r.e[j].key_off >= LC_AP_K_LEVEL; ++j)
+        if (r.e[j].key_off - LC_AP_K_LEVEL == t)
+            return true;
+    return false;
+}
+
+// The body of the piece's Log record -- Time, its contents, Time_ns -- into sink s (LcSlsCount64 / LcSlsWrite).
+// Returns the number of contents; 0 = erased, no record.
+template <class S>
+LC_HD uint32_t lc_split_apsara_sls_body(const LcSplitApsaraSlsCfg& c, const uint8_t* src, const LcSplitApsaraSlsRow& r,
+                                        S& s) {
+    const uint32_t st = r.status & 7u;
+    const bool ok = st == LC_AP_ST_OK, kept = ok || st == LC_AP_ST_EMPTY || st == LC_AP_ST_NOT_FOUND;
+    if (st == LC_AP_ST_DISCARDED || (!kept && !c.keep_fail))
+        return 0u; // too old, or ShouldEraseEvent: nothing but the offset content is left
+    {
+        const uint32_t t = ok ? (uint32_t)r.sec : c.time;
+        uint8_t h[6];
+        h[0] = 0x08;
+        const uint32_t n = 1 + lc_put_varint(h + 1, t < (1u << 28) ? (1u << 28) : t); // always 5 bytes
+        s.put(h, n);
+    }
+    const uint64_t pos = c.src_pos + r.po;
+    const uint32_t nd = lc_dec_digits(pos);
+    uint32_t k = 0;
+    auto piece = [&](const uint8_t* key, uint32_t kl) {
+        lc_sls_pair_open(s, key, kl, r.plen);
+        s.copy(src + r.po, r.plen);
+        ++k;
+    };
+    auto digits = [&]() {
+        lc_sls_pair_open(s, c.okey, c.oklen, nd);
+        lc_sls_digits(s, pos, nd);
+        ++k;
+    };
+    if (ok) {
+        // DelContent(SourceKey) unless a key:value key is SourceKey: "microtime", else a base field, else the piece
+        enum : uint32_t { DEL_NONE, DEL_PIECE, DEL_MICRO, DEL_BASE };
+        uint32_t del = DEL_NONE;
+        if (!(r.status & LC_AP_ST_OVER)) {
+            if (c.sk_micro)
+                del = DEL_MICRO;
+            else if (c.sk_base != LC_AP_SLS_NONE && lc_ap_sls_has_base(r, c.sk_base))
+                del = DEL_BASE;
+            else
+                del = DEL_PIECE;
+        }
+        if (del != DEL_PIECE)
+            piece(c.skey, c.sklen);
+        if (c.has_offset)
+            digits();
+        for (uint32_t j = 0; j < r.m; ++j) {
+            const LcApEntry& x = r.e[j];
+            if (x.key_off >= LC_AP_K_LEVEL) {
+                const uint32_t t = x.key_off - LC_AP_K_LEVEL;
+                if (del == DEL_BASE && t == c.sk_base)
+                    continue;
+                lc_sls_pair_open(s, c.names + lc_ap_sls_base_at(t), lc_ap_sls_base_len(t), x.val_len);
+            } else {
+                lc_sls_pair_open(s, src + x.key_off, x.key_len, x.val_len);
+            }
+            s.copy(src + x.val_off, x.val_len);
+            ++k;
+        }
+        if (del != DEL_MICRO) {
+            const bool neg = r.micro < 0; // "%ld": a wrapped logTime_in_micro renders negative
+            const uint64_t mag = neg ? 0u - (uint64_t)r.micro : (uint64_t)r.micro;
+            const uint32_t md = lc_dec_digits(mag);
+            lc_sls_pair_open(s, c.names + 11, 9u, md + (neg ? 1u : 0u));
+            if (neg) {
+                const uint8_t minus = '-';
+                s.put(&minus, 1);
+            }
+            lc_sls_digits(s, mag, md);
+            ++k;
+        }
+        if (c.keep_succeed) {
+            bool present = (c.rk_sk && del != DEL_PIECE) || (c.has_offset && c.rk_off) ||
+                           (c.rk_micro && del != DEL_MICRO) ||
+                           (c.rk_base != LC_AP_SLS_NONE && lc_ap_sls_has_base(r, c.rk_base) &&
+                            !(del == DEL_BASE && c.rk_base == c.sk_base));
+            for (uint32_t j = 0; j < r.m && !present; ++j) {
+                const LcApEntry& x = r.e[j];
+                if (x.key_off < LC_AP_K_LEVEL && x.key_len == c.rklen) {
+                    uint32_t b = 0;
+                    while (b < x.key_len && src[x.key_off + b] == c.rkey[b])
+                        ++b;
+                    present = b == x.key_len;
+                }
+            }
+            if (!present)
+                piece(c.rkey, c.rklen);
+        }
+    } else if (kept) {
+        piece(c.skey, c.sklen); // an empty value: the piece is kept untouched
+        if (c.has_offset)
+            digits();
+    } else {
+        if (c.has_offset)
+            digits();
+        if (!(c.has_offset && c.rk_off))
+            piece(c.rkey, c.rklen);
+        if (c.copy_raw && !(c.has_offset && c.raw_off) && !c.rk_raw)
+            piece(c.names, 11u);
+    }
+    const bool has_ns = ok ? c.enable_ns != 0 : c.has_ns != 0;
+    if (has_ns) {
+        const uint32_t ns = ok ? r.nsec : c.ns;
+        const uint8_t h[5] = {0x25, (uint8_t)ns, (uint8_t)(ns >> 8), (uint8_t)(ns >> 16), (uint8_t)(ns >> 24)};
+        s.put(h, 5);
+    }
+    return k;
+}
+
+// The piece's counter verdicts as bits of ProcessorParseApsaraNative's counters in lc_apsara_parse's order
+// (LC_TS_C_*): discarded also counts a failed piece ShouldEraseEvent erases.
+LC_HD uint32_t lc_split_apsara_verdict(const LcSplitApsaraSlsCfg& c, uint32_t status) {
+    const uint32_t st = status & 7u;
+    if (st == LC_AP_ST_OK)
+        return 1u << LC_TS_C_OUT_SUCCESSFUL;
+    if (st == LC_AP_ST_NOT_FOUND)
+        return 1u << LC_TS_C_KEY_NOT_FOUND;
+    if (st == LC_AP_ST_EMPTY)
+        return 1u << LC_TS_C_OUT_FAILED;
+    if (st == LC_AP_ST_DISCARDED)
+        return (1u << LC_TS_C_HISTORY_FAILURE) | (1u << LC_TS_C_DISCARDED);
+    return (1u << LC_TS_C_OUT_FAILED) | (c.keep_fail ? 0u : 1u << LC_TS_C_DISCARDED);
+}
+
+// Host side: the configuration of the chain, with the key pointers as given and `names` at a host LC_AP_SLS_NAMES (the
+// device caller points them at its copies).  offset_key == nullptr: no log.file.offset metadata; time_ns 0xFFFFFFFF:
+// the source event writes no Time_ns.  Returns nullptr, or why the chain is refused: an offset key equal to SourceKey
+// (the split would replace the piece by its digits, and the Apsara stage would parse those), and a source Time_ns
+// without enable_ns (the pieces that keep the source time would write Time_ns and the parsed ones would not, a mix no
+// configuration of the reference produces).
+inline const char* lc_split_apsara_sls_setup(const char* source_key, uint32_t source_len, const char* renamed_key,
+                                             uint32_t renamed_len, const char* offset_key, uint32_t offset_len,
+                                             int keep_fail, int keep_succeed, int copy_raw, uint64_t src_pos,
+                                             uint32_t time, uint32_t time_ns, int enable_ns,
+                                             LcSplitApsaraSlsCfg* c) {
+    auto eq = [](const char* a, uint32_t al, const char* b, uint32_t bl) {
+        return al == bl && (al == 0 || !memcmp(a, b, al));
+    };
+    static const char* const kNames = LC_AP_SLS_NAMES;
+    auto base_of = [&](const char* k, uint32_t kl) {
+        for (uint32_t t = 0; t < 4; ++t)
+            if (eq(k, kl, kNames + lc_ap_sls_base_at(t), lc_ap_sls_base_len(t)))
+                return t;
+        return (uint32_t)LC_AP_SLS_NONE;
+    };
+    if (!c)
+        return "bad arguments";
+    if (offset_key && eq(offset_key, offset_len, source_key, source_len))
+        return "the offset key equals SourceKey";
+    if (time_ns != 0xFFFFFFFFu && !enable_ns)
+        return "a source time_ns needs enable_ns";
+    memset(c, 0, sizeof *c);
+    c->skey = reinterpret_cast<const uint8_t*>(source_key);
+    c->rkey = reinterpret_cast<const uint8_t*>(renamed_key);
+    c->okey = reinterpret_cast<const uint8_t*>(offset_key);
+    c->names = reinterpret_cast<const uint8_t*>(kNames);
+    c->sklen = source_len;
+    c->rklen = renamed_len;
+    c->oklen = offset_key ? offset_len : 0u;
+    c->has_offset = offset_key != nullptr;
+    c->keep_fail = keep_fail != 0;
+    c->keep_succeed = keep_succeed != 0;
+    c->copy_raw = copy_raw != 0;
+    c->enable_ns = enable_ns != 0;
+    c->sk_base = base_of(source_key, source_len);
+    c->sk_micro = eq(source_key, source_len, kNames + 11, 9);
+    c->rk_base = base_of(renamed_key, renamed_len);
+    c->rk_sk = eq(renamed_key, renamed_len, source_key, source_len);
+    c->rk_off = offset_key && eq(renamed_key, renamed_len, offset_key, offset_len);
+    c->rk_micro = eq(renamed_key, renamed_len, kNames + 11, 9);
+    c->rk_raw = eq(renamed_key, renamed_len, kNames, 11);
+    c->raw_off = offset_key && eq(kNames, 11, offset_key, offset_len);
+    c->src_pos = src_pos;
+    c->time = time;
+    c->has_ns = time_ns != 0xFFFFFFFFu;
+    c->ns = c->has_ns ? time_ns : 0u;
+    return nullptr;
+}

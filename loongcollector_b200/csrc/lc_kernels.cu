@@ -4837,4 +4837,79 @@ void launch_split_json_sls_emit(const LcSplitJsonSlsCfg& c, const SplitJsonSlsTa
                                                                                       d_out);
 }
 
+// ---- f4, split -> Apsara chain (lc_exec.cuh: lc_split_apsara_sls_body, lc_split_apsara_verdict).  The size pass runs
+// one thread per piece, the emit pass one warp per piece.  counters: u64 [6] += lc_apsara_parse's five, then pieces
+// whose record would reach 4 GiB.
+__device__ __forceinline__ LcSplitApsaraSlsRow split_apsara_sls_row(const SplitApsaraSlsTables& t, uint64_t i) {
+    LcSplitApsaraSlsRow r;
+    const uint64_t f = t.first[i];
+    r.po = t.off[i];
+    r.plen = t.len[i];
+    r.status = t.status[i];
+    r.sec = t.sec[i];
+    r.nsec = t.nsec[i];
+    r.micro = t.micro[i];
+    r.e = t.ent + f;
+    r.m = (r.status & 7u) == LC_AP_ST_OK ? (uint32_t)(t.first[i + 1] - f) : 0u;
+    return r;
+}
+
+__global__ void __launch_bounds__(256)
+    split_apsara_sls_size_kernel(LcSplitApsaraSlsCfg c, SplitApsaraSlsTables t, uint64_t n,
+                                 uint32_t* __restrict__ rec_size, uint32_t* __restrict__ body_size,
+                                 unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t bits = 0, big = 0;
+    if (i < n) {
+        const LcSplitApsaraSlsRow r = split_apsara_sls_row(t, i);
+        LcSlsCount64 s{0};
+        const uint32_t cnt = lc_split_apsara_sls_body(c, t.src, r, s);
+        big = s.n + 16 > 0xFFFFFFFFull;
+        const uint32_t body = cnt && !big ? (uint32_t)s.n : 0u;
+        rec_size[i] = body ? 1 + lc_varint_size(body) + body : 0u;
+        body_size[i] = body;
+        bits = lc_split_apsara_verdict(c, r.status) | (big << LC_AP_SLS_COUNTERS);
+    }
+    for (uint32_t k = 0; k <= LC_AP_SLS_COUNTERS; ++k) {
+        const uint32_t v = __reduce_add_sync(0xFFFFFFFFu, (bits >> k) & 1u);
+        if ((threadIdx.x & 31) == 0 && v)
+            atomicAdd(counters + k, (unsigned long long)v);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+    split_apsara_sls_emit_kernel(LcSplitApsaraSlsCfg c, SplitApsaraSlsTables t, uint64_t n,
+                                 const uint64_t* __restrict__ rec_off, const uint32_t* __restrict__ body_size,
+                                 uint8_t* __restrict__ out) {
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n)
+        return;
+    const uint32_t body = body_size[i];
+    if (!body)
+        return; // erased: no record
+    const LcSplitApsaraSlsRow r = split_apsara_sls_row(t, i);
+    uint8_t h[6];
+    h[0] = 0x0A;
+    const uint32_t hn = 1 + lc_put_varint(h + 1, body);
+    LcSlsWrite s{out + rec_off[i], 0u, hn + body, threadIdx.x & 31, 32};
+    s.put(h, hn);
+    lc_split_apsara_sls_body(c, t.src, r, s);
+}
+
+void launch_split_apsara_sls_sizes(const LcSplitApsaraSlsCfg& c, const SplitApsaraSlsTables& t, uint64_t n,
+                                   uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                   cudaStream_t st) {
+    if (n)
+        split_apsara_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_size, d_body_size,
+                                                                                   d_counters);
+}
+
+void launch_split_apsara_sls_emit(const LcSplitApsaraSlsCfg& c, const SplitApsaraSlsTables& t, uint64_t n,
+                                  const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                  cudaStream_t st) {
+    if (n)
+        split_apsara_sls_emit_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, t, n, d_rec_off,
+                                                                                        d_body_size, d_out);
+}
+
 } // namespace lck

@@ -23,6 +23,7 @@ struct LcApEntry;
 struct LcJsonEntry;
 struct LcSplitJsonSlsCfg;
 struct LcJsonSlsEv;
+struct LcSplitApsaraSlsCfg;
 struct LcLz4Chunk;
 
 namespace lck {
@@ -454,5 +455,27 @@ void launch_split_json_sls_sizes(const LcSplitJsonSlsCfg& c, const SplitJsonSlsT
 void launch_split_json_sls_emit(const LcSplitJsonSlsCfg& c, const SplitJsonSlsTables& t, uint64_t n,
                                 const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
                                 cudaStream_t st);
+
+// f4, split -> Apsara chain (lc_exec.cuh: LcSplitApsaraSlsCfg, keys on the device): the pieces off / len of the source
+// value src, parsed by lc_apsara_parse_dev (src as its base) into status / sec / nsec / micro / first / ent.  Sizes as
+// for launch_sls_sizes; d_counters: u64 [6] += lc_apsara_parse's five (discarded with the failed pieces erased), then
+// the pieces whose record would reach 4 GiB.
+struct SplitApsaraSlsTables {
+    const uint8_t* src;
+    const uint32_t* off;
+    const uint32_t* len;
+    const uint8_t* status;
+    const int64_t* sec;
+    const uint32_t* nsec;
+    const int64_t* micro;
+    const uint64_t* first;
+    const LcApEntry* ent;
+};
+void launch_split_apsara_sls_sizes(const LcSplitApsaraSlsCfg& c, const SplitApsaraSlsTables& t, uint64_t n,
+                                   uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                   cudaStream_t st);
+void launch_split_apsara_sls_emit(const LcSplitApsaraSlsCfg& c, const SplitApsaraSlsTables& t, uint64_t n,
+                                  const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                  cudaStream_t st);
 
 } // namespace lck

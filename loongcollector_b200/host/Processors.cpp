@@ -3865,4 +3865,145 @@ bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGrou
 #undef SPLIT_JSON_STAGE_ARGS
 #undef SPLIT_JSON_STAGE_OPTS
 
+// ------------------------------------------------------------------------------------------------ split -> Apsara
+// The Apsara stage of the split -> Apsara chain: a ProcessorParseApsaraNative's configuration, "now" and history
+// discard as the chain calls take them, the host check of lc_split_apsara_sls_setup, and the counters Process would
+// move.  The device calls take a group of exactly one source event: the time cache runs over the whole group in event
+// order and would otherwise have to carry across calls.
+struct SplitApsaraStage {
+    ProcessorParseApsaraNative& a;
+    const PipelineEventGroup& group;
+    int64_t now;
+    SplitApsaraStage(ProcessorParseApsaraNative& ap, const PipelineEventGroup& g)
+        : a(ap), group(g), now((int64_t)time(nullptr)) {}
+    const std::string& Renamed() const { return a.mCommonParserOptions.mRenamedSourceKey; }
+    const CommonParserOptions& Opt() const { return a.mCommonParserOptions; }
+    const lc_apsara_t* Program() const { return a.mProgram; }
+    int32_t DiscardInterval() const { return a.mDiscardOldData ? a.mDiscardInterval : -1; }
+    // whether the chain's device calls take this stage behind a splitter reading sourceKey
+    bool Accepts(const std::string& sourceKey, const StringView* okey) const {
+        LcSplitApsaraSlsCfg c;
+        return group.GetEvents().size() == 1 && a.mProgram && a.mSourceKey == sourceKey &&
+               !lc_split_apsara_sls_setup(a.mSourceKey.data(), (uint32_t)a.mSourceKey.size(), Renamed().data(),
+                                          (uint32_t)Renamed().size(), okey ? okey->data() : nullptr,
+                                          okey ? (uint32_t)okey->size() : 0u, Opt().mKeepingSourceWhenParseFail,
+                                          Opt().mKeepingSourceWhenParseSucceed, Opt().mCopingRawLog, 0, 0,
+                                          LC_SLS_NO_NS, 0, &c);
+    }
+    // the device calls' counters[5] (key_not_found, out_failed, history_failure, discarded, out_successful) as the
+    // chain driver takes a stage's: successful, out_failed, discarded (every piece the stage erased), none removed by a
+    // filter, then key_not_found and history_failure
+    static void Fold(const uint64_t c5[5], uint64_t rctr[8]) {
+        const uint64_t f[8] = {c5[4], c5[1], c5[3], 0, c5[0], c5[2], 0, 0};
+        memcpy(rctr, f, sizeof f);
+    }
+    void Add(const uint64_t ctr[6]) const {
+        a.mOutSuccessfulEventsTotal.Add(ctr[0]);
+        a.mOutFailedEventsTotal.Add(ctr[1]);
+        a.mDiscardedEventsTotal.Add(ctr[2]);
+        a.mOutKeyNotFoundEventsTotal.Add(ctr[4]);
+        a.mHistoryFailureTotal.Add(ctr[5]);
+    }
+    void Process(PipelineEventGroup& g) const { a.Process(g); }
+};
+#define SPLIT_APSARA_STAGE_ARGS(x)                                                                                     \
+    (x).Program(), src(val), val.size()
+#define SPLIT_APSARA_STAGE_OPTS(x)                                                                                     \
+    (x).Renamed().data(), (uint32_t)(x).Renamed().size(), (x).Opt().mKeepingSourceWhenParseFail,                      \
+        (x).Opt().mKeepingSourceWhenParseSucceed, (x).Opt().mCopingRawLog, okey ? okey->data() : nullptr,            \
+        okey ? (uint32_t)okey->size() : 0u, pos, time, ns, enableNs, (x).now, (x).DiscardInterval()
+
+bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseApsaraNative& next,
+                                                 bool enableNs, std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseApsaraNative& next,
+                                                    bool enableNs, std::string& block, uint64_t& rawSize,
+                                                    std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitLogStringNative::ChainSerializeSls(PipelineEventGroup& group, ProcessorParseApsaraNative& next,
+                                                      bool enableNs, std::string& out, uint64_t* rawSize,
+                                                      std::string& err) {
+    const SplitApsaraStage x(next, group);
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c5[5] = {0, 0, 0, 0, 0};
+        const int rc = lc_split_apsara_parse_sls(Engine(), SPLIT_APSARA_STAGE_ARGS(x), (uint8_t)mSplitChar,
+                                                 SPLIT_APSARA_STAGE_OPTS(x), o, cap, len, nev, c5);
+        SplitApsaraStage::Fold(c5, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c5[5] = {0, 0, 0, 0, 0};
+        const int rc = lc_split_apsara_parse_sls_lz4(Engine(), SPLIT_APSARA_STAGE_ARGS(x), (uint8_t)mSplitChar,
+                                                     SPLIT_APSARA_STAGE_OPTS(x), tail, tailLen, o, cap, len, raw, nev,
+                                                     c5);
+        SplitApsaraStage::Fold(c5, rctr);
+        return rc;
+    };
+    uint64_t unused[3] = {0, 0, 0};
+    return SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_split_apsara_parse_sls",
+        "lc_split_apsara_parse_sls_lz4", unused);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseApsaraNative& next,
+                                                          bool enableNs, std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSlsLz4(PipelineEventGroup& group,
+                                                             ProcessorParseApsaraNative& next, bool enableNs,
+                                                             std::string& block, uint64_t& rawSize,
+                                                             std::string& err) {
+    return ChainSerializeSls(group, next, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGroup& group,
+                                                               ProcessorParseApsaraNative& next, bool enableNs,
+                                                               std::string& out, uint64_t* rawSize, std::string& err) {
+    const SplitApsaraStage x(next, group);
+    const bool discard = mMultiline.mUnmatchedContentTreatment == MultilineOptions::UnmatchedContentTreatment::DISCARD;
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c5[5] = {0, 0, 0, 0, 0};
+        const int rc = lc_multiline_split_apsara_parse_sls(Engine(), SPLIT_APSARA_STAGE_ARGS(x), mStart.get(),
+                                                           mContinue.get(), mEnd.get(), discard,
+                                                           SPLIT_APSARA_STAGE_OPTS(x), o, cap, len, nev, c5, sctr);
+        SplitApsaraStage::Fold(c5, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c5[5] = {0, 0, 0, 0, 0};
+        const int rc = lc_multiline_split_apsara_parse_sls_lz4(Engine(), SPLIT_APSARA_STAGE_ARGS(x), mStart.get(),
+                                                               mContinue.get(), mEnd.get(), discard,
+                                                               SPLIT_APSARA_STAGE_OPTS(x), tail, tailLen, o, cap, len,
+                                                               raw, nev, c5, sctr);
+        SplitApsaraStage::Fold(c5, rctr);
+        return rc;
+    };
+    // matched_events, input lines, unmatched lines: moved as Process moves them (:82-84,106-107)
+    uint64_t ctr[3] = {0, 0, 0};
+    const bool ok = SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_multiline_split_apsara_parse_sls",
+        "lc_multiline_split_apsara_parse_sls_lz4", ctr);
+    mMatchedEventsTotal.Add(ctr[0]);
+    mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
+    mUnmatchedLinesTotal.Add(ctr[2]);
+    return ok;
+}
+#undef SPLIT_APSARA_STAGE_ARGS
+#undef SPLIT_APSARA_STAGE_OPTS
+
 } // namespace logtail

@@ -204,12 +204,27 @@ public:
     // device (lc_split_json_parse_sls_lz4); other groups compress SerializeSls's bytes.
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& block,
                          uint64_t& rawSize, std::string& err);
+    // The split -> Apsara chain: Process(group), then next.Process(group) (next: the processor_parse_apsara_native
+    // behind this one, reading SourceKey), then SLSEventGroupSerializer::Serialize: the same bytes or error message, and
+    // the same counter updates on both processors.  On a flat group of ONE source event without EnableRawContent (a
+    // reader chunk: the time cache runs over the whole group), whose Apsara SourceKey is this SourceKey and whose
+    // configuration lc_split_apsara_parse_sls accepts, the event is split, parsed and serialised in one device pass
+    // (log.file.offset metadata included; now = time(NULL), the history discard as next has it) and only the wire
+    // bytes come back; the group's events are left as they were.  Otherwise the three calls run.
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseApsaraNative& next, bool enableNs, std::string& out,
+                      std::string& err);
+    // The same followed by LZ4Compressor::Compress; a device-path group is compressed on the device
+    // (lc_split_apsara_parse_sls_lz4).
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseApsaraNative& next, bool enableNs,
+                         std::string& block, uint64_t& rawSize, std::string& err);
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& out,
                            uint64_t* rawSize, std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseApsaraNative& next, bool enableNs,
+                           std::string& out, uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative* filter,
                            bool enableNs, std::string& out, uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
@@ -275,12 +290,19 @@ public:
                       std::string& err);
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& block,
                          uint64_t& rawSize, std::string& err);
+    // The split -> Apsara chain, as ProcessorSplitLogStringNative's (lc_multiline_split_apsara_parse_sls[_lz4]).
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseApsaraNative& next, bool enableNs, std::string& out,
+                      std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseApsaraNative& next, bool enableNs,
+                         std::string& block, uint64_t& rawSize, std::string& err);
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& out,
                            uint64_t* rawSize, std::string& err);
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseApsaraNative& next, bool enableNs,
+                           std::string& out, uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseRegexNative& next, ProcessorFilterNative* filter,
                            bool enableNs, std::string& out, uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next, bool enableNs,
@@ -477,6 +499,7 @@ protected:
 
 private:
     lc_apsara_t* mProgram = nullptr;
+    friend struct SplitApsaraStage; // the split -> Apsara chain's SerializeSls
 };
 
 // processor_parse_json_native (ProcessorParseJsonNative.cpp: ProcessEvent, JsonLogLineParserSimdJson): the groups of

@@ -292,10 +292,12 @@ char* lc_host_chain_serialize_sls(lc_host_processor_t* delim, lc_host_processor_
         auto* pm = dynamic_cast<ProcessorSplitMultilineLogStringNative*>(d);
         auto* sd = (ps || pm) ? dynamic_cast<ProcessorParseDelimiterNative*>(second) : nullptr;
         auto* sj = (ps || pm) ? dynamic_cast<ProcessorParseJsonNative*>(second) : nullptr;
-        if (!((pd || ps || pm) && r) && !sd && !sj)
+        auto* sa = (ps || pm) ? dynamic_cast<ProcessorParseApsaraNative*>(second) : nullptr;
+        if (!((pd || ps || pm) && r) && !sd && !sj && !sa)
             throw std::runtime_error("not a processor_parse_delimiter_native or a splitter, and a "
                                      "processor_parse_regex_native; nor a splitter and a "
-                                     "processor_parse_delimiter_native or processor_parse_json_native");
+                                     "processor_parse_delimiter_native, processor_parse_json_native or "
+                                     "processor_parse_apsara_native");
         // the chain's SerializeSls / SerializeSlsLz4 on whichever processor comes first, with the second as next
         auto chain = [&](auto* p, auto& next, PipelineEventGroup& g, std::string& res, uint64_t& raw,
                          std::string& err) {
@@ -325,7 +327,8 @@ char* lc_host_chain_serialize_sls(lc_host_processor_t* delim, lc_host_processor_
         } else {
             ok = r    ? first(*r, group, res, raw, err)
                  : sd ? first(*sd, group, res, raw, err)
-                      : first(*sj, group, res, raw, err);
+                 : sj ? first(*sj, group, res, raw, err)
+                      : first(*sa, group, res, raw, err);
         }
         if (d->EngineErrors() + second->EngineErrors() != errs)
             throw std::runtime_error("engine error inside Process: " + d->LastError() + second->LastError());
