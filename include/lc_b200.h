@@ -1158,6 +1158,91 @@ int lc_multiline_split_json_parse_sls_lz4(lc_engine_t* e, const lc_json_t* js, c
                                           uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
                                           uint64_t counters[3], uint64_t ml_counters[3]);
 
+/* ---- f4: the split -> JSON -> timestamp chain (the split -> JSON chain, then ProcessorParseTimestampNative with
+ * SourceKey tkey, ProcessorParseTimestampNative.cpp:100-235; a JSON-lines file whose logs take their time from one of
+ * their members) to the SLS wire format.  Pieces and the JSON stage are exactly the split -> JSON chain's (same
+ * arguments, offset metadata, refusals, record layout and erase rule).  The row rule:
+ *   - The timestamp stage sees the pieces the JSON stage kept, in piece order, as ONE group (the second-level cache
+ *     starts empty per call).  A piece the JSON stage erased (failed, without keep_fail) is no event of the stage: no
+ *     counter, no cache step.  A parsed piece left without contents ({} without an offset key or keep_succeed) is an
+ *     event: it counts key_not_found and still has no record.
+ *   - Its value under tkey, keys comparing by their rendered bytes ("time" and "\u0074ime" are one key):
+ *       a parsed piece (LC_JSON_OK): the rendered value of the LAST member keyed tkey (so tkey == SourceKey finds a
+ *       member that overwrote it), else the piece when tkey is renamed_key and keep_succeed is set, else none
+ *       (LC_TS_NOT_FOUND; tkey == SourceKey without such a member included: the stage deleted SourceKey);
+ *       a kept failure (LC_JSON_FAILED, LC_JSON_EMPTY): the piece when tkey is renamed_key, or when tkey is
+ *       "__raw_log__" and copy_raw is set, else none.
+ *     A value is read over [off, off + len) followed by NUL bytes, as lc_timestamp_parse reads every value: an
+ *     integer member is its digit span ("ts":1700000000), -0 is "0", and a non-integer number is its %f rendering.
+ *   - LC_TS_OK: the record's Time is the parsed seconds truncated to 32 bits (raised to at least 2^28 as every
+ *     record's); with enable_ns Time_ns is the parsed nanoseconds.  LC_TS_NOT_FOUND, LC_TS_FAILED: the source event's
+ *     time / time_ns.  LC_TS_DISCARDED: no record.
+ *   - Refused with LC_ERR_INVALID_ARG beyond the split -> JSON chain's refusals: tkey equal to offset_key, and a
+ *     time_ns other than LC_SLS_NO_NS with enable_ns == 0 (some records would carry Time_ns and others not).
+ *   - counters[8] (may be NULL) = the JSON stage's out_successful, out_failed, discarded, then the timestamp stage's
+ *     key_not_found, out_failed, history_failure, discarded, out_successful.
+ *
+ * lc_split_json_timestamp_tap_dev: from the DEVICE piece and JSON tables (as for lc_sls_serialize_split_json_dev) and
+ * the JSON stage's configuration, writes the value table d_val_off / d_val_len[n] that lc_timestamp_parse_dev takes
+ * with one group over d_val (ev_len LC_TS_NO_KEY: erased by the JSON stage, or no value), and copies each value into
+ * d_val: a value in the chunk to its own offset, a value in the arena to src_len + its arena offset.  val_cap must be
+ * at least src_len + the arena's bytes (lc_json_parse_dev's *arena_bytes); a value that would end past val_cap gets
+ * no value.  Only the tkey values are copied; the other bytes of d_val are left as they are.  It queues the work on
+ * the engine's stream and returns without waiting.
+ * lc_sls_serialize_split_json_timestamp_dev: lc_sls_serialize_split_json_dev's arguments plus the DEVICE results of
+ * that lc_timestamp_parse_dev call (d_ts_status, d_ts_sec, d_ts_nsec) and enable_ns.  Sizing query, capacity and the
+ * 2 GiB / 2^30 / 4 GiB rules are the sibling's. */
+int lc_split_json_timestamp_tap_dev(lc_engine_t* e, const lc_json_t* js, const uint8_t* d_src, uint64_t src_len,
+                                    const uint32_t* d_off, const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                    const uint64_t* d_first, const lc_json_entry_t* d_entries, const uint8_t* d_arena,
+                                    const char* renamed_key, uint32_t renamed_key_len, int keep_fail,
+                                    int keep_succeed, int copy_raw, const char* offset_key, uint32_t offset_key_len,
+                                    const char* tkey, uint32_t tkey_len, uint8_t* d_val, uint64_t val_cap,
+                                    uint32_t* d_val_off, uint32_t* d_val_len);
+int lc_sls_serialize_split_json_timestamp_dev(
+    lc_engine_t* e, const lc_json_t* js, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+    const uint32_t* d_len, uint64_t n, const uint8_t* d_status, const uint64_t* d_first,
+    const lc_json_entry_t* d_entries, const uint8_t* d_arena, const char* renamed_key, uint32_t renamed_key_len,
+    int keep_fail, int keep_succeed, int copy_raw, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+    uint32_t time, uint32_t time_ns, const uint8_t* d_ts_status, const int64_t* d_ts_sec, const uint32_t* d_ts_nsec,
+    int enable_ns, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len, uint64_t counters[8]);
+
+/* The same with a HOST source value: upload it once, split, run the JSON passes, the tap, both timestamp passes (ts
+ * compiled by lc_timestamp_compile; now = time(NULL) of the call, discard_interval as for lc_timestamp_parse, -1 = no
+ * history discard), size and emit (and LZ4), and bring back only the bytes.  The value and timestamp tables stay in
+ * the engine's buffers.  *n_events, ml_counters, the tail, raw_len and the behaviour on LC_ERR_CAPACITY are as for
+ * lc_split_json_parse_sls.  A chunk whose pieces are all erased or discarded gives 0 bytes (the LZ4 calls: the block
+ * of the tail alone). */
+int lc_split_json_timestamp_parse_sls(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                                      uint8_t split_char, const char* renamed_key, uint32_t renamed_key_len,
+                                      int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+                                      uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+                                      const char* tkey, uint32_t tkey_len, const struct lc_timestamp* ts, int64_t now,
+                                      int32_t discard_interval, int enable_ns, uint8_t* out, uint64_t out_cap,
+                                      uint64_t* out_len, uint64_t* n_events, uint64_t counters[8]);
+int lc_split_json_timestamp_parse_sls_lz4(
+    lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len, uint8_t split_char,
+    const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw,
+    const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+    const char* tkey, uint32_t tkey_len, const struct lc_timestamp* ts, int64_t now, int32_t discard_interval,
+    int enable_ns, const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
+    uint64_t* raw_len, uint64_t* n_events, uint64_t counters[8]);
+int lc_multiline_split_json_timestamp_parse_sls(
+    lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+    const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, const char* renamed_key,
+    uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+    uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns, const char* tkey, uint32_t tkey_len,
+    const struct lc_timestamp* ts, int64_t now, int32_t discard_interval, int enable_ns, uint8_t* out,
+    uint64_t out_cap, uint64_t* out_len, uint64_t* n_events, uint64_t counters[8], uint64_t ml_counters[3]);
+int lc_multiline_split_json_timestamp_parse_sls_lz4(
+    lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+    const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, const char* renamed_key,
+    uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+    uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns, const char* tkey, uint32_t tkey_len,
+    const struct lc_timestamp* ts, int64_t now, int32_t discard_interval, int enable_ns, const uint8_t* tail,
+    uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+    uint64_t counters[8], uint64_t ml_counters[3]);
+
 /* ---- f4: the split -> Apsara chain (ProcessorSplitLogStringNative or ProcessorSplitMultilineLogStringNative, then
  * ProcessorParseApsaraNative with the same SourceKey -- input_file, processor_parse_apsara_native, a flusher) to the
  * SLS wire format.  The source event is flat, as for the split -> JSON chain: SourceKey (ap's) -> the value, with its

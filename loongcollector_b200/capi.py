@@ -139,6 +139,20 @@ def lib():
         [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
     L.lc_multiline_split_json_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sj_cfg + \
         [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
+    # the split -> JSON -> timestamp chain: the split -> JSON arguments with the timestamp stage behind time_ns
+    sjt_ts = [C.c_char_p, u32, vp, C.c_int64, i32, i32]  # tkey, tkey_len, ts, now, discard_interval, enable_ns
+    L.lc_split_json_timestamp_tap_dev.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, C.c_char_p, u32, i32,
+                                                  i32, i32, C.c_char_p, u32, C.c_char_p, u32, vp, u64, vp, vp]
+    L.lc_sls_serialize_split_json_timestamp_dev.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp, vp, vp] + sj_cfg + \
+        [vp, vp, vp, i32, vp, u64, C.POINTER(u64), vp]
+    L.lc_split_json_timestamp_parse_sls.argtypes = [vp, vp, vp, u64, u8] + sj_cfg + sjt_ts + \
+        [vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_split_json_timestamp_parse_sls_lz4.argtypes = [vp, vp, vp, u64, u8] + sj_cfg + sjt_ts + \
+        [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_multiline_split_json_timestamp_parse_sls.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sj_cfg + sjt_ts + \
+        [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
+    L.lc_multiline_split_json_timestamp_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sj_cfg + \
+        sjt_ts + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
     sa_cfg = [C.c_char_p, u32, i32, i32, i32] + sr_tail + [i32]  # renamed_key .. enable_ns of the split -> Apsara chain
     sa_now = [C.c_int64, i32]  # now, discard_interval
     L.lc_sls_serialize_split_apsara_dev.argtypes = [vp, vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, vp, vp] + sa_cfg + \
@@ -1488,19 +1502,21 @@ class Engine:
         return int(need.value), ctr
 
     def _split_json(self, fn, js, buf, extra, renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos,
-                    time, time_ns, out_cap, ml, tail):
+                    time, time_ns, out_cap, ml, tail, ts_args=None):
         """one host-buffer split -> JSON call, sized by an estimate first and by the exact size when that was short;
-        tail None: the wire bytes, else records ‖ tail as one LZ4 block.  Returns (bytes, raw_len, n_events,
-        counters[3], ml_counters[3] or None)"""
+        tail None: the wire bytes, else records ‖ tail as one LZ4 block; ts_args: the timestamp stage of the
+        split -> JSON -> timestamp calls (_ts_args).  Returns (bytes, raw_len, n_events, counters[3], or [8] with
+        ts_args, ml_counters[3] or None)"""
         a = _u8(buf)
-        cfg = self._sj_cfg(renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos, time, time_ns)
+        cfg = self._sj_cfg(renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos, time, time_ns) + \
+            (ts_args or [])
         tl = None if tail is None else np.frombuffer(bytes(tail), np.uint8)
         est = 2 * a.size + 4096 + (0 if tl is None else tl.size)
         cap = int(out_cap if out_cap is not None else est + est // 255 + 16)
         for _ in range(2):
             out = np.empty(max(cap, 1), np.uint8)
             need, raw, nev = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
-            ctr, mctr = np.zeros(3, np.uint64), np.zeros(3, np.uint64)
+            ctr, mctr = np.zeros(8 if ts_args else 3, np.uint64), np.zeros(3, np.uint64)
             z = [] if tl is None else [_p(tl) if tl.size else None, tl.size]
             outs = [_p(out), cap, C.byref(need)] + ([] if tl is None else [C.byref(raw)]) + [C.byref(nev), _p(ctr)]
             rc = fn(self._h, js._h, _p(a), a.size, *extra, *cfg, *z, *outs, *([_p(mctr)] if ml else []))
@@ -1549,6 +1565,89 @@ class Engine:
         return self._split_json(
             lib().lc_multiline_split_json_parse_sls_lz4, js, buf, [_rh(start), _rh(cont), _rh(end), int(bool(discard))],
             renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos, time, time_ns, out_cap, True, tail)
+
+    def split_json_timestamp_tap_dev(self, js, d_src, src_len, d_off, d_len, n, d_status, d_first, d_entries,
+                                     d_arena, renamed_key, tkey, d_val, val_cap, d_val_off, d_val_len,
+                                     keep_fail=False, keep_succeed=False, copy_raw=False, offset_key=None):
+        """The timestamp stage's value table (d_val_off, d_val_len; LC_TS_NO_KEY = no value) over d_val, with each
+        value copied into d_val (val_cap >= src_len + the arena's bytes), from the device piece and JSON tables of
+        the split -> JSON chain (lc_split_json_timestamp_tap_dev); queued, not waited for."""
+        r = renamed_key or b""
+        _check(lib().lc_split_json_timestamp_tap_dev(
+            self._h, js._h, _p(d_src), src_len, _p(d_off), _p(d_len), n, _p(d_status), _p(d_first), _p(d_entries),
+            _p(d_arena), r, len(r), int(bool(keep_fail)), int(bool(keep_succeed)), int(bool(copy_raw)),
+            *self._sr_tail(offset_key, 0, 0, None)[:2], tkey, len(tkey), _p(d_val), val_cap, _p(d_val_off),
+            _p(d_val_len)))
+
+    def sls_serialize_split_json_timestamp_dev(self, js, d_src, src_len, d_off, d_len, n, d_status, d_first,
+                                               d_entries, d_arena, renamed_key, d_ts_status, d_ts_sec, d_ts_nsec,
+                                               enable_ns=False, keep_fail=False, keep_succeed=False, copy_raw=False,
+                                               offset_key=None, src_pos=0, time=0, time_ns=None, d_out=None,
+                                               out_cap=0):
+        """sls_serialize_split_json_dev with each record's time from the device results of timestamp_parse_dev over
+        the tap's value table (lc_sls_serialize_split_json_timestamp_dev).  Returns (byte count, counters[8] = the
+        JSON stage's three, then key_not_found, out_failed, history_failure, discarded, out_successful); with d_out
+        None the byte count needed."""
+        need = C.c_uint64(0)
+        ctr = np.zeros(8, np.uint64)
+        rc = lib().lc_sls_serialize_split_json_timestamp_dev(
+            self._h, js._h, _p(d_src), src_len, _p(d_off), _p(d_len), n, _p(d_status), _p(d_first), _p(d_entries),
+            _p(d_arena), *self._sj_cfg(renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos, time,
+                                       time_ns), _p(d_ts_status), _p(d_ts_sec), _p(d_ts_nsec), int(bool(enable_ns)),
+            _p(d_out), out_cap, C.byref(need), _p(ctr))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value), ctr  # a sizing query
+        _check(rc)
+        return int(need.value), ctr
+
+    def split_json_timestamp_parse_sls(self, js, buf, split_char, renamed_key, tkey, ts, now, discard_interval=-1,
+                                       enable_ns=False, keep_fail=False, keep_succeed=False, copy_raw=False,
+                                       offset_key=None, src_pos=0, time=0, time_ns=None, out_cap=None):
+        """split_json_parse_sls with ProcessorParseTimestampNative (SourceKey tkey, the compiled Timestamp ts) behind
+        the JSON stage (lc_split_json_timestamp_parse_sls).  Returns (bytes, number of pieces, counters[8])."""
+        data, _raw, nev, ctr, _m = self._split_json(
+            lib().lc_split_json_timestamp_parse_sls, js, buf, [split_char], renamed_key, keep_fail, keep_succeed,
+            copy_raw, offset_key, src_pos, time, time_ns, out_cap, False, None,
+            self._ts_args(tkey, ts, now, discard_interval, enable_ns))
+        return data, nev, ctr
+
+    def split_json_timestamp_parse_sls_lz4(self, js, buf, split_char, renamed_key, tkey, ts, now,
+                                           discard_interval=-1, enable_ns=False, keep_fail=False,
+                                           keep_succeed=False, copy_raw=False, offset_key=None, src_pos=0, time=0,
+                                           time_ns=None, tail=b"", out_cap=None):
+        """split_json_timestamp_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_split_json_timestamp_parse_sls_lz4).  Returns (block, raw_len, number of pieces, counters[8])."""
+        data, raw, nev, ctr, _m = self._split_json(
+            lib().lc_split_json_timestamp_parse_sls_lz4, js, buf, [split_char], renamed_key, keep_fail, keep_succeed,
+            copy_raw, offset_key, src_pos, time, time_ns, out_cap, False, tail,
+            self._ts_args(tkey, ts, now, discard_interval, enable_ns))
+        return data, raw, nev, ctr
+
+    def multiline_split_json_timestamp_parse_sls(self, js, buf, start, cont, end, discard, renamed_key, tkey, ts, now,
+                                                 discard_interval=-1, enable_ns=False, keep_fail=False,
+                                                 keep_succeed=False, copy_raw=False, offset_key=None, src_pos=0,
+                                                 time=0, time_ns=None, out_cap=None):
+        """The same with the multiline splitter (lc_multiline_split_json_timestamp_parse_sls).  Returns (bytes,
+        number of events, counters[8], splitter counters[3])."""
+        data, _raw, nev, ctr, mctr = self._split_json(
+            lib().lc_multiline_split_json_timestamp_parse_sls, js, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], renamed_key, keep_fail, keep_succeed, copy_raw,
+            offset_key, src_pos, time, time_ns, out_cap, True, None,
+            self._ts_args(tkey, ts, now, discard_interval, enable_ns))
+        return data, nev, ctr, mctr
+
+    def multiline_split_json_timestamp_parse_sls_lz4(self, js, buf, start, cont, end, discard, renamed_key, tkey, ts,
+                                                     now, discard_interval=-1, enable_ns=False, keep_fail=False,
+                                                     keep_succeed=False, copy_raw=False, offset_key=None, src_pos=0,
+                                                     time=0, time_ns=None, tail=b"", out_cap=None):
+        """multiline_split_json_timestamp_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_multiline_split_json_timestamp_parse_sls_lz4).  Returns (block, raw_len, number of events,
+        counters[8], splitter counters[3])."""
+        return self._split_json(
+            lib().lc_multiline_split_json_timestamp_parse_sls_lz4, js, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], renamed_key, keep_fail, keep_succeed, copy_raw,
+            offset_key, src_pos, time, time_ns, out_cap, True, tail,
+            self._ts_args(tkey, ts, now, discard_interval, enable_ns))
 
     def _sa_cfg(self, renamed_key, keep_fail, keep_succeed, copy_raw, offset_key, src_pos, time, time_ns, enable_ns):
         r = renamed_key or b""

@@ -135,6 +135,9 @@ struct lc_engine {
     // split -> JSON -> SLS chain: the resolve's per-entry winners, per-piece records, list of pieces to sort (behind
     // its count) and sort scratch; the chain's piece and JSON tables are in, out_a, out_b and the js_* buffers
     DevBuf sj_win, sj_ev, sj_list, sj_sort;
+    // split -> JSON -> timestamp chain: the value buffer the tap copies each piece's value into (chunk bytes, then arena
+    // bytes); its value and timestamp tables are the split -> regex -> timestamp chain's st_* buffers
+    DevBuf sjt_val;
     // split -> Apsara -> SLS chain: its one-group table; the piece and Apsara tables are in, out_a, out_b and the ap_*
     // buffers
     DevBuf sa_grp;
@@ -360,7 +363,7 @@ void lc_engine_destroy(lc_engine_t* e) {
                       &e->ap_micro, &e->ap_first, &e->ap_ent, &e->js_conf, &e->js_nent, &e->js_narena,
                       &e->js_slow, &e->js_list, &e->js_afirst, &e->js_small, &e->js_status, &e->js_first, &e->js_ent,
                       &e->js_arena, &e->js_cnt, &e->js_pow5, &e->sj_win, &e->sj_ev, &e->sj_list, &e->sj_sort,
-                      &e->sa_grp};
+                      &e->sa_grp, &e->sjt_val};
     for (DevBuf* b : bufs)
         b->release();
     for (auto& kv : e->blobs)
@@ -4760,23 +4763,29 @@ int lc_json_parse(lc_engine_t* e, const lc_json_t* js, const uint8_t* base, uint
 namespace {
 
 // lc_split_json_sls_setup over js's SourceKey, with SourceKey, RenamedSourceKey, the offset key and "__raw_log__"
-// staged on the device (`sls_plan`, which neither splitter nor the JSON stage uses) and *c pointing at them
+// staged on the device (`sls_plan`, which neither splitter nor the JSON stage uses) and *c pointing at them.  With ta
+// (the timestamp calls), the timestamp stage's SourceKey is checked into *tc (lc_split_json_ts_setup) and staged
+// behind them.
 int split_json_sls_config(lc_engine_t* e, const char* what, const lc_json_t* js, SPLIT_JSON_PARAMS,
-                          LcSplitJsonSlsCfg* c) {
+                          LcSplitJsonSlsCfg* c, const TsArgs* ta = nullptr, LcSplitJsonTsCfg* tc = nullptr) {
     if (!js || (renamed_key_len && !renamed_key) || (offset_key_len && !offset_key))
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
-    const uint32_t oklen = offset_key ? offset_key_len : 0u;
-    if ((uint64_t)js->skey.size() + renamed_key_len + oklen + 16 > 0xFFFFFFFFull)
+    const uint32_t oklen = offset_key ? offset_key_len : 0u, tklen = ta ? ta->tkey_len : 0u;
+    if ((uint64_t)js->skey.size() + renamed_key_len + oklen + tklen + 16 > 0xFFFFFFFFull)
         return fail(LC_ERR_TOO_LARGE, std::string(what) + ": keys must stay below 4 GiB");
     const char* why = lc_split_json_sls_setup(js->skey.data(), (uint32_t)js->skey.size(), renamed_key,
                                               renamed_key_len, offset_key, oklen, keep_fail, keep_succeed, copy_raw,
                                               src_pos, time, time_ns, c);
+    if (!why && ta)
+        why = lc_split_json_ts_setup(*c, ta->tkey, tklen, ta->enable_ns, tc);
     if (why)
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
     std::string keys = js->skey;
     keys.append(renamed_key ? renamed_key : "", renamed_key_len);
     keys.append(offset_key ? offset_key : "", oklen);
     keys.append("__raw_log__", 11);
+    if (ta)
+        keys.append(ta->tkey ? ta->tkey : "", tklen);
     CU_TRY(e->sls_plan.ensure(keys.size() + 1));
     if (!keys.empty())
         CU_TRY(cudaMemcpyAsync(e->sls_plan.p, keys.data(), keys.size(), cudaMemcpyHostToDevice, e->stream));
@@ -4785,15 +4794,48 @@ int split_json_sls_config(lc_engine_t* e, const char* what, const lc_json_t* js,
     c->rkey = d + c->sklen;
     c->okey = d + c->sklen + c->rklen;
     c->raw = c->okey + c->oklen;
+    if (ta)
+        tc->tkey = c->raw + 11;
     return LC_OK;
+}
+
+// The split -> JSON -> timestamp chain's tap and timestamp passes over the n pieces of t (a: the arena's bytes): the
+// value buffer `sjt_val` and the value table into st_val, then lc_timestamp_parse_dev's two passes with the whole
+// source value as one group into *ts (st_status, st_sec, st_nsec).  The stage's counters are the size pass's, so the
+// passes' own go to ts_cnt unread.
+int split_json_ts_run(lc_engine_t* e, const LcSplitJsonSlsCfg& c, LcSplitJsonTsCfg tc, const TsArgs& ta,
+                      const lck::SplitJsonSlsTables& t, uint64_t n, uint64_t src_len, uint64_t a,
+                      lck::TsRowTables* ts) {
+    CU_TRY(e->st_val.ensure(n * 8 + 8));
+    CU_TRY(e->st_sec.ensure(n * 8));
+    CU_TRY(e->st_nsec.ensure(n * 4));
+    CU_TRY(e->st_status.ensure(n));
+    CU_TRY(e->ts_cnt.ensure(5 * sizeof(uint64_t)));
+    CU_TRY(e->sjt_val.ensure(src_len + a + 16));
+    tc.arena_at = src_len;
+    tc.val_cap = src_len + a;
+    uint32_t* off = e->st_val.as<uint32_t>();
+    uint32_t *len = off + n, *grp = off + 2 * n;
+    const uint32_t g[2] = {0u, (uint32_t)n};
+    CU_TRY(cudaMemcpyAsync(grp, g, sizeof g, cudaMemcpyHostToDevice, e->stream));
+    lck::launch_split_json_ts_tap(c, tc, t, n, e->sjt_val.as<uint8_t>(), off, len, e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    const int rc = ts_run(e, ta.ts, e->sjt_val.as<uint8_t>(), LcTsSpans{off, len, nullptr, 1}, n, grp, 1, ta.now,
+                          ta.discard_interval, e->st_sec.as<int64_t>(), e->st_nsec.as<uint32_t>(),
+                          e->st_status.as<uint8_t>(), e->ts_cnt.as<uint64_t>());
+    *ts = lck::TsRowTables{e->st_status.as<uint8_t>(), e->st_sec.as<int64_t>(), e->st_nsec.as<uint32_t>()};
+    return rc;
 }
 
 // The resolve pass, the size pass and the emit of the chain over the n pieces of t (m entries in all; t.win and t.ev
 // are set here): into d_out (the device-fed call), or back to the host buffer out, or -- with z -- records ‖ tail as
-// one LZ4 block.  counters[3] = successful, failed, discarded; set whenever the size pass ran.
+// one LZ4 block.  counters[3] = successful, failed, discarded; set whenever the size pass ran.  With tc (the timestamp
+// calls), each record's time comes from the timestamp tables ts and counters has LC_SRTS_COUNTERS entries.
 int split_json_sls_run(lc_engine_t* e, const char* what, const LcSplitJsonSlsCfg& c, lck::SplitJsonSlsTables t,
                        uint64_t n, uint64_t m, uint8_t* d_out, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
-                       uint64_t* counters, const Lz4Tail* z) {
+                       uint64_t* counters, const Lz4Tail* z, const LcSplitJsonTsCfg* tc = nullptr,
+                       const lck::TsRowTables* ts = nullptr) {
     CU_TRY(e->sj_win.ensure(m * 4 + 4));
     CU_TRY(e->sj_ev.ensure(n * sizeof(LcJsonSlsEv)));
     CU_TRY(e->sj_list.ensure(n * 4 + 4));
@@ -4805,40 +4847,50 @@ int split_json_sls_run(lc_engine_t* e, const char* what, const LcSplitJsonSlsCfg
     lck::launch_json_resolve(c, t, n, m, nlist + 1, nlist, e->sj_sort.as<uint32_t>(), e->stream);
     e->launches += 2;
     CU_TRY(cudaGetLastError());
-    uint64_t ctr[4] = {0};
+    const uint32_t nstage = tc ? LC_SRTS_COUNTERS : 3u;
+    uint64_t ctr[LC_SRTS_COUNTERS + 1] = {0}; // + pieces whose record would reach 4 GiB
     SlsTo to;
     to.host = out;
     to.z = z;
-    to.too_large = 3;
+    to.too_large = (int)nstage;
     const int rc = serialize_sls_dev(
-        e, what, n, 4,
+        e, what, n, nstage + 1,
         [&](uint32_t* rec, uint32_t* body, unsigned long long* d_ctr) {
-            lck::launch_split_json_sls_sizes(c, t, n, rec, body, d_ctr, e->stream);
+            if (tc)
+                lck::launch_split_json_ts_sls_sizes(c, *tc, t, *ts, n, rec, body, d_ctr, e->stream);
+            else
+                lck::launch_split_json_sls_sizes(c, t, n, rec, body, d_ctr, e->stream);
         },
         [&](const uint64_t* rec_off, const uint32_t* body, uint8_t* dst) {
-            lck::launch_split_json_sls_emit(c, t, n, rec_off, body, dst, e->stream);
+            if (tc)
+                lck::launch_split_json_ts_sls_emit(c, *tc, t, *ts, n, rec_off, body, dst, e->stream);
+            else
+                lck::launch_split_json_sls_emit(c, t, n, rec_off, body, dst, e->stream);
         },
         d_out, out_cap, out_len, ctr, to);
     if (counters)
-        memcpy(counters, ctr, 3 * sizeof(uint64_t));
+        memcpy(counters, ctr, nstage * sizeof(uint64_t));
     return rc;
 }
 
 // Host-buffer split + JSON + serialise (lc_split_json_parse_sls and the multiline / LZ4 siblings): the JSON stage
-// runs js_count / js_emit over the pieces into the js_* buffers of lc_json_parse, then split_json_sls_run.
+// runs js_count / js_emit over the pieces into the js_* buffers of lc_json_parse, then split_json_sls_run.  With ta
+// (the _timestamp_ calls), the tap and the timestamp passes run between them and counters has LC_SRTS_COUNTERS
+// entries.
 template <class Split>
 int split_json_sls_host(lc_engine_t* e, const char* what, const lc_json_t* js, const uint8_t* buf, uint64_t len,
                         Split split, SPLIT_JSON_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
-                        uint64_t* n_events, uint64_t* counters, const Lz4Tail* z) {
+                        uint64_t* n_events, uint64_t* counters, const Lz4Tail* z, const TsArgs* ta = nullptr) {
     LcSplitJsonSlsCfg c;
+    LcSplitJsonTsCfg tc;
     auto begin = [&]() {
         if (counters)
-            memset(counters, 0, 3 * sizeof(uint64_t));
+            memset(counters, 0, (ta ? LC_SRTS_COUNTERS : 3) * sizeof(uint64_t));
         if (len >= LC_JSON_ARENA)
             return fail(LC_ERR_TOO_LARGE, std::string(what) + ": the source value must be < 2 GiB");
         return (int)LC_OK;
     };
-    auto config = [&]() { return split_json_sls_config(e, what, js, SPLIT_JSON_ARGS, &c); };
+    auto config = [&]() { return split_json_sls_config(e, what, js, SPLIT_JSON_ARGS, &c, ta, &tc); };
     auto run = [&](uint64_t n) {
         if (n >= (1ull << 30))
             return fail(LC_ERR_TOO_LARGE, std::string(what) + ": < 2^30 pieces per call");
@@ -4862,20 +4914,64 @@ int split_json_sls_host(lc_engine_t* e, const char* what, const lc_json_t* js, c
         }
         const lck::SplitJsonSlsTables t{d_src, off, ln, e->js_status.as<uint8_t>(), e->js_first.as<uint64_t>(),
                                         e->js_ent.as<LcJsonEntry>(), e->js_arena.as<uint8_t>(), nullptr, nullptr};
-        return split_json_sls_run(e, what, c, t, n, m, nullptr, out, out_cap, out_len, counters, z);
+        lck::TsRowTables ts{};
+        if (ta) {
+            rc = split_json_ts_run(e, c, tc, *ta, t, n, len, a, &ts);
+            if (rc)
+                return rc;
+        }
+        return split_json_sls_run(e, what, c, t, n, m, nullptr, out, out_cap, out_len, counters, z,
+                                  ta ? &tc : nullptr, &ts);
     };
-    return split_chain_sls_host(e, what, buf, len, split, js != nullptr, begin, config, run, out, out_cap, out_len,
-                                n_events, z);
+    return split_chain_sls_host(e, what, buf, len, split, js != nullptr && (!ta || ta->ts), begin, config, run, out,
+                                out_cap, out_len, n_events, z);
 }
 
 template <class Split>
 int split_json_lz4_host(lc_engine_t* e, const char* what, const lc_json_t* js, const uint8_t* buf, uint64_t len,
                         Split split, SPLIT_JSON_PARAMS, const uint8_t* tail, uint64_t tail_len, uint8_t* out,
                         uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
-                        uint64_t* counters) {
+                        uint64_t* counters, const TsArgs* ta = nullptr) {
     const Lz4Tail z{tail, tail_len, raw_len};
     return split_json_sls_host(e, what, js, buf, len, split, SPLIT_JSON_ARGS, out, out_cap, out_len, n_events,
-                               counters, &z);
+                               counters, &z, ta);
+}
+
+// lc_sls_serialize_split_json_dev and its _timestamp_ sibling (tc, ts: the timestamp tables; counters then has
+// LC_SRTS_COUNTERS entries)
+int split_json_sls_dev(lc_engine_t* e, const char* what, const lc_json_t* js, const uint8_t* d_src, uint64_t src_len,
+                       const uint32_t* d_off, const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                       const uint64_t* d_first, const lc_json_entry_t* d_entries, const uint8_t* d_arena,
+                       SPLIT_JSON_PARAMS, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len, uint64_t* counters,
+                       const LcSplitJsonTsCfg* tc = nullptr, const lck::TsRowTables* ts = nullptr) {
+    if (!e || !js || !out_len || (n && (!d_src || !d_off || !d_len || !d_status || !d_first)) ||
+        (n && tc && (!ts->status || !ts->sec || !ts->nsec)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (counters)
+        memset(counters, 0, (tc ? LC_SRTS_COUNTERS : 3) * sizeof(uint64_t));
+    if (src_len >= LC_JSON_ARENA || n >= (1ull << 30))
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": the source value must be < 2 GiB, < 2^30 pieces per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcSplitJsonSlsCfg c;
+    rc = split_json_sls_config(e, what, js, SPLIT_JSON_ARGS, &c);
+    if (rc)
+        return rc;
+    const char* why = tc ? lc_split_regex_ts_ns_check(c, (int)tc->enable_ns) : nullptr;
+    if (why)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    if (n == 0)
+        return LC_OK;
+    uint64_t m = 0;
+    CU_TRY(cudaMemcpyAsync(&m, d_first + n, 8, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(cudaStreamSynchronize(e->stream));
+    if (m && (!d_entries || !d_arena))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    const lck::SplitJsonSlsTables t{d_src, d_off, d_len, d_status, d_first,
+                                    reinterpret_cast<const LcJsonEntry*>(d_entries), d_arena, nullptr, nullptr};
+    return split_json_sls_run(e, what, c, t, n, m, d_out, nullptr, out_cap, out_len, counters, nullptr, tc, ts);
 }
 
 } // namespace
@@ -4895,29 +4991,8 @@ int lc_sls_serialize_split_json_dev(lc_engine_t* e, const lc_json_t* js, const u
                                     const uint64_t* d_first, const lc_json_entry_t* d_entries, const uint8_t* d_arena,
                                     SPLIT_JSON_PARAMS, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len,
                                     uint64_t counters[3]) {
-    static const char* what = "lc_sls_serialize_split_json_dev";
-    if (!e || !js || !out_len || (n && (!d_src || !d_off || !d_len || !d_status || !d_first)))
-        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
-    *out_len = 0;
-    if (counters)
-        memset(counters, 0, 3 * sizeof(uint64_t));
-    if (src_len >= LC_JSON_ARENA || n >= (1ull << 30))
-        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": the source value must be < 2 GiB, < 2^30 pieces per call");
-    int rc = bind(e);
-    if (rc)
-        return rc;
-    LcSplitJsonSlsCfg c;
-    rc = split_json_sls_config(e, what, js, SPLIT_JSON_ARGS, &c);
-    if (rc || n == 0)
-        return rc;
-    uint64_t m = 0;
-    CU_TRY(cudaMemcpyAsync(&m, d_first + n, 8, cudaMemcpyDeviceToHost, e->stream));
-    CU_TRY(cudaStreamSynchronize(e->stream));
-    if (m && (!d_entries || !d_arena))
-        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
-    const lck::SplitJsonSlsTables t{d_src, d_off, d_len, d_status, d_first,
-                                    reinterpret_cast<const LcJsonEntry*>(d_entries), d_arena, nullptr, nullptr};
-    return split_json_sls_run(e, what, c, t, n, m, d_out, nullptr, out_cap, out_len, counters, nullptr);
+    return split_json_sls_dev(e, "lc_sls_serialize_split_json_dev", js, d_src, src_len, d_off, d_len, n, d_status,
+                              d_first, d_entries, d_arena, SPLIT_JSON_ARGS, d_out, out_cap, out_len, counters);
 }
 
 int lc_split_json_parse_sls(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len, uint8_t split_char,
@@ -4961,6 +5036,114 @@ int lc_multiline_split_json_parse_sls_lz4(lc_engine_t* e, const lc_json_t* js, c
     return split_json_lz4_host(e, "lc_multiline_split_json_parse_sls_lz4", js, buf, len, ML_SPLIT, SPLIT_JSON_ARGS,
                                tail, tail_len, out, out_cap, out_len, raw_len, n_events, counters);
 }
+
+int lc_split_json_timestamp_tap_dev(lc_engine_t* e, const lc_json_t* js, const uint8_t* d_src, uint64_t src_len,
+                                    const uint32_t* d_off, const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                    const uint64_t* d_first, const lc_json_entry_t* d_entries, const uint8_t* d_arena,
+                                    const char* renamed_key, uint32_t renamed_key_len, int keep_fail,
+                                    int keep_succeed, int copy_raw, const char* offset_key, uint32_t offset_key_len,
+                                    const char* tkey, uint32_t tkey_len, uint8_t* d_val, uint64_t val_cap,
+                                    uint32_t* d_val_off, uint32_t* d_val_len) {
+    static const char* what = "lc_split_json_timestamp_tap_dev";
+    if (!e || !js || (n && (!d_src || !d_off || !d_len || !d_status || !d_first || !d_val || !d_val_off ||
+                            !d_val_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    if (src_len >= LC_JSON_ARENA || n >= (1ull << 30))
+        return fail(LC_ERR_TOO_LARGE, std::string(what) + ": the source value must be < 2 GiB, < 2^30 pieces per call");
+    if (n && val_cap < src_len)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": the value buffer must hold src_len + arena bytes");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    const uint64_t src_pos = 0;
+    const uint32_t time = 0, time_ns = LC_SLS_NO_NS;
+    const TsArgs ta{tkey, tkey_len, nullptr, 0, -1, 0};
+    LcSplitJsonSlsCfg c;
+    LcSplitJsonTsCfg tc;
+    rc = split_json_sls_config(e, what, js, SPLIT_JSON_ARGS, &c, &ta, &tc);
+    if (rc || n == 0)
+        return rc;
+    tc.arena_at = src_len;
+    tc.val_cap = val_cap;
+    const lck::SplitJsonSlsTables t{d_src, d_off, d_len, d_status, d_first,
+                                    reinterpret_cast<const LcJsonEntry*>(d_entries), d_arena, nullptr, nullptr};
+    lck::launch_split_json_ts_tap(c, tc, t, n, d_val, d_val_off, d_val_len, e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    return LC_OK;
+}
+
+int lc_sls_serialize_split_json_timestamp_dev(lc_engine_t* e, const lc_json_t* js, const uint8_t* d_src,
+                                              uint64_t src_len, const uint32_t* d_off, const uint32_t* d_len,
+                                              uint64_t n, const uint8_t* d_status, const uint64_t* d_first,
+                                              const lc_json_entry_t* d_entries, const uint8_t* d_arena,
+                                              SPLIT_JSON_PARAMS, const uint8_t* d_ts_status, const int64_t* d_ts_sec,
+                                              const uint32_t* d_ts_nsec, int enable_ns, uint8_t* d_out,
+                                              uint64_t out_cap, uint64_t* out_len, uint64_t counters[8]) {
+    LcSplitJsonTsCfg tc;
+    memset(&tc, 0, sizeof tc);
+    tc.enable_ns = enable_ns != 0;
+    const lck::TsRowTables ts{d_ts_status, d_ts_sec, d_ts_nsec};
+    return split_json_sls_dev(e, "lc_sls_serialize_split_json_timestamp_dev", js, d_src, src_len, d_off, d_len, n,
+                              d_status, d_first, d_entries, d_arena, SPLIT_JSON_ARGS, d_out, out_cap, out_len,
+                              counters, &tc, &ts);
+}
+
+#define TS_ARGS_OF_CALL const TsArgs ta{tkey, tkey_len, ts, now, discard_interval, enable_ns};
+
+int lc_split_json_timestamp_parse_sls(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                                      uint8_t split_char, SPLIT_JSON_PARAMS, const char* tkey, uint32_t tkey_len,
+                                      const lc_timestamp_t* ts, int64_t now, int32_t discard_interval, int enable_ns,
+                                      uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                      uint64_t counters[8]) {
+    TS_ARGS_OF_CALL
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_json_sls_host(e, "lc_split_json_timestamp_parse_sls", js, buf, len, split, SPLIT_JSON_ARGS, out,
+                               out_cap, out_len, n_events, counters, nullptr, &ta);
+}
+
+int lc_split_json_timestamp_parse_sls_lz4(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len,
+                                          uint8_t split_char, SPLIT_JSON_PARAMS, const char* tkey, uint32_t tkey_len,
+                                          const lc_timestamp_t* ts, int64_t now, int32_t discard_interval,
+                                          int enable_ns, const uint8_t* tail, uint64_t tail_len, uint8_t* out,
+                                          uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                                          uint64_t counters[8]) {
+    TS_ARGS_OF_CALL
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_json_lz4_host(e, "lc_split_json_timestamp_parse_sls_lz4", js, buf, len, split, SPLIT_JSON_ARGS, tail,
+                               tail_len, out, out_cap, out_len, raw_len, n_events, counters, &ta);
+}
+
+int lc_multiline_split_json_timestamp_parse_sls(lc_engine_t* e, const lc_json_t* js, const uint8_t* buf,
+                                                uint64_t len, const lc_regex_t* start, const lc_regex_t* cont,
+                                                const lc_regex_t* end, int discard_unmatched, SPLIT_JSON_PARAMS,
+                                                const char* tkey, uint32_t tkey_len, const lc_timestamp_t* ts,
+                                                int64_t now, int32_t discard_interval, int enable_ns, uint8_t* out,
+                                                uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                                uint64_t counters[8], uint64_t ml_counters[3]) {
+    TS_ARGS_OF_CALL
+    return split_json_sls_host(e, "lc_multiline_split_json_timestamp_parse_sls", js, buf, len, ML_SPLIT,
+                               SPLIT_JSON_ARGS, out, out_cap, out_len, n_events, counters, nullptr, &ta);
+}
+
+int lc_multiline_split_json_timestamp_parse_sls_lz4(
+    lc_engine_t* e, const lc_json_t* js, const uint8_t* buf, uint64_t len, const lc_regex_t* start,
+    const lc_regex_t* cont, const lc_regex_t* end, int discard_unmatched, SPLIT_JSON_PARAMS, const char* tkey,
+    uint32_t tkey_len, const lc_timestamp_t* ts, int64_t now, int32_t discard_interval, int enable_ns,
+    const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
+    uint64_t* n_events, uint64_t counters[8], uint64_t ml_counters[3]) {
+    TS_ARGS_OF_CALL
+    return split_json_lz4_host(e, "lc_multiline_split_json_timestamp_parse_sls_lz4", js, buf, len, ML_SPLIT,
+                               SPLIT_JSON_ARGS, tail, tail_len, out, out_cap, out_len, raw_len, n_events, counters,
+                               &ta);
+}
+#undef TS_ARGS_OF_CALL
 
 } // extern "C"
 #undef ML_SPLIT

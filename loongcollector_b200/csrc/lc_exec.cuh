@@ -4156,7 +4156,9 @@ struct LcSplitRegexTsCfg {
 // Host side: whether the source event's Time_ns agrees with enable_ns.  time_ns is the source event's Time_ns as the
 // serialiser writes it, so a source Time_ns without enable_ns would give Time_ns to the records that keep the source
 // time and not to the parsed ones, a mix no configuration of the reference produces.  Returns nullptr, or why not.
-inline const char* lc_split_regex_ts_ns_check(const LcSplitRegexSlsCfg& c, int enable_ns) {
+// Cfg: the configuration of the chain in front of the timestamp stage (LcSplitRegexSlsCfg, LcSplitJsonSlsCfg).
+template <class Cfg>
+inline const char* lc_split_regex_ts_ns_check(const Cfg& c, int enable_ns) {
     return c.has_ns && !enable_ns ? "a source time_ns needs enable_ns" : nullptr;
 }
 
@@ -4209,8 +4211,9 @@ LC_HD LcSplitRegexTsTime lc_split_regex_ts_time(const LcSplitRegexSlsCfg& c, con
 // The row's counter verdicts as bits of the LC_SRTS_COUNTERS counters: the regex stage's (lc_split_regex_verdict),
 // then -- when the regex stage kept the piece -- the timestamp stage's key_not_found, out_failed, history_failure,
 // discarded, out_successful.
-LC_HD uint32_t lc_split_regex_ts_verdict(const LcSplitRegexSlsCfg& c, uint32_t status, uint32_t ts) {
-    const LcSplitRegexVerdict v = lc_split_regex_verdict(c, status);
+// The stage verdicts of a chain's row (lc_split_*_verdict) and, when the stage kept the piece, the timestamp stage's
+// key_not_found, out_failed, history_failure, discarded, out_successful as bits 3.. of the LC_SRTS_COUNTERS counters.
+LC_HD uint32_t lc_split_ts_verdict_bits(const LcSplitRegexVerdict& v, uint32_t ts) {
     uint32_t bits = v.ok | (v.failed << 1) | (v.erased << 2);
     if (v.erased)
         return bits;
@@ -4223,6 +4226,10 @@ LC_HD uint32_t lc_split_regex_ts_verdict(const LcSplitRegexSlsCfg& c, uint32_t s
     else
         bits |= 1u << (3 + LC_TS_C_OUT_SUCCESSFUL);
     return bits;
+}
+
+LC_HD uint32_t lc_split_regex_ts_verdict(const LcSplitRegexSlsCfg& c, uint32_t status, uint32_t ts) {
+    return lc_split_ts_verdict_bits(lc_split_regex_verdict(c, status), ts);
 }
 
 // ================================================================================================ Apsara parse
@@ -5723,14 +5730,15 @@ struct LcSplitJsonSlsRow {
 };
 
 // The body of the piece's Log record -- Time, its contents, Time_ns -- into sink s (LcSlsCount64 / LcSlsWrite), with
-// the source event's time and ns.  Returns the number of contents; 0 = erased or empty, no record.
+// the record's own time and ns (has_ns = 0: no Time_ns).  Returns the number of contents; 0 = erased or empty, no
+// record.
 template <class S>
 LC_HD uint32_t lc_split_json_sls_body(const LcSplitJsonSlsCfg& c, const uint8_t* src, const uint8_t* arena,
-                                      const LcSplitJsonSlsRow& r, S& s) {
+                                      const LcSplitJsonSlsRow& r, uint32_t time, uint32_t has_ns, uint32_t ns, S& s) {
     {
         uint8_t h[6];
         h[0] = 0x08;
-        const uint32_t n = 1 + lc_put_varint(h + 1, c.time < (1u << 28) ? (1u << 28) : c.time); // always 5 bytes
+        const uint32_t n = 1 + lc_put_varint(h + 1, time < (1u << 28) ? (1u << 28) : time); // always 5 bytes
         s.put(h, n);
     }
     const uint64_t pos = c.src_pos + r.po;
@@ -5775,11 +5783,18 @@ LC_HD uint32_t lc_split_json_sls_body(const LcSplitJsonSlsCfg& c, const uint8_t*
         if (c.copy_raw && !(c.has_offset && c.raw_is_off) && !c.ren_is_raw)
             piece(c.raw, 11u);
     }
-    if (c.has_ns) {
-        const uint8_t h[5] = {0x25, (uint8_t)c.ns, (uint8_t)(c.ns >> 8), (uint8_t)(c.ns >> 16), (uint8_t)(c.ns >> 24)};
+    if (has_ns) {
+        const uint8_t h[5] = {0x25, (uint8_t)ns, (uint8_t)(ns >> 8), (uint8_t)(ns >> 16), (uint8_t)(ns >> 24)};
         s.put(h, 5);
     }
     return k;
+}
+
+// ... with the source event's time and ns, as every split piece inherits them
+template <class S>
+LC_HD uint32_t lc_split_json_sls_body(const LcSplitJsonSlsCfg& c, const uint8_t* src, const uint8_t* arena,
+                                      const LcSplitJsonSlsRow& r, S& s) {
+    return lc_split_json_sls_body(c, src, arena, r, c.time, c.has_ns, c.ns, s);
 }
 
 // The piece's counter verdicts (0 / 1): ProcessorParseJsonNative's out_successful (every piece not erased),
@@ -5824,6 +5839,122 @@ inline const char* lc_split_json_sls_setup(const char* source_key, uint32_t sour
     c->has_ns = time_ns != 0xFFFFFFFFu;
     c->ns = c->has_ns ? time_ns : 0u;
     return nullptr;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, split -> JSON -> timestamp chain: ProcessorParseTimestampNative (ProcessorParseTimestampNative.cpp:100-235, the
+// SourceKey tkey) behind the split -> JSON chain, whose pieces and JSON stage are unchanged.
+//   - The timestamp stage sees the pieces the JSON stage kept, in piece order, as one group: a piece the JSON stage
+//     erased is not an event of the stage (no counter, no cache step).
+//   - Its value under tkey (keys compare by their rendered bytes): in a parsed piece, the rendered value of the LAST
+//     member keyed tkey, else the piece when tkey is RenamedSourceKey with keep_succeed, else none; in a kept failure,
+//     the piece when tkey is RenamedSourceKey, or "__raw_log__" with copy_raw, else none.  tkey equal to the offset key
+//     is refused.  Both an erased piece and no value give the tap's LC_TS_NO_KEY; the counters come from the size
+//     pass, which tells the two apart.
+//   - A value lies in the chunk (a member span or the piece) or in the arena (escaped strings, %f renderings), and the
+//     timestamp passes read one base: the tap copies each value into a buffer of src_len + arena bytes, a chunk value
+//     to its own offset and an arena value to src_len + its arena offset.  Pieces and arena spans are disjoint, so no
+//     two values share bytes.  The value is read over [off, off + len) followed by NUL bytes, as every timestamp value
+//     is.
+//   - The record's time is lc_split_regex_ts_time's rule: LC_TS_OK sets Time (and Time_ns with enable_ns),
+//     LC_TS_NOT_FOUND / LC_TS_FAILED keep the source event's, LC_TS_DISCARDED leaves no record.
+struct LcSplitJsonTsCfg {
+    const uint8_t* tkey; // the timestamp stage's SourceKey (a device copy on the device, as LcSplitJsonSlsCfg's keys)
+    uint32_t tklen;
+    uint32_t piece_ok;   // a parsed piece without a member keyed tkey holds the piece under tkey
+    uint32_t piece_fail; // a kept failure holds the piece under tkey
+    uint32_t enable_ns;  // mEnableTimestampNanosecond: a parsed time writes Time_ns
+    uint64_t arena_at;   // where the arena's bytes start in the value buffer (src_len)
+    uint64_t val_cap;    // the value buffer's size: a value that would not fit gets no value
+};
+
+// Host side: check tkey and the source Time_ns against the chain's configuration c, as lc_split_json_sls_setup left
+// it (key pointers on the host).  Returns nullptr, or why the chain is refused: tkey equal to the offset key (the
+// value would be the offset digits or an offset member), or a source Time_ns without enable_ns.
+inline const char* lc_split_json_ts_setup(const LcSplitJsonSlsCfg& c, const char* tkey, uint32_t tkey_len,
+                                          int enable_ns, LcSplitJsonTsCfg* t) {
+    if (!t || (tkey_len && !tkey))
+        return "bad arguments";
+    const char* why = lc_split_regex_ts_ns_check(c, enable_ns);
+    if (why)
+        return why;
+    const uint8_t* k = reinterpret_cast<const uint8_t*>(tkey);
+    if (c.has_offset && lc_json_key_cmp(k, tkey_len, c.okey, c.oklen) == 0)
+        return "the timestamp key equals the offset key";
+    memset(t, 0, sizeof *t);
+    t->tkey = k;
+    t->tklen = tkey_len;
+    const bool ren = lc_json_key_cmp(k, tkey_len, c.rkey, c.rklen) == 0;
+    t->piece_ok = ren && c.keep_succeed;
+    t->piece_fail = ren || (c.copy_raw && lc_json_key_cmp(k, tkey_len, c.raw, 11u) == 0);
+    t->enable_ns = enable_ns != 0;
+    return nullptr;
+}
+
+// The last of a parsed piece's m members e[0, m) whose key is tkey (LC_JSON_SLS_NONE: none), W lanes scanning W
+// members per step from the last one backward; v: W words of per-warp scratch (shared memory on the device).  Every
+// lane calls it and gets the same answer.
+LC_HD uint32_t lc_json_ts_last_member(const LcSplitJsonTsCfg& t, const uint8_t* src, const uint8_t* arena,
+                                      const LcJsonEntry* e, uint32_t m, uint32_t* v, uint32_t lane, uint32_t W) {
+    for (uint32_t top = m; top > 0;) {
+        const uint32_t nv = top < W ? top : W;
+        LC_LANES(l) {
+            uint32_t hit = 0;
+            if (l < nv) {
+                const LcJsonEntry& x = e[top - 1 - l];
+                hit = x.key_len == t.tklen &&
+                      lc_json_key_cmp(lc_json_span(src, arena, x.key_off), x.key_len, t.tkey, t.tklen) == 0;
+            }
+            v[l] = hit;
+        }
+        const uint32_t b = lc_lz4_ballot(v, lane, W);
+        LC_WARP_SYNC();
+        if (b)
+            return top - 1 - lc_lo_bit(b);
+        top -= nv;
+    }
+    return LC_JSON_SLS_NONE;
+}
+
+// The tap's value of one piece (its JSON status, the piece src[po, + plen), its entries e and lc_json_ts_last_member's
+// answer w): *from = where its bytes are (an entry offset: LC_JSON_ARENA tags the arena), *off / *len = where the
+// timestamp passes read it in the value buffer; *len = LC_TS_NO_KEY when the JSON stage erased the piece or left no
+// value under tkey.
+LC_HD void lc_split_json_ts_value(const LcSplitJsonSlsCfg& c, const LcSplitJsonTsCfg& t, uint32_t status, uint32_t po,
+                                  uint32_t plen, const LcJsonEntry* e, uint32_t w, uint32_t* from, uint32_t* off,
+                                  uint32_t* len) {
+    const bool ok = (status & 0x7Fu) == LC_JSON_ST_OK;
+    *from = *off = 0;
+    *len = LC_TS_NO_KEY;
+    uint32_t vo, vl;
+    if (!ok && !c.keep_fail)
+        return; // erased: no event of the stage
+    if (ok && w != LC_JSON_SLS_NONE)
+        vo = e[w].val_off, vl = e[w].val_len;
+    else if (ok ? t.piece_ok : t.piece_fail)
+        vo = po, vl = plen;
+    else
+        return;
+    const uint64_t at = vo & LC_JSON_ARENA ? t.arena_at + (vo & ~LC_JSON_ARENA) : (uint64_t)vo;
+    if (at + vl > t.val_cap)
+        return;
+    *from = vo;
+    *off = (uint32_t)at;
+    *len = vl;
+}
+
+// The record's time after the timestamp stage (ts: the stage's LC_TS_ST_* of the row, sec / nsec its time)
+LC_HD LcSplitRegexTsTime lc_split_json_ts_time(const LcSplitJsonSlsCfg& c, const LcSplitJsonTsCfg& t, uint32_t ts,
+                                               int64_t sec, uint32_t nsec) {
+    if (ts == LC_TS_ST_OK)
+        return {1u, (uint32_t)sec, t.enable_ns, nsec};
+    return {ts != LC_TS_ST_DISCARDED, c.time, c.has_ns, c.ns};
+}
+
+// The row's counter verdicts as bits of the LC_SRTS_COUNTERS counters: the JSON stage's (lc_split_json_verdict), then
+// -- when the JSON stage kept the piece -- the timestamp stage's five.
+LC_HD uint32_t lc_split_json_ts_verdict(const LcSplitJsonSlsCfg& c, uint32_t status, uint32_t ts) {
+    return lc_split_ts_verdict_bits(lc_split_json_verdict(c, status), ts);
 }
 
 // ------------------------------------------------------------------------------------------------------------

@@ -4837,6 +4837,132 @@ void launch_split_json_sls_emit(const LcSplitJsonSlsCfg& c, const SplitJsonSlsTa
                                                                                       d_out);
 }
 
+// ---- f4, split -> JSON -> timestamp chain (lc_exec.cuh: lc_json_ts_last_member, lc_split_json_ts_value, _time,
+// _verdict).  The tap runs one warp per piece: the lanes scan the piece's members backward for tkey, then share the
+// copy of its value into the value buffer, so a long value (a 1 MiB string member) costs its warp n / 512 steps
+// rather than n.  The size pass (one thread per piece) and the emit pass (one warp per piece) run
+// lc_split_json_sls_body with each record's own time.
+
+// n bytes s -> d by the 32 lanes of a warp: 16-byte words when both share their alignment (a chunk value, copied to
+// its own offset), else bytes
+__device__ __forceinline__ void split_json_ts_copy(uint8_t* __restrict__ d, const uint8_t* __restrict__ s, uint32_t n,
+                                                   uint32_t lane) {
+    uint32_t i = 0;
+    if ((((uintptr_t)d ^ (uintptr_t)s) & 15u) == 0) {
+        const uint32_t head = (uint32_t)((16u - ((uintptr_t)d & 15u)) & 15u);
+        i = head < n ? head : n;
+        if (lane < i)
+            d[lane] = s[lane];
+        const uint32_t words = (n - i) >> 4;
+        uint4* dw = reinterpret_cast<uint4*>(d + i);
+        const uint4* sw = reinterpret_cast<const uint4*>(s + i);
+        for (uint32_t k = lane; k < words; k += 32)
+            dw[k] = sw[k];
+        i += words << 4;
+    }
+    for (uint32_t k = i + lane; k < n; k += 32)
+        d[k] = s[k];
+}
+
+__global__ void __launch_bounds__(256)
+    split_json_ts_tap_kernel(LcSplitJsonSlsCfg c, LcSplitJsonTsCfg tc, SplitJsonSlsTables t, uint64_t n,
+                             uint8_t* __restrict__ val, uint32_t* __restrict__ off, uint32_t* __restrict__ len) {
+    __shared__ uint32_t ws[8][32];
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (i >= n)
+        return;
+    const LcJsonEntry* e = t.ent + t.first[i];
+    const uint32_t w = lc_json_ts_last_member(tc, t.src, t.arena, e, split_json_members(t, i), ws[threadIdx.x >> 5],
+                                              lane, 32);
+    uint32_t from, o, l;
+    lc_split_json_ts_value(c, tc, t.status[i], t.off[i], t.len[i], e, w, &from, &o, &l);
+    if (lane == 0) {
+        off[i] = o;
+        len[i] = l;
+    }
+    if (l != LC_TS_NO_KEY)
+        split_json_ts_copy(val + o, lc_json_span(t.src, t.arena, from), l, lane);
+}
+
+// counters: u64 [9] += the LC_SRTS_COUNTERS verdicts (one atomic per warp and counter), then pieces whose record
+// would reach 4 GiB
+__global__ void __launch_bounds__(256)
+    split_json_ts_sls_size_kernel(LcSplitJsonSlsCfg c, LcSplitJsonTsCfg tc, SplitJsonSlsTables t, TsRowTables ts,
+                                  uint64_t n, uint32_t* __restrict__ rec_size, uint32_t* __restrict__ body_size,
+                                  unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t bits = 0, big = 0;
+    if (i < n) {
+        const LcSplitJsonSlsRow r = split_json_sls_row(t, i);
+        const uint32_t st = ts.status[i];
+        const LcSplitRegexTsTime tm = lc_split_json_ts_time(c, tc, st, ts.sec[i], ts.nsec[i]);
+        LcSlsCount64 s{0};
+        const uint32_t cnt = tm.keep ? lc_split_json_sls_body(c, t.src, t.arena, r, tm.time, tm.has_ns, tm.ns, s) : 0u;
+        big = s.n + 16 > 0xFFFFFFFFull;
+        const uint32_t body = cnt && !big ? (uint32_t)s.n : 0u;
+        rec_size[i] = body ? 1 + lc_varint_size(body) + body : 0u;
+        body_size[i] = body;
+        bits = lc_split_json_ts_verdict(c, r.status, st);
+    }
+#pragma unroll
+    for (uint32_t k = 0; k < LC_SRTS_COUNTERS; ++k) {
+        const uint32_t v = __reduce_add_sync(0xFFFFFFFFu, (bits >> k) & 1u);
+        if ((threadIdx.x & 31) == 0 && v)
+            atomicAdd(counters + k, (unsigned long long)v);
+    }
+    big = __reduce_add_sync(0xFFFFFFFFu, big);
+    if ((threadIdx.x & 31) == 0 && big)
+        atomicAdd(counters + LC_SRTS_COUNTERS, (unsigned long long)big);
+}
+
+__global__ void __launch_bounds__(256)
+    split_json_ts_sls_emit_kernel(LcSplitJsonSlsCfg c, LcSplitJsonTsCfg tc, SplitJsonSlsTables t, TsRowTables ts,
+                                  uint64_t n, const uint64_t* __restrict__ rec_off,
+                                  const uint32_t* __restrict__ body_size, uint8_t* __restrict__ out) {
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n)
+        return;
+    const uint32_t body = body_size[i];
+    if (!body)
+        return; // erased, discarded or LogEvent::Empty: no record
+    const LcSplitJsonSlsRow r = split_json_sls_row(t, i);
+    // lc_split_json_ts_time's rule for a piece with a record, as selects on the kernel parameters: a struct of the
+    // three kept live across the body costs this kernel 20 bytes of spills
+    const bool ok = ts.status[i] == LC_TS_ST_OK;
+    uint8_t h[6];
+    h[0] = 0x0A;
+    const uint32_t hn = 1 + lc_put_varint(h + 1, body);
+    LcSlsWrite s{out + rec_off[i], 0u, hn + body, threadIdx.x & 31, 32};
+    s.put(h, hn);
+    lc_split_json_sls_body(c, t.src, t.arena, r, ok ? (uint32_t)ts.sec[i] : c.time, ok ? tc.enable_ns : c.has_ns,
+                           ok ? ts.nsec[i] : c.ns, s);
+}
+
+void launch_split_json_ts_tap(const LcSplitJsonSlsCfg& c, const LcSplitJsonTsCfg& tc, const SplitJsonSlsTables& t,
+                              uint64_t n, uint8_t* d_val, uint32_t* d_off, uint32_t* d_len, cudaStream_t st) {
+    if (n)
+        split_json_ts_tap_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, tc, t, n, d_val, d_off, d_len);
+}
+
+void launch_split_json_ts_sls_sizes(const LcSplitJsonSlsCfg& c, const LcSplitJsonTsCfg& tc,
+                                    const SplitJsonSlsTables& t, const TsRowTables& ts, uint64_t n,
+                                    uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                    cudaStream_t st) {
+    if (n)
+        split_json_ts_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, tc, t, ts, n, d_rec_size,
+                                                                                    d_body_size, d_counters);
+}
+
+void launch_split_json_ts_sls_emit(const LcSplitJsonSlsCfg& c, const LcSplitJsonTsCfg& tc,
+                                   const SplitJsonSlsTables& t, const TsRowTables& ts, uint64_t n,
+                                   const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                   cudaStream_t st) {
+    if (n)
+        split_json_ts_sls_emit_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, tc, t, ts, n, d_rec_off,
+                                                                                         d_body_size, d_out);
+}
+
 // ---- f4, split -> Apsara chain (lc_exec.cuh: lc_split_apsara_sls_body, lc_split_apsara_verdict).  The size pass runs
 // one thread per piece, the emit pass one warp per piece.  counters: u64 [6] += lc_apsara_parse's five, then pieces
 // whose record would reach 4 GiB.

@@ -22,6 +22,7 @@ struct LcApEv;
 struct LcApEntry;
 struct LcJsonEntry;
 struct LcSplitJsonSlsCfg;
+struct LcSplitJsonTsCfg;
 struct LcJsonSlsEv;
 struct LcSplitApsaraSlsCfg;
 struct LcLz4Chunk;
@@ -455,6 +456,22 @@ void launch_split_json_sls_sizes(const LcSplitJsonSlsCfg& c, const SplitJsonSlsT
 void launch_split_json_sls_emit(const LcSplitJsonSlsCfg& c, const SplitJsonSlsTables& t, uint64_t n,
                                 const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
                                 cudaStream_t st);
+// f4, split -> JSON -> timestamp chain (lc_exec.cuh: LcSplitJsonTsCfg).  launch_split_json_ts_tap: the dense value
+// table (d_off, d_len) over d_val that the timestamp passes take, with each value copied into d_val (tc.val_cap bytes:
+// the chunk's bytes at their own offsets, the arena's from tc.arena_at); LC_TS_NO_KEY: erased by the JSON stage, or no
+// value.  It needs no resolve pass.  The size and emit passes are launch_split_json_sls_*'s (t.win / t.ev set) with
+// each record's time from the timestamp tables ts; d_counters: u64 [9] += the chain's 8 counters (LC_SRTS_COUNTERS),
+// then pieces whose record would reach 4 GiB.
+void launch_split_json_ts_tap(const LcSplitJsonSlsCfg& c, const LcSplitJsonTsCfg& tc, const SplitJsonSlsTables& t,
+                              uint64_t n, uint8_t* d_val, uint32_t* d_off, uint32_t* d_len, cudaStream_t st);
+void launch_split_json_ts_sls_sizes(const LcSplitJsonSlsCfg& c, const LcSplitJsonTsCfg& tc,
+                                    const SplitJsonSlsTables& t, const TsRowTables& ts, uint64_t n,
+                                    uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                    cudaStream_t st);
+void launch_split_json_ts_sls_emit(const LcSplitJsonSlsCfg& c, const LcSplitJsonTsCfg& tc,
+                                   const SplitJsonSlsTables& t, const TsRowTables& ts, uint64_t n,
+                                   const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                   cudaStream_t st);
 
 // f4, split -> Apsara chain (lc_exec.cuh: LcSplitApsaraSlsCfg, keys on the device): the pieces off / len of the source
 // value src, parsed by lc_apsara_parse_dev (src as its base) into status / sec / nsec / micro / first / ent.  Sizes as

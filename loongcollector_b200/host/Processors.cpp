@@ -3862,6 +3862,153 @@ bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGrou
     mUnmatchedLinesTotal.Add(ctr[2]);
     return ok;
 }
+
+// The JSON and timestamp stages of the split -> JSON -> timestamp chain: the JSON stage as SplitJsonStage has it, the
+// timestamp stage's SourceKey, program, "now" and history discard as the chain calls take them (SPLIT_JSON_TS_ARGS),
+// and the counters both Process calls would move.  The device calls take a group of exactly one source event: the
+// second-level cache would otherwise have to carry across calls.
+struct SplitJsonTsStage {
+    SplitJsonStage s;
+    ProcessorParseTimestampNative& t;
+    const PipelineEventGroup& group;
+    int64_t now;
+    SplitJsonTsStage(ProcessorParseJsonNative& json, ProcessorParseTimestampNative& ts, const PipelineEventGroup& g)
+        : s{json}, t(ts), group(g), now((int64_t)time(nullptr)) {}
+    int32_t DiscardInterval() const { return t.mDiscardOldData ? t.mDiscardInterval : -1; }
+    const lc_timestamp_t* Program() const { return t.mProgram; }
+    // whether the chain's device calls take both stages behind a splitter reading sourceKey: lc_split_json_sls_setup
+    // and lc_split_json_ts_setup
+    bool Accepts(const std::string& sourceKey, const StringView* okey) const {
+        const ProcessorParseJsonNative& j = s.j;
+        if (group.GetEvents().size() != 1 || !t.mProgram || !s.Accepts(sourceKey, okey))
+            return false;
+        LcSplitJsonSlsCfg c;
+        lc_split_json_sls_setup(j.mSourceKey.data(), (uint32_t)j.mSourceKey.size(), s.Renamed().data(),
+                                (uint32_t)s.Renamed().size(), okey ? okey->data() : nullptr,
+                                okey ? (uint32_t)okey->size() : 0u, s.Opt().mKeepingSourceWhenParseFail,
+                                s.Opt().mKeepingSourceWhenParseSucceed, s.Opt().mCopingRawLog, 0, 0, LC_SLS_NO_NS, &c);
+        LcSplitJsonTsCfg tc;
+        return !lc_split_json_ts_setup(c, t.mSourceKey.data(), (uint32_t)t.mSourceKey.size(), 0, &tc);
+    }
+    // the device calls' counters[8] (the JSON stage's three, then the timestamp stage's key_not_found, out_failed,
+    // history_failure, discarded, out_successful) as the chain driver takes a stage's: [2] + [3] = the events the
+    // chain erased or discarded
+    static void Fold(const uint64_t c8[8], uint64_t rctr[8]) {
+        const uint64_t f[8] = {c8[0], c8[1], c8[2], c8[6], c8[3], c8[4], c8[5], c8[7]};
+        memcpy(rctr, f, sizeof f);
+    }
+    void Add(const uint64_t ctr[8]) const {
+        s.Add(ctr);
+        t.mDiscardedEventsTotal.Add(ctr[3]);
+        t.mOutKeyNotFoundEventsTotal.Add(ctr[4]);
+        t.mOutFailedEventsTotal.Add(ctr[5]);
+        t.mHistoryFailureTotal.Add(ctr[6]);
+        t.mOutSuccessfulEventsTotal.Add(ctr[7]);
+    }
+    void Process(PipelineEventGroup& g) const {
+        s.Process(g);
+        t.Process(g);
+    }
+};
+// the timestamp calls' arguments behind time_ns
+#define SPLIT_JSON_TS_ARGS(x)                                                                                          \
+    (x).t.mSourceKey.data(), (uint32_t)(x).t.mSourceKey.size(), (x).Program(), (x).now, (x).DiscardInterval()
+
+bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next,
+                                                 ProcessorParseTimestampNative& timestamp, bool enableNs,
+                                                 std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, timestamp, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseJsonNative& next,
+                                                    ProcessorParseTimestampNative& timestamp, bool enableNs,
+                                                    std::string& block, uint64_t& rawSize, std::string& err) {
+    return ChainSerializeSls(group, next, timestamp, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitLogStringNative::ChainSerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next,
+                                                      ProcessorParseTimestampNative& timestamp, bool enableNs,
+                                                      std::string& out, uint64_t* rawSize, std::string& err) {
+    const SplitJsonTsStage x(next, timestamp, group);
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_split_json_timestamp_parse_sls(Engine(), SPLIT_JSON_STAGE_ARGS(x.s), (uint8_t)mSplitChar,
+                                                         SPLIT_JSON_STAGE_OPTS(x.s), SPLIT_JSON_TS_ARGS(x), enableNs,
+                                                         o, cap, len, nev, c8);
+        SplitJsonTsStage::Fold(c8, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_split_json_timestamp_parse_sls_lz4(
+            Engine(), SPLIT_JSON_STAGE_ARGS(x.s), (uint8_t)mSplitChar, SPLIT_JSON_STAGE_OPTS(x.s),
+            SPLIT_JSON_TS_ARGS(x), enableNs, tail, tailLen, o, cap, len, raw, nev, c8);
+        SplitJsonTsStage::Fold(c8, rctr);
+        return rc;
+    };
+    uint64_t unused[3] = {0, 0, 0};
+    return SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_split_json_timestamp_parse_sls",
+        "lc_split_json_timestamp_parse_sls_lz4", unused);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next,
+                                                          ProcessorParseTimestampNative& timestamp, bool enableNs,
+                                                          std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, timestamp, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseJsonNative& next,
+                                                             ProcessorParseTimestampNative& timestamp, bool enableNs,
+                                                             std::string& block, uint64_t& rawSize, std::string& err) {
+    return ChainSerializeSls(group, next, timestamp, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGroup& group,
+                                                               ProcessorParseJsonNative& next,
+                                                               ProcessorParseTimestampNative& timestamp,
+                                                               bool enableNs, std::string& out, uint64_t* rawSize,
+                                                               std::string& err) {
+    const SplitJsonTsStage x(next, timestamp, group);
+    const bool discard = mMultiline.mUnmatchedContentTreatment == MultilineOptions::UnmatchedContentTreatment::DISCARD;
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_multiline_split_json_timestamp_parse_sls(
+            Engine(), SPLIT_JSON_STAGE_ARGS(x.s), mStart.get(), mContinue.get(), mEnd.get(), discard,
+            SPLIT_JSON_STAGE_OPTS(x.s), SPLIT_JSON_TS_ARGS(x), enableNs, o, cap, len, nev, c8, sctr);
+        SplitJsonTsStage::Fold(c8, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c8[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_multiline_split_json_timestamp_parse_sls_lz4(
+            Engine(), SPLIT_JSON_STAGE_ARGS(x.s), mStart.get(), mContinue.get(), mEnd.get(), discard,
+            SPLIT_JSON_STAGE_OPTS(x.s), SPLIT_JSON_TS_ARGS(x), enableNs, tail, tailLen, o, cap, len, raw, nev, c8,
+            sctr);
+        SplitJsonTsStage::Fold(c8, rctr);
+        return rc;
+    };
+    // matched_events, input lines, unmatched lines: moved as Process moves them (:82-84,106-107)
+    uint64_t ctr[3] = {0, 0, 0};
+    const bool ok = SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_multiline_split_json_timestamp_parse_sls",
+        "lc_multiline_split_json_timestamp_parse_sls_lz4", ctr);
+    mMatchedEventsTotal.Add(ctr[0]);
+    mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
+    mUnmatchedLinesTotal.Add(ctr[2]);
+    return ok;
+}
+#undef SPLIT_JSON_TS_ARGS
 #undef SPLIT_JSON_STAGE_ARGS
 #undef SPLIT_JSON_STAGE_OPTS
 

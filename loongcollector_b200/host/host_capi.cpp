@@ -364,22 +364,28 @@ char* lc_host_chain3_serialize_sls(lc_host_processor_t* split, lc_host_processor
     if (raw_len_out)
         *raw_len_out = 0;
     try {
-        // (splitter, regex, filter), (splitter, regex, timestamp) or (splitter, delimiter, regex)
+        // (splitter, regex, filter), (splitter, regex, timestamp), (splitter, JSON, timestamp) or (splitter,
+        // delimiter, regex)
         Processor* d = split->proc.get();
         Processor* b = regex->proc.get();
         Processor* c = filter->proc.get();
         auto* r = dynamic_cast<ProcessorParseRegexNative*>(b);
+        auto* js = dynamic_cast<ProcessorParseJsonNative*>(b);
         auto* f = dynamic_cast<ProcessorFilterNative*>(c);
         auto* ts = dynamic_cast<ProcessorParseTimestampNative*>(c);
         auto* dl = dynamic_cast<ProcessorParseDelimiterNative*>(b);
         auto* dr = dynamic_cast<ProcessorParseRegexNative*>(c);
         auto* ps = dynamic_cast<ProcessorSplitLogStringNative*>(d);
         auto* pm = dynamic_cast<ProcessorSplitMultilineLogStringNative*>(d);
-        if (!(ps || pm) || !((r && f) || (r && ts) || (dl && dr)))
+        if (!(ps || pm) || !((r && f) || (r && ts) || (js && ts) || (dl && dr)))
             throw std::runtime_error("not a splitter followed by a processor_parse_regex_native and a "
-                                     "processor_filter_regex_native or a processor_parse_timestamp_native, or by a "
+                                     "processor_filter_regex_native or a processor_parse_timestamp_native, by a "
+                                     "processor_parse_json_native and a processor_parse_timestamp_native, or by a "
                                      "processor_parse_delimiter_native and a processor_parse_regex_native");
         auto chain = [&](auto* p, PipelineEventGroup& g, std::string& res, uint64_t& raw, std::string& err) {
+            if (js)
+                return mode == 2 ? p->SerializeSlsLz4(g, *js, *ts, enable_ns != 0, res, raw, err)
+                                 : p->SerializeSls(g, *js, *ts, enable_ns != 0, res, err);
             if (dl)
                 return mode == 2 ? p->SerializeSlsLz4(g, *dl, *dr, enable_ns != 0, res, raw, err)
                                  : p->SerializeSls(g, *dl, *dr, enable_ns != 0, res, err);
