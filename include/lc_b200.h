@@ -65,7 +65,10 @@ const char* lc_version(void);
 const char* lc_last_error(void);
 /* Number of visible CUDA devices (0 if none / runtime unusable). */
 int lc_device_count(void);
-/* Creates an engine bound to CUDA device `device` with its own stream, workspace and pinned staging. */
+/* Creates an engine bound to CUDA device `device` with its own stream, workspace and pinned staging.  The own stream
+ * is a blocking stream: it is ordered with the legacy default stream (PyTorch's default stream), so device buffers
+ * filled there before a *_dev call are complete when its kernels read them, and work queued there afterwards waits
+ * for the engine's. */
 int lc_engine_create(int device, lc_engine_t** out);
 void lc_engine_destroy(lc_engine_t* e);
 /* Blocks until all work queued on the engine's stream is complete. */

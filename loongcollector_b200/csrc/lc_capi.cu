@@ -313,7 +313,9 @@ int lc_engine_create(int device, lc_engine_t** out) {
         return fail(LC_ERR_CUDA, "out of host memory");
     e->device = device;
     CU_TRY(cudaSetDevice(device));
-    CU_TRY(cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking));
+    // a blocking stream: device buffers a caller filled on the legacy default stream (PyTorch's default stream) are
+    // ready before a *_dev call's kernels read them, and that stream's later work waits for the engine's writes
+    CU_TRY(cudaStreamCreateWithFlags(&e->own_stream, cudaStreamDefault));
     e->stream = e->own_stream;
     CU_TRY(cudaDeviceGetAttribute(&e->num_sms, cudaDevAttrMultiProcessorCount, device));
     CU_TRY(cudaDeviceGetAttribute(&e->smem_per_block_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));

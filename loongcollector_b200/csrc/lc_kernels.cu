@@ -1635,16 +1635,25 @@ struct TdfaAbs {
 // one LEA.HI -- (entry >> 16) + index -- instead of a mask and an add, one instruction less on the dependent chain of
 // every pair: PRMT PRMT LDS.U8 LDS.U8 IMAD LEA.HI LDS + two predicated STS.U16 for capture boundaries.
 // ROWX = the address of the current row: `row` for the first pair of a chunk, (e_prev >> 16) afterwards.
+// The capture stores keep the field test, the address and the store in one asm block each, so that ptxas takes the
+// predicate and the masked field from one LOP3 instead of masking the second field twice.
+__device__ __forceinline__ void sts_u16_reg_a(uint32_t e, uint32_t regs_m2, uint32_t pos) {
+    asm volatile("{\n\t.reg .pred p;\n\t.reg .u32 f;\n\tand.b32 f, %0, 0x7F;\n\tsetp.ne.u32 p, f, 0;\n\t"
+                 "add.u32 f, f, %1;\n\t@p st.shared.u16 [f], %2;\n\t}"
+                 ::"r"(e), "r"(regs_m2), "h"((unsigned short)pos) : "memory");
+}
+__device__ __forceinline__ void sts_u16_reg_b(uint32_t e, uint32_t regs_m2, uint32_t pos) {
+    asm volatile("{\n\t.reg .pred p;\n\t.reg .u32 f;\n\tand.b32 f, %0, 0x7F00;\n\tsetp.ne.u32 p, f, 0;\n\t"
+                 "shr.u32 f, f, 8;\n\tadd.u32 f, f, %1;\n\t@p st.shared.u16 [f], %2;\n\t}"
+                 ::"r"(e), "r"(regs_m2), "h"((unsigned short)pos) : "memory");
+}
 #define LCS_PAIR(ROWX, X, HI, POS)                                                                                     \
     {                                                                                                                  \
         const uint32_t c0 = lds_u8(__byte_perm((X), t.cls, (HI) ? 0x7652 : 0x7650));                                   \
         const uint32_t c1 = lds_u8(__byte_perm((X), t.cls, (HI) ? 0x7653 : 0x7651));                                   \
         const uint32_t e = lds_u32((ROWX) + (c0 * t.ncls + c1));                                                       \
-        const uint32_t sa = e & 0x7Fu, sb = e & 0x7F00u;                                                               \
-        if (sa)                                                                                                        \
-            sts_u16(regs_m2 + sa, (POS));                                                                              \
-        if (sb)                                                                                                        \
-            sts_u16(regs_m2 + (sb >> 8), (POS) + 1);                                                                   \
+        sts_u16_reg_a(e, regs_m2, (POS));                                                                              \
+        sts_u16_reg_b(e, regs_m2, (POS) + 1);                                                                          \
         e_prev = e;                                                                                                    \
     }
 
@@ -1754,23 +1763,29 @@ __device__ __forceinline__ uint32_t tdfa_walk_lines(const LcTdfaView& v, const T
     for (uint32_t s0 = 0; s0 < max_nch; s0 += LCT_STAGE_CHUNKS) {
         L.stage(s0); // chunks s0..s0+7 of the warp's 32 lines are in the tile when this returns
         // ---- every lane walks its own line through the tile
-        if (row != dead) {
-            if (has_head && s0 == 0)
-                row = tdfa_partial_chunk(v, t, row, L.own(0), 0, mis, len, regs_m2, rg, sink);
-            const uint32_t ka = kf_lo > s0 ? kf_lo : s0;
-            const uint32_t kb = kf_hi < s0 + LCT_STAGE_CHUNKS ? kf_hi : s0 + LCT_STAGE_CHUNKS;
-            for (uint32_t k = ka; k < kb; ++k) {
-                const uint4 vv = lds_u128_v(L.own(k));
-                {
-                    // run skipping: inside [^"]* / .* / after the line has died the state maps every byte but (at
-                    // most) two back to itself without touching a register -- a chunk without those bytes is a no-op
-                    const uint32_t sk = lds_u32(t.skip + __umulhi(row - t.t2, t.inv_row) * 4);
-                    if (sk) {
-                        const uint32_t w[4] = {vv.x, vv.y, vv.z, vv.w};
-                        if (!lc_tdfa_chunk_has_exit(sk, w))
-                            continue;
-                    }
-                }
+        if (row != dead && has_head && s0 == 0)
+            row = tdfa_partial_chunk(v, t, row, L.own(0), 0, mis, len, regs_m2, rg, sink);
+        // The fully paired chunks go in warp lockstep: in step j every lane that is alive and has a j-th fully
+        // paired chunk in this stage walks that chunk of its own line, and the others sit the step out.  Run
+        // skipping is decided for the warp as a whole, since a warp only saves issue slots when all of its walking
+        // lanes skip: inside [^"]* / .* the state maps every byte but (at most) two back to itself without touching a
+        // register, so a chunk without those bytes is a no-op.  The exit test runs only when the vote says every
+        // walking lane is in such a state; otherwise they all walk their chunk, which is exact either way.
+        const uint32_t ka = kf_lo > s0 ? kf_lo : s0;
+        const uint32_t kb = kf_hi < s0 + LCT_STAGE_CHUNKS ? kf_hi : s0 + LCT_STAGE_CHUNKS;
+        const uint32_t nk = row != dead && kb > ka ? kb - ka : 0;
+        for (uint32_t j = 0; __any_sync(0xFFFFFFFFu, j < nk); ++j) {
+            const uint32_t k = ka + j;
+            // (both loads are in bounds for every lane: its own tile row, and the skip word of a valid row)
+            const uint4 vv = lds_u128_v(L.own(k));
+            const uint32_t sk = lds_u32(t.skip + __umulhi(row - t.t2, t.inv_row) * 4);
+            const bool walk = row != dead && j < nk;
+            if (__all_sync(0xFFFFFFFFu, sk != 0 || !walk)) {
+                const uint32_t w[4] = {vv.x, vv.y, vv.z, vv.w};
+                if (!__any_sync(0xFFFFFFFFu, walk && lc_tdfa_chunk_has_exit(sk, w)))
+                    continue;
+            }
+            if (walk) {
                 const uint32_t pos0 = k * 16 - mis;
                 const uint32_t row_in = row;
                 uint32_t e_prev;
@@ -1786,9 +1801,9 @@ __device__ __forceinline__ uint32_t tdfa_walk_lines(const LcTdfaView& v, const T
                 if (SLOW && row == sink) // some step set several registers: redo this chunk step by step
                     row = t.t2 + t.row_bytes * tdfa_chunk_slow(v, __umulhi(row_in - t.t2, t.inv_row), vv, pos0, rg);
             }
-            if (has_tail && k_tail - s0 < LCT_STAGE_CHUNKS)
-                row = tdfa_partial_chunk(v, t, row, L.own(k_tail), k_tail * 16, mis, len, regs_m2, rg, sink);
         }
+        if (row != dead && has_tail && k_tail - s0 < LCT_STAGE_CHUNKS)
+            row = tdfa_partial_chunk(v, t, row, L.own(k_tail), k_tail * 16, mis, len, regs_m2, rg, sink);
         __syncwarp();
     }
     return row;
