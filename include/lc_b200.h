@@ -885,6 +885,104 @@ int lc_multiline_split_delim_regex_parse_sls_lz4(
     const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len,
     uint64_t* n_events, uint64_t counters[8], uint64_t ml_counters[3]);
 
+/* ---- f4: the split -> delimiter -> timestamp chain (the split -> delimiter chain, then ProcessorParseTimestampNative
+ * with SourceKey tkey, ProcessorParseTimestampNative.cpp:100-235; a CSV / TSV file whose logs take their time from
+ * one of their columns) to the SLS wire format.  Pieces and the delimiter stage are exactly the split -> delimiter
+ * chain's (same arguments, offset metadata, refusals, record layout, empty-record handling and erase rule).  The row
+ * rule:
+ *   - The timestamp stage sees the pieces the delimiter stage did not erase, in piece order, as ONE group (the
+ *     second-level cache starts empty per call).  A failed piece erased without keep_fail is no event of the stage: no
+ *     counter, no cache step.  A piece kept without a record (no contents left) is an event: it counts key_not_found.
+ *   - Its value under tkey is what ProcessorParseDelimiterNative::ProcessEvent (:206-364, AddLog :411-419) leaves
+ *     there.  The keys are distinct, so tkey names at most one column j; a "_" in discard mode names none.
+ *       blank or empty piece (LC_DELIM_BLANK, left untouched): the piece when tkey is source_key, else none;
+ *       parsed piece (LC_DELIM_OK), the first rule that applies: column j when the row reaches it (nf > j), with
+ *       doubled quotes collapsed as AddFieldWithUnQuote does; the piece when tkey is source_key and source_key is one
+ *       of the keys (a short row keeps it); the piece when keep_succeed is set and tkey is renamed_key; else none;
+ *       kept failure (LC_DELIM_PARSE_FAIL, LC_DELIM_COLUMNS with keep_fail; source_key was deleted): the piece when tkey
+ *       is renamed_key, or when tkey is "__raw_log__" and copy_raw is set, else none.
+ *     A value is read over [off, off + len) followed by NUL bytes, as lc_timestamp_parse reads every value.
+ *   - LC_TS_OK: the record's Time is the parsed seconds truncated to 32 bits (raised to at least 2^28 as every
+ *     record's); with enable_ns Time_ns is the parsed nanoseconds.  LC_TS_NOT_FOUND, LC_TS_FAILED: the source event's
+ *     time / time_ns.  LC_TS_DISCARDED: no record.
+ *   - Refused with LC_ERR_INVALID_ARG beyond the split -> delimiter chain's refusals: tkey equal to offset_key; unless
+ *     discard, a tkey of the form __column<digits>__ (a generated overflow key could hold it on some rows only); and a
+ *     time_ns other than LC_SLS_NO_NS with enable_ns == 0 (some records would carry Time_ns and others not).
+ *   - counters[9] (may be NULL) = the delimiter stage's successful, failed, discarded, blank (as
+ *     lc_split_delim_parse_sls counts them), then the timestamp stage's key_not_found, out_failed, history_failure,
+ *     discarded, out_successful.
+ *
+ * lc_split_delim_timestamp_tap_dev: from the DEVICE piece and delimiter tables (as for
+ * lc_sls_serialize_split_delim_dev) and the delimiter stage's configuration, writes the value table d_val_off /
+ * d_val_len[n] that lc_timestamp_parse_dev takes with one group over d_val (d_val_len LC_TS_NO_KEY: erased by the
+ * delimiter stage, or no value), and copies each value into d_val at its own offset in d_src; a column with doubled
+ * quotes is collapsed there.  val_cap must be at least src_len.  Only the tkey values are copied; the other bytes of
+ * d_val are left as they are.  It queues the work on the engine's stream and returns without waiting.
+ * lc_sls_serialize_split_delim_timestamp_dev: lc_sls_serialize_split_delim_dev's arguments plus the DEVICE results of
+ * that lc_timestamp_parse_dev call (d_ts_status, d_ts_sec, d_ts_nsec) and enable_ns.  Sizing query, capacity and the
+ * 4 GiB / 2^30 rules are the sibling's. */
+int lc_split_delim_timestamp_tap_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+                                     const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                     const uint32_t* d_nfields, const uint32_t* d_f_off, const uint32_t* d_f_len,
+                                     const uint32_t* d_f_dq, uint32_t max_fields, const uint8_t* sep, uint32_t sep_len,
+                                     uint8_t quote, int extend, int discard, const char* const* keys,
+                                     const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+                                     uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+                                     int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+                                     uint32_t offset_key_len, const char* tkey, uint32_t tkey_len, uint8_t* d_val,
+                                     uint64_t val_cap, uint32_t* d_val_off, uint32_t* d_val_len);
+int lc_sls_serialize_split_delim_timestamp_dev(
+    lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+    const uint8_t* d_status, const uint32_t* d_nfields, const uint32_t* d_f_off, const uint32_t* d_f_len,
+    const uint32_t* d_f_dq, uint32_t max_fields, const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend,
+    int discard, const char* const* keys, const uint32_t* key_lens, uint32_t nkeys, const char* source_key,
+    uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len, int keep_fail, int keep_succeed,
+    int copy_raw, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns,
+    const uint8_t* d_ts_status, const int64_t* d_ts_sec, const uint32_t* d_ts_nsec, int enable_ns, uint8_t* d_out,
+    uint64_t out_cap, uint64_t* out_len, uint64_t counters[9]);
+
+/* The same with a HOST source value: upload it once, split, run lc_delim_parse_dev (allow_short, max_fields as for
+ * lc_split_delim_parse_sls), the tap, both timestamp passes (ts compiled by lc_timestamp_compile; now = time(NULL) of
+ * the call, discard_interval as for lc_timestamp_parse, -1 = no history discard), size and emit (and LZ4), and bring
+ * back only the bytes.  The value and timestamp tables stay in the engine's buffers.  *n_events, ml_counters, the
+ * tail, raw_len and the behaviour on LC_ERR_CAPACITY are as for lc_split_delim_parse_sls.  A chunk whose pieces are
+ * all erased or discarded gives 0 bytes (the LZ4 calls: the block of the tail alone). */
+int lc_split_delim_timestamp_parse_sls(
+    lc_engine_t* e, const uint8_t* buf, uint64_t len, uint8_t split_char, const uint8_t* sep, uint32_t sep_len,
+    uint8_t quote, int extend, int discard, int allow_short, uint32_t max_fields, const char* const* keys,
+    const uint32_t* key_lens, uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+    uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+    uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns, const char* tkey, uint32_t tkey_len,
+    const struct lc_timestamp* ts, int64_t now, int32_t discard_interval, int enable_ns, uint8_t* out,
+    uint64_t out_cap, uint64_t* out_len, uint64_t* n_events, uint64_t counters[9]);
+int lc_split_delim_timestamp_parse_sls_lz4(
+    lc_engine_t* e, const uint8_t* buf, uint64_t len, uint8_t split_char, const uint8_t* sep, uint32_t sep_len,
+    uint8_t quote, int extend, int discard, int allow_short, uint32_t max_fields, const char* const* keys,
+    const uint32_t* key_lens, uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key,
+    uint32_t renamed_key_len, int keep_fail, int keep_succeed, int copy_raw, const char* offset_key,
+    uint32_t offset_key_len, uint64_t src_pos, uint32_t time, uint32_t time_ns, const char* tkey, uint32_t tkey_len,
+    const struct lc_timestamp* ts, int64_t now, int32_t discard_interval, int enable_ns, const uint8_t* tail,
+    uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+    uint64_t counters[9]);
+int lc_multiline_split_delim_timestamp_parse_sls(
+    lc_engine_t* e, const uint8_t* buf, uint64_t len, const lc_regex_t* start, const lc_regex_t* cont,
+    const lc_regex_t* end, int discard_unmatched, const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend,
+    int discard, int allow_short, uint32_t max_fields, const char* const* keys, const uint32_t* key_lens,
+    uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+    int keep_fail, int keep_succeed, int copy_raw, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+    uint32_t time, uint32_t time_ns, const char* tkey, uint32_t tkey_len, const struct lc_timestamp* ts, int64_t now,
+    int32_t discard_interval, int enable_ns, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+    uint64_t counters[9], uint64_t ml_counters[3]);
+int lc_multiline_split_delim_timestamp_parse_sls_lz4(
+    lc_engine_t* e, const uint8_t* buf, uint64_t len, const lc_regex_t* start, const lc_regex_t* cont,
+    const lc_regex_t* end, int discard_unmatched, const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend,
+    int discard, int allow_short, uint32_t max_fields, const char* const* keys, const uint32_t* key_lens,
+    uint32_t nkeys, const char* source_key, uint32_t source_key_len, const char* renamed_key, uint32_t renamed_key_len,
+    int keep_fail, int keep_succeed, int copy_raw, const char* offset_key, uint32_t offset_key_len, uint64_t src_pos,
+    uint32_t time, uint32_t time_ns, const char* tkey, uint32_t tkey_len, const struct lc_timestamp* ts, int64_t now,
+    int32_t discard_interval, int enable_ns, const uint8_t* tail, uint64_t tail_len, uint8_t* out, uint64_t out_cap,
+    uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events, uint64_t counters[9], uint64_t ml_counters[3]);
+
 /* LZ4 compression of serialised groups (FlusherSLS's default compressor, LZ4Compressor::Compress =
  * LZ4_compress_default): segment g = d_in[d_seg_off[g], + d_seg_len[g]) becomes one LZ4 *block* (not a frame), the
  * blocks packed back to back in d_out: block g = d_out[d_blk_off[g], + d_blk_len[g]).  The bytes are deterministic;

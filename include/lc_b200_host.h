@@ -83,7 +83,9 @@ char* lc_host_chain_serialize_sls(lc_host_processor_t* delim, lc_host_processor_
  * 2 are split's SerializeSls / SerializeSlsLz4(group, regex, timestamp).  And the split -> JSON -> timestamp chain:
  * regex is then a "processor_parse_json_native" reading the splitter's SourceKey and filter a
  * "processor_parse_timestamp_native", and modes 0 and 2 are split's SerializeSls / SerializeSlsLz4(group, json,
- * timestamp). */
+ * timestamp).  Likewise the split -> delimiter -> timestamp chain: regex is then a "processor_parse_delimiter_native"
+ * reading the splitter's SourceKey and filter a "processor_parse_timestamp_native", and modes 0 and 2 are split's
+ * SerializeSls / SerializeSlsLz4(group, delimiter, timestamp). */
 char* lc_host_chain3_serialize_sls(lc_host_processor_t* split, lc_host_processor_t* regex, lc_host_processor_t* filter,
                                    const char* group_json, int enable_ns, int mode, unsigned long long* len_out,
                                    unsigned long long* raw_len_out, char** err_out, char** fail_out);

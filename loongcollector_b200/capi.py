@@ -224,6 +224,20 @@ def lib():
         [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
     L.lc_multiline_split_delim_regex_parse_sls_lz4.argtypes = [vp, vp, vp, u64, vp, vp, vp, i32] + sdr_cfg + \
         [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
+    # the split -> delimiter -> timestamp chain: the split -> delimiter arguments with the timestamp stage behind time_ns
+    L.lc_split_delim_timestamp_tap_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, vp, u32, vp, u32, u8, i32,
+                                                   i32] + sls_cfg + [C.c_char_p, u32, C.c_char_p, u32, vp, u64, vp, vp]
+    L.lc_sls_serialize_split_delim_timestamp_dev.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, vp, u32, vp, u32,
+                                                             u8, i32, i32] + sls_cfg + sr_tail + \
+        [vp, vp, vp, i32, vp, u64, C.POINTER(u64), vp]
+    L.lc_split_delim_timestamp_parse_sls.argtypes = [vp, vp, u64, u8] + sd_cfg + sls_cfg + sr_tail + sjt_ts + \
+        [vp, u64, C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_split_delim_timestamp_parse_sls_lz4.argtypes = [vp, vp, u64, u8] + sd_cfg + sls_cfg + sr_tail + sjt_ts + \
+        [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp]
+    L.lc_multiline_split_delim_timestamp_parse_sls.argtypes = [vp, vp, u64, vp, vp, vp, i32] + sd_cfg + sls_cfg + \
+        sr_tail + sjt_ts + [vp, u64, C.POINTER(u64), C.POINTER(u64), vp, vp]
+    L.lc_multiline_split_delim_timestamp_parse_sls_lz4.argtypes = [vp, vp, u64, vp, vp, vp, i32] + sd_cfg + \
+        sls_cfg + sr_tail + sjt_ts + [vp, u64, vp, u64, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp, vp]
     _LIB = L
     return L
 
@@ -1176,10 +1190,11 @@ class Engine:
 
     def _split_delim(self, fn, buf, extra, sep, quote, treatment, keys, source_key, renamed_key, keep_fail,
                      keep_succeed, copy_raw, allow_short, max_fields, offset_key, src_pos, time, time_ns, out_cap, ml,
-                     tail):
+                     tail, ts_args=None):
         """one host-buffer split -> delimiter call, sized by an estimate first and by the exact size when that was
-        short; tail None: the wire bytes, else records ‖ tail as one LZ4 block.  Returns (bytes, raw_len, n_events,
-        counters[4], ml_counters[3] or None)"""
+        short; tail None: the wire bytes, else records ‖ tail as one LZ4 block; ts_args: the timestamp stage of the
+        split -> delimiter -> timestamp calls (_ts_args).  Returns (bytes, raw_len, n_events, counters[4], or [9] with
+        ts_args, ml_counters[3] or None)"""
         a = _u8(buf)
         sp = np.frombuffer(sep, np.uint8)
         mf = int(max_fields if max_fields is not None else len(keys) + 16)
@@ -1192,11 +1207,11 @@ class Engine:
         for _ in range(2):
             out = np.empty(max(cap, 1), np.uint8)
             need, raw, nev = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
-            ctr, mctr = np.zeros(4, np.uint64), np.zeros(3, np.uint64)
+            ctr, mctr = np.zeros(9 if ts_args else 4, np.uint64), np.zeros(3, np.uint64)
             z = [] if tl is None else [_p(tl) if tl.size else None, tl.size]
             outs = [_p(out), cap, C.byref(need)] + ([] if tl is None else [C.byref(raw)]) + [C.byref(nev), _p(ctr)]
             rc = fn(self._h, _p(a), a.size, *extra, *dcfg, *cfg, *self._sr_tail(offset_key, src_pos, time, time_ns),
-                    *z, *outs, *([_p(mctr)] if ml else []))
+                    *(ts_args or []), *z, *outs, *([_p(mctr)] if ml else []))
             if rc == LC_ERR_CAPACITY and out_cap is None:
                 cap = int(need.value)
                 continue
@@ -1250,6 +1265,100 @@ class Engine:
             lib().lc_multiline_split_delim_parse_sls_lz4, buf, [_rh(start), _rh(cont), _rh(end), int(bool(discard))],
             sep, quote, treatment, keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw, allow_short,
             max_fields, offset_key, src_pos, time, time_ns, out_cap, True, tail)
+
+    def split_delim_timestamp_tap_dev(self, d_src, src_len, d_off, d_len, n, d_status, d_nf, d_fo, d_fl, d_fd,
+                                      max_fields, sep: bytes, quote, treatment, keys, source_key, tkey, d_val, val_cap,
+                                      d_val_off, d_val_len, renamed_key=None, keep_fail=False, keep_succeed=False,
+                                      copy_raw=False, offset_key=None):
+        """The timestamp stage's value table (d_val_off, d_val_len; LC_TS_NO_KEY = no value) over d_val, with each
+        value copied into d_val (val_cap >= src_len) at its own offset, from the device piece and delimiter tables of
+        the split -> delimiter chain (lc_split_delim_timestamp_tap_dev); queued, not waited for."""
+        sp = np.frombuffer(sep, np.uint8)
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        _check(lib().lc_split_delim_timestamp_tap_dev(
+            self._h, _p(d_src), src_len, _p(d_off), _p(d_len), n, _p(d_status), _p(d_nf), _p(d_fo), _p(d_fl),
+            _p(d_fd), max_fields, _p(sp), len(sep), quote, int(treatment == "extend"), int(treatment == "discard"),
+            *cfg, *self._sr_tail(offset_key, 0, 0, None)[:2], tkey, len(tkey), _p(d_val), val_cap, _p(d_val_off),
+            _p(d_val_len)))
+
+    def sls_serialize_split_delim_timestamp_dev(self, d_src, src_len, d_off, d_len, n, d_status, d_nf, d_fo, d_fl,
+                                                d_fd, max_fields, sep: bytes, quote, treatment, keys, source_key,
+                                                d_ts_status, d_ts_sec, d_ts_nsec, enable_ns=False, renamed_key=None,
+                                                keep_fail=False, keep_succeed=False, copy_raw=False, offset_key=None,
+                                                src_pos=0, time=0, time_ns=None, d_out=None, out_cap=0):
+        """sls_serialize_split_delim_dev with each record's time from the device results of timestamp_parse_dev over
+        the tap's value table (lc_sls_serialize_split_delim_timestamp_dev).  Returns (byte count, counters[9] = the
+        delimiter stage's four, then key_not_found, out_failed, history_failure, discarded, out_successful); with
+        d_out None the byte count needed."""
+        sp = np.frombuffer(sep, np.uint8)
+        _keep, cfg = self._delim_sls_cfg(keys, source_key, renamed_key, keep_fail, keep_succeed, copy_raw)
+        need = C.c_uint64(0)
+        ctr = np.zeros(9, np.uint64)
+        rc = lib().lc_sls_serialize_split_delim_timestamp_dev(
+            self._h, _p(d_src), src_len, _p(d_off), _p(d_len), n, _p(d_status), _p(d_nf), _p(d_fo), _p(d_fl),
+            _p(d_fd), max_fields, _p(sp), len(sep), quote, int(treatment == "extend"), int(treatment == "discard"),
+            *cfg, *self._sr_tail(offset_key, src_pos, time, time_ns), _p(d_ts_status), _p(d_ts_sec), _p(d_ts_nsec),
+            int(bool(enable_ns)), _p(d_out), out_cap, C.byref(need), _p(ctr))
+        if rc == LC_ERR_CAPACITY and d_out is None:
+            return int(need.value), ctr  # a sizing query
+        _check(rc)
+        return int(need.value), ctr
+
+    def split_delim_timestamp_parse_sls(self, buf, split_char, sep: bytes, quote, treatment, keys, source_key, tkey,
+                                        ts, now, discard_interval=-1, enable_ns=False, renamed_key=None,
+                                        keep_fail=False, keep_succeed=False, copy_raw=False, allow_short=True,
+                                        max_fields=None, offset_key=None, src_pos=0, time=0, time_ns=None,
+                                        out_cap=None):
+        """split_delim_parse_sls with ProcessorParseTimestampNative (SourceKey tkey, the compiled Timestamp ts) behind
+        the delimiter stage (lc_split_delim_timestamp_parse_sls).  Returns (bytes, number of pieces, counters[9])."""
+        data, _raw, nev, ctr, _m = self._split_delim(
+            lib().lc_split_delim_timestamp_parse_sls, buf, [split_char], sep, quote, treatment, keys, source_key,
+            renamed_key, keep_fail, keep_succeed, copy_raw, allow_short, max_fields, offset_key, src_pos, time,
+            time_ns, out_cap, False, None, self._ts_args(tkey, ts, now, discard_interval, enable_ns))
+        return data, nev, ctr
+
+    def split_delim_timestamp_parse_sls_lz4(self, buf, split_char, sep: bytes, quote, treatment, keys, source_key,
+                                            tkey, ts, now, discard_interval=-1, enable_ns=False, renamed_key=None,
+                                            keep_fail=False, keep_succeed=False, copy_raw=False, allow_short=True,
+                                            max_fields=None, offset_key=None, src_pos=0, time=0, time_ns=None,
+                                            tail=b"", out_cap=None):
+        """split_delim_timestamp_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_split_delim_timestamp_parse_sls_lz4).  Returns (block, raw_len, number of pieces, counters[9])."""
+        data, raw, nev, ctr, _m = self._split_delim(
+            lib().lc_split_delim_timestamp_parse_sls_lz4, buf, [split_char], sep, quote, treatment, keys, source_key,
+            renamed_key, keep_fail, keep_succeed, copy_raw, allow_short, max_fields, offset_key, src_pos, time,
+            time_ns, out_cap, False, tail, self._ts_args(tkey, ts, now, discard_interval, enable_ns))
+        return data, raw, nev, ctr
+
+    def multiline_split_delim_timestamp_parse_sls(self, buf, start, cont, end, discard, sep: bytes, quote, treatment,
+                                                  keys, source_key, tkey, ts, now, discard_interval=-1,
+                                                  enable_ns=False, renamed_key=None, keep_fail=False,
+                                                  keep_succeed=False, copy_raw=False, allow_short=True,
+                                                  max_fields=None, offset_key=None, src_pos=0, time=0, time_ns=None,
+                                                  out_cap=None):
+        """The same with the multiline splitter (lc_multiline_split_delim_timestamp_parse_sls).  Returns (bytes,
+        number of events, counters[9], splitter counters[3])."""
+        data, _raw, nev, ctr, mctr = self._split_delim(
+            lib().lc_multiline_split_delim_timestamp_parse_sls, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], sep, quote, treatment, keys, source_key,
+            renamed_key, keep_fail, keep_succeed, copy_raw, allow_short, max_fields, offset_key, src_pos, time,
+            time_ns, out_cap, True, None, self._ts_args(tkey, ts, now, discard_interval, enable_ns))
+        return data, nev, ctr, mctr
+
+    def multiline_split_delim_timestamp_parse_sls_lz4(self, buf, start, cont, end, discard, sep: bytes, quote,
+                                                      treatment, keys, source_key, tkey, ts, now, discard_interval=-1,
+                                                      enable_ns=False, renamed_key=None, keep_fail=False,
+                                                      keep_succeed=False, copy_raw=False, allow_short=True,
+                                                      max_fields=None, offset_key=None, src_pos=0, time=0,
+                                                      time_ns=None, tail=b"", out_cap=None):
+        """multiline_split_delim_timestamp_parse_sls's records followed by `tail` as ONE LZ4 block
+        (lc_multiline_split_delim_timestamp_parse_sls_lz4).  Returns (block, raw_len, number of events,
+        counters[9], splitter counters[3])."""
+        return self._split_delim(
+            lib().lc_multiline_split_delim_timestamp_parse_sls_lz4, buf,
+            [_rh(start), _rh(cont), _rh(end), int(bool(discard))], sep, quote, treatment, keys, source_key,
+            renamed_key, keep_fail, keep_succeed, copy_raw, allow_short, max_fields, offset_key, src_pos, time,
+            time_ns, out_cap, True, tail, self._ts_args(tkey, ts, now, discard_interval, enable_ns))
 
     def sls_serialize_split_delim_regex_dev(self, d_src, src_len, d_off, d_len, n, d_status, d_nf, d_fo, d_fl, d_fd,
                                             max_fields, delim, regex, d_val_off, d_val_len, d_re_status, d_cap_off,

@@ -136,7 +136,8 @@ struct lc_engine {
     // its count) and sort scratch; the chain's piece and JSON tables are in, out_a, out_b and the js_* buffers
     DevBuf sj_win, sj_ev, sj_list, sj_sort;
     // split -> JSON -> timestamp chain: the value buffer the tap copies each piece's value into (chunk bytes, then arena
-    // bytes); its value and timestamp tables are the split -> regex -> timestamp chain's st_* buffers
+    // bytes); its value and timestamp tables are the split -> regex -> timestamp chain's st_* buffers.  The split ->
+    // delimiter -> timestamp chain uses the same three (its values are chunk bytes only).
     DevBuf sjt_val;
     // split -> Apsara -> SLS chain: its one-group table; the piece and Apsara tables are in, out_a, out_b and the ap_*
     // buffers
@@ -3436,10 +3437,11 @@ int lc_multiline_split_regex_timestamp_parse_sls_lz4(
 namespace {
 
 // lc_delim_sls_setup + lc_split_delim_sls_link: the delimiter's key strings are staged in `dr_keys`, the offset key in
-// `sls_plan`; neither splitter, nor lc_delim_parse_dev, nor the serialiser uses them.
+// `sls_plan`; neither splitter, nor lc_delim_parse_dev, nor the serialiser uses them.  With ta (the timestamp calls),
+// the timestamp stage's SourceKey is checked and resolved into *tc (lc_split_delim_ts_setup).
 int split_delim_sls_config(lc_engine_t* e, const char* what, uint32_t max_fields, const uint8_t* sep,
                            uint32_t sep_len, uint8_t quote, int extend, int discard, DELIM_KEY_PARAMS, OFFSET_PARAMS,
-                           LcSplitDelimSlsCfg* c) {
+                           LcSplitDelimSlsCfg* c, const TsArgs* ta = nullptr, LcSplitDelimTsCfg* tc = nullptr) {
     LcDelimSlsCfg d;
     int rc = delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, DELIM_KEY_ARGS, &d,
                               &e->dr_keys);
@@ -3447,6 +3449,9 @@ int split_delim_sls_config(lc_engine_t* e, const char* what, uint32_t max_fields
         return rc;
     const char* why = lc_split_delim_sls_link(d, keys, key_lens, source_key, source_key_len, renamed_key,
                                               renamed_key_len, offset_key, offset_key_len, src_pos, time, time_ns, c);
+    if (!why && ta)
+        why = lc_split_delim_ts_setup(*c, keys, key_lens, source_key, source_key_len, renamed_key, renamed_key_len,
+                                      offset_key, offset_key_len, ta->tkey, ta->tkey_len, ta->enable_ns, tc);
     if (why)
         return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
     if (offset_key) {
@@ -3463,26 +3468,61 @@ int split_delim_sls_config(lc_engine_t* e, const char* what, uint32_t max_fields
 
 // The size pass and the emit of the chain over the n pieces of t (serialize_sls_dev): into d_out (the device-fed
 // call), or back to the host buffer out, or -- with z -- records ‖ tail as one LZ4 block.  counters[4] (or nullptr) =
-// successful, failed, discarded, blank; set whenever the size pass ran.
+// successful, failed, discarded, blank; set whenever the size pass ran.  With tc (the timestamp calls), each record's
+// time comes from the timestamp tables ts and counters has LC_SDTS_COUNTERS entries.
 int split_delim_sls_run(lc_engine_t* e, const char* what, const LcSplitDelimSlsCfg& c, const lck::DelimSlsTables& t,
                         uint64_t n, uint8_t* d_out, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
-                        uint64_t* counters, const Lz4Tail* z) {
-    uint64_t ctr[5] = {0, 0, 0, 0, 0}; // + pieces whose record would reach 4 GiB
+                        uint64_t* counters, const Lz4Tail* z, const LcSplitDelimTsCfg* tc = nullptr,
+                        const lck::TsRowTables* ts = nullptr) {
+    const uint32_t nstage = tc ? LC_SDTS_COUNTERS : 4u;
+    uint64_t ctr[LC_SDTS_COUNTERS + 1] = {0}; // + pieces whose record would reach 4 GiB
     SlsTo to;
     to.host = out;
     to.z = z;
-    to.too_large = 4;
+    to.too_large = (int)nstage;
     const int rc = serialize_sls_dev(
-        e, what, n, 5,
+        e, what, n, nstage + 1,
         [&](uint32_t* rec, uint32_t* body, unsigned long long* d_ctr) {
-            lck::launch_split_delim_sls_sizes(c, t, n, rec, body, d_ctr, e->stream);
+            if (tc)
+                lck::launch_split_delim_ts_sls_sizes(c, *tc, t, *ts, n, rec, body, d_ctr, e->stream);
+            else
+                lck::launch_split_delim_sls_sizes(c, t, n, rec, body, d_ctr, e->stream);
         },
         [&](const uint64_t* rec_off, const uint32_t* body, uint8_t* dst) {
-            lck::launch_split_delim_sls_emit(c, t, n, rec_off, body, dst, e->stream);
+            if (tc)
+                lck::launch_split_delim_ts_sls_emit(c, *tc, t, *ts, n, rec_off, body, dst, e->stream);
+            else
+                lck::launch_split_delim_sls_emit(c, t, n, rec_off, body, dst, e->stream);
         },
         d_out, out_cap, out_len, ctr, to);
     if (counters)
-        memcpy(counters, ctr, 4 * sizeof(uint64_t));
+        memcpy(counters, ctr, nstage * sizeof(uint64_t));
+    return rc;
+}
+
+// The split -> delimiter -> timestamp chain's tap and timestamp passes over the n pieces of t: the value buffer
+// `sjt_val` (as long as the source value) and the value table into st_val, then lc_timestamp_parse_dev's two passes
+// with the whole source value as one group into *ts (st_status, st_sec, st_nsec).  The stage's counters are the size
+// pass's, so the passes' own go to ts_cnt unread.
+int split_delim_ts_run(lc_engine_t* e, const LcSplitDelimSlsCfg& c, const LcSplitDelimTsCfg& tc, const TsArgs& ta,
+                       const lck::DelimSlsTables& t, uint64_t n, uint64_t src_len, lck::TsRowTables* ts) {
+    CU_TRY(e->st_val.ensure(n * 8 + 8));
+    CU_TRY(e->st_sec.ensure(n * 8));
+    CU_TRY(e->st_nsec.ensure(n * 4));
+    CU_TRY(e->st_status.ensure(n));
+    CU_TRY(e->ts_cnt.ensure(5 * sizeof(uint64_t)));
+    CU_TRY(e->sjt_val.ensure(src_len + 16));
+    uint32_t* off = e->st_val.as<uint32_t>();
+    uint32_t *len = off + n, *grp = off + 2 * n;
+    const uint32_t g[2] = {0u, (uint32_t)n};
+    CU_TRY(cudaMemcpyAsync(grp, g, sizeof g, cudaMemcpyHostToDevice, e->stream));
+    lck::launch_split_delim_ts_tap(c, tc, t, n, e->sjt_val.as<uint8_t>(), off, len, e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    const int rc = ts_run(e, ta.ts, e->sjt_val.as<uint8_t>(), LcTsSpans{off, len, nullptr, 1}, n, grp, 1, ta.now,
+                          ta.discard_interval, e->st_sec.as<int64_t>(), e->st_nsec.as<uint32_t>(),
+                          e->st_status.as<uint8_t>(), e->ts_cnt.as<uint64_t>());
+    *ts = lck::TsRowTables{e->st_status.as<uint8_t>(), e->st_sec.as<int64_t>(), e->st_nsec.as<uint32_t>()};
     return rc;
 }
 
@@ -3491,20 +3531,22 @@ int split_delim_sls_run(lc_engine_t* e, const char* what, const LcSplitDelimSlsC
 // flags), the delimiter tables in dr_status (status), dr_val_off (column counts), out_d / out_e / dr_cap_off (f_off /
 // f_len / f_dq, [n][max_fields]), the key strings in dr_keys and sls_plan.  The splitters, lc_delim_parse_dev (its
 // tiled kernel stages in shared memory) and the serialiser (lab_sizes, cnt, lab_off, state, desc, lab, z_*) use none
-// of the others'.
+// of the others'.  With ta (the _timestamp_ calls), the tap and the timestamp passes (sjt_val, st_*, ts_*) run between
+// the delimiter stage and the size pass and counters has LC_SDTS_COUNTERS entries.
 template <class Split>
 int split_delim_sls_host(lc_engine_t* e, const char* what, const uint8_t* buf, uint64_t len, Split split,
                          SPLIT_DELIM_PARAMS, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
-                         uint64_t counters[4], const Lz4Tail* z) {
+                         uint64_t* counters, const Lz4Tail* z, const TsArgs* ta = nullptr) {
     LcSplitDelimSlsCfg c;
+    LcSplitDelimTsCfg tc;
     auto begin = [&]() {
         if (counters)
-            memset(counters, 0, 4 * sizeof(uint64_t));
+            memset(counters, 0, (ta ? LC_SDTS_COUNTERS : 4) * sizeof(uint64_t));
         return (int)LC_OK;
     };
     auto config = [&]() {
         return split_delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, DELIM_KEY_ARGS,
-                                      OFFSET_ARGS, &c);
+                                      OFFSET_ARGS, &c, ta, &tc);
     };
     auto run = [&](uint64_t n) {
         if (n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32))
@@ -3525,10 +3567,17 @@ int split_delim_sls_host(lc_engine_t* e, const char* what, const uint8_t* buf, u
                                     e->dr_cap_off.as<uint32_t>());
         if (rc)
             return rc;
-        return split_delim_sls_run(e, what, c, t, n, nullptr, out, out_cap, out_len, counters, z);
+        lck::TsRowTables ts{};
+        if (ta) {
+            rc = split_delim_ts_run(e, c, tc, *ta, t, n, len, &ts);
+            if (rc)
+                return rc;
+        }
+        return split_delim_sls_run(e, what, c, t, n, nullptr, out, out_cap, out_len, counters, z, ta ? &tc : nullptr,
+                                   &ts);
     };
-    return split_chain_sls_host(e, what, buf, len, split, sep != nullptr, begin, config, run, out, out_cap, out_len,
-                                n_events, z);
+    return split_chain_sls_host(e, what, buf, len, split, sep != nullptr && (!ta || ta->ts), begin, config, run, out,
+                                out_cap, out_len, n_events, z);
 }
 
 } // namespace
@@ -3855,6 +3904,149 @@ int lc_multiline_split_delim_regex_parse_sls_lz4(lc_engine_t* e, const lc_regex_
 #undef SPLIT_DELIM_REGEX_ARGS
 
 } // extern "C"
+
+// ------------------------------------------------------------------------- split -> delimiter -> timestamp -> SLS
+// (the multiline splitter's own counters[3] are added to ml_counters as lc_multiline_split_dev adds them)
+#define ML_SPLIT                                                                                                       \
+    [&](uint64_t* n) {                                                                                                 \
+        return lc_multiline_split_dev(e, e->in.as<uint8_t>(), len, start, cont, end, discard_unmatched,               \
+                                      e->out_a.as<uint32_t>(), e->out_b.as<uint32_t>(), e->out_c.as<uint8_t>(), len,  \
+                                      n, ml_counters);                                                                 \
+    }
+#define TS_ARGS_OF_CALL const TsArgs ta{tkey, tkey_len, ts, now, discard_interval, enable_ns};
+
+extern "C" {
+
+int lc_split_delim_timestamp_tap_dev(lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off,
+                                     const uint32_t* d_len, uint64_t n, const uint8_t* d_status,
+                                     const uint32_t* d_nfields, const uint32_t* d_f_off, const uint32_t* d_f_len,
+                                     const uint32_t* d_f_dq, uint32_t max_fields, const uint8_t* sep, uint32_t sep_len,
+                                     uint8_t quote, int extend, int discard, DELIM_KEY_PARAMS, const char* offset_key,
+                                     uint32_t offset_key_len, const char* tkey, uint32_t tkey_len, uint8_t* d_val,
+                                     uint64_t val_cap, uint32_t* d_val_off, uint32_t* d_val_len) {
+    static const char* what = "lc_split_delim_timestamp_tap_dev";
+    if (!e || (tkey_len && !tkey) ||
+        (n && (!d_src || !d_off || !d_len || !d_status || !d_nfields || !d_f_off || !d_f_len || !d_f_dq || !d_val ||
+               !d_val_off || !d_val_len)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    if (src_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 pieces and < 2^32 columns per call");
+    if (n && val_cap < src_len)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": the value buffer must hold src_len bytes");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    const uint64_t src_pos = 0;
+    const uint32_t time = 0, time_ns = LC_SLS_NO_NS;
+    const TsArgs ta{tkey, tkey_len, nullptr, 0, -1, 0};
+    LcSplitDelimSlsCfg c;
+    LcSplitDelimTsCfg tc;
+    rc = split_delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, DELIM_KEY_ARGS, OFFSET_ARGS,
+                                &c, &ta, &tc);
+    if (rc || n == 0)
+        return rc;
+    const lck::DelimSlsTables t{d_src, d_off, d_len, d_status, d_nfields, d_f_off, d_f_len, d_f_dq};
+    lck::launch_split_delim_ts_tap(c, tc, t, n, d_val, d_val_off, d_val_len, e->stream);
+    e->launches++;
+    CU_TRY(cudaGetLastError());
+    return LC_OK;
+}
+
+int lc_sls_serialize_split_delim_timestamp_dev(
+    lc_engine_t* e, const uint8_t* d_src, uint64_t src_len, const uint32_t* d_off, const uint32_t* d_len, uint64_t n,
+    const uint8_t* d_status, const uint32_t* d_nfields, const uint32_t* d_f_off, const uint32_t* d_f_len,
+    const uint32_t* d_f_dq, uint32_t max_fields, const uint8_t* sep, uint32_t sep_len, uint8_t quote, int extend,
+    int discard, DELIM_KEY_PARAMS, OFFSET_PARAMS, const uint8_t* d_ts_status, const int64_t* d_ts_sec,
+    const uint32_t* d_ts_nsec, int enable_ns, uint8_t* d_out, uint64_t out_cap, uint64_t* out_len,
+    uint64_t counters[9]) {
+    static const char* what = "lc_sls_serialize_split_delim_timestamp_dev";
+    if (!e || !out_len ||
+        (n && (!d_src || !d_off || !d_len || !d_status || !d_nfields || !d_f_off || !d_f_len || !d_f_dq ||
+               !d_ts_status || !d_ts_sec || !d_ts_nsec)))
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": bad arguments");
+    *out_len = 0;
+    if (counters)
+        memset(counters, 0, LC_SDTS_COUNTERS * sizeof(uint64_t));
+    if (src_len >= 0xFFFFFFF0ull || n >= (1ull << 30) || n * (uint64_t)max_fields >= (1ull << 32))
+        return fail(LC_ERR_TOO_LARGE, "buffer must be < 4 GiB, < 2^30 pieces and < 2^32 columns per call");
+    int rc = bind(e);
+    if (rc)
+        return rc;
+    LcSplitDelimSlsCfg c;
+    rc = split_delim_sls_config(e, what, max_fields, sep, sep_len, quote, extend, discard, DELIM_KEY_ARGS, OFFSET_ARGS,
+                                &c);
+    if (rc)
+        return rc;
+    const char* why = lc_split_regex_ts_ns_check(c, enable_ns);
+    if (why)
+        return fail(LC_ERR_INVALID_ARG, std::string(what) + ": " + why);
+    if (n == 0)
+        return LC_OK;
+    LcSplitDelimTsCfg tc;
+    memset(&tc, 0, sizeof tc);
+    tc.enable_ns = enable_ns != 0;
+    const lck::DelimSlsTables t{d_src, d_off, d_len, d_status, d_nfields, d_f_off, d_f_len, d_f_dq};
+    const lck::TsRowTables ts{d_ts_status, d_ts_sec, d_ts_nsec};
+    return split_delim_sls_run(e, what, c, t, n, d_out, nullptr, out_cap, out_len, counters, nullptr, &tc, &ts);
+}
+
+int lc_split_delim_timestamp_parse_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len, uint8_t split_char,
+                                       SPLIT_DELIM_PARAMS, const char* tkey, uint32_t tkey_len,
+                                       const lc_timestamp_t* ts, int64_t now, int32_t discard_interval, int enable_ns,
+                                       uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                       uint64_t counters[9]) {
+    TS_ARGS_OF_CALL
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    return split_delim_sls_host(e, "lc_split_delim_timestamp_parse_sls", buf, len, split, SPLIT_DELIM_ARGS, out,
+                                out_cap, out_len, n_events, counters, nullptr, &ta);
+}
+
+int lc_split_delim_timestamp_parse_sls_lz4(lc_engine_t* e, const uint8_t* buf, uint64_t len, uint8_t split_char,
+                                           SPLIT_DELIM_PARAMS, const char* tkey, uint32_t tkey_len,
+                                           const lc_timestamp_t* ts, int64_t now, int32_t discard_interval,
+                                           int enable_ns, const uint8_t* tail, uint64_t tail_len, uint8_t* out,
+                                           uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+                                           uint64_t counters[9]) {
+    TS_ARGS_OF_CALL
+    auto split = [&](uint64_t* n) {
+        return lc_split_lines_dev(e, e->in.as<uint8_t>(), len, split_char, e->out_a.as<uint32_t>(),
+                                  e->out_b.as<uint32_t>(), len, n);
+    };
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return split_delim_sls_host(e, "lc_split_delim_timestamp_parse_sls_lz4", buf, len, split, SPLIT_DELIM_ARGS, out,
+                                out_cap, out_len, n_events, counters, &z, &ta);
+}
+
+int lc_multiline_split_delim_timestamp_parse_sls(lc_engine_t* e, const uint8_t* buf, uint64_t len,
+                                                 const lc_regex_t* start, const lc_regex_t* cont,
+                                                 const lc_regex_t* end, int discard_unmatched, SPLIT_DELIM_PARAMS,
+                                                 const char* tkey, uint32_t tkey_len, const lc_timestamp_t* ts,
+                                                 int64_t now, int32_t discard_interval, int enable_ns, uint8_t* out,
+                                                 uint64_t out_cap, uint64_t* out_len, uint64_t* n_events,
+                                                 uint64_t counters[9], uint64_t ml_counters[3]) {
+    TS_ARGS_OF_CALL
+    return split_delim_sls_host(e, "lc_multiline_split_delim_timestamp_parse_sls", buf, len, ML_SPLIT,
+                                SPLIT_DELIM_ARGS, out, out_cap, out_len, n_events, counters, nullptr, &ta);
+}
+
+int lc_multiline_split_delim_timestamp_parse_sls_lz4(
+    lc_engine_t* e, const uint8_t* buf, uint64_t len, const lc_regex_t* start, const lc_regex_t* cont,
+    const lc_regex_t* end, int discard_unmatched, SPLIT_DELIM_PARAMS, const char* tkey, uint32_t tkey_len,
+    const lc_timestamp_t* ts, int64_t now, int32_t discard_interval, int enable_ns, const uint8_t* tail,
+    uint64_t tail_len, uint8_t* out, uint64_t out_cap, uint64_t* out_len, uint64_t* raw_len, uint64_t* n_events,
+    uint64_t counters[9], uint64_t ml_counters[3]) {
+    TS_ARGS_OF_CALL
+    const Lz4Tail z{tail, tail_len, raw_len};
+    return split_delim_sls_host(e, "lc_multiline_split_delim_timestamp_parse_sls_lz4", buf, len, ML_SPLIT,
+                                SPLIT_DELIM_ARGS, out, out_cap, out_len, n_events, counters, &z, &ta);
+}
+
+} // extern "C"
+#undef TS_ARGS_OF_CALL
+#undef ML_SPLIT
 
 // ------------------------------------------------------------------------------------------------ LZ4
 namespace {

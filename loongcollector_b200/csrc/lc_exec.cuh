@@ -2106,6 +2106,19 @@ LC_HD uint32_t lc_split_delim_sls_body(const LcSplitDelimSlsCfg& c, const uint8_
     return lc_delim_sls_body(c.d, src, r, s, x);
 }
 
+// ... with the record's own time and ns (has_ns = 0: no Time_ns).  It hands the body a copy of the row with that
+// time rather than the other way round: forwarding the row's own time through this overload changes the instruction
+// schedule of the split -> delimiter emit kernel.
+template <class S>
+LC_HD uint32_t lc_split_delim_sls_body(const LcSplitDelimSlsCfg& c, const uint8_t* src, const LcDelimSlsRow& r,
+                                       uint32_t time, uint32_t has_ns, uint32_t ns, S& s) {
+    LcDelimSlsRow q = r;
+    q.time = time;
+    q.has_ns = has_ns != 0;
+    q.ns = ns;
+    return lc_split_delim_sls_body(c, src, q, s);
+}
+
 // The row's counter verdicts (0 / 1), as lc_delim_parse_sls counts them: successful, failed, discarded, blank.
 struct LcDelimSlsVerdict {
     uint32_t ok, failed, erased, blank;
@@ -4230,6 +4243,141 @@ LC_HD uint32_t lc_split_ts_verdict_bits(const LcSplitRegexVerdict& v, uint32_t t
 
 LC_HD uint32_t lc_split_regex_ts_verdict(const LcSplitRegexSlsCfg& c, uint32_t status, uint32_t ts) {
     return lc_split_ts_verdict_bits(lc_split_regex_verdict(c, status), ts);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// f4, split -> delimiter -> timestamp chain: ProcessorParseTimestampNative (ProcessorParseTimestampNative.cpp:100-235,
+// the SourceKey tkey) behind the split -> delimiter chain, whose pieces and delimiter stage are unchanged.
+//   - The timestamp stage sees the pieces the delimiter stage did not erase, in piece order, as one group: a failed
+//     piece erased without KeepingSourceWhenParseFail is not an event of the stage (no counter, no cache step).  A
+//     piece kept without contents is an event: it counts key_not_found.
+//   - Its value is what ProcessorParseDelimiterNative::ProcessEvent (ProcessorParseDelimiterNative.cpp:206-364,
+//     AddLog :411-419) leaves under tkey.  The keys are distinct (lc_delim_sls_setup), so tkey names at most one
+//     column j; a skipped "_" in discard mode names none.
+//       blank piece (left untouched):  the piece when tkey is SourceKey, else none
+//       parsed piece:                  column j unquoted (AddFieldWithUnQuote) when the row reaches it; else the piece
+//                                      when tkey is SourceKey and SourceKey is one of the keys (mSourceKeyOverwritten:
+//                                      a short row keeps it), or when tkey is RenamedSourceKey with
+//                                      KeepingSourceWhenParseSucceed; else none
+//       kept failure:                  the piece when tkey is RenamedSourceKey, or "__raw_log__" with CopingRawLog
+//                                      (SourceKey was deleted); else none
+//     tkey equal to the offset key is refused, and -- unless overflow columns are discarded -- so is a tkey of the
+//     form __column<digits>__, which a generated overflow key would hold on some rows only.
+//   - Every value lies inside its own piece, so the tap copies each to its own offset of a value buffer as long as the
+//     chunk; a column with doubled quotes is collapsed there in place (never longer than the column).  The value is
+//     read over [off, off + len) followed by NUL bytes, as every timestamp value is.
+//   - The record's time is lc_split_regex_ts_time's rule: LC_TS_OK sets Time (and Time_ns with enable_ns),
+//     LC_TS_NOT_FOUND / LC_TS_FAILED keep the source event's, LC_TS_DISCARDED leaves no record.
+struct LcSplitDelimTsCfg {
+    uint32_t col;       // the column keyed tkey (not a skipped "_"), or LC_DELIM_SLS_NONE
+    uint32_t is_src;    // tkey == SourceKey
+    uint32_t is_ren;    // tkey == RenamedSourceKey
+    uint32_t is_raw;    // tkey == "__raw_log__"
+    uint32_t enable_ns; // mEnableTimestampNanosecond: a parsed time writes Time_ns
+};
+
+// counters[9] of the chain: the delimiter stage's four, then the timestamp stage's five in lc_timestamp_parse's order
+#define LC_SDTS_COUNTERS 9
+
+// Host side: check tkey and the source Time_ns against the chain's configuration c (lc_split_delim_sls_link accepted
+// it with the same keys, SourceKey, RenamedSourceKey and offset key; offset_key == nullptr: no log.file.offset
+// metadata) and resolve tkey into *t.  Returns nullptr, or why the chain is refused.
+inline const char* lc_split_delim_ts_setup(const LcSplitDelimSlsCfg& c, const char* const* keys,
+                                           const uint32_t* key_lens, const char* source_key, uint32_t source_len,
+                                           const char* renamed_key, uint32_t renamed_len, const char* offset_key,
+                                           uint32_t offset_len, const char* tkey, uint32_t tkey_len, int enable_ns,
+                                           LcSplitDelimTsCfg* t) {
+    if (!t || (tkey_len && !tkey))
+        return "bad arguments";
+    auto eq = [](const char* a, uint32_t la, const char* b, uint32_t lb) {
+        return la == lb && (la == 0 || !memcmp(a, b, la));
+    };
+    const char* why = lc_split_regex_ts_ns_check(c, enable_ns);
+    if (why)
+        return why;
+    if (offset_key && eq(tkey, tkey_len, offset_key, offset_len))
+        return "the timestamp key equals the offset key";
+    uint32_t idx;
+    if (c.d.mode != LC_DELIM_SLS_DISCARD && tkey_len && lc_delim_column_form(tkey, tkey_len, &idx))
+        return "a timestamp key of the form __column<digits>__ collides with the generated overflow keys";
+    memset(t, 0, sizeof *t);
+    t->col = LC_DELIM_SLS_NONE;
+    for (uint32_t k = 0; k < c.d.nkeys; ++k)
+        if (eq(keys[k], key_lens[k], tkey, tkey_len) &&
+            !(c.d.mode == LC_DELIM_SLS_DISCARD && key_lens[k] == 1 && keys[k][0] == '_'))
+            t->col = k;
+    t->is_src = eq(tkey, tkey_len, source_key, source_len);
+    t->is_ren = eq(tkey, tkey_len, renamed_key, renamed_len);
+    t->is_raw = eq(tkey, tkey_len, "__raw_log__", 11);
+    t->enable_ns = enable_ns != 0;
+    return nullptr;
+}
+
+// The tap's value of one piece: src[off, + n) holding dq doubled quotes, which the value buffer gets collapsed to
+// n - dq bytes at off; n = LC_TS_NO_KEY when the delimiter stage erased the piece or left no value under tkey.
+struct LcSplitDelimTsValue {
+    uint32_t off, n, dq;
+};
+LC_HD LcSplitDelimTsValue lc_split_delim_ts_value(const LcSplitDelimSlsCfg& c, const LcSplitDelimTsCfg& t,
+                                                  const LcDelimSlsRow& r) {
+    const LcSplitDelimTsValue none{0u, LC_TS_NO_KEY, 0u}, piece{r.eo, r.elen, 0u};
+    if (r.status == 2) // LC_DELIM_BLANK: untouched
+        return t.is_src ? piece : none;
+    if (r.status != 0) // failed: RenamedSourceKey [, "__raw_log__"] -> piece when kept, else erased
+        return c.d.keep_fail && (t.is_ren || (c.d.copy_raw && t.is_raw)) ? piece : none;
+    if (t.col < r.nf) // col < nkeys < max_fields: always in the table
+        return {r.fo[t.col], r.fl[t.col], c.d.use_quote ? r.fd[t.col] : 0u};
+    return (t.is_src && c.d.src_overwritten) || (t.is_ren && c.d.keep_succeed) ? piece : none;
+}
+
+// The tap's collapse of a column s[0, n) holding doubled quotes q q (a column the state machine parsed holds no lone
+// quote) into d[0, n - its pairs), AddFieldWithUnQuote's rule, W lanes taking W bytes per step: a quote is dropped when
+// it is the second of its pair, which each lane tells from the run of quotes up to it (odd: the run that reaches the
+// step's first byte holds an odd count so far).  v: W words of per-warp scratch (shared memory on the device).  Every
+// lane calls it.
+LC_HD void lc_split_delim_ts_collapse(uint8_t* d, const uint8_t* s, uint32_t n, uint8_t q, uint32_t* v,
+                                      uint32_t lane, uint32_t W) {
+    uint32_t w = 0, odd = 0;
+    for (uint32_t b = 0; b < n; b += W) {
+        const uint32_t nv = n - b < W ? n - b : W;
+        LC_LANES(l) { v[l] = l < nv && s[b + l] == q; }
+        const uint32_t qm = lc_lz4_ballot(v, lane, W);
+        LC_WARP_SYNC();
+        LC_LANES(l) {
+            uint32_t drop = 0;
+            if ((qm >> l) & 1) {
+                const uint32_t nq = ~qm & lc_ts_below(l); // the non-quotes below: the run starts after the last
+                drop = ((nq ? l - lc_hi_bit(nq) : l + 1 + odd) & 1) == 0;
+            }
+            v[l] = drop;
+        }
+        const uint32_t keep = lc_ts_below(nv) & ~lc_lz4_ballot(v, lane, W);
+        LC_WARP_SYNC();
+        LC_LANES(l) {
+            if ((keep >> l) & 1)
+                d[w + lc_popc(keep & lc_ts_below(l))] = s[b + l];
+        }
+        w += lc_popc(keep);
+        const uint32_t nq = ~qm & lc_ts_below(nv);
+        odd = nq ? (nv - 1 - lc_hi_bit(nq)) & 1 : (odd + nv) & 1;
+    }
+}
+
+// The record's time after the timestamp stage (ts: the stage's LC_TS_ST_* of the row, sec / nsec its time)
+LC_HD LcSplitRegexTsTime lc_split_delim_ts_time(const LcSplitDelimSlsCfg& c, const LcSplitDelimTsCfg& t, uint32_t ts,
+                                                int64_t sec, uint32_t nsec) {
+    if (ts == LC_TS_ST_OK)
+        return {1u, (uint32_t)sec, t.enable_ns, nsec};
+    return {ts != LC_TS_ST_DISCARDED, c.time, c.has_ns, c.ns};
+}
+
+// The row's counter verdicts as bits of the LC_SDTS_COUNTERS counters: the delimiter stage's successful, failed,
+// discarded, blank (lc_delim_sls_verdict), then -- when the delimiter stage kept the piece -- the timestamp stage's
+// key_not_found, out_failed, history_failure, discarded, out_successful.
+LC_HD uint32_t lc_split_delim_ts_verdict(const LcSplitDelimSlsCfg& c, uint32_t status, uint32_t ts) {
+    const LcDelimSlsVerdict d = lc_delim_sls_verdict(c.d, status);
+    const uint32_t t = lc_split_ts_verdict_bits(LcSplitRegexVerdict{0u, 0u, d.erased}, ts) >> 3;
+    return d.ok | (d.failed << 1) | (d.erased << 2) | (d.blank << 3) | (t << 4);
 }
 
 // ================================================================================================ Apsara parse

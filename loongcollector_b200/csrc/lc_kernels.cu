@@ -4978,6 +4978,112 @@ void launch_split_json_ts_sls_emit(const LcSplitJsonSlsCfg& c, const LcSplitJson
                                                                                          d_body_size, d_out);
 }
 
+// ---- f4, split -> delimiter -> timestamp chain (lc_exec.cuh: lc_split_delim_ts_value, _collapse, _time, _verdict).
+// The tap runs one warp per piece and copies its value into the value buffer at the value's own offset: every value
+// lies inside its piece and a collapsed column is never longer than the column, so no two values share bytes.  Unlike
+// the delimiter -> regex tap (lc_delim_regex_tap), it needs no sizing pass for side copies and no region behind the
+// source.  A plain value is the warp's shared copy (split_json_ts_copy); a column with doubled quotes is collapsed
+// 32 bytes per step.  The size pass (one thread per piece) and the emit pass (one warp per piece) are the split ->
+// delimiter chain's, with each record's own time.
+__global__ void __launch_bounds__(256)
+    split_delim_ts_tap_kernel(LcSplitDelimSlsCfg c, LcSplitDelimTsCfg tc, DelimSlsTables t, uint64_t n,
+                              uint8_t* __restrict__ val, uint32_t* __restrict__ off, uint32_t* __restrict__ len) {
+    __shared__ uint32_t ws[8][32];
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (i >= n)
+        return;
+    const LcSplitDelimTsValue v = lc_split_delim_ts_value(c, tc, split_delim_sls_row(c, t, i));
+    if (lane == 0) {
+        off[i] = v.off;
+        len[i] = v.n == LC_TS_NO_KEY ? LC_TS_NO_KEY : v.n - v.dq;
+    }
+    if (v.n == LC_TS_NO_KEY)
+        return;
+    if (v.dq)
+        lc_split_delim_ts_collapse(val + v.off, t.base + v.off, v.n, c.d.quote, ws[threadIdx.x >> 5], lane, 32);
+    else
+        split_json_ts_copy(val + v.off, t.base + v.off, v.n, lane);
+}
+
+// counters: u64 [10] += the LC_SDTS_COUNTERS verdicts (one atomic per warp and counter), then pieces whose record
+// would reach 4 GiB
+__global__ void __launch_bounds__(256)
+    split_delim_ts_sls_size_kernel(LcSplitDelimSlsCfg c, LcSplitDelimTsCfg tc, DelimSlsTables t, TsRowTables ts,
+                                   uint64_t n, uint32_t* __restrict__ rec_size, uint32_t* __restrict__ body_size,
+                                   unsigned long long* __restrict__ counters) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t bits = 0, big = 0;
+    if (i < n) {
+        const LcDelimSlsRow r = split_delim_sls_row(c, t, i);
+        const uint32_t st = ts.status[i];
+        const LcSplitRegexTsTime tm = lc_split_delim_ts_time(c, tc, st, ts.sec[i], ts.nsec[i]);
+        LcSlsCount64 s{0};
+        const uint32_t cnt = tm.keep ? lc_split_delim_sls_body(c, t.base, r, tm.time, tm.has_ns, tm.ns, s) : 0u;
+        big = s.n + 16 > 0xFFFFFFFFull;
+        const uint32_t body = cnt && !big ? (uint32_t)s.n : 0u;
+        rec_size[i] = body ? 1 + lc_varint_size(body) + body : 0u;
+        body_size[i] = body;
+        bits = lc_split_delim_ts_verdict(c, r.status, st);
+    }
+#pragma unroll
+    for (uint32_t k = 0; k < LC_SDTS_COUNTERS; ++k) {
+        const uint32_t v = __reduce_add_sync(0xFFFFFFFFu, (bits >> k) & 1u);
+        if ((threadIdx.x & 31) == 0 && v)
+            atomicAdd(counters + k, (unsigned long long)v);
+    }
+    big = __reduce_add_sync(0xFFFFFFFFu, big);
+    if ((threadIdx.x & 31) == 0 && big)
+        atomicAdd(counters + LC_SDTS_COUNTERS, (unsigned long long)big);
+}
+
+__global__ void __launch_bounds__(256)
+    split_delim_ts_sls_emit_kernel(LcSplitDelimSlsCfg c, LcSplitDelimTsCfg tc, DelimSlsTables t, TsRowTables ts,
+                                   uint64_t n, const uint64_t* __restrict__ rec_off,
+                                   const uint32_t* __restrict__ body_size, uint8_t* __restrict__ out) {
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n)
+        return;
+    const uint32_t body = body_size[i];
+    if (!body)
+        return; // erased, discarded or without contents: no record
+    const LcDelimSlsRow r = split_delim_sls_row(c, t, i);
+    // lc_split_delim_ts_time's rule for a piece with a record, as selects on the kernel parameters (as in the split ->
+    // JSON -> timestamp emit kernel, which a struct of the three kept live across the body made spill)
+    const bool ok = ts.status[i] == LC_TS_ST_OK;
+    uint8_t h[6];
+    h[0] = 0x0A;
+    const uint32_t hn = 1 + lc_put_varint(h + 1, body);
+    LcSlsWrite s{out + rec_off[i], 0u, hn + body, threadIdx.x & 31, 32};
+    s.put(h, hn);
+    lc_split_delim_sls_body(c, t.base, r, ok ? (uint32_t)ts.sec[i] : c.time, ok ? tc.enable_ns : c.has_ns,
+                            ok ? ts.nsec[i] : c.ns, s);
+}
+
+void launch_split_delim_ts_tap(const LcSplitDelimSlsCfg& c, const LcSplitDelimTsCfg& tc, const DelimSlsTables& t,
+                               uint64_t n, uint8_t* d_val, uint32_t* d_off, uint32_t* d_len, cudaStream_t st) {
+    if (n)
+        split_delim_ts_tap_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, tc, t, n, d_val, d_off, d_len);
+}
+
+void launch_split_delim_ts_sls_sizes(const LcSplitDelimSlsCfg& c, const LcSplitDelimTsCfg& tc,
+                                     const DelimSlsTables& t, const TsRowTables& ts, uint64_t n,
+                                     uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                     cudaStream_t st) {
+    if (n)
+        split_delim_ts_sls_size_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c, tc, t, ts, n, d_rec_size,
+                                                                                     d_body_size, d_counters);
+}
+
+void launch_split_delim_ts_sls_emit(const LcSplitDelimSlsCfg& c, const LcSplitDelimTsCfg& tc,
+                                    const DelimSlsTables& t, const TsRowTables& ts, uint64_t n,
+                                    const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                    cudaStream_t st) {
+    if (n)
+        split_delim_ts_sls_emit_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(c, tc, t, ts, n, d_rec_off,
+                                                                                          d_body_size, d_out);
+}
+
 // ---- f4, split -> Apsara chain (lc_exec.cuh: lc_split_apsara_sls_body, lc_split_apsara_verdict).  The size pass runs
 // one thread per piece, the emit pass one warp per piece.  counters: u64 [6] += lc_apsara_parse's five, then pieces
 // whose record would reach 4 GiB.

@@ -11,6 +11,7 @@ struct LcSpanSlsCfg;
 struct LcSplitRegexSlsCfg;
 struct LcSplitDelimSlsCfg;
 struct LcSplitDelimRegexSlsCfg;
+struct LcSplitDelimTsCfg;
 struct LcFilterSlsCfg;
 struct LcSplitRegexTsCfg;
 struct LcLz4Seq;
@@ -340,6 +341,23 @@ void launch_split_delim_regex_sls_sizes(const LcSplitDelimRegexSlsCfg& c, const 
 void launch_split_delim_regex_sls_emit(const LcSplitDelimRegexSlsCfg& c, const DelimRegexSlsTables& t, uint64_t n,
                                        const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
                                        cudaStream_t st);
+
+// f4, split -> delimiter -> timestamp chain (lc_exec.cuh: LcSplitDelimTsCfg).  launch_split_delim_ts_tap: the value
+// table (d_off, d_len) over d_val that the timestamp passes take, with each value copied into d_val (at least as long
+// as the source value) at its own offset, a column with doubled quotes collapsed; LC_TS_NO_KEY: erased by the
+// delimiter stage, or no value.  The size and emit passes are launch_split_delim_sls_*'s with each record's time from
+// the timestamp tables ts; d_counters: u64 [10] += the chain's 9 counters (LC_SDTS_COUNTERS), then pieces whose
+// record would reach 4 GiB.
+void launch_split_delim_ts_tap(const LcSplitDelimSlsCfg& c, const LcSplitDelimTsCfg& tc, const DelimSlsTables& t,
+                               uint64_t n, uint8_t* d_val, uint32_t* d_off, uint32_t* d_len, cudaStream_t st);
+void launch_split_delim_ts_sls_sizes(const LcSplitDelimSlsCfg& c, const LcSplitDelimTsCfg& tc,
+                                     const DelimSlsTables& t, const TsRowTables& ts, uint64_t n,
+                                     uint32_t* d_rec_size, uint32_t* d_body_size, unsigned long long* d_counters,
+                                     cudaStream_t st);
+void launch_split_delim_ts_sls_emit(const LcSplitDelimSlsCfg& c, const LcSplitDelimTsCfg& tc,
+                                    const DelimSlsTables& t, const TsRowTables& ts, uint64_t n,
+                                    const uint64_t* d_rec_off, const uint32_t* d_body_size, uint8_t* d_out,
+                                    cudaStream_t st);
 
 // f4, split-fed: Log records of the pieces of one source value (lc_exec.cuh: LcSpanSlsCfg, keys on the device).
 // rec_size[k] = bytes of piece k's record (never 0); the emit pass writes the `total` bytes from the record offsets,

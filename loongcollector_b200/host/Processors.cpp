@@ -2265,6 +2265,61 @@ struct SplitRegexTsStage {
 #define SPLIT_REGEX_TS_ARGS(x)                                                                                         \
     (x).t.mSourceKey.data(), (uint32_t)(x).t.mSourceKey.size(), (x).Program(), (x).now, (x).DiscardInterval()
 
+// The delimiter and timestamp stages of the split -> delimiter -> timestamp chain: the delimiter stage as
+// SplitDelimStage has it, the timestamp stage's SourceKey, program, "now" and history discard as the chain calls take
+// them (SPLIT_REGEX_TS_ARGS), and the counters both Process calls would move.  The device calls take a group of exactly
+// one source event: the second-level cache would otherwise have to carry across calls.
+struct SplitDelimTsStage {
+    SplitDelimStage s;
+    ProcessorParseTimestampNative& t;
+    const PipelineEventGroup& group;
+    int64_t now;
+    SplitDelimTsStage(ProcessorParseDelimiterNative& delim, ProcessorParseTimestampNative& ts,
+                      const PipelineEventGroup& g)
+        : s(delim), t(ts), group(g), now((int64_t)time(nullptr)) {}
+    int32_t DiscardInterval() const { return t.mDiscardOldData ? t.mDiscardInterval : -1; }
+    const lc_timestamp_t* Program() const { return t.mProgram; }
+    // whether the chain's device calls take both stages behind a splitter reading sourceKey: SplitDelimStage's checks
+    // and lc_split_delim_ts_setup (which reads the key count and the overflow mode of the delimiter stage)
+    bool Accepts(const std::string& sourceKey, const StringView* okey) const {
+        const ProcessorParseDelimiterNative& d = s.d;
+        if (group.GetEvents().size() != 1 || !t.mProgram || !s.Accepts(sourceKey, okey))
+            return false;
+        LcSplitDelimSlsCfg c;
+        memset(&c, 0, sizeof c);
+        c.d.nkeys = (uint32_t)d.mKeys.size();
+        c.d.mode = d.mExtractingPartialFields ? LC_DELIM_SLS_DISCARD
+                                              : (s.Extend() ? LC_DELIM_SLS_EXTEND : LC_DELIM_SLS_KEEP);
+        LcSplitDelimTsCfg tc;
+        return !lc_split_delim_ts_setup(c, s.kp.data(), s.kl.data(), d.mSourceKey.data(),
+                                        (uint32_t)d.mSourceKey.size(), s.Renamed().data(),
+                                        (uint32_t)s.Renamed().size(), okey ? okey->data() : nullptr,
+                                        okey ? (uint32_t)okey->size() : 0u, t.mSourceKey.data(),
+                                        (uint32_t)t.mSourceKey.size(), 0, &tc);
+    }
+    // the device calls' counters[9] (the delimiter stage's successful, failed, discarded, blank, then the timestamp
+    // stage's key_not_found, out_failed, history_failure, discarded, out_successful) as the chain driver takes a
+    // stage's: successful, out_failed (a blank value counts as failed, :220-242), discarded, then the timestamp stage's
+    // discarded (so that [2] + [3] are the events the chain erased or discarded), key_not_found, out_failed,
+    // history_failure, out_successful
+    static void Fold(const uint64_t c9[9], uint64_t rctr[8]) {
+        const uint64_t f[8] = {c9[0], c9[1] + c9[3], c9[2], c9[7], c9[4], c9[5], c9[6], c9[8]};
+        memcpy(rctr, f, sizeof f);
+    }
+    void Add(const uint64_t ctr[8]) const {
+        s.Add(ctr);
+        t.mDiscardedEventsTotal.Add(ctr[3]);
+        t.mOutKeyNotFoundEventsTotal.Add(ctr[4]);
+        t.mOutFailedEventsTotal.Add(ctr[5]);
+        t.mHistoryFailureTotal.Add(ctr[6]);
+        t.mOutSuccessfulEventsTotal.Add(ctr[7]);
+    }
+    void Process(PipelineEventGroup& g) const {
+        s.Process(g);
+        t.Process(g);
+    }
+};
+
 namespace {
 // The split -> parse chain of either splitter, with the parse stage x (SplitRegexStage, SplitDelimStage,
 // SplitDelimRegexStage): `process(group)` is the splitter's Process; the device calls are sls(val, okey, pos, time, ns,
@@ -2809,6 +2864,106 @@ bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGrou
         group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
         [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_multiline_split_delim_parse_sls",
         "lc_multiline_split_delim_parse_sls_lz4", ctr);
+    mMatchedEventsTotal.Add(ctr[0]);
+    mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
+    mUnmatchedLinesTotal.Add(ctr[2]);
+    return ok;
+}
+
+bool ProcessorSplitLogStringNative::SerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                                                 ProcessorParseTimestampNative& timestamp, bool enableNs,
+                                                 std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, timestamp, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitLogStringNative::SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                                                    ProcessorParseTimestampNative& timestamp, bool enableNs,
+                                                    std::string& block, uint64_t& rawSize, std::string& err) {
+    return ChainSerializeSls(group, next, timestamp, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitLogStringNative::ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                                                      ProcessorParseTimestampNative& timestamp, bool enableNs,
+                                                      std::string& out, uint64_t* rawSize, std::string& err) {
+    const SplitDelimTsStage x(next, timestamp, group);
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_split_delim_timestamp_parse_sls(
+            Engine(), src(val), val.size(), (uint8_t)mSplitChar, SPLIT_DELIM_STAGE_ARGS(x.s),
+            okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos, time, ns, SPLIT_REGEX_TS_ARGS(x),
+            enableNs, o, cap, len, nev, c9);
+        SplitDelimTsStage::Fold(c9, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t*) {
+        uint64_t c9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_split_delim_timestamp_parse_sls_lz4(
+            Engine(), src(val), val.size(), (uint8_t)mSplitChar, SPLIT_DELIM_STAGE_ARGS(x.s),
+            okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos, time, ns, SPLIT_REGEX_TS_ARGS(x),
+            enableNs, tail, tailLen, o, cap, len, raw, nev, c9);
+        SplitDelimTsStage::Fold(c9, rctr);
+        return rc;
+    };
+    uint64_t unused[3] = {0, 0, 0};
+    return SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_split_delim_timestamp_parse_sls",
+        "lc_split_delim_timestamp_parse_sls_lz4", unused);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSls(PipelineEventGroup& group,
+                                                          ProcessorParseDelimiterNative& next,
+                                                          ProcessorParseTimestampNative& timestamp, bool enableNs,
+                                                          std::string& out, std::string& err) {
+    return ChainSerializeSls(group, next, timestamp, enableNs, out, nullptr, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::SerializeSlsLz4(PipelineEventGroup& group,
+                                                             ProcessorParseDelimiterNative& next,
+                                                             ProcessorParseTimestampNative& timestamp, bool enableNs,
+                                                             std::string& block, uint64_t& rawSize, std::string& err) {
+    return ChainSerializeSls(group, next, timestamp, enableNs, block, &rawSize, err);
+}
+
+bool ProcessorSplitMultilineLogStringNative::ChainSerializeSls(PipelineEventGroup& group,
+                                                               ProcessorParseDelimiterNative& next,
+                                                               ProcessorParseTimestampNative& timestamp,
+                                                               bool enableNs, std::string& out, uint64_t* rawSize,
+                                                               std::string& err) {
+    const SplitDelimTsStage x(next, timestamp, group);
+    const bool discard = mMultiline.mUnmatchedContentTreatment == MultilineOptions::UnmatchedContentTreatment::DISCARD;
+    auto src = [](StringView v) { return reinterpret_cast<const uint8_t*>(v.data()); };
+    auto sls = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns, uint8_t* o,
+                   uint64_t cap, uint64_t* len, uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_multiline_split_delim_timestamp_parse_sls(
+            Engine(), src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
+            SPLIT_DELIM_STAGE_ARGS(x.s), okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos, time,
+            ns, SPLIT_REGEX_TS_ARGS(x), enableNs, o, cap, len, nev, c9, sctr);
+        SplitDelimTsStage::Fold(c9, rctr);
+        return rc;
+    };
+    auto lz4 = [&](StringView val, const StringView* okey, uint64_t pos, uint32_t time, uint32_t ns,
+                   const uint8_t* tail, uint64_t tailLen, uint8_t* o, uint64_t cap, uint64_t* len, uint64_t* raw,
+                   uint64_t* nev, uint64_t* rctr, uint64_t* sctr) {
+        uint64_t c9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        const int rc = lc_multiline_split_delim_timestamp_parse_sls_lz4(
+            Engine(), src(val), val.size(), mStart.get(), mContinue.get(), mEnd.get(), discard,
+            SPLIT_DELIM_STAGE_ARGS(x.s), okey ? okey->data() : nullptr, okey ? (uint32_t)okey->size() : 0u, pos, time,
+            ns, SPLIT_REGEX_TS_ARGS(x), enableNs, tail, tailLen, o, cap, len, raw, nev, c9, sctr);
+        SplitDelimTsStage::Fold(c9, rctr);
+        return rc;
+    };
+    // matched_events, input lines, unmatched lines: moved as Process moves them (:82-84,106-107)
+    uint64_t ctr[3] = {0, 0, 0};
+    const bool ok = SplitRegexChainSls(
+        group, x, nullptr, false, mSourceKey, mEnableRawContent, enableNs, out, rawSize, err,
+        [&](PipelineEventGroup& g) { Process(g); }, sls, lz4, "lc_multiline_split_delim_timestamp_parse_sls",
+        "lc_multiline_split_delim_timestamp_parse_sls_lz4", ctr);
     mMatchedEventsTotal.Add(ctr[0]);
     mMatchedLinesTotal.Add(ctr[1] - ctr[2]);
     mUnmatchedLinesTotal.Add(ctr[2]);

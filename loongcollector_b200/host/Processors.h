@@ -228,10 +228,24 @@ public:
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseJsonNative& next,
                          ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& block,
                          uint64_t& rawSize, std::string& err);
+    // The split -> delimiter -> timestamp chain: Process(group), next.Process(group), timestamp.Process(group)
+    // (timestamp: the processor_parse_timestamp_native behind next), then SLSEventGroupSerializer::Serialize: the
+    // same bytes or error message, and the same counter updates on all three processors.  The device path
+    // (lc_split_delim_timestamp_parse_sls[_lz4]) applies under SerializeSls(group, next)'s conditions when the group
+    // holds exactly one source event (the reader's shape: the second-level cache then spans the group) and the chain
+    // accepts timestamp's SourceKey; "now" is read once per call.  Otherwise the four calls run.
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                      ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& out, std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                         ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& block,
+                         uint64_t& rawSize, std::string& err);
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                           ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& out,
+                           uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& out,
                            uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next,
@@ -316,10 +330,20 @@ public:
     bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseJsonNative& next,
                          ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& block,
                          uint64_t& rawSize, std::string& err);
+    // The split -> delimiter -> timestamp chain, as ProcessorSplitLogStringNative's
+    // (lc_multiline_split_delim_timestamp_parse_sls[_lz4]).
+    bool SerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                      ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& out, std::string& err);
+    bool SerializeSlsLz4(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                         ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& block,
+                         uint64_t& rawSize, std::string& err);
 protected:
     bool IsSupportedEvent(const PipelineEventPtr& e) const override { return e.Is<LogEvent>(); }
 
 private:
+    bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseDelimiterNative& next,
+                           ProcessorParseTimestampNative& timestamp, bool enableNs, std::string& out,
+                           uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next, bool enableNs, std::string& out,
                            uint64_t* rawSize, std::string& err);
     bool ChainSerializeSls(PipelineEventGroup& group, ProcessorParseJsonNative& next,
@@ -492,6 +516,7 @@ protected:
 private:
     friend struct SplitRegexTsStage; // the split -> regex -> timestamp chain's SerializeSls
     friend struct SplitJsonTsStage;  // the split -> JSON -> timestamp chain's
+    friend struct SplitDelimTsStage; // the split -> delimiter -> timestamp chain's
     lc_timestamp_t* mProgram = nullptr;
 };
 

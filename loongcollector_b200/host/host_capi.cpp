@@ -364,8 +364,8 @@ char* lc_host_chain3_serialize_sls(lc_host_processor_t* split, lc_host_processor
     if (raw_len_out)
         *raw_len_out = 0;
     try {
-        // (splitter, regex, filter), (splitter, regex, timestamp), (splitter, JSON, timestamp) or (splitter,
-        // delimiter, regex)
+        // (splitter, regex, filter), (splitter, regex, timestamp), (splitter, JSON, timestamp), (splitter, delimiter,
+        // regex) or (splitter, delimiter, timestamp)
         Processor* d = split->proc.get();
         Processor* b = regex->proc.get();
         Processor* c = filter->proc.get();
@@ -377,15 +377,19 @@ char* lc_host_chain3_serialize_sls(lc_host_processor_t* split, lc_host_processor
         auto* dr = dynamic_cast<ProcessorParseRegexNative*>(c);
         auto* ps = dynamic_cast<ProcessorSplitLogStringNative*>(d);
         auto* pm = dynamic_cast<ProcessorSplitMultilineLogStringNative*>(d);
-        if (!(ps || pm) || !((r && f) || (r && ts) || (js && ts) || (dl && dr)))
+        if (!(ps || pm) || !((r && f) || (r && ts) || (js && ts) || (dl && dr) || (dl && ts)))
             throw std::runtime_error("not a splitter followed by a processor_parse_regex_native and a "
                                      "processor_filter_regex_native or a processor_parse_timestamp_native, by a "
                                      "processor_parse_json_native and a processor_parse_timestamp_native, or by a "
-                                     "processor_parse_delimiter_native and a processor_parse_regex_native");
+                                     "processor_parse_delimiter_native and a processor_parse_regex_native or a "
+                                     "processor_parse_timestamp_native");
         auto chain = [&](auto* p, PipelineEventGroup& g, std::string& res, uint64_t& raw, std::string& err) {
             if (js)
                 return mode == 2 ? p->SerializeSlsLz4(g, *js, *ts, enable_ns != 0, res, raw, err)
                                  : p->SerializeSls(g, *js, *ts, enable_ns != 0, res, err);
+            if (dl && ts)
+                return mode == 2 ? p->SerializeSlsLz4(g, *dl, *ts, enable_ns != 0, res, raw, err)
+                                 : p->SerializeSls(g, *dl, *ts, enable_ns != 0, res, err);
             if (dl)
                 return mode == 2 ? p->SerializeSlsLz4(g, *dl, *dr, enable_ns != 0, res, raw, err)
                                  : p->SerializeSls(g, *dl, *dr, enable_ns != 0, res, err);
